@@ -1,6 +1,6 @@
 # Build / test entry points. The reference's Makefile is a bare `nvcc -shared` of csrc/* into
-# communicator.so with no arch flags (/root/reference/Makefile:3-19); here every unit is compiled for
-# sm_100a only (see adapcc_b200/build.py for the exact nvcc line).
+# communicator.so with no arch flags; here every unit is compiled for sm_90a (H100) only
+# (see adapcc_b200/build.py for the exact nvcc line).
 PY ?= python
 
 all: lib

@@ -1,9 +1,9 @@
-"""adapcc_b200 — a Blackwell-native adaptive collective-communication library.
+"""adapcc_b200 — a Hopper-native adaptive collective-communication library.
 
 Capabilities and API of JoeyYoung/adapcc (``AdapCC.init/setup/clear``, ``communicator.all_reduce /
 reduce / boardcast``, ``cuda_allreduce_hook`` for torch DDP, XML strategy/topology files, strategy
 synthesizer, on-the-fly link profiling, relay/straggler control, ``reconstruct_topology``),
-re-designed for 8xB200 over NVLink 5 / NVSwitch: the collectives are hand-written sm_100a kernels
+re-designed for H100 servers over NVLink / NVSwitch: the collectives are hand-written sm_90a kernels
 that move data with in-kernel peer loads/stores and NVLS multimem instructions on VMM symmetric
 memory, fused with the bucket's cast/scale/reduction.
 """

@@ -1,10 +1,10 @@
-"""tcgen05 GEMM (+bias+GELU epilogue) vs cuBLAS(+separate GELU kernel), device-timed.
+"""wgmma GEMM (+bias+GELU epilogue) vs cuBLAS(+separate GELU kernel), device-timed.
 
     python -m adapcc_b200.bench.gemm_bench [--m 8192 --n 3072 --k 768] [--iters 50] [--json out.json]
 
 Each arm: 5 warm-up calls, then 5 batches of ``iters`` back-to-back launches between two CUDA events on the
 launching stream; the median batch is reported as TFLOP/s = 2 M N K / t. No explicit L2 flush: at the default shape
-one call streams 70-120 MB (A 12.6 MB, W 4.7 MB, one or two 50 MB outputs), about the size of the 126 MB L2, so the
+one call streams 70-120 MB (A 12.6 MB, W 4.7 MB, one or two 50 MB outputs), more than the H100's 50 MB L2, so the
 outputs of one call evict the operands of the next; the JSON records this.
 """
 from __future__ import annotations
@@ -39,7 +39,7 @@ def main() -> int:
     ap.add_argument("--n", type=int, default=3072)
     ap.add_argument("--k", type=int, default=768)
     ap.add_argument("--iters", type=int, default=50)
-    ap.add_argument("--variants", default="0", help="comma list of tcgen05 kernel variants to time (0 validated; 1, 2 once they pass their tests)")
+    ap.add_argument("--variants", default="0", help="comma list of GEMM kernel variants (0-3) to time")
     ap.add_argument("--json", default="")
     a = ap.parse_args()
     from adapcc_b200.ops.gemm import linear_act
@@ -66,8 +66,8 @@ def main() -> int:
         out, pre = linear_act(x, w, b, "gelu", save_pre=True, variant=v)
         torch.cuda.synchronize()
         err = float((out.float() - ref.float()).abs().max())
-        add(f"tcgen05 variant {v}: gelu(xW^T+b), no pre", lambda v=v: linear_act(x, w, b, "gelu", variant=v), err)
-        add(f"tcgen05 variant {v}: gelu(xW^T+b) + pre", lambda v=v: linear_act(x, w, b, "gelu", save_pre=True, variant=v))
+        add(f"wgmma variant {v}: gelu(xW^T+b), no pre", lambda v=v: linear_act(x, w, b, "gelu", variant=v), err)
+        add(f"wgmma variant {v}: gelu(xW^T+b) + pre", lambda v=v: linear_act(x, w, b, "gelu", save_pre=True, variant=v))
         if v == 3 and a.n % 256 == 0:
             # the MLP backward: dH = (dY . W2) * gelu'(pre) (+ the up-projection's bias gradient = column sums of dH)
             aux = ref_pre
@@ -76,8 +76,8 @@ def main() -> int:
                 lambda: torch.ops.aten.gelu_backward(x @ w.t(), aux, approximate="tanh"))
             add("cuBLAS matmul + gelu_backward + colsum kernels",
                 lambda: torch.ops.aten.gelu_backward(x @ w.t(), aux, approximate="tanh").float().sum(0))
-            add("tcgen05 variant 3: (xW^T) * gelu'(aux)", lambda: linear_act(x, w, None, "dgelu", aux=aux, variant=3))
-            add("tcgen05 variant 3: dgelu + bias-grad column sums",
+            add("wgmma variant 3: (xW^T) * gelu'(aux)", lambda: linear_act(x, w, None, "dgelu", aux=aux, variant=3))
+            add("wgmma variant 3: dgelu + bias-grad column sums",
                 lambda: linear_act(x, w, None, "dgelu", aux=aux, colsum=cs, variant=3))
     res = {"shape": [a.m, a.n, a.k], "dtype": "bf16", "iters": a.iters,
            "l2": "working set per call (inputs + 1-2 outputs, 70-120 MB at the default shape) streams through L2",

@@ -1,7 +1,7 @@
 """Tree micro-benchmarks — what the authors explored in nccl-perf/tree/*.cu
 (/root/reference/nccl-perf/tree/{tree,tree_chunk,send_recv,all_reduce}.cu; report_tree_chunk128.txt:
 a hand-built 4-GPU ncclSend/ncclRecv reduction tree with a separate 2-input reduceKernel took
-1.6-2.1 s per rank at 128-byte chunks, 196 608 kernel launches). Here the same comparison on B200:
+1.6-2.1 s per rank at 128-byte chunks, 196 608 kernel launches). Here the same comparison on H100:
 
   * ``nccl_sendrecv_tree``: the reference-style tree built from batched isend/irecv + an add per hop,
   * ``adapcc_tree``      : our single-kernel strategy tree (reduce CTAs + broadcast CTAs),

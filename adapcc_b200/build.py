@@ -1,9 +1,9 @@
 """In-tree build of the native runtime (``adapcc_b200/_C/libadapcc.so``).
 
-The reference builds ``communicator.so`` with a bare ``nvcc -shared`` and no arch flags
-(/root/reference/Makefile:3-19). Here every translation unit is compiled for sm_100a only,
-with -lineinfo so ncu's source page maps to our code, and linked into ONE shared object that
-Python loads with ctypes (and that exports the reference's six C symbols).
+The reference builds ``communicator.so`` with a bare ``nvcc -shared`` and no arch flags. Here
+every translation unit is compiled for sm_90a (H100: wgmma, TMA, clusters, setmaxnreg need the
+arch-specific target) with -lineinfo so profilers map kernels to our source, and linked into ONE
+shared object that Python loads with ctypes (and that exports the reference's six C symbols).
 
 Usage: ``python -m adapcc_b200.build [--force] [--verbose]``
 """
@@ -23,7 +23,7 @@ OUT_DIR = PKG / "_C"
 BUILD_DIR = PKG / "_C" / "obj"
 LIB = OUT_DIR / "libadapcc.so"
 
-GENCODE = ["-gencode", "arch=compute_100a,code=sm_100a"]
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
               "-Xptxas", "-v"]
 CXX_FLAGS = ["-O2", "-std=c++17", "-fPIC"]

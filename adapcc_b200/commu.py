@@ -8,7 +8,7 @@ API and workflow parity with /root/reference/commu.py:40-435:
 * rank 0 hosts the gRPC coordinator, every rank runs a controller thread that heartbeats once per
   step and drives relays.
 
-What changed (B200-first):
+What changed (GPU-first):
 
 * a collective is ONE asynchronous kernel launch on a CUDA stream (no background pthread blocked
   inside ``initThreads``, no ``time.sleep(3)`` hand-shake, no blocking ``ctypes`` call);
@@ -123,8 +123,8 @@ class CudaCommu:
             if world_rank == 0:
                 # The coordinator answers two blocking RPCs per rank per step. Hosted as a THREAD of rank 0 (the
                 # reference's layout, /root/reference/commu.py:80-84) its handlers compete for rank 0's GIL with a
-                # launch-bound training loop: one hand-off per 5 ms switch interval -> 16 ms per negotiation on 8
-                # ranks (profiles/straggler_8xB200.json) against a 9 ms step. Default on CUDA jobs: a separate
+                # launch-bound training loop: one hand-off per 5 ms switch interval, i.e. several ms per negotiation,
+                # about a training step's length. Default on CUDA jobs: a separate
                 # PROCESS (same module, same protocol); `coordinator_process=False` keeps the in-process object
                 # (tests and tools that read `communicator.coordinator` directly).
                 as_process = bool(_arg(args, "coordinator_process",

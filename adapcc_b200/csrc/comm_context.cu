@@ -220,9 +220,8 @@ int CommContext::pick_algo(int algo, long long wire_bytes, int op, int wire, boo
   if (algo == ONE_SHOT || algo == TWO_SHOT || algo == NVLS) return algo;
   if (algo != AUTO) { set_error("bad algo %d", algo); return -1; }
   const bool nvls_pref = nvls_ok && wire_bytes >= tun.nvls_min_bytes && world_ >= tun.nvls_min_ranks;
-  // zero-copy tensors never need the staging pass a one-shot would add: measured on 8xB200 the
-  // in-place NVLS / two-shot kernels are at least as fast as one-shot from 1 KB up
-  // (profiles/allreduce_sweep_8xB200.md)
+  // zero-copy tensors never need the staging pass a one-shot would add, so the in-place NVLS / two-shot
+  // kernels are taken at every size (not yet re-measured on an 8-GPU H100 system)
   if (w.zero_copy) return nvls_pref ? NVLS : TWO_SHOT;
   if (wire_bytes <= tun.one_shot_max_bytes) return ONE_SHOT;
   return nvls_pref ? NVLS : TWO_SHOT;
@@ -328,9 +327,9 @@ int CommContext::reduce(const void* in, void* out, long long count, int dtype, i
     char* pout = (char*)out + (size_t)done * esize;
     if (w.zero_copy && done) { set_error("internal: zero-copy op split into pieces"); return -1; }
     const long long wire_bytes = n * (long long)wsize;
-    // measured on 8xB200 (profiles/allreduce_sweep_8xB200.md): splitting the grid into stager and link
-    // CTAs helps the staged two-shot (+14 % at 1 GiB, +15 % at n=2) but not staged NVLS, which is bound
-    // by local HBM traffic (6 bytes moved per payload byte), so NVLS opts in only when asked to
+    // splitting the grid into stager and link CTAs overlaps the staged two-shot's HBM copies with its link
+    // traffic; staged NVLS is bound by local HBM traffic (6 bytes moved per payload byte) and gains nothing
+    // from the split, so NVLS opts in only when asked to
     const bool pipe_algo = a == TWO_SHOT || (a == NVLS && tun.pipe_nvls);
     const bool pipelined = !w.zero_copy && !root_only_op && pipe_algo && tun.pipe_min_bytes > 0 &&
                            wire_bytes >= tun.pipe_min_bytes &&

@@ -23,7 +23,7 @@ struct Tunables {
   int relay_mode = RELAY_FORWARD;
   long long timeout_ms = 30000;
   long long pipe_min_bytes = 32ll << 20;   // staged ops at least this large use the pipelined kernel (0 = never)
-  int pipe_nvls = 0;                        // also pipeline staged NVLS ops (slower on 8xB200: HBM-bound)
+  int pipe_nvls = 0;                        // also pipeline staged NVLS ops (HBM-bound on an NVSwitch box)
   int pipe_stagers = 48, pipe_links = 48;   // CTAs of its two sub-grids
   long long pipe_piece_bytes = 16ll << 20;
   int force_kernel = 0;                // run kernels even for a single participant (smoke / ncu)

@@ -2,7 +2,7 @@
 //
 // Replaces the reference's csrc/include/init.h limits (MAX_DEVICES 16, MAX_TRANS 8,
 // MAX_CHUNK_NUM 512, 1.6 GB/child staging; /root/reference/csrc/include/init.h:14-25)
-// with a design sized for one 8xB200 NVSwitch box: no per-child staging slots, no
+// with a design sized for one 8-GPU NVSwitch box: no per-child staging slots, no
 // per-chunk IPC events, sizes are 64-bit.
 #pragma once
 #include <cuda.h>

@@ -4,7 +4,7 @@
 // numa_run_on_node to find the NIC's NUMA node, pairwise D2H bandwidth drops to find GPUs
 // behind one PCIe switch, H2D under NIC load to find the GPU closest to the NIC, then dumps
 // topology/topo_detect_<rank>.xml as <cpu><pcie>[<nic/>]<gpu id/>…
-// (/root/reference/csrc/detect.cu:209-427). On B200 none of that has to be guessed: NVML,
+// (/root/reference/csrc/detect.cu:209-427). On an NVSwitch box none of that has to be guessed: NVML,
 // the CUDA P2P attributes and sysfs report it. We emit the same XML schema (so the control
 // plane's gather step is unchanged) plus attributes the synthesizer uses on NVSwitch
 // systems: NVLink link counts, P2P performance rank, native atomics, multicast (NVLS).

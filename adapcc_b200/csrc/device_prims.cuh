@@ -3,7 +3,7 @@
 //     reference's per-chunk cudaIpc events + SysV shm bool + CPU spin,
 //     /root/reference/csrc/trans.cu:58-100),
 //   * 16-byte "pack" load/store/convert helpers (fp32 / bf16 / fp16 wire formats),
-//   * NVLS multimem.ld_reduce / multimem.st wrappers (sm_90+; we build sm_100a only).
+//   * NVLS multimem.ld_reduce / multimem.st wrappers (sm_90+; we build sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>

@@ -1,9 +1,9 @@
-// Low-latency ("LL") one-shot all-reduce for small messages. Validated on 2xB200 in round 2 (gpurun call 2: numerics
-// incl. odd tails and back-to-back ops mixed with barrier-protocol ops; 4.2 us at 1 KB vs 9.3 us for the barrier kernels);
-// AUTO picks it for all-rank messages <= 32 KB (CommContext::allreduce).
+// Low-latency ("LL") one-shot all-reduce for small messages (numerics incl. odd tails and back-to-back ops mixed with
+// barrier-protocol ops: tests/gpu_collectives_worker.py, which needs at least 2 GPUs); AUTO picks it for all-rank
+// messages <= 32 KB (CommContext::allreduce).
 //
 // The direct one-shot kernel (kernels_direct.cuh) costs two flag barriers per op: publish, barrier, pull,
-// barrier — four NVLink latencies (11.3 us for 1 KB on 8 GPUs, profiles/allreduce_sweep_8xB200.md). Here the
+// barrier — four NVLink latencies. Here the
 // flag travels WITH the data, the way NCCL's LL protocol does it (third-party/nccl/src/device/prims_ll.h in the
 // reference tree), but push-based over NVSwitch peer memory:
 //

@@ -1,9 +1,8 @@
 // Pipelined staged all-reduce for LARGE tensors that are not in the symmetric heap.
 //
 // The plain staged kernel (kernels_direct.cuh) runs stage-in -> NVLink phase -> stage-out with all
-// CTAs in lockstep, so HBM copies and link traffic never overlap: measured 568 GB/s at 1 GiB on
-// 8xB200 against 835 GB/s for the zero-copy path and 726 GB/s for NCCL (profiles/
-// allreduce_sweep_8xB200.md). Here the message is cut into pieces and the grid into two sub-grids,
+// CTAs in lockstep, so HBM copies and link traffic never overlap, and large staged tensors fall well
+// behind the zero-copy path. Here the message is cut into pieces and the grid into two sub-grids,
 // the same idea as the tree kernel's reduce/broadcast split (and the reference's thread pair per
 // tree, /root/reference/csrc/allreduce.cu:735-742):
 //

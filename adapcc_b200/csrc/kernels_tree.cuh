@@ -7,7 +7,7 @@
 //   * reduce runs leaf -> root, broadcast root -> leaf on the same tree, and a chunk starts
 //     its way down as soon as the root has reduced it (reduce/broadcast pipelining),
 //   * relay control: ranks that are not active contribute nothing but still forward.
-// What is different (B200-first): no pthread per tree, no copy engine, no IPC events, no
+// What is different (GPU-first): no pthread per tree, no copy engine, no IPC events, no
 // host sync per chunk. A parent PULLS its children's partial sums with 128-bit peer loads
 // over NVLink straight out of the child's symmetric window (so there is no per-child
 // staging slot), reduces in fp32 registers and publishes the chunk with one

@@ -3,7 +3,7 @@
 // The reference's MoE workload uses the vendored fastmoe (/root/reference/models/moe/train_moe.py;
 // third-party/fastmoe/cuda/local_exchange.cuh:5-69 count/assign-pos kernels,
 // global_exchange.h:11-98 grouped ncclSend/ncclRecv all-to-all-v, parallel_linear.cuh per-expert
-// cuBLAS GEMMs). B200-first equivalent: the token exchange is NOT a collective library call — each
+// cuBLAS GEMMs). GPU-first equivalent: the token exchange is NOT a collective library call — each
 // rank's kernel stores token rows straight into the destination rank's expert buffer over NVLink
 // (dispatch) and loads result rows straight out of it (combine); slot assignment is a device-side
 // atomic counter per expert; ranks only meet at per-CTA flag barriers on the signal pad.

@@ -3,19 +3,23 @@
 // GPT-2's input layer is x[t] = wte[ids[t]] + wpe[pos[t]] + wte[token_type[t]]
 // (/root/reference/models/gpt2/train_gpt2_ddp.py:157-159 -> transformers' GPT2Model): three gathers and two adds
 // forward, and — the expensive part — three sort-based `embedding_dense_backward` passes (16 radix-sort launches,
-// segment scans, 0.35 ms per step on B200) plus two 77 MB accumulate kernels backward. Here:
+// segment scans) plus two 77 MB accumulate kernels backward. Here:
 //
 //   forward : one kernel, one warp per token row, the K looked-up rows summed in fp32 registers, bf16 out.
-//   backward: three small launches, no sort, no host-visible sizes (CUDA-graph capturable):
+//   backward: three small launches, no sort, no host-visible sizes (CUDA-graph capturable), bit-for-bit repeatable:
 //     1. claim   : every lookup (k, t) does atomicMin(owner[table_k, idx], lookup id) — the smallest lookup id that
-//                  hits a table row becomes the row's OWNER for this step;
-//     2. scatter : every lookup adds its dY row into the owner's fp32 scratch row with red.global.add.v4.f32
-//                  (duplicates — repeated tokens, the two token-type rows hit by thousands of tokens — accumulate in
-//                  fp32, like ATen's segment reduction, not in bf16); rows hit many times within a 64-lookup tile are
-//                  pre-summed in registers first;
-//     3. commit  : each owner adds its scratch row into the table's bf16 gradient row (which may already hold another
-//                  contribution, e.g. the tied LM head's dW), zeroes the scratch row and releases the owner slot, so
-//                  both work buffers are back to their initial state for the next step.
+//                  hits a table row becomes the row's OWNER for this step — and atomicMax(maxbits[table_k, idx],
+//                  max |dY[t, :]|) (the float bits of a non-negative value order like the integers);
+//     2. scatter : every lookup adds its dY row into the owner's scratch row as 64-bit FIXED POINT (red.add.u64),
+//                  scaled by 2^shift with shift = 62 - log2(#lookups) - exponent(row max): no sum can overflow, the
+//                  resolution is 2^-46 or finer of the row's largest entry, and integer addition gives the same bits
+//                  in every order (an fp32 red.add would not: duplicates — repeated tokens, the two token-type rows hit
+//                  by thousands of tokens — arrive in a different order every run); rows hit many times within a
+//                  64-lookup tile are pre-summed in registers (in a fixed order) first;
+//     3. commit  : each owner converts its scratch row back (NaN if the row's dY held a non-finite value), adds it into
+//                  the table's bf16 gradient row (which may already hold another contribution, e.g. the tied LM head's
+//                  dW), zeroes the scratch row and releases the owner and maxbits slots, so all work buffers are back
+//                  to their initial state for the next step.
 //   Lookups that share a table (ids and token types both index wte) share owner slots, so a row hit through both is
 //   still committed exactly once.
 #include <cuda_bf16.h>
@@ -69,32 +73,54 @@ embed_sum_fwd_kernel(const __grid_constant__ EmbedFwdArgs a, int n, int D, __nv_
   }
 }
 
+// one warp per lookup
 __global__ void __launch_bounds__(256)
-embed_bwd_claim_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int* __restrict__ owner) {
-  const int i = (int)(blockIdx.x * (long long)blockDim.x + threadIdx.x);
+embed_bwd_claim_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, const __nv_bfloat16* __restrict__ dy,
+                       int* __restrict__ owner, unsigned int* __restrict__ maxbits) {
+  const int i = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (i >= a.K * n) return;
   const int k = i / n, t = i - k * n;
-  atomicMin(owner + a.owner_base[k] + (int)a.idx[k][t], i);
+  const int slot = a.owner_base[k] + (int)a.idx[k][t];
+  unsigned int m = 0;
+  for (int c = lane; c < (D >> 3); c += 32) {
+    float f[8];
+    unpack<__nv_bfloat16>(ld16(dy + (long long)t * D + c * 8), f);
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m = max(m, __float_as_uint(fabsf(f[e])));      // NaN / inf order above every finite
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  if (lane == 0) {
+    atomicMin(owner + slot, i);
+    atomicMax(maxbits + slot, m);
+  }
 }
 
-__device__ __forceinline__ void red_add_v4(float* p, float a, float b, float c, float d) {
-  asm volatile("red.relaxed.gpu.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(a), "f"(b), "f"(c), "f"(d)
-               : "memory");
+// 2^shift scales a row whose largest |entry| has float bits `mb` so that up to 2^lookup_bits such entries sum below 2^62
+__device__ __forceinline__ int embed_shift(unsigned int mb, int lookup_bits) {
+  const int ex = (int)((mb >> 23) & 0xffu);
+  const int e = ex == 0 ? -126 : ex - 127;                   // |entry| < 2^(e + 1)
+  return 62 - lookup_bits - (e + 1);
 }
 
-// scratch[owner, :] += dY[t, :] for a TILE of 64 consecutive lookups per CTA. Rows hit by many lookups of the tile (the
+__device__ __forceinline__ void red_add_fixed(long long* p, float v, int shift) {
+  atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)__float2ll_rn(ldexpf(v, shift)));
+}
+
+// scratch[owner, :] += dY[t, :] (fixed point) for a TILE of 64 consecutive lookups per CTA. Rows hit by many lookups of the tile (the
 // two token-type rows are hit by every token) are first summed in registers and leave as ONE reduction per tile and
 // thread group instead of one per lookup: up to 4 "hot" owners per tile (>= 4 hits), found with 64 x 64 compares in
-// shared memory. Everything else (token ids, positions: mostly unique inside a tile) goes straight to
-// red.global.add.v4.f32. First version (one warp per lookup, every lookup its own reductions): 136 us of the GPT-2 step,
-// 4096-deep same-address contention on the token-type rows.
+// shared memory. Everything else (token ids, positions: mostly unique inside a tile) goes straight to the scratch row.
 constexpr int kEmbTile = 64, kEmbHot = 4, kEmbGroup = 128;       // 2 thread groups x 128 threads; group g: lookups j = g mod 2
 
 __global__ void __launch_bounds__(2 * kEmbGroup)
 embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, const __nv_bfloat16* __restrict__ dy,
-                         const int* __restrict__ owner, float* __restrict__ scratch) {
+                         const int* __restrict__ owner, const unsigned int* __restrict__ maxbits,
+                         long long* __restrict__ scratch, int lookup_bits) {
   __shared__ int s_own[kEmbTile];
   __shared__ int s_row[kEmbTile];
+  __shared__ int s_shift[kEmbTile];
+  __shared__ int s_hot_shift[kEmbHot];
   __shared__ int s_hot_key[kEmbHot];
   __shared__ int s_hot_of[kEmbTile];
   __shared__ int s_nhot;
@@ -104,14 +130,17 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
   if (j == 0) s_nhot = 0;
   if (j < kEmbTile) {
     const int i = i0 + j;
-    int own = -1, row = 0;
+    int own = -1, row = 0, shift = 0;
     if (i < total) {
       const int k = i / n;
       row = i - k * n;
-      own = owner[a.owner_base[k] + (int)a.idx[k][row]];
+      const int slot = a.owner_base[k] + (int)a.idx[k][row];
+      own = owner[slot];
+      shift = embed_shift(maxbits[slot], lookup_bits);
     }
     s_own[j] = own;
     s_row[j] = row;
+    s_shift[j] = shift;
   }
   __syncthreads();
   if (j < kEmbTile && s_own[j] >= 0) {
@@ -126,7 +155,10 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
     }
     if (first && cnt >= 4) {
       const int slot = atomicAdd(&s_nhot, 1);
-      if (slot < kEmbHot) s_hot_key[slot] = own;
+      if (slot < kEmbHot) {
+        s_hot_key[slot] = own;
+        s_hot_shift[slot] = s_shift[j];
+      }
     }
   }
   __syncthreads();
@@ -153,9 +185,9 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
       unpack<__nv_bfloat16>(ld16(dy + (long long)s_row[jj] * D + c * 8), f);
       const int h = s_hot_of[jj];
       if (h < 0) {
-        float* dst = scratch + (long long)own * D + c * 8;
-        red_add_v4(dst, f[0], f[1], f[2], f[3]);
-        red_add_v4(dst + 4, f[4], f[5], f[6], f[7]);
+        long long* dst = scratch + (long long)own * D + c * 8;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) red_add_fixed(dst + e, f[e], s_shift[jj]);
       } else {
 #pragma unroll
         for (int q = 0; q < kEmbHot; ++q)
@@ -168,38 +200,45 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
 #pragma unroll
     for (int q = 0; q < kEmbHot; ++q)
       if (q < nhot) {
-        float* dst = scratch + (long long)s_hot_key[q] * D + c * 8;
-        red_add_v4(dst, acc[q][0], acc[q][1], acc[q][2], acc[q][3]);
-        red_add_v4(dst + 4, acc[q][4], acc[q][5], acc[q][6], acc[q][7]);
+        long long* dst = scratch + (long long)s_hot_key[q] * D + c * 8;
+#pragma unroll
+        for (int e = 0; e < 8; ++e) red_add_fixed(dst + e, acc[q][e], s_hot_shift[q]);
       }
   }
 }
 
-// one warp per lookup; only owners act: grad[idx, :] += scratch[i, :]; scratch[i, :] = 0; owner slot released
+// one warp per lookup; only owners act: grad[idx, :] += scratch[i, :]; scratch[i, :] = 0; owner / maxbits slots released
 __global__ void __launch_bounds__(256)
 embed_bwd_commit_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, int* __restrict__ owner,
-                        float* __restrict__ scratch) {
+                        unsigned int* __restrict__ maxbits, long long* __restrict__ scratch, int lookup_bits) {
   const int i = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (i >= a.K * n) return;
   const int k = i / n, t = i - k * n;
   const long long row = a.idx[k][t];
   int* slot = owner + a.owner_base[k] + (int)row;
   if (*slot != i) return;                       // warp-uniform: every lane reads the same word
-  float* s = scratch + (long long)i * D;
+  unsigned int* mb_slot = maxbits + (slot - owner);
+  const unsigned int mb = *mb_slot;
+  const bool finite = mb < 0x7f800000u;
+  const int shift = embed_shift(mb, lookup_bits);
+  long long* s = scratch + (long long)i * D;
   __nv_bfloat16* g = a.grad[k] + row * (long long)D;
   const int nvec = D >> 3;
   for (int c = lane; c < nvec; c += 32) {
     float f[8];
     unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(g + c * 8), f);
-    const float4 s0 = *reinterpret_cast<const float4*>(s + c * 8), s1 = *reinterpret_cast<const float4*>(s + c * 8 + 4);
-    f[0] += s0.x; f[1] += s0.y; f[2] += s0.z; f[3] += s0.w;
-    f[4] += s1.x; f[5] += s1.y; f[6] += s1.z; f[7] += s1.w;
+#pragma unroll
+    for (int e = 0; e < 8; ++e) {
+      f[e] += finite ? (float)ldexp((double)s[c * 8 + e], -shift) : __int_as_float(0x7fc00000);
+      s[c * 8 + e] = 0;
+    }
     *reinterpret_cast<uint4*>(g + c * 8) = pack<__nv_bfloat16>(f);
-    *reinterpret_cast<float4*>(s + c * 8) = make_float4(0.f, 0.f, 0.f, 0.f);
-    *reinterpret_cast<float4*>(s + c * 8 + 4) = make_float4(0.f, 0.f, 0.f, 0.f);
   }
   __syncwarp();
-  if (lane == 0) *slot = INT_MAX;
+  if (lane == 0) {
+    *slot = INT_MAX;
+    *mb_slot = 0u;
+  }
 }
 
 __global__ void embed_fill_int_kernel(int* p, long long n, int v) {
@@ -230,10 +269,11 @@ int adapcc_embed_sum_fwd(void* const* tables, void* const* idx, int K, int n, in
   return 0;
 }
 
-// owner: int32 [sum of distinct table rows], all INT_MAX between calls; scratch: fp32 [K * n, D], all zero between
-// calls (adapcc_embed_bwd_reset establishes both). grads[k]: bf16 [rows_k, D], accumulated into.
+// owner: int32 [sum of distinct table rows], all INT_MAX between calls; maxbits: uint32, same size, all zero between
+// calls; scratch: int64 [K * n, D], all zero between calls (adapcc_embed_bwd_reset establishes all three).
+// grads[k]: bf16 [rows_k, D], accumulated into.
 int adapcc_embed_sum_bwd(const void* dy, void* const* idx, void* const* grads, const int* owner_base, int K, int n,
-                         int D, int* owner, float* scratch, void* stream) {
+                         int D, int* owner, unsigned int* maxbits, long long* scratch, void* stream) {
   if (n <= 0) return 0;
   if (K < 1 || K > kEmbedMaxLookups || D % 8 != 0) { set_error("embed_sum_bwd: 1 <= K <= %d lookups, D %% 8 == 0", kEmbedMaxLookups); return -1; }
   if ((long long)K * n >= INT_MAX) { set_error("embed_sum_bwd: too many lookups"); return -1; }
@@ -247,20 +287,24 @@ int adapcc_embed_sum_bwd(const void* dy, void* const* idx, void* const* grads, c
   }
   cudaStream_t s = (cudaStream_t)stream;
   const int total = K * n;
-  embed_bwd_claim_kernel<<<(total + 255) / 256, 256, 0, s>>>(a, n, owner);
+  int lookup_bits = 0;                               // total <= 2^lookup_bits
+  while ((1LL << lookup_bits) < (long long)total) ++lookup_bits;
   const int wpb = 8;
+  embed_bwd_claim_kernel<<<(total + wpb - 1) / wpb, wpb * 32, 0, s>>>(a, n, D, (const __nv_bfloat16*)dy, owner, maxbits);
   embed_bwd_scatter_kernel<<<(total + kEmbTile - 1) / kEmbTile, 2 * kEmbGroup, 0, s>>>(a, n, D, (const __nv_bfloat16*)dy, owner,
-                                                                                   scratch);
-  embed_bwd_commit_kernel<<<(total + wpb - 1) / wpb, wpb * 32, 0, s>>>(a, n, D, owner, scratch);
+                                                                                   maxbits, scratch, lookup_bits);
+  embed_bwd_commit_kernel<<<(total + wpb - 1) / wpb, wpb * 32, 0, s>>>(a, n, D, owner, maxbits, scratch, lookup_bits);
   CUDA_TRY(cudaGetLastError());
   count_launch(3);
   return 0;
 }
 
-int adapcc_embed_bwd_reset(int* owner, long long n_owner, float* scratch, long long scratch_elems, void* stream) {
+int adapcc_embed_bwd_reset(int* owner, unsigned int* maxbits, long long n_owner, long long* scratch,
+                           long long scratch_elems, void* stream) {
   cudaStream_t s = (cudaStream_t)stream;
   if (n_owner > 0) embed_fill_int_kernel<<<(int)std::min<long long>(1024, (n_owner + 255) / 256), 256, 0, s>>>(owner, n_owner, INT_MAX);
-  if (scratch_elems > 0) CUDA_TRY(cudaMemsetAsync(scratch, 0, (size_t)scratch_elems * sizeof(float), s));
+  if (n_owner > 0) CUDA_TRY(cudaMemsetAsync(maxbits, 0, (size_t)n_owner * sizeof(unsigned int), s));
+  if (scratch_elems > 0) CUDA_TRY(cudaMemsetAsync(scratch, 0, (size_t)scratch_elems * sizeof(long long), s));
   CUDA_TRY(cudaGetLastError());
   if (n_owner > 0) count_launch();
   return 0;

@@ -1,9 +1,8 @@
 // Fused LayerNorm forward / backward and column-sum (bias-gradient) kernels for the transformer
 // workloads (GPT-2, ViT). The reference trains stock HF / vit-pytorch modules
-// (/root/reference/models/gpt2/train_gpt2_ddp.py:157-159, models/vit/train_vit.py:30-40); measured on
-// B200 (profiles/launches_gpt2_eager.md) the eager LayerNorm backward (GammaBetaBackward +
-// grad_input kernels) and the bias-gradient reductions cost 3.4 ms of a 17 ms step — more than
-// attention. These kernels are memory-bound single-pass replacements:
+// (/root/reference/models/gpt2/train_gpt2_ddp.py:157-159, models/vit/train_vit.py:30-40), whose eager
+// LayerNorm backward (GammaBetaBackward + grad_input kernels) and bias-gradient reductions are
+// separate multi-pass kernels. These kernels are memory-bound single-pass replacements:
 //   ln_fwd : one warp per row, row held in registers (D = 256*VPL, VPL<=4), writes y, mean, rstd
 //   ln_bwd : one warp per row for dx; per-lane fp32 accumulators for dgamma/dbeta, reduced per CTA
 //            into a [grid, D] partial buffer, finalised by colsum_finalize
@@ -163,8 +162,8 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restr
 
 // out[c] (bf16 or fp32) = sum_p part[p][c]. Block = 32 columns x 32 row lanes: every row lane sums
 // a strided subset of the partial rows (128-byte coalesced row segments), then the 32 lanes are
-// combined through shared memory. (The first version walked all partial rows with one thread per
-// column: 25 us per call, 2.4 ms per GPT-2 step — see profiles/launches_gpt2_eager.md history.)
+// combined through shared memory (one thread per column walking all partial rows leaves most of the
+// memory bandwidth unused).
 template <typename O>
 __global__ void __launch_bounds__(1024)
 colsum_finalize_kernel(const float* __restrict__ part, int nparts, int cols, O* __restrict__ out) {
@@ -245,11 +244,24 @@ using namespace adapcc;
 
 extern "C" {
 
+// SMs of the current device (132 on an H100 SXM), read once.
+static int sm_count() {
+  static int sms = 0;
+  if (sms == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) {
+      (void)cudaGetLastError();
+      sms = 132;
+    }
+  }
+  return sms;
+}
+
 // Persistent grid: at most `per_sm` CTAs per SM (what the launch bounds make resident), shrunk so that
-// every CTA runs the same number of row-group iterations (8192 rows, 444 slots -> 342 CTAs x 3).
+// every CTA runs the same number of row-group iterations (8192 rows, 396 slots on 132 SMs -> 342 CTAs x 3).
 static int ln_grid(int rows, int per_sm) {
   const int groups = std::max(1, (rows + kLnWarps - 1) / kLnWarps);
-  const int cap = 148 * per_sm;
+  const int cap = sm_count() * per_sm;
   const int iters = (groups + cap - 1) / cap;
   return (groups + iters - 1) / iters;
 }

@@ -3,7 +3,7 @@
 // and, where the NVSwitch supports it, bound to one multicast object (NVLS
 // multimem.ld_reduce / multimem.st).
 //
-// This is the B200-native replacement for the reference's POSIX/SysV shared-memory
+// This is the native replacement for the reference's POSIX/SysV shared-memory
 // tables of cudaIpcMemHandle_t / cudaIpcEventHandle_t and the receiver-allocated 1.6 GB
 // per-child staging buffers (/root/reference/csrc/shm_ipc.cpp:5-96,
 // /root/reference/csrc/allreduce.cu:442-495): one VMM allocation per rank, no IPC events,

@@ -5,11 +5,12 @@ ctx 1024, vocab 50257 + 5 special tokens) on PersonaChat-shaped batches
 ``input_ids/token_type_ids/lm_labels [B, C, T]``, ``mc_token_ids [B, C]``, ``mc_labels [B]`` with
 loss = lm_coef * LM cross-entropy + mc_coef * multiple-choice cross-entropy
 (/root/reference/models/gpt2/train_gpt2_ddp.py:28-31,100-107,157-195). This is the same
-architecture written for B200 training:
+architecture written for H100 training:
 
 * parameters live in bf16 (fp32 master copy inside the fused optimizer), so gradients are born in
   bf16 and the gradient all-reduce moves half the bytes with fp32 accumulation in the kernel;
-* attention goes through ``scaled_dot_product_attention`` (flash kernels), MLP through cuBLAS;
+* attention goes through ``scaled_dot_product_attention`` (flash kernels; the backward in its deterministic mode, so a
+  step computes the same bits every run), MLP through the fused GEMMs;
 * the LM head + cross-entropy is one fused pass per row chunk: bf16 logits from the GEMM, a softmax-CE
   kernel that overwrites them in place with their gradient, and the two backward GEMMs right away — fp32
   logits / probabilities (50 304 x 8192 x 4 B = 1.6 GB each in the stock path) never exist;
@@ -51,8 +52,57 @@ class GPT2Config:
         return cls(vocab_size=512, n_positions=64, n_embd=64, n_layer=2, n_head=4, lm_chunk_rows=64)
 
 
+class _Deterministic:
+    """PyTorch's deterministic algorithms switched on (not warn-only) inside the block, the previous setting restored.
+    Filling freshly allocated tensors with NaN (what the mode also does by default) is switched off inside: attention
+    writes every element it allocates, so the fill would only cost time."""
+
+    def __enter__(self):
+        import torch.utils.deterministic as det
+
+        self.prev = (torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled(),
+                     det.fill_uninitialized_memory)
+        torch.use_deterministic_algorithms(True)
+        det.fill_uninitialized_memory = False
+
+    def __exit__(self, *exc):
+        import torch.utils.deterministic as det
+
+        torch.use_deterministic_algorithms(self.prev[0], warn_only=self.prev[1])
+        det.fill_uninitialized_memory = self.prev[2]
+
+
+class _CausalAttention(torch.autograd.Function):
+    """Causal ``scaled_dot_product_attention`` run, forward and backward, with PyTorch's deterministic algorithms
+    switched on and restored afterwards: the flash backward then sums dQ in a fixed order instead of with atomics, so
+    the same inputs give the same gradient bits every run (PyTorch settles the mode when the forward runs, so both
+    passes need it). At GPT-2 small's shape on an H100: 0.44 ms per layer forward + backward instead of 0.26."""
+
+    @staticmethod
+    def forward(ctx, q, k, v):
+        with torch.enable_grad(), _Deterministic():
+            inner = [t.detach().requires_grad_(True) for t in (q, k, v)]
+            out = F.scaled_dot_product_attention(*inner, is_causal=True)
+        ctx.inner, ctx.out = inner, out
+        return out.detach()
+
+    @staticmethod
+    def backward(ctx, dout):
+        with _Deterministic():
+            grads = torch.autograd.grad(ctx.out, ctx.inner, dout)
+        del ctx.inner, ctx.out
+        return grads
+
+
+def causal_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor) -> torch.Tensor:
+    """Causal attention [B, H, T, Dh]; repeatable backward on CUDA (see ``_CausalAttention``)."""
+    if q.is_cuda and torch.is_grad_enabled() and (q.requires_grad or k.requires_grad or v.requires_grad):
+        return _CausalAttention.apply(q, k, v)
+    return F.scaled_dot_product_attention(q, k, v, is_causal=True)
+
+
 class Block(nn.Module):
-    """Pre-LN transformer block; the MLP runs as two GEMMs with the activation passes in tcgen05 epilogues when
+    """Pre-LN transformer block; the MLP runs as two GEMMs with the activation passes in GEMM epilogues when
     supported (ops/gemm.py), residual adds optionally fused into the following LayerNorm (``forward_deferred``)."""
 
     def __init__(self, cfg: GPT2Config):
@@ -66,9 +116,9 @@ class Block(nn.Module):
         self.ln_2 = FusedLayerNorm(d, eps=cfg.layer_norm_epsilon)
         self.c_fc = FusedLinear(d, 4 * d)
         self.c_proj2 = FusedLinear(4 * d, d)
-        # the MLP's activation passes live in our tcgen05 GEMM's epilogues (ops/gemm.py, csrc/gemm_tcgen05_pp.cu):
+        # the MLP's activation passes live in our wgmma GEMM's epilogues (ops/gemm.py, csrc/gemm_wgmma.cu):
         # 2 (default): c_fc + bias + GELU forward AND dGELU + the c_fc bias gradient in the backward GEMM dY.W2 — no
-        #    stand-alone GELU / GELU-backward / column-sum kernel (measured -0.32 ms per GPT-2 step on B200);
+        #    stand-alone GELU / GELU-backward / column-sum kernel;
         # 1: forward fusion only; 0: cuBLAS + separate activation kernels
         self.tc_mlp = int(os.environ.get("ADAPCC_TCGEN05_MLP", "2") or 0)
 
@@ -86,7 +136,7 @@ class Block(nn.Module):
         # split along the feature dim (views; measured 6 % faster fwd+bwd than the packed permute:
         # the backward writes dq/dk/dv straight into one [B, T, 3D] buffer layout-wise)
         q, k, v = (t.view(B, T, self.n_head, D // self.n_head).transpose(1, 2) for t in self.c_attn(h).split(D, dim=-1))
-        a = F.scaled_dot_product_attention(q, k, v, is_causal=True)
+        a = causal_attention(q, k, v)
         return self.c_proj(a.transpose(1, 2).reshape(B, T, D))
 
     def forward_deferred(self, x: torch.Tensor, delta: Optional[torch.Tensor]):
@@ -211,7 +261,7 @@ class GPT2DoubleHeads(nn.Module):
         # batches score only the last candidate's reply, i.e. ~1/8 of the rows at the bench shape.
         self.lm_row_capacity = 0
         # residual adds fused into the following LayerNorm (fwd) / its input gradient (bwd)
-        # (default on since the fused tcgen05 MLP: A/B in one gpurun call 8.53 vs 8.58-8.66 ms per step)
+        # (default on since the fused MLP GEMMs)
         self.fuse_add_ln = os.environ.get("ADAPCC_FUSE_ADD_LN", "1") == "1"
         # wte[ids] + wpe[pos] + wte[token types] as one kernel, sort-free fp32-accumulating backward
         # (csrc/ops_embed.cu); the flat engine gives both tables a gradient sink (parallel/engine.py)

@@ -1,6 +1,6 @@
 """ViT workload. The reference's script (/root/reference/models/vit/train_vit.py:30-63) trains
 ``vit_pytorch.ViT(image_size=256, patch_size=32, dim=1024, depth=6, heads=16, mlp_dim=2048)`` on
-synthetic batches of 256 images under plain DDP; BASELINE.json names ViT-B/16 for the B200 config
+synthetic batches of 256 images under plain DDP; BASELINE.json names ViT-B/16 for the H100 config
 ("ViT-B/16 DDP with reconstruct_topology every 500 steps"). Both shapes are available here; the
 model is a standard pre-norm ViT on ``scaled_dot_product_attention``."""
 from __future__ import annotations

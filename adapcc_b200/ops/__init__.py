@@ -1,4 +1,4 @@
-"""Hand-written sm_100a ops used by the training engine and the workloads (bound through the same
+"""Hand-written sm_90a ops used by the training engine and the workloads (bound through the same
 in-tree ``libadapcc.so`` as the collectives). Every function launches on the current CUDA stream
 and fails loudly if the native library is missing — there is no silent PyTorch fallback on a GPU.
 """
@@ -36,8 +36,8 @@ def _lib():
         lib.adapcc_fused_ce_scaled.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
         lib.adapcc_embed_sum_fwd.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
         lib.adapcc_embed_sum_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
-                                             c_void_p, c_void_p]
-        lib.adapcc_embed_bwd_reset.argtypes = [c_void_p, c_longlong, c_void_p, c_longlong, c_void_p]
+                                             c_void_p, c_void_p, c_void_p]
+        lib.adapcc_embed_bwd_reset.argtypes = [c_void_p, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p]
         _bound = True
     return lib
 
@@ -139,16 +139,18 @@ _embed_work = {}
 
 
 def _embed_buffers(device, n_owner: int, scratch_elems: int):
-    """(owner int32 [n_owner] all INT_MAX, scratch fp32 [scratch_elems] all zero): the backward kernels leave both in
-    exactly that state again, so they are initialised once per (device, size)."""
+    """(owner int32 [n_owner] all INT_MAX, maxbits int32 [n_owner] all zero, scratch int64 fixed point [scratch_elems]
+    all zero): the backward kernels leave all three in exactly that state again, so they are initialised once per
+    (device, size)."""
     key = (device.index, n_owner, scratch_elems)
     buf = _embed_work.get(key)
     if buf is None:
         owner = torch.empty(n_owner, dtype=torch.int32, device=device)
-        scratch = torch.empty(scratch_elems, dtype=torch.float32, device=device)
-        _ck(_lib().adapcc_embed_bwd_reset(c_void_p(owner.data_ptr()), n_owner, c_void_p(scratch.data_ptr()),
-                                          scratch_elems, _stream()), "embed_bwd_reset")
-        buf = _embed_work[key] = (owner, scratch)
+        maxbits = torch.empty(n_owner, dtype=torch.int32, device=device)
+        scratch = torch.empty(scratch_elems, dtype=torch.int64, device=device)
+        _ck(_lib().adapcc_embed_bwd_reset(c_void_p(owner.data_ptr()), c_void_p(maxbits.data_ptr()), n_owner,
+                                          c_void_p(scratch.data_ptr()), scratch_elems, _stream()), "embed_bwd_reset")
+        buf = _embed_work[key] = (owner, maxbits, scratch)
     return buf
 
 
@@ -181,7 +183,7 @@ class _EmbedSumFn(torch.autograd.Function):
         for t in tables:                                   # owner slots: one range per distinct table
             base.append(off)
             off += t.shape[0]
-        owner, scratch = _embed_buffers(dy.device, off, K * n * D)
+        owner, maxbits, scratch = _embed_buffers(dy.device, off, K * n * D)
         sinks = [_sink(t) for t in tables]
         grads, ret = [], []
         for t, s in zip(tables, sinks):
@@ -194,8 +196,8 @@ class _EmbedSumFn(torch.autograd.Function):
                 ret.append(g)
         ob = (c_int * K)(*[base[j] for j in spec])
         _ck(_lib().adapcc_embed_sum_bwd(c_void_p(dy.data_ptr()), _ptr_array(idx), _ptr_array([grads[j] for j in spec]),
-                                        ob, K, n, D, c_void_p(owner.data_ptr()), c_void_p(scratch.data_ptr()),
-                                        _stream()), "embed_sum_bwd")
+                                        ob, K, n, D, c_void_p(owner.data_ptr()), c_void_p(maxbits.data_ptr()),
+                                        c_void_p(scratch.data_ptr()), _stream()), "embed_sum_bwd")
         for s in sinks:
             if s is not None:
                 s.done()

@@ -1,12 +1,10 @@
-"""tcgen05 GEMMs with fused epilogues (csrc/gemm_tcgen05.cu: variants 0-2; csrc/gemm_tcgen05_pp.cu: variant 3).
+"""Hopper GEMMs with fused epilogues (csrc/gemm_wgmma.cu: TMA + mbarrier pipeline + wgmma, variants 0-3).
 
 ``linear_act(x, weight, bias, act)`` computes ``act(x @ weight.T + bias)`` for bf16 CUDA tensors with the
-accumulator in TMEM and the activation applied in the epilogue; ``linear_gelu`` / ``mlp_gelu`` are the autograd forms
-(the pre-activation is written by the same kernel; the backward GEMM applies gelu' and accumulates the bias gradient in
-its epilogue). The GPT-2 MLP uses ``mlp_gelu`` by default (``ADAPCC_TCGEN05_MLP=0`` restores cuBLAS + separate
-activation kernels). Measured on B200 at 8192 x 3072 x 768: forward 46 us vs 61 us (cuBLAS + GELU kernel), backward
-52 us incl. the bias gradient vs 70 us + a column-sum pass; the plain GEMM (no epilogue work) is still faster in cuBLAS
-(35 us vs 39 us), which is why only the fused uses are routed here. Numbers: profiles/gemm_tcgen05.md.
+accumulator in registers and the activation applied in the epilogue; ``linear_gelu`` / ``mlp_gelu`` are the autograd
+forms (the pre-activation is written by the same kernel; the backward GEMM applies gelu' and accumulates the bias
+gradient in its epilogue). The GPT-2 MLP uses ``mlp_gelu`` by default (``ADAPCC_TCGEN05_MLP=0`` restores cuBLAS +
+separate activation kernels; the variable keeps its original name so existing launch scripts still work).
 """
 from __future__ import annotations
 
@@ -27,7 +25,7 @@ def _lib():
     lib = load_library()
     if not _bound:
         lib.adapcc_gemm_bias_act_v.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p]
-        lib.adapcc_gemm_pp.argtypes = [c_void_p] * 6 + [c_int] * 4 + [c_void_p]
+        lib.adapcc_gemm_pp.argtypes = [c_void_p] * 7 + [c_int] * 4 + [c_void_p]
         _bound = True
     return lib
 
@@ -38,11 +36,10 @@ def supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
 
 
 def default_variant() -> int:
-    """0: one output tile per CTA. 1: persistent CTAs with a double-buffered TMEM accumulator. 2: CTA pairs
-    (``tcgen05.mma.cta_group::2``, 256 x 256 tile per pair). 3 (default): persistent CTA pairs + double-buffered TMEM +
-    coalescing epilogue (csrc/gemm_tcgen05_pp.cu), the only one that beats cuBLAS + separate activation kernel
-    (profiles/gemm_tcgen05.md); shapes it does not cover (N % 256 != 0) fall back to variant 1. All four pass the numerics
-    tests on B200."""
+    """0: one output tile per CTA. 1: persistent CTAs. 2: two-CTA clusters that share the W slab by TMA multicast,
+    one 256 x 256 tile per cluster. 3 (default): persistent two-CTA clusters, the only variant with the column-sum
+    output the MLP backward uses; shapes it does not cover (N % 256 != 0) go to variant 1. All four are checked against
+    fp32 references by the GPU tests (tests/test_gpu_tcgen05*.py; the file names predate the H100 port)."""
     return int(os.environ.get("ADAPCC_TCGEN05_VARIANT", "3"))
 
 
@@ -52,11 +49,10 @@ def linear_act(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
                colsum: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
     """-> (result, pre-activation or None). x [..., K], weight [N, K], bias [N]; bf16.
 
-    act "none" / "gelu": result = act(x @ weight.T + bias), optionally also the pre-activation (validated on B200).
+    act "none" / "gelu": result = act(x @ weight.T + bias), optionally also the pre-activation.
     act "dgelu":    result = (x @ weight.T) * gelu'(aux)      — the MLP backward with the activation's derivative in
                     the epilogue (aux = the saved pre-activation, same shape as the result).
-    act "residual": result = x @ weight.T + bias + aux        — projection with the residual add in the epilogue.
-    (All modes validated on B200: tests/test_gpu_tcgen05.py, tests/test_gpu_tcgen05_pp.py.)"""
+    act "residual": result = x @ weight.T + bias + aux        — projection with the residual add in the epilogue."""
     if not supported(x, weight):
         raise NativeError("linear_act: needs bf16 CUDA tensors with K % 64 == 0 and N % 128 == 0")
     n, k = weight.shape
@@ -67,8 +63,7 @@ def linear_act(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
     out = torch.empty(m, n, dtype=torch.bfloat16, device=x.device)
     v_req = default_variant() if variant is None else int(variant)
     if v_req == 3 and n % 256 == 0 and code <= 2:
-        # variant 3 (csrc/gemm_tcgen05_pp.cu): persistent CTA pairs, double-buffered TMEM, coalescing epilogue;
-        # act "dgelu" can also accumulate the column sums of its result (the up-projection's bias gradient)
+        # variant 3: persistent two-CTA clusters; act "dgelu" can also accumulate the column sums of its result (the up-projection's bias gradient)
         if code == 2:
             if aux is None or aux.numel() != m * n or aux.dtype != torch.bfloat16:
                 raise NativeError("linear_act(dgelu): aux must be a bf16 tensor with the result's shape")
@@ -78,10 +73,13 @@ def linear_act(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
         if colsum is not None and (code != 2 or colsum.dtype != torch.float32 or colsum.numel() != n):
             raise NativeError("linear_act: colsum is an fp32 [N] accumulator of the dgelu mode")
         b = bias.contiguous() if bias is not None else None
+        # per-row-tile column sums, added in a fixed order by the library: the same inputs give the same bits
+        work = torch.empty((m + 127) // 128, n, dtype=torch.float32, device=x.device) if colsum is not None else None
         rc = _lib().adapcc_gemm_pp(c_void_p(x2.data_ptr()), c_void_p(w.data_ptr()),
                                    c_void_p(b.data_ptr() if b is not None else 0), c_void_p(out.data_ptr()),
                                    c_void_p(pre.data_ptr() if pre is not None else 0),
-                                   c_void_p(colsum.data_ptr() if colsum is not None else 0), m, n, k, code,
+                                   c_void_p(colsum.data_ptr() if colsum is not None else 0),
+                                   c_void_p(work.data_ptr() if work is not None else 0), m, n, k, code,
                                    c_void_p(torch.cuda.current_stream().cuda_stream))
         if rc != 0:
             raise NativeError(f"gemm_pp failed: {last_error()}")
@@ -90,7 +88,7 @@ def linear_act(x: torch.Tensor, weight: torch.Tensor, bias: Optional[torch.Tenso
     if colsum is not None:
         raise NativeError("linear_act: colsum needs variant 3 (N % 256 == 0)")
     if v_req == 3:
-        v_req = 1                                       # shapes variant 3 does not cover: the persistent 1-CTA kernel
+        v_req = 1                                       # shapes variant 3 does not cover: persistent single CTAs
     if code >= 2:
         if aux is None or aux.numel() != m * n or aux.dtype != torch.bfloat16:
             raise NativeError(f"linear_act({act}): aux must be a bf16 tensor with the result's shape")
@@ -127,7 +125,7 @@ class _LinearGeluFn(torch.autograd.Function):
 
 
 def linear_gelu(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor) -> torch.Tensor:
-    """gelu_tanh(x @ weight.T + bias) with the bias and activation in the tcgen05 GEMM's epilogue."""
+    """gelu_tanh(x @ weight.T + bias) with the bias and activation in the GEMM's epilogue."""
     return _LinearGeluFn.apply(x, weight, bias)
 
 
@@ -164,5 +162,5 @@ class _MLPFn(torch.autograd.Function):
 
 
 def mlp_gelu(x, w1, b1, w2, b2):
-    """Transformer MLP ``linear(gelu(linear(x)))`` with both activation passes fused into tcgen05 GEMM epilogues."""
+    """Transformer MLP ``linear(gelu(linear(x)))`` with both activation passes fused into GEMM epilogues."""
     return _MLPFn.apply(x, w1, b1, w2, b2)

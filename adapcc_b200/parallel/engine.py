@@ -1,4 +1,4 @@
-"""Flat-buffer data-parallel training engine (the B200-native fast path next to the DDP hook).
+"""Flat-buffer data-parallel training engine (the native fast path next to the DDP hook).
 
 The reference drives gradient communication through torch DDP buckets and a *blocking* hook
 (/root/reference/train_ddp.py:35-41, /root/reference/commu.py:385-435). This engine keeps the same

@@ -1,4 +1,4 @@
-"""CPU reference executor: interprets the same tree roles / work items as the sm_100a tree kernel,
+"""CPU reference executor: interprets the same tree roles / work items as the sm_90a tree kernel,
 over ``torch.distributed`` point-to-point (gloo). It is (a) the oracle GPU tests compare against,
 (b) the plumbing path for BASELINE config 1 (world_size=2, strategy/4.xml, no GPU), and (c) the
 fallback data plane when a job runs with ``--backend gloo`` (the reference accepts that flag but

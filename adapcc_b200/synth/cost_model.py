@@ -57,12 +57,12 @@ class LinkModel:
 
 
 # One hop of the strategy-tree kernel costs more than a link latency: the parent polls the child's flag over NVLink
-# (a round trip), then pulls; measured 44 us for a one-chunk 6-hop all-reduce on 8xB200 -> ~3.5 alpha per hop.
+# (a round trip), then pulls; measured 44 us for a one-chunk 6-hop all-reduce on 8 B200 GPUs -> ~3.5 alpha per hop.
 TREE_HOP_ALPHAS = 3.5
 # The FIRST chunk of a lane crosses every hop at the rate of ONE CTA pulling over NVLink (512 threads x 16-byte loads,
 # latency-bound), not at the link rate; later chunks overlap across the kernel's lanes and stream at a fraction of the link
-# rate (flag polling and the staging passes share the ports). Both fitted on the 8xB200 measurements of the kernel with
-# 3 trees (round 2: profiles/raw/sweep_8xB200_r2.json) and 4 trees (round 1): every size 64 KB - 1 GiB within +-32 %.
+# rate (flag polling and the staging passes share the ports). Both fitted on 8-GPU B200 measurements of the kernel with
+# 3 trees (tests/golden/sweep_8xB200_r2.json) and 4 trees: every size 64 KB - 1 GiB within +-32 %.
 TREE_LANE_GBS = 30.0
 TREE_STREAM_EFF = 0.72
 
@@ -134,8 +134,8 @@ def strategy_time(strategy: Strategy, lm: LinkModel, total_bytes: float, chunk_b
                                   for t in strategy.trees)
 
 
-# Constants of the direct-algorithm model, calibrated on the committed 8xB200 sweep
-# (profiles/allreduce_sweep_8xB200_final.json; tests/test_synth.py checks the model against that file):
+# Constants of the direct-algorithm model, calibrated on an 8-GPU B200 sweep (not yet re-fitted for H100)
+# (tests/golden/allreduce_sweep_8xB200_final.json; tests/test_synth.py checks the model against that file):
 LAUNCH_US = 5.2            # fixed cost of one collective kernel (launch, first touch, last-block bookkeeping)
 BARRIER_ALPHAS = 1.5       # one per-CTA flag barrier = a peer store + a local poll ~ 1.5 link latencies
 STAGE_PASS_US = 3.3        # latency of one staging pass (stage-in or stage-out) over the window

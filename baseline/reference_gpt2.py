@@ -218,7 +218,7 @@ def run(a, ClockSampler=None) -> int:
                        "seq_len": seq, "parallelism": f"dp{world}", "engine": "torch DDP (stock, bucket_cap_mb=25)",
                        "optimizer": "torch.optim.AdamW(lr=%g, eps=1e-6, wd=0) + clip %.1f" % (hp["lr"], hp["max_norm"]),
                        "precision": precision, "attn_implementation": getattr(model.module.config, "_attn_implementation", None),
-                       "l2": "working set (params+grads+optimizer state ~2 GB/step) exceeds the 126 MB L2; no flush needed"},
+                       "l2": "working set (params+grads+optimizer state ~2 GB/step) exceeds the 50 MB L2; no flush needed"},
             "e2e": {"value": tokens / (ms_e2e * 1e-3), "unit": "tokens/s", "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "last_loss": last},
             "gpu_launches": 0, "clocks": clocks}), flush=True)

@@ -10,18 +10,22 @@ Per-GPU batch is fixed (weak scaling): B=4 (the reference's ``--train_batch_size
     python bench.py --gpus N --steps K --warmup W            # our arm
     python bench.py --impl reference ...                     # the unmodified reference (see DESIGN.md)
     python bench.py --impl nccl ...                          # same model/engine, NCCL all-reduce
+    python bench.py ... --dump-outputs DIR                   # also write the last timed step's results as .npy
 
-For N>1 launch under torchrun (the driver does); with no torchrun env and N>1 the script
-re-launches itself through ``python -m torch.distributed.run``.
+For N>1 launch under torchrun; with no torchrun env and N>1 the script re-launches itself through
+``python -m torch.distributed.run``. Nothing is written inside the repository: the library's work
+directory (strategy / topology files) is a fresh temporary directory.
 """
 from __future__ import annotations
 
 import argparse
 import json
 import os
+import shutil
 import statistics
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 from types import SimpleNamespace
@@ -62,11 +66,38 @@ def parse():
     ap.add_argument("--allow_cpu", action="store_true", help="--impl reference only: gloo/CPU plumbing test")
     ap.add_argument("--no_nccl_arm", action="store_true",
                     help="skip the in-process NCCL arm (same engine, same buckets) that fills vs_baseline at N > 1")
-    return ap.parse_args()
+    ap.add_argument("--dump-outputs", dest="dump_outputs", default=None, metavar="DIR",
+                    help="after the device-timed steps, write what the last of them computed to DIR/<name>.npy: the "
+                         "loss, and a fixed seeded sample of the updated parameters and of the gradients (float32)")
+    a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be at least 1")
+    return a
+
+
+DUMP_SAMPLE = 1 << 22          # elements sampled from the parameter and gradient vectors (2 x 16 MB as float32)
+
+
+def dump_outputs(path, loss, params, grads):
+    """``loss`` (float32 [1]) and the same seeded ``DUMP_SAMPLE`` positions of the flat parameter and gradient vectors
+    (float32), so two builds run with the same arguments can be compared output for output."""
+    import numpy as np
+    import torch
+
+    os.makedirs(path, exist_ok=True)
+    np.save(os.path.join(path, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    flat_p = torch.cat([p.detach().reshape(-1) for p in params])
+    g = torch.Generator(device="cpu").manual_seed(0)
+    idx = torch.randint(0, flat_p.numel(), (min(DUMP_SAMPLE, flat_p.numel()),), generator=g).sort().values
+    idx = idx.to(flat_p.device)
+    np.save(os.path.join(path, "params_sample.npy"), flat_p[idx].float().cpu().numpy())
+    if grads is not None:
+        flat_g = torch.cat([x.detach().reshape(-1) for x in grads])
+        np.save(os.path.join(path, "grads_sample.npy"), flat_g[idx].float().cpu().numpy())
 
 
 class ClockSampler:
-    """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """Samples nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -189,7 +220,10 @@ def main():
     n_params = model.num_parameters()
 
     # ---- the library's public API: AdapCC.init -> setup -> communicator ---------------------------
-    work = os.path.join(ROOT, "gpurun_out", "bench_work")
+    work = [tempfile.mkdtemp(prefix="adapcc_bench_") if rank == 0 else None]
+    if world > 1:
+        dist.broadcast_object_list(work, src=0)     # one shared work directory for all ranks
+    work = work[0]
     os.makedirs(os.path.join(work, "strategy"), exist_ok=True)
     grad_bytes = n_params * 2
     args = SimpleNamespace(port=5000, strategy_file=os.path.join(work, "strategy", f"bench_{world}.xml"),
@@ -302,10 +336,18 @@ def main():
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     for _ in range(a.steps):
-        step_dev()
+        loss_dev = step_dev()
     e1.record()
     barrier()
     launches = lib.adapcc_launch_count() - c0
+    if a.dump_outputs and rank == 0:
+        # the graph replay returns nothing: its loss lives in the engine's static output
+        if engine is not None:
+            loss_dev = engine._static_loss if use_graph else loss_dev
+            dump_outputs(a.dump_outputs, loss_dev, [engine.flat_param], [engine.flat_grad])
+        else:
+            ps = [p for p in model.parameters()]
+            dump_outputs(a.dump_outputs, loss_dev, ps, [p.grad if p.grad is not None else torch.zeros_like(p) for p in ps])
     if use_graph and engine is not None:
         launches = engine.native_launches_per_step * a.steps
     ms_dev = max_over_ranks(e0.elapsed_time(e1) / a.steps)
@@ -368,13 +410,13 @@ def main():
                        "optimizer": "adamw+clip1.0 (fused)", "grad_dtype": "bf16", "zero_copy_grads": zero_copy,
                        "buckets": n_buckets, "zero1": zero1_flag,
                        "lm_rows": a.lm_rows, "lm_chunk_rows": cfg.lm_chunk_rows, "relay_control": bool(a.relay_control and a.engine == "ddp"),
-                       "mlp": {0: "cublas + activation kernels", 1: "tcgen05 fused fwd", 2: "tcgen05 fused fwd+bwd"}.get(
+                       "mlp": {0: "cublas + activation kernels", 1: "wgmma fused fwd", 2: "wgmma fused fwd+bwd"}.get(
                            getattr(model.module.h[0] if hasattr(model, "module") else model.h[0], "tc_mlp", 0), "?"),
                        "fuse_add_ln": bool(getattr(model, "fuse_add_ln", False)),
-                       "l2": "working set (params+grads+optimizer state ~2 GB/step) exceeds the 126 MB L2; no flush needed"},
+                       "l2": "working set (params+grads+optimizer state ~2 GB/step) exceeds the 50 MB L2; no flush needed"},
             "e2e": {"value": tokens_per_step / (ms_e2e * 1e-3), "unit": "tokens/s", "ms_per_step": ms_e2e,
                     "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4, "last_loss": last},
-            "gpu_launches": int(launches), "clocks": clocks,
+            "gpu_launches": int(launches), "clocks": clocks, "device": torch.cuda.get_device_name(dev),
         }
         if allreduce_check is not None:
             out["allreduce_check"] = allreduce_check
@@ -392,6 +434,8 @@ def main():
     if world > 1:
         dist.barrier()
         dist.destroy_process_group()
+    if rank == 0:
+        shutil.rmtree(work, ignore_errors=True)
     return 0
 
 

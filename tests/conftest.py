@@ -7,16 +7,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-REFERENCE = "/root/reference"
-
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with -m gpu)")
 
 
 @pytest.fixture(scope="session")
-def reference_dir():
-    return REFERENCE if os.path.isdir(REFERENCE) else None
+def reference_strategy_dir():
+    """The reference project's strategy XML files (its own dialect included), stored as test data."""
+    return os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "reference_strategy")
 
 
 # The reference's 4-GPU sample strategy (same topology as /root/reference/strategy/4.xml), including

@@ -416,8 +416,9 @@ def test_reference_c_abi_symbols(dev, tmp_path, monkeypatch):
 
 
 def test_fused_embedding_sum_matches_torch(dev):
-    """One-kernel embedding sum and its sort-free backward (fp32 accumulation of duplicate rows, in-place add into an
-    existing gradient) against F.embedding on fp32 copies; two rounds: the work buffers must come back clean."""
+    """One-kernel embedding sum and its sort-free backward (fixed-point accumulation of duplicate rows, in-place add
+    into an existing gradient) against F.embedding on fp32 copies; two rounds: the work buffers must come back clean;
+    the same backward repeated gives the same bits."""
     from adapcc_b200.ops import fused_embedding_sum
 
     torch.manual_seed(5)
@@ -445,6 +446,11 @@ def test_fused_embedding_sum_matches_torch(dev):
         untouched[ids.reshape(-1)] = False
         untouched[tt.reshape(-1)] = False
         assert torch.all(wte.grad[untouched] == 0)
+        first = (wte.grad.clone(), wpe.grad.clone())
+        for _ in range(3):
+            wte.grad = wpe.grad = None
+            fused_embedding_sum([wte, wpe], [(0, ids), (1, pos), (0, tt)]).backward(dy)
+            assert torch.equal(wte.grad, first[0]) and torch.equal(wpe.grad, first[1])
 
 
 def test_fused_ce_grad_scale(dev):
@@ -461,3 +467,28 @@ def test_fused_ce_grad_scale(dev):
     lb = fused_ce_(b, labels, vocab, grad_scale=scale)
     assert torch.equal(la, lb)                                       # row losses are not scaled
     assert torch.allclose(b.float(), a.float() * 0.125, atol=2e-3, rtol=2e-2)
+
+
+def test_causal_attention_backward_is_repeatable(dev):
+    """GPT-2's attention: same gradients as plain SDPA (up to bf16 rounding), identical bits on every repetition, and
+    PyTorch's deterministic-algorithms setting left as it was."""
+    from adapcc_b200.models.gpt2 import causal_attention
+
+    torch.manual_seed(9)
+    q, k, v = (torch.randn(4, 12, 512, 64, device=dev).bfloat16().requires_grad_(True) for _ in range(3))
+    do = torch.randn(4, 12, 512, 64, device=dev).bfloat16()
+    F = torch.nn.functional
+    F.scaled_dot_product_attention(q, k, v, is_causal=True).backward(do)
+    ref = [t.grad.clone() for t in (q, k, v)]
+    first = None
+    for _ in range(4):
+        for t in (q, k, v):
+            t.grad = None
+        causal_attention(q, k, v).backward(do)
+        got = [t.grad.clone() for t in (q, k, v)]
+        for a, b in zip(got, ref):
+            assert torch.allclose(a.float(), b.float(), atol=2e-2, rtol=2e-2)
+        if first is None:
+            first = got
+        assert all(torch.equal(a, b) for a, b in zip(got, first))
+    assert not torch.are_deterministic_algorithms_enabled()

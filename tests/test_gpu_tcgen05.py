@@ -1,15 +1,13 @@
-"""tcgen05 GEMM with fused bias + GELU epilogue (csrc/gemm_tcgen05.cu) against a plain PyTorch fp32 reference.
-Variant 0 passed on B200 for every shape below except the last (added afterwards: the full GPT-2 c_fc shape, 768 CTAs
-of the same per-tile kernel) and for the autograd test — log/gpu_tcgen05_test.log."""
+"""wgmma GEMM with fused bias + GELU epilogue (csrc/gemm_wgmma.cu) against a plain PyTorch fp32 reference: ragged M,
+both tile widths, K up to 3072, the full GPT-2 c_fc shape, the aux epilogues and autograd."""
 import os
 
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
-# variants 0 (tile per CTA), 1 (persistent CTAs, double-buffered TMEM) and 2 (CTA pairs, cta_group::2) all passed on
-# B200 (round 2, gpurun call 1: gpurun_out/c1_tcgen05_v*.log); variant 3 (persistent pairs + coalescing epilogue,
-# csrc/gemm_tcgen05_pp.cu) is tested in tests/test_gpu_tcgen05_pp.py
+# variants 0 (tile per CTA), 1 (persistent CTAs) and 2 (two-CTA clusters sharing W by TMA multicast); variant 3
+# (persistent two-CTA clusters, column-sum output) is tested in tests/test_gpu_tcgen05_pp.py
 VARIANTS = [int(v) for v in os.environ.get("ADAPCC_TCGEN05_TEST_VARIANTS", "0,1,2").split(",") if v.strip()]
 
 

@@ -1,6 +1,6 @@
-"""tcgen05 GEMM variant 3 — persistent CTA pairs, double-buffered TMEM accumulator, coalescing epilogue
-(csrc/gemm_tcgen05_pp.cu) — against plain PyTorch fp32 references: identity / GELU(+pre) / dGELU(+column sums),
-ragged M, one to many tiles per pair, and the fused MLP autograd path built on it."""
+"""wgmma GEMM variant 3 — persistent two-CTA clusters sharing the W slab by TMA multicast (csrc/gemm_wgmma.cu) —
+against plain PyTorch fp32 references: identity / GELU(+pre) / dGELU(+column sums), ragged M, one to many tiles per
+cluster, and the fused MLP autograd path built on it."""
 import pytest
 import torch
 
@@ -50,6 +50,10 @@ def test_pp_dgelu_and_colsum(dev, m, n, k):
     assert torch.allclose(got.float(), want, atol=4e-2, rtol=3e-2), (got.float() - want).abs().max()
     ref_cs = got.float().sum(0)                                   # sums of the bf16 values the kernel wrote
     assert torch.allclose(colsum, ref_cs, atol=2e-2 * max(1.0, float(ref_cs.abs().max())), rtol=1e-2)
+    for _ in range(3):                                            # the column sums are added in a fixed order
+        again = torch.zeros_like(colsum)
+        got2, _ = linear_act(x, w, None, "dgelu", aux=aux, colsum=again, variant=3)
+        assert torch.equal(got2, got) and torch.equal(again, colsum)
 
 
 def test_pp_fused_mlp_autograd(dev, monkeypatch):

@@ -94,16 +94,14 @@ def test_cost_model_orders_algorithms():
 
 
 def test_cost_model_tracks_the_measured_8xb200_sweep():
-    """The direct-algorithm model against the committed measurement (profiles/allreduce_sweep_8xB200_final.json, alpha
-    and bandwidth as the native profiler reports them on that box): every (algorithm, size, staged / zero-copy) time
-    within 35 %, and the algorithm it picks within 5 % of the fastest measured one at every size."""
+    """The direct-algorithm model against the sweep its constants were fitted to (tests/golden/
+    allreduce_sweep_8xB200_final.json, alpha and bandwidth as the native profiler reported them on that 8-GPU box):
+    every (algorithm, size, staged / zero-copy) time within 35 %, and the algorithm it picks within 5 % of the fastest
+    measured one at every size."""
     import json
     import os
 
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles",
-                        "allreduce_sweep_8xB200_final.json")
-    if not os.path.exists(path):
-        pytest.skip("measurement file not present")
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "allreduce_sweep_8xB200_final.json")
     rows = [r for r in json.load(open(path))["rows"] if "two_shot" in r]
     assert len(rows) >= 6
     lm = LinkModel.uniform(8, 2.0, 700.0)
@@ -120,8 +118,8 @@ def test_cost_model_tracks_the_measured_8xb200_sweep():
 
 
 def test_tree_cost_model_against_the_measured_tree_kernel():
-    """The strategy-tree kernel on 8xB200 with 256 KB device chunks, rotated binary trees: 4 trees (round 1,
-    profiles/allreduce_sweep_8xB200.md, column `tree`) and 3 trees (round 2, profiles/raw/sweep_8xB200_r2.json). The model
+    """The strategy-tree kernel on 8 GPUs (the 8xB200 sweeps the model was fitted to) with 256 KB device chunks, rotated
+    binary trees: 4 trees and 3 trees (tests/golden/sweep_8xB200_r2.json). The model
     (one-CTA lane rate for the first chunk of a lane, a streaming efficiency for the rest) is within 35 % at every size
     from 64 KB to 1 GiB — including the 1-16 MB plateau the link-rate model missed by 3x — and never makes a tree win on
     a uniform switch."""
@@ -140,21 +138,20 @@ def test_tree_cost_model_against_the_measured_tree_kernel():
             ratio = strategy_time(s, lm, nbytes, 256 << 10) * 1e6 / m
             assert 0.74 < ratio < 1.35, (nt, nbytes, ratio)
             assert pick_algorithm(lm, nbytes, strategy=s, chunk_bytes=256 << 10) != "tree"
-    # if present, the round-2 measurement file itself (same numbers, read from the committed JSON)
+    # the 3-tree measurement file itself (same numbers, read from the stored JSON)
     import json
     import os
 
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "profiles", "raw", "sweep_8xB200_r2.json")
-    if os.path.exists(path):
-        d = json.load(open(path))
-        rows = [r for r in d.get("sweep", d.get("rows", [])) if "tree" in r and "nccl" in r]    # not the CTA-count rows
-        s = make_strategy(8, 3, "binary")
-        seen = 0
-        for r in rows:
-            ratio = strategy_time(s, lm, r["bytes"], 256 << 10) / r["tree"]
-            assert 0.74 < ratio < 1.35, (r["bytes"], ratio)
-            seen += 1
-        assert seen >= 6
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "sweep_8xB200_r2.json")
+    d = json.load(open(path))
+    rows = [r for r in d.get("sweep", d.get("rows", [])) if "tree" in r and "nccl" in r]    # not the CTA-count rows
+    s = make_strategy(8, 3, "binary")
+    seen = 0
+    for r in rows:
+        ratio = strategy_time(s, lm, r["bytes"], 256 << 10) / r["tree"]
+        assert 0.74 < ratio < 1.35, (r["bytes"], ratio)
+        seen += 1
+    assert seen >= 6
 
 
 def test_multiround_broadcast_milp():
@@ -172,7 +169,7 @@ def test_multiround_broadcast_milp():
 
 
 def test_synth_cli_shape_and_measured_profile(tmp_path):
-    """``python -m adapcc_b200.synth``: nominal server shapes, and the measured 4xB200 profile shipped in topology/."""
+    """``python -m adapcc_b200.synth``: nominal server shapes, and a measured 4-GPU profile (tests/golden/measured_4xB200)."""
     from adapcc_b200.synth.__main__ import main
 
     out = tmp_path / "s" / "shape.xml"
@@ -180,11 +177,10 @@ def test_synth_cli_shape_and_measured_profile(tmp_path):
     s = Strategy.from_file(str(out), 6)
     s.validate(6)
     assert len(s.trees) == 2 and {t.root for t in s.trees} == {0, 4}          # one root per server (parity rule)
-    prof = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "topology", "measured_4xB200")
-    if os.path.isdir(prof):
-        out2 = tmp_path / "m.xml"
-        assert main(["--profile-dir", prof, "--policy", "par-trees", "--out", str(out2)]) == 0
-        Strategy.from_file(str(out2), 4).validate(4)
+    prof = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "measured_4xB200")
+    out2 = tmp_path / "m.xml"
+    assert main(["--profile-dir", prof, "--policy", "par-trees", "--out", str(out2)]) == 0
+    Strategy.from_file(str(out2), 4).validate(4)
 
 
 def test_algorithm_plan_bands_follow_the_profile():
@@ -269,7 +265,7 @@ def test_plan_encoding_and_pick_properties():
 
 
 def test_cost_model_report_reproduces_from_the_committed_sweeps(tmp_path):
-    """tools/cost_model_report.py on profiles/raw/sweep_{8,2}xB200_r2.json: at every measured size the plan's pick is the
+    """tools/cost_model_report.py on tests/golden/sweep_{8,2}xB200_r2.json: at every measured size the plan's pick is the
     fastest measured variant or within 3 % of it (staged and heap tensors, 8 GPUs where the model was fitted and 2 GPUs
     as a hold-out)."""
     import importlib.util
@@ -277,8 +273,6 @@ def test_cost_model_report_reproduces_from_the_committed_sweeps(tmp_path):
     import re
 
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    if not os.path.exists(os.path.join(root, "profiles", "raw", "sweep_8xB200_r2.json")):
-        pytest.skip("measurement files not present")
     spec = importlib.util.spec_from_file_location("cost_model_report", os.path.join(root, "tools", "cost_model_report.py"))
     mod = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(mod)

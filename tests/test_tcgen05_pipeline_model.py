@@ -1,14 +1,18 @@
-"""Model check of the persistent tcgen05 GEMM's barrier protocol (csrc/gemm_tcgen05.cu, variant 1) on CPU.
+"""Model check, on CPU, of the mbarrier protocol of the GEMM in csrc/gemm_wgmma.cu (the file name predates the port).
 
-The kernel's three roles — TMA producer, MMA issuer, four epilogue warps — synchronise only through mbarriers
-(phase-parity waits, expect_tx / complete_tx, tcgen05.commit arrivals) with hand-computed stage / phase indices.
-This reproduces exactly those index computations as coroutines over a small mbarrier model, with an asynchronous
-"TMA engine" and an in-order asynchronous "tensor core", under random schedules, and checks that
-  * a shared-memory stage is never overwritten before the MMAs reading it have executed,
-  * an accumulator is never written while the epilogue still drains it, and every epilogue sees exactly the
-    K-slabs of its own tile,
+Per CTA: one TMA producer thread and two consumer warpgroups, synchronised only through mbarriers with hand-computed
+stage / phase indices. `full[s]` completes on the transferred bytes (expect_tx / complete_tx); `empty[s]` counts one
+arrival per consumer warpgroup of EVERY CTA of the cluster. In a two-CTA cluster each producer loads its own A slab and
+half of the W slab, which it multicasts into the same stage of both CTAs — so bytes may complete on a CTA's `full[s]`
+before its own producer has posted expect_tx, and a stage may only be refilled once the consumers of both CTAs have
+released it. A consumer keeps one wgmma group in flight and releases a stage when the group that read it has retired.
+This reproduces those index computations as coroutines over a small mbarrier model, with an asynchronous TMA engine
+(completions in any order) and an asynchronous tensor core per consumer, under random schedules, and checks that
+  * a stage is never overwritten before every wgmma reading it has executed,
+  * every wgmma reads exactly its own tile's and K-slab's A rows and both halves of its W slab,
   * nothing deadlocks.
-A deliberately wrong parity (the classic off-by-one) must be caught."""
+Deliberately wrong variants (a wrong phase parity, a release before the wgmma group retired, a release to the local CTA
+only) must be caught."""
 import random
 from collections import deque
 
@@ -40,90 +44,100 @@ class MBar:
         return self.phase != parity
 
 
-def simulate(tiles_per_cta, num_kb, seed, bug=None, max_steps=300_000):
+def simulate(tiles, num_kb, seed, cluster=1, bug=None, max_steps=400_000):
+    """`tiles` per CTA (cluster); bug: None, "producer_parity", "acc_parity" (a consumer releases a stage as soon as its
+    wgmma group is committed, while the group in flight still reads it) or "local_release" (consumers arrive only on
+    their own CTA's `empty`, which then counts 2)."""
     rng = random.Random(seed)
-    full = [MBar(1) for _ in range(STAGES)]
-    empty = [MBar(1) for _ in range(STAGES)]
-    acc_full = [MBar(1) for _ in range(2)]
-    acc_empty = [MBar(4) for _ in range(2)]
-    smem = [None] * STAGES                   # (tile, kb) currently held by a stage
-    acc = [[], []]                           # K-slabs accumulated into each TMEM accumulator
-    acc_readers = [0, 0]                     # epilogue warps currently reading an accumulator
-    tma_q, tc_q = deque(), deque()           # asynchronous engines
+    C, CONS = cluster, 2
+    per_cta = CONS if bug == "local_release" else CONS * C
+    full = [[MBar(1) for _ in range(STAGES)] for _ in range(C)]
+    empty = [[MBar(per_cta) for _ in range(STAGES)] for _ in range(C)]
+    smem_a = [[None] * STAGES for _ in range(C)]                  # [cta][stage] -> (tile, kb, cta)
+    smem_w = [[[None] * C for _ in range(STAGES)] for _ in range(C)]  # [cta][stage][half] -> (tile, kb)
+    tma_q = []
+    tc_q = {(r, c): deque() for r in range(C) for c in range(CONS)}   # in-order wgmma groups per consumer
     seen = []
 
-    def producer():
+    def producer(r):
         it = 0
-        for tile in range(tiles_per_cta):
+        for t in range(tiles):
             for kb in range(num_kb):
                 s, ph = it % STAGES, (it // STAGES) & 1
                 want = ph ^ 1 if bug != "producer_parity" else ph
-                while not empty[s].done(want):
+                while not empty[r][s].done(want):
                     yield
-                full[s].arrive(expect_tx=2)
-                tma_q.append((s, (tile, kb)))             # A slab
-                tma_q.append((s, (tile, kb)))             # W slab
+                full[r][s].arrive(expect_tx=2 + 2)                # A (2 units) + the whole W slab (2 units)
+                tma_q.append(("A", r, s, (t, kb, r)))
+                if C == 1:
+                    tma_q.append(("W", r, s, (t, kb)))
+                else:
+                    tma_q.append(("Wh", r, s, (t, kb)))           # half r, multicast to every CTA
                 it += 1
                 yield
 
-    def mma():
+    def consumer(r, c):
+        q = tc_q[(r, c)]
         it = 0
-        for local in range(tiles_per_cta):
-            a, aph = local & 1, (local >> 1) & 1
-            want = aph ^ 1 if bug != "acc_parity" else aph
-            while not acc_empty[a].done(want):
-                yield
+
+        def release(s):
+            for d in ([r] if bug == "local_release" or C == 1 else range(C)):
+                empty[d][s].arrive()
+
+        for t in range(tiles):
+            prev = None
             for kb in range(num_kb):
                 s, ph = it % STAGES, (it // STAGES) & 1
-                while not full[s].done(ph):
+                while not full[r][s].done(ph):
                     yield
-                tc_q.append(("mma", s, a, (local, kb), kb == 0))
-                tc_q.append(("commit", empty[s]))
+                q.append((s, (t, kb)))                            # wgmma group reading stage s
+                if bug == "acc_parity":
+                    release(s)
+                else:
+                    while len(q) > 1:                             # wgmma.wait_group 1
+                        yield
+                    if prev is not None:
+                        release(prev)
+                    prev = s
                 it += 1
                 yield
-            tc_q.append(("commit", acc_full[a]))
-            yield
-
-    def epilogue(warp):
-        for local in range(tiles_per_cta):
-            a, aph = local & 1, (local >> 1) & 1
-            while not acc_full[a].done(aph):
+            while q:                                              # wgmma.wait_group 0
                 yield
-            acc_readers[a] += 1
-            for _ in range(2):                            # column chunks
-                got = list(acc[a])
-                assert got == [(local, kb) for kb in range(num_kb)], f"warp {warp} tile {local}: accumulator holds {got}"
-                yield
-            acc_readers[a] -= 1
-            seen.append((warp, local))
-            acc_empty[a].arrive()
+            if prev is not None and bug != "acc_parity":
+                release(prev)
+            seen.append((r, c, t))
             yield
 
     def tma_engine():
         while True:
             if tma_q and rng.random() < 0.6:
-                s, what = tma_q.popleft()
-                smem[s] = what                            # a late overwrite is caught when the MMA executes
-                full[s].complete_tx(1)
-            yield
-
-    def tensor_core():
-        while True:
-            if tc_q and rng.random() < 0.6:
-                op = tc_q.popleft()
-                if op[0] == "commit":
-                    op[1].arrive()
+                op = tma_q.pop(rng.randrange(min(len(tma_q), 4)))  # completions in any order
+                kind, r, s, what = op
+                if kind == "A":
+                    smem_a[r][s] = what
+                    full[r][s].complete_tx(2)
+                elif kind == "W":
+                    smem_w[r][s][0] = what
+                    full[r][s].complete_tx(2)
                 else:
-                    _, s, a, what, first = op
-                    assert smem[s] == what, f"MMA for {what} found {smem[s]} in stage {s}"
-                    assert acc_readers[a] == 0, f"MMA for {what} writes accumulator {a} while it is being drained"
-                    if first:
-                        acc[a] = []
-                    acc[a].append(what)
+                    for d in range(C):
+                        smem_w[d][s][r] = what
+                        full[d][s].complete_tx(1)
             yield
 
-    roles = {"producer": producer(), "mma": mma(), **{f"epi{w}": epilogue(w) for w in range(4)}}
-    engines = [tma_engine(), tensor_core()]
+    def tensor_core(r, c):
+        q = tc_q[(r, c)]
+        while True:
+            if q and rng.random() < 0.5:
+                s, (t, kb) = q[0]
+                assert smem_a[r][s] == (t, kb, r), f"CTA {r} wgmma for {(t, kb)} found A {smem_a[r][s]} in stage {s}"
+                assert smem_w[r][s] == [(t, kb)] * C, f"CTA {r} wgmma for {(t, kb)} found W {smem_w[r][s]} in stage {s}"
+                q.popleft()
+            yield
+
+    roles = {f"p{r}": producer(r) for r in range(C)}
+    roles.update({f"c{r}{c}": consumer(r, c) for r in range(C) for c in range(CONS)})
+    engines = [tma_engine()] + [tensor_core(r, c) for r in range(C) for c in range(CONS)]
     steps = 0
     while roles:
         steps += 1
@@ -138,7 +152,7 @@ def simulate(tiles_per_cta, num_kb, seed, bug=None, max_steps=300_000):
             except StopIteration:
                 del roles[name]
                 break
-    assert sorted(seen) == sorted((w, t) for w in range(4) for t in range(tiles_per_cta))
+    assert sorted(seen) == sorted((r, c, t) for r in range(C) for c in range(CONS) for t in range(tiles))
 
 
 @pytest.mark.parametrize("tiles,num_kb", [(1, 1), (1, 12), (2, 3), (5, 12), (7, 5), (6, 48)])
@@ -149,6 +163,8 @@ def test_persistent_pipeline_indices_are_consistent(tiles, num_kb):
 
 @pytest.mark.parametrize("bug", ["producer_parity", "acc_parity"])
 def test_model_catches_a_wrong_parity(bug):
+    """producer_parity: the producer waits on the wrong phase of `empty`; acc_parity: a consumer releases a stage while
+    its in-flight wgmma group still reads it."""
     caught = 0
     for seed in range(10):
         try:
@@ -158,100 +174,28 @@ def test_model_catches_a_wrong_parity(bug):
     assert caught == 10
 
 
-def simulate_pair(num_kb, seed, stages=6, bug=None, max_steps=200_000):
-    """Variant 2 (CTA pair): both CTAs produce, only the leader issues MMAs; the leader's full[s] counts the TMA bytes
-    of both CTAs, commits arrive on empty[s] / acc_full of BOTH CTAs at once (multicast)."""
-    rng = random.Random(seed)
-    full = [MBar(1) for _ in range(stages)]                       # leader's copy only
-    empty = [[MBar(1) for _ in range(stages)] for _ in range(2)]
-    acc_full = [MBar(1), MBar(1)]
-    smem = [[None] * stages for _ in range(2)]                    # [cta][stage] -> kb held
-    acc = []
-    tma_q, tc_q = deque(), deque()
-    done = []
-
-    def producer(cta):
-        for kb in range(num_kb):
-            s, ph = kb % stages, (kb // stages) & 1
-            while not empty[cta][s].done(ph ^ 1 if bug != "pair_parity" else ph):
-                yield
-            if cta == 0:
-                full[s].arrive(expect_tx=4)                       # A and W slabs of both CTAs
-            tma_q.append((cta, s, kb))
-            tma_q.append((cta, s, kb))
-            yield
-
-    def mma():
-        for kb in range(num_kb):
-            s, ph = kb % stages, (kb // stages) & 1
-            while not full[s].done(ph):
-                yield
-            tc_q.append(("mma", s, kb))
-            tc_q.append(("commit", [empty[0][s], empty[1][s]]))
-            yield
-        tc_q.append(("commit", acc_full))
-        yield
-
-    def epilogue(cta):
-        while not acc_full[cta].done(0):
-            yield
-        assert acc == list(range(num_kb)), acc
-        done.append(cta)
-        yield
-
-    def tma_engine():
-        while True:
-            if tma_q and rng.random() < 0.6:
-                i = rng.randrange(min(len(tma_q), 3))             # the two CTAs' loads complete in any order
-                cta, s, kb = tma_q[i]
-                del tma_q[i]
-                smem[cta][s] = kb
-                full[s].complete_tx(1)
-            yield
-
-    def tensor_core():
-        while True:
-            if tc_q and rng.random() < 0.6:
-                op = tc_q.popleft()
-                if op[0] == "commit":
-                    for b in op[1]:
-                        b.arrive()
-                else:
-                    _, s, kb = op
-                    assert smem[0][s] == kb and smem[1][s] == kb, (kb, smem[0][s], smem[1][s])
-                    acc.append(kb)
-            yield
-
-    roles = {"p0": producer(0), "p1": producer(1), "mma": mma(), "e0": epilogue(0), "e1": epilogue(1)}
-    engines = [tma_engine(), tensor_core()]
-    steps = 0
-    while roles:
-        steps += 1
-        if steps > max_steps:
-            raise TimeoutError(f"deadlock: {sorted(roles)}")
-        for e in engines:
-            next(e)
-        name = rng.choice(sorted(roles))
-        for _ in range(rng.randint(1, 5)):
-            try:
-                next(roles[name])
-            except StopIteration:
-                del roles[name]
-                break
-    assert sorted(done) == [0, 1]
-
-
 @pytest.mark.parametrize("num_kb", [1, 5, 6, 12, 48])
 def test_cta_pair_protocol_is_consistent(num_kb):
     for seed in range(15):
-        simulate_pair(num_kb, seed)
+        simulate(3, num_kb, seed, cluster=2)
 
 
 def test_cta_pair_model_catches_a_wrong_parity():
     caught = 0
     for seed in range(10):
         try:
-            simulate_pair(24, seed, bug="pair_parity", max_steps=30_000)
+            simulate(3, 24, seed, cluster=2, bug="producer_parity", max_steps=30_000)
+        except (AssertionError, TimeoutError):
+            caught += 1
+    assert caught == 10
+
+
+def test_cluster_model_catches_a_release_to_the_local_cta_only():
+    """If consumers released a stage only in their own CTA, the peer's multicast could overwrite W under a wgmma."""
+    caught = 0
+    for seed in range(10):
+        try:
+            simulate(3, 24, seed, cluster=2, bug="local_release", max_steps=60_000)
         except (AssertionError, TimeoutError):
             caught += 1
     assert caught == 10

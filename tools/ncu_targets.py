@@ -51,8 +51,8 @@ def main():
         for _ in range(3):
             ln(xx).backward(torch.randn(8192, 768, device=dev).bfloat16())
     if which in ("all", "gemm"):
-        # the tcgen05 GEMM at the GPT-2 MLP up-projection shape, both variants
-        # (ncu -k regex:gemm_bias_act_tcgen05 --set full ... python tools/ncu_targets.py gemm [variants, e.g. 0,1])
+        # the wgmma GEMM at the GPT-2 MLP up-projection shape, both variants
+        # (ncu -k regex:gemm_bias_act_wgmma --set full ... python tools/ncu_targets.py gemm [variants, e.g. 0,1])
         from adapcc_b200.ops.gemm import linear_act
         variants = [int(t) for t in (sys.argv[2] if len(sys.argv) > 2 else "0").split(",")]
         a = torch.randn(8192, 768, device=dev).bfloat16()

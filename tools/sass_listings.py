@@ -1,6 +1,6 @@
 """Writes profiles/sass/<kernel>.sass: the full ``cuobjdump -sass`` listing of ONE instantiation per hot kernel family
 (the one the GPT-2 bench / the sweeps actually launch), so the instruction-level evidence — NVLS multimem ops, peer
-128-bit loads/stores, system-scope flag protocol, tcgen05 / TMA / TMEM — can be read next to the counts in
+128-bit loads/stores, system-scope flag protocol, wgmma / TMA / mbarrier — can be read next to the counts in
 profiles/sass_summary.md. Run on the build box (no GPU needed): ``python tools/sass_listings.py``."""
 import os
 import re
@@ -22,8 +22,8 @@ WANT = [
     ("allreduce_pipelined_two_shot_f32", r"allreduce_pipelined_kernel<float, float, 0, 2, 8>"),
     ("zero_adamw_bcast", r"zero_adamw_bcast_kernel"),
     ("moe_push", r"moe_push_kernel"),
-    ("gemm_pair_persistent_gelu", r"gemm_pair_persistent_kernel<1>"),
-    ("gemm_pair_persistent_dgelu", r"gemm_pair_persistent_kernel<2>"),
+    ("gemm_cluster_gelu", r"gemm_bias_act_wgmma_kernel<256, 1, 2>"),
+    ("gemm_cluster_dgelu", r"gemm_bias_act_wgmma_kernel<256, 2, 2>"),
     ("adamw_bf16", r"adamw_kernel<__nv_bfloat16, __nv_bfloat16>"),
     ("fused_ce_smem", r"fused_ce_smem_kernel"),
     ("embed_bwd_scatter", r"embed_bwd_scatter_kernel"),
@@ -38,7 +38,7 @@ def main():
     blocks = re.split(r"\n\s*Function : \S+\n", sass)[1:]
     out_dir = os.path.join(ROOT, "profiles", "sass")
     os.makedirs(out_dir, exist_ok=True)
-    index = ["# SASS listings (cuobjdump -sass adapcc_b200/_C/libadapcc.so, sm_100a), one instantiation per kernel family", ""]
+    index = ["# SASS listings (cuobjdump -sass adapcc_b200/_C/libadapcc.so, sm_90a), one instantiation per kernel family", ""]
     for fname, pat in WANT:
         for name, body in zip(names, blocks):
             if re.search(pat, name):

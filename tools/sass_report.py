@@ -30,13 +30,13 @@ def main():
             for k in KEYS:
                 if op.startswith(k):
                     d["c"][k] += 1
-    out = ["# SASS evidence (cuobjdump -sass adapcc_b200/_C/libadapcc.so, sm_100a)", "",
+    out = ["# SASS evidence (cuobjdump -sass adapcc_b200/_C/libadapcc.so, sm_90a)", "",
            "Counts are summed over all template instantiations of a kernel family. `LDGMC.*` is "
            "`multimem.ld_reduce` (in-switch NVLS reduction), `STG.E.128.STRONG.SYS` on a multicast address is "
            "`multimem.st`; `LDG.E.NA.128` / `STG.E.128` on mapped peer pointers are the 128-bit NVLink loads/stores; "
            "`MEMBAR.ALL.SYS` + `ST*.STRONG.SYS` / `LD*.STRONG.SYS` + `CCTL.IVALL` are the st.release.sys / "
-           "ld.acquire.sys flag protocol. `UTCHMMA` = tcgen05.mma (kind::f16), `UTCBAR` = tcgen05.commit, `UTMALDG` = TMA tensor "
-           "load, `LDTM` = tcgen05.ld (TMEM -> registers), `UTCATOMSWS` = tcgen05.alloc, `SYNCS` = mbarrier ops.", "",
+           "ld.acquire.sys flag protocol. `HGMMA` = wgmma.mma_async, `USETMAXREG` = setmaxnreg, `UTMALDG` = TMA tensor "
+           "load (`.MULTICAST` = to every CTA of the cluster), `SYNCS` = mbarrier ops.", "",
            "| kernel family | instantiations | SASS instr | " + " | ".join(KEYS) + " |",
            "|---|---|---|" + "---|" * len(KEYS)]
     for k, d in fam.items():

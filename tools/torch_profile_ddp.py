@@ -6,8 +6,8 @@
 For every profiled step of rank 0 it lists each gradient-bucket collective (start relative to the step's first kernel,
 duration, whether it overlapped compute), the end of the last backward compute kernel, the start of the optimizer
 (`sumsq_kernel`) — the gap between the two is the EXPOSED communication tail — and the step length; plus the same step's
-compute-kernel time so SM contention shows up as inflation against the 1-GPU table
-(profiles/gpt2_step_kernels_torch_profiler.md). Times are device timestamps (CUPTI), not wall clock.
+compute-kernel time so SM contention shows up as inflation against the 1-GPU table of
+tools/torch_profile_step.py. Times are device timestamps (CUPTI), not wall clock.
 """
 from __future__ import annotations
 
