@@ -6,7 +6,7 @@
 // cuBLAS GEMMs). GPU-first equivalent: the token exchange is NOT a collective library call — each
 // rank's kernel stores token rows straight into the destination rank's expert buffer over NVLink
 // (dispatch) and loads result rows straight out of it (combine); slot assignment is a device-side
-// atomic counter per expert; ranks only meet at per-CTA flag barriers on the signal pad.
+// stable rank per expert (token order); ranks only meet at per-CTA flag barriers on the signal pad.
 //
 // Buffer layout on every rank (symmetric heap): [E_local][world][capacity][d]  — expert-major, so
 // the expert MLP is one batched GEMM over [E_local, world*capacity, d] with static shapes (CUDA
@@ -22,15 +22,42 @@ struct MoePeers {
   char* buf[kMaxRanks];      // rank r's buffer in MY address space
 };
 
-// slot assignment: pos[i] = arrival index of assignment i within its expert (or -1 past capacity)
-__global__ void moe_assign_kernel(const int* __restrict__ expert, int n_assign, int n_expert, int capacity,
-                                  int* __restrict__ counts, int* __restrict__ pos) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n_assign) return;
-  const int e = expert[i];
-  if (e < 0 || e >= n_expert) { pos[i] = -1; return; }
-  const int p = atomicAdd(&counts[e], 1);
-  pos[i] = p < capacity ? p : -1;
+// slot assignment by STABLE rank: pos[i] = #{j < i : expert[j] == expert[i]}, or -1 when that rank is >= capacity or
+// the expert id is invalid; counts[e] = the uncapped number of assignments to e. An expert keeps its first `capacity`
+// assignments in token order (the drop rule of MoEMLP._local), and the buffer's row order, hence the bits of the
+// expert GEMMs' weight gradients, is the same on every run (an atomic counter hands out slots in arrival order).
+// One CTA per expert scans all assignments in chunks of blockDim: ballot + popc within a warp, warp totals through
+// shared memory. No host-visible sizes, so it stays CUDA-graph capturable.
+constexpr int kMoeAssignThreads = 1024;
+__global__ void __launch_bounds__(kMoeAssignThreads)
+moe_assign_kernel(const int* __restrict__ expert, int n_assign, int n_expert, int capacity, int* __restrict__ counts,
+                  int* __restrict__ pos) {
+  __shared__ int warp_hits[kMoeAssignThreads / 32];
+  const int e = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
+  int base = 0;                                       // hits of expert e before this chunk
+  for (int i0 = 0; i0 < n_assign; i0 += blockDim.x) {
+    const int i = i0 + threadIdx.x;
+    const int x = i < n_assign ? expert[i] : -1;
+    const bool hit = x == e;
+    const unsigned int b = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) warp_hits[warp] = __popc(b);
+    __syncthreads();
+    int before = base, total = 0;
+    for (int w = 0; w < nwarps; ++w) {
+      const int h = warp_hits[w];
+      if (w < warp) before += h;
+      total += h;
+    }
+    if (hit) {
+      const int r = before + __popc(b & ((1u << lane) - 1u));
+      pos[i] = r < capacity ? r : -1;
+    } else if (e == 0 && i < n_assign && (x < 0 || x >= n_expert)) {
+      pos[i] = -1;
+    }
+    base += total;
+    __syncthreads();                                  // warp_hits is rewritten by the next chunk
+  }
+  if (threadIdx.x == 0) counts[e] = base;
 }
 
 // push: row i of src ([n_assign, d] bf16) -> buffer of rank (e / E_local), slot (e % E_local, me, pos).
@@ -110,11 +137,14 @@ int adapcc_barrier(void* h, const int* active, int n_active, void* stream) {
   return c->device_barrier(act, (cudaStream_t)stream);
 }
 
+// expert: int32 [n_assign]; pos: int32 [n_assign] (stable rank within the expert, -1 = dropped); counts: int32
+// [n_expert], overwritten with the uncapped totals.
 int adapcc_moe_assign(const int* expert, int n_assign, int n_expert, int capacity, int* counts, int* pos,
                       void* stream) {
+  if (n_expert <= 0) { set_error("moe_assign: n_expert must be positive"); return -1; }
   if (n_assign <= 0) return 0;
-  moe_assign_kernel<<<(n_assign + 255) / 256, 256, 0, (cudaStream_t)stream>>>(expert, n_assign, n_expert, capacity,
-                                                                              counts, pos);
+  moe_assign_kernel<<<n_expert, kMoeAssignThreads, 0, (cudaStream_t)stream>>>(expert, n_assign, n_expert, capacity,
+                                                                             counts, pos);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;

@@ -11,15 +11,18 @@
 //                  hits a table row becomes the row's OWNER for this step — and atomicMax(maxbits[table_k, idx],
 //                  max |dY[t, :]|) (the float bits of a non-negative value order like the integers);
 //     2. scatter : every lookup adds its dY row into the owner's scratch row as 64-bit FIXED POINT (red.add.u64),
-//                  scaled by 2^shift with shift = 62 - log2(#lookups) - exponent(row max): no sum can overflow, the
-//                  resolution is 2^-46 or finer of the row's largest entry, and integer addition gives the same bits
-//                  in every order (an fp32 red.add would not: duplicates — repeated tokens, the two token-type rows hit
-//                  by thousands of tokens — arrive in a different order every run); rows hit many times within a
-//                  64-lookup tile are pre-summed in registers (in a fixed order) first;
-//     3. commit  : each owner converts its scratch row back (NaN if the row's dY held a non-finite value), adds it into
-//                  the table's bf16 gradient row (which may already hold another contribution, e.g. the tied LM head's
-//                  dW), zeroes the scratch row and releases the owner and maxbits slots, so all work buffers are back
-//                  to their initial state for the next step.
+//                  scaled by 2^shift with shift = 62 - lookup_bits - (exponent(row max) + 1), lookup_bits =
+//                  ceil(log2(#lookups)): every entry becomes the integer round(float(entry * 2^shift)), no sum can
+//                  overflow, the resolution is 2^-46 or finer of the row's largest entry, and integer addition gives
+//                  the same bits in every order (an fp32 red.add would not: duplicates — repeated tokens, the two
+//                  token-type rows hit by thousands of tokens — arrive in a different order every run); rows hit
+//                  many times within a 64-lookup tile are pre-summed as the same integers in int64 registers first;
+//     3. commit  : each owner converts its scratch row S back, grad = bf16_rn(float(old) + float(double(S) * 2^-shift))
+//                  (NaN if the row's dY held a non-finite value), into the table's bf16 gradient row (which may already
+//                  hold another contribution, e.g. the tied LM head's dW), zeroes the scratch row and releases the owner
+//                  and maxbits slots, so all work buffers are back to their initial state for the next step.
+//   Neither the order duplicates arrive in nor how the scatter groups them changes a bit of the result
+//   (tests/test_gpu_kernels_reference.py checks it against an exact emulation of this arithmetic).
 //   Lookups that share a table (ids and token types both index wte) share owner slots, so a row hit through both is
 //   still committed exactly once.
 #include <cuda_bf16.h>
@@ -103,14 +106,19 @@ __device__ __forceinline__ int embed_shift(unsigned int mb, int lookup_bits) {
   return 62 - lookup_bits - (e + 1);
 }
 
-__device__ __forceinline__ void red_add_fixed(long long* p, float v, int shift) {
-  atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)__float2ll_rn(ldexpf(v, shift)));
+// one dY entry as fixed point: round(v * 2^shift); every path through the scatter adds exactly these integers
+__device__ __forceinline__ long long to_fixed(float v, int shift) { return __float2ll_rn(ldexpf(v, shift)); }
+
+__device__ __forceinline__ void red_add_fixed(long long* p, long long q) {
+  atomicAdd(reinterpret_cast<unsigned long long*>(p), (unsigned long long)q);
 }
 
 // scratch[owner, :] += dY[t, :] (fixed point) for a TILE of 64 consecutive lookups per CTA. Rows hit by many lookups of the tile (the
-// two token-type rows are hit by every token) are first summed in registers and leave as ONE reduction per tile and
-// thread group instead of one per lookup: up to 4 "hot" owners per tile (>= 4 hits), found with 64 x 64 compares in
-// shared memory. Everything else (token ids, positions: mostly unique inside a tile) goes straight to the scratch row.
+// two token-type rows are hit by every token) are first summed in int64 registers and leave as ONE reduction per tile
+// and thread group instead of one per lookup: up to 4 "hot" owners per tile (>= 4 hits), found with 64 x 64 compares
+// in shared memory. Everything else (token ids, positions: mostly unique inside a tile) goes straight to the scratch
+// row. Both paths add the same integers, so when a tile has more than 4 candidates, which of them become hot (warp
+// order decides) does not change any bit of the result.
 constexpr int kEmbTile = 64, kEmbHot = 4, kEmbGroup = 128;       // 2 thread groups x 128 threads; group g: lookups j = g mod 2
 
 __global__ void __launch_bounds__(2 * kEmbGroup)
@@ -120,7 +128,6 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
   __shared__ int s_own[kEmbTile];
   __shared__ int s_row[kEmbTile];
   __shared__ int s_shift[kEmbTile];
-  __shared__ int s_hot_shift[kEmbHot];
   __shared__ int s_hot_key[kEmbHot];
   __shared__ int s_hot_of[kEmbTile];
   __shared__ int s_nhot;
@@ -155,10 +162,7 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
     }
     if (first && cnt >= 4) {
       const int slot = atomicAdd(&s_nhot, 1);
-      if (slot < kEmbHot) {
-        s_hot_key[slot] = own;
-        s_hot_shift[slot] = s_shift[j];
-      }
+      if (slot < kEmbHot) s_hot_key[slot] = own;
     }
   }
   __syncthreads();
@@ -173,11 +177,11 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
   const int g = threadIdx.x / kEmbGroup, tg = threadIdx.x - g * kEmbGroup;
   const int nvec = D >> 3;
   for (int c = tg; c < nvec; c += kEmbGroup) {
-    float acc[kEmbHot][8];
+    long long acc[kEmbHot][8];
 #pragma unroll
     for (int q = 0; q < kEmbHot; ++q)
 #pragma unroll
-      for (int e = 0; e < 8; ++e) acc[q][e] = 0.f;
+      for (int e = 0; e < 8; ++e) acc[q][e] = 0;
     for (int jj = g; jj < kEmbTile; jj += 2) {
       const int own = s_own[jj];
       if (own < 0) continue;
@@ -187,13 +191,13 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
       if (h < 0) {
         long long* dst = scratch + (long long)own * D + c * 8;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) red_add_fixed(dst + e, f[e], s_shift[jj]);
+        for (int e = 0; e < 8; ++e) red_add_fixed(dst + e, to_fixed(f[e], s_shift[jj]));
       } else {
 #pragma unroll
         for (int q = 0; q < kEmbHot; ++q)
           if (q == h) {
 #pragma unroll
-            for (int e = 0; e < 8; ++e) acc[q][e] += f[e];
+            for (int e = 0; e < 8; ++e) acc[q][e] += to_fixed(f[e], s_shift[jj]);
           }
       }
     }
@@ -202,7 +206,7 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
       if (q < nhot) {
         long long* dst = scratch + (long long)s_hot_key[q] * D + c * 8;
 #pragma unroll
-        for (int e = 0; e < 8; ++e) red_add_fixed(dst + e, acc[q][e], s_hot_shift[q]);
+        for (int e = 0; e < 8; ++e) red_add_fixed(dst + e, acc[q][e]);
       }
   }
 }

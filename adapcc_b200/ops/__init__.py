@@ -123,6 +123,11 @@ def fused_ce_(logits: torch.Tensor, labels: torch.Tensor, vocab: int,
     are not), so a mean loss's 1/n needs no extra pass over the gradient or over the GEMMs fed by it."""
     assert logits.dtype == torch.bfloat16 and logits.is_contiguous() and logits.dim() == 2
     rows, stride = logits.shape
+    # the kernel reads labels[row] as int64 for every row: anything else would be read out of bounds
+    if (labels.dtype != torch.int64 or not labels.is_contiguous() or labels.numel() != rows
+            or labels.device != logits.device):
+        raise ValueError(f"fused_ce_: labels must be a contiguous int64 tensor of {rows} elements on "
+                         f"{logits.device}, got {labels.dtype} {tuple(labels.shape)} on {labels.device}")
     row_loss = torch.empty(rows, dtype=torch.float32, device=logits.device)
     gs = None
     if grad_scale is not None:
@@ -206,11 +211,13 @@ class _EmbedSumFn(torch.autograd.Function):
 
 def fused_embedding_sum(tables, lookups) -> torch.Tensor:
     """``sum_k tables[j_k][idx_k]`` for ``lookups = [(j_k, idx_k), ...]`` (idx_k: int64, all the same number of
-    elements n) -> [n, D]. bf16 CUDA tables: one forward kernel and a sort-free three-launch backward that accumulates
-    duplicate rows in fp32 (csrc/ops_embed.cu). Anything else: plain ``F.embedding`` sums."""
+    elements n) -> [n, D]. bf16 CUDA tables with int64 CUDA indices: one forward kernel and a sort-free three-launch
+    backward that accumulates duplicate rows in 64-bit fixed point (csrc/ops_embed.cu). Anything else: plain
+    ``F.embedding`` sums."""
     t0 = tables[0]
     fused = (t0.is_cuda and all(t.dtype == torch.bfloat16 and t.is_contiguous() and t.shape[1] == t0.shape[1]
-                                for t in tables) and t0.shape[1] % 8 == 0 and 1 <= len(lookups) <= 4)
+                                for t in tables) and t0.shape[1] % 8 == 0 and 1 <= len(lookups) <= 4
+             and all(ix.dtype == torch.int64 and ix.device == t0.device for _, ix in lookups))
     if not fused:
         out = None
         for j, ix in lookups:

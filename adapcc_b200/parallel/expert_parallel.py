@@ -9,9 +9,10 @@ functions:
 * ``combine(out_buffer, expert, pos)`` -> rows [A, d] (forward: every rank PULLS its rows' results;
   backward: pushes the rows' grads into the owners' grad buffers).
 
-``A`` = tokens x top_k assignments. Slot assignment (``assign``) is a device-side atomic counter per
-expert with a fixed per-(expert, source) capacity; assignments past capacity are dropped (their rows
-come back as zeros), which keeps every shape static — the whole MoE layer is CUDA-graph capturable.
+``A`` = tokens x top_k assignments. Slot assignment (``assign``) gives each assignment its stable rank
+among the assignments to the same expert (token order) with a fixed per-(expert, source) capacity;
+assignments past capacity are dropped (their rows come back as zeros), the same rule as
+``MoEMLP._local``, and every shape stays static — the whole MoE layer is CUDA-graph capturable.
 Replaces fastmoe's count/assign-pos + grouped ncclSend/ncclRecv exchange
 (/root/reference/third-party/fastmoe/cuda/local_exchange.cuh, global_exchange.h).
 """
@@ -71,7 +72,12 @@ class ExpertExchange:
             raise NativeError(f"barrier failed: {last_error()}")
 
     def assign(self, expert: torch.Tensor):
-        """expert: int32 [A] global expert ids -> (pos int32 [A], counts int32 [n_expert])."""
+        """expert: int32 [A] global expert ids -> (pos int32 [A], counts int32 [n_expert]).
+
+        pos[i] = number of earlier assignments to the same expert, or -1 when that is >= capacity (dropped) or the id
+        is out of range; counts = uncapped assignments per expert. Identical on every run."""
+        if expert.dtype != torch.int32 or not expert.is_cuda or not expert.is_contiguous():
+            raise TypeError(f"assign: expert ids must be a contiguous int32 CUDA tensor, got {expert.dtype}")
         counts = torch.zeros(self.n_expert, dtype=torch.int32, device=expert.device)
         pos = torch.empty_like(expert)
         if self.comm.lib.adapcc_moe_assign(c_void_p(expert.data_ptr()), expert.numel(), self.n_expert, self.capacity,

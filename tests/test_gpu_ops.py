@@ -174,12 +174,16 @@ def test_graft_smoke(dev):
     g.smoke()
 
 
-@pytest.mark.parametrize("d", [256, 768, 1024])
-def test_fused_layernorm_matches_torch(dev, d):
+# 4099 rows at every width (ids: the width alone), and single-row / sub-CTA / one-past-a-CTA row counts
+LN_CASES = ([pytest.param(d, 4099, id=str(d)) for d in (256, 512, 768, 1024)]
+            + [pytest.param(d, r, id=f"{d}-rows{r}") for d in (256, 512, 768, 1024) for r in (1, 7, 9)])
+
+
+@pytest.mark.parametrize("d,rows", LN_CASES)
+def test_fused_layernorm_matches_torch(dev, d, rows):
     from adapcc_b200.ops.layers import FusedLayerNorm
 
-    torch.manual_seed(d)
-    rows = 4099
+    torch.manual_seed(d + rows)
     ln = FusedLayerNorm(d).to(dev).bfloat16()
     with torch.no_grad():
         ln.weight.copy_(torch.randn(d) * 0.5 + 1)
@@ -201,7 +205,7 @@ def test_fused_layernorm_matches_torch(dev, d):
         assert err < 2e-2, err
 
 
-@pytest.mark.parametrize("d", [256, 768])
+@pytest.mark.parametrize("d", [256, 512, 768])
 def test_fused_add_layernorm_matches_torch(dev, d):
     """(x, res) -> (x + res, LN(x + res)) and its backward with a residual-stream gradient."""
     from adapcc_b200.ops.layers import FusedLayerNorm
@@ -358,19 +362,35 @@ def test_fused_linear_bias_grad(dev):
 
 def test_moe_exchange_single_rank_matches_local_reference(dev):
     """Expert 'parallel' exchange kernels with world=1 (push/pull through the symmetric heap) must
-    reproduce the pure-PyTorch local-expert path, forward and backward."""
+    reproduce the pure-PyTorch local-expert path, forward and backward; two identical runs give
+    bit-identical expert gradients."""
+    _moe_exchange_matches_local(dev, overflow=False)
+
+
+def test_moe_exchange_overflow_matches_local_reference(dev):
+    """The same with most tokens dropped: the gate's bias sends every token to expert 0 and
+    capacity_factor 0.5 leaves room for a quarter of them; both paths must keep the same first
+    `capacity` tokens (in token order)."""
+    _moe_exchange_matches_local(dev, overflow=True)
+
+
+def _moe_exchange_matches_local(dev, overflow):
     from adapcc_b200.models.moe import MoEMLP
     from adapcc_b200.parallel.expert_parallel import ExpertExchange
     from adapcc_b200.runtime.native import NativeComm
 
-    comm = NativeComm(f"moe-{os.getpid()}", 0, 1, 0, staging_bytes=4 << 20, heap_bytes=64 << 20)
+    comm = NativeComm(f"moe-{os.getpid()}-{overflow}", 0, 1, 0, staging_bytes=4 << 20, heap_bytes=64 << 20)
     try:
         torch.manual_seed(11)
         E, d, h, T, k = 4, 64, 128, 96, 2
-        ref = MoEMLP(E, d, h, top_k=k).to(dev).bfloat16()
+        cf = 0.5 if overflow else 2.0
+        ref = MoEMLP(E, d, h, top_k=k, capacity_factor=cf).to(dev).bfloat16()
+        if overflow:
+            with torch.no_grad():
+                ref.gate.bias[0] += 8.0
         cap = ref.capacity(T)
         ex = ExpertExchange(comm, E, cap, d)
-        moe = MoEMLP(E, d, h, top_k=k, exchange=ex).to(dev).bfloat16()
+        moe = MoEMLP(E, d, h, top_k=k, capacity_factor=cf, exchange=ex).to(dev).bfloat16()
         moe.load_state_dict(ref.state_dict())
         x = torch.randn(T, d, device=dev).bfloat16()
         x1, x2 = x.clone().requires_grad_(True), x.clone().requires_grad_(True)
@@ -384,6 +404,17 @@ def test_moe_exchange_single_rank_matches_local_reference(dev):
         assert torch.allclose(x1.grad.float(), x2.grad.float(), atol=3e-2, rtol=3e-2)
         assert torch.allclose(ref.w1.grad.float(), moe.w1.grad.float(), atol=3e-2, rtol=3e-2)
         assert torch.allclose(ref.gate.weight.grad.float(), moe.gate.weight.grad.float(), atol=5e-2, rtol=5e-2)
+        if overflow:
+            expert = torch.topk(ref.gate(x).float(), k, dim=-1).indices.reshape(-1).to(torch.int32)
+            assert int((expert == 0).sum()) > cap                       # the case really drops tokens
+        first = [p.grad.clone() for p in (moe.w1, moe.w2, moe.b1, moe.b2)]
+        for p in moe.parameters():
+            p.grad = None
+        x3 = x.clone().requires_grad_(True)
+        moe(x3).backward(g)
+        comm.check()
+        for p, want in zip((moe.w1, moe.w2, moe.b1, moe.b2), first):
+            assert torch.equal(p.grad, want)
     finally:
         comm.close()
 
