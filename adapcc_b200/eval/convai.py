@@ -32,8 +32,11 @@ from ..data.tokenizer import DialogTokenizer
 # ----------------------------------------------------------------------------------------------------------------
 # model access (the training forward only returns losses)
 # ----------------------------------------------------------------------------------------------------------------
-def _lm_logits(model, h: torch.Tensor) -> torch.Tensor:
-    return (h.float() @ model.wte.weight.float().t())[..., : model.cfg.vocab_size]
+def _lm_logits(model, h: torch.Tensor, head: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 logits of hidden states ``h``; ``head``: the fp32 copy of the tied table, when the caller keeps one."""
+    if head is None:
+        head = model.wte.weight.float()
+    return (h.float() @ head.t())[..., : model.cfg.vocab_size]
 
 
 @torch.no_grad()
@@ -69,14 +72,33 @@ def sample_reply(model, tokenizer: DialogTokenizer, persona, history, max_length
                  device="cpu", generator: Optional[torch.Generator] = None) -> List[int]:
     """Generate a reply token by token: the input is rebuilt from persona + history + the partial reply each step, so
     speaker tokens and token types stay those of training (the reference's ``sample_sequence``, interact.py:59-87);
-    special tokens end the reply, and are re-drawn while the reply is shorter than ``min_length``."""
+    special tokens end the reply, and are re-drawn while the reply is shorter than ``min_length``.
+
+    When an input is the previous one plus the newest token, that token costs one cached decode step
+    (``GPT2DoubleHeads.decode_step``, graph-replayed on CUDA with the native kernels); when history truncation moved
+    the prefix, the input is prefilled into the cache again."""
+    from ..models.gpt2 import decoder
+
     special = set(tokenizer.special_ids)
     out: List[int] = []
+    head = model.wte.weight.float()                            # the fp32 LM head, converted once per call
+    cache = dec = prev = None
     for step in range(max_length):
         inst = build_input_from_segments(persona, history, out, tokenizer, with_eos=False, max_len=model.cfg.n_positions)
-        ids = torch.tensor(inst.input_ids, device=device).unsqueeze(0)
-        tt = torch.tensor(inst.token_type_ids, device=device).unsqueeze(0)
-        logits = _lm_logits(model, model.hidden(ids, tt)[0, -1]) / max(temperature, 1e-6)
+        cur = (inst.input_ids, inst.token_type_ids)
+        if (prev is not None and len(cur[0]) == len(prev[0]) + 1 and cur[0][:-1] == prev[0]
+                and cur[1][:-1] == prev[1]):
+            if dec is None:
+                dec = decoder(model, cache)
+            h = dec(torch.tensor(cur[0][-1:], device=device), torch.tensor(cur[1][-1:], device=device))[0]
+        else:
+            if cache is None:
+                cache = model.new_cache(1)
+            ids = torch.tensor(inst.input_ids, device=device).unsqueeze(0)
+            tt = torch.tensor(inst.token_type_ids, device=device).unsqueeze(0)
+            h = model.hidden(ids, tt, cache=cache)[0, -1]
+        prev = cur
+        logits = _lm_logits(model, h, head) / max(temperature, 1e-6)
         probs = F.softmax(top_filtering(logits, top_k, top_p), dim=-1)
         nxt = int(torch.argmax(probs)) if no_sample else int(torch.multinomial(probs, 1, generator=generator))
         if step < min_length and nxt in special:

@@ -23,7 +23,7 @@ from __future__ import annotations
 import math
 import os
 from dataclasses import dataclass
-from typing import Optional, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn as nn
@@ -101,6 +101,69 @@ def causal_attention(q: torch.Tensor, k: torch.Tensor, v: torch.Tensor) -> torch
     return F.scaled_dot_product_attention(q, k, v, is_causal=True)
 
 
+class KVCache:
+    """Keys and values of every layer for incremental decoding (``GPT2DoubleHeads.new_cache``): ``k`` / ``v``
+    [L, B, H, t_max, Dh] in the model's dtype, ``lens`` (int32 [B] on the device: tokens cached per row, what the
+    kernels read), ``host_lens`` (the same numbers on the host, which issues every step and so always knows them) and
+    ``work``, the split-partials workspace of the native decode-attention kernel (bf16 on CUDA; None otherwise),
+    allocated once so a captured step reuses it."""
+
+    def __init__(self, n_layer: int, batch: int, n_head: int, t_max: int, head_dim: int, dtype: torch.dtype, device):
+        self.batch, self.t_max = int(batch), int(t_max)
+        self.k = torch.zeros(n_layer, batch, n_head, t_max, head_dim, dtype=dtype, device=device)
+        self.v = torch.zeros_like(self.k)
+        self.lens = torch.zeros(batch, dtype=torch.int32, device=self.k.device)
+        self.host_lens: List[int] = [0] * self.batch
+        self.work = None
+        if self.k.is_cuda and dtype == torch.bfloat16:
+            from ..ops import decode_attention_work_numel
+            self.work = torch.empty(decode_attention_work_numel(batch, n_head, head_dim, t_max), dtype=torch.float32,
+                                    device=self.k.device)
+
+    def reset(self, lengths: Sequence[int], T: int) -> None:
+        """Lengths after a prefill of T (right-padded) positions."""
+        lengths = [int(n) for n in lengths]
+        if len(lengths) != self.batch or T > self.t_max or any(not 1 <= n <= T for n in lengths):
+            raise ValueError(f"KVCache: a prefill of {T} positions (at most t_max = {self.t_max}) needs {self.batch} "
+                             f"lengths in [1, {T}], got {lengths}")
+        self.host_lens = lengths
+        self.lens.copy_(torch.tensor(lengths, dtype=torch.int32))
+
+    def check_room(self) -> None:
+        if max(self.host_lens) >= self.t_max:
+            raise ValueError(f"KVCache: full (t_max = {self.t_max}, lengths {self.host_lens}); prefill again")
+
+    def advance(self) -> None:
+        """After the last layer of a step: every row holds one more token."""
+        self.lens.add_(1)
+        self.advance_host()
+
+    def advance_host(self) -> None:
+        self.host_lens = [n + 1 for n in self.host_lens]
+
+
+def decode_attention(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
+                     work: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """One layer of decode attention: ``qkv`` [B, 3·H·Dh] (q | k | v of each row's new token), caches [B, H, t_max, Dh],
+    ``lens`` int32 [B]. Stores the new k / v at position ``lens[b]`` and returns softmax(q·K[0..lens[b]]ᵀ/√Dh)·V [B, H·Dh]
+    with an fp32 softmax. With ``work`` (bf16 CUDA caches) this is the native kernel (``ops.decode_attention_``);
+    otherwise the same computation in PyTorch, the reference the CPU tests use."""
+    B, H, t_max, Dh = k_cache.shape
+    if work is not None:
+        from ..ops import decode_attention_
+        out = torch.empty(B, H * Dh, dtype=qkv.dtype, device=qkv.device)
+        return decode_attention_(qkv, k_cache, v_cache, lens, out, work)
+    q, k, v = qkv.reshape(B, 3, H, Dh).unbind(1)
+    pos = lens.long()
+    rows = torch.arange(B, device=qkv.device)
+    k_cache[rows, :, pos] = k
+    v_cache[rows, :, pos] = v
+    s = torch.einsum("bhd,bhtd->bht", q.float(), k_cache.float()) / math.sqrt(Dh)
+    s = s.masked_fill(torch.arange(t_max, device=qkv.device) > pos[:, None, None], float("-inf"))
+    p = torch.softmax(s, dim=-1)
+    return torch.einsum("bht,bhtd->bhd", p, v_cache.float()).to(qkv.dtype).reshape(B, H * Dh)
+
+
 class Block(nn.Module):
     """Pre-LN transformer block; the MLP runs as two GEMMs with the activation passes in GEMM epilogues when
     supported (ops/gemm.py), residual adds optionally fused into the following LayerNorm (``forward_deferred``)."""
@@ -131,15 +194,21 @@ class Block(nn.Module):
                 return self.c_proj2(linear_gelu(h, self.c_fc.weight, self.c_fc.bias))
         return self.c_proj2(F.gelu(self.c_fc(h), approximate="tanh"))
 
-    def _attn(self, h: torch.Tensor) -> torch.Tensor:
+    def _attn(self, h: torch.Tensor, cache: Optional["KVCache"] = None, layer: int = 0) -> torch.Tensor:
+        if cache is not None and h.dim() == 2:       # decode: one new token per row [B, D] against the cache
+            return self.c_proj(decode_attention(self.c_attn(h), cache.k[layer], cache.v[layer], cache.lens, cache.work))
         B, T, D = h.shape
         # split along the feature dim (views; measured 6 % faster fwd+bwd than the packed permute:
         # the backward writes dq/dk/dv straight into one [B, T, 3D] buffer layout-wise)
         q, k, v = (t.view(B, T, self.n_head, D // self.n_head).transpose(1, 2) for t in self.c_attn(h).split(D, dim=-1))
+        if cache is not None:                         # prefill: keep this layer's keys and values
+            cache.k[layer, :, :, :T].copy_(k.detach())
+            cache.v[layer, :, :, :T].copy_(v.detach())
         a = causal_attention(q, k, v)
         return self.c_proj(a.transpose(1, 2).reshape(B, T, D))
 
-    def forward_deferred(self, x: torch.Tensor, delta: Optional[torch.Tensor]):
+    def forward_deferred(self, x: torch.Tensor, delta: Optional[torch.Tensor], cache: Optional["KVCache"] = None,
+                         layer: int = 0):
         """Same block with every residual add fused into the LayerNorm that follows it: takes the
         residual stream ``x`` and the previous block's not-yet-added MLP output ``delta``, returns
         (stream, this block's not-yet-added MLP output)."""
@@ -147,11 +216,11 @@ class Block(nn.Module):
             h = self.ln_1(x)
         else:
             x, h = self.ln_1.forward_add(x, delta)
-        x, h = self.ln_2.forward_add(x, self._attn(h))
+        x, h = self.ln_2.forward_add(x, self._attn(h, cache, layer))
         return x, self._mlp(h)
 
-    def forward(self, x: torch.Tensor) -> torch.Tensor:
-        x = x + self._attn(self.ln_1(x))
+    def forward(self, x: torch.Tensor, cache: Optional["KVCache"] = None, layer: int = 0) -> torch.Tensor:
+        x = x + self._attn(self.ln_1(x), cache, layer)
         return x + self._mlp(self.ln_2(x))
 
 
@@ -284,8 +353,15 @@ class GPT2DoubleHeads(nn.Module):
     def num_parameters(self) -> int:
         return sum(p.numel() for p in self.parameters())
 
-    def hidden(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor]) -> torch.Tensor:
+    def hidden(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], cache: Optional["KVCache"] = None,
+               lengths: Optional[Sequence[int]] = None) -> torch.Tensor:
+        """Final-LayerNorm hidden states [N, T, D]. With ``cache`` this is also the prefill of incremental decoding:
+        every layer's keys and values of positions 0..T-1 go into the cache and its lengths become ``lengths`` (the real
+        length of each right-padded row; default T for all). Causal attention makes the padding invisible to the real
+        tokens, and ``decode_step`` overwrites the padded slots."""
         N, T = input_ids.shape
+        if cache is not None:
+            cache.reset(lengths if lengths is not None else [T] * N, T)
         if (self.fused_embed and input_ids.is_cuda and self.wte.weight.dtype == torch.bfloat16
                 and self.wpe.weight.dtype == torch.bfloat16):
             from ..ops import fused_embedding_sum
@@ -300,14 +376,52 @@ class GPT2DoubleHeads(nn.Module):
             x = self.wte(input_ids) + self.wpe(pos)[None]
             if token_type_ids is not None:
                 x = x + self.wte(token_type_ids)
+        return self._blocks(x, cache)
+
+    def _blocks(self, x: torch.Tensor, cache: Optional["KVCache"]) -> torch.Tensor:
         if self.fuse_add_ln:
             delta = None
-            for blk in self.h:
-                x, delta = blk.forward_deferred(x, delta)
+            for i, blk in enumerate(self.h):
+                x, delta = blk.forward_deferred(x, delta, cache, i)
             return self.ln_f.forward_add(x, delta)[1]
-        for blk in self.h:
-            x = blk(x)
+        for i, blk in enumerate(self.h):
+            x = blk(x, cache, i)
         return self.ln_f(x)
+
+    def new_cache(self, batch: int, t_max: Optional[int] = None) -> "KVCache":
+        """An empty KV cache for ``batch`` rows of up to ``t_max`` (default ``n_positions``) tokens, on the model's
+        device and in its dtype."""
+        cfg = self.cfg
+        t_max = cfg.n_positions if t_max is None else int(t_max)
+        if not 1 <= t_max <= cfg.n_positions:
+            raise ValueError(f"new_cache: t_max must be in [1, {cfg.n_positions}], got {t_max}")
+        w = self.wte.weight
+        return KVCache(cfg.n_layer, batch, cfg.n_head, t_max, cfg.n_embd // cfg.n_head, w.dtype, w.device)
+
+    @torch.no_grad()
+    def decode_step(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], cache: "KVCache") -> torch.Tensor:
+        """One step of incremental decoding: ``input_ids`` [B] (and ``token_type_ids`` [B]) are the next token of each
+        row, at position ``cache.lens[b]``; returns their final-LayerNorm hidden state [B, D] and advances the cache by
+        one. The same modules and fused-add LayerNorm structure as ``hidden``; attention runs over the cache through
+        ``decode_attention``. No host sync, so a step can be captured in a CUDA graph (``DecodeGraph``). Raises
+        ``ValueError`` before launching anything if a row's cache is full."""
+        B = input_ids.shape[0]
+        if input_ids.dim() != 1 or B != cache.batch:
+            raise ValueError(f"decode_step: input_ids must be [{cache.batch}], got {tuple(input_ids.shape)}")
+        cache.check_room()
+        pos = cache.lens.long()
+        if (self.fused_embed and input_ids.is_cuda and self.wte.weight.dtype == torch.bfloat16
+                and self.wpe.weight.dtype == torch.bfloat16):
+            from ..ops import fused_embedding_sum
+            lookups = [(0, input_ids), (1, pos)] + ([(0, token_type_ids)] if token_type_ids is not None else [])
+            x = fused_embedding_sum([self.wte.weight, self.wpe.weight], lookups)
+        else:
+            x = self.wte(input_ids) + self.wpe(pos)
+            if token_type_ids is not None:
+                x = x + self.wte(token_type_ids)
+        h = self._blocks(x, cache)
+        cache.advance()
+        return h
 
     def forward(self, input_ids, token_type_ids=None, mc_token_ids=None, lm_labels=None, mc_labels=None,
                 lm_coef: float = 1.0, mc_coef: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
@@ -351,6 +465,51 @@ class GPT2DoubleHeads(nn.Module):
         return loss, lm_loss, mc_loss
 
 
+class DecodeGraph:
+    """``model.decode_step`` for one cache captured in a CUDA graph and replayed (the pattern of
+    ``FlatDataParallel.capture``): the token ids (and token types) go through static input buffers, the cache's device
+    state is read and advanced inside the graph, so one capture serves every later step of that cache, also after a new
+    prefill into it. Replays give the same bits as eager steps. The returned hidden state [B, D] is a static buffer that
+    the next replay overwrites."""
+
+    def __init__(self, model: "GPT2DoubleHeads", cache: KVCache, token_types: bool = True):
+        dev = cache.lens.device
+        self.cache = cache
+        self.ids = torch.zeros(cache.batch, dtype=torch.long, device=dev)
+        self.tt = torch.zeros_like(self.ids) if token_types else None
+        lens0, host0 = cache.lens.clone(), list(cache.host_lens)
+        s = torch.cuda.Stream(device=dev)
+        s.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(s):                     # warm-up: allocator and cuBLAS settle; writes only slot lens[b],
+            model.decode_step(self.ids, self.tt, cache)   # which the next real step overwrites
+        torch.cuda.current_stream(dev).wait_stream(s)
+        cache.lens.copy_(lens0)
+        cache.host_lens = host0
+        self.graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(self.graph):
+            self.h = model.decode_step(self.ids, self.tt, cache)
+        cache.host_lens = host0                        # capturing ran the host side of a step, not the step
+
+    def __call__(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
+        if (token_type_ids is None) != (self.tt is None):
+            raise ValueError("DecodeGraph: token types given at capture and at replay must match")
+        self.cache.check_room()
+        self.ids.copy_(input_ids, non_blocking=True)
+        if self.tt is not None:
+            self.tt.copy_(token_type_ids, non_blocking=True)
+        self.graph.replay()
+        self.cache.advance_host()
+        return self.h
+
+
+def decoder(model: "GPT2DoubleHeads", cache: KVCache, token_types: bool = True):
+    """``(ids [B], tt [B] | None) -> h [B, D]``, one decode step into ``cache``: graph-replayed (``DecodeGraph``) when
+    the cache runs on the native kernel (bf16 on CUDA), eager ``decode_step`` otherwise."""
+    if cache.work is not None:
+        return DecodeGraph(model, cache, token_types)
+    return lambda ids, tt=None: model.decode_step(ids, tt, cache)
+
+
 @torch.no_grad()
 def sample_sequence(model: "GPT2DoubleHeads", input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor] = None,
                     max_new_tokens: int = 20, temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9,
@@ -358,14 +517,26 @@ def sample_sequence(model: "GPT2DoubleHeads", input_ids: torch.Tensor, token_typ
                     generator: Optional[torch.Generator] = None) -> torch.Tensor:
     """Nucleus / top-k sampling of a reply, one token at a time (the decoding loop of the reference's interact.py:
     ``top_filtering`` + ``sample_sequence``, /root/reference/models/gpt2/interact.py). ``input_ids`` [1, T]; new tokens
-    get ``reply_type`` as their token type when given. No KV cache: a demo / evaluation path, not a serving engine."""
+    get ``reply_type`` as their token type when given. The prompt is prefilled into a KV cache once and every new token
+    costs one ``decode_step`` (graph-replayed on CUDA with the native kernels); once the sequence outgrows
+    ``n_positions`` the window slides, every position moves, and each token re-runs the model over the window."""
     ids = input_ids.clone()
     tt = token_type_ids.clone() if token_type_ids is not None else None
-    vocab = model.cfg.vocab_size
+    vocab, n_pos = model.cfg.vocab_size, model.cfg.n_positions
+    head = model.wte.weight.float()                            # the fp32 LM head, converted once per call
+    cache = step = None
     for _ in range(max_new_tokens):
-        window = slice(max(0, ids.shape[1] - model.cfg.n_positions), None)
-        h = model.hidden(ids[:, window], tt[:, window] if tt is not None else None)
-        logits = (h[:, -1].float() @ model.wte.weight.float().t())[:, :vocab] / max(temperature, 1e-6)
+        T = ids.shape[1]
+        if T > n_pos:                                          # sliding window: the cache no longer applies
+            h = model.hidden(ids[:, T - n_pos:], tt[:, T - n_pos:] if tt is not None else None)[:, -1]
+        elif cache is None:
+            cache = model.new_cache(ids.shape[0])
+            h = model.hidden(ids, tt, cache=cache)[:, -1]
+        else:
+            if step is None:
+                step = decoder(model, cache, tt is not None)
+            h = step(ids[:, -1], tt[:, -1] if tt is not None else None)
+        logits = (h.float() @ head.t())[:, :vocab] / max(temperature, 1e-6)
         if top_k > 0:
             kth = torch.topk(logits, min(top_k, vocab)).values[:, -1:]
             logits = logits.masked_fill(logits < kth, float("-inf"))

@@ -38,6 +38,9 @@ def _lib():
         lib.adapcc_embed_sum_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                              c_void_p, c_void_p, c_void_p]
         lib.adapcc_embed_bwd_reset.argtypes = [c_void_p, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p]
+        lib.adapcc_decode_attn.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_void_p]
+        lib.adapcc_decode_attn_work.argtypes = [c_int] * 4
+        lib.adapcc_decode_attn_work.restype = c_longlong
         _bound = True
     return lib
 
@@ -227,3 +230,48 @@ def fused_embedding_sum(tables, lookups) -> torch.Tensor:
     spec = tuple(int(j) for j, _ in lookups)
     idx = tuple(ix.reshape(-1).contiguous() for _, ix in lookups)
     return _EmbedSumFn.apply(spec, *idx, *tables)
+
+
+# ---- decode attention over a KV cache (csrc/ops_decode.cu) -------------------------------------------------------
+def decode_attention_work_numel(batch: int, n_head: int, head_dim: int, t_max: int) -> int:
+    """fp32 elements of the split-partials workspace ``decode_attention_`` needs for this cache shape."""
+    return int(_lib().adapcc_decode_attn_work(batch, n_head, head_dim, t_max))
+
+
+def decode_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
+                      out: torch.Tensor, work: torch.Tensor) -> torch.Tensor:
+    """Attention of one new token per row over a KV cache, in place. ``qkv`` bf16 [B, 3·H·Dh] (q | k | v of the new
+    token; rows may be strided), ``k_cache`` / ``v_cache`` bf16 [B, H, t_max, Dh], ``lens`` int32 [B] (tokens already
+    cached per row; read, never written). Stores the new k / v at position ``lens[b]`` and writes
+    ``out[b] = softmax(q·K[0..lens[b]]ᵀ / √Dh)·V[0..lens[b]]`` (bf16 [B, H·Dh], fp32 softmax and accumulation). A row
+    with ``lens[b]`` outside [0, t_max) is left alone and its output is zero. ``work``: fp32, at least
+    ``decode_attention_work_numel`` elements. Repeatable bit for bit; no host sync, so it can be captured in a graph."""
+    def bad(msg):
+        raise ValueError(f"decode_attention_: {msg}")
+
+    for name, t in (("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)):
+        if t.dtype != torch.bfloat16:
+            bad(f"{name} must be bf16, got {t.dtype}")
+    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
+        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
+            f"and {tuple(v_cache.shape)}")
+    B, H, t_max, Dh = k_cache.shape
+    if qkv.dim() != 2 or qkv.shape != (B, 3 * H * Dh) or qkv.stride(1) != 1:
+        bad(f"qkv must be [{B}, {3 * H * Dh}] with unit column stride, got {tuple(qkv.shape)} stride {qkv.stride()}")
+    if out.shape != (B, H * Dh) or not out.is_contiguous():
+        bad(f"out must be a contiguous [{B}, {H * Dh}] tensor, got {tuple(out.shape)}")
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
+        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    if work.dtype != torch.float32 or not work.is_contiguous():
+        bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
+    dev = k_cache.device
+    if dev.type != "cuda" or any(t.device != dev for t in (qkv, v_cache, lens, out, work)):
+        bad(f"all tensors must be on one CUDA device, got qkv {qkv.device}, k_cache {dev}, v_cache {v_cache.device}, "
+            f"lens {lens.device}, out {out.device}, work {work.device}")
+    need = decode_attention_work_numel(B, H, Dh, t_max)
+    if work.numel() < need:
+        bad(f"work holds {work.numel()} elements, {need} needed")
+    _ck(_lib().adapcc_decode_attn(c_void_p(qkv.data_ptr()), c_void_p(k_cache.data_ptr()), c_void_p(v_cache.data_ptr()),
+                                  c_void_p(lens.data_ptr()), c_void_p(out.data_ptr()), B, H, Dh, t_max, qkv.stride(0),
+                                  c_void_p(work.data_ptr()), _stream()), "decode_attn")
+    return out
