@@ -14,11 +14,18 @@
 //
 // One CTA = 384 threads, a 128 x BN output tile at a time (BN = 256 when N % 256 == 0, else 128):
 //   warpgroup 0, one thread : TMA producer — cp.async.bulk.tensor.2d of the A (128 x 64) and W (BN x 64) K slabs,
-//                             128-byte swizzled, into a ring of 4 (BN 256) or 6 (BN 128) stages; `full[s]` completes
-//                             on the transferred bytes
+//                             128-byte swizzled, into a ring of Cfg::kStages stages; `full[s]` completes on the
+//                             transferred bytes
 //   warpgroups 1, 2         : 64 rows each — 4 x wgmma.m64nBNk16 per slab, one wgmma group kept in flight; a slab is
 //                             released (`empty[s]`) once the group that read it has retired; then the epilogue
-//                             (bias + activation in fp32, bf16 stores) straight from the accumulator registers
+//                             (bias + activation in fp32 on the accumulator registers, as before any bf16 rounding)
+// Epilogue: each consumer warp owns 16 rows and a ring of Cfg::kEpiBufs 16 x 64 bf16 staging buffers (2 KB,
+// 128-byte swizzled). Per 64-column sub-tile it packs its results to bf16, writes them with stmatrix, fences the
+// generic proxy against the async one and one lane issues a TMA store (cp.async.bulk.tensor, bulk_group) of the
+// sub-tile; the tensor map's bounds clip rows >= M. A buffer is written again only once the store that last read it
+// has (cp.async.bulk.wait_group.read), so the stores drain to HBM under the next tile's wgmmas. ACT 2 / 3 read `aux`
+// the same way in reverse: a TMA load into the staging buffer (issued during the tile's middle slab, completing on a
+// per-buffer mbarrier), ldmatrix into the fragment layout, and the result is stored back in place.
 // Grid policies (the `variant` argument):
 //   0: one tile per CTA.   1: persistent CTAs (grid = SMs) — the producer streams the next tile's slabs while the
 //   consumers run the epilogue.   2 / 3: clusters of two CTAs on vertically adjacent tiles that share W: each CTA
@@ -43,16 +50,26 @@ constexpr int kBK = 64;            // K slab: 64 bf16 = 128 B = one swizzle-128B
 constexpr int kMmaK = 16;          // K per wgmma for 16-bit inputs
 constexpr int kThreads = 384;
 constexpr int kMaxDevices = 64;    // per-device launch setup slots
+constexpr int kEpiRows = 16;       // rows of one consumer warp's staging sub-tile (its wgmma fragment rows)
+constexpr uint32_t kEpiBytes = kEpiRows * kBK * 2;   // 2 KB: 16 rows x 64 bf16, 128-byte swizzled
+constexpr uint32_t kSmemOptIn = 232448;               // sm_90 per-block dynamic shared memory limit
 
 template <int BN>
 struct Cfg {
-  static constexpr int kStages = BN == 256 ? 4 : 6;                  // 192 KB of operand ring either way
+  static constexpr int kStages = BN == 256 ? 3 : 5;
   static constexpr uint32_t kABytes = kBM * kBK * 2;                 // 16 KB
   static constexpr uint32_t kBBytes = BN * kBK * 2;                  // 16 / 32 KB
   static constexpr uint32_t kStageBytes = kABytes + kBBytes;
-  static constexpr uint32_t kColsumOffset = kStages * kStageBytes;   // fp32 [8 warps][BN]: column sums (ACT 2)
-  static constexpr uint32_t kBarOffset = kColsumOffset + 8 * BN * 4; // full[S], empty[S]
-  static constexpr uint32_t kDynamic = kBarOffset + 2 * kStages * 8 + 1024;   // + slack for the 1024-B alignment
+  // what the ring, the column-sum buffer, the ring's barriers and the alignment slack leave, in staging buffers per
+  // consumer warp (each with its aux mbarrier); more than BN / 64 would never be used
+  static constexpr uint32_t kFixed = kStages * kStageBytes + 8 * BN * 4 + 2 * kStages * 8 + 1024;
+  static constexpr int kEpiBufs = (int)std::min<uint32_t>(BN / 64, (kSmemOptIn - kFixed) / (8 * (kEpiBytes + 8)));
+  static_assert(kEpiBufs >= 1, "no shared memory left for the epilogue staging buffers");
+  static constexpr uint32_t kEpiOffset = kStages * kStageBytes;      // [8 warps][kEpiBufs] staging buffers
+  static constexpr uint32_t kColsumOffset = kEpiOffset + 8 * kEpiBufs * kEpiBytes;   // fp32 [8 warps][BN] (ACT 2)
+  static constexpr uint32_t kBarOffset = kColsumOffset + 8 * BN * 4; // full[S], empty[S], aux[8 warps][kEpiBufs]
+  static constexpr uint32_t kDynamic = kBarOffset + (2 * kStages + 8 * kEpiBufs) * 8 + 1024;   // + alignment slack
+  static_assert(kDynamic <= kSmemOptIn, "shared memory over the opt-in limit");
 };
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -90,11 +107,14 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void mbar_arrive(uint32_t bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
 }
-// arrive on the barrier at `bar`'s offset in CTA `cta` of the cluster
+// arrive on the barrier at `bar`'s offset in CTA `cta` of the cluster. Default (.release.cta) semantics: the arrival
+// only has to follow the wgmmas that read the stage, which wgmma.wait_group has already retired. A .release.cluster
+// arrive compiles to MEMBAR.ALL.GPU, which waits for this thread's outstanding global stores and held every stage
+// refill of the pair up behind it.
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
   uint32_t remote;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
+  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -120,6 +140,42 @@ __device__ __forceinline__ void tma_load_2d_multicast(uint32_t dst, const CUtens
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
       " [%0], [%1, {%3, %4}], [%2], %5;"
       ::"r"(dst), "l"(map), "r"(bar), "r"(c_inner), "r"(c_outer), "h"(mask) : "memory");
+}
+// shared -> global; the box's rows past the tensor map's bounds are not written
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c_inner, int c_outer) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(src), "r"(c_inner), "r"(c_outer) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's most recent bulk groups may still be reading their shared-memory source
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// generic-proxy shared-memory writes become visible to the async proxy (a following TMA store)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ---- staging sub-tiles: 8 x 8 b16 matrices between the wgmma fragment layout and shared memory ---------------------
+// x4: matrix q's row r is addressed by lane 8 q + r; a thread's register q holds row lane / 4, columns 2 (lane % 4)
+// and + 1 of matrix q — for the accumulator, the pair d[4 i + 2 h], d[4 i + 2 h + 1].
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};"
+               ::"r"(addr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+}
+__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3) : "r"(addr) : "memory");
+}
+// A warp's 16 x 64 sub-tile as 4 x4 groups: group p holds the column groups 2p, 2p + 1 (8 columns = one 16-B chunk
+// each) of rows 0-7 and 8-15, i.e. matrices (h 0, 2p), (h 1, 2p), (h 0, 2p + 1), (h 1, 2p + 1); registers
+// v[4p .. 4p + 3] in that order. The buffer is in the TMA's 128-byte swizzled layout: chunk c of row r sits at
+// r * 128 + ((c ^ (r % 8)) * 16), so the 8 rows of a matrix fall on 8 different bank groups.
+__device__ __forceinline__ uint32_t stage_addr(uint32_t buf, int lane, int p) {
+  const int r = (lane & 7) + 8 * ((lane >> 3) & 1), chunk = 2 * p + (lane >> 4);
+  return buf + (uint32_t)(r * 128 + ((chunk ^ (r & 7)) << 4));
+}
+__device__ __forceinline__ void stage_write(uint32_t buf, int lane, const uint32_t (&v)[16]) {
+#pragma unroll
+  for (int p = 0; p < 4; ++p) stmatrix_x4(stage_addr(buf, lane, p), v[4 * p], v[4 * p + 1], v[4 * p + 2], v[4 * p + 3]);
 }
 
 // ---- wgmma ---------------------------------------------------------------------------------------
@@ -228,15 +284,16 @@ __device__ __forceinline__ float2 unpack_bf16x2(uint32_t w) {
 
 // CLUSTER = 1: CTAs walk tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  CLUSTER = 2: clusters walk pair tiles
 // (256 x BN) the same way and CTA r of the cluster owns rows 128 r .. 128 r + 127 of the pair tile.
+// map_out / map_pre: [M, N] bf16, 64 x 16 boxes, 128-byte swizzle (map_pre is unused when has_pre == 0).
 // colsum_rows (ACT 2, optional): fp32 [tiles_m, N], row m_blk receives the column sums of row tile m_blk.
 template <int BN, int ACT, int CLUSTER>
 __global__ void __launch_bounds__(kThreads, 1)
 gemm_bias_act_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_w,
-                           const __nv_bfloat16* __restrict__ bias, __nv_bfloat16* __restrict__ out,
-                           __nv_bfloat16* __restrict__ pre, float* __restrict__ colsum_rows, int M, int N, int K,
-                           int tiles_n, int num_tiles) {
+                           const __grid_constant__ CUtensorMap map_out, const __grid_constant__ CUtensorMap map_pre,
+                           const __nv_bfloat16* __restrict__ bias, int has_pre, float* __restrict__ colsum_rows, int M,
+                           int N, int K, int tiles_n, int num_tiles) {
   using C = Cfg<BN>;
-  constexpr int S = C::kStages;
+  constexpr int S = C::kStages, NB = C::kEpiBufs, J = BN / 64;   // J: 64-column sub-tiles per tile
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                   // swizzle-128B tiles need 1024-B alignment
@@ -256,10 +313,13 @@ gemm_bias_act_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __gr
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_out) : "memory");
+    if (has_pre) asm volatile("prefetch.tensormap [%0];" ::"l"(&map_pre) : "memory");
     for (int s = 0; s < S; ++s) {
       mbar_init(full(s), 1);
       mbar_init(empty(s), 2 * CLUSTER);                          // one arrive per consumer warpgroup of each CTA
     }
+    for (int b = 0; b < 8 * NB; ++b) mbar_init(bar0 + 8u * (2 * S + b), 1);   // aux loads: expect_tx + bytes
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -303,9 +363,18 @@ gemm_bias_act_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __gr
         }
       }
     };
+    // this warp's 16 rows: staging ring buf(b), aux barrier abar(b) (parity bit b of aux_phase)
+    const int gw = c * 4 + warp;
+    const uint32_t epi0 = base + C::kEpiOffset + (uint32_t)(gw * NB) * kEpiBytes;
+    auto buf = [&](int b) { return epi0 + (uint32_t)b * kEpiBytes; };
+    auto abar = [&](int b) { return bar0 + 8u * (2 * S + gw * NB + b); };
+    uint32_t aux_phase = 0, epi_it = 0;
     uint32_t it = 0;
     for (int t = group; t < num_tiles; t += num_groups) {
       const int m_blk = (t / tiles_n) * CLUSTER + (int)rank, n_blk = t % tiles_n;
+      const int row_w = m_blk * kBM + c * 64 + warp * 16;       // first row of this warp's sub-tiles
+      // a warp whose rows lie wholly below M (always so in a cluster CTA past the last row tile) moves no data
+      const bool rows_in = row_w < M;
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
@@ -323,6 +392,17 @@ gemm_bias_act_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __gr
           wgmma_tile<BN>(acc, da, db);
         }
         wgmma_commit();
+        if (ACT >= 2 && kb == num_kb / 2 && rows_in && lane == 0) {
+          // under the wgmmas of the middle slab: once the previous tile's stores have read the ring, load this tile's
+          // first NB aux sub-tiles into it — half a mainloop after those stores were issued, half a mainloop before the
+          // epilogue needs the loads
+          bulk_wait_read<0>();
+#pragma unroll
+          for (int b = 0; b < NB; ++b) {
+            mbar_expect_tx(abar(b), kEpiBytes);
+            tma_load_2d(buf(b), &map_pre, n_blk * BN + 64 * b, row_w, abar(b));
+          }
+        }
         wgmma_wait<1>();                                          // the previous slab's group has retired
         if (prev >= 0) release(prev);
         prev = s;
@@ -330,61 +410,109 @@ gemm_bias_act_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __gr
       wgmma_wait<0>();
       if (prev >= 0) release(prev);
 
-      // ===== epilogue from the accumulator registers =====
-      const int row_a = m_blk * kBM + c * 64 + warp * 16 + (lane >> 2);
+      // ===== epilogue: fp32 math on the accumulator registers, bf16 sub-tiles out through shared memory + TMA =====
+      const int row_a = row_w + (lane >> 2);
       const bool valid[2] = {row_a < M, row_a + 8 < M};
       const int col_base = n_blk * BN + 2 * (lane & 3);
+      // TMA-store sub-tile j of this warp's rows from staging buffer b, once every lane's writes to it are fenced
+      auto store_sub = [&](uint32_t b, const CUtensorMap* map, int j) {
+        fence_proxy_async();
+        __syncwarp();
+        if (lane == 0) {
+          tma_store_2d(map, buf((int)b), n_blk * BN + 64 * j, row_w);
+          bulk_commit();
+        }
+      };
 #pragma unroll
-      for (int i = 0; i < BN / 8; ++i) {
-        const int col = col_base + 8 * i;
-        float2 bv = make_float2(0.f, 0.f);
-        if (ACT != 2 && bias != nullptr) bv = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + col)));
-        float cs0 = 0.f, cs1 = 0.f;
+      for (int j = 0; j < J; ++j) {
+        // ov: the result, v[2 ii + h]. For ACT 2 / 3 the aux sub-tile in buffer j % NB is read one x4 group (column
+        // groups 2p, 2p + 1) at a time into the same registers and the group's results are written back in place.
+        uint32_t ov[16], uv[16];
+        const int ab = j % NB;
+        if (ACT >= 2 && rows_in) {
+          mbar_wait(abar(ab), (aux_phase >> ab) & 1u);
+          aux_phase ^= 1u << ab;
+        }
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const size_t off = (size_t)(row_a + 8 * h) * (size_t)N + (size_t)col;
-          const float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
-          uint32_t o;
-          if (ACT >= 2) {
-            const float2 ax = valid[h] ? unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(pre + off)))
-                                       : make_float2(0.f, 0.f);
-            if (ACT == 2) {
-              o = pack_bf16x2(v0 * gelu_tanh_grad(ax.x), v1 * gelu_tanh_grad(ax.y));
-              if (valid[h]) {                                     // sums of the bf16 values written
-                const float2 r = unpack_bf16x2(o);
-                cs0 += r.x;
-                cs1 += r.y;
+        for (int ii = 0; ii < 8; ++ii) {
+          const int i = 8 * j + ii;
+          if (ACT >= 2 && (ii & 1) == 0) {
+            if (rows_in)
+              ldmatrix_x4(stage_addr(buf(ab), lane, ii / 2), ov[2 * ii], ov[2 * ii + 1], ov[2 * ii + 2], ov[2 * ii + 3]);
+            else
+              ov[2 * ii] = ov[2 * ii + 1] = ov[2 * ii + 2] = ov[2 * ii + 3] = 0u;
+          }
+          const int col = col_base + 8 * i;
+          float2 bv = make_float2(0.f, 0.f);
+          if (ACT != 2 && bias != nullptr) bv = unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(bias + col)));
+          float cs0 = 0.f, cs1 = 0.f;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const float v0 = acc[4 * i + 2 * h], v1 = acc[4 * i + 2 * h + 1];
+            uint32_t o;
+            if (ACT >= 2) {
+              const float2 ax = valid[h] ? unpack_bf16x2(ov[2 * ii + h]) : make_float2(0.f, 0.f);
+              if (ACT == 2) {
+                o = pack_bf16x2(v0 * gelu_tanh_grad(ax.x), v1 * gelu_tanh_grad(ax.y));
+                if (valid[h]) {                                   // sums of the bf16 values written
+                  const float2 r = unpack_bf16x2(o);
+                  cs0 += r.x;
+                  cs1 += r.y;
+                }
+              } else {
+                // bf16-round the projection first, then add: what `x + linear(h)` computes on bf16 tensors
+                const float2 pr = unpack_bf16x2(pack_bf16x2(v0 + bv.x, v1 + bv.y));
+                o = pack_bf16x2(pr.x + ax.x, pr.y + ax.y);
               }
             } else {
-              // bf16-round the projection first, then add: what `x + linear(h)` computes on bf16 tensors
-              const float2 pr = unpack_bf16x2(pack_bf16x2(v0 + bv.x, v1 + bv.y));
-              o = pack_bf16x2(pr.x + ax.x, pr.y + ax.y);
+              const uint32_t u = pack_bf16x2(v0 + bv.x, v1 + bv.y);
+              if (ACT == 1) {
+                // the activation sees the bf16-rounded pre-activation, exactly like gelu(linear(x)) on bf16 tensors
+                const float2 r = unpack_bf16x2(u);
+                o = pack_bf16x2(gelu_tanh(r.x), gelu_tanh(r.y));
+              } else {
+                o = u;
+              }
+              uv[2 * ii + h] = u;
             }
-          } else {
-            const uint32_t u = pack_bf16x2(v0 + bv.x, v1 + bv.y);
-            if (ACT == 1) {
-              // the activation sees the bf16-rounded pre-activation, exactly like gelu(linear(x)) on bf16 tensors
-              const float2 r = unpack_bf16x2(u);
-              o = pack_bf16x2(gelu_tanh(r.x), gelu_tanh(r.y));
-            } else {
-              o = u;
-            }
-            if (pre != nullptr && valid[h]) *reinterpret_cast<uint32_t*>(pre + off) = u;
+            ov[2 * ii + h] = o;
           }
-          if (valid[h]) *reinterpret_cast<uint32_t*>(out + off) = o;
-        }
-        if (ACT == 2 && colsum_rows != nullptr) {
-          // the 8 lanes of a column pair (lane / 4 = 0..7), then this warp's slot of the shared buffer
+          if (ACT >= 2 && (ii & 1) == 1 && rows_in)
+            stmatrix_x4(stage_addr(buf(ab), lane, ii / 2), ov[2 * ii - 2], ov[2 * ii - 1], ov[2 * ii], ov[2 * ii + 1]);
+          if (ACT == 2 && colsum_rows != nullptr) {
+            // the 8 lanes of a column pair (lane / 4 = 0..7), then this warp's slot of the shared buffer
 #pragma unroll
-          for (int x = 4; x < 32; x <<= 1) {
-            cs0 += __shfl_xor_sync(0xffffffffu, cs0, x);
-            cs1 += __shfl_xor_sync(0xffffffffu, cs1, x);
+            for (int x = 4; x < 32; x <<= 1) {
+              cs0 += __shfl_xor_sync(0xffffffffu, cs0, x);
+              cs1 += __shfl_xor_sync(0xffffffffu, cs1, x);
+            }
+            if (lane < 4) {
+              float* slot = colbuf + gw * BN + 8 * i + 2 * lane;
+              slot[0] = cs0;
+              slot[1] = cs1;
+            }
           }
-          if (lane < 4) {
-            float* slot = colbuf + (c * 4 + warp) * BN + 8 * i + 2 * lane;
-            slot[0] = cs0;
-            slot[1] = cs1;
+        }
+        if (!rows_in) continue;
+        if (ACT >= 2) {
+          store_sub(ab, &map_out, j);
+          if (j + NB < J && lane == 0) {
+            bulk_wait_read<0>();                                  // the store has read the buffer: refill it
+            mbar_expect_tx(abar(ab), kEpiBytes);
+            tma_load_2d(buf(ab), &map_pre, n_blk * BN + 64 * (j + NB), row_w, abar(ab));
           }
+        } else {
+          // ring reuse: with one commit per buffer use, <= NB - 1 groups still reading means the next buffer is free
+          if (has_pre) {
+            if (lane == 0) bulk_wait_read<NB - 1>();
+            __syncwarp();
+            stage_write(buf(epi_it % NB), lane, uv);
+            store_sub(epi_it++ % NB, &map_pre, j);
+          }
+          if (lane == 0) bulk_wait_read<NB - 1>();
+          __syncwarp();
+          stage_write(buf(epi_it % NB), lane, ov);
+          store_sub(epi_it++ % NB, &map_out, j);
         }
       }
       if (ACT == 2 && colsum_rows != nullptr) {
@@ -402,6 +530,7 @@ gemm_bias_act_wgmma_kernel(const __grid_constant__ CUtensorMap map_a, const __gr
         asm volatile("bar.sync 1, 256;" ::: "memory");
       }
     }
+    if (lane == 0) bulk_wait_all();                               // the staging buffers outlive every store
   }
   if (CLUSTER > 1) cluster_sync_all();                            // no CTA leaves while its peer may still signal it
 }
@@ -467,9 +596,11 @@ static int launch(const void* a, const void* w, const void* bias, void* out, voi
     if (setup[dev] == cudaSuccess) setup[dev] = cudaDeviceGetAttribute(&sms[dev], cudaDevAttrMultiProcessorCount, dev);
   });
   CUDA_TRY(setup[dev]);
-  CUtensorMap ma, mw;
+  CUtensorMap ma, mw, mo, mp = {};
   if (make_map(&ma, a, M, K, kBM)) return -1;
   if (make_map(&mw, w, N, K, BN / CLUSTER)) return -1;          // in a cluster each CTA loads half of the W slab
+  if (make_map(&mo, out, M, N, kEpiRows)) return -1;            // one consumer warp's 16 x 64 staging sub-tile
+  if (pre != nullptr && make_map(&mp, pre, M, N, kEpiRows)) return -1;
   const int tiles_n = N / BN, tiles_m = (M + kBM - 1) / kBM;
   const int num_tiles = tiles_n * ((tiles_m + CLUSTER - 1) / CLUSTER);
   const int groups = persistent ? std::min(num_tiles, sms[dev] / CLUSTER) : num_tiles;
@@ -485,9 +616,8 @@ static int launch(const void* a, const void* w, const void* bias, void* out, voi
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mw, (const __nv_bfloat16*)bias, (__nv_bfloat16*)out,
-                              (__nv_bfloat16*)pre, colsum != nullptr ? colsum_work : nullptr, M, N, K, tiles_n,
-                              num_tiles));
+  CUDA_TRY(cudaLaunchKernelEx(&cfg, kern, ma, mw, mo, mp, (const __nv_bfloat16*)bias, pre != nullptr ? 1 : 0,
+                              colsum != nullptr ? colsum_work : nullptr, M, N, K, tiles_n, num_tiles));
   count_launch();
   if (colsum != nullptr) {
     colsum_rows_add_kernel<<<(N + 255) / 256, 256, 0, s>>>(colsum_work, colsum, tiles_m, N);
