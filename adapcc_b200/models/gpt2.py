@@ -423,6 +423,126 @@ class GPT2DoubleHeads(nn.Module):
         cache.advance()
         return h
 
+    @torch.no_grad()
+    def generate(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
+                 token_type_ids: Optional[torch.Tensor] = None, reply_type=None, max_new_tokens: int = 20,
+                 temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9, stop_ids: Sequence[int] = (),
+                 suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, seed=0) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
+
+        ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
+        ``reply_type`` (an int or a [B] tensor) is the token type of the new tokens; by default each row's last prompt
+        token type when ``token_type_ids`` is given. ``seed``: an int (row b uses ``seed + b``) or an int64 [B] tensor.
+        While fewer than ``min_new_tokens`` tokens are generated, ``suppress_ids`` cannot be drawn; a token in
+        ``stop_ids`` ends its row. ``temperature == 0`` is greedy. The draw of each token is defined in
+        ``ops/sampling.py``: a row's tokens depend on its prompt, its seed and the scalars, not on the other rows.
+
+        Returns ``(tokens, n_new)``: int64 [B, max_new_tokens] (-1 after a row stopped) and the tokens per row.
+
+        The prompts are prefilled into a KV cache of ``max(lengths) + max_new_tokens`` positions (``ValueError`` if that
+        exceeds ``n_positions``: there is no sliding window here, ``sample_sequence`` has one). On CUDA with bf16
+        weights the LM head and the sampler are native kernels (``ops.lm_head_logits_``, ``ops.sample_tokens_``) and
+        every token after the first replays one CUDA graph of decode step, LM head and sampler, which feeds the drawn ids
+        back into its own input; the host reads the done flags once every 8 tokens, a step late, to stop early.
+        Elsewhere the same loop runs eagerly with fp32 PyTorch logits and ``ops.sampling.sample_reference``."""
+        from ..ops.sampling import sample_reference
+
+        cfg = self.cfg
+        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
+            raise ValueError(f"generate: input_ids must be [B, T], got {tuple(input_ids.shape)}")
+        B, T = input_ids.shape
+        dev = input_ids.device
+        lengths = [T] * B if lengths is None else [int(n) for n in lengths]
+        if len(lengths) != B or any(not 1 <= n <= T for n in lengths):
+            raise ValueError(f"generate: need {B} lengths in [1, {T}], got {lengths}")
+        if int(max_new_tokens) < 1:
+            raise ValueError(f"generate: max_new_tokens must be >= 1, got {max_new_tokens}")
+        if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1 or int(min_new_tokens) < 0:
+            raise ValueError(f"generate: need temperature >= 0, top_k >= 0, 0 < top_p <= 1 and min_new_tokens >= 0, "
+                             f"got {temperature}, {top_k}, {top_p}, {min_new_tokens}")
+        t_max = max(lengths) + int(max_new_tokens)
+        if t_max > cfg.n_positions:
+            raise ValueError(f"generate: the longest prompt ({max(lengths)}) plus max_new_tokens ({max_new_tokens}) "
+                             f"exceeds n_positions = {cfg.n_positions}; sample_sequence slides the window instead")
+        if isinstance(seed, torch.Tensor):
+            if seed.dtype != torch.int64 or seed.numel() != B:
+                raise ValueError(f"generate: a seed tensor must be int64 with {B} elements, got {seed.dtype} "
+                                 f"{tuple(seed.shape)}")
+            seeds = seed.reshape(B).to(dev)
+        else:
+            seeds = (int(seed) + torch.arange(B, dtype=torch.int64)).to(dev)
+        last = torch.tensor(lengths, device=dev) - 1
+        tt_new = None
+        if reply_type is not None:
+            tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
+        elif token_type_ids is not None:
+            tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
+        cache = self.new_cache(B, t_max)
+        h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
+        n = int(max_new_tokens)
+        tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
+        if cache.work is None:                      # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
+            head = self.wte.weight.float()
+            done = torch.zeros(B, dtype=torch.int32)
+            for i in range(n):
+                if i:
+                    h = self.decode_step(nxt.to(dev), tt_new, cache)
+                nxt, tok, done = sample_reference(h.float() @ head.t(), cfg.vocab_size, temperature, top_k, top_p,
+                                                  seeds, cache.lens, i, min_new_tokens, suppress_ids, stop_ids, done)
+                tokens[:, i] = tok.to(dev)
+                if bool(done.all()):
+                    break
+            return tokens, (tokens >= 0).sum(1)
+
+        from ..ops import LM_HEAD_MAX_ROWS, lm_head_logits_, sample_tokens_
+
+        if B > LM_HEAD_MAX_ROWS:
+            raise ValueError(f"generate: at most {LM_HEAD_MAX_ROWS} rows per call on the native path, got {B}")
+        weight = self.wte.weight
+        logits = torch.empty(B, weight.shape[0], dtype=torch.float32, device=dev)
+        next_ids = torch.zeros(B, dtype=torch.int64, device=dev)
+        done = torch.zeros(B, dtype=torch.int32, device=dev)
+        step = torch.zeros(1, dtype=torch.int32, device=dev)
+        sup = torch.tensor(list(suppress_ids), dtype=torch.int32, device=dev)
+        stop = torch.tensor(list(stop_ids), dtype=torch.int32, device=dev)
+
+        def head_and_sample(hidden):
+            lm_head_logits_(hidden, weight, logits)
+            sample_tokens_(logits, cfg.vocab_size, temperature, top_k, top_p, seeds, cache.lens, step,
+                           min_new_tokens, sup, stop, done, next_ids, tokens)
+
+        head_and_sample(h)                          # the first token, from the prefill's last positions
+        if n == 1:
+            return tokens, (tokens >= 0).sum(1)
+        # DecodeGraph's warm-up and capture, with the LM head and the sampler inside the graph
+        lens0, host0 = cache.lens.clone(), list(cache.host_lens)
+        s = torch.cuda.Stream(device=dev)
+        s.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(s):                  # writes only slot lens[b], which the first replay overwrites
+            self.decode_step(next_ids, tt_new, cache)
+        torch.cuda.current_stream(dev).wait_stream(s)
+        cache.lens.copy_(lens0)
+        cache.host_lens = host0
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            head_and_sample(self.decode_step(next_ids, tt_new, cache))
+        cache.host_lens = host0
+        flags = torch.empty(B, dtype=torch.int32, pin_memory=True)
+        copied = None
+        for i in range(1, n):
+            cache.check_room()
+            graph.replay()
+            cache.advance_host()
+            if i % 8 == 0:                          # the flags copied 8 tokens ago are ready by now: no stall
+                if copied is not None:
+                    copied.synchronize()
+                    if bool(flags.all()):
+                        break
+                flags.copy_(done, non_blocking=True)
+                copied = torch.cuda.Event()
+                copied.record()
+        return tokens, (tokens >= 0).sum(1)
+
     def forward(self, input_ids, token_type_ids=None, mc_token_ids=None, lm_labels=None, mc_labels=None,
                 lm_coef: float = 1.0, mc_coef: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """-> (loss, lm_loss, mc_loss). Shapes as in the reference: [B, C, T] ids/labels, [B, C]

@@ -41,6 +41,10 @@ def _lib():
         lib.adapcc_decode_attn.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_void_p]
         lib.adapcc_decode_attn_work.argtypes = [c_int] * 4
         lib.adapcc_decode_attn_work.restype = c_longlong
+        lib.adapcc_lm_head_logits.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]
+        lib.adapcc_sample_tokens.argtypes = ([c_void_p, c_int, c_int, c_int, c_float, c_int, c_float]
+                                             + [c_void_p] * 3 + [c_int, c_void_p, c_int, c_void_p, c_int]
+                                             + [c_void_p] * 3 + [c_int, c_void_p])
         _bound = True
     return lib
 
@@ -275,3 +279,86 @@ def decode_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.T
                                   c_void_p(lens.data_ptr()), c_void_p(out.data_ptr()), B, H, Dh, t_max, qkv.stride(0),
                                   c_void_p(work.data_ptr()), _stream()), "decode_attn")
     return out
+
+
+# ---- LM head and token sampling for generation (csrc/ops_sample.cu) ------------------------------------------------
+LM_HEAD_MAX_ROWS = 64          # h rows the LM-head kernel takes per call (its h tile lives in shared memory)
+SAMPLE_MAX_VOCAB = 56 * 1024   # vocabulary the sampler holds in shared memory per row
+SAMPLE_MAX_IDS = 1024          # ids per suppress / stop list
+
+
+def lm_head_logits_(h: torch.Tensor, weight: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
+    """``out[b, i] = sum_d h[b, d] * weight[i, d]`` in place: ``h`` bf16 [B, D] with unit column stride (B <= 64),
+    ``weight`` the contiguous bf16 [V, D] table, ``out`` contiguous fp32 [B, V]. fp32 accumulation in an order fixed by
+    d alone, so a row's bits do not depend on B or the other rows; ``weight`` is read once per call. No host sync."""
+    def bad(msg):
+        raise ValueError(f"lm_head_logits_: {msg}")
+
+    if h.dtype != torch.bfloat16 or weight.dtype != torch.bfloat16 or out.dtype != torch.float32:
+        bad(f"need bf16 h and weight and an fp32 out, got {h.dtype}, {weight.dtype}, {out.dtype}")
+    if weight.dim() != 2 or not weight.is_contiguous():
+        bad(f"weight must be a contiguous [V, D] tensor, got {tuple(weight.shape)} stride {weight.stride()}")
+    V, D = weight.shape
+    if h.dim() != 2 or h.shape[1] != D or h.stride(1) != 1 or not 1 <= h.shape[0] <= LM_HEAD_MAX_ROWS:
+        bad(f"h must be [B, {D}] with unit column stride and 1 <= B <= {LM_HEAD_MAX_ROWS}, got {tuple(h.shape)} "
+            f"stride {h.stride()}")
+    B = h.shape[0]
+    if out.shape != (B, V) or not out.is_contiguous():
+        bad(f"out must be a contiguous [{B}, {V}] tensor, got {tuple(out.shape)}")
+    if D % 8 != 0 or D > 1024 or h.stride(0) % 8 != 0:
+        bad(f"D must be a multiple of 8 up to 1024 and h's row stride a multiple of 8, got D={D} stride {h.stride(0)}")
+    dev = weight.device
+    if dev.type != "cuda" or h.device != dev or out.device != dev:
+        bad(f"all tensors must be on one CUDA device, got h {h.device}, weight {dev}, out {out.device}")
+    _ck(_lib().adapcc_lm_head_logits(c_void_p(h.data_ptr()), h.stride(0), c_void_p(weight.data_ptr()), V, D,
+                                     c_void_p(out.data_ptr()), B, _stream()), "lm_head_logits")
+    return out
+
+
+def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int, top_p: float,
+                   seeds: torch.Tensor, pos: torch.Tensor, step: torch.Tensor, min_new: int,
+                   suppress_ids: Optional[torch.Tensor], stop_ids: Optional[torch.Tensor], done: torch.Tensor,
+                   next_ids: torch.Tensor, tokens: torch.Tensor) -> None:
+    """One seeded top-k / top-p draw per row, on the device (the definition in ``ops/sampling.py``, which computes the
+    same in fp64). ``logits`` fp32 [B, ld] (the first ``vocab`` columns used), ``seeds`` int64 [B], ``pos`` int32 [B]
+    (position of the drawn token: the Philox counter), ``step`` int32 [1] (tokens generated so far; incremented),
+    ``suppress_ids`` / ``stop_ids`` int32 lists or None, ``done`` int32 [B]. Writes the token into ``next_ids`` int64
+    [B] and column ``step`` of ``tokens`` int64 [B, max_new] (-1 for a stop id or a finished row) and sets ``done`` on
+    a stop id. ``temperature == 0`` is greedy. No host sync, so it can be captured in a CUDA graph."""
+    def bad(msg):
+        raise ValueError(f"sample_tokens_: {msg}")
+
+    if not temperature >= 0 or not top_k >= 0 or not 0 < top_p <= 1:
+        bad(f"need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
+        bad(f"logits must be fp32 [B, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
+    B = logits.shape[0]
+    if not 1 <= vocab <= min(logits.shape[1], SAMPLE_MAX_VOCAB):
+        bad(f"vocab must be in [1, min(ld = {logits.shape[1]}, {SAMPLE_MAX_VOCAB})], got {vocab}")
+    for name, t, dt in (("seeds", seeds, torch.int64), ("pos", pos, torch.int32), ("done", done, torch.int32),
+                        ("next_ids", next_ids, torch.int64)):
+        if t.dtype != dt or not t.is_contiguous() or t.numel() != B:
+            bad(f"{name} must be a contiguous {dt} tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if step.dtype != torch.int32 or step.numel() != 1:
+        bad(f"step must be a 1-element int32 tensor, got {step.dtype} {tuple(step.shape)}")
+    if tokens.dtype != torch.int64 or tokens.dim() != 2 or tokens.shape[0] != B or not tokens.is_contiguous():
+        bad(f"tokens must be a contiguous int64 [{B}, max_new] tensor, got {tokens.dtype} {tuple(tokens.shape)}")
+    lists = []
+    for name, t in (("suppress_ids", suppress_ids), ("stop_ids", stop_ids)):
+        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 1
+                              or t.numel() > SAMPLE_MAX_IDS):
+            bad(f"{name} must be a contiguous 1-D int32 tensor of at most {SAMPLE_MAX_IDS} ids, got "
+                f"{t.dtype} {tuple(t.shape)}")
+        lists.append((c_void_p(t.data_ptr() if t is not None and t.numel() else None),
+                      t.numel() if t is not None else 0))
+    dev = logits.device
+    others = [seeds, pos, step, done, next_ids, tokens] + [t for t in (suppress_ids, stop_ids) if t is not None]
+    if dev.type != "cuda" or any(t.device != dev for t in others):
+        bad(f"all tensors must be on one CUDA device, got logits on {dev} and "
+            f"{sorted(set(str(t.device) for t in others))}")
+    (sup, n_sup), (stop, n_stop) = lists
+    _ck(_lib().adapcc_sample_tokens(c_void_p(logits.data_ptr()), logits.stride(0), int(vocab), B, float(temperature),
+                                    int(top_k), float(top_p), c_void_p(seeds.data_ptr()), c_void_p(pos.data_ptr()),
+                                    c_void_p(step.data_ptr()), int(min_new), sup, n_sup, stop, n_stop,
+                                    c_void_p(done.data_ptr()), c_void_p(next_ids.data_ptr()),
+                                    c_void_p(tokens.data_ptr()), tokens.shape[1], _stream()), "sample_tokens")

@@ -32,6 +32,10 @@ def main():
     p.add_argument("--temperature", type=float, default=0.7)
     p.add_argument("--top_k", type=int, default=20)
     p.add_argument("--top_p", type=float, default=0.9)
+    p.add_argument("--batch_size", type=int, default=0,
+                   help="f1: generate this many replies at a time with GPT2DoubleHeads.generate (0: one by one). The "
+                        "batched path truncates history so the reply fits up front and suppresses special tokens "
+                        "before filtering, so its F1 is a different sample")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -43,7 +47,8 @@ def main():
     if a.eval_type == "f1":
         kw = dict(max_length=a.max_length, min_length=a.min_length, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p,
                   no_sample=a.no_sample)
-    res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed, **kw)
+    res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
+                           a.batch_size, **kw)
     print(json.dumps(res))
 
 
