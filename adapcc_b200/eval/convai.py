@@ -27,18 +27,12 @@ import torch.nn.functional as F
 
 from ..data.personachat import IGNORE, build_input_from_segments
 from ..data.tokenizer import DialogTokenizer
+from ..ops.sampling import top_filtering
 
 
 # ----------------------------------------------------------------------------------------------------------------
 # model access (the training forward only returns losses)
 # ----------------------------------------------------------------------------------------------------------------
-def _lm_logits(model, h: torch.Tensor, head: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """fp32 logits of hidden states ``h``; ``head``: the fp32 copy of the tied table, when the caller keeps one."""
-    if head is None:
-        head = model.wte.weight.float()
-    return (h.float() @ head.t())[..., : model.cfg.vocab_size]
-
-
 @torch.no_grad()
 def mc_scores(model, input_ids: torch.Tensor, token_type_ids: torch.Tensor, mc_token_ids: torch.Tensor) -> torch.Tensor:
     """Multiple-choice logits ``[B, C]`` for ``[B, C, T]`` inputs."""
@@ -51,21 +45,6 @@ def mc_scores(model, input_ids: torch.Tensor, token_type_ids: torch.Tensor, mc_t
 # ----------------------------------------------------------------------------------------------------------------
 # sampling
 # ----------------------------------------------------------------------------------------------------------------
-def top_filtering(logits: torch.Tensor, top_k: int = 0, top_p: float = 0.9, threshold: float = -float("inf")) -> torch.Tensor:
-    """Top-k, nucleus and absolute-threshold filtering of a 1-D logit vector (returns a new tensor)."""
-    logits = logits.clone()
-    if top_k > 0:
-        kth = torch.topk(logits, min(top_k, logits.numel())).values[-1]
-        logits[logits < kth] = -float("inf")
-    if top_p > 0.0:
-        srt, idx = torch.sort(logits, descending=True)
-        beyond = torch.cumsum(F.softmax(srt, dim=-1), dim=-1) > top_p
-        beyond = torch.cat([beyond.new_zeros(1), beyond[:-1]])          # keep the token that crosses the threshold
-        logits[idx[beyond]] = -float("inf")
-    logits[logits < threshold] = -float("inf")
-    return logits
-
-
 @torch.no_grad()
 def sample_reply(model, tokenizer: DialogTokenizer, persona, history, max_length: int = 20, min_length: int = 1,
                  temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9, no_sample: bool = False,
@@ -77,28 +56,22 @@ def sample_reply(model, tokenizer: DialogTokenizer, persona, history, max_length
     When an input is the previous one plus the newest token, that token costs one cached decode step
     (``GPT2DoubleHeads.decode_step``, graph-replayed on CUDA with the native kernels); when history truncation moved
     the prefix, the input is prefilled into the cache again."""
-    from ..models.gpt2 import decoder
+    from ..models.gpt2 import CachedDecoder
 
     special = set(tokenizer.special_ids)
     out: List[int] = []
     head = model.wte.weight.float()                            # the fp32 LM head, converted once per call
-    cache = dec = prev = None
+    dec, prev = CachedDecoder(model), None
     for step in range(max_length):
         inst = build_input_from_segments(persona, history, out, tokenizer, with_eos=False, max_len=model.cfg.n_positions)
         cur = (inst.input_ids, inst.token_type_ids)
         if (prev is not None and len(cur[0]) == len(prev[0]) + 1 and cur[0][:-1] == prev[0]
                 and cur[1][:-1] == prev[1]):
-            if dec is None:
-                dec = decoder(model, cache)
-            h = dec(torch.tensor(cur[0][-1:], device=device), torch.tensor(cur[1][-1:], device=device))[0]
+            h = dec.extend(torch.tensor([cur[0][-1:]], device=device), torch.tensor([cur[1][-1:]], device=device))
         else:
-            if cache is None:
-                cache = model.new_cache(1)
-            ids = torch.tensor(inst.input_ids, device=device).unsqueeze(0)
-            tt = torch.tensor(inst.token_type_ids, device=device).unsqueeze(0)
-            h = model.hidden(ids, tt, cache=cache)[0, -1]
+            h = dec.restart(torch.tensor([cur[0]], device=device), torch.tensor([cur[1]], device=device))
         prev = cur
-        logits = _lm_logits(model, h, head) / max(temperature, 1e-6)
+        logits = model.lm_logits(h[0], head) / max(temperature, 1e-6)   # 1-D h: the GEMV the draws were made with
         probs = F.softmax(top_filtering(logits, top_k, top_p), dim=-1)
         nxt = int(torch.argmax(probs)) if no_sample else int(torch.multinomial(probs, 1, generator=generator))
         if step < min_length and nxt in special:
@@ -160,7 +133,7 @@ def evaluate_tensors(model, loader: Iterable[Dict[str, torch.Tensor]], device="c
         keep = labels != IGNORE
         if keep.any():
             rows = gold[:, :-1].reshape(-1, gold.shape[-1])[keep]
-            nll_sum += float(F.cross_entropy(_lm_logits(model, rows), labels[keep], reduction="sum"))
+            nll_sum += float(F.cross_entropy(model.lm_logits(rows), labels[keep], reduction="sum"))
             n_tok += int(keep.sum())
     nll = nll_sum / max(1, n_tok)
     return {"hits@1": hits / max(1, total), "nll": nll, "ppl": math.exp(min(nll, 50.0)), "examples": total, "tokens": n_tok,
@@ -208,7 +181,7 @@ def next_word_probability(model, tokenizer: DialogTokenizer, persona, history, p
     inst = build_input_from_segments(persona, history, partial, tokenizer, with_eos=False, max_len=model.cfg.n_positions)
     ids = torch.tensor(inst.input_ids, device=device).unsqueeze(0)
     tt = torch.tensor(inst.token_type_ids, device=device).unsqueeze(0)
-    probs = F.softmax(_lm_logits(model, model.hidden(ids, tt)[0, -1]), dim=-1)
+    probs = F.softmax(model.lm_logits(model.hidden(ids, tt)[0, -1]), dim=-1)
     dist: Dict[str, float] = {}
     for prefix, words in prefix2words.items():
         p = float(probs[prefix])

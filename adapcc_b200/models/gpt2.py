@@ -23,13 +23,14 @@ from __future__ import annotations
 import math
 import os
 from dataclasses import dataclass
-from typing import List, Optional, Sequence, Tuple
+from typing import Callable, List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.layers import FusedLayerNorm, FusedLinear
+from ..ops.sampling import sample_reference, top_filtering
 
 
 @dataclass
@@ -362,21 +363,32 @@ class GPT2DoubleHeads(nn.Module):
         N, T = input_ids.shape
         if cache is not None:
             cache.reset(lengths if lengths is not None else [T] * N, T)
-        if (self.fused_embed and input_ids.is_cuda and self.wte.weight.dtype == torch.bfloat16
+        return self._blocks(self._embed(input_ids, token_type_ids), cache)
+
+    def _embed(self, ids: torch.Tensor, tt: Optional[torch.Tensor], pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """wte[ids] + wpe[pos] (+ wte[tt]), added in that order: [*ids.shape, D]; ``pos`` defaults to 0..T-1 in every
+        row of ids [N, T]. One ``fused_embedding_sum`` for bf16 CUDA tables if ``fused_embed``."""
+        if (self.fused_embed and ids.is_cuda and self.wte.weight.dtype == torch.bfloat16
                 and self.wpe.weight.dtype == torch.bfloat16):
             from ..ops import fused_embedding_sum
-            key = (N, T, input_ids.device)
-            pos = self._pos_cache.get(key)
-            if pos is None:
-                pos = self._pos_cache[key] = torch.arange(T, device=input_ids.device).repeat(N)
-            lookups = [(0, input_ids), (1, pos)] + ([(0, token_type_ids)] if token_type_ids is not None else [])
-            x = fused_embedding_sum([self.wte.weight, self.wpe.weight], lookups).view(N, T, -1)
-        else:
-            pos = torch.arange(T, device=input_ids.device)
-            x = self.wte(input_ids) + self.wpe(pos)[None]
-            if token_type_ids is not None:
-                x = x + self.wte(token_type_ids)
-        return self._blocks(x, cache)
+            if pos is None:                  # cached: a captured training step reads the same positions every replay
+                N, T = ids.shape
+                pos = self._pos_cache.get((N, T, ids.device))
+                if pos is None:
+                    pos = self._pos_cache[(N, T, ids.device)] = torch.arange(T, device=ids.device).repeat(N)
+            lookups = [(0, ids), (1, pos)] + ([(0, tt)] if tt is not None else [])
+            return fused_embedding_sum([self.wte.weight, self.wpe.weight], lookups).view(*ids.shape, -1)
+        # the default positions broadcast over the rows, so wpe's gradient is summed over them before the lookup
+        x = self.wte(ids) + self.wpe(torch.arange(ids.shape[-1], device=ids.device) if pos is None else pos)
+        if tt is not None:
+            x = x + self.wte(tt)
+        return x
+
+    def lm_logits(self, h: torch.Tensor, head: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """fp32 logits [..., vocab_size] of ``h`` [..., D] through the tied head; ``head``: a kept fp32 ``wte.weight``."""
+        if head is None:
+            head = self.wte.weight.float()
+        return (h.float() @ head.t())[..., :self.cfg.vocab_size]
 
     def _blocks(self, x: torch.Tensor, cache: Optional["KVCache"]) -> torch.Tensor:
         if self.fuse_add_ln:
@@ -409,17 +421,7 @@ class GPT2DoubleHeads(nn.Module):
         if input_ids.dim() != 1 or B != cache.batch:
             raise ValueError(f"decode_step: input_ids must be [{cache.batch}], got {tuple(input_ids.shape)}")
         cache.check_room()
-        pos = cache.lens.long()
-        if (self.fused_embed and input_ids.is_cuda and self.wte.weight.dtype == torch.bfloat16
-                and self.wpe.weight.dtype == torch.bfloat16):
-            from ..ops import fused_embedding_sum
-            lookups = [(0, input_ids), (1, pos)] + ([(0, token_type_ids)] if token_type_ids is not None else [])
-            x = fused_embedding_sum([self.wte.weight, self.wpe.weight], lookups)
-        else:
-            x = self.wte(input_ids) + self.wpe(pos)
-            if token_type_ids is not None:
-                x = x + self.wte(token_type_ids)
-        h = self._blocks(x, cache)
+        h = self._blocks(self._embed(input_ids, token_type_ids, cache.lens.long()), cache)
         cache.advance()
         return h
 
@@ -445,8 +447,6 @@ class GPT2DoubleHeads(nn.Module):
         every token after the first replays one CUDA graph of decode step, LM head and sampler, which feeds the drawn ids
         back into its own input; the host reads the done flags once every 8 tokens, a step late, to stop early.
         Elsewhere the same loop runs eagerly with fp32 PyTorch logits and ``ops.sampling.sample_reference``."""
-        from ..ops.sampling import sample_reference
-
         cfg = self.cfg
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
             raise ValueError(f"generate: input_ids must be [B, T], got {tuple(input_ids.shape)}")
@@ -487,7 +487,7 @@ class GPT2DoubleHeads(nn.Module):
             for i in range(n):
                 if i:
                     h = self.decode_step(nxt.to(dev), tt_new, cache)
-                nxt, tok, done = sample_reference(h.float() @ head.t(), cfg.vocab_size, temperature, top_k, top_p,
+                nxt, tok, done = sample_reference(self.lm_logits(h, head), cfg.vocab_size, temperature, top_k, top_p,
                                                   seeds, cache.lens, i, min_new_tokens, suppress_ids, stop_ids, done)
                 tokens[:, i] = tok.to(dev)
                 if bool(done.all()):
@@ -514,25 +514,12 @@ class GPT2DoubleHeads(nn.Module):
         head_and_sample(h)                          # the first token, from the prefill's last positions
         if n == 1:
             return tokens, (tokens >= 0).sum(1)
-        # DecodeGraph's warm-up and capture, with the LM head and the sampler inside the graph
-        lens0, host0 = cache.lens.clone(), list(cache.host_lens)
-        s = torch.cuda.Stream(device=dev)
-        s.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(s):                  # writes only slot lens[b], which the first replay overwrites
-            self.decode_step(next_ids, tt_new, cache)
-        torch.cuda.current_stream(dev).wait_stream(s)
-        cache.lens.copy_(lens0)
-        cache.host_lens = host0
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            head_and_sample(self.decode_step(next_ids, tt_new, cache))
-        cache.host_lens = host0
+        # the sampler writes each token's ids into the graph's own input buffer
+        graph = DecodeGraph(self, cache, tt_new is not None, head=head_and_sample, ids=next_ids, tt=tt_new)
         flags = torch.empty(B, dtype=torch.int32, pin_memory=True)
         copied = None
         for i in range(1, n):
-            cache.check_room()
             graph.replay()
-            cache.advance_host()
             if i % 8 == 0:                          # the flags copied 8 tokens ago are ready by now: no stall
                 if copied is not None:
                     copied.synchronize()
@@ -590,13 +577,18 @@ class DecodeGraph:
     ``FlatDataParallel.capture``): the token ids (and token types) go through static input buffers, the cache's device
     state is read and advanced inside the graph, so one capture serves every later step of that cache, also after a new
     prefill into it. Replays give the same bits as eager steps. The returned hidden state [B, D] is a static buffer that
-    the next replay overwrites."""
+    the next replay overwrites.
 
-    def __init__(self, model: "GPT2DoubleHeads", cache: KVCache, token_types: bool = True):
+    ``head`` runs on the step's hidden state inside the graph (the warm-up step leaves it out, so it may change state).
+    ``ids`` / ``tt``: input buffers to read instead of the graph's own (``tt`` replaces the one ``token_types`` asks
+    for), for a caller that fills them on the device and steps with ``replay``. ``generate`` uses all three."""
+
+    def __init__(self, model: "GPT2DoubleHeads", cache: KVCache, token_types: bool = True,
+                 head: Optional[Callable] = None, ids: Optional[torch.Tensor] = None, tt: Optional[torch.Tensor] = None):
         dev = cache.lens.device
         self.cache = cache
-        self.ids = torch.zeros(cache.batch, dtype=torch.long, device=dev)
-        self.tt = torch.zeros_like(self.ids) if token_types else None
+        self.ids = torch.zeros(cache.batch, dtype=torch.long, device=dev) if ids is None else ids
+        self.tt = tt if tt is not None or not token_types else torch.zeros_like(self.ids)
         lens0, host0 = cache.lens.clone(), list(cache.host_lens)
         s = torch.cuda.Stream(device=dev)
         s.wait_stream(torch.cuda.current_stream(dev))
@@ -608,26 +600,62 @@ class DecodeGraph:
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
             self.h = model.decode_step(self.ids, self.tt, cache)
+            if head is not None:
+                head(self.h)
         cache.host_lens = host0                        # capturing ran the host side of a step, not the step
 
     def __call__(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor] = None) -> torch.Tensor:
         if (token_type_ids is None) != (self.tt is None):
             raise ValueError("DecodeGraph: token types given at capture and at replay must match")
-        self.cache.check_room()
         self.ids.copy_(input_ids, non_blocking=True)
         if self.tt is not None:
             self.tt.copy_(token_type_ids, non_blocking=True)
+        return self.replay()
+
+    def replay(self) -> torch.Tensor:
+        """One step on what the input buffers hold now, without copying anything into them."""
+        self.cache.check_room()
         self.graph.replay()
         self.cache.advance_host()
         return self.h
 
 
-def decoder(model: "GPT2DoubleHeads", cache: KVCache, token_types: bool = True):
-    """``(ids [B], tt [B] | None) -> h [B, D]``, one decode step into ``cache``: graph-replayed (``DecodeGraph``) when
-    the cache runs on the native kernel (bf16 on CUDA), eager ``decode_step`` otherwise."""
-    if cache.work is not None:
-        return DecodeGraph(model, cache, token_types)
-    return lambda ids, tt=None: model.decode_step(ids, tt, cache)
+class CachedDecoder:
+    """The KV cache of a sequential sampling loop (``sample_sequence``, ``eval.convai.sample_reply``): ``restart``
+    starts a sequence of B rows, ``extend`` appends one token per row; both return the last position's hidden state
+    [B, D]. While the sequence fits into ``n_positions`` a token is one decode step (a ``DecodeGraph`` replay on the
+    native kernel, eager otherwise); beyond that ``hidden`` runs uncached over the last ``n_positions`` tokens."""
+
+    def __init__(self, model: "GPT2DoubleHeads"):
+        self.model, self.n_pos = model, model.cfg.n_positions
+        self.cache = self.graph = None
+
+    def restart(self, ids: torch.Tensor, tt: Optional[torch.Tensor]) -> torch.Tensor:
+        """A new sequence ``ids`` [B, T], token types ``tt`` [B, T] or None; prefilled into the cache if T fits."""
+        self.parts, self.T = [(ids, tt)], ids.shape[1]       # the sequence in pieces, concatenated when a window needs it
+        if self.T > self.n_pos:
+            return self._window()
+        if self.cache is None:
+            self.cache = self.model.new_cache(ids.shape[0])
+        return self.model.hidden(ids, tt, cache=self.cache)[:, -1]
+
+    def extend(self, ids: torch.Tensor, tt: Optional[torch.Tensor]) -> torch.Tensor:
+        """Append ``ids`` [B, 1] with token types ``tt`` [B, 1] (None if ``restart`` had none)."""
+        self.parts.append((ids, tt))
+        self.T += 1
+        if self.T > self.n_pos:
+            return self._window()
+        ids, tt = ids[:, -1], tt[:, -1] if tt is not None else None   # T fits, so the cache holds all but this token
+        if self.cache.work is None:
+            return self.model.decode_step(ids, tt, self.cache)
+        if self.graph is None:
+            self.graph = DecodeGraph(self.model, self.cache, tt is not None)
+        return self.graph(ids, tt)
+
+    def _window(self) -> torch.Tensor:
+        ids, tt = (torch.cat(p, 1) if p[0] is not None else None for p in zip(*self.parts))
+        self.parts = [(ids, tt)]
+        return self.model.hidden(ids[:, -self.n_pos:], tt[:, -self.n_pos:] if tt is not None else None)[:, -1]
 
 
 @torch.no_grad()
@@ -637,43 +665,23 @@ def sample_sequence(model: "GPT2DoubleHeads", input_ids: torch.Tensor, token_typ
                     generator: Optional[torch.Generator] = None) -> torch.Tensor:
     """Nucleus / top-k sampling of a reply, one token at a time (the decoding loop of the reference's interact.py:
     ``top_filtering`` + ``sample_sequence``, /root/reference/models/gpt2/interact.py). ``input_ids`` [1, T]; new tokens
-    get ``reply_type`` as their token type when given. The prompt is prefilled into a KV cache once and every new token
-    costs one ``decode_step`` (graph-replayed on CUDA with the native kernels); once the sequence outgrows
-    ``n_positions`` the window slides, every position moves, and each token re-runs the model over the window."""
-    ids = input_ids.clone()
-    tt = token_type_ids.clone() if token_type_ids is not None else None
-    vocab, n_pos = model.cfg.vocab_size, model.cfg.n_positions
+    get ``reply_type`` as their token type when given, else the prompt's last one. The prompt is prefilled into a KV
+    cache once and every new token costs one ``decode_step`` (graph-replayed on CUDA with the native kernels); once the
+    sequence outgrows ``n_positions`` the window slides and each token re-runs the model over it (``CachedDecoder``)."""
     head = model.wte.weight.float()                            # the fp32 LM head, converted once per call
-    cache = step = None
-    for _ in range(max_new_tokens):
-        T = ids.shape[1]
-        if T > n_pos:                                          # sliding window: the cache no longer applies
-            h = model.hidden(ids[:, T - n_pos:], tt[:, T - n_pos:] if tt is not None else None)[:, -1]
-        elif cache is None:
-            cache = model.new_cache(ids.shape[0])
-            h = model.hidden(ids, tt, cache=cache)[:, -1]
-        else:
-            if step is None:
-                step = decoder(model, cache, tt is not None)
-            h = step(ids[:, -1], tt[:, -1] if tt is not None else None)
-        logits = (h.float() @ head.t())[:, :vocab] / max(temperature, 1e-6)
-        if top_k > 0:
-            kth = torch.topk(logits, min(top_k, vocab)).values[:, -1:]
-            logits = logits.masked_fill(logits < kth, float("-inf"))
-        if 0.0 < top_p < 1.0:
-            srt, idx = torch.sort(logits, descending=True)
-            cum = torch.softmax(srt, -1).cumsum(-1)
-            drop = cum > top_p
-            drop[:, 1:] = drop[:, :-1].clone()                  # keep the first token that crosses the threshold
-            drop[:, 0] = False
-            logits = logits.masked_fill(torch.zeros_like(drop).scatter(1, idx, drop), float("-inf"))
+    dec = CachedDecoder(model)
+    if token_type_ids is not None and reply_type is None:
+        reply_type = int(token_type_ids[0, -1])
+    out = []
+    for i in range(max_new_tokens):
+        h = (dec.extend(nxt, torch.full_like(nxt, reply_type) if token_type_ids is not None else None) if i
+             else dec.restart(input_ids, token_type_ids))
+        logits = top_filtering(model.lm_logits(h, head) / max(temperature, 1e-6), top_k, top_p)
         nxt = torch.multinomial(torch.softmax(logits, -1), 1, generator=generator)
-        ids = torch.cat([ids, nxt], 1)
-        if tt is not None:
-            tt = torch.cat([tt, torch.full_like(nxt, reply_type if reply_type is not None else int(tt[0, -1]))], 1)
+        out.append(nxt)
         if eos_token is not None and int(nxt) == eos_token:
             break
-    return ids[:, input_ids.shape[1]:]
+    return torch.cat(out, 1) if out else input_ids[:, :0]
 
 
 def lm_rows_needed(lm_labels: torch.Tensor, multiple: int = 256) -> int:

@@ -48,6 +48,23 @@ def uniform(seed: int, pos: int) -> float:
     return (philox4x32_10((pos, 0, 0, 0), (seed & _MASK, seed >> 32))[0] >> 8) * 2.0 ** -24
 
 
+def top_filtering(logits: torch.Tensor, top_k: int = 0, top_p: float = 0.9, threshold: float = -float("inf")) -> torch.Tensor:
+    """The sort-based top-k / nucleus / threshold filter of the sequential sampling loops (steps 4 and 6 of the
+    definition, in the logits' own precision): logits [..., V] with the dropped entries at -inf along the last
+    dimension; the input is left as it is. The nucleus step runs only for ``0 < top_p < 1``."""
+    if top_k > 0:
+        kth = torch.topk(logits, min(top_k, logits.shape[-1])).values[..., -1:]
+        logits = logits.masked_fill(logits < kth, float("-inf"))
+    if 0.0 < top_p < 1.0:
+        srt, idx = torch.sort(logits, descending=True)
+        drop = torch.softmax(srt, -1).cumsum(-1) > top_p
+        drop = torch.cat([torch.zeros_like(drop[..., :1]), drop[..., :-1]], -1)   # keep the token that crosses top_p
+        logits = logits.masked_fill(torch.zeros_like(drop).scatter(-1, idx, drop), float("-inf"))
+    if threshold > -float("inf"):
+        logits = logits.masked_fill(logits < threshold, float("-inf"))
+    return logits
+
+
 def reference_row(logits, temperature: float, top_k: int, top_p: float, seed: int, pos: int, step: int = 0,
                   min_new: int = 0, suppress_ids: Sequence[int] = ()) -> Dict[str, object]:
     """One row of the definition (steps 1-7) in fp64. ``logits``: the row's ``vocab`` fp32 values. Returns the token

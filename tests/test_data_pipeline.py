@@ -141,6 +141,14 @@ def test_metrics_helpers():
     assert torch.equal(logits, torch.tensor([2.0, 1.0, 0.5, -1.0, -3.0]))           # input untouched
 
 
+def test_top_filtering_keeps_every_token_at_top_p_1():
+    # the fp32 cumulative softmax of a GPT-2-sized row passes 1.0 by rounding before its last entry: top_p = 1 must
+    # not turn that into dropped tokens
+    logits = torch.randn(50257, generator=torch.Generator().manual_seed(0)) * 3
+    assert torch.isfinite(top_filtering(logits, top_k=0, top_p=1.0)).all()
+    assert int(torch.isfinite(top_filtering(logits, top_k=40, top_p=1.0)).sum()) == 40
+
+
 def test_train_evaluate_interact_end_to_end(tmp_path):
     """examples/train_gpt2_personachat.py on 2 gloo ranks (tokenizer built by rank 0, distributed loaders, DDP + the
     communicator's hook, linear lr decay, validation all-reduced, checkpoint), then the evaluation and chat scripts."""
