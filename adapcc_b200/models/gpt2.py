@@ -530,6 +530,128 @@ class GPT2DoubleHeads(nn.Module):
                 copied.record()
         return tokens, (tokens >= 0).sum(1)
 
+    @torch.no_grad()
+    def beam_search(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
+                    token_type_ids: Optional[torch.Tensor] = None, reply_type=None, num_beams: int = 4,
+                    max_new_tokens: int = 20, length_penalty: float = 1.0, stop_ids: Sequence[int] = (),
+                    suppress_ids: Sequence[int] = (), min_new_tokens: int = 0
+                    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
+
+        ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
+        ``reply_type`` and the token types of new tokens work as in ``generate``. A token in ``stop_ids`` (at most 8)
+        finishes a hypothesis; while fewer than ``min_new_tokens`` tokens are generated, ``suppress_ids`` cannot be
+        chosen. A hypothesis of L tokens (its stop token included) scores ``sum of log-probabilities / L **
+        length_penalty``. An item stops as soon as no live beam can beat its K-th finished hypothesis, which never
+        changes its result. An item's result depends on its prompt and the scalars only, not on the other items.
+
+        Returns ``(tokens, n_new, scores)``: the best hypothesis of each item as int64 [B, max_new_tokens] (the stop
+        token excluded, padded with -1), its length int64 [B] and its normalised score fp32 [B].
+
+        Each prompt is prefilled once and its keys and values copied to its ``num_beams`` rows of a cache of
+        ``max(lengths) + max_new_tokens`` positions (more than ``n_positions`` is a ``ValueError``). On CUDA with bf16
+        weights every token after the first replays one CUDA graph of decode step, LM head (``ops.lm_head_logits_``),
+        selection (``ops.beam_step_``) and cache reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the
+        host reads the done flags once every 8 tokens, a period late. Elsewhere the same loop runs eagerly with fp32
+        PyTorch logits, ``ops.beam.BeamReference`` and torch indexing."""
+        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, LM_HEAD_MAX_ROWS
+        from ..ops.beam import BeamReference, best_hypotheses
+
+        cfg = self.cfg
+        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
+            raise ValueError(f"beam_search: input_ids must be [B, T], got {tuple(input_ids.shape)}")
+        B, T = input_ids.shape
+        K, n = int(num_beams), int(max_new_tokens)
+        dev = input_ids.device
+        lengths = [T] * B if lengths is None else [int(x) for x in lengths]
+        if len(lengths) != B or any(not 1 <= x <= T for x in lengths):
+            raise ValueError(f"beam_search: need {B} lengths in [1, {T}], got {lengths}")
+        if not 1 <= K <= BEAM_MAX_BEAMS:
+            raise ValueError(f"beam_search: num_beams must be in [1, {BEAM_MAX_BEAMS}], got {num_beams}")
+        if n < 1 or int(min_new_tokens) < 0:
+            raise ValueError(f"beam_search: need max_new_tokens >= 1 and min_new_tokens >= 0, got {max_new_tokens}, "
+                             f"{min_new_tokens}")
+        if len(stop_ids) > BEAM_MAX_STOP or len(suppress_ids) > BEAM_MAX_SUPPRESS:
+            raise ValueError(f"beam_search: at most {BEAM_MAX_STOP} stop ids and {BEAM_MAX_SUPPRESS} suppressed ids, "
+                             f"got {len(stop_ids)} and {len(suppress_ids)}")
+        t_max = max(lengths) + n
+        if t_max > cfg.n_positions:
+            raise ValueError(f"beam_search: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds "
+                             f"n_positions = {cfg.n_positions}")
+        weight = self.wte.weight
+        native = weight.is_cuda and weight.dtype == torch.bfloat16
+        if native and B * K > LM_HEAD_MAX_ROWS:
+            raise ValueError(f"beam_search: at most {LM_HEAD_MAX_ROWS} beam rows (batch x num_beams) per call on the "
+                             f"native path, got {B} x {K}")
+        last = torch.tensor(lengths, device=dev) - 1
+        tt_new = None
+        if reply_type is not None:
+            tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
+        elif token_type_ids is not None:
+            tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
+        if tt_new is not None:
+            tt_new = tt_new.repeat_interleave(K)
+        # one prefill per prompt, its keys and values copied to the prompt's K rows (the beams share that region)
+        pre = self.new_cache(B, T)
+        h = self.hidden(input_ids, token_type_ids, cache=pre, lengths=lengths)[torch.arange(B, device=dev), last]
+        cache = self.new_cache(B * K, t_max)
+        cache.reset([x for x in lengths for _ in range(K)], T)
+        cache.k[:, :, :, :T].copy_(pre.k.repeat_interleave(K, dim=1))
+        cache.v[:, :, :, :T].copy_(pre.v.repeat_interleave(K, dim=1))
+        del pre
+        h = h.repeat_interleave(K, dim=0).contiguous()
+        V = cfg.vocab_size
+        if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
+            ref = BeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens)
+            head = weight.float()
+            for i in range(n):
+                if i:
+                    h = self.decode_step(nxt.to(dev), tt_new, cache)
+                nxt, parent = ref.step(self.lm_logits(h, head))
+                rows = parent.to(dev)
+                cache.k.copy_(cache.k[:, rows])
+                cache.v.copy_(cache.v[:, rows])
+                if ref.done.all():
+                    break
+            return tuple(t.to(dev) for t in ref.result())
+
+        from ..ops import BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
+
+        st = BeamState(B, K, n, length_penalty, dev)
+        logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
+        sup = torch.tensor(list(suppress_ids), dtype=torch.int32, device=dev)
+        stop = torch.tensor(list(stop_ids), dtype=torch.int32, device=dev)
+        prompt_len = cache.lens.clone()
+        scratch = torch.empty(kv_reorder_scratch_numel(cache.k, n), dtype=cache.k.dtype, device=dev)
+
+        def select(hidden):
+            lm_head_logits_(hidden, weight, logits)
+            beam_step_(logits, V, st, min_new_tokens, sup, stop)
+            kv_reorder_(cache.k, cache.v, st.parent, prompt_len, cache.lens, n, scratch)
+
+        select(h)                                   # the first selection, from the prefill's last positions
+        if n > 1:
+            # beam_step_ writes the new beams' tokens into the graph's own input buffer
+            graph = DecodeGraph(self, cache, tt_new is not None, head=select, ids=st.next_ids, tt=tt_new)
+            flags = torch.empty(B, dtype=torch.int32, pin_memory=True)
+            copied = None
+            for i in range(1, n):
+                graph.replay()
+                if i % 8 == 0:                      # the flags copied 8 tokens ago are ready by now: no stall
+                    if copied is not None:
+                        copied.synchronize()
+                        if bool(flags.all()):
+                            break
+                    flags.copy_(st.done, non_blocking=True)
+                    copied = torch.cuda.Event()
+                    copied.record()
+        count = st.fin_count.cpu().tolist()
+        score, n_tok, src = st.fin_score.cpu().tolist(), st.fin_n.cpu().tolist(), st.fin_src.cpu().tolist()
+        fin = [list(zip(score[b], n_tok[b], src[b]))[:count[b]] for b in range(B)]
+        hist_tok = st.hist_tok.view(n, B, K).cpu().numpy()
+        hist_back = st.hist_back.view(n, B, K).cpu().numpy()
+        return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n))
+
     def forward(self, input_ids, token_type_ids=None, mc_token_ids=None, lm_labels=None, mc_labels=None,
                 lm_coef: float = 1.0, mc_coef: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """-> (loss, lm_loss, mc_loss). Shapes as in the reference: [B, C, T] ids/labels, [B, C]

@@ -45,6 +45,11 @@ def _lib():
         lib.adapcc_sample_tokens.argtypes = ([c_void_p, c_int, c_int, c_int, c_float, c_int, c_float]
                                              + [c_void_p] * 3 + [c_int, c_void_p, c_int, c_void_p, c_int]
                                              + [c_void_p] * 3 + [c_int, c_void_p])
+        lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
+                                         + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
+                                         + [c_void_p] * 10 + [c_void_p])
+        lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p,
+                                                                                                c_void_p]
         _bound = True
     return lib
 
@@ -362,3 +367,132 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
                                     c_void_p(step.data_ptr()), int(min_new), sup, n_sup, stop, n_stop,
                                     c_void_p(done.data_ptr()), c_void_p(next_ids.data_ptr()),
                                     c_void_p(tokens.data_ptr()), tokens.shape[1], _stream()), "sample_tokens")
+
+
+# ---- beam search selection and KV-cache reordering (csrc/ops_beam.cu) ----------------------------------------------
+BEAM_MAX_BEAMS = 16            # beams per item
+BEAM_MAX_STOP = 8              # stop ids (each row keeps its K + n_stop best candidates)
+BEAM_MAX_SUPPRESS = 1024       # suppressed ids
+
+
+class BeamState:
+    """Device state of a batched beam search of ``batch`` items with ``num_beams`` beams each and up to ``max_new``
+    tokens, as ``beam_step_`` reads and writes it. Rows are ``b * num_beams + k``.
+
+    ``scores`` fp32 [B·K] running log-probability sums (beam 0 of each item at 0, the others dead at -inf);
+    ``step`` int32 [1]; ``done`` int32 [B]; ``next_ids`` int64 [B·K] the new beams' tokens (the decode step's input);
+    ``parent`` int32 [B·K] the row each new beam continues; ``hist_tok`` int64 / ``hist_back`` int32 [max_new, B·K]
+    each step's tokens and parent beams (0..K-1); the finished sets ``fin_score`` fp32, ``fin_n`` and ``fin_src`` int32
+    [B, K] (best first: normalised score, tokens without the stop token, and the beam whose history at step
+    ``fin_n - 1`` holds them) with ``fin_count`` int32 [B]; ``pen`` fp32 [max_new + 1], ``pen[L] = L ** length_penalty``
+    rounded to fp32 once on the host, so the kernel needs no ``powf``."""
+
+    def __init__(self, batch: int, num_beams: int, max_new: int, length_penalty: float, device):
+        B, K, n = int(batch), int(num_beams), int(max_new)
+        if B < 1 or not 1 <= K <= BEAM_MAX_BEAMS or n < 1:
+            raise ValueError(f"BeamState: need batch >= 1, 1 <= num_beams <= {BEAM_MAX_BEAMS} and max_new >= 1, got "
+                             f"{batch}, {num_beams}, {max_new}")
+        self.batch, self.num_beams, self.max_new, self.length_penalty = B, K, n, float(length_penalty)
+        i32, dev = dict(dtype=torch.int32, device=device), device
+        self.scores = torch.full((B, K), float("-inf"), dtype=torch.float32, device=dev)
+        self.scores[:, 0] = 0.0
+        self.scores = self.scores.reshape(B * K)
+        self.step = torch.zeros(1, **i32)
+        self.done = torch.zeros(B, **i32)
+        self.next_ids = torch.zeros(B * K, dtype=torch.int64, device=dev)
+        self.parent = torch.arange(B * K, **i32)
+        self.hist_tok = torch.full((n, B * K), -1, dtype=torch.int64, device=dev)
+        self.hist_back = torch.zeros(n, B * K, **i32)
+        self.fin_score = torch.full((B, K), float("-inf"), dtype=torch.float32, device=dev)
+        self.fin_n = torch.zeros(B, K, **i32)
+        self.fin_src = torch.zeros(B, K, **i32)
+        self.fin_count = torch.zeros(B, **i32)
+        self.pen = torch.tensor([float(L) ** self.length_penalty if L else 1.0 for L in range(n + 1)],
+                                dtype=torch.float64).to(device=dev, dtype=torch.float32)
+        self.cand = torch.empty(B * K, K + BEAM_MAX_STOP, dtype=torch.int64, device=dev)
+
+    def tensors(self):
+        """Every device tensor of the state (what ``beam_step_`` checks for one device)."""
+        return (self.scores, self.step, self.done, self.next_ids, self.parent, self.hist_tok, self.hist_back,
+                self.fin_score, self.fin_n, self.fin_src, self.fin_count, self.pen, self.cand)
+
+
+def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int = 0,
+               suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None) -> None:
+    """One beam-search selection for every item, on the device (the definition in ``ops/beam.py``, which computes the
+    same in fp64). ``logits`` fp32 [B·K, ld] (the first ``vocab`` columns used) are the beams' next-token logits;
+    ``suppress_ids`` (removed while ``state.step < min_new``) and ``stop_ids`` (at most 8; they finish a hypothesis)
+    are int32 lists or None. Updates ``state``: the new beams' tokens go into ``state.next_ids``, their parents into
+    ``state.parent`` (for ``kv_reorder_``), and ``state.step`` is incremented. No host sync, so it can be captured in a
+    CUDA graph."""
+    def bad(msg):
+        raise ValueError(f"beam_step_: {msg}")
+
+    if not isinstance(state, BeamState):
+        bad(f"state must be a BeamState, got {type(state).__name__}")
+    B, K = state.batch, state.num_beams
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1 or logits.shape[0] != B * K:
+        bad(f"logits must be fp32 [{B * K}, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
+    if not 1 <= vocab <= logits.shape[1] or K * vocab >= 1 << 32:
+        bad(f"vocab must be in [1, ld = {logits.shape[1]}] with num_beams * vocab < 2^32, got {vocab}")
+    if int(min_new) < 0:
+        bad(f"min_new must be >= 0, got {min_new}")
+    lists = []
+    for name, t, cap in (("suppress_ids", suppress_ids, BEAM_MAX_SUPPRESS), ("stop_ids", stop_ids, BEAM_MAX_STOP)):
+        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 1 or t.numel() > cap):
+            bad(f"{name} must be a contiguous 1-D int32 tensor of at most {cap} ids, got {t.dtype} {tuple(t.shape)}")
+        lists.append((c_void_p(t.data_ptr() if t is not None and t.numel() else None),
+                      t.numel() if t is not None else 0))
+    dev = logits.device
+    others = list(state.tensors()) + [t for t in (suppress_ids, stop_ids) if t is not None]
+    if dev.type != "cuda" or any(t.device != dev for t in others):
+        bad(f"all tensors must be on one CUDA device, got logits on {dev} and "
+            f"{sorted(set(str(t.device) for t in others))}")
+    (sup, n_sup), (stop, n_stop) = lists
+    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
+    _ck(_lib().adapcc_beam_step(p(logits), logits.stride(0), int(vocab), B, K, p(state.scores), p(state.step),
+                                int(min_new), sup, n_sup, stop, n_stop, p(state.pen), int(state.length_penalty > 0),
+                                state.max_new, p(state.done), p(state.cand), p(state.next_ids), p(state.parent),
+                                p(state.hist_tok), p(state.hist_back), p(state.fin_score), p(state.fin_n),
+                                p(state.fin_src), p(state.fin_count), _stream()), "beam_step")
+
+
+def kv_reorder_scratch_numel(k_cache: torch.Tensor, max_new: int) -> int:
+    """bf16 elements of the scratch ``kv_reorder_`` needs for caches shaped like ``k_cache`` [L, R, H, t_max, Dh]."""
+    L, R, H, _, Dh = k_cache.shape
+    return R * int(max_new) * L * 2 * H * Dh
+
+
+def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tensor, prompt_len: torch.Tensor,
+                lens: torch.Tensor, max_new: int, scratch: torch.Tensor) -> None:
+    """In place, for every layer l and row r with ``parent[r] != r``: ``k[l, r, :, pos] = k[l, parent[r], :, pos]`` and
+    the same for ``v``, over the generated positions ``pos = prompt_len[r] + t``, ``0 <= t < max_new``, ``pos <
+    lens[r]``. The caches are bf16 [L, R, H, t_max, Dh]; ``parent``, ``prompt_len`` and ``lens`` int32 [R]. Every
+    source is read into ``scratch`` (bf16, ``kv_reorder_scratch_numel`` elements) before anything is written, so cycles
+    and many-to-one maps come out right. The grid follows ``max_new``, not the lengths, so one capture serves every
+    step. No host sync."""
+    def bad(msg):
+        raise ValueError(f"kv_reorder_: {msg}")
+
+    if k_cache.dtype != torch.bfloat16 or v_cache.dtype != torch.bfloat16 or scratch.dtype != torch.bfloat16:
+        bad(f"k_cache, v_cache and scratch must be bf16, got {k_cache.dtype}, {v_cache.dtype}, {scratch.dtype}")
+    if (k_cache.dim() != 5 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape
+            or not v_cache.is_contiguous()):
+        bad(f"k_cache / v_cache must be contiguous [L, R, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} and "
+            f"{tuple(v_cache.shape)}")
+    L, R, H, t_max, Dh = k_cache.shape
+    if Dh % 8 != 0 or R > 65535 or int(max_new) < 1:
+        bad(f"need Dh a multiple of 8, R <= 65535 and max_new >= 1, got Dh={Dh} R={R} max_new={max_new}")
+    for name, t in (("parent", parent), ("prompt_len", prompt_len), ("lens", lens)):
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != R:
+            bad(f"{name} must be a contiguous int32 tensor of {R} elements, got {t.dtype} {tuple(t.shape)}")
+    need = kv_reorder_scratch_numel(k_cache, max_new)
+    if not scratch.is_contiguous() or scratch.numel() < need:
+        bad(f"scratch must be contiguous with at least {need} elements, got {scratch.numel()}")
+    dev = k_cache.device
+    if dev.type != "cuda" or any(t.device != dev for t in (v_cache, parent, prompt_len, lens, scratch)):
+        bad("all tensors must be on one CUDA device")
+    _ck(_lib().adapcc_kv_reorder(c_void_p(k_cache.data_ptr()), c_void_p(v_cache.data_ptr()), L, R, H, t_max, Dh,
+                                 c_void_p(parent.data_ptr()), c_void_p(prompt_len.data_ptr()),
+                                 c_void_p(lens.data_ptr()), int(max_new), c_void_p(scratch.data_ptr()), _stream()),
+        "kv_reorder")

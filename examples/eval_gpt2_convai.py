@@ -36,6 +36,8 @@ def main():
                    help="f1: generate this many replies at a time with GPT2DoubleHeads.generate (0: one by one). The "
                         "batched path truncates history so the reply fits up front and suppresses special tokens "
                         "before filtering, so its F1 is a different sample")
+    p.add_argument("--num_beams", type=int, default=0,
+                   help="f1: decode the replies with GPT2DoubleHeads.beam_search and this many beams (0: sample)")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -48,7 +50,7 @@ def main():
         kw = dict(max_length=a.max_length, min_length=a.min_length, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p,
                   no_sample=a.no_sample)
     res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
-                           a.batch_size, **kw)
+                           a.batch_size, a.num_beams, **kw)
     print(json.dumps(res))
 
 

@@ -1,0 +1,149 @@
+#!/usr/bin/env python
+"""GPT-2 small beam search: ``GPT2DoubleHeads.beam_search`` against greedy ``generate`` at the same number of rows, and
+the selection and cache-reordering kernels on their own.
+
+Prints one JSON line with the device name and power limit read in the same run. Needs a CUDA device (there is no CPU
+fallback) and writes nothing into the repository.
+
+* ``search``: ms per generated token, prefill and graph capture included (64 new tokens, bf16, seeded random weights,
+  no stop ids, so every call runs all 64 tokens), for B = 1 / 8 items, K = 4 / 8 beams and prompts of 128 / 512 tokens.
+  Next to each, ``generate(temperature=0)`` at B·K rows does the same decode-step and LM-head work, so the difference
+  is what beam search adds (selection, cache reordering, the B·K-row cache copy). Medians of ``--reps`` runs after one
+  warm-up run.
+* ``kernels``: ``beam_step_`` (vocab 50257) and ``kv_reorder_`` (12 layers, 12 heads, Dh 64, every row taking another
+  row's cache) at 64 rows (8 items x 8 beams) with 16 and 64 generated positions, 50 launches captured in a CUDA graph
+  and timed with CUDA events over ``--launches`` launches. GB/s for the reorder counts the generated region read and
+  written twice (into the scratch and back).
+
+Usage: ``python tools/beam_bench.py [--reps 3] [--launches 1000]``
+"""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+import torch  # noqa: E402
+
+NEW_TOKENS = 64
+GRAPH_LAUNCHES = 50
+
+
+def _gpu_info():
+    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i",
+                        str(torch.cuda.current_device())], capture_output=True, text=True)
+    name, power = (r.stdout.strip().split(", ") + ["?", "?"])[:2] if r.returncode == 0 else ("?", "?")
+    return {"device": torch.cuda.get_device_name(), "nvidia_smi_name": name, "power_limit": power}
+
+
+def _median_ms(fn, reps):
+    fn()                                                           # warm-up of this shape
+    times = []
+    for _ in range(reps):
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        fn()
+        torch.cuda.synchronize()
+        times.append((time.perf_counter() - t0) * 1e3)
+    return statistics.median(times)
+
+
+def bench_search(model, reps):
+    rows = []
+    g = torch.Generator(device="cuda").manual_seed(0)
+    for B in (1, 8):
+        for K in (4, 8):
+            for T in (128, 512):
+                prompt = torch.randint(0, model.cfg.vocab_size, (B, T), device="cuda", generator=g)
+                wide = prompt.repeat_interleave(K, dim=0)
+                beam = _median_ms(lambda: model.beam_search(prompt, num_beams=K, max_new_tokens=NEW_TOKENS), reps)
+                greedy = _median_ms(lambda: model.generate(wide, max_new_tokens=NEW_TOKENS, temperature=0.0), reps)
+                rows.append({"batch": B, "beams": K, "prompt": T,
+                             "beam_search_ms_per_token": round(beam / NEW_TOKENS, 3),
+                             "generate_rows_ms_per_token": round(greedy / NEW_TOKENS, 3),
+                             "beam_cost_ms_per_token": round((beam - greedy) / NEW_TOKENS, 3)})
+    return rows
+
+
+def _graph_us(fn, launches):
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        fn()
+    torch.cuda.current_stream().wait_stream(s)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        for _ in range(GRAPH_LAUNCHES):
+            fn()
+    graph.replay()
+    reps = max(1, launches // GRAPH_LAUNCHES)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        graph.replay()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) * 1e3 / (reps * GRAPH_LAUNCHES)
+
+
+def bench_kernels(model, launches):
+    from adapcc_b200.ops import BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
+
+    B, K = 8, 8
+    cfg = model.cfg
+    W = model.wte.weight
+    g = torch.Generator(device="cuda").manual_seed(1)
+    h = torch.randn(B * K, cfg.n_embd, device="cuda", generator=g).to(torch.bfloat16)
+    logits = torch.empty(B * K, W.shape[0], dtype=torch.float32, device="cuda")
+    lm_us = _graph_us(lambda: lm_head_logits_(h, W, logits), launches)
+    logits.copy_(torch.randn(B * K, W.shape[0], device="cuda", generator=g) * 3)
+    # room for every launch: the step never reaches max_new and, without stop ids, no item finishes
+    max_new = launches + 4 * GRAPH_LAUNCHES
+    st = BeamState(B, K, max_new, 1.0, "cuda")
+    st.scores.zero_()
+    step_us = _graph_us(lambda: beam_step_(logits, cfg.vocab_size, st), launches)
+    out = {"rows": B * K, "lm_head_us": round(lm_us, 2), "beam_step_us": round(step_us, 2), "kv_reorder": []}
+    L, H, Dh, T = cfg.n_layer, cfg.n_head, cfg.n_embd // cfg.n_head, 512
+    for gen in (16, 64):
+        cache = model.new_cache(B * K, T + 64)
+        cache.k.normal_(generator=g)
+        cache.v.normal_(generator=g)
+        prompt_len = torch.full((B * K,), T, dtype=torch.int32, device="cuda")
+        lens = prompt_len + gen
+        parent = torch.arange(B * K, dtype=torch.int32, device="cuda").roll(1)
+        scratch = torch.empty(kv_reorder_scratch_numel(cache.k, 64), dtype=torch.bfloat16, device="cuda")
+        us = _graph_us(lambda: kv_reorder_(cache.k, cache.v, parent, prompt_len, lens, 64, scratch), launches)
+        moved = B * K * gen * L * 2 * H * Dh * 2                       # bytes of the generated region, k and v
+        out["kv_reorder"].append({"generated": gen, "us": round(us, 2), "MB_moved": round(moved / 1e6, 1),
+                                  "GBps": round(4 * moved / (us * 1e-6) / 1e9, 1)})
+        del cache, scratch
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
+    ap.add_argument("--reps", type=int, default=3)
+    ap.add_argument("--launches", type=int, default=1000)
+    args = ap.parse_args()
+    if not torch.cuda.is_available():
+        sys.exit("beam_bench: needs a CUDA device")
+    from adapcc_b200.models.gpt2 import GPT2Config, GPT2DoubleHeads
+    from adapcc_b200.runtime.native import load_library
+
+    load_library(build_if_missing=False)
+    torch.cuda.set_device(0)
+    info = _gpu_info()
+    torch.manual_seed(0)
+    model = GPT2DoubleHeads(GPT2Config()).to(device="cuda", dtype=torch.bfloat16).eval()
+    result = dict(info, new_tokens=NEW_TOKENS, kernels=bench_kernels(model, args.launches),
+                  search=bench_search(model, args.reps))
+    print(json.dumps(result))
+
+
+if __name__ == "__main__":
+    main()
