@@ -30,6 +30,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.layers import FusedLayerNorm, FusedLinear
+from ..ops.repeats import check_repeat_args, penalize_repeats_reference
 from ..ops.sampling import sample_reference, top_filtering
 
 
@@ -429,7 +430,8 @@ class GPT2DoubleHeads(nn.Module):
     def generate(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
                  token_type_ids: Optional[torch.Tensor] = None, reply_type=None, max_new_tokens: int = 20,
                  temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9, stop_ids: Sequence[int] = (),
-                 suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, seed=0) -> Tuple[torch.Tensor, torch.Tensor]:
+                 suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, seed=0, repetition_penalty: float = 1.0,
+                 no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -438,15 +440,18 @@ class GPT2DoubleHeads(nn.Module):
         While fewer than ``min_new_tokens`` tokens are generated, ``suppress_ids`` cannot be drawn; a token in
         ``stop_ids`` ends its row. ``temperature == 0`` is greedy. The draw of each token is defined in
         ``ops/sampling.py``: a row's tokens depend on its prompt, its seed and the scalars, not on the other rows.
+        ``repetition_penalty`` (1: off) and ``no_repeat_ngram_size`` (0: off) act on each row's logits first, over its
+        prompt and the tokens generated so far (``ops/repeats.py``).
 
         Returns ``(tokens, n_new)``: int64 [B, max_new_tokens] (-1 after a row stopped) and the tokens per row.
 
         The prompts are prefilled into a KV cache of ``max(lengths) + max_new_tokens`` positions (``ValueError`` if that
         exceeds ``n_positions``: there is no sliding window here, ``sample_sequence`` has one). On CUDA with bf16
         weights the LM head and the sampler are native kernels (``ops.lm_head_logits_``, ``ops.sample_tokens_``) and
-        every token after the first replays one CUDA graph of decode step, LM head and sampler, which feeds the drawn ids
-        back into its own input; the host reads the done flags once every 8 tokens, a step late, to stop early.
-        Elsewhere the same loop runs eagerly with fp32 PyTorch logits and ``ops.sampling.sample_reference``."""
+        every token after the first replays one CUDA graph of decode step, LM head (``ops.penalize_repeats_`` when a
+        repetition control is on) and sampler, which feeds the drawn ids back into its own input; the host reads the
+        done flags once every 8 tokens, a step late, to stop early. Elsewhere the same loop runs eagerly with fp32
+        PyTorch logits, ``ops.repeats.penalize_repeats_reference`` and ``ops.sampling.sample_reference``."""
         cfg = self.cfg
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
             raise ValueError(f"generate: input_ids must be [B, T], got {tuple(input_ids.shape)}")
@@ -460,6 +465,8 @@ class GPT2DoubleHeads(nn.Module):
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1 or int(min_new_tokens) < 0:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0, 0 < top_p <= 1 and min_new_tokens >= 0, "
                              f"got {temperature}, {top_k}, {top_p}, {min_new_tokens}")
+        check_repeat_args("generate", repetition_penalty, no_repeat_ngram_size)
+        repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
         t_max = max(lengths) + int(max_new_tokens)
         if t_max > cfg.n_positions:
             raise ValueError(f"generate: the longest prompt ({max(lengths)}) plus max_new_tokens ({max_new_tokens}) "
@@ -481,20 +488,29 @@ class GPT2DoubleHeads(nn.Module):
         h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
         n = int(max_new_tokens)
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
+        if repeats:                                 # the rows' sequences: prompt, then each consumed token
+            seq = torch.zeros(B, t_max, dtype=torch.int32, device=dev)
+            seq[:, :T] = input_ids
         if cache.work is None:                      # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = self.wte.weight.float()
             done = torch.zeros(B, dtype=torch.int32)
             for i in range(n):
                 if i:
                     h = self.decode_step(nxt.to(dev), tt_new, cache)
-                nxt, tok, done = sample_reference(self.lm_logits(h, head), cfg.vocab_size, temperature, top_k, top_p,
+                logits = self.lm_logits(h, head)
+                if repeats:
+                    if i:
+                        seq[torch.arange(B, device=dev), cache.lens.long() - 1] = nxt.to(dev, torch.int32)
+                    logits = penalize_repeats_reference(logits, [seq[b, :x] for b, x in enumerate(cache.host_lens)],
+                                                        cfg.vocab_size, repetition_penalty, no_repeat_ngram_size)
+                nxt, tok, done = sample_reference(logits, cfg.vocab_size, temperature, top_k, top_p,
                                                   seeds, cache.lens, i, min_new_tokens, suppress_ids, stop_ids, done)
                 tokens[:, i] = tok.to(dev)
                 if bool(done.all()):
                     break
             return tokens, (tokens >= 0).sum(1)
 
-        from ..ops import LM_HEAD_MAX_ROWS, lm_head_logits_, sample_tokens_
+        from ..ops import LM_HEAD_MAX_ROWS, lm_head_logits_, penalize_repeats_, sample_tokens_
 
         if B > LM_HEAD_MAX_ROWS:
             raise ValueError(f"generate: at most {LM_HEAD_MAX_ROWS} rows per call on the native path, got {B}")
@@ -505,9 +521,13 @@ class GPT2DoubleHeads(nn.Module):
         step = torch.zeros(1, dtype=torch.int32, device=dev)
         sup = torch.tensor(list(suppress_ids), dtype=torch.int32, device=dev)
         stop = torch.tensor(list(stop_ids), dtype=torch.int32, device=dev)
+        prompt_len = cache.lens.clone() if repeats else None
 
         def head_and_sample(hidden):
             lm_head_logits_(hidden, weight, logits)
+            if repeats:
+                penalize_repeats_(logits, cfg.vocab_size, seq, prompt_len, cache.lens, step, next_ids, None, 1,
+                                  repetition_penalty, no_repeat_ngram_size)
             sample_tokens_(logits, cfg.vocab_size, temperature, top_k, top_p, seeds, cache.lens, step,
                            min_new_tokens, sup, stop, done, next_ids, tokens)
 
@@ -534,8 +554,8 @@ class GPT2DoubleHeads(nn.Module):
     def beam_search(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
                     token_type_ids: Optional[torch.Tensor] = None, reply_type=None, num_beams: int = 4,
                     max_new_tokens: int = 20, length_penalty: float = 1.0, stop_ids: Sequence[int] = (),
-                    suppress_ids: Sequence[int] = (), min_new_tokens: int = 0
-                    ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
+                    no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -544,6 +564,9 @@ class GPT2DoubleHeads(nn.Module):
         chosen. A hypothesis of L tokens (its stop token included) scores ``sum of log-probabilities / L **
         length_penalty``. An item stops as soon as no live beam can beat its K-th finished hypothesis, which never
         changes its result. An item's result depends on its prompt and the scalars only, not on the other items.
+        ``repetition_penalty`` (1: off) and ``no_repeat_ngram_size`` (0: off) act on each beam's logits before the
+        log-softmax, over its prompt and its own hypothesis (``ops/repeats.py``), so its log-probabilities are
+        renormalised over the ids that remain.
 
         Returns ``(tokens, n_new, scores)``: the best hypothesis of each item as int64 [B, max_new_tokens] (the stop
         token excluded, padded with -1), its length int64 [B] and its normalised score fp32 [B].
@@ -551,9 +574,10 @@ class GPT2DoubleHeads(nn.Module):
         Each prompt is prefilled once and its keys and values copied to its ``num_beams`` rows of a cache of
         ``max(lengths) + max_new_tokens`` positions (more than ``n_positions`` is a ``ValueError``). On CUDA with bf16
         weights every token after the first replays one CUDA graph of decode step, LM head (``ops.lm_head_logits_``),
-        selection (``ops.beam_step_``) and cache reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the
-        host reads the done flags once every 8 tokens, a period late. Elsewhere the same loop runs eagerly with fp32
-        PyTorch logits, ``ops.beam.BeamReference`` and torch indexing."""
+        the repetition controls when on (``ops.penalize_repeats_``), selection (``ops.beam_step_``) and cache
+        reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the host reads the done flags once every 8
+        tokens, a period late. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
+        ``ops.repeats.penalize_repeats_reference``, ``ops.beam.BeamReference`` and torch indexing."""
         from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, LM_HEAD_MAX_ROWS
         from ..ops.beam import BeamReference, best_hypotheses
 
@@ -574,6 +598,8 @@ class GPT2DoubleHeads(nn.Module):
         if len(stop_ids) > BEAM_MAX_STOP or len(suppress_ids) > BEAM_MAX_SUPPRESS:
             raise ValueError(f"beam_search: at most {BEAM_MAX_STOP} stop ids and {BEAM_MAX_SUPPRESS} suppressed ids, "
                              f"got {len(stop_ids)} and {len(suppress_ids)}")
+        check_repeat_args("beam_search", repetition_penalty, no_repeat_ngram_size)
+        repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
         t_max = max(lengths) + n
         if t_max > cfg.n_positions:
             raise ValueError(f"beam_search: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds "
@@ -601,21 +627,33 @@ class GPT2DoubleHeads(nn.Module):
         del pre
         h = h.repeat_interleave(K, dim=0).contiguous()
         V = cfg.vocab_size
+        if repeats:                                 # each beam's sequence: the prompt, then its hypothesis
+            seq = torch.zeros(B * K, t_max, dtype=torch.int32, device=dev)
+            seq[:, :T] = input_ids.repeat_interleave(K, dim=0)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             ref = BeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens)
             head = weight.float()
             for i in range(n):
                 if i:
                     h = self.decode_step(nxt.to(dev), tt_new, cache)
-                nxt, parent = ref.step(self.lm_logits(h, head))
+                logits = self.lm_logits(h, head)
+                if repeats:
+                    if i:
+                        seq[torch.arange(B * K, device=dev), cache.lens.long() - 1] = nxt.to(dev, torch.int32)
+                    logits = penalize_repeats_reference(logits, [seq[r, :x] for r, x in enumerate(cache.host_lens)],
+                                                        V, repetition_penalty, no_repeat_ngram_size)
+                nxt, parent = ref.step(logits)
                 rows = parent.to(dev)
                 cache.k.copy_(cache.k[:, rows])
                 cache.v.copy_(cache.v[:, rows])
+                if repeats:
+                    seq = seq[rows]
                 if ref.done.all():
                     break
             return tuple(t.to(dev) for t in ref.result())
 
-        from ..ops import BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
+        from ..ops import (BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_,
+                           penalize_repeats_)
 
         st = BeamState(B, K, n, length_penalty, dev)
         logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
@@ -626,6 +664,9 @@ class GPT2DoubleHeads(nn.Module):
 
         def select(hidden):
             lm_head_logits_(hidden, weight, logits)
+            if repeats:
+                penalize_repeats_(logits, V, seq, prompt_len, cache.lens, st.step, st.next_ids, st.parent, K,
+                                  repetition_penalty, no_repeat_ngram_size)
             beam_step_(logits, V, st, min_new_tokens, sup, stop)
             kv_reorder_(cache.k, cache.v, st.parent, prompt_len, cache.lens, n, scratch)
 

@@ -5,6 +5,7 @@ and fails loudly if the native library is missing — there is no silent PyTorch
 from __future__ import annotations
 
 import ctypes
+import math
 from ctypes import c_float, c_int, c_longlong, c_void_p
 from typing import Optional
 
@@ -50,6 +51,8 @@ def _lib():
                                          + [c_void_p] * 10 + [c_void_p])
         lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p,
                                                                                                 c_void_p]
+        lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
+                                                + [c_int, c_float, c_int, c_void_p])
         _bound = True
     return lib
 
@@ -496,3 +499,54 @@ def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tens
                                  c_void_p(parent.data_ptr()), c_void_p(prompt_len.data_ptr()),
                                  c_void_p(lens.data_ptr()), int(max_new), c_void_p(scratch.data_ptr()), _stream()),
         "kv_reorder")
+
+
+# ---- repetition penalty and no-repeat n-gram blocking (csrc/ops_repeats.cu) ----------------------------------------
+REPEATS_MAX_GROUP = 16         # rows per parent group (beams per item)
+REPEATS_MAX_LEN = 1024         # sequence positions per row (GPT-2's n_positions)
+
+
+def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, prompt_len: torch.Tensor,
+                      lens: torch.Tensor, step: torch.Tensor, ids: torch.Tensor, parent: Optional[torch.Tensor],
+                      group: int, penalty: float, ngram: int) -> None:
+    """The repetition penalty and no-repeat n-gram blocking of every row, in place, on the device (the definition in
+    ``ops/repeats.py``, which this kernel equals bit for bit). ``logits`` fp32 [R, ld] (the first ``vocab`` columns
+    used); ``seq`` int32 [R, t_max] the rows' sequences, kept up to date here; ``prompt_len`` and ``lens`` int32 [R];
+    ``step`` int32 [1] (the counter of ``generate`` / ``BeamState``); ``ids`` int64 [R] the tokens the decode step just
+    consumed; ``parent`` int32 [R] or None, each row's parent inside its group of ``group`` consecutive rows.
+
+    With ``*step > 0`` the sequences first advance: a row with a parent takes the parent's generated region
+    ``seq[parent[r], prompt_len[r]:lens[r] - 1]`` (cycles and many-to-one maps come out right), then
+    ``seq[r, lens[r] - 1] = ids[r]``. With ``*step == 0`` the sequence is the prompt as stored. Row r's sequence is then
+    ``seq[r, :lens[r]]``; ``penalty`` (1: off) and ``ngram`` (0: off) are applied to it. The grid depends on R and
+    ``group`` only and there is no host sync, so one capture serves every token."""
+    def bad(msg):
+        raise ValueError(f"penalize_repeats_: {msg}")
+
+    if not (math.isfinite(penalty) and penalty > 0) or int(ngram) < 0:
+        bad(f"need a finite penalty > 0 and ngram >= 0, got {penalty}, {ngram}")
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
+        bad(f"logits must be fp32 [R, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
+    R = logits.shape[0]
+    if not 1 <= vocab <= logits.shape[1]:
+        bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
+    if not 1 <= int(group) <= REPEATS_MAX_GROUP or R % int(group) != 0:
+        bad(f"group must be in [1, {REPEATS_MAX_GROUP}] and divide R = {R}, got {group}")
+    if (seq.dtype != torch.int32 or seq.dim() != 2 or seq.shape[0] != R or not seq.is_contiguous()
+            or not 1 <= seq.shape[1] <= REPEATS_MAX_LEN):
+        bad(f"seq must be a contiguous int32 [{R}, t_max] tensor with t_max <= {REPEATS_MAX_LEN}, got {seq.dtype} "
+            f"{tuple(seq.shape)}")
+    for name, t, dt, n in (("prompt_len", prompt_len, torch.int32, R), ("lens", lens, torch.int32, R),
+                           ("step", step, torch.int32, 1), ("ids", ids, torch.int64, R),
+                           ("parent", parent, torch.int32, R)):
+        if t is not None and (t.dtype != dt or not t.is_contiguous() or t.numel() != n):
+            bad(f"{name} must be a contiguous {dt} tensor of {n} elements, got {t.dtype} {tuple(t.shape)}")
+    dev = logits.device
+    others = [t for t in (seq, prompt_len, lens, step, ids, parent) if t is not None]
+    if dev.type != "cuda" or any(t.device != dev for t in others):
+        bad(f"all tensors must be on one CUDA device, got logits on {dev} and "
+            f"{sorted(set(str(t.device) for t in others))}")
+    p = lambda t: c_void_p(t.data_ptr() if t is not None else None)                  # noqa: E731
+    _ck(_lib().adapcc_penalize_repeats(p(logits), logits.stride(0), int(vocab), R, p(seq), seq.shape[1],
+                                       p(prompt_len), p(lens), p(step), p(ids), p(parent), int(group),
+                                       float(penalty), int(ngram), _stream()), "penalize_repeats")

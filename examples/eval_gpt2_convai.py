@@ -38,6 +38,10 @@ def main():
                         "before filtering, so its F1 is a different sample")
     p.add_argument("--num_beams", type=int, default=0,
                    help="f1: decode the replies with GPT2DoubleHeads.beam_search and this many beams (0: sample)")
+    p.add_argument("--repetition_penalty", type=float, default=1.0,
+                   help="f1: penalty on ids already in the prompt or reply (1: off); replies go through the batched path")
+    p.add_argument("--no_repeat_ngram_size", type=int, default=0,
+                   help="f1: never repeat an n-gram of the prompt or reply (0: off); replies go through the batched path")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -48,7 +52,8 @@ def main():
     kw = {}
     if a.eval_type == "f1":
         kw = dict(max_length=a.max_length, min_length=a.min_length, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p,
-                  no_sample=a.no_sample)
+                  no_sample=a.no_sample, repetition_penalty=a.repetition_penalty,
+                  no_repeat_ngram_size=a.no_repeat_ngram_size)
     res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
                            a.batch_size, a.num_beams, **kw)
     print(json.dumps(res))
