@@ -4,9 +4,8 @@
 //   beam_rows   : one 512-thread CTA per beam row. Three passes over the row in global memory (no shared-memory copy,
 //                 so any vocabulary size works): the maximum m, Z = sum_i expf(l_i - m), then every candidate's score
 //                 c_i = s + ((l_i - m) - logf(Z)) as a 64-bit key (order-preserving float bits, then the inverted id, so
-//                 a tie goes to the lower id). Each thread keeps its four best keys in registers; each warp takes its
-//                 N = K + n_stop best by N rounds of a warp maximum (a lane that runs out of kept keys rescans its ids
-//                 below the last winner), and warp 0 merges the 16 warp lists into the row's N best.
+//                 a tie goes to the lower id), of which the row's N = K + n_stop best are kept (topk_rows.cuh, shared
+//                 with contrastive search).
 //   beam_select : one warp per item. The K rows' N best, re-keyed by the flat index j * V + i, are walked in rank order
 //                 (rounds of a warp maximum): the first K non-stop candidates become the new beams, stop candidates
 //                 ranked before the K-th are offered to the finished set, and the done rule is applied (DESIGN.md §4a).
@@ -22,17 +21,15 @@
 #include <cstdint>
 
 #include "common.h"
+#include "topk_rows.cuh"
 
 namespace adapcc {
 
-constexpr int kBeamThreads = 512;
-constexpr int kBeamWarps = kBeamThreads / 32;
 constexpr int kBeamMaxK = 16;
 constexpr int kBeamMaxStop = 8;
 constexpr int kBeamMaxN = kBeamMaxK + kBeamMaxStop;   // candidates kept per row
 constexpr int kBeamMaxSuppress = 1024;
 constexpr int kReorderThreads = 256;
-constexpr uint32_t kBeamNegInfKey = 0x007FFFFFu;      // key(-inf): candidates at -inf are never taken
 
 struct BeamArgs {
   const float* logits;         // [B * K, ld], the first `vocab` columns used
@@ -59,82 +56,11 @@ struct BeamArgs {
   int* fin_count;              // [B]
 };
 
-__device__ __forceinline__ uint32_t beam_f2key(float f) {
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-__device__ __forceinline__ float beam_key2f(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
-__device__ __forceinline__ unsigned long long warp_max_u64(unsigned long long v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// every thread gets the same bits: a shuffle tree per warp, then the warp partials by the same tree in warp order
-__device__ __forceinline__ float beam_block_sum(float* red, float v) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  v = lane < kBeamWarps ? red[lane] : 0.f;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
-__device__ __forceinline__ float beam_block_max(float* red, float v) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  v = lane < kBeamWarps ? red[lane] : -INFINITY;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-struct RowView {
-  const float* l;
-  const uint32_t* bits;        // removed ids (null: none)
-  int V;
-  float s, m, lz;
-  __device__ __forceinline__ bool removed(int i) const { return bits && ((bits[i >> 5] >> (i & 31)) & 1u); }
-};
-
-// this thread's four best candidate keys strictly below `bound`, best first (0: none)
-__device__ __forceinline__ void scan_top4(const RowView& rv, unsigned long long bound, unsigned long long (&t)[4]) {
-  t[0] = t[1] = t[2] = t[3] = 0ull;
-  for (int i = threadIdx.x; i < rv.V; i += kBeamThreads) {
-    if (rv.removed(i)) continue;
-    const float c = rv.s + ((__ldg(rv.l + i) - rv.m) - rv.lz);
-    const uint32_t k32 = beam_f2key(c);
-    if (k32 <= kBeamNegInfKey) continue;
-    const unsigned long long key = ((unsigned long long)k32 << 32) | (0xFFFFFFFFu - (uint32_t)i);
-    if (key >= bound || key <= t[3]) continue;
-    t[3] = key;
-#pragma unroll
-    for (int q = 3; q > 0; --q)
-      if (t[q] > t[q - 1]) {
-        const unsigned long long x = t[q];
-        t[q] = t[q - 1];
-        t[q - 1] = x;
-      }
-  }
-}
-
 __global__ void __launch_bounds__(kBeamThreads, 1) beam_rows_kernel(const __grid_constant__ BeamArgs a) {
   extern __shared__ uint32_t s_bits[];                // removed ids, one bit each (only while step < min_new)
   __shared__ float s_red[kBeamWarps];
   __shared__ unsigned long long s_top[kBeamWarps * kBeamMaxN];
-  const int row = blockIdx.x, b = row / a.K, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, N = a.N;
+  const int row = blockIdx.x, b = row / a.K, tid = threadIdx.x, N = a.N;
   unsigned long long* out = a.cand + (long long)row * N;
   const float s = a.scores[row];
   if (a.done[b] || !(s > -INFINITY)) {                // a finished item or a dead beam offers nothing
@@ -168,38 +94,7 @@ __global__ void __launch_bounds__(kBeamThreads, 1) beam_rows_kernel(const __grid
   z = beam_block_sum(s_red, z);
   rv.m = m;
   rv.lz = logf(z);
-  unsigned long long t[4];
-  scan_top4(rv, ~0ull, t);
-  bool more = t[3] != 0ull;                           // four kept: the thread may hold further candidates
-  for (int r = 0; r < N; ++r) {
-    const unsigned long long w = warp_max_u64(t[0]);
-    if (w == 0ull) break;
-    if (lane == 0) s_top[warp * N + r] = w;
-    if (t[0] == w) {
-      t[0] = t[1];
-      t[1] = t[2];
-      t[2] = t[3];
-      t[3] = 0ull;
-      if (t[0] == 0ull && more) {
-        scan_top4(rv, w, t);
-        more = t[3] != 0ull;
-      }
-    }
-  }
-  __syncthreads();
-  if (warp == 0) {
-    unsigned long long bound = ~0ull;
-    for (int r = 0; r < N; ++r) {
-      unsigned long long best = 0ull;
-      for (int e = lane; e < kBeamWarps * N; e += 32) {
-        const unsigned long long v = s_top[e];
-        if (v < bound && v > best) best = v;
-      }
-      best = warp_max_u64(best);
-      if (lane == 0) out[r] = best;
-      bound = best;
-    }
-  }
+  row_top_keys<false>(rv, N, s_top, out);
 }
 
 struct FinishedSet {

@@ -166,6 +166,32 @@ def decode_attention(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Te
     return torch.einsum("bht,bhtd->bhd", p, v_cache.float()).to(qkv.dtype).reshape(B, H * Dh)
 
 
+class CandidateKV:
+    """What a candidate step of contrastive search attends over: ``top_k`` candidate tokens per row of ``cache``, the
+    candidates of row b in rows ``b·k .. b·k + k - 1``. Candidate (b, j) attends over the row's cached positions and its
+    own new key and value at ``cache.lens[b]``; the cache is only read, and every layer's new keys and values go to
+    ``side`` [n_layer, 2, B·k, D] (model dtype) for the winner's commit. With ``work`` (bf16 CUDA caches) this is the
+    native kernel (``ops.cand_attention_``); otherwise ``decode_attention`` in PyTorch on a k-fold copy of the rows."""
+
+    def __init__(self, cache: "KVCache", top_k: int, side: torch.Tensor, work: Optional[torch.Tensor] = None):
+        self.cache, self.top_k, self.side, self.work = cache, int(top_k), side, work
+
+    def attend(self, qkv: torch.Tensor, layer: int) -> torch.Tensor:
+        """Layer ``layer``'s attention of the candidates ``qkv`` [B·k, 3·H·Dh] -> [B·k, H·Dh]."""
+        c, K = self.cache, self.top_k
+        B, H, t_max, Dh = c.k[layer].shape
+        if self.work is not None:
+            from ..ops import cand_attention_
+            out = torch.empty(B * K, H * Dh, dtype=qkv.dtype, device=qkv.device)
+            return cand_attention_(qkv, c.k[layer], c.v[layer], c.lens, K, out, self.side[layer, 0],
+                                   self.side[layer, 1], self.work)
+        q, k, v = qkv.reshape(B * K, 3, H * Dh).unbind(1)
+        self.side[layer, 0].copy_(k)
+        self.side[layer, 1].copy_(v)
+        return decode_attention(qkv, c.k[layer].repeat_interleave(K, 0), c.v[layer].repeat_interleave(K, 0),
+                                c.lens.repeat_interleave(K))
+
+
 class Block(nn.Module):
     """Pre-LN transformer block; the MLP runs as two GEMMs with the activation passes in GEMM epilogues when
     supported (ops/gemm.py), residual adds optionally fused into the following LayerNorm (``forward_deferred``)."""
@@ -197,6 +223,8 @@ class Block(nn.Module):
         return self.c_proj2(F.gelu(self.c_fc(h), approximate="tanh"))
 
     def _attn(self, h: torch.Tensor, cache: Optional["KVCache"] = None, layer: int = 0) -> torch.Tensor:
+        if isinstance(cache, CandidateKV):           # contrastive search: k candidate tokens per cache row
+            return self.c_proj(cache.attend(self.c_attn(h), layer))
         if cache is not None and h.dim() == 2:       # decode: one new token per row [B, D] against the cache
             return self.c_proj(decode_attention(self.c_attn(h), cache.k[layer], cache.v[layer], cache.lens, cache.work))
         B, T, D = h.shape
@@ -693,6 +721,161 @@ class GPT2DoubleHeads(nn.Module):
         hist_back = st.hist_back.view(n, B, K).cpu().numpy()
         return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n))
 
+    def _candidate_hidden(self, ids: torch.Tensor, tt: Optional[torch.Tensor], cand: "CandidateKV") -> torch.Tensor:
+        """The final hidden states [B·k, D] of ``cand.top_k`` candidate tokens ``ids`` [B·k] per cache row, each at its
+        row's position ``lens[b]``: the blocks of ``decode_step`` with attention through ``cand``. The cache is read
+        only; its lengths do not move."""
+        pos = cand.cache.lens.long().repeat_interleave(cand.top_k)
+        return self._blocks(self._embed(ids, tt, pos), cand)
+
+    @torch.no_grad()
+    def contrastive_search(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
+                           token_type_ids: Optional[torch.Tensor] = None, reply_type=None, top_k: int = 4,
+                           penalty_alpha: float = 0.6, max_new_tokens: int = 20, stop_ids: Sequence[int] = (),
+                           suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
+                           no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Batched contrastive search (Su et al., 2022; HuggingFace's ``penalty_alpha`` + ``top_k``); the definition is
+        in ``ops/contrastive.py``.
+
+        Each step takes the ``top_k`` most likely next tokens of a row, runs one decode step for each of them, and emits
+        the candidate with the best ``(1 - penalty_alpha) p - penalty_alpha s``, where ``s`` is the largest cosine
+        between the candidate's final hidden state and the hidden states of the row's sequence so far (its prompt
+        without padding, then its emitted tokens). ``penalty_alpha = 0`` or ``top_k = 1`` is greedy decoding.
+        ``input_ids``, ``lengths``, ``reply_type``, token types, ``stop_ids``, ``suppress_ids``, ``min_new_tokens``,
+        the repetition controls and the return value ``(tokens, n_new)`` work as in ``generate``.
+
+        The prompts are prefilled into a KV cache of ``max(lengths) + max_new_tokens`` positions (more than
+        ``n_positions`` is a ``ValueError``) and the context is taken from the prefill's hidden states. On CUDA with
+        bf16 weights (at most 64 rows) every token replays one CUDA graph: the candidate step (``ops.cand_attention_``
+        attends for all k candidates over the shared cache), re-rank and commit (``ops.contrastive_rerank_``), the LM
+        head on the winners, ``ops.penalize_repeats_`` when on, and the next candidates (``ops.contrastive_select_``);
+        the host reads the done flags once every 8 tokens, a period late. Elsewhere the same loop runs eagerly:
+        candidates decode through ``decode_attention`` on a k-fold copy of the rows and the selection runs in fp64
+        (``ops/contrastive.py``)."""
+        from ..ops import CONTRASTIVE_MAX_K, LM_HEAD_MAX_ROWS
+        from ..ops.contrastive import check_contrastive_args, rerank_row, select_candidates
+
+        cfg = self.cfg
+        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
+            raise ValueError(f"contrastive_search: input_ids must be [B, T], got {tuple(input_ids.shape)}")
+        B, T = input_ids.shape
+        dev = input_ids.device
+        lengths = [T] * B if lengths is None else [int(x) for x in lengths]
+        if len(lengths) != B or any(not 1 <= x <= T for x in lengths):
+            raise ValueError(f"contrastive_search: need {B} lengths in [1, {T}], got {lengths}")
+        check_contrastive_args("contrastive_search", top_k, penalty_alpha, CONTRASTIVE_MAX_K)
+        K, n, alpha = int(top_k), int(max_new_tokens), float(penalty_alpha)
+        if n < 1 or int(min_new_tokens) < 0:
+            raise ValueError(f"contrastive_search: need max_new_tokens >= 1 and min_new_tokens >= 0, got "
+                             f"{max_new_tokens}, {min_new_tokens}")
+        check_repeat_args("contrastive_search", repetition_penalty, no_repeat_ngram_size)
+        repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
+        t_max = max(lengths) + n
+        if t_max > cfg.n_positions:
+            raise ValueError(f"contrastive_search: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) "
+                             f"exceeds n_positions = {cfg.n_positions}")
+        weight = self.wte.weight
+        native = weight.is_cuda and weight.dtype == torch.bfloat16
+        if native and B > LM_HEAD_MAX_ROWS:
+            raise ValueError(f"contrastive_search: at most {LM_HEAD_MAX_ROWS} rows per call on the native path, got {B}")
+        last = torch.tensor(lengths, device=dev) - 1
+        tt_new = None
+        if reply_type is not None:
+            tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
+        elif token_type_ids is not None:
+            tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
+        tt_cand = tt_new.repeat_interleave(K) if tt_new is not None else None
+        cache = self.new_cache(B, t_max)
+        hs = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)
+        h = hs[torch.arange(B, device=dev), last].contiguous()
+        V, L, H = cfg.vocab_size, cfg.n_layer, cfg.n_head
+        D = cfg.n_embd
+        if repeats:                                 # the rows' sequences: prompt, then each emitted token
+            seq = torch.zeros(B, t_max, dtype=torch.int32, device=dev)
+            seq[:, :T] = input_ids
+        if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
+            head = weight.float()
+            cand = CandidateKV(cache, K, torch.zeros(L, 2, B * K, D, dtype=weight.dtype, device=dev))
+            ctx = [hs[b, :x] for b, x in enumerate(lengths)]
+            stop = set(int(s) for s in stop_ids)
+            done = torch.zeros(B, dtype=torch.bool)
+            tokens = torch.full((B, n), -1, dtype=torch.int64)
+            rows = torch.arange(B, device=dev)
+            win = None
+            for i in range(n):
+                logits = self.lm_logits(h, head)
+                if repeats:
+                    if i:
+                        seq[rows, cache.lens.long() - 1] = win.to(dev, torch.int32)
+                    logits = penalize_repeats_reference(logits, [seq[b, :x] for b, x in enumerate(cache.host_lens)],
+                                                        V, repetition_penalty, no_repeat_ngram_size)
+                ids, probs = select_candidates(logits, V, K, i, min_new_tokens, suppress_ids, done)
+                cache.check_room()
+                hc = self._candidate_hidden(ids.clamp(min=0).reshape(-1).to(dev), tt_cand, cand)
+                hk = hc.view(B, K, D)
+                pick, win = [], torch.zeros(B, dtype=torch.int64)
+                for b in range(B):
+                    r = rerank_row(ids[b].numpy(), probs[b].numpy(), hk[b].double().cpu().numpy(),
+                                   ctx[b].double().cpu().numpy(), alpha)
+                    pick.append(b * K + r["rank"])
+                    win[b] = r["token"]
+                    if not done[b]:
+                        if r["token"] in stop:
+                            done[b] = True
+                        else:
+                            tokens[b, i] = r["token"]
+                pick = torch.tensor(pick, device=dev)
+                pos = cache.lens.long()
+                cache.k[:, rows, :, pos] = cand.side[:, 0, pick].view(L, B, H, D // H).transpose(0, 1)
+                cache.v[:, rows, :, pos] = cand.side[:, 1, pick].view(L, B, H, D // H).transpose(0, 1)
+                cache.advance()
+                h = hc[pick]
+                ctx = [torch.cat([ctx[b], h[b:b + 1]]) for b in range(B)]
+                if bool(done.all()):
+                    break
+            return tokens.to(dev), (tokens >= 0).sum(1).to(dev)
+
+        from ..ops import (ContrastiveState, contrastive_context_init_, contrastive_rerank_, contrastive_select_,
+                           lm_head_logits_, penalize_repeats_)
+
+        st = ContrastiveState(B, K, n, t_max, L, H, D // H, dev)
+        contrastive_context_init_(hs.contiguous(), cache.lens, st)
+        del hs
+        cand = CandidateKV(cache, K, st.side, st.work)
+        logits = torch.empty(B, weight.shape[0], dtype=torch.float32, device=dev)
+        sup = torch.tensor(list(suppress_ids), dtype=torch.int32, device=dev)
+        stop = torch.tensor(list(stop_ids), dtype=torch.int32, device=dev)
+        prompt_len = cache.lens.clone() if repeats else None
+
+        def select(hidden):
+            lm_head_logits_(hidden, weight, logits)
+            if repeats:
+                penalize_repeats_(logits, V, seq, prompt_len, cache.lens, st.step, st.win_ids, None, 1,
+                                  repetition_penalty, no_repeat_ngram_size)
+            contrastive_select_(logits, V, st, min_new_tokens, sup)
+
+        def commit_and_select(hc):
+            contrastive_rerank_(hc, st, alpha, cache.k, cache.v, cache.lens, stop)
+            select(st.win_h)
+
+        select(h)                                   # the first candidates, from the prefill's last positions
+        # contrastive_select_ writes the candidates into the graph's own input buffer; the commit advances the cache
+        graph = DecodeGraph(self, cache, tt_cand is not None, head=commit_and_select, ids=st.next_ids, tt=tt_cand,
+                            step=lambda ids, tt, c: self._candidate_hidden(ids, tt, cand))
+        flags = torch.empty(B, dtype=torch.int32, pin_memory=True)
+        copied = None
+        for i in range(1, n + 1):
+            graph.replay()
+            if i % 8 == 0 and i < n:                # the flags copied 8 tokens ago are ready by now: no stall
+                if copied is not None:
+                    copied.synchronize()
+                    if bool(flags.all()):
+                        break
+                flags.copy_(st.done, non_blocking=True)
+                copied = torch.cuda.Event()
+                copied.record()
+        return st.tokens, (st.tokens >= 0).sum(1)
+
     def forward(self, input_ids, token_type_ids=None, mc_token_ids=None, lm_labels=None, mc_labels=None,
                 lm_coef: float = 1.0, mc_coef: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """-> (loss, lm_loss, mc_loss). Shapes as in the reference: [B, C, T] ids/labels, [B, C]
@@ -744,25 +927,29 @@ class DecodeGraph:
 
     ``head`` runs on the step's hidden state inside the graph (the warm-up step leaves it out, so it may change state).
     ``ids`` / ``tt``: input buffers to read instead of the graph's own (``tt`` replaces the one ``token_types`` asks
-    for), for a caller that fills them on the device and steps with ``replay``. ``generate`` uses all three."""
+    for), for a caller that fills them on the device and steps with ``replay``. ``generate`` uses all three. ``step``
+    replaces ``model.decode_step`` as the captured step, called as ``step(ids, tt, cache)``; it and ``head`` together
+    must leave the cache one token longer per replay (``contrastive_search``: a candidate step, then a commit)."""
 
     def __init__(self, model: "GPT2DoubleHeads", cache: KVCache, token_types: bool = True,
-                 head: Optional[Callable] = None, ids: Optional[torch.Tensor] = None, tt: Optional[torch.Tensor] = None):
+                 head: Optional[Callable] = None, ids: Optional[torch.Tensor] = None, tt: Optional[torch.Tensor] = None,
+                 step: Optional[Callable] = None):
         dev = cache.lens.device
         self.cache = cache
+        step = model.decode_step if step is None else step
         self.ids = torch.zeros(cache.batch, dtype=torch.long, device=dev) if ids is None else ids
         self.tt = tt if tt is not None or not token_types else torch.zeros_like(self.ids)
         lens0, host0 = cache.lens.clone(), list(cache.host_lens)
         s = torch.cuda.Stream(device=dev)
         s.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(s):                     # warm-up: allocator and cuBLAS settle; writes only slot lens[b],
-            model.decode_step(self.ids, self.tt, cache)   # which the next real step overwrites
+            step(self.ids, self.tt, cache)             # which the next real step overwrites
         torch.cuda.current_stream(dev).wait_stream(s)
         cache.lens.copy_(lens0)
         cache.host_lens = host0
         self.graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self.graph):
-            self.h = model.decode_step(self.ids, self.tt, cache)
+            self.h = step(self.ids, self.tt, cache)
             if head is not None:
                 head(self.h)
         cache.host_lens = host0                        # capturing ran the host side of a step, not the step

@@ -53,6 +53,16 @@ def _lib():
                                                                                                 c_void_p]
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
                                                 + [c_int, c_float, c_int, c_void_p])
+        lib.adapcc_cs_sim_numel.argtypes = [c_int] * 3
+        lib.adapcc_cs_sim_numel.restype = c_longlong
+        lib.adapcc_cand_attn.argtypes = [c_void_p] * 7 + [c_int] * 6 + [c_void_p, c_void_p]
+        lib.adapcc_cs_select.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int]
+                                         + [c_void_p] * 5)
+        lib.adapcc_cs_rerank.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_float, c_void_p,
+                                          c_void_p, c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p, c_int]
+                                         + [c_void_p] * 5 + [c_int] * 3 + [c_void_p])
+        lib.adapcc_cs_context_init.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
+                                               c_void_p]
         _bound = True
     return lib
 
@@ -550,3 +560,201 @@ def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, promp
     _ck(_lib().adapcc_penalize_repeats(p(logits), logits.stride(0), int(vocab), R, p(seq), seq.shape[1],
                                        p(prompt_len), p(lens), p(step), p(ids), p(parent), int(group),
                                        float(penalty), int(ngram), _stream()), "penalize_repeats")
+
+
+# ---- contrastive search: candidate attention, selection, re-rank and commit (csrc/ops_contrastive.cu) ---------------
+CONTRASTIVE_MAX_K = 16         # candidates per row
+CONTRASTIVE_MAX_D = 1024       # hidden size the re-rank kernels hold per lane
+CONTRASTIVE_MAX_IDS = 1024     # ids per suppress / stop list
+
+
+def cand_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor, top_k: int,
+                    out: torch.Tensor, side_k: torch.Tensor, side_v: torch.Tensor, work: torch.Tensor) -> torch.Tensor:
+    """Decode attention of ``top_k`` candidate tokens per cache row. ``qkv`` bf16 [B·k, 3·H·Dh] (q | k | v of candidate
+    j of row b in row ``b·k + j``; unit column stride), ``k_cache`` / ``v_cache`` bf16 [B, H, t_max, Dh], ``lens``
+    int32 [B]. Candidate (b, j) attends over the row's cached positions ``0..lens[b]-1`` and its own new key and value at
+    ``lens[b]``: ``out[b·k + j]`` (bf16 [B·k, H·Dh]) is bit-identical to ``decode_attention_`` on a row that holds that
+    token. The cache is only read (each cached element once per CTA for all k queries); the new keys and values go to
+    ``side_k`` / ``side_v`` (bf16 [B·k, H·Dh]). ``work``: fp32, ``decode_attention_work_numel(B·k, ...)`` elements.
+    The grid depends on t_max, B and k only; no host sync."""
+    def bad(msg):
+        raise ValueError(f"cand_attention_: {msg}")
+
+    for name, t in (("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out), ("side_k", side_k),
+                    ("side_v", side_v)):
+        if t.dtype != torch.bfloat16:
+            bad(f"{name} must be bf16, got {t.dtype}")
+    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
+        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
+            f"and {tuple(v_cache.shape)}")
+    B, H, t_max, Dh = k_cache.shape
+    K = int(top_k)
+    if not 1 <= K <= CONTRASTIVE_MAX_K:
+        bad(f"top_k must be in [1, {CONTRASTIVE_MAX_K}], got {top_k}")
+    if qkv.dim() != 2 or qkv.shape != (B * K, 3 * H * Dh) or qkv.stride(1) != 1:
+        bad(f"qkv must be [{B * K}, {3 * H * Dh}] with unit column stride, got {tuple(qkv.shape)} stride {qkv.stride()}")
+    for name, t in (("out", out), ("side_k", side_k), ("side_v", side_v)):
+        if t.shape != (B * K, H * Dh) or not t.is_contiguous():
+            bad(f"{name} must be a contiguous [{B * K}, {H * Dh}] tensor, got {tuple(t.shape)}")
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
+        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    if work.dtype != torch.float32 or not work.is_contiguous():
+        bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
+    dev = k_cache.device
+    if dev.type != "cuda" or any(t.device != dev for t in (qkv, v_cache, lens, out, side_k, side_v, work)):
+        bad("all tensors must be on one CUDA device")
+    need = decode_attention_work_numel(B * K, H, Dh, t_max)
+    if work.numel() < need:
+        bad(f"work holds {work.numel()} elements, {need} needed")
+    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
+    _ck(_lib().adapcc_cand_attn(p(qkv), p(k_cache), p(v_cache), p(lens), p(out), p(side_k), p(side_v), B, K, H, Dh,
+                                t_max, qkv.stride(0), p(work), _stream()), "cand_attn")
+    return out
+
+
+class ContrastiveState:
+    """Device state of a batched contrastive search of ``batch`` rows with ``top_k`` candidates each, up to ``max_new``
+    tokens and a cache of ``t_max`` positions (``n_layer`` layers, ``n_head`` heads of ``head_dim``), as
+    ``contrastive_select_`` and ``contrastive_rerank_`` read and write it. Candidate j of row b is row ``b·k + j``.
+
+    ``step`` int32 [1] (tokens emitted); ``done`` int32 [B]; ``next_ids`` int64 [B·k] the candidates' ids (the candidate
+    step's input; 0 in an invalid slot), ``cand_tok`` int32 [B·k] the same with -1 in an invalid slot, ``cand_p`` fp32
+    [B·k] their probabilities; ``tokens`` int64 [B, max_new] the output (-1 after a stop); ``win_ids`` int64 [B] and
+    ``win_h`` bf16 [B, D] each row's emitted candidate and its hidden state; ``ctx`` bf16 [B, t_max, D] and
+    ``ctx_norm`` fp32 [B, t_max] the rows' context; ``side`` bf16 [n_layer, 2, B·k, D] the candidates' new keys and
+    values; ``sim`` fp32 the re-rank scratch; ``work`` fp32 the candidate attention's split partials."""
+
+    def __init__(self, batch: int, top_k: int, max_new: int, t_max: int, n_layer: int, n_head: int, head_dim: int,
+                 device):
+        B, K, n = int(batch), int(top_k), int(max_new)
+        D = n_head * head_dim
+        if B < 1 or not 1 <= K <= CONTRASTIVE_MAX_K or n < 1 or not 1 <= t_max or D > CONTRASTIVE_MAX_D:
+            raise ValueError(f"ContrastiveState: need batch >= 1, 1 <= top_k <= {CONTRASTIVE_MAX_K}, max_new >= 1, "
+                             f"t_max >= 1 and a hidden size <= {CONTRASTIVE_MAX_D}, got {batch}, {top_k}, {max_new}, "
+                             f"{t_max}, {D}")
+        self.batch, self.top_k, self.max_new, self.t_max = B, K, n, int(t_max)
+        self.n_layer, self.n_head, self.head_dim = int(n_layer), int(n_head), int(head_dim)
+        i32, dev = dict(dtype=torch.int32, device=device), device
+        bf = dict(dtype=torch.bfloat16, device=dev)
+        self.step = torch.zeros(1, **i32)
+        self.done = torch.zeros(B, **i32)
+        self.next_ids = torch.zeros(B * K, dtype=torch.int64, device=dev)
+        self.cand_tok = torch.full((B * K,), -1, **i32)
+        self.cand_p = torch.zeros(B * K, dtype=torch.float32, device=dev)
+        self.tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
+        self.win_ids = torch.zeros(B, dtype=torch.int64, device=dev)
+        self.win_h = torch.zeros(B, D, **bf)
+        self.ctx = torch.zeros(B, self.t_max, D, **bf)
+        self.ctx_norm = torch.zeros(B, self.t_max, dtype=torch.float32, device=dev)
+        self.side = torch.zeros(self.n_layer, 2, B * K, D, **bf)
+        self.sim = torch.empty(int(_lib().adapcc_cs_sim_numel(B, K, self.t_max)), dtype=torch.float32, device=dev)
+        self.work = torch.empty(decode_attention_work_numel(B * K, n_head, head_dim, self.t_max), dtype=torch.float32,
+                                device=dev)
+
+    def tensors(self):
+        """Every device tensor of the state (what the ops check for one device)."""
+        return (self.step, self.done, self.next_ids, self.cand_tok, self.cand_p, self.tokens, self.win_ids, self.win_h,
+                self.ctx, self.ctx_norm, self.side, self.sim, self.work)
+
+
+def _id_list(who, name, t):
+    if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 1
+                          or t.numel() > CONTRASTIVE_MAX_IDS):
+        raise ValueError(f"{who}: {name} must be a contiguous 1-D int32 tensor of at most {CONTRASTIVE_MAX_IDS} ids, "
+                         f"got {t.dtype} {tuple(t.shape)}")
+    return c_void_p(t.data_ptr() if t is not None and t.numel() else None), t.numel() if t is not None else 0
+
+
+def _same_device(who, dev, tensors):
+    if dev.type != "cuda" or any(t.device != dev for t in tensors):
+        raise ValueError(f"{who}: all tensors must be on one CUDA device, got {dev} and "
+                         f"{sorted(set(str(t.device) for t in tensors))}")
+
+
+def contrastive_select_(logits: torch.Tensor, vocab: int, state: ContrastiveState, min_new: int = 0,
+                        suppress_ids: Optional[torch.Tensor] = None) -> None:
+    """The candidates of every row, on the device (the definition in ``ops/contrastive.py``): the ``top_k`` ids with
+    the largest logits of ``logits`` fp32 [B, ld] (the first ``vocab`` columns; ties to the lower id, -inf never),
+    each with ``p = exp(l - m) / Z`` over the remaining ids; ``suppress_ids`` (int32 list or None) are removed while
+    ``state.step < min_new``. A row that is done gets none. Writes ``state.next_ids``, ``cand_tok`` and ``cand_p``.
+    No host sync."""
+    def bad(msg):
+        raise ValueError(f"contrastive_select_: {msg}")
+
+    if not isinstance(state, ContrastiveState):
+        bad(f"state must be a ContrastiveState, got {type(state).__name__}")
+    B, K = state.batch, state.top_k
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1 or logits.shape[0] != B:
+        bad(f"logits must be fp32 [{B}, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
+    if not 1 <= vocab <= logits.shape[1]:
+        bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
+    if int(min_new) < 0:
+        bad(f"min_new must be >= 0, got {min_new}")
+    sup, n_sup = _id_list("contrastive_select_", "suppress_ids", suppress_ids)
+    _same_device("contrastive_select_", logits.device,
+                 list(state.tensors()) + ([suppress_ids] if suppress_ids is not None else []))
+    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
+    _ck(_lib().adapcc_cs_select(p(logits), logits.stride(0), int(vocab), B, K, p(state.step), int(min_new), sup, n_sup,
+                                p(state.done), p(state.next_ids), p(state.cand_tok), p(state.cand_p), _stream()),
+        "cs_select")
+
+
+def contrastive_rerank_(hc: torch.Tensor, state: ContrastiveState, alpha: float, k_cache: torch.Tensor,
+                        v_cache: torch.Tensor, lens: torch.Tensor, stop_ids: Optional[torch.Tensor] = None) -> None:
+    """Re-rank every row's candidates and commit the winner, on the device (the definition in ``ops/contrastive.py``).
+    ``hc`` bf16 [B·k, D] (unit column stride) are the candidates' final hidden states; candidate j scores
+    ``(1 - alpha) p_j - alpha max_c cos(h_j, c)`` over the row's context ``state.ctx[b, :lens[b]]`` (a zero norm gives
+    cosine 0) and the best wins, ties to the lower rank; a row without a candidate emits id 0. Writes column
+    ``state.step`` of ``state.tokens`` (-1 for a stop id, which also sets ``done``, or a row already done),
+    ``state.win_ids`` and ``state.win_h``; appends the winner's hidden state and norm to the context at ``lens[b]``;
+    copies its keys and values from ``state.side`` into ``k_cache`` / ``v_cache`` (bf16 [n_layer, B, H, t_max, Dh]) at
+    ``lens[b]``; then advances ``lens`` (int32 [B]) and ``state.step``. No host sync."""
+    def bad(msg):
+        raise ValueError(f"contrastive_rerank_: {msg}")
+
+    if not isinstance(state, ContrastiveState):
+        bad(f"state must be a ContrastiveState, got {type(state).__name__}")
+    if not 0.0 <= float(alpha) <= 1.0:
+        bad(f"alpha must be in [0, 1], got {alpha}")
+    B, K, t_max = state.batch, state.top_k, state.t_max
+    Lyr, H, Dh = state.n_layer, state.n_head, state.head_dim
+    D = H * Dh
+    if hc.dtype != torch.bfloat16 or hc.dim() != 2 or hc.shape != (B * K, D) or hc.stride(1) != 1 or hc.stride(0) % 8:
+        bad(f"hc must be bf16 [{B * K}, {D}] with unit column stride and a row stride that is a multiple of 8, got "
+            f"{hc.dtype} {tuple(hc.shape)} stride {hc.stride()}")
+    for name, t in (("k_cache", k_cache), ("v_cache", v_cache)):
+        if t.dtype != torch.bfloat16 or t.shape != (Lyr, B, H, t_max, Dh) or not t.is_contiguous():
+            bad(f"{name} must be a contiguous bf16 [{Lyr}, {B}, {H}, {t_max}, {Dh}] tensor, got {t.dtype} "
+                f"{tuple(t.shape)}")
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
+        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    stop, n_stop = _id_list("contrastive_rerank_", "stop_ids", stop_ids)
+    _same_device("contrastive_rerank_", hc.device, list(state.tensors()) + [k_cache, v_cache, lens]
+                 + ([stop_ids] if stop_ids is not None else []))
+    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
+    _ck(_lib().adapcc_cs_rerank(p(hc), hc.stride(0), B, K, D, p(state.cand_tok), p(state.cand_p), float(alpha),
+                                p(state.ctx), p(state.ctx_norm), t_max, p(state.sim), p(lens), p(state.done), stop,
+                                n_stop, p(state.step), p(state.tokens), state.max_new, p(state.win_ids),
+                                p(state.win_h), p(state.side), p(k_cache), p(v_cache), Lyr, H, Dh, _stream()),
+        "cs_rerank")
+
+
+def contrastive_context_init_(h: torch.Tensor, lens: torch.Tensor, state: ContrastiveState) -> None:
+    """The rows' context from a prefill: ``state.ctx[b, p] = h[b, p]`` and its fp32 norm for ``p < lens[b]``, ``h`` the
+    contiguous bf16 [B, T, D] final hidden states, ``lens`` int32 [B] the prompt lengths. No host sync."""
+    def bad(msg):
+        raise ValueError(f"contrastive_context_init_: {msg}")
+
+    if not isinstance(state, ContrastiveState):
+        bad(f"state must be a ContrastiveState, got {type(state).__name__}")
+    B, D = state.batch, state.n_head * state.head_dim
+    if h.dtype != torch.bfloat16 or h.dim() != 3 or h.shape[0] != B or h.shape[2] != D or not h.is_contiguous():
+        bad(f"h must be a contiguous bf16 [{B}, T, {D}] tensor, got {h.dtype} {tuple(h.shape)}")
+    if not 1 <= h.shape[1] <= state.t_max:
+        bad(f"h holds {h.shape[1]} positions, the context at most {state.t_max}")
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
+        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    _same_device("contrastive_context_init_", h.device, [lens, state.ctx, state.ctx_norm])
+    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
+    _ck(_lib().adapcc_cs_context_init(p(h), B, h.shape[1], D, p(lens), p(state.ctx), p(state.ctx_norm), state.t_max,
+                                      _stream()), "cs_context_init")

@@ -42,6 +42,9 @@ def main():
                    help="f1: penalty on ids already in the prompt or reply (1: off); replies go through the batched path")
     p.add_argument("--no_repeat_ngram_size", type=int, default=0,
                    help="f1: never repeat an n-gram of the prompt or reply (0: off); replies go through the batched path")
+    p.add_argument("--penalty_alpha", type=float, default=0.0,
+                   help="f1: > 0 decodes the replies with GPT2DoubleHeads.contrastive_search, this degeneration penalty "
+                        "and --top_k candidates (0: sample); replies go through the batched path")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -53,7 +56,7 @@ def main():
     if a.eval_type == "f1":
         kw = dict(max_length=a.max_length, min_length=a.min_length, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p,
                   no_sample=a.no_sample, repetition_penalty=a.repetition_penalty,
-                  no_repeat_ngram_size=a.no_repeat_ngram_size)
+                  no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha)
     res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
                            a.batch_size, a.num_beams, **kw)
     print(json.dumps(res))
