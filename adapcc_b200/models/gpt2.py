@@ -192,6 +192,44 @@ class CandidateKV:
                                 c.lens.repeat_interleave(K))
 
 
+class _Repeats:
+    """The repetition controls of a batched decoder over the R rows of its cache: ``seq`` int32 [R, t_max] each row's
+    sequence (its prompt, then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the penalty and the
+    n-gram size. ``create`` returns None when both controls are off, so then nothing is allocated or launched."""
+
+    def __init__(self, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int):
+        B, T = input_ids.shape
+        self.seq = torch.zeros(cache.batch, cache.t_max, dtype=torch.int32, device=input_ids.device)
+        self.seq[:, :T] = input_ids.repeat_interleave(cache.batch // B, dim=0)
+        self.prompt_len = cache.lens.clone()
+        self.vocab, self.penalty, self.ngram = vocab, penalty, ngram
+
+    @classmethod
+    def create(cls, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float,
+               ngram: int) -> Optional["_Repeats"]:
+        return cls(input_ids, cache, vocab, penalty, ngram) if penalty != 1.0 or ngram > 0 else None
+
+    def eager(self, logits: torch.Tensor, cache: KVCache, consumed: Optional[torch.Tensor]) -> torch.Tensor:
+        """``penalize_repeats_reference`` over every row's sequence, after storing ``consumed`` [R] (the tokens the last
+        decode step consumed; None before the first one) at ``lens - 1``."""
+        if consumed is not None:
+            dev = self.seq.device
+            self.seq[torch.arange(cache.batch, device=dev), cache.lens.long() - 1] = consumed.to(dev, torch.int32)
+        return penalize_repeats_reference(logits, [self.seq[r, :x] for r, x in enumerate(cache.host_lens)],
+                                          self.vocab, self.penalty, self.ngram)
+
+    def reorder(self, rows: torch.Tensor) -> None:
+        """Row r continues row ``rows[r]`` (a beam its parent)."""
+        self.seq = self.seq[rows]
+
+    def native(self, logits: torch.Tensor, lens: torch.Tensor, step: torch.Tensor, ids: torch.Tensor,
+               parent: Optional[torch.Tensor] = None, group: int = 1) -> None:
+        """``ops.penalize_repeats_`` on ``logits`` in place; it also stores ``ids`` and follows ``parent``."""
+        from ..ops import penalize_repeats_
+        penalize_repeats_(logits, self.vocab, self.seq, self.prompt_len, lens, step, ids, parent, group,
+                          self.penalty, self.ngram)
+
+
 class Block(nn.Module):
     """Pre-LN transformer block; the MLP runs as two GEMMs with the activation passes in GEMM epilogues when
     supported (ops/gemm.py), residual adds optionally fused into the following LayerNorm (``forward_deferred``)."""
@@ -454,6 +492,44 @@ class GPT2DoubleHeads(nn.Module):
         cache.advance()
         return h
 
+    def _decode_setup(self, who: str, input_ids: torch.Tensor, lengths: Optional[Sequence[int]],
+                      token_type_ids: Optional[torch.Tensor], reply_type, max_new_tokens: int, min_new_tokens: int,
+                      repetition_penalty: float, no_repeat_ngram_size: int, num_beams: int = 1):
+        """The checks and prompt quantities the batched decoders share, before anything is launched:
+        ``(B, T, lengths, n, t_max, last, tt_new, native)``. ``last`` [B] is each prompt's last position, ``tt_new`` [B]
+        the token type of new tokens (None without token types), and ``native`` says whether the bf16 CUDA kernels
+        run; they take at most ``LM_HEAD_MAX_ROWS`` rows, ``num_beams`` per prompt. Errors name ``who``."""
+        from ..ops import LM_HEAD_MAX_ROWS
+
+        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
+            raise ValueError(f"{who}: input_ids must be [B, T], got {tuple(input_ids.shape)}")
+        B, T = input_ids.shape
+        dev = input_ids.device
+        lengths = [T] * B if lengths is None else [int(x) for x in lengths]
+        if len(lengths) != B or any(not 1 <= x <= T for x in lengths):
+            raise ValueError(f"{who}: need {B} lengths in [1, {T}], got {lengths}")
+        n = int(max_new_tokens)
+        if n < 1 or int(min_new_tokens) < 0:
+            raise ValueError(f"{who}: need max_new_tokens >= 1 and min_new_tokens >= 0, got {max_new_tokens}, "
+                             f"{min_new_tokens}")
+        check_repeat_args(who, repetition_penalty, no_repeat_ngram_size)
+        t_max = max(lengths) + n
+        if t_max > self.cfg.n_positions:
+            raise ValueError(f"{who}: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds "
+                             f"n_positions = {self.cfg.n_positions}")
+        weight = self.wte.weight
+        native = weight.is_cuda and weight.dtype == torch.bfloat16
+        if native and B * num_beams > LM_HEAD_MAX_ROWS:
+            what, got = ("rows", B) if num_beams == 1 else ("beam rows (batch x num_beams)", f"{B} x {num_beams}")
+            raise ValueError(f"{who}: at most {LM_HEAD_MAX_ROWS} {what} per call on the native path, got {got}")
+        last = torch.tensor(lengths, device=dev) - 1
+        tt_new = None
+        if reply_type is not None:
+            tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
+        elif token_type_ids is not None:
+            tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
+        return B, T, lengths, n, t_max, last, tt_new, native
+
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
                  token_type_ids: Optional[torch.Tensor] = None, reply_type=None, max_new_tokens: int = 20,
@@ -480,25 +556,13 @@ class GPT2DoubleHeads(nn.Module):
         repetition control is on) and sampler, which feeds the drawn ids back into its own input; the host reads the
         done flags once every 8 tokens, a step late, to stop early. Elsewhere the same loop runs eagerly with fp32
         PyTorch logits, ``ops.repeats.penalize_repeats_reference`` and ``ops.sampling.sample_reference``."""
-        cfg = self.cfg
-        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
-            raise ValueError(f"generate: input_ids must be [B, T], got {tuple(input_ids.shape)}")
-        B, T = input_ids.shape
-        dev = input_ids.device
-        lengths = [T] * B if lengths is None else [int(n) for n in lengths]
-        if len(lengths) != B or any(not 1 <= n <= T for n in lengths):
-            raise ValueError(f"generate: need {B} lengths in [1, {T}], got {lengths}")
-        if int(max_new_tokens) < 1:
-            raise ValueError(f"generate: max_new_tokens must be >= 1, got {max_new_tokens}")
-        if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1 or int(min_new_tokens) < 0:
-            raise ValueError(f"generate: need temperature >= 0, top_k >= 0, 0 < top_p <= 1 and min_new_tokens >= 0, "
-                             f"got {temperature}, {top_k}, {top_p}, {min_new_tokens}")
-        check_repeat_args("generate", repetition_penalty, no_repeat_ngram_size)
-        repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
-        t_max = max(lengths) + int(max_new_tokens)
-        if t_max > cfg.n_positions:
-            raise ValueError(f"generate: the longest prompt ({max(lengths)}) plus max_new_tokens ({max_new_tokens}) "
-                             f"exceeds n_positions = {cfg.n_positions}; sample_sequence slides the window instead")
+        if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
+            raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
+                             f"{top_k}, {top_p}")
+        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+            "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
+            repetition_penalty, no_repeat_ngram_size)
+        dev, V = input_ids.device, self.cfg.vocab_size
         if isinstance(seed, torch.Tensor):
             if seed.dtype != torch.int64 or seed.numel() != B:
                 raise ValueError(f"generate: a seed tensor must be int64 with {B} elements, got {seed.dtype} "
@@ -506,76 +570,46 @@ class GPT2DoubleHeads(nn.Module):
             seeds = seed.reshape(B).to(dev)
         else:
             seeds = (int(seed) + torch.arange(B, dtype=torch.int64)).to(dev)
-        last = torch.tensor(lengths, device=dev) - 1
-        tt_new = None
-        if reply_type is not None:
-            tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
-        elif token_type_ids is not None:
-            tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
         cache = self.new_cache(B, t_max)
         h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
-        n = int(max_new_tokens)
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
-        if repeats:                                 # the rows' sequences: prompt, then each consumed token
-            seq = torch.zeros(B, t_max, dtype=torch.int32, device=dev)
-            seq[:, :T] = input_ids
-        if cache.work is None:                      # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
+        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
+        if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = self.wte.weight.float()
             done = torch.zeros(B, dtype=torch.int32)
             for i in range(n):
                 if i:
                     h = self.decode_step(nxt.to(dev), tt_new, cache)
                 logits = self.lm_logits(h, head)
-                if repeats:
-                    if i:
-                        seq[torch.arange(B, device=dev), cache.lens.long() - 1] = nxt.to(dev, torch.int32)
-                    logits = penalize_repeats_reference(logits, [seq[b, :x] for b, x in enumerate(cache.host_lens)],
-                                                        cfg.vocab_size, repetition_penalty, no_repeat_ngram_size)
-                nxt, tok, done = sample_reference(logits, cfg.vocab_size, temperature, top_k, top_p,
+                if reps is not None:
+                    logits = reps.eager(logits, cache, nxt if i else None)
+                nxt, tok, done = sample_reference(logits, V, temperature, top_k, top_p,
                                                   seeds, cache.lens, i, min_new_tokens, suppress_ids, stop_ids, done)
                 tokens[:, i] = tok.to(dev)
                 if bool(done.all()):
                     break
             return tokens, (tokens >= 0).sum(1)
 
-        from ..ops import LM_HEAD_MAX_ROWS, lm_head_logits_, penalize_repeats_, sample_tokens_
+        from ..ops import lm_head_logits_, sample_tokens_
 
-        if B > LM_HEAD_MAX_ROWS:
-            raise ValueError(f"generate: at most {LM_HEAD_MAX_ROWS} rows per call on the native path, got {B}")
         weight = self.wte.weight
         logits = torch.empty(B, weight.shape[0], dtype=torch.float32, device=dev)
         next_ids = torch.zeros(B, dtype=torch.int64, device=dev)
         done = torch.zeros(B, dtype=torch.int32, device=dev)
         step = torch.zeros(1, dtype=torch.int32, device=dev)
-        sup = torch.tensor(list(suppress_ids), dtype=torch.int32, device=dev)
-        stop = torch.tensor(list(stop_ids), dtype=torch.int32, device=dev)
-        prompt_len = cache.lens.clone() if repeats else None
+        sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
 
         def head_and_sample(hidden):
             lm_head_logits_(hidden, weight, logits)
-            if repeats:
-                penalize_repeats_(logits, cfg.vocab_size, seq, prompt_len, cache.lens, step, next_ids, None, 1,
-                                  repetition_penalty, no_repeat_ngram_size)
-            sample_tokens_(logits, cfg.vocab_size, temperature, top_k, top_p, seeds, cache.lens, step,
+            if reps is not None:
+                reps.native(logits, cache.lens, step, next_ids)
+            sample_tokens_(logits, V, temperature, top_k, top_p, seeds, cache.lens, step,
                            min_new_tokens, sup, stop, done, next_ids, tokens)
 
         head_and_sample(h)                          # the first token, from the prefill's last positions
-        if n == 1:
-            return tokens, (tokens >= 0).sum(1)
-        # the sampler writes each token's ids into the graph's own input buffer
-        graph = DecodeGraph(self, cache, tt_new is not None, head=head_and_sample, ids=next_ids, tt=tt_new)
-        flags = torch.empty(B, dtype=torch.int32, pin_memory=True)
-        copied = None
-        for i in range(1, n):
-            graph.replay()
-            if i % 8 == 0:                          # the flags copied 8 tokens ago are ready by now: no stall
-                if copied is not None:
-                    copied.synchronize()
-                    if bool(flags.all()):
-                        break
-                flags.copy_(done, non_blocking=True)
-                copied = torch.cuda.Event()
-                copied.record()
+        if n > 1:
+            # the sampler writes each token's ids into the graph's own input buffer
+            DecodeGraph(self, cache, tt_new is not None, head=head_and_sample, ids=next_ids, tt=tt_new).run(n - 1, done)
         return tokens, (tokens >= 0).sum(1)
 
     @torch.no_grad()
@@ -606,43 +640,19 @@ class GPT2DoubleHeads(nn.Module):
         reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the host reads the done flags once every 8
         tokens, a period late. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
         ``ops.repeats.penalize_repeats_reference``, ``ops.beam.BeamReference`` and torch indexing."""
-        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, LM_HEAD_MAX_ROWS
+        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS
         from ..ops.beam import BeamReference, best_hypotheses
 
-        cfg = self.cfg
-        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
-            raise ValueError(f"beam_search: input_ids must be [B, T], got {tuple(input_ids.shape)}")
-        B, T = input_ids.shape
-        K, n = int(num_beams), int(max_new_tokens)
-        dev = input_ids.device
-        lengths = [T] * B if lengths is None else [int(x) for x in lengths]
-        if len(lengths) != B or any(not 1 <= x <= T for x in lengths):
-            raise ValueError(f"beam_search: need {B} lengths in [1, {T}], got {lengths}")
+        K = int(num_beams)
         if not 1 <= K <= BEAM_MAX_BEAMS:
             raise ValueError(f"beam_search: num_beams must be in [1, {BEAM_MAX_BEAMS}], got {num_beams}")
-        if n < 1 or int(min_new_tokens) < 0:
-            raise ValueError(f"beam_search: need max_new_tokens >= 1 and min_new_tokens >= 0, got {max_new_tokens}, "
-                             f"{min_new_tokens}")
         if len(stop_ids) > BEAM_MAX_STOP or len(suppress_ids) > BEAM_MAX_SUPPRESS:
             raise ValueError(f"beam_search: at most {BEAM_MAX_STOP} stop ids and {BEAM_MAX_SUPPRESS} suppressed ids, "
                              f"got {len(stop_ids)} and {len(suppress_ids)}")
-        check_repeat_args("beam_search", repetition_penalty, no_repeat_ngram_size)
-        repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
-        t_max = max(lengths) + n
-        if t_max > cfg.n_positions:
-            raise ValueError(f"beam_search: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds "
-                             f"n_positions = {cfg.n_positions}")
-        weight = self.wte.weight
-        native = weight.is_cuda and weight.dtype == torch.bfloat16
-        if native and B * K > LM_HEAD_MAX_ROWS:
-            raise ValueError(f"beam_search: at most {LM_HEAD_MAX_ROWS} beam rows (batch x num_beams) per call on the "
-                             f"native path, got {B} x {K}")
-        last = torch.tensor(lengths, device=dev) - 1
-        tt_new = None
-        if reply_type is not None:
-            tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
-        elif token_type_ids is not None:
-            tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
+        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+            "beam_search", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
+            repetition_penalty, no_repeat_ngram_size, num_beams=K)
+        dev, V, weight = input_ids.device, self.cfg.vocab_size, self.wte.weight
         if tt_new is not None:
             tt_new = tt_new.repeat_interleave(K)
         # one prefill per prompt, its keys and values copied to the prompt's K rows (the beams share that region)
@@ -654,10 +664,7 @@ class GPT2DoubleHeads(nn.Module):
         cache.v[:, :, :, :T].copy_(pre.v.repeat_interleave(K, dim=1))
         del pre
         h = h.repeat_interleave(K, dim=0).contiguous()
-        V = cfg.vocab_size
-        if repeats:                                 # each beam's sequence: the prompt, then its hypothesis
-            seq = torch.zeros(B * K, t_max, dtype=torch.int32, device=dev)
-            seq[:, :T] = input_ids.repeat_interleave(K, dim=0)
+        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             ref = BeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens)
             head = weight.float()
@@ -665,55 +672,37 @@ class GPT2DoubleHeads(nn.Module):
                 if i:
                     h = self.decode_step(nxt.to(dev), tt_new, cache)
                 logits = self.lm_logits(h, head)
-                if repeats:
-                    if i:
-                        seq[torch.arange(B * K, device=dev), cache.lens.long() - 1] = nxt.to(dev, torch.int32)
-                    logits = penalize_repeats_reference(logits, [seq[r, :x] for r, x in enumerate(cache.host_lens)],
-                                                        V, repetition_penalty, no_repeat_ngram_size)
+                if reps is not None:
+                    logits = reps.eager(logits, cache, nxt if i else None)
                 nxt, parent = ref.step(logits)
                 rows = parent.to(dev)
                 cache.k.copy_(cache.k[:, rows])
                 cache.v.copy_(cache.v[:, rows])
-                if repeats:
-                    seq = seq[rows]
+                if reps is not None:
+                    reps.reorder(rows)
                 if ref.done.all():
                     break
             return tuple(t.to(dev) for t in ref.result())
 
-        from ..ops import (BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_,
-                           penalize_repeats_)
+        from ..ops import BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
 
         st = BeamState(B, K, n, length_penalty, dev)
         logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
-        sup = torch.tensor(list(suppress_ids), dtype=torch.int32, device=dev)
-        stop = torch.tensor(list(stop_ids), dtype=torch.int32, device=dev)
+        sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
         prompt_len = cache.lens.clone()
         scratch = torch.empty(kv_reorder_scratch_numel(cache.k, n), dtype=cache.k.dtype, device=dev)
 
         def select(hidden):
             lm_head_logits_(hidden, weight, logits)
-            if repeats:
-                penalize_repeats_(logits, V, seq, prompt_len, cache.lens, st.step, st.next_ids, st.parent, K,
-                                  repetition_penalty, no_repeat_ngram_size)
+            if reps is not None:
+                reps.native(logits, cache.lens, st.step, st.next_ids, st.parent, K)
             beam_step_(logits, V, st, min_new_tokens, sup, stop)
             kv_reorder_(cache.k, cache.v, st.parent, prompt_len, cache.lens, n, scratch)
 
         select(h)                                   # the first selection, from the prefill's last positions
         if n > 1:
             # beam_step_ writes the new beams' tokens into the graph's own input buffer
-            graph = DecodeGraph(self, cache, tt_new is not None, head=select, ids=st.next_ids, tt=tt_new)
-            flags = torch.empty(B, dtype=torch.int32, pin_memory=True)
-            copied = None
-            for i in range(1, n):
-                graph.replay()
-                if i % 8 == 0:                      # the flags copied 8 tokens ago are ready by now: no stall
-                    if copied is not None:
-                        copied.synchronize()
-                        if bool(flags.all()):
-                            break
-                    flags.copy_(st.done, non_blocking=True)
-                    copied = torch.cuda.Event()
-                    copied.record()
+            DecodeGraph(self, cache, tt_new is not None, head=select, ids=st.next_ids, tt=tt_new).run(n - 1, st.done)
         count = st.fin_count.cpu().tolist()
         score, n_tok, src = st.fin_score.cpu().tolist(), st.fin_n.cpu().tolist(), st.fin_src.cpu().tolist()
         fin = [list(zip(score[b], n_tok[b], src[b]))[:count[b]] for b in range(B)]
@@ -752,47 +741,22 @@ class GPT2DoubleHeads(nn.Module):
         the host reads the done flags once every 8 tokens, a period late. Elsewhere the same loop runs eagerly:
         candidates decode through ``decode_attention`` on a k-fold copy of the rows and the selection runs in fp64
         (``ops/contrastive.py``)."""
-        from ..ops import CONTRASTIVE_MAX_K, LM_HEAD_MAX_ROWS
+        from ..ops import CONTRASTIVE_MAX_K
         from ..ops.contrastive import check_contrastive_args, rerank_row, select_candidates
 
-        cfg = self.cfg
-        if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
-            raise ValueError(f"contrastive_search: input_ids must be [B, T], got {tuple(input_ids.shape)}")
-        B, T = input_ids.shape
-        dev = input_ids.device
-        lengths = [T] * B if lengths is None else [int(x) for x in lengths]
-        if len(lengths) != B or any(not 1 <= x <= T for x in lengths):
-            raise ValueError(f"contrastive_search: need {B} lengths in [1, {T}], got {lengths}")
         check_contrastive_args("contrastive_search", top_k, penalty_alpha, CONTRASTIVE_MAX_K)
-        K, n, alpha = int(top_k), int(max_new_tokens), float(penalty_alpha)
-        if n < 1 or int(min_new_tokens) < 0:
-            raise ValueError(f"contrastive_search: need max_new_tokens >= 1 and min_new_tokens >= 0, got "
-                             f"{max_new_tokens}, {min_new_tokens}")
-        check_repeat_args("contrastive_search", repetition_penalty, no_repeat_ngram_size)
-        repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
-        t_max = max(lengths) + n
-        if t_max > cfg.n_positions:
-            raise ValueError(f"contrastive_search: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) "
-                             f"exceeds n_positions = {cfg.n_positions}")
-        weight = self.wte.weight
-        native = weight.is_cuda and weight.dtype == torch.bfloat16
-        if native and B > LM_HEAD_MAX_ROWS:
-            raise ValueError(f"contrastive_search: at most {LM_HEAD_MAX_ROWS} rows per call on the native path, got {B}")
-        last = torch.tensor(lengths, device=dev) - 1
-        tt_new = None
-        if reply_type is not None:
-            tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
-        elif token_type_ids is not None:
-            tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
+        K, alpha = int(top_k), float(penalty_alpha)
+        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+            "contrastive_search", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
+            repetition_penalty, no_repeat_ngram_size)
+        cfg, dev, weight = self.cfg, input_ids.device, self.wte.weight
         tt_cand = tt_new.repeat_interleave(K) if tt_new is not None else None
         cache = self.new_cache(B, t_max)
         hs = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)
         h = hs[torch.arange(B, device=dev), last].contiguous()
         V, L, H = cfg.vocab_size, cfg.n_layer, cfg.n_head
         D = cfg.n_embd
-        if repeats:                                 # the rows' sequences: prompt, then each emitted token
-            seq = torch.zeros(B, t_max, dtype=torch.int32, device=dev)
-            seq[:, :T] = input_ids
+        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = weight.float()
             cand = CandidateKV(cache, K, torch.zeros(L, 2, B * K, D, dtype=weight.dtype, device=dev))
@@ -804,11 +768,8 @@ class GPT2DoubleHeads(nn.Module):
             win = None
             for i in range(n):
                 logits = self.lm_logits(h, head)
-                if repeats:
-                    if i:
-                        seq[rows, cache.lens.long() - 1] = win.to(dev, torch.int32)
-                    logits = penalize_repeats_reference(logits, [seq[b, :x] for b, x in enumerate(cache.host_lens)],
-                                                        V, repetition_penalty, no_repeat_ngram_size)
+                if reps is not None:
+                    logits = reps.eager(logits, cache, win)
                 ids, probs = select_candidates(logits, V, K, i, min_new_tokens, suppress_ids, done)
                 cache.check_room()
                 hc = self._candidate_hidden(ids.clamp(min=0).reshape(-1).to(dev), tt_cand, cand)
@@ -836,22 +797,19 @@ class GPT2DoubleHeads(nn.Module):
             return tokens.to(dev), (tokens >= 0).sum(1).to(dev)
 
         from ..ops import (ContrastiveState, contrastive_context_init_, contrastive_rerank_, contrastive_select_,
-                           lm_head_logits_, penalize_repeats_)
+                           lm_head_logits_)
 
         st = ContrastiveState(B, K, n, t_max, L, H, D // H, dev)
         contrastive_context_init_(hs.contiguous(), cache.lens, st)
         del hs
         cand = CandidateKV(cache, K, st.side, st.work)
         logits = torch.empty(B, weight.shape[0], dtype=torch.float32, device=dev)
-        sup = torch.tensor(list(suppress_ids), dtype=torch.int32, device=dev)
-        stop = torch.tensor(list(stop_ids), dtype=torch.int32, device=dev)
-        prompt_len = cache.lens.clone() if repeats else None
+        sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
 
         def select(hidden):
             lm_head_logits_(hidden, weight, logits)
-            if repeats:
-                penalize_repeats_(logits, V, seq, prompt_len, cache.lens, st.step, st.win_ids, None, 1,
-                                  repetition_penalty, no_repeat_ngram_size)
+            if reps is not None:
+                reps.native(logits, cache.lens, st.step, st.win_ids)
             contrastive_select_(logits, V, st, min_new_tokens, sup)
 
         def commit_and_select(hc):
@@ -862,18 +820,7 @@ class GPT2DoubleHeads(nn.Module):
         # contrastive_select_ writes the candidates into the graph's own input buffer; the commit advances the cache
         graph = DecodeGraph(self, cache, tt_cand is not None, head=commit_and_select, ids=st.next_ids, tt=tt_cand,
                             step=lambda ids, tt, c: self._candidate_hidden(ids, tt, cand))
-        flags = torch.empty(B, dtype=torch.int32, pin_memory=True)
-        copied = None
-        for i in range(1, n + 1):
-            graph.replay()
-            if i % 8 == 0 and i < n:                # the flags copied 8 tokens ago are ready by now: no stall
-                if copied is not None:
-                    copied.synchronize()
-                    if bool(flags.all()):
-                        break
-                flags.copy_(st.done, non_blocking=True)
-                copied = torch.cuda.Event()
-                copied.record()
+        graph.run(n, st.done)                       # the first replay commits the first token
         return st.tokens, (st.tokens >= 0).sum(1)
 
     def forward(self, input_ids, token_type_ids=None, mc_token_ids=None, lm_labels=None, mc_labels=None,
@@ -968,6 +915,23 @@ class DecodeGraph:
         self.graph.replay()
         self.cache.advance_host()
         return self.h
+
+    def run(self, replays: int, done: torch.Tensor) -> None:
+        """``replays`` replays, stopping early once every flag of ``done`` (int32, on the device) is set. Every 8
+        replays before the last the flags are copied to a pinned buffer, and the host reads that copy 8 replays later,
+        when it is long finished, so the host never waits for the device."""
+        flags = torch.empty(done.numel(), dtype=done.dtype, pin_memory=True)
+        copied = None
+        for i in range(1, replays + 1):
+            self.replay()
+            if i % 8 == 0 and i < replays:
+                if copied is not None:
+                    copied.synchronize()
+                    if bool(flags.all()):
+                        break
+                flags.copy_(done, non_blocking=True)
+                copied = torch.cuda.Event()
+                copied.record()
 
 
 class CachedDecoder:

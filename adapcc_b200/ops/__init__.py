@@ -80,6 +80,27 @@ def _ck(rc: int, what: str) -> None:
         raise NativeError(f"{what} failed: {last_error()}")
 
 
+def _ptr(t: Optional[torch.Tensor]) -> c_void_p:
+    """``t``'s data pointer; a null pointer for None."""
+    return c_void_p(t.data_ptr() if t is not None else None)
+
+
+def _id_list(who: str, name: str, t: Optional[torch.Tensor], cap: int):
+    """(pointer, count) of an optional id list, which must be a contiguous 1-D int32 tensor of at most ``cap`` ids."""
+    if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 1 or t.numel() > cap):
+        raise ValueError(f"{who}: {name} must be a contiguous 1-D int32 tensor of at most {cap} ids, got {t.dtype} "
+                         f"{tuple(t.shape)}")
+    return c_void_p(t.data_ptr() if t is not None and t.numel() else None), t.numel() if t is not None else 0
+
+
+def _same_device(who: str, dev: torch.device, tensors) -> None:
+    """``ValueError`` unless ``dev`` is a CUDA device and every tensor of ``tensors`` (None skipped) is on it."""
+    tensors = [t for t in tensors if t is not None]
+    if dev.type != "cuda" or any(t.device != dev for t in tensors):
+        raise ValueError(f"{who}: all tensors must be on one CUDA device, got {dev} and "
+                         f"{sorted(set(str(t.device) for t in tensors))}")
+
+
 def sumsq_(grad: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     """out (1-element fp32, already zeroed) += sum(grad**2)."""
     _ck(_lib().adapcc_sumsq(c_void_p(grad.data_ptr()), grad.numel(), _dt(grad), c_void_p(out.data_ptr()), _stream()),
@@ -361,25 +382,13 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
         bad(f"step must be a 1-element int32 tensor, got {step.dtype} {tuple(step.shape)}")
     if tokens.dtype != torch.int64 or tokens.dim() != 2 or tokens.shape[0] != B or not tokens.is_contiguous():
         bad(f"tokens must be a contiguous int64 [{B}, max_new] tensor, got {tokens.dtype} {tuple(tokens.shape)}")
-    lists = []
-    for name, t in (("suppress_ids", suppress_ids), ("stop_ids", stop_ids)):
-        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 1
-                              or t.numel() > SAMPLE_MAX_IDS):
-            bad(f"{name} must be a contiguous 1-D int32 tensor of at most {SAMPLE_MAX_IDS} ids, got "
-                f"{t.dtype} {tuple(t.shape)}")
-        lists.append((c_void_p(t.data_ptr() if t is not None and t.numel() else None),
-                      t.numel() if t is not None else 0))
-    dev = logits.device
-    others = [seeds, pos, step, done, next_ids, tokens] + [t for t in (suppress_ids, stop_ids) if t is not None]
-    if dev.type != "cuda" or any(t.device != dev for t in others):
-        bad(f"all tensors must be on one CUDA device, got logits on {dev} and "
-            f"{sorted(set(str(t.device) for t in others))}")
-    (sup, n_sup), (stop, n_stop) = lists
-    _ck(_lib().adapcc_sample_tokens(c_void_p(logits.data_ptr()), logits.stride(0), int(vocab), B, float(temperature),
-                                    int(top_k), float(top_p), c_void_p(seeds.data_ptr()), c_void_p(pos.data_ptr()),
-                                    c_void_p(step.data_ptr()), int(min_new), sup, n_sup, stop, n_stop,
-                                    c_void_p(done.data_ptr()), c_void_p(next_ids.data_ptr()),
-                                    c_void_p(tokens.data_ptr()), tokens.shape[1], _stream()), "sample_tokens")
+    sup, n_sup = _id_list("sample_tokens_", "suppress_ids", suppress_ids, SAMPLE_MAX_IDS)
+    stop, n_stop = _id_list("sample_tokens_", "stop_ids", stop_ids, SAMPLE_MAX_IDS)
+    _same_device("sample_tokens_", logits.device, (seeds, pos, step, done, next_ids, tokens, suppress_ids, stop_ids))
+    _ck(_lib().adapcc_sample_tokens(_ptr(logits), logits.stride(0), int(vocab), B, float(temperature), int(top_k),
+                                    float(top_p), _ptr(seeds), _ptr(pos), _ptr(step), int(min_new), sup, n_sup, stop,
+                                    n_stop, _ptr(done), _ptr(next_ids), _ptr(tokens), tokens.shape[1], _stream()),
+        "sample_tokens")
 
 
 # ---- beam search selection and KV-cache reordering (csrc/ops_beam.cu) ----------------------------------------------
@@ -450,24 +459,15 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
         bad(f"vocab must be in [1, ld = {logits.shape[1]}] with num_beams * vocab < 2^32, got {vocab}")
     if int(min_new) < 0:
         bad(f"min_new must be >= 0, got {min_new}")
-    lists = []
-    for name, t, cap in (("suppress_ids", suppress_ids, BEAM_MAX_SUPPRESS), ("stop_ids", stop_ids, BEAM_MAX_STOP)):
-        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 1 or t.numel() > cap):
-            bad(f"{name} must be a contiguous 1-D int32 tensor of at most {cap} ids, got {t.dtype} {tuple(t.shape)}")
-        lists.append((c_void_p(t.data_ptr() if t is not None and t.numel() else None),
-                      t.numel() if t is not None else 0))
-    dev = logits.device
-    others = list(state.tensors()) + [t for t in (suppress_ids, stop_ids) if t is not None]
-    if dev.type != "cuda" or any(t.device != dev for t in others):
-        bad(f"all tensors must be on one CUDA device, got logits on {dev} and "
-            f"{sorted(set(str(t.device) for t in others))}")
-    (sup, n_sup), (stop, n_stop) = lists
-    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
-    _ck(_lib().adapcc_beam_step(p(logits), logits.stride(0), int(vocab), B, K, p(state.scores), p(state.step),
-                                int(min_new), sup, n_sup, stop, n_stop, p(state.pen), int(state.length_penalty > 0),
-                                state.max_new, p(state.done), p(state.cand), p(state.next_ids), p(state.parent),
-                                p(state.hist_tok), p(state.hist_back), p(state.fin_score), p(state.fin_n),
-                                p(state.fin_src), p(state.fin_count), _stream()), "beam_step")
+    sup, n_sup = _id_list("beam_step_", "suppress_ids", suppress_ids, BEAM_MAX_SUPPRESS)
+    stop, n_stop = _id_list("beam_step_", "stop_ids", stop_ids, BEAM_MAX_STOP)
+    _same_device("beam_step_", logits.device, state.tensors() + (suppress_ids, stop_ids))
+    _ck(_lib().adapcc_beam_step(_ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores),
+                                _ptr(state.step), int(min_new), sup, n_sup, stop, n_stop, _ptr(state.pen),
+                                int(state.length_penalty > 0), state.max_new, _ptr(state.done), _ptr(state.cand),
+                                _ptr(state.next_ids), _ptr(state.parent), _ptr(state.hist_tok), _ptr(state.hist_back),
+                                _ptr(state.fin_score), _ptr(state.fin_n), _ptr(state.fin_src), _ptr(state.fin_count),
+                                _stream()), "beam_step")
 
 
 def kv_reorder_scratch_numel(k_cache: torch.Tensor, max_new: int) -> int:
@@ -502,13 +502,9 @@ def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tens
     need = kv_reorder_scratch_numel(k_cache, max_new)
     if not scratch.is_contiguous() or scratch.numel() < need:
         bad(f"scratch must be contiguous with at least {need} elements, got {scratch.numel()}")
-    dev = k_cache.device
-    if dev.type != "cuda" or any(t.device != dev for t in (v_cache, parent, prompt_len, lens, scratch)):
-        bad("all tensors must be on one CUDA device")
-    _ck(_lib().adapcc_kv_reorder(c_void_p(k_cache.data_ptr()), c_void_p(v_cache.data_ptr()), L, R, H, t_max, Dh,
-                                 c_void_p(parent.data_ptr()), c_void_p(prompt_len.data_ptr()),
-                                 c_void_p(lens.data_ptr()), int(max_new), c_void_p(scratch.data_ptr()), _stream()),
-        "kv_reorder")
+    _same_device("kv_reorder_", k_cache.device, (v_cache, parent, prompt_len, lens, scratch))
+    _ck(_lib().adapcc_kv_reorder(_ptr(k_cache), _ptr(v_cache), L, R, H, t_max, Dh, _ptr(parent), _ptr(prompt_len),
+                                 _ptr(lens), int(max_new), _ptr(scratch), _stream()), "kv_reorder")
 
 
 # ---- repetition penalty and no-repeat n-gram blocking (csrc/ops_repeats.cu) ----------------------------------------
@@ -551,14 +547,9 @@ def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, promp
                            ("parent", parent, torch.int32, R)):
         if t is not None and (t.dtype != dt or not t.is_contiguous() or t.numel() != n):
             bad(f"{name} must be a contiguous {dt} tensor of {n} elements, got {t.dtype} {tuple(t.shape)}")
-    dev = logits.device
-    others = [t for t in (seq, prompt_len, lens, step, ids, parent) if t is not None]
-    if dev.type != "cuda" or any(t.device != dev for t in others):
-        bad(f"all tensors must be on one CUDA device, got logits on {dev} and "
-            f"{sorted(set(str(t.device) for t in others))}")
-    p = lambda t: c_void_p(t.data_ptr() if t is not None else None)                  # noqa: E731
-    _ck(_lib().adapcc_penalize_repeats(p(logits), logits.stride(0), int(vocab), R, p(seq), seq.shape[1],
-                                       p(prompt_len), p(lens), p(step), p(ids), p(parent), int(group),
+    _same_device("penalize_repeats_", logits.device, (seq, prompt_len, lens, step, ids, parent))
+    _ck(_lib().adapcc_penalize_repeats(_ptr(logits), logits.stride(0), int(vocab), R, _ptr(seq), seq.shape[1],
+                                       _ptr(prompt_len), _ptr(lens), _ptr(step), _ptr(ids), _ptr(parent), int(group),
                                        float(penalty), int(ngram), _stream()), "penalize_repeats")
 
 
@@ -600,15 +591,12 @@ def cand_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Ten
         bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
     if work.dtype != torch.float32 or not work.is_contiguous():
         bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
-    dev = k_cache.device
-    if dev.type != "cuda" or any(t.device != dev for t in (qkv, v_cache, lens, out, side_k, side_v, work)):
-        bad("all tensors must be on one CUDA device")
+    _same_device("cand_attention_", k_cache.device, (qkv, v_cache, lens, out, side_k, side_v, work))
     need = decode_attention_work_numel(B * K, H, Dh, t_max)
     if work.numel() < need:
         bad(f"work holds {work.numel()} elements, {need} needed")
-    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
-    _ck(_lib().adapcc_cand_attn(p(qkv), p(k_cache), p(v_cache), p(lens), p(out), p(side_k), p(side_v), B, K, H, Dh,
-                                t_max, qkv.stride(0), p(work), _stream()), "cand_attn")
+    _ck(_lib().adapcc_cand_attn(_ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(lens), _ptr(out), _ptr(side_k),
+                                _ptr(side_v), B, K, H, Dh, t_max, qkv.stride(0), _ptr(work), _stream()), "cand_attn")
     return out
 
 
@@ -657,20 +645,6 @@ class ContrastiveState:
                 self.ctx, self.ctx_norm, self.side, self.sim, self.work)
 
 
-def _id_list(who, name, t):
-    if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.dim() != 1
-                          or t.numel() > CONTRASTIVE_MAX_IDS):
-        raise ValueError(f"{who}: {name} must be a contiguous 1-D int32 tensor of at most {CONTRASTIVE_MAX_IDS} ids, "
-                         f"got {t.dtype} {tuple(t.shape)}")
-    return c_void_p(t.data_ptr() if t is not None and t.numel() else None), t.numel() if t is not None else 0
-
-
-def _same_device(who, dev, tensors):
-    if dev.type != "cuda" or any(t.device != dev for t in tensors):
-        raise ValueError(f"{who}: all tensors must be on one CUDA device, got {dev} and "
-                         f"{sorted(set(str(t.device) for t in tensors))}")
-
-
 def contrastive_select_(logits: torch.Tensor, vocab: int, state: ContrastiveState, min_new: int = 0,
                         suppress_ids: Optional[torch.Tensor] = None) -> None:
     """The candidates of every row, on the device (the definition in ``ops/contrastive.py``): the ``top_k`` ids with
@@ -690,13 +664,11 @@ def contrastive_select_(logits: torch.Tensor, vocab: int, state: ContrastiveStat
         bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
     if int(min_new) < 0:
         bad(f"min_new must be >= 0, got {min_new}")
-    sup, n_sup = _id_list("contrastive_select_", "suppress_ids", suppress_ids)
-    _same_device("contrastive_select_", logits.device,
-                 list(state.tensors()) + ([suppress_ids] if suppress_ids is not None else []))
-    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
-    _ck(_lib().adapcc_cs_select(p(logits), logits.stride(0), int(vocab), B, K, p(state.step), int(min_new), sup, n_sup,
-                                p(state.done), p(state.next_ids), p(state.cand_tok), p(state.cand_p), _stream()),
-        "cs_select")
+    sup, n_sup = _id_list("contrastive_select_", "suppress_ids", suppress_ids, CONTRASTIVE_MAX_IDS)
+    _same_device("contrastive_select_", logits.device, state.tensors() + (suppress_ids,))
+    _ck(_lib().adapcc_cs_select(_ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.step), int(min_new), sup,
+                                n_sup, _ptr(state.done), _ptr(state.next_ids), _ptr(state.cand_tok), _ptr(state.cand_p),
+                                _stream()), "cs_select")
 
 
 def contrastive_rerank_(hc: torch.Tensor, state: ContrastiveState, alpha: float, k_cache: torch.Tensor,
@@ -728,15 +700,13 @@ def contrastive_rerank_(hc: torch.Tensor, state: ContrastiveState, alpha: float,
                 f"{tuple(t.shape)}")
     if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
         bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
-    stop, n_stop = _id_list("contrastive_rerank_", "stop_ids", stop_ids)
-    _same_device("contrastive_rerank_", hc.device, list(state.tensors()) + [k_cache, v_cache, lens]
-                 + ([stop_ids] if stop_ids is not None else []))
-    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
-    _ck(_lib().adapcc_cs_rerank(p(hc), hc.stride(0), B, K, D, p(state.cand_tok), p(state.cand_p), float(alpha),
-                                p(state.ctx), p(state.ctx_norm), t_max, p(state.sim), p(lens), p(state.done), stop,
-                                n_stop, p(state.step), p(state.tokens), state.max_new, p(state.win_ids),
-                                p(state.win_h), p(state.side), p(k_cache), p(v_cache), Lyr, H, Dh, _stream()),
-        "cs_rerank")
+    stop, n_stop = _id_list("contrastive_rerank_", "stop_ids", stop_ids, CONTRASTIVE_MAX_IDS)
+    _same_device("contrastive_rerank_", hc.device, state.tensors() + (k_cache, v_cache, lens, stop_ids))
+    _ck(_lib().adapcc_cs_rerank(_ptr(hc), hc.stride(0), B, K, D, _ptr(state.cand_tok), _ptr(state.cand_p),
+                                float(alpha), _ptr(state.ctx), _ptr(state.ctx_norm), t_max, _ptr(state.sim),
+                                _ptr(lens), _ptr(state.done), stop, n_stop, _ptr(state.step), _ptr(state.tokens),
+                                state.max_new, _ptr(state.win_ids), _ptr(state.win_h), _ptr(state.side),
+                                _ptr(k_cache), _ptr(v_cache), Lyr, H, Dh, _stream()), "cs_rerank")
 
 
 def contrastive_context_init_(h: torch.Tensor, lens: torch.Tensor, state: ContrastiveState) -> None:
@@ -755,6 +725,5 @@ def contrastive_context_init_(h: torch.Tensor, lens: torch.Tensor, state: Contra
     if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
         bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
     _same_device("contrastive_context_init_", h.device, [lens, state.ctx, state.ctx_norm])
-    p = lambda t: c_void_p(t.data_ptr())                                             # noqa: E731
-    _ck(_lib().adapcc_cs_context_init(p(h), B, h.shape[1], D, p(lens), p(state.ctx), p(state.ctx_norm), state.t_max,
-                                      _stream()), "cs_context_init")
+    _ck(_lib().adapcc_cs_context_init(_ptr(h), B, h.shape[1], D, _ptr(lens), _ptr(state.ctx), _ptr(state.ctx_norm),
+                                      state.t_max, _stream()), "cs_context_init")
