@@ -90,7 +90,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9, no_sample: bool = False,
                    device="cpu", seeds: Optional[Sequence[int]] = None, num_beams: int = 0,
                    repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
-                   penalty_alpha: float = 0.0) -> List[List[int]]:
+                   penalty_alpha: float = 0.0, prompt_lookup_num_tokens: int = 0) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -100,7 +100,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     ``min_length`` (removed before the top-k / top-p filtering, where ``sample_reply`` re-draws after it).
     ``seeds``: one per dialogue (default 0, 1, ...). ``repetition_penalty`` and ``no_repeat_ngram_size`` go to
     ``generate`` / ``beam_search`` / ``contrastive_search`` (``ops/repeats.py``); the prompt counts as part of each
-    reply's sequence."""
+    reply's sequence. ``prompt_lookup_num_tokens`` > 0 (with ``no_sample``) verifies up to that many draft tokens per
+    step, copied from the prompt and the reply so far; the replies are the greedy ones (``ops/lookup.py``)."""
     insts = [build_input_from_segments(persona, history, [], tokenizer, with_eos=False,
                                        max_len=model.cfg.n_positions - max_length) for persona, history in dialogs]
     lengths = [len(i.input_ids) for i in insts]
@@ -125,7 +126,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     tokens, n_new = model.generate(ids, lengths, tt, reply_type, max_new_tokens=max_length,
                                    temperature=0.0 if no_sample else temperature, top_k=top_k, top_p=top_p,
                                    stop_ids=special, suppress_ids=special, min_new_tokens=min_length, seed=seed,
-                                   **repeats)
+                                   prompt_lookup_num_tokens=prompt_lookup_num_tokens, **repeats)
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
 
 
@@ -213,7 +214,7 @@ def next_word_probability(model, tokenizer: DialogTokenizer, persona, history, p
 def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_type: str = "f1", max_history: int = 2,
                      max_examples: int = 0, device="cpu", seed: int = 0, batch_size: int = 0, num_beams: int = 0,
                      repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, penalty_alpha: float = 0.0,
-                     **sample_kw) -> Dict[str, float]:
+                     prompt_lookup_num_tokens: int = 0, **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -229,13 +230,17 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``generate`` / ``beam_search`` (``ops/repeats.py``), also on that batched path.
 
     ``penalty_alpha > 0`` with ``f1``: the replies are decoded by contrastive search with ``top_k`` candidates
+    (:func:`sample_replies`), on that batched path.
+
+    ``prompt_lookup_num_tokens > 0`` with ``f1`` and ``no_sample``: greedy replies with prompt lookup decoding
     (:func:`sample_replies`), on that batched path."""
     repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
-    if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0) and eval_type == "f1":
+    lookup = prompt_lookup_num_tokens > 0
+    if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup) and eval_type == "f1":
         return _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples, device, seed,
                                     max(batch_size, 1), num_beams=num_beams, repetition_penalty=repetition_penalty,
                                     no_repeat_ngram_size=no_repeat_ngram_size, penalty_alpha=penalty_alpha,
-                                    **sample_kw)
+                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -192,6 +192,37 @@ class CandidateKV:
                                 c.lens.repeat_interleave(K))
 
 
+class VerifyKV:
+    """What a verify step of prompt-lookup decoding attends over: ``slots`` (k + 1) slots per row of ``cache``, slot j
+    of row b in row ``b·(k+1) + j`` at position ``cache.lens[b] + j``, the first ``nq[b]`` of them real (int32 [B]).
+    Real slot j attends over the row's cached positions and the new keys and values of its slots ``0..j``, which are
+    stored at their positions; pad slots write nothing and give zero. The lengths do not move. With ``work`` (bf16 CUDA
+    caches) this is the native kernel (``ops.verify_attention_``); otherwise masked fp32 attention in PyTorch."""
+
+    def __init__(self, cache: "KVCache", slots: int, nq: torch.Tensor, work: Optional[torch.Tensor] = None):
+        self.cache, self.slots, self.nq, self.work = cache, int(slots), nq, work
+
+    def attend(self, qkv: torch.Tensor, layer: int) -> torch.Tensor:
+        """Layer ``layer``'s attention of the slots ``qkv`` [B·(k+1), 3·H·Dh] -> [B·(k+1), H·Dh]."""
+        c, S = self.cache, self.slots
+        kc, vc = c.k[layer], c.v[layer]
+        B, H, t_max, Dh = kc.shape
+        if self.work is not None:
+            from ..ops import verify_attention_
+            out = torch.empty(B * S, H * Dh, dtype=qkv.dtype, device=qkv.device)
+            return verify_attention_(qkv, kc, vc, c.lens, self.nq, S - 1, out, self.work)
+        q, k, v = qkv.reshape(B, S, 3, H, Dh).unbind(2)
+        pos = c.lens.long()[:, None] + torch.arange(S, device=qkv.device)                       # [B, S]
+        real = (torch.arange(S, device=qkv.device) < self.nq.to(qkv.device).long()[:, None]) & (pos < t_max)
+        rows, slot = real.nonzero(as_tuple=True)
+        kc[rows, :, pos[rows, slot]] = k[rows, slot]
+        vc[rows, :, pos[rows, slot]] = v[rows, slot]
+        s = torch.einsum("bjhd,bhtd->bjht", q.float(), kc.float()) / math.sqrt(Dh)
+        s = s.masked_fill(torch.arange(t_max, device=qkv.device) > pos[:, :, None, None], float("-inf"))
+        o = torch.einsum("bjht,bhtd->bjhd", torch.softmax(s, dim=-1), vc.float()) * real[:, :, None, None]
+        return o.to(qkv.dtype).reshape(B * S, H * Dh)
+
+
 class _Repeats:
     """The repetition controls of a batched decoder over the R rows of its cache: ``seq`` int32 [R, t_max] each row's
     sequence (its prompt, then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the penalty and the
@@ -261,7 +292,7 @@ class Block(nn.Module):
         return self.c_proj2(F.gelu(self.c_fc(h), approximate="tanh"))
 
     def _attn(self, h: torch.Tensor, cache: Optional["KVCache"] = None, layer: int = 0) -> torch.Tensor:
-        if isinstance(cache, CandidateKV):           # contrastive search: k candidate tokens per cache row
+        if isinstance(cache, (CandidateKV, VerifyKV)):   # contrastive search / prompt lookup: k + 1 slots per row
             return self.c_proj(cache.attend(self.c_attn(h), layer))
         if cache is not None and h.dim() == 2:       # decode: one new token per row [B, D] against the cache
             return self.c_proj(decode_attention(self.c_attn(h), cache.k[layer], cache.v[layer], cache.lens, cache.work))
@@ -494,11 +525,13 @@ class GPT2DoubleHeads(nn.Module):
 
     def _decode_setup(self, who: str, input_ids: torch.Tensor, lengths: Optional[Sequence[int]],
                       token_type_ids: Optional[torch.Tensor], reply_type, max_new_tokens: int, min_new_tokens: int,
-                      repetition_penalty: float, no_repeat_ngram_size: int, num_beams: int = 1):
+                      repetition_penalty: float, no_repeat_ngram_size: int, num_beams: int = 1,
+                      rows_name: str = "beam rows (batch x num_beams)"):
         """The checks and prompt quantities the batched decoders share, before anything is launched:
         ``(B, T, lengths, n, t_max, last, tt_new, native)``. ``last`` [B] is each prompt's last position, ``tt_new`` [B]
         the token type of new tokens (None without token types), and ``native`` says whether the bf16 CUDA kernels
-        run; they take at most ``LM_HEAD_MAX_ROWS`` rows, ``num_beams`` per prompt. Errors name ``who``."""
+        run; they take at most ``LM_HEAD_MAX_ROWS`` rows, ``num_beams`` per prompt (called ``rows_name`` in the error
+        when more than one). Errors name ``who``."""
         from ..ops import LM_HEAD_MAX_ROWS
 
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
@@ -520,7 +553,7 @@ class GPT2DoubleHeads(nn.Module):
         weight = self.wte.weight
         native = weight.is_cuda and weight.dtype == torch.bfloat16
         if native and B * num_beams > LM_HEAD_MAX_ROWS:
-            what, got = ("rows", B) if num_beams == 1 else ("beam rows (batch x num_beams)", f"{B} x {num_beams}")
+            what, got = ("rows", B) if num_beams == 1 else (rows_name, f"{B} x {num_beams}")
             raise ValueError(f"{who}: at most {LM_HEAD_MAX_ROWS} {what} per call on the native path, got {got}")
         last = torch.tensor(lengths, device=dev) - 1
         tt_new = None
@@ -535,7 +568,8 @@ class GPT2DoubleHeads(nn.Module):
                  token_type_ids: Optional[torch.Tensor] = None, reply_type=None, max_new_tokens: int = 20,
                  temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9, stop_ids: Sequence[int] = (),
                  suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, seed=0, repetition_penalty: float = 1.0,
-                 no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+                 no_repeat_ngram_size: int = 0, prompt_lookup_num_tokens: int = 0,
+                 max_matching_ngram_size: int = 2) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -555,10 +589,27 @@ class GPT2DoubleHeads(nn.Module):
         every token after the first replays one CUDA graph of decode step, LM head (``ops.penalize_repeats_`` when a
         repetition control is on) and sampler, which feeds the drawn ids back into its own input; the host reads the
         done flags once every 8 tokens, a step late, to stop early. Elsewhere the same loop runs eagerly with fp32
-        PyTorch logits, ``ops.repeats.penalize_repeats_reference`` and ``ops.sampling.sample_reference``."""
+        PyTorch logits, ``ops.repeats.penalize_repeats_reference`` and ``ops.sampling.sample_reference``.
+
+        ``prompt_lookup_num_tokens`` = k > 0 (HuggingFace's prompt lookup decoding; greedy only, without the repetition
+        controls) verifies up to k draft tokens per row and step, copied from the row's own prompt and reply after the
+        earliest earlier occurrence of its last ``max_matching_ngram_size`` (or fewer) tokens; the result is the greedy
+        tokens. The definition is in ``ops/lookup.py``. On the native path (``B·(k+1)`` at most 64 rows) every verify
+        step replays one CUDA graph: the model on k + 1 slots per row (``ops.verify_attention_``), the LM head,
+        acceptance (``ops.lookup_accept_``) and the next drafts (``ops.lookup_draft_``); the host polls the done flags
+        every ``LOOKUP_POLL_PERIOD`` replays. Afterwards ``self.lookup_stats`` holds the rows' emitted tokens (a stop id
+        included) and verify steps, int32 [B], and the graph replays issued."""
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
+        K = prompt_lookup_num_tokens
+        if K != 0:
+            from ..ops import LOOKUP_MAX_NGRAM, LOOKUP_MAX_TOKENS
+            from ..ops.lookup import check_lookup_args
+            check_lookup_args("generate", K, max_matching_ngram_size, LOOKUP_MAX_TOKENS, LOOKUP_MAX_NGRAM, temperature,
+                              repetition_penalty, no_repeat_ngram_size)
+            return self._generate_lookup(input_ids, lengths, token_type_ids, reply_type, max_new_tokens, stop_ids,
+                                         suppress_ids, min_new_tokens, int(K), int(max_matching_ngram_size))
         B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size)
@@ -709,6 +760,76 @@ class GPT2DoubleHeads(nn.Module):
         hist_tok = st.hist_tok.view(n, B, K).cpu().numpy()
         hist_back = st.hist_back.view(n, B, K).cpu().numpy()
         return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n))
+
+    def _generate_lookup(self, input_ids, lengths, token_type_ids, reply_type, max_new_tokens, stop_ids, suppress_ids,
+                         min_new_tokens, K: int, ngram: int) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``generate`` at temperature 0 with prompt lookup of up to ``K`` drafts (``ops/lookup.py``)."""
+        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+            "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens, 1.0, 0,
+            num_beams=K + 1, rows_name="verify rows (batch x (prompt_lookup_num_tokens + 1))")
+        cfg, dev, weight, V, S = self.cfg, input_ids.device, self.wte.weight, self.cfg.vocab_size, K + 1
+        tt_v = tt_new.repeat_interleave(S) if tt_new is not None else None
+        cache = self.new_cache(B, t_max)
+        h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
+        # the prompt's last token plays the row's last emitted token x_b, whose logits the prefill gave: lens = len - 1
+        cache.lens.sub_(1)
+        if not native:                              # CPU / not bf16: the definition on fp32 PyTorch logits
+            from ..ops.lookup import lookup_accept, lookup_draft
+            head = weight.float()
+            seq = torch.zeros(B, t_max, dtype=torch.int32)
+            seq[:, :T] = input_ids.cpu()
+            lens = cache.lens.cpu()
+            emitted, done, steps = (torch.zeros(B, dtype=torch.int32) for _ in range(3))
+            tokens = torch.full((B, n), -1, dtype=torch.int64)
+            ids, nq = torch.zeros(B * S, dtype=torch.int64), torch.ones(B, dtype=torch.int32)
+            lookup_accept(self.lm_logits(h, head), V, ids, nq, seq, lens, emitted, done, tokens, None, min_new_tokens,
+                          suppress_ids, stop_ids)
+            while not bool(done.all()):             # every live row emits at least one token per step
+                ids, pos, nq = lookup_draft(seq, lens, emitted, done, K, n, ngram)
+                cache.lens.copy_(lens)
+                hv = self._verify_hidden(ids.to(dev), pos.to(dev), tt_v, VerifyKV(cache, S, nq.to(dev)))
+                lookup_accept(self.lm_logits(hv, head), V, ids, nq, seq, lens, emitted, done, tokens, steps,
+                              min_new_tokens, suppress_ids, stop_ids)
+            self.lookup_stats = {"emitted": emitted, "steps": steps, "replays": int(steps.max())}
+            return tokens.to(dev), (tokens >= 0).sum(1).to(dev)
+
+        from ..ops import LookupState, decode_attention_work_numel, lm_head_logits_, lookup_accept_, lookup_draft_
+
+        st = LookupState(B, K, n, t_max, ngram, dev)
+        st.seq[:, :T] = input_ids
+        logits = torch.empty(B * S, weight.shape[0], dtype=torch.float32, device=dev)
+        sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
+        lm_head_logits_(h, weight, logits[:B])      # the first token, from the prefill's last positions
+        lookup_accept_(logits[:B], V, st, cache.lens, min_new_tokens, sup, stop, count=False)
+        lookup_draft_(st, cache.lens)
+        replays = 0
+        if n > 1:
+            H = cfg.n_head
+            work = torch.empty(decode_attention_work_numel(B * S, H, cfg.n_embd // H, t_max), dtype=torch.float32,
+                               device=dev)
+            verify = VerifyKV(cache, S, st.nq, work)
+
+            def accept_and_draft(hv):
+                lm_head_logits_(hv, weight, logits)
+                lookup_accept_(logits, V, st, cache.lens, min_new_tokens, sup, stop)
+                lookup_draft_(st, cache.lens)
+
+            # lookup_draft_ writes the next slots into the graph's own input buffers; lookup_accept_ advances the
+            # cache by the tokens it emits, up to k + 1 per replay, while the host counts one per replay. A live row
+            # emits at least one token per replay, so at most n - 1 replays follow the first token and the host's
+            # lengths stay at most max(lengths) + n - 1 < t_max: check_room never fires.
+            graph = DecodeGraph(self, cache, tt_v is not None, head=accept_and_draft, ids=st.ids, tt=tt_v,
+                                step=lambda ids, tt, c: self._verify_hidden(ids, st.pos, tt, verify))
+            replays = graph.run(n - 1, st.done, period=LOOKUP_POLL_PERIOD)
+        self.lookup_stats = {"emitted": st.emitted, "steps": st.steps, "replays": replays}
+        return st.tokens, (st.tokens >= 0).sum(1)
+
+    def _verify_hidden(self, ids: torch.Tensor, pos: torch.Tensor, tt: Optional[torch.Tensor],
+                       verify: "VerifyKV") -> torch.Tensor:
+        """The final hidden states [B·(k+1), D] of the verify slots ``ids`` at positions ``pos`` (int64 [B·(k+1)]): the
+        blocks of ``decode_step`` with attention through ``verify``. The real slots' keys and values go into the cache;
+        its lengths do not move."""
+        return self._blocks(self._embed(ids, tt, pos), verify)
 
     def _candidate_hidden(self, ids: torch.Tensor, tt: Optional[torch.Tensor], cand: "CandidateKV") -> torch.Tensor:
         """The final hidden states [B·k, D] of ``cand.top_k`` candidate tokens ``ids`` [B·k] per cache row, each at its
@@ -865,6 +986,11 @@ class GPT2DoubleHeads(nn.Module):
         return loss, lm_loss, mc_loss
 
 
+# DecodeGraph.run's poll period for prompt-lookup generation, where one replay can emit up to k + 1 tokens per row:
+# on GPT-2 small (8 rows, 64 new tokens, H100) it left 2-3 replays after the last row finished, against 9-10 at 8
+LOOKUP_POLL_PERIOD = 2
+
+
 class DecodeGraph:
     """``model.decode_step`` for one cache captured in a CUDA graph and replayed (the pattern of
     ``FlatDataParallel.capture``): the token ids (and token types) go through static input buffers, the cache's device
@@ -916,22 +1042,23 @@ class DecodeGraph:
         self.cache.advance_host()
         return self.h
 
-    def run(self, replays: int, done: torch.Tensor) -> None:
-        """``replays`` replays, stopping early once every flag of ``done`` (int32, on the device) is set. Every 8
-        replays before the last the flags are copied to a pinned buffer, and the host reads that copy 8 replays later,
-        when it is long finished, so the host never waits for the device."""
+    def run(self, replays: int, done: torch.Tensor, period: int = 8) -> int:
+        """``replays`` replays, stopping early once every flag of ``done`` (int32, on the device) is set; returns the
+        replays issued. Every ``period`` replays before the last the flags are copied to a pinned buffer, and the host
+        reads that copy ``period`` replays later, when it is long finished, so the host never waits for the device."""
         flags = torch.empty(done.numel(), dtype=done.dtype, pin_memory=True)
         copied = None
         for i in range(1, replays + 1):
             self.replay()
-            if i % 8 == 0 and i < replays:
+            if i % period == 0 and i < replays:
                 if copied is not None:
                     copied.synchronize()
                     if bool(flags.all()):
-                        break
+                        return i
                 flags.copy_(done, non_blocking=True)
                 copied = torch.cuda.Event()
                 copied.record()
+        return replays
 
 
 class CachedDecoder:

@@ -63,6 +63,10 @@ def _lib():
                                          + [c_void_p] * 5 + [c_int] * 3 + [c_void_p])
         lib.adapcc_cs_context_init.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                                c_void_p]
+        lib.adapcc_verify_attn.argtypes = [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]
+        lib.adapcc_lookup_accept.argtypes = ([c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_int]
+                                             + [c_void_p] * 4 + [c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p])
+        lib.adapcc_lookup_draft.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 7
         _bound = True
     return lib
 
@@ -727,3 +731,142 @@ def contrastive_context_init_(h: torch.Tensor, lens: torch.Tensor, state: Contra
     _same_device("contrastive_context_init_", h.device, [lens, state.ctx, state.ctx_norm])
     _ck(_lib().adapcc_cs_context_init(_ptr(h), B, h.shape[1], D, _ptr(lens), _ptr(state.ctx), _ptr(state.ctx_norm),
                                       state.t_max, _stream()), "cs_context_init")
+
+
+# ---- prompt-lookup speculative decoding: verify attention, acceptance, drafts (csrc/ops_lookup.cu) -----------------
+LOOKUP_MAX_TOKENS = 15         # drafts per row: k + 1 <= 16 slots, each CTA of the verify attention runs them in turn
+LOOKUP_MAX_NGRAM = 16          # max_matching_ngram_size
+LOOKUP_MAX_IDS = 1024          # ids per suppress / stop list
+
+
+def verify_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
+                      nq: torch.Tensor, k: int, out: torch.Tensor, work: torch.Tensor) -> torch.Tensor:
+    """Decode attention of ``k + 1`` slots per cache row. ``qkv`` bf16 [B·(k+1), 3·H·Dh] (q | k | v of slot j of row b
+    in row ``b·(k+1) + j``; unit column stride), ``k_cache`` / ``v_cache`` bf16 [B, H, t_max, Dh], ``lens`` and ``nq``
+    int32 [B] (read only). Row b's first ``nq[b]`` slots are real (at most k + 1 and the positions left in the cache);
+    slot j sits at position ``lens[b] + j`` and attends over the cached keys ``0..lens[b]-1`` plus the new keys of the
+    row's slots ``0..j``, read from ``qkv``. ``out[b·(k+1) + j]`` (bf16 [B·(k+1), H·Dh]) is bit-identical to
+    ``decode_attention_`` with ``lens = lens[b] + j`` on a cache that already holds slots ``0..j-1``; a pad slot's
+    output is zero. The real slots' keys and values are stored at ``lens[b] + j``; nothing else is written, and each
+    cached element is read once per CTA for all of a row's slots. ``work``: fp32, ``decode_attention_work_numel(B·(k+1),
+    ...)`` elements. The grid depends on t_max, B and k only; no host sync."""
+    def bad(msg):
+        raise ValueError(f"verify_attention_: {msg}")
+
+    for name, t in (("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)):
+        if t.dtype != torch.bfloat16:
+            bad(f"{name} must be bf16, got {t.dtype}")
+    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
+        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
+            f"and {tuple(v_cache.shape)}")
+    B, H, t_max, Dh = k_cache.shape
+    if not 0 <= int(k) <= LOOKUP_MAX_TOKENS:
+        bad(f"k must be in [0, {LOOKUP_MAX_TOKENS}], got {k}")
+    S = int(k) + 1
+    if qkv.dim() != 2 or qkv.shape != (B * S, 3 * H * Dh) or qkv.stride(1) != 1:
+        bad(f"qkv must be [{B * S}, {3 * H * Dh}] with unit column stride, got {tuple(qkv.shape)} stride {qkv.stride()}")
+    if out.shape != (B * S, H * Dh) or not out.is_contiguous():
+        bad(f"out must be a contiguous [{B * S}, {H * Dh}] tensor, got {tuple(out.shape)}")
+    for name, t in (("lens", lens), ("nq", nq)):
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != B:
+            bad(f"{name} must be a contiguous int32 tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if work.dtype != torch.float32 or not work.is_contiguous():
+        bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
+    _same_device("verify_attention_", k_cache.device, (qkv, v_cache, lens, nq, out, work))
+    need = decode_attention_work_numel(B * S, H, Dh, t_max)
+    if work.numel() < need:
+        bad(f"work holds {work.numel()} elements, {need} needed")
+    _ck(_lib().adapcc_verify_attn(_ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(lens), _ptr(nq), _ptr(out), B, S, H,
+                                  Dh, t_max, qkv.stride(0), _ptr(work), _stream()), "verify_attn")
+    return out
+
+
+class LookupState:
+    """Device state of a batched prompt-lookup generation of ``batch`` rows with up to ``k`` drafts each, up to
+    ``max_new`` tokens, a cache of ``t_max`` positions and n-grams of up to ``ngram`` tokens, as ``lookup_accept_`` and
+    ``lookup_draft_`` read and write it. Slot j of row b is row ``b·(k+1) + j``.
+
+    ``ids`` int64 [B·(k+1)] the verify step's input (slot 0 the row's last token, then its drafts, 0 in a pad slot),
+    ``pos`` int64 [B·(k+1)] their positions, ``nq`` int32 [B] the real slots (1 at the start: the prefill's logits);
+    ``seq`` int32 [B, t_max] each row's sequence (the caller stores the prompts); ``emitted`` int32 [B] the tokens
+    emitted (a stop id included); ``done`` int32 [B]; ``tokens`` int64 [B, max_new] the output (-1 where nothing was
+    emitted); ``steps`` int32 [B] verify steps per live row; ``g`` int32 [B·(k+1)] the slots' arg-maxes."""
+
+    def __init__(self, batch: int, k: int, max_new: int, t_max: int, ngram: int, device):
+        B, K, n = int(batch), int(k), int(max_new)
+        if (B < 1 or not 1 <= K <= LOOKUP_MAX_TOKENS or n < 1 or int(t_max) < 1
+                or not 1 <= int(ngram) <= LOOKUP_MAX_NGRAM):
+            raise ValueError(f"LookupState: need batch >= 1, 1 <= k <= {LOOKUP_MAX_TOKENS}, max_new >= 1, t_max >= 1 "
+                             f"and 1 <= ngram <= {LOOKUP_MAX_NGRAM}, got {batch}, {k}, {max_new}, {t_max}, {ngram}")
+        self.batch, self.k, self.max_new, self.t_max, self.ngram = B, K, n, int(t_max), int(ngram)
+        S = K + 1
+        i32, i64 = dict(dtype=torch.int32, device=device), dict(dtype=torch.int64, device=device)
+        self.ids = torch.zeros(B * S, **i64)
+        self.pos = torch.zeros(B * S, **i64)
+        self.nq = torch.ones(B, **i32)
+        self.seq = torch.zeros(B, self.t_max, **i32)
+        self.emitted = torch.zeros(B, **i32)
+        self.done = torch.zeros(B, **i32)
+        self.tokens = torch.full((B, n), -1, **i64)
+        self.steps = torch.zeros(B, **i32)
+        self.g = torch.zeros(B * S, **i32)
+
+    def tensors(self):
+        """Every device tensor of the state (what the ops check for one device)."""
+        return (self.ids, self.pos, self.nq, self.seq, self.emitted, self.done, self.tokens, self.steps, self.g)
+
+
+def lookup_accept_(logits: torch.Tensor, vocab: int, state: LookupState, lens: torch.Tensor, min_new: int = 0,
+                   suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None,
+                   count: bool = True) -> None:
+    """Acceptance of every row, on the device (the definition in ``ops/lookup.py``). ``logits`` fp32 [B·ls, ld] (the
+    first ``vocab`` columns used) holds ``ls`` slots per row: k + 1 after a verify step, 1 for the prefill's logits
+    (with ``state.nq`` all 1 and ``lens`` one less than the prompt lengths). Each real slot's arg-max (ties to the
+    lower id; ``suppress_ids`` removed while ``emitted + j < min_new``) is emitted while the next slot's draft in
+    ``state.ids`` equals it; a stop id (not written) or ``state.max_new`` tokens end the row. Updates ``state.tokens``,
+    ``seq``, ``emitted``, ``done`` and, with ``count``, ``steps``, and advances ``lens`` (int32 [B]) by the number
+    emitted. No host sync."""
+    def bad(msg):
+        raise ValueError(f"lookup_accept_: {msg}")
+
+    if not isinstance(state, LookupState):
+        bad(f"state must be a LookupState, got {type(state).__name__}")
+    B, S = state.batch, state.k + 1
+    if (logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1
+            or logits.shape[0] not in (B, B * S)):
+        bad(f"logits must be fp32 [{B}, ld] or [{B * S}, ld] with unit column stride, got {logits.dtype} "
+            f"{tuple(logits.shape)}")
+    if not 1 <= vocab <= logits.shape[1]:
+        bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
+    if int(min_new) < 0:
+        bad(f"min_new must be >= 0, got {min_new}")
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
+        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    sup, n_sup = _id_list("lookup_accept_", "suppress_ids", suppress_ids, LOOKUP_MAX_IDS)
+    stop, n_stop = _id_list("lookup_accept_", "stop_ids", stop_ids, LOOKUP_MAX_IDS)
+    _same_device("lookup_accept_", logits.device, state.tensors() + (lens, suppress_ids, stop_ids))
+    _ck(_lib().adapcc_lookup_accept(_ptr(logits), logits.stride(0), int(vocab), B, S, logits.shape[0] // B,
+                                    int(min_new), sup, n_sup, stop, n_stop, _ptr(state.g), _ptr(state.ids),
+                                    _ptr(state.nq), _ptr(state.seq), state.t_max, _ptr(lens), _ptr(state.emitted),
+                                    _ptr(state.done), _ptr(state.tokens), state.max_new,
+                                    _ptr(state.steps if count else None), _stream()), "lookup_accept")
+
+
+def lookup_draft_(state: LookupState, lens: torch.Tensor) -> None:
+    """The next verify step's input for every row, on the device (the definition in ``ops/lookup.py``): a live row's
+    drafts are the tokens after the earliest earlier occurrence of its sequence's last m tokens (m from
+    ``state.ngram`` down to 1), at most ``min(k, max_new - emitted - 1)``. Writes ``state.ids`` (slot 0 the last token
+    ``seq[b, lens[b]]``, then the drafts, 0 in a pad slot), ``state.pos`` (``lens[b] + j`` clamped to ``t_max - 1``)
+    and ``state.nq`` (1 + drafts; 0 for a done row). No host sync."""
+    def bad(msg):
+        raise ValueError(f"lookup_draft_: {msg}")
+
+    if not isinstance(state, LookupState):
+        bad(f"state must be a LookupState, got {type(state).__name__}")
+    B = state.batch
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
+        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    _same_device("lookup_draft_", lens.device, state.tensors())
+    _ck(_lib().adapcc_lookup_draft(_ptr(state.seq), state.t_max, B, state.k + 1, state.ngram, state.max_new,
+                                   _ptr(lens), _ptr(state.emitted), _ptr(state.done), _ptr(state.ids), _ptr(state.pos),
+                                   _ptr(state.nq), _stream()), "lookup_draft")

@@ -45,6 +45,9 @@ def main():
     p.add_argument("--penalty_alpha", type=float, default=0.0,
                    help="f1: > 0 decodes the replies with GPT2DoubleHeads.contrastive_search, this degeneration penalty "
                         "and --top_k candidates (0: sample); replies go through the batched path")
+    p.add_argument("--prompt_lookup_num_tokens", type=int, default=0,
+                   help="f1 with --no_sample: verify up to this many draft tokens per step, copied from the prompt and "
+                        "the reply (prompt lookup decoding; 0: off); the replies are the greedy ones")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -56,7 +59,8 @@ def main():
     if a.eval_type == "f1":
         kw = dict(max_length=a.max_length, min_length=a.min_length, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p,
                   no_sample=a.no_sample, repetition_penalty=a.repetition_penalty,
-                  no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha)
+                  no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha,
+                  prompt_lookup_num_tokens=a.prompt_lookup_num_tokens)
     res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
                            a.batch_size, a.num_beams, **kw)
     print(json.dumps(res))
