@@ -1,15 +1,8 @@
 // Contrastive search for GPT-2 generation (Su et al., "A Contrastive Framework for Neural Text Generation") on the
 // device, so a token is one CUDA graph replay: candidate decode step, re-rank and commit, LM head, repetition controls,
-// candidate selection. The definition is in ops/contrastive.py and DESIGN.md §4a.
+// candidate selection. The definition is in ops/contrastive.py and DESIGN.md §4a. The candidates' attention is
+// adapcc_cand_attn in ops_decode.cu; this file selects the candidates, re-ranks them and commits the winner.
 //
-//   cand_attn     : decode attention of k candidate tokens per cache row. Candidate (b, j) attends over the row's cached
-//                   keys 0..lens[b]-1 plus its own new key at position lens[b], taken from its c_attn output. Grid
-//                   (splits of t_max, H, B) as in decode_attn_split_kernel (ops_decode.cu): each CTA stages its split's
-//                   cached K / V tile in shared memory once and runs the k queries over it one after the other, each
-//                   with the thread layout, split size and summation order of the decode kernel, so a candidate's
-//                   output is bit-identical to decode_attention_ on a row that holds that token. The cache is only
-//                   read; each candidate's new k / v go to a side buffer for the commit.
-//   cand_combine  : the decode kernel's combine, with row b * k + j reading lens[b].
 //   cs_select     : one 512-thread CTA per row: the k largest logits (topk_rows.cuh, ranked by the logit itself, ties
 //                   to the lower id), each with p = expf(l - m) / Z over the remaining ids; suppress_ids are removed
 //                   while step < min_new. Writes the ids into the candidate step's input buffer.
@@ -33,162 +26,12 @@
 
 namespace adapcc {
 
-constexpr int kCsSplit = 64;                        // = kDecodeSplit (ops_decode.cu): the same splits, the same bits
-constexpr int kCsAttnThreads = 128;                 // = kDecodeThreads
-constexpr int kCsMaxDh = 128;                       // = kDecodeMaxDh
 constexpr int kCsMaxK = 16;                         // candidates per row
 constexpr int kCsMaxD = 1024;                       // hidden size (four 16-byte vectors per lane)
 constexpr int kCsSimPos = 64;                       // context positions per cs_sim CTA
 constexpr int kCsSimThreads = 256;
 constexpr int kCsMaxSuppress = 1024;
 constexpr int kCsMaxStop = 1024;
-
-struct CandAttnArgs {
-  const __nv_bfloat16* qkv;   // [B * k, qkv_stride]: q | k | v of each candidate, H * Dh each
-  const __nv_bfloat16* k_cache;  // [B, H, t_max, Dh], read only
-  const __nv_bfloat16* v_cache;
-  const int* lens;            // [B]
-  float* work;                // [B * k, H, n_splits, Dh + 2]
-  __nv_bfloat16* out;         // [B * k, H * Dh]
-  __nv_bfloat16* side_k;      // [B * k, H * Dh]: each candidate's new key
-  __nv_bfloat16* side_v;
-  int kq, H, Dh, t_max, qkv_stride, n_splits;
-};
-
-template <int S>
-__global__ void __launch_bounds__(kCsAttnThreads) cand_attn_split_kernel(const __grid_constant__ CandAttnArgs a) {
-  __shared__ __align__(16) __nv_bfloat16 s_k[S * kCsMaxDh];   // the split's cached keys and values, shared by the k
-  __shared__ __align__(16) __nv_bfloat16 s_v[S * kCsMaxDh];   // queries
-  __shared__ float s_p[S];
-  __shared__ float s_acc[kCsAttnThreads * 8];
-  __shared__ float s_red[kCsAttnThreads / 32];
-  const int s = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int L = a.lens[b];
-  if (L < 0 || L >= a.t_max) return;
-  const int j0 = s * S;
-  if (j0 > L) return;
-  const int n = min(S, L + 1 - j0);                 // keys of this split: j0 .. j0 + n - 1 (key L is the candidate's)
-  const int np = min(S, L - j0);                    // of them cached
-  const int Dh = a.Dh, nvec = Dh >> 3, D = a.H * Dh;
-  int G = 1;
-  while (G < nvec) G <<= 1;
-  const int tid = threadIdx.x, c = tid & (G - 1), grp = tid / G, ngrp = kCsAttnThreads / G;
-  const bool act = c < nvec;
-  const long long head = ((long long)b * a.H + h) * a.t_max * Dh;
-  for (int e = tid; e < np * nvec; e += kCsAttnThreads) {
-    const int jj = e / nvec, cc = e - jj * nvec;
-    const long long g = head + (long long)(j0 + jj) * Dh + cc * 8;
-    *reinterpret_cast<uint4*>(s_k + jj * Dh + cc * 8) = *reinterpret_cast<const uint4*>(a.k_cache + g);
-    *reinterpret_cast<uint4*>(s_v + jj * Dh + cc * 8) = *reinterpret_cast<const uint4*>(a.v_cache + g);
-  }
-  __syncthreads();
-  const float scale = 1.0f / sqrtf((float)Dh);
-  const int lane = tid & 31, warp = tid >> 5;
-  for (int qi = 0; qi < a.kq; ++qi) {
-    const long long bq = (long long)b * a.kq + qi;
-    const __nv_bfloat16* qrow = a.qkv + bq * a.qkv_stride + h * Dh;
-    float q[8];
-    if (act) unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(qrow + c * 8), q);
-    // 1. scores (decode_attn_split_kernel's layout and order)
-#pragma unroll 4
-    for (int base = 0; base < n; base += ngrp) {
-      const int jj = base + grp, j = j0 + jj;
-      float d = 0.f;
-      if (act && jj < n) {
-        float k[8];
-        unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(j == L ? qrow + D + c * 8 : s_k + jj * Dh + c * 8), k);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) d = fmaf(q[e], k[e], d);
-      }
-      for (int o = G >> 1; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-      if (c == 0 && jj < n) s_p[jj] = d * scale;
-    }
-    __syncthreads();
-    // 2. max and sum of exp over the split
-    float m = -INFINITY;
-    for (int jj = tid; jj < n; jj += kCsAttnThreads) m = fmaxf(m, s_p[jj]);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
-    if (lane == 0) s_red[warp] = m;
-    __syncthreads();
-    m = s_red[0];
-#pragma unroll
-    for (int w = 1; w < kCsAttnThreads / 32; ++w) m = fmaxf(m, s_red[w]);
-    __syncthreads();
-    float l = 0.f;
-    for (int jj = tid; jj < n; jj += kCsAttnThreads) {
-      const float p = expf(s_p[jj] - m);
-      s_p[jj] = p;
-      l += p;
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) l += __shfl_xor_sync(0xffffffffu, l, o);
-    if (lane == 0) s_red[warp] = l;
-    __syncthreads();
-    // 3. P.V
-    float acc[8];
-#pragma unroll
-    for (int e = 0; e < 8; ++e) acc[e] = 0.f;
-    if (act) {
-#pragma unroll 4
-      for (int jj = grp; jj < n; jj += ngrp) {
-        const int j = j0 + jj;
-        float v[8];
-        unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(j == L ? qrow + 2 * D + c * 8 : s_v + jj * Dh + c * 8), v);
-        const float p = s_p[jj];
-#pragma unroll
-        for (int e = 0; e < 8; ++e) acc[e] = fmaf(p, v[e], acc[e]);
-      }
-    }
-#pragma unroll
-    for (int e = 0; e < 8; ++e) s_acc[grp * (G * 8) + c * 8 + e] = acc[e];
-    __syncthreads();
-    float* w = a.work + ((bq * a.H + h) * a.n_splits + s) * (Dh + 2);
-    if (tid < Dh) {
-      float r = 0.f;
-      for (int g = 0; g < ngrp; ++g) r += s_acc[g * (G * 8) + tid];
-      w[2 + tid] = r;
-    }
-    if (L < j0 + S && tid < nvec) {                 // the candidate's new k / v go to the side buffer, not the cache
-      const long long o = bq * D + h * Dh + tid * 8;
-      *reinterpret_cast<uint4*>(a.side_k + o) = *reinterpret_cast<const uint4*>(qrow + D + tid * 8);
-      *reinterpret_cast<uint4*>(a.side_v + o) = *reinterpret_cast<const uint4*>(qrow + 2 * D + tid * 8);
-    }
-    if (tid == 0) {
-      float sum = 0.f;
-#pragma unroll
-      for (int i = 0; i < kCsAttnThreads / 32; ++i) sum += s_red[i];
-      w[0] = m;
-      w[1] = sum;
-    }
-    __syncthreads();                                // s_p, s_red and s_acc are reused by the next query
-  }
-}
-
-// one CTA per (h, candidate row): decode_attn_combine_kernel with the cache row's lens
-template <int S>
-__global__ void __launch_bounds__(kCsMaxDh) cand_attn_combine_kernel(const __grid_constant__ CandAttnArgs a) {
-  const int h = blockIdx.x, bq = blockIdx.y, t = threadIdx.x, Dh = a.Dh;
-  if (t >= Dh) return;
-  __nv_bfloat16* o = a.out + (long long)bq * a.H * Dh + h * Dh;
-  const int L = a.lens[bq / a.kq];
-  if (L < 0 || L >= a.t_max) {
-    o[t] = __float2bfloat16_rn(0.f);
-    return;
-  }
-  const int ns = L / S + 1;
-  const float* w = a.work + ((long long)bq * a.H + h) * a.n_splits * (Dh + 2);
-  float M = -INFINITY;
-  for (int s = 0; s < ns; ++s) M = fmaxf(M, w[s * (Dh + 2)]);
-  float l = 0.f, acc = 0.f;
-  for (int s = 0; s < ns; ++s) {
-    const float* ws = w + s * (Dh + 2);
-    const float f = expf(ws[0] - M);
-    l = fmaf(ws[1], f, l);
-    acc = fmaf(ws[2 + t], f, acc);
-  }
-  o[t] = __float2bfloat16_rn(acc / l);
-}
 
 // ---- candidate selection -----------------------------------------------------------------------------------------
 struct SelectArgs {
@@ -452,7 +295,6 @@ __global__ void __launch_bounds__(32) cs_context_init_kernel(const __nv_bfloat16
   if (lane == 0) ctx_norm[(long long)b * t_max + p] = nrm;
 }
 
-inline int cs_splits(int t_max) { return (t_max + kCsSplit - 1) / kCsSplit; }
 inline int cs_chunks(int t_max) { return (t_max + kCsSimPos - 1) / kCsSimPos; }
 
 }  // namespace adapcc
@@ -465,58 +307,6 @@ extern "C" {
 long long adapcc_cs_sim_numel(int B, int kq, int t_max) {
   if (B < 1 || kq < 1 || t_max < 1) return 0;
   return (long long)B * cs_chunks(t_max) * kq;
-}
-
-// qkv: bf16 [B * kq, qkv_stride]; k_cache / v_cache: bf16 [B, H, t_max, Dh] (read only); lens: int32 [B]; out: bf16
-// [B * kq, H * Dh]; side_k / side_v: bf16 [B * kq, H * Dh]; work: fp32, adapcc_decode_attn_work(B * kq, ...) elements
-int adapcc_cand_attn(const void* qkv, const void* k_cache, const void* v_cache, const int* lens, void* out,
-                     void* side_k, void* side_v, int B, int kq, int H, int Dh, int t_max, int qkv_stride, void* work,
-                     void* stream) {
-  if (B < 1 || H < 1 || kq < 1 || kq > kCsMaxK || B > 65535 || H > 65535 || (long long)B * kq > 65535 || t_max < 1) {
-    set_error("cand_attn: need 1 <= B, H, B * kq <= 65535, 1 <= kq <= %d and t_max >= 1 (B=%d kq=%d H=%d t_max=%d)",
-              kCsMaxK, B, kq, H, t_max);
-    return -1;
-  }
-  if (Dh < 8 || Dh > kCsMaxDh || Dh % 8 != 0) {
-    set_error("cand_attn: head dim must be a multiple of 8 in [8, %d], got %d", kCsMaxDh, Dh);
-    return -1;
-  }
-  if (qkv_stride < 3 * H * Dh || qkv_stride % 8 != 0) {
-    set_error("cand_attn: qkv row stride %d must be a multiple of 8 and >= 3 * H * Dh = %d", qkv_stride, 3 * H * Dh);
-    return -1;
-  }
-  if (((uintptr_t)qkv | (uintptr_t)k_cache | (uintptr_t)v_cache | (uintptr_t)out | (uintptr_t)side_k |
-       (uintptr_t)side_v) & 15) {
-    set_error("cand_attn: qkv, caches, output and side buffers must be 16-byte aligned");
-    return -1;
-  }
-  if (!lens || !work || ((uintptr_t)lens | (uintptr_t)work) & 3) {
-    set_error("cand_attn: lens and work must be non-null and 4-byte aligned");
-    return -1;
-  }
-  CandAttnArgs a{};
-  a.qkv = (const __nv_bfloat16*)qkv;
-  a.k_cache = (const __nv_bfloat16*)k_cache;
-  a.v_cache = (const __nv_bfloat16*)v_cache;
-  a.lens = lens;
-  a.work = (float*)work;
-  a.out = (__nv_bfloat16*)out;
-  a.side_k = (__nv_bfloat16*)side_k;
-  a.side_v = (__nv_bfloat16*)side_v;
-  a.kq = kq;
-  a.H = H;
-  a.Dh = Dh;
-  a.t_max = t_max;
-  a.qkv_stride = qkv_stride;
-  a.n_splits = cs_splits(t_max);
-  cudaStream_t s = (cudaStream_t)stream;
-  cand_attn_split_kernel<kCsSplit><<<dim3(a.n_splits, H, B), kCsAttnThreads, 0, s>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  cand_attn_combine_kernel<kCsSplit><<<dim3(H, B * kq), kCsMaxDh, 0, s>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  return 0;
 }
 
 // logits fp32 [B, ld]; step int32 [1]; suppress int32 list (null when empty); done int32 [B]; next_ids int64, cand_tok

@@ -285,6 +285,38 @@ def decode_attention_work_numel(batch: int, n_head: int, head_dim: int, t_max: i
     return int(_lib().adapcc_decode_attn_work(batch, n_head, head_dim, t_max))
 
 
+def _check_decode_attn(who: str, kq: int, qkv, k_cache, v_cache, lens, out, work, nq=None, side_k=None, side_v=None):
+    """``ValueError`` (prefixed ``who``) unless the tensors fit a decode-style attention of ``kq`` queries per cache row
+    (``csrc/ops_decode.cu``); returns the cache shape (B, H, t_max, Dh)."""
+    def bad(msg):
+        raise ValueError(f"{who}: {msg}")
+
+    rows = [(name, t) for name, t in (("out", out), ("side_k", side_k), ("side_v", side_v)) if t is not None]
+    for name, t in [("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache)] + rows:
+        if t.dtype != torch.bfloat16:
+            bad(f"{name} must be bf16, got {t.dtype}")
+    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
+        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
+            f"and {tuple(v_cache.shape)}")
+    B, H, t_max, Dh = k_cache.shape
+    R = B * kq
+    if qkv.dim() != 2 or qkv.shape != (R, 3 * H * Dh) or qkv.stride(1) != 1:
+        bad(f"qkv must be [{R}, {3 * H * Dh}] with unit column stride, got {tuple(qkv.shape)} stride {qkv.stride()}")
+    for name, t in rows:
+        if t.shape != (R, H * Dh) or not t.is_contiguous():
+            bad(f"{name} must be a contiguous [{R}, {H * Dh}] tensor, got {tuple(t.shape)}")
+    for name, t in (("lens", lens), ("nq", nq)):
+        if t is not None and (t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != B):
+            bad(f"{name} must be a contiguous int32 tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if work.dtype != torch.float32 or not work.is_contiguous():
+        bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
+    _same_device(who, k_cache.device, (qkv, v_cache, lens, nq, out, side_k, side_v, work))
+    need = decode_attention_work_numel(R, H, Dh, t_max)
+    if work.numel() < need:
+        bad(f"work holds {work.numel()} elements, {need} needed")
+    return B, H, t_max, Dh
+
+
 def decode_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
                       out: torch.Tensor, work: torch.Tensor) -> torch.Tensor:
     """Attention of one new token per row over a KV cache, in place. ``qkv`` bf16 [B, 3·H·Dh] (q | k | v of the new
@@ -293,34 +325,9 @@ def decode_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.T
     ``out[b] = softmax(q·K[0..lens[b]]ᵀ / √Dh)·V[0..lens[b]]`` (bf16 [B, H·Dh], fp32 softmax and accumulation). A row
     with ``lens[b]`` outside [0, t_max) is left alone and its output is zero. ``work``: fp32, at least
     ``decode_attention_work_numel`` elements. Repeatable bit for bit; no host sync, so it can be captured in a graph."""
-    def bad(msg):
-        raise ValueError(f"decode_attention_: {msg}")
-
-    for name, t in (("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)):
-        if t.dtype != torch.bfloat16:
-            bad(f"{name} must be bf16, got {t.dtype}")
-    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
-        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
-            f"and {tuple(v_cache.shape)}")
-    B, H, t_max, Dh = k_cache.shape
-    if qkv.dim() != 2 or qkv.shape != (B, 3 * H * Dh) or qkv.stride(1) != 1:
-        bad(f"qkv must be [{B}, {3 * H * Dh}] with unit column stride, got {tuple(qkv.shape)} stride {qkv.stride()}")
-    if out.shape != (B, H * Dh) or not out.is_contiguous():
-        bad(f"out must be a contiguous [{B}, {H * Dh}] tensor, got {tuple(out.shape)}")
-    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
-        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
-    if work.dtype != torch.float32 or not work.is_contiguous():
-        bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
-    dev = k_cache.device
-    if dev.type != "cuda" or any(t.device != dev for t in (qkv, v_cache, lens, out, work)):
-        bad(f"all tensors must be on one CUDA device, got qkv {qkv.device}, k_cache {dev}, v_cache {v_cache.device}, "
-            f"lens {lens.device}, out {out.device}, work {work.device}")
-    need = decode_attention_work_numel(B, H, Dh, t_max)
-    if work.numel() < need:
-        bad(f"work holds {work.numel()} elements, {need} needed")
-    _ck(_lib().adapcc_decode_attn(c_void_p(qkv.data_ptr()), c_void_p(k_cache.data_ptr()), c_void_p(v_cache.data_ptr()),
-                                  c_void_p(lens.data_ptr()), c_void_p(out.data_ptr()), B, H, Dh, t_max, qkv.stride(0),
-                                  c_void_p(work.data_ptr()), _stream()), "decode_attn")
+    B, H, t_max, Dh = _check_decode_attn("decode_attention_", 1, qkv, k_cache, v_cache, lens, out, work)
+    _ck(_lib().adapcc_decode_attn(_ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(lens), _ptr(out), B, H, Dh, t_max,
+                                  qkv.stride(0), _ptr(work), _stream()), "decode_attn")
     return out
 
 
@@ -572,33 +579,11 @@ def cand_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Ten
     token. The cache is only read (each cached element once per CTA for all k queries); the new keys and values go to
     ``side_k`` / ``side_v`` (bf16 [B·k, H·Dh]). ``work``: fp32, ``decode_attention_work_numel(B·k, ...)`` elements.
     The grid depends on t_max, B and k only; no host sync."""
-    def bad(msg):
-        raise ValueError(f"cand_attention_: {msg}")
-
-    for name, t in (("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out), ("side_k", side_k),
-                    ("side_v", side_v)):
-        if t.dtype != torch.bfloat16:
-            bad(f"{name} must be bf16, got {t.dtype}")
-    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
-        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
-            f"and {tuple(v_cache.shape)}")
-    B, H, t_max, Dh = k_cache.shape
     K = int(top_k)
     if not 1 <= K <= CONTRASTIVE_MAX_K:
-        bad(f"top_k must be in [1, {CONTRASTIVE_MAX_K}], got {top_k}")
-    if qkv.dim() != 2 or qkv.shape != (B * K, 3 * H * Dh) or qkv.stride(1) != 1:
-        bad(f"qkv must be [{B * K}, {3 * H * Dh}] with unit column stride, got {tuple(qkv.shape)} stride {qkv.stride()}")
-    for name, t in (("out", out), ("side_k", side_k), ("side_v", side_v)):
-        if t.shape != (B * K, H * Dh) or not t.is_contiguous():
-            bad(f"{name} must be a contiguous [{B * K}, {H * Dh}] tensor, got {tuple(t.shape)}")
-    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
-        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
-    if work.dtype != torch.float32 or not work.is_contiguous():
-        bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
-    _same_device("cand_attention_", k_cache.device, (qkv, v_cache, lens, out, side_k, side_v, work))
-    need = decode_attention_work_numel(B * K, H, Dh, t_max)
-    if work.numel() < need:
-        bad(f"work holds {work.numel()} elements, {need} needed")
+        raise ValueError(f"cand_attention_: top_k must be in [1, {CONTRASTIVE_MAX_K}], got {top_k}")
+    B, H, t_max, Dh = _check_decode_attn("cand_attention_", K, qkv, k_cache, v_cache, lens, out, work, side_k=side_k,
+                                         side_v=side_v)
     _ck(_lib().adapcc_cand_attn(_ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(lens), _ptr(out), _ptr(side_k),
                                 _ptr(side_v), B, K, H, Dh, t_max, qkv.stride(0), _ptr(work), _stream()), "cand_attn")
     return out
@@ -750,32 +735,10 @@ def verify_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.T
     output is zero. The real slots' keys and values are stored at ``lens[b] + j``; nothing else is written, and each
     cached element is read once per CTA for all of a row's slots. ``work``: fp32, ``decode_attention_work_numel(B·(k+1),
     ...)`` elements. The grid depends on t_max, B and k only; no host sync."""
-    def bad(msg):
-        raise ValueError(f"verify_attention_: {msg}")
-
-    for name, t in (("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out)):
-        if t.dtype != torch.bfloat16:
-            bad(f"{name} must be bf16, got {t.dtype}")
-    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
-        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
-            f"and {tuple(v_cache.shape)}")
-    B, H, t_max, Dh = k_cache.shape
     if not 0 <= int(k) <= LOOKUP_MAX_TOKENS:
-        bad(f"k must be in [0, {LOOKUP_MAX_TOKENS}], got {k}")
+        raise ValueError(f"verify_attention_: k must be in [0, {LOOKUP_MAX_TOKENS}], got {k}")
     S = int(k) + 1
-    if qkv.dim() != 2 or qkv.shape != (B * S, 3 * H * Dh) or qkv.stride(1) != 1:
-        bad(f"qkv must be [{B * S}, {3 * H * Dh}] with unit column stride, got {tuple(qkv.shape)} stride {qkv.stride()}")
-    if out.shape != (B * S, H * Dh) or not out.is_contiguous():
-        bad(f"out must be a contiguous [{B * S}, {H * Dh}] tensor, got {tuple(out.shape)}")
-    for name, t in (("lens", lens), ("nq", nq)):
-        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != B:
-            bad(f"{name} must be a contiguous int32 tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
-    if work.dtype != torch.float32 or not work.is_contiguous():
-        bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
-    _same_device("verify_attention_", k_cache.device, (qkv, v_cache, lens, nq, out, work))
-    need = decode_attention_work_numel(B * S, H, Dh, t_max)
-    if work.numel() < need:
-        bad(f"work holds {work.numel()} elements, {need} needed")
+    B, H, t_max, Dh = _check_decode_attn("verify_attention_", S, qkv, k_cache, v_cache, lens, out, work, nq=nq)
     _ck(_lib().adapcc_verify_attn(_ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(lens), _ptr(nq), _ptr(out), B, S, H,
                                   Dh, t_max, qkv.stride(0), _ptr(work), _stream()), "verify_attn")
     return out

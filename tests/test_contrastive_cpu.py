@@ -223,14 +223,14 @@ def test_sample_replies_with_contrastive_search(tiny):
     assert r["examples"] == 1 and 0.0 <= r["f1"] <= 1.0
 
 
-def test_build_log_shows_contrastive_kernels_for_sm90a_without_spills():
+def test_build_log_shows_contrastive_select_and_rerank_kernels_for_sm90a_without_spills():
     import __graft_entry__
 
     __graft_entry__.build()
     log = open(os.path.join(ROOT, "adapcc_b200", "_C", "build.log")).read()
     assert re.search(r"-gencode arch=compute_90a,code=sm_90a \S.*ops_contrastive\.cu", log)
-    for kernel in ("cand_attn_split_kernel", "cand_attn_combine_kernel", "cs_select_kernel", "cs_sim_kernel",
-                   "cs_commit_kernel", "cs_context_init_kernel", "beam_rows_kernel"):
+    for kernel in ("cs_select_kernel", "cs_sim_kernel", "cs_commit_kernel", "cs_context_init_kernel",
+                   "beam_rows_kernel"):
         hits = re.findall(r"Compiling entry function '(\w*%s\w*)' for 'sm_90a'" % kernel, log)
         assert hits, kernel
         for name in hits:

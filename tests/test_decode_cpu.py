@@ -183,6 +183,8 @@ def test_build_log_shows_decode_kernels_for_sm90a_without_spills():
     for kernel in ("decode_attn_split_kernel", "decode_attn_combine_kernel"):
         hits = re.findall(r"Compiling entry function '(\w*%s\w*)' for 'sm_90a'" % kernel, log)
         assert hits, kernel
+        if kernel == "decode_attn_split_kernel":     # both variants: K / V read from global memory, and staged
+            assert any("ILb0E" in h for h in hits) and any("ILb1E" in h for h in hits), hits
         for name in hits:
             props = re.search(r"Function properties for %s\s+(\d+) bytes stack frame, (\d+) bytes spill stores, "
                               r"(\d+) bytes spill loads" % name, log)

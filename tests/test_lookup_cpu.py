@@ -249,14 +249,13 @@ def test_sample_replies_with_prompt_lookup(tiny):
     assert r == w
 
 
-def test_build_log_shows_lookup_kernels_for_sm90a_without_spills():
+def test_build_log_shows_lookup_accept_and_draft_kernels_for_sm90a_without_spills():
     import __graft_entry__
 
     __graft_entry__.build()
     log = open(os.path.join(ROOT, "adapcc_b200", "_C", "build.log")).read()
     assert re.search(r"-gencode arch=compute_90a,code=sm_90a \S.*ops_lookup\.cu", log)
-    for kernel in ("verify_attn_split_kernel", "verify_attn_combine_kernel", "lk_argmax_kernel", "lk_accept_kernel",
-                   "lk_draft_kernel"):
+    for kernel in ("lk_argmax_kernel", "lk_accept_kernel", "lk_draft_kernel"):
         hits = re.findall(r"Compiling entry function '(\w*%s\w*)' for 'sm_90a'" % kernel, log)
         assert hits, kernel
         for name in hits:
