@@ -114,6 +114,9 @@ struct SampleArgs {
   long long* next_ids;       // [B]
   long long* tokens;         // [B, max_new]
   int max_new;
+  // truncation filters after top-p (DESIGN.md §4a); `filters` is set iff one of them is on
+  float min_p, typical_p, epsilon, eta;
+  bool filters;
 };
 
 // order-preserving: a < b (floats, no NaN) <=> key(a) < key(b)
@@ -145,6 +148,7 @@ __device__ __forceinline__ uint32_t philox_w0(uint32_t c0, uint32_t k0, uint32_t
 
 struct SampleSmem {
   float f[kSampleWarps];
+  float g[kSampleWarps];
   int i[3][kSampleWarps];
   unsigned long long u[kSampleWarps];
 };
@@ -181,6 +185,29 @@ __device__ __forceinline__ void block_sum(SampleSmem& sm, float& f, int& a, int&
   }
 }
 
+// two fp32 block sums with the same fixed order as block_sum
+__device__ __forceinline__ void block_sum2(SampleSmem& sm, float& f, float& g) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    f += __shfl_xor_sync(0xffffffffu, f, o);
+    g += __shfl_xor_sync(0xffffffffu, g, o);
+  }
+  __syncthreads();
+  if (lane == 0) {
+    sm.f[warp] = f;
+    sm.g[warp] = g;
+  }
+  __syncthreads();
+  f = sm.f[lane];
+  g = sm.g[lane];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    f += __shfl_xor_sync(0xffffffffu, f, o);
+    g += __shfl_xor_sync(0xffffffffu, g, o);
+  }
+}
+
 __device__ __forceinline__ unsigned long long block_max(SampleSmem& sm, unsigned long long v) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
@@ -192,6 +219,97 @@ __device__ __forceinline__ unsigned long long block_max(SampleSmem& sm, unsigned
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
+}
+
+// z = sum of e_i = exp(x_i - m) and s1 = sum of e_i (x_i - m) over the finite ids, in block_sum's fixed order
+__device__ __forceinline__ void row_moments(const float* s_x, SampleSmem& sm, int V, float m, float& z, float& s1) {
+  z = 0.f;
+  s1 = 0.f;
+  for (int i = threadIdx.x; i < V; i += kSampleThreads) {
+    const float x = s_x[i];
+    if (x != -INFINITY) {
+      const float y = x - m, e = expf(y);
+      z += e;
+      s1 += e * y;
+    }
+  }
+  block_sum2(sm, z, s1);
+}
+
+// The truncation filters after top-p, in HuggingFace's order: min-p, typical, epsilon, eta. The kept set {key >= tau}
+// is first written into the row (-inf for every other id), and each filter removes ids the same way, so afterwards
+// the survivors are exactly the finite ids. A filter that is off costs nothing; p_i = e_i / Z over the current
+// survivors, with e_i = exp(x_i - m) and m the row maximum, which top-k, top-p and min-p always keep.
+__device__ __noinline__ void filter_row(float* s_x, SampleSmem& sm, const SampleArgs& a, uint32_t tau, float m,
+                                        uint32_t mkey) {
+  const int tid = threadIdx.x, V = a.vocab;
+  // materialise top-k / top-p; min-p keeps e_i >= min_p, i.e. p_i >= min_p p_max
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const float x = s_x[i];
+    if (f2key(x) < tau || (a.min_p > 0.f && expf(x - m) < a.min_p)) s_x[i] = -INFINITY;
+  }
+  uint32_t kmax = mkey;                             // key of the largest survivor: typical may remove the maximum
+  if (a.typical_p < 1.f) {
+    // H = log Z - mu with mu = sum p_i (x_i - m), so the deviation |-log p_i - H| is d_i = |(x_i - m) - mu|. The
+    // cut-off d* is the smallest d with G(d) = (mass of d_i <= d) >= p Z, found by bisection over the order-preserving
+    // keys of d. Invariant: G(lo) < p Z <= G(hi); G(lo) is carried and each pass adds the mass in (lo, mid]. Once no
+    // key lies strictly inside the half that holds d*, that half's upper end is d*. hi starts at key(+inf), so rounding
+    // that keeps every G below p Z keeps every id.
+    float z, s1;
+    row_moments(s_x, sm, V, m, z, s1);
+    const float mu = s1 / z, pz = a.typical_p * z;
+    uint32_t lo = f2key(0.f) - 1, hi = f2key(INFINITY);
+    float g_lo = 0.f;
+    while (hi - lo > 1) {
+      const uint32_t mid = lo + (hi - lo) / 2;
+      float s = 0.f;
+      int nl = 0, nh = 0, unused = 0;
+      for (int i = tid; i < V; i += kSampleThreads) {
+        const float x = s_x[i];
+        if (x != -INFINITY) {
+          const uint32_t k = f2key(fabsf((x - m) - mu));
+          if (k > lo && k <= hi) {
+            if (k <= mid) s += expf(x - m);
+            nl += k < mid;
+            nh += k > mid && k < hi;
+          }
+        }
+      }
+      block_sum(sm, s, nl, nh, unused);
+      const float g = g_lo + s;
+      if (g >= pz) {
+        hi = mid;
+        if (nl == 0) break;
+      } else {
+        lo = mid;
+        g_lo = g;
+        if (nh == 0) break;
+      }
+    }
+    unsigned long long best = 0;
+    for (int i = tid; i < V; i += kSampleThreads) {
+      const float x = s_x[i];
+      if (x != -INFINITY) {
+        if (f2key(fabsf((x - m) - mu)) > hi) s_x[i] = -INFINITY;
+        else best = max(best, (unsigned long long)f2key(x));
+      }
+    }
+    kmax = (uint32_t)block_max(sm, best);
+  }
+  // epsilon keeps p_i >= epsilon, eta keeps p_i >= min(eta, sqrt(eta) exp(-H)) with exp(-H) Z = exp(mu); both keep
+  // the largest survivors (ties together) as well, which only matters when no p_i reaches the threshold
+  for (int f = 0; f < 2; ++f) {
+    const float c = f == 0 ? a.epsilon : a.eta;
+    if (!(c > 0.f)) continue;
+    float z, s1;
+    row_moments(s_x, sm, V, m, z, s1);
+    const float t = f == 0 ? c * z : fminf(c * z, sqrtf(c) * expf(s1 / z));
+    for (int i = tid; i < V; i += kSampleThreads) {
+      const float x = s_x[i];
+      if (x != -INFINITY && expf(x - m) < t && f2key(x) != kmax) s_x[i] = -INFINITY;
+    }
+  }
+  __syncthreads();                                  // the draw reads other threads' ids
 }
 
 __global__ void __launch_bounds__(kSampleThreads, 1)
@@ -308,7 +426,11 @@ sample_tokens_kernel(const __grid_constant__ SampleArgs a) {
       }
       tau = hi;
     }
-    // the draw: the smallest i whose inclusive prefix of surviving weights exceeds u Z'. Thread t owns the contiguous
+    if (a.filters) {
+      filter_row(s_x, sm, a, tau, m, mkey);
+      tau = kNegInfKey + 1;                         // the survivors are the finite ids
+    }
+    // the draw:the smallest i whose inclusive prefix of surviving weights exceeds u Z'. Thread t owns the contiguous
     // ids [t C, t C + C) (C odd, so a warp's reads hit 32 different banks); prefix = (sum of the lower threads' chunks,
     // by a shuffle scan and warp totals in order) + the running sum inside the chunk.
     const int C = ((V + kSampleThreads - 1) / kSampleThreads) | 1;
@@ -421,11 +543,13 @@ int adapcc_lm_head_logits(const void* h, int ld_h, const void* w, int V, int D, 
 }
 
 // logits: fp32 [B, ld]; seeds int64 [B]; pos int32 [B]; step: int32 [1] on the device; suppress / stop: int32 lists
-// on the device (may be null when empty); done int32 [B]; next_ids int64 [B]; tokens int64 [B, max_new]
-int adapcc_sample_tokens(const float* logits, int ld, int vocab, int B, float temperature, int top_k, float top_p,
-                         const long long* seeds, const int* pos, int* step, int min_new, const int* suppress,
-                         int n_suppress, const int* stop, int n_stop, int* done, long long* next_ids, long long* tokens,
-                         int max_new, void* stream) {
+// on the device (may be null when empty); done int32 [B]; next_ids int64 [B]; tokens int64 [B, max_new]; the
+// filters are off at min_p = 0, typical_p = 1, epsilon = 0 and eta = 0
+int adapcc_sample_tokens_filtered(const float* logits, int ld, int vocab, int B, float temperature, int top_k,
+                                  float top_p, float min_p, float typical_p, float epsilon, float eta,
+                                  const long long* seeds, const int* pos, int* step, int min_new, const int* suppress,
+                                  int n_suppress, const int* stop, int n_stop, int* done, long long* next_ids,
+                                  long long* tokens, int max_new, void* stream) {
   if (B < 1 || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab || max_new < 1) {
     set_error("sample_tokens: need B >= 1, 1 <= vocab <= %d, ld >= vocab, max_new >= 1 (B=%d vocab=%d ld=%d "
               "max_new=%d)", kSampleMaxVocab, B, vocab, ld, max_new);
@@ -434,6 +558,12 @@ int adapcc_sample_tokens(const float* logits, int ld, int vocab, int B, float te
   if (!(temperature >= 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
     set_error("sample_tokens: need temperature >= 0, top_k >= 0, 0 < top_p <= 1 (got %g, %d, %g)", temperature, top_k,
               top_p);
+    return -1;
+  }
+  if (!(min_p >= 0.f && min_p <= 1.f) || !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) ||
+      !(eta >= 0.f && eta < 1.f)) {
+    set_error("sample_tokens: need 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= epsilon < 1, 0 <= eta < 1 (got %g, %g, "
+              "%g, %g)", min_p, typical_p, epsilon, eta);
     return -1;
   }
   if (n_suppress < 0 || n_stop < 0 || n_suppress > kSampleMaxList || n_stop > kSampleMaxList ||
@@ -456,7 +586,8 @@ int adapcc_sample_tokens(const float* logits, int ld, int vocab, int B, float te
   });
   CUDA_TRY(setup[dev]);
   SampleArgs a{logits, ld, vocab, temperature, top_p, top_k, seeds, pos, step, min_new, suppress, n_suppress,
-               stop, n_stop, done, next_ids, tokens, max_new};
+               stop, n_stop, done, next_ids, tokens, max_new, min_p, typical_p, epsilon, eta,
+               min_p > 0.f || typical_p < 1.f || epsilon > 0.f || eta > 0.f};
   cudaStream_t s = (cudaStream_t)stream;
   sample_tokens_kernel<<<B, kSampleThreads, (size_t)vocab * sizeof(float), s>>>(a);
   CUDA_TRY(cudaGetLastError());
@@ -465,6 +596,16 @@ int adapcc_sample_tokens(const float* logits, int ld, int vocab, int B, float te
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;
+}
+
+// adapcc_sample_tokens_filtered with every filter off
+int adapcc_sample_tokens(const float* logits, int ld, int vocab, int B, float temperature, int top_k, float top_p,
+                         const long long* seeds, const int* pos, int* step, int min_new, const int* suppress,
+                         int n_suppress, const int* stop, int n_stop, int* done, long long* next_ids, long long* tokens,
+                         int max_new, void* stream) {
+  return adapcc_sample_tokens_filtered(logits, ld, vocab, B, temperature, top_k, top_p, 0.f, 1.f, 0.f, 0.f, seeds, pos,
+                                       step, min_new, suppress, n_suppress, stop, n_stop, done, next_ids, tokens,
+                                       max_new, stream);
 }
 
 }  // extern "C"

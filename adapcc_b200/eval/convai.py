@@ -90,7 +90,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9, no_sample: bool = False,
                    device="cpu", seeds: Optional[Sequence[int]] = None, num_beams: int = 0,
                    repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
-                   penalty_alpha: float = 0.0, prompt_lookup_num_tokens: int = 0) -> List[List[int]]:
+                   penalty_alpha: float = 0.0, prompt_lookup_num_tokens: int = 0, min_p: float = 0.0,
+                   typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -101,7 +102,9 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     ``seeds``: one per dialogue (default 0, 1, ...). ``repetition_penalty`` and ``no_repeat_ngram_size`` go to
     ``generate`` / ``beam_search`` / ``contrastive_search`` (``ops/repeats.py``); the prompt counts as part of each
     reply's sequence. ``prompt_lookup_num_tokens`` > 0 (with ``no_sample``) verifies up to that many draft tokens per
-    step, copied from the prompt and the reply so far; the replies are the greedy ones (``ops/lookup.py``)."""
+    step, copied from the prompt and the reply so far; the replies are the greedy ones (``ops/lookup.py``).
+    ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff`` go to ``generate`` (the truncation filters of the
+    sampler, ``ops/sampling.py``)."""
     insts = [build_input_from_segments(persona, history, [], tokenizer, with_eos=False,
                                        max_len=model.cfg.n_positions - max_length) for persona, history in dialogs]
     lengths = [len(i.input_ids) for i in insts]
@@ -126,7 +129,9 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     tokens, n_new = model.generate(ids, lengths, tt, reply_type, max_new_tokens=max_length,
                                    temperature=0.0 if no_sample else temperature, top_k=top_k, top_p=top_p,
                                    stop_ids=special, suppress_ids=special, min_new_tokens=min_length, seed=seed,
-                                   prompt_lookup_num_tokens=prompt_lookup_num_tokens, **repeats)
+                                   prompt_lookup_num_tokens=prompt_lookup_num_tokens, min_p=min_p,
+                                   typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                                   **repeats)
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
 
 
@@ -214,7 +219,8 @@ def next_word_probability(model, tokenizer: DialogTokenizer, persona, history, p
 def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_type: str = "f1", max_history: int = 2,
                      max_examples: int = 0, device="cpu", seed: int = 0, batch_size: int = 0, num_beams: int = 0,
                      repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, penalty_alpha: float = 0.0,
-                     prompt_lookup_num_tokens: int = 0, **sample_kw) -> Dict[str, float]:
+                     prompt_lookup_num_tokens: int = 0, min_p: float = 0.0, typical_p: float = 1.0,
+                     epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -233,14 +239,19 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     (:func:`sample_replies`), on that batched path.
 
     ``prompt_lookup_num_tokens > 0`` with ``f1`` and ``no_sample``: greedy replies with prompt lookup decoding
-    (:func:`sample_replies`), on that batched path."""
+    (:func:`sample_replies`), on that batched path.
+
+    ``min_p > 0``, ``typical_p < 1``, ``epsilon_cutoff > 0`` or ``eta_cutoff > 0`` with ``f1``: the truncation
+    filters of ``generate``'s sampler (``ops/sampling.py``), on that batched path."""
     repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
     lookup = prompt_lookup_num_tokens > 0
-    if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup) and eval_type == "f1":
+    filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
+    filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0
+    if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup or filtered) and eval_type == "f1":
         return _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples, device, seed,
                                     max(batch_size, 1), num_beams=num_beams, repetition_penalty=repetition_penalty,
                                     no_repeat_ngram_size=no_repeat_ngram_size, penalty_alpha=penalty_alpha,
-                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, **sample_kw)
+                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters, **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -31,7 +31,7 @@ import torch.nn.functional as F
 
 from ..ops.layers import FusedLayerNorm, FusedLinear
 from ..ops.repeats import check_repeat_args, penalize_repeats_reference
-from ..ops.sampling import sample_reference, top_filtering
+from ..ops.sampling import check_filter_args, sample_reference, top_filtering
 
 
 @dataclass
@@ -569,7 +569,8 @@ class GPT2DoubleHeads(nn.Module):
                  temperature: float = 0.7, top_k: int = 0, top_p: float = 0.9, stop_ids: Sequence[int] = (),
                  suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, seed=0, repetition_penalty: float = 1.0,
                  no_repeat_ngram_size: int = 0, prompt_lookup_num_tokens: int = 0,
-                 max_matching_ngram_size: int = 2) -> Tuple[torch.Tensor, torch.Tensor]:
+                 max_matching_ngram_size: int = 2, min_p: float = 0.0, typical_p: float = 1.0,
+                 epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -579,7 +580,10 @@ class GPT2DoubleHeads(nn.Module):
         ``stop_ids`` ends its row. ``temperature == 0`` is greedy. The draw of each token is defined in
         ``ops/sampling.py``: a row's tokens depend on its prompt, its seed and the scalars, not on the other rows.
         ``repetition_penalty`` (1: off) and ``no_repeat_ngram_size`` (0: off) act on each row's logits first, over its
-        prompt and the tokens generated so far (``ops/repeats.py``).
+        prompt and the tokens generated so far (``ops/repeats.py``). ``min_p`` (0: off), ``typical_p`` (1: off),
+        ``epsilon_cutoff`` (0: off) and ``eta_cutoff`` (0: off) are HuggingFace's truncation samplers: at temperature
+        > 0 they filter, in that order, the ids that top-k and top-p kept, just before the draw (inside
+        ``ops.sample_tokens_`` on the native path); at temperature 0 they have no effect.
 
         Returns ``(tokens, n_new)``: int64 [B, max_new_tokens] (-1 after a row stopped) and the tokens per row.
 
@@ -602,6 +606,8 @@ class GPT2DoubleHeads(nn.Module):
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
+        check_filter_args("generate", min_p, typical_p, epsilon_cutoff, eta_cutoff)
+        filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
         K = prompt_lookup_num_tokens
         if K != 0:
             from ..ops import LOOKUP_MAX_NGRAM, LOOKUP_MAX_TOKENS
@@ -634,8 +640,8 @@ class GPT2DoubleHeads(nn.Module):
                 logits = self.lm_logits(h, head)
                 if reps is not None:
                     logits = reps.eager(logits, cache, nxt if i else None)
-                nxt, tok, done = sample_reference(logits, V, temperature, top_k, top_p,
-                                                  seeds, cache.lens, i, min_new_tokens, suppress_ids, stop_ids, done)
+                nxt, tok, done = sample_reference(logits, V, temperature, top_k, top_p, seeds, cache.lens, i,
+                                                  min_new_tokens, suppress_ids, stop_ids, done, **filters)
                 tokens[:, i] = tok.to(dev)
                 if bool(done.all()):
                     break
@@ -655,7 +661,7 @@ class GPT2DoubleHeads(nn.Module):
             if reps is not None:
                 reps.native(logits, cache.lens, step, next_ids)
             sample_tokens_(logits, V, temperature, top_k, top_p, seeds, cache.lens, step,
-                           min_new_tokens, sup, stop, done, next_ids, tokens)
+                           min_new_tokens, sup, stop, done, next_ids, tokens, **filters)
 
         head_and_sample(h)                          # the first token, from the prefill's last positions
         if n > 1:

@@ -46,6 +46,10 @@ def _lib():
         lib.adapcc_sample_tokens.argtypes = ([c_void_p, c_int, c_int, c_int, c_float, c_int, c_float]
                                              + [c_void_p] * 3 + [c_int, c_void_p, c_int, c_void_p, c_int]
                                              + [c_void_p] * 3 + [c_int, c_void_p])
+        lib.adapcc_sample_tokens_filtered.argtypes = ([c_void_p, c_int, c_int, c_int, c_float, c_int]
+                                                      + [c_float] * 5 + [c_void_p] * 3
+                                                      + [c_int, c_void_p, c_int, c_void_p, c_int]
+                                                      + [c_void_p] * 3 + [c_int, c_void_p])
         lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                          + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                          + [c_void_p] * 10 + [c_void_p])
@@ -368,18 +372,25 @@ def lm_head_logits_(h: torch.Tensor, weight: torch.Tensor, out: torch.Tensor) ->
 def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int, top_p: float,
                    seeds: torch.Tensor, pos: torch.Tensor, step: torch.Tensor, min_new: int,
                    suppress_ids: Optional[torch.Tensor], stop_ids: Optional[torch.Tensor], done: torch.Tensor,
-                   next_ids: torch.Tensor, tokens: torch.Tensor) -> None:
+                   next_ids: torch.Tensor, tokens: torch.Tensor, min_p: float = 0.0, typical_p: float = 1.0,
+                   epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> None:
     """One seeded top-k / top-p draw per row, on the device (the definition in ``ops/sampling.py``, which computes the
     same in fp64). ``logits`` fp32 [B, ld] (the first ``vocab`` columns used), ``seeds`` int64 [B], ``pos`` int32 [B]
     (position of the drawn token: the Philox counter), ``step`` int32 [1] (tokens generated so far; incremented),
     ``suppress_ids`` / ``stop_ids`` int32 lists or None, ``done`` int32 [B]. Writes the token into ``next_ids`` int64
     [B] and column ``step`` of ``tokens`` int64 [B, max_new] (-1 for a stop id or a finished row) and sets ``done`` on
-    a stop id. ``temperature == 0`` is greedy. No host sync, so it can be captured in a CUDA graph."""
+    a stop id. ``temperature == 0`` is greedy. No host sync, so it can be captured in a CUDA graph.
+
+    ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff`` (HuggingFace's truncation samplers; off at 0, 1,
+    0 and 0) filter the ids that top-p kept, in that order, before the draw; they have no effect at temperature 0."""
     def bad(msg):
         raise ValueError(f"sample_tokens_: {msg}")
 
     if not temperature >= 0 or not top_k >= 0 or not 0 < top_p <= 1:
         bad(f"need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
+    from .sampling import check_filter_args
+
+    check_filter_args("sample_tokens_", min_p, typical_p, epsilon_cutoff, eta_cutoff)
     if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
         bad(f"logits must be fp32 [B, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
     B = logits.shape[0]
@@ -396,9 +407,11 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
     sup, n_sup = _id_list("sample_tokens_", "suppress_ids", suppress_ids, SAMPLE_MAX_IDS)
     stop, n_stop = _id_list("sample_tokens_", "stop_ids", stop_ids, SAMPLE_MAX_IDS)
     _same_device("sample_tokens_", logits.device, (seeds, pos, step, done, next_ids, tokens, suppress_ids, stop_ids))
-    _ck(_lib().adapcc_sample_tokens(_ptr(logits), logits.stride(0), int(vocab), B, float(temperature), int(top_k),
-                                    float(top_p), _ptr(seeds), _ptr(pos), _ptr(step), int(min_new), sup, n_sup, stop,
-                                    n_stop, _ptr(done), _ptr(next_ids), _ptr(tokens), tokens.shape[1], _stream()),
+    _ck(_lib().adapcc_sample_tokens_filtered(_ptr(logits), logits.stride(0), int(vocab), B, float(temperature),
+                                             int(top_k), float(top_p), float(min_p), float(typical_p),
+                                             float(epsilon_cutoff), float(eta_cutoff), _ptr(seeds), _ptr(pos),
+                                             _ptr(step), int(min_new), sup, n_sup, stop, n_stop, _ptr(done),
+                                             _ptr(next_ids), _ptr(tokens), tokens.shape[1], _stream()),
         "sample_tokens")
 
 

@@ -48,6 +48,17 @@ def main():
     p.add_argument("--prompt_lookup_num_tokens", type=int, default=0,
                    help="f1 with --no_sample: verify up to this many draft tokens per step, copied from the prompt and "
                         "the reply (prompt lookup decoding; 0: off); the replies are the greedy ones")
+    p.add_argument("--min_p", type=float, default=0.0,
+                   help="f1: keep ids with at least this fraction of the top id's probability (0: off); replies go "
+                        "through the batched path")
+    p.add_argument("--typical_p", type=float, default=1.0,
+                   help="f1: locally typical sampling, keep this much mass of the ids closest to the entropy (1: off); "
+                        "replies go through the batched path")
+    p.add_argument("--epsilon_cutoff", type=float, default=0.0,
+                   help="f1: keep ids with probability at least this (0: off); replies go through the batched path")
+    p.add_argument("--eta_cutoff", type=float, default=0.0,
+                   help="f1: eta sampling, keep ids with probability at least min(eta, sqrt(eta) exp(-entropy)) "
+                        "(0: off); replies go through the batched path")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -60,7 +71,8 @@ def main():
         kw = dict(max_length=a.max_length, min_length=a.min_length, temperature=a.temperature, top_k=a.top_k, top_p=a.top_p,
                   no_sample=a.no_sample, repetition_penalty=a.repetition_penalty,
                   no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha,
-                  prompt_lookup_num_tokens=a.prompt_lookup_num_tokens)
+                  prompt_lookup_num_tokens=a.prompt_lookup_num_tokens, min_p=a.min_p, typical_p=a.typical_p,
+                  epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff)
     res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
                            a.batch_size, a.num_beams, **kw)
     print(json.dumps(res))
