@@ -11,6 +11,11 @@
 //   lk_draft       : one CTA per row: the earliest earlier occurrence of the sequence's last m tokens (m from the
 //                    n-gram size down to 1); the tokens after it are the drafts. Writes the next step's ids, positions
 //                    and real-slot count.
+//   lk_round       : one thread per row, assisted generation (a draft model proposes the drafts, ops/assisted.py): the
+//                    start of a round from the target's state alone: slot 0, positions, real-slot count, the draft's
+//                    first input and positions, and the draft cache's lengths. The drafts are drawn by
+//                    sample_slots_kernel (ops_sample.cu), and adapcc_lookup_accept_drawn runs lk_accept on the slots'
+//                    tokens that kernel drew.
 //
 // Every grid depends on B, k and t_max only, so one capture serves every step. A row's results depend only on its own
 // logits, cache and sequence.
@@ -163,6 +168,38 @@ __global__ void __launch_bounds__(kLkDraftThreads) lk_draft_kernel(const __grid_
   if (tid == 0) a.nq[b] = live ? 1 + nd : 0;
 }
 
+// ---- round set-up of assisted generation (a draft model proposes the drafts) ---------------------------------------
+struct RoundArgs {
+  const int* seq;              // [B, t_max]
+  int t_max, B, kq, max_new, n_pos;
+  const int* lens;             // [B]: the target cache's lengths
+  const int* emitted;          // [B]
+  const int* done;             // [B]
+  long long* ids;              // [B * kq]: slot 0 the last token, the drafts' slots 0 (the draft draws fill them)
+  long long* pos;              // [B * kq]: lens[b] + j, clamped to t_max - 1
+  int* nq;                     // [B]: 1 + min(k, max_new - emitted - 1), 0 for a done row
+  long long* d_in;             // [B]: the draft's first input, the last token
+  int* d_lens;                 // [B]: the draft cache's lengths, set to the target's
+  long long* d_pos;            // [kq, B]: the draft's positions at its step j, lens[b] + j clamped to n_pos - 1
+};
+
+__global__ void lk_round_kernel(const __grid_constant__ RoundArgs a) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= a.B) return;
+  const int L = min(max(a.lens[b], 0), a.t_max - 1), K = a.kq - 1;
+  const bool live = !a.done[b];
+  const long long x = live ? a.seq[(long long)b * a.t_max + L] : 0;
+  for (int j = 0; j < a.kq; ++j) {
+    const long long o = (long long)b * a.kq + j;
+    a.ids[o] = j == 0 ? x : 0;
+    a.pos[o] = min(L + j, a.t_max - 1);
+    a.d_pos[(long long)j * a.B + b] = min(L + j, a.n_pos - 1);
+  }
+  a.nq[b] = live ? 1 + max(0, min(K, a.max_new - a.emitted[b] - 1)) : 0;
+  a.d_in[b] = x;
+  a.d_lens[b] = L;
+}
+
 }  // namespace adapcc
 
 using namespace adapcc;
@@ -225,6 +262,53 @@ int adapcc_lookup_draft(const int* seq, int t_max, int B, int kq, int ngram, int
   }
   DraftArgs a{seq, t_max, B, kq, ngram, max_new, lens, emitted, done, ids, pos, nq};
   lk_draft_kernel<<<B, kLkDraftThreads, 0, (cudaStream_t)stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// lk_accept alone on g already drawn by adapcc_sample_slots: g int32, ids int64 [B * kq]; nq, lens, emitted, done
+// int32 [B]; seq int32 [B, t_max]; stop int32 list (null when empty); tokens int64 [B, max_new]; steps int32 [B] or null
+int adapcc_lookup_accept_drawn(int B, int kq, int ls, const int* stop, int n_stop, const int* g, const long long* ids,
+                               const int* nq, int* seq, int t_max, int* lens, int* emitted, int* done,
+                               long long* tokens, int max_new, int* steps, void* stream) {
+  if (B < 1 || B > 65535 || kq < 1 || kq > kLkMaxSlots || (ls != 1 && ls != kq) || t_max < 1 || max_new < 1) {
+    set_error("lookup_accept_drawn: need 1 <= B <= 65535, 1 <= kq <= %d, ls in {1, kq}, t_max, max_new >= 1 (B=%d "
+              "kq=%d ls=%d)", kLkMaxSlots, B, kq, ls);
+    return -1;
+  }
+  if (n_stop < 0 || n_stop > kLkMaxIds || (n_stop && !stop)) {
+    set_error("lookup_accept_drawn: at most %d stop ids (got %d)", kLkMaxIds, n_stop);
+    return -1;
+  }
+  if (!g || !ids || !nq || !seq || !lens || !emitted || !done || !tokens) {
+    set_error("lookup_accept_drawn: null pointer");
+    return -1;
+  }
+  AcceptArgs a{nullptr, 0, 0, B, kq, ls, emitted, 0, nullptr, 0, const_cast<int*>(g), ids, nq, seq, t_max, lens,
+               emitted, done, stop, n_stop, tokens, max_new, steps};
+  lk_accept_kernel<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// seq int32 [B, t_max]; lens, emitted, done int32 [B]; ids, pos int64 [B * kq]; nq int32 [B]; d_in int64 [B]; d_lens
+// int32 [B]; d_pos int64 [kq, B]
+int adapcc_assist_round(const int* seq, int t_max, int B, int kq, int max_new, int n_pos, const int* lens,
+                        const int* emitted, const int* done, long long* ids, long long* pos, int* nq, long long* d_in,
+                        int* d_lens, long long* d_pos, void* stream) {
+  if (B < 1 || B > 65535 || kq < 1 || kq > kLkMaxSlots || t_max < 1 || max_new < 1 || n_pos < 1) {
+    set_error("assist_round: need 1 <= B <= 65535, 1 <= kq <= %d, t_max, max_new, n_pos >= 1 (B=%d kq=%d t_max=%d "
+              "n_pos=%d)", kLkMaxSlots, B, kq, t_max, n_pos);
+    return -1;
+  }
+  if (!seq || !lens || !emitted || !done || !ids || !pos || !nq || !d_in || !d_lens || !d_pos) {
+    set_error("assist_round: null pointer");
+    return -1;
+  }
+  RoundArgs a{seq, t_max, B, kq, max_new, n_pos, lens, emitted, done, ids, pos, nq, d_in, d_lens, d_pos};
+  lk_round_kernel<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;

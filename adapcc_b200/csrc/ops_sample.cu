@@ -10,6 +10,8 @@
 //             The top-k threshold and the top-p cut-off are found by bisection over the order-preserving integer
 //             encoding of x (counts for top-k, masses for top-p), with no sort. The draw is an inclusive scan over the
 //             surviving weights in index order.
+//   slots   : the draws of assisted generation, one CTA per verify slot or draft (grid (slots, B)), through the same
+//             row body as `sample`, with a per-slot Philox counter and step (DESIGN.md §4a).
 //
 // Every floating-point sum runs in fp32 in an order fixed by the thread layout (per-thread loops in index order,
 // shuffle trees, warp partials added in warp order), never by arrival. A row's token depends on its logits, its seed,
@@ -38,6 +40,7 @@ constexpr int kSampleWarps = kSampleThreads / 32;
 constexpr int kSampleMaxVocab = 56 * 1024;   // x of a row in shared memory: 224 KB
 constexpr int kSampleMaxList = 1024;
 constexpr int kOpsMaxDevices = 64;
+constexpr int kSlotMaxSlots = 16;            // verify slots per row (LOOKUP_MAX_TOKENS + 1)
 constexpr uint32_t kNegInfKey = 0x007FFFFFu; // key(-inf): ids at -inf (removed ones included) are never candidates
 
 __global__ void __launch_bounds__(kHeadThreads)
@@ -312,22 +315,13 @@ __device__ __noinline__ void filter_row(float* s_x, SampleSmem& sm, const Sample
   __syncthreads();                                  // the draw reads other threads' ids
 }
 
-__global__ void __launch_bounds__(kSampleThreads, 1)
-sample_tokens_kernel(const __grid_constant__ SampleArgs a) {
-  extern __shared__ float s_x[];                    // [vocab]
-  __shared__ SampleSmem sm;
-  const int b = blockIdx.x, tid = threadIdx.x, V = a.vocab;
-  const int step = *a.step;                         // incremented by the next kernel on the stream, after every CTA
-  long long* tok_out = a.tokens + (long long)b * a.max_new + step;
-  if (a.done[b]) {                                  // a finished row keeps done set and pads its reply with -1
-    if (tid == 0) {
-      if (step < a.max_new) *tok_out = -1;
-      a.next_ids[b] = 0;
-    }
-    return;
-  }
+// One row of the definition (DESIGN.md §4a, steps 1-7) by the whole CTA: the logits row `l`, the tokens generated so
+// far `step` (the min-length rule), the Philox counter `pos` and the row's seed. Returns the token, the same in every
+// thread. sample_tokens_kernel and sample_slots_kernel both draw through it, so their tokens are the same bits.
+__device__ __forceinline__ int draw_row(float* s_x, SampleSmem& sm, const SampleArgs& a, const float* l, int step,
+                                        int pos, long long seed) {
+  const int tid = threadIdx.x, V = a.vocab;
   const bool greedy = a.temperature == 0.f;
-  const float* l = a.logits + (long long)b * a.ld;
   for (int i = tid; i < V; i += kSampleThreads) s_x[i] = greedy ? l[i] : __fdiv_rn(l[i], a.temperature);
   __syncthreads();
   if (step < a.min_new) {                           // the min-length rule comes before any filtering
@@ -468,8 +462,8 @@ sample_tokens_kernel(const __grid_constant__ SampleArgs a) {
     float off = __shfl_sync(0xffffffffu, tot, (warp + 31) & 31);
     if (warp == 0) off = 0.f;
     excl = off + excl;
-    const uint32_t w0 = philox_w0((uint32_t)a.pos[b], (uint32_t)(unsigned long long)a.seeds[b],
-                                  (uint32_t)((unsigned long long)a.seeds[b] >> 32));
+    const uint32_t w0 = philox_w0((uint32_t)pos, (uint32_t)(unsigned long long)seed,
+                                  (uint32_t)((unsigned long long)seed >> 32));
     const float target = (float)(w0 >> 8) * 0x1p-24f * zp;
     int found = INT_MAX;
     if (i0 < i1) {
@@ -490,6 +484,24 @@ sample_tokens_kernel(const __grid_constant__ SampleArgs a) {
     token = first != (unsigned long long)INT_MAX ? (int)first
                                                  : (int)block_max(sm, (unsigned long long)(last + 1)) - 1;
   }
+  return token;
+}
+
+__global__ void __launch_bounds__(kSampleThreads, 1)
+sample_tokens_kernel(const __grid_constant__ SampleArgs a) {
+  extern __shared__ float s_x[];                    // [vocab]
+  __shared__ SampleSmem sm;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int step = *a.step;                         // incremented by the next kernel on the stream, after every CTA
+  long long* tok_out = a.tokens + (long long)b * a.max_new + step;
+  if (a.done[b]) {                                  // a finished row keeps done set and pads its reply with -1
+    if (tid == 0) {
+      if (step < a.max_new) *tok_out = -1;
+      a.next_ids[b] = 0;
+    }
+    return;
+  }
+  const int token = draw_row(s_x, sm, a, a.logits + (long long)b * a.ld, step, a.pos[b], a.seeds[b]);
   if (tid == 0) {
     bool stopped = false;
     for (int j = 0; j < a.n_stop; ++j) stopped |= a.stop[j] == token;
@@ -500,6 +512,44 @@ sample_tokens_kernel(const __grid_constant__ SampleArgs a) {
 }
 
 __global__ void step_incr_kernel(int* step) { *step += 1; }
+
+// ---- per-slot draws of speculative decoding (DESIGN.md §4a, assisted generation) -------------------------------------
+struct SlotArgs {
+  SampleArgs s;              // logits [B * kq, ld], the scalars, suppress list and seeds [B]; the rest unused
+  int B, kq, S, slot0;       // kq logits rows per row b; CTA x draws slot j = slot0 + x of S slots per row
+  const int* lens;           // [B]: the row's cached tokens; slot j draws the token at sequence index lens + j + 1
+  const int* emitted;        // [B]: tokens emitted so far; slot j is generated step emitted + j
+  const int* done;           // [B]
+  const int* nq;             // [B]: the row's real verify slots
+  int* g;                    // verify: g[b * S + j] (slot j real iff j < nq)
+  long long* ids;            // draft: ids[b * S + j + 1] and next[b] (draft j + 1 real iff j + 1 < nq; else 0)
+  long long* next;
+};
+
+__global__ void __launch_bounds__(kSampleThreads, 1)
+sample_slots_kernel(const __grid_constant__ SlotArgs a) {
+  extern __shared__ float s_x[];                    // [vocab]
+  __shared__ SampleSmem sm;
+  const int x = blockIdx.x, b = blockIdx.y, j = a.slot0 + x;
+  const bool draft = a.ids != nullptr;
+  if (a.done[b] || j + (draft ? 1 : 0) >= a.nq[b]) {   // a done row or a pad slot: nothing is drawn
+    if (draft && threadIdx.x == 0) {
+      a.ids[(long long)b * a.S + j + 1] = 0;
+      a.next[b] = 0;
+    }
+    return;
+  }
+  const int token = draw_row(s_x, sm, a.s, a.s.logits + ((long long)b * a.kq + x) * a.s.ld, a.emitted[b] + j,
+                             a.lens[b] + j + 1, a.s.seeds[b]);
+  if (threadIdx.x == 0) {
+    if (draft) {
+      a.ids[(long long)b * a.S + j + 1] = token;
+      a.next[b] = token;
+    } else {
+      a.g[(long long)b * a.S + j] = token;
+    }
+  }
+}
 
 }  // namespace adapcc
 
@@ -593,6 +643,57 @@ int adapcc_sample_tokens_filtered(const float* logits, int ld, int vocab, int B,
   CUDA_TRY(cudaGetLastError());
   count_launch();
   step_incr_kernel<<<1, 1, 0, s>>>(step);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// logits fp32 [B * kq, ld]; seeds int64 [B]; lens, emitted, done, nq int32 [B]; suppress: int32 list (null when
+// empty). Verify draws: g int32 [B * S], ids = next = null. Draft draws (kq = 1: draft j + 1 needs draft j): ids int64
+// [B * S] and next int64 [B], g null.
+int adapcc_sample_slots(const float* logits, int ld, int vocab, int B, int kq, int S, int slot0, float temperature,
+                        int top_k, float top_p, float min_p, float typical_p, float epsilon, float eta,
+                        const long long* seeds, const int* lens, const int* emitted, const int* done, const int* nq,
+                        int min_new, const int* suppress, int n_suppress, int* g, long long* ids, long long* next,
+                        void* stream) {
+  const bool draft = ids != nullptr;
+  if (B < 1 || B > 65535 || S < 1 || S > kSlotMaxSlots || kq < 1 || (draft && kq != 1) || slot0 < 0 ||
+      slot0 + kq + (draft ? 1 : 0) > S || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab) {
+    set_error("sample_slots: need 1 <= B <= 65535, 1 <= S <= %d, kq >= 1 (1 for drafts), 0 <= slot0, slot0 + kq (+ 1 "
+              "for drafts) <= S, 1 <= vocab <= %d, ld >= vocab (B=%d S=%d kq=%d slot0=%d vocab=%d ld=%d)", kSlotMaxSlots,
+              kSampleMaxVocab, B, S, kq, slot0, vocab, ld);
+    return -1;
+  }
+  if (!(temperature >= 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f) || !(min_p >= 0.f && min_p <= 1.f) ||
+      !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) || !(eta >= 0.f && eta < 1.f)) {
+    set_error("sample_slots: need temperature >= 0, top_k >= 0, 0 < top_p <= 1, 0 <= min_p <= 1, 0 < typical_p <= 1, "
+              "0 <= epsilon < 1, 0 <= eta < 1 (got %g, %d, %g, %g, %g, %g, %g)", temperature, top_k, top_p, min_p,
+              typical_p, epsilon, eta);
+    return -1;
+  }
+  if (n_suppress < 0 || n_suppress > kSampleMaxList || (n_suppress && !suppress)) {
+    set_error("sample_slots: a suppress list of at most %d ids (got %d)", kSampleMaxList, n_suppress);
+    return -1;
+  }
+  if (!logits || !seeds || !lens || !emitted || !done || !nq || (draft ? (!next || g) : (!g || next))) {
+    set_error("sample_slots: null pointer, or not exactly one of g and (ids, next)");
+    return -1;
+  }
+  static std::once_flag once[kOpsMaxDevices];
+  static cudaError_t setup[kOpsMaxDevices];
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= kOpsMaxDevices) { set_error("sample_slots: device %d out of range", dev); return -1; }
+  std::call_once(once[dev], [&] {
+    setup[dev] = cudaFuncSetAttribute(sample_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kSampleMaxVocab * (int)sizeof(float));
+  });
+  CUDA_TRY(setup[dev]);
+  SampleArgs s{logits, ld, vocab, temperature, top_p, top_k, seeds, nullptr, nullptr, min_new, suppress, n_suppress,
+               nullptr, 0, nullptr, nullptr, nullptr, 1, min_p, typical_p, epsilon, eta,
+               min_p > 0.f || typical_p < 1.f || epsilon > 0.f || eta > 0.f};
+  SlotArgs a{s, B, kq, S, slot0, lens, emitted, done, nq, g, ids, next};
+  sample_slots_kernel<<<dim3(kq, B), kSampleThreads, (size_t)vocab * sizeof(float), (cudaStream_t)stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;

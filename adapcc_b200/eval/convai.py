@@ -91,7 +91,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    device="cpu", seeds: Optional[Sequence[int]] = None, num_beams: int = 0,
                    repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
                    penalty_alpha: float = 0.0, prompt_lookup_num_tokens: int = 0, min_p: float = 0.0,
-                   typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> List[List[int]]:
+                   typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
+                   assistant_model=None, num_assistant_tokens: int = 4) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -104,7 +105,12 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     reply's sequence. ``prompt_lookup_num_tokens`` > 0 (with ``no_sample``) verifies up to that many draft tokens per
     step, copied from the prompt and the reply so far; the replies are the greedy ones (``ops/lookup.py``).
     ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff`` go to ``generate`` (the truncation filters of the
-    sampler, ``ops/sampling.py``)."""
+    sampler, ``ops/sampling.py``). ``assistant_model`` (a draft model) and ``num_assistant_tokens`` go to ``generate``
+    (assisted generation, ``ops/assisted.py``): the replies are the ones drawn without it; with ``num_beams`` or
+    ``penalty_alpha`` it is a ``ValueError``."""
+    if assistant_model is not None and (num_beams > 0 or penalty_alpha > 0):
+        raise ValueError("sample_replies: assistant_model drafts for sampling and greedy generation only, not with "
+                         f"num_beams > 0 or penalty_alpha > 0 (got {num_beams}, {penalty_alpha})")
     insts = [build_input_from_segments(persona, history, [], tokenizer, with_eos=False,
                                        max_len=model.cfg.n_positions - max_length) for persona, history in dialogs]
     lengths = [len(i.input_ids) for i in insts]
@@ -131,6 +137,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                                    stop_ids=special, suppress_ids=special, min_new_tokens=min_length, seed=seed,
                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, min_p=min_p,
                                    typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                                   assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
                                    **repeats)
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
 
@@ -220,7 +227,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      max_examples: int = 0, device="cpu", seed: int = 0, batch_size: int = 0, num_beams: int = 0,
                      repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, penalty_alpha: float = 0.0,
                      prompt_lookup_num_tokens: int = 0, min_p: float = 0.0, typical_p: float = 1.0,
-                     epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, **sample_kw) -> Dict[str, float]:
+                     epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model=None,
+                     num_assistant_tokens: int = 4, **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -242,16 +250,23 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     (:func:`sample_replies`), on that batched path.
 
     ``min_p > 0``, ``typical_p < 1``, ``epsilon_cutoff > 0`` or ``eta_cutoff > 0`` with ``f1``: the truncation
-    filters of ``generate``'s sampler (``ops/sampling.py``), on that batched path."""
+    filters of ``generate``'s sampler (``ops/sampling.py``), on that batched path.
+
+    ``assistant_model`` (a draft model) with ``f1``: assisted generation with up to ``num_assistant_tokens`` drafts per
+    round (``ops/assisted.py``), on that batched path; the replies are those of the batched path without it."""
     repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
     lookup = prompt_lookup_num_tokens > 0
     filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
     filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0
-    if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup or filtered) and eval_type == "f1":
+    assisted = assistant_model is not None
+    if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup or filtered
+            or assisted) and eval_type == "f1":
         return _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples, device, seed,
                                     max(batch_size, 1), num_beams=num_beams, repetition_penalty=repetition_penalty,
                                     no_repeat_ngram_size=no_repeat_ngram_size, penalty_alpha=penalty_alpha,
-                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters, **sample_kw)
+                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters,
+                                    assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
+                                    **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -261,6 +261,16 @@ class _Repeats:
                           self.penalty, self.ngram)
 
 
+def _row_seeds(seed, B: int, dev) -> torch.Tensor:
+    """``generate``'s per-row seeds, int64 [B] on ``dev``: an int (row b uses ``seed + b``) or an int64 [B] tensor."""
+    if isinstance(seed, torch.Tensor):
+        if seed.dtype != torch.int64 or seed.numel() != B:
+            raise ValueError(f"generate: a seed tensor must be int64 with {B} elements, got {seed.dtype} "
+                             f"{tuple(seed.shape)}")
+        return seed.reshape(B).to(dev)
+    return (int(seed) + torch.arange(B, dtype=torch.int64)).to(dev)
+
+
 class Block(nn.Module):
     """Pre-LN transformer block; the MLP runs as two GEMMs with the activation passes in GEMM epilogues when
     supported (ops/gemm.py), residual adds optionally fused into the following LayerNorm (``forward_deferred``)."""
@@ -570,7 +580,8 @@ class GPT2DoubleHeads(nn.Module):
                  suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, seed=0, repetition_penalty: float = 1.0,
                  no_repeat_ngram_size: int = 0, prompt_lookup_num_tokens: int = 0,
                  max_matching_ngram_size: int = 2, min_p: float = 0.0, typical_p: float = 1.0,
-                 epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor]:
+                 epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model: "GPT2DoubleHeads" = None,
+                 num_assistant_tokens: int = 4) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -602,12 +613,30 @@ class GPT2DoubleHeads(nn.Module):
         step replays one CUDA graph: the model on k + 1 slots per row (``ops.verify_attention_``), the LM head,
         acceptance (``ops.lookup_accept_``) and the next drafts (``ops.lookup_draft_``); the host polls the done flags
         every ``LOOKUP_POLL_PERIOD`` replays. Afterwards ``self.lookup_stats`` holds the rows' emitted tokens (a stop id
-        included) and verify steps, int32 [B], and the graph replays issued."""
+        included) and verify steps, int32 [B], and the graph replays issued.
+
+        ``assistant_model`` (HuggingFace's assisted generation; a ``GPT2DoubleHeads`` with the same vocabulary, bf16 on
+        the same device on the native path; not with prompt lookup or the repetition controls) drafts up to
+        ``num_assistant_tokens`` = k tokens per row and round, which the model verifies in one step. Every emitted token
+        is drawn from the same seed, position and step as in plain ``generate``, greedy or sampled, so given the same
+        per-position logits the tokens are those of plain ``generate``; the draft changes only the speed. The definition
+        is in ``ops/assisted.py``. On the native path (``B·(k+1)`` at most 64 rows) a round replays one CUDA graph: the
+        draft's k + 1 decode steps with k draws (``ops.sample_slots_``), the model on k + 1 slots per row, the LM head,
+        the slots' draws and acceptance (``ops.lookup_accept_drawn_``; ``ops.lookup_accept_`` at temperature 0).
+        Afterwards ``self.assist_stats`` holds what ``lookup_stats`` holds for prompt lookup."""
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
         check_filter_args("generate", min_p, typical_p, epsilon_cutoff, eta_cutoff)
         filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
+        if assistant_model is not None:
+            from ..ops import LOOKUP_MAX_TOKENS
+            from ..ops.assisted import check_assist_args
+            check_assist_args("generate", self, assistant_model, num_assistant_tokens, LOOKUP_MAX_TOKENS,
+                              prompt_lookup_num_tokens, repetition_penalty, no_repeat_ngram_size)
+            return self._generate_assisted(assistant_model, int(num_assistant_tokens), input_ids, lengths,
+                                           token_type_ids, reply_type, max_new_tokens, temperature, top_k, top_p,
+                                           stop_ids, suppress_ids, min_new_tokens, seed, filters)
         K = prompt_lookup_num_tokens
         if K != 0:
             from ..ops import LOOKUP_MAX_NGRAM, LOOKUP_MAX_TOKENS
@@ -620,13 +649,7 @@ class GPT2DoubleHeads(nn.Module):
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size)
         dev, V = input_ids.device, self.cfg.vocab_size
-        if isinstance(seed, torch.Tensor):
-            if seed.dtype != torch.int64 or seed.numel() != B:
-                raise ValueError(f"generate: a seed tensor must be int64 with {B} elements, got {seed.dtype} "
-                                 f"{tuple(seed.shape)}")
-            seeds = seed.reshape(B).to(dev)
-        else:
-            seeds = (int(seed) + torch.arange(B, dtype=torch.int64)).to(dev)
+        seeds = _row_seeds(seed, B, dev)
         cache = self.new_cache(B, t_max)
         h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
@@ -828,6 +851,114 @@ class GPT2DoubleHeads(nn.Module):
                                 step=lambda ids, tt, c: self._verify_hidden(ids, st.pos, tt, verify))
             replays = graph.run(n - 1, st.done, period=LOOKUP_POLL_PERIOD)
         self.lookup_stats = {"emitted": st.emitted, "steps": st.steps, "replays": replays}
+        return st.tokens, (st.tokens >= 0).sum(1)
+
+    def _generate_assisted(self, draft: "GPT2DoubleHeads", K: int, input_ids, lengths, token_type_ids, reply_type,
+                           max_new_tokens, temperature, top_k, top_p, stop_ids, suppress_ids, min_new_tokens, seed,
+                           filters) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``generate`` with ``draft`` proposing up to ``K`` tokens per row and round (``ops/assisted.py``)."""
+        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+            "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens, 1.0, 0,
+            num_beams=K + 1, rows_name="verify rows (batch x (num_assistant_tokens + 1))")
+        dc = draft.cfg
+        if t_max > dc.n_positions:
+            raise ValueError(f"generate: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds the "
+                             f"assistant_model's n_positions = {dc.n_positions}")
+        cfg, dev, weight, V, S = self.cfg, input_ids.device, self.wte.weight, self.cfg.vocab_size, K + 1
+        seeds = _row_seeds(seed, B, dev)
+        tt_v = tt_new.repeat_interleave(S) if tt_new is not None else None
+        cache = self.new_cache(B, t_max)
+        h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
+        # the prompt's last token plays the row's last emitted token x_b, whose logits the prefill gave: lens = len - 1
+        cache.lens.sub_(1)
+        # The draft's cache has K more positions than the model's: a round runs all K + 1 draft steps, and those past a
+        # row's cap write there (their positions are clamped to n_positions - 1); nothing a real slot reads.
+        dcache = KVCache(dc.n_layer, B, dc.n_head, t_max + K, dc.n_embd // dc.n_head, draft.wte.weight.dtype, dev)
+        draft.hidden(input_ids, token_type_ids, cache=dcache, lengths=lengths)
+        if not native:                              # CPU / not bf16: the definition on fp32 PyTorch logits
+            from ..ops.assisted import assist_round, draw_slots
+            from ..ops.lookup import lookup_accept
+            head, dhead = weight.float(), draft.wte.weight.float()
+            seq = torch.zeros(B, t_max, dtype=torch.int32)
+            seq[:, :T] = input_ids.cpu()
+            lens = cache.lens.cpu()
+            emitted, done, steps = (torch.zeros(B, dtype=torch.int32) for _ in range(3))
+            tokens = torch.full((B, n), -1, dtype=torch.int64)
+            kw = dict(min_new=min_new_tokens, suppress_ids=suppress_ids, **filters)
+            scal = (V, temperature, top_k, top_p, seeds.cpu().tolist())
+            ids, nq = torch.zeros(B * S, dtype=torch.int64), torch.ones(B, dtype=torch.int32)
+            g = draw_slots(self.lm_logits(h, head), *scal, lens, emitted, done, nq, **kw)
+            lookup_accept(None, V, ids, nq, seq, lens, emitted, done, tokens, None, stop_ids=stop_ids, drawn=g)
+            rounds = 0
+            while not bool(done.all()):             # every live row emits at least one token per round
+                ids, pos, nq, d_in, d_pos = assist_round(seq, lens, emitted, done, K, n, dc.n_positions)
+                dcache.lens.copy_(lens)
+                ids = ids.view(B, S)
+                for j in range(S):
+                    hd = draft._blocks(draft._embed(d_in.to(dev), tt_new, d_pos[j].to(dev)), dcache)
+                    dcache.lens.add_(1)
+                    if j < K:
+                        d = draw_slots(draft.lm_logits(hd, dhead), *scal, lens, emitted, done, nq, j, True, **kw)
+                        d_in = torch.from_numpy(d[:, 0]).clamp(min=0)
+                        ids[:, j + 1] = d_in
+                ids = ids.reshape(-1)
+                cache.lens.copy_(lens)
+                hv = self._verify_hidden(ids.to(dev), pos.to(dev), tt_v, VerifyKV(cache, S, nq.to(dev)))
+                g = draw_slots(self.lm_logits(hv, head), *scal, lens, emitted, done, nq, **kw)
+                lookup_accept(None, V, ids, nq, seq, lens, emitted, done, tokens, steps, stop_ids=stop_ids, drawn=g)
+                rounds += 1
+            self.assist_stats = {"emitted": emitted, "steps": steps, "replays": rounds}
+            return tokens.to(dev), (tokens >= 0).sum(1).to(dev)
+
+        from ..ops import (AssistState, assist_round_, decode_attention_work_numel, lm_head_logits_, lookup_accept_,
+                           lookup_accept_drawn_, sample_slots_)
+
+        st = AssistState(B, K, n, t_max, dev)
+        st.seq[:, :T] = input_ids
+        dweight = draft.wte.weight
+        logits = torch.empty(B * S, weight.shape[0], dtype=torch.float32, device=dev)
+        dlogits = torch.empty(B, dweight.shape[0], dtype=torch.float32, device=dev)
+        sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
+        draw = (V, temperature, top_k, top_p, seeds, st, cache.lens)
+
+        def accept(lg, first=False):
+            if temperature == 0:                    # greedy verification: the arg-max kernel of prompt lookup
+                lookup_accept_(lg, V, st, cache.lens, min_new_tokens, sup, stop, count=not first)
+            else:
+                sample_slots_(lg, *draw, 0, min_new_tokens, sup, **filters)
+                lookup_accept_drawn_(st, cache.lens, stop, count=not first, first=first)
+
+        lm_head_logits_(h, weight, logits[:B])      # the first token, from the prefill's last positions
+        accept(logits[:B], first=True)
+        replays = 0
+        if n > 1:
+            H = cfg.n_head
+            work = torch.empty(decode_attention_work_numel(B * S, H, cfg.n_embd // H, t_max), dtype=torch.float32,
+                               device=dev)
+            verify = VerifyKV(cache, S, st.nq, work)
+
+            def round_step(ids, tt, c):
+                # a round depends on the model's state alone: its set-up also resets the draft cache's lengths
+                assist_round_(st, cache.lens, dcache.lens, dc.n_positions)
+                for j in range(S):
+                    hd = draft._blocks(draft._embed(st.d_in, tt_new, st.d_pos[j]), dcache)
+                    dcache.lens.add_(1)
+                    if j < K:
+                        lm_head_logits_(hd, dweight, dlogits)
+                        sample_slots_(dlogits, *draw, j, min_new_tokens, sup, draft=True, **filters)
+                return self._verify_hidden(st.ids, st.pos, tt_v, verify)
+
+            def head_and_accept(hv):
+                lm_head_logits_(hv, weight, logits)
+                accept(logits)
+
+            # lookup_accept_ advances the cache by the tokens it emits, up to k + 1 per replay, while the host counts
+            # one per replay; as for prompt lookup, at most n - 1 replays follow the first token, so check_room never
+            # fires
+            graph = DecodeGraph(self, cache, tt_v is not None, head=head_and_accept, ids=st.ids, tt=tt_v,
+                                step=round_step)
+            replays = graph.run(n - 1, st.done, period=LOOKUP_POLL_PERIOD)
+        self.assist_stats = {"emitted": st.emitted, "steps": st.steps, "replays": replays}
         return st.tokens, (st.tokens >= 0).sum(1)
 
     def _verify_hidden(self, ids: torch.Tensor, pos: torch.Tensor, tt: Optional[torch.Tensor],

@@ -71,6 +71,11 @@ def _lib():
         lib.adapcc_lookup_accept.argtypes = ([c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_int]
                                              + [c_void_p] * 4 + [c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p])
         lib.adapcc_lookup_draft.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 7
+        lib.adapcc_sample_slots.argtypes = ([c_void_p] + [c_int] * 6 + [c_float, c_int] + [c_float] * 5
+                                            + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 4)
+        lib.adapcc_lookup_accept_drawn.argtypes = ([c_int] * 3 + [c_void_p, c_int] + [c_void_p] * 4 + [c_int]
+                                                   + [c_void_p] * 4 + [c_int, c_void_p, c_void_p])
+        lib.adapcc_assist_round.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 10
         _bound = True
     return lib
 
@@ -846,3 +851,112 @@ def lookup_draft_(state: LookupState, lens: torch.Tensor) -> None:
     _ck(_lib().adapcc_lookup_draft(_ptr(state.seq), state.t_max, B, state.k + 1, state.ngram, state.max_new,
                                    _ptr(lens), _ptr(state.emitted), _ptr(state.done), _ptr(state.ids), _ptr(state.pos),
                                    _ptr(state.nq), _stream()), "lookup_draft")
+
+
+# ---- assisted generation: per-slot draws (csrc/ops_sample.cu), drawn acceptance and round set-up (ops_lookup.cu) ----
+class AssistState(LookupState):
+    """A ``LookupState`` for assisted generation, where a draft model proposes the drafts (``ops/assisted.py``), plus
+    the draft's input buffers: ``d_in`` int64 [B] the token the draft consumes next and ``d_pos`` int64 [k+1, B] its
+    positions at each of its k + 1 steps of a round (``lens[b] + j`` clamped to the model's ``n_positions - 1``)."""
+
+    def __init__(self, batch: int, k: int, max_new: int, t_max: int, device):
+        super().__init__(batch, k, max_new, t_max, 1, device)
+        self.d_in = torch.zeros(self.batch, dtype=torch.int64, device=device)
+        self.d_pos = torch.zeros(self.k + 1, self.batch, dtype=torch.int64, device=device)
+
+    def tensors(self):
+        """Every device tensor of the state, the draft's buffers included."""
+        return super().tensors() + (self.d_in, self.d_pos)
+
+
+def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int, top_p: float, seeds: torch.Tensor,
+                  state: LookupState, lens: torch.Tensor, slot0: int = 0, min_new: int = 0,
+                  suppress_ids: Optional[torch.Tensor] = None, draft: bool = False, min_p: float = 0.0,
+                  typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> None:
+    """The draws of speculative decoding, one CTA per slot, on the device. ``logits`` fp32 [B·kq, ld] (the first
+    ``vocab`` columns used) holds ``kq`` slots per row; its slot x of row b is slot ``j = slot0 + x``, drawn as
+    ``sample_tokens_`` draws a row (the same bits) with the Philox counter ``lens[b] + j + 1`` (``lens`` int32 [B]) and
+    step ``state.emitted[b] + j``; ``seeds`` int64 [B]. A done row (``state.done``) draws nothing.
+
+    Verify draws (``draft=False``): slot j is real iff ``j < state.nq[b]`` and its token goes to ``state.g[b·(k+1) +
+    j]``; pad slots are left alone. Draft draws (``draft=True``, an ``AssistState``, one logits row per row): the token
+    is draft j + 1, real iff
+    ``j + 1 < state.nq[b]``; it goes to ``state.ids[b·(k+1) + j + 1]`` and ``state.d_in[b]`` (0 for a pad draft or a
+    done row). No host sync."""
+    def bad(msg):
+        raise ValueError(f"sample_slots_: {msg}")
+
+    if not isinstance(state, LookupState) or (draft and not isinstance(state, AssistState)):
+        bad(f"state must be a {'AssistState' if draft else 'LookupState'}, got {type(state).__name__}")
+    if not temperature >= 0 or not top_k >= 0 or not 0 < top_p <= 1:
+        bad(f"need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
+    from .sampling import check_filter_args
+
+    check_filter_args("sample_slots_", min_p, typical_p, epsilon_cutoff, eta_cutoff)
+    B, S = state.batch, state.k + 1
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1 or logits.shape[0] % B:
+        bad(f"logits must be fp32 [{B}·kq, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
+    kq = logits.shape[0] // B
+    if draft and kq != 1:
+        bad(f"draft draws take one logits row per row (draft j + 1 depends on draft j), got {kq}")
+    if not 0 <= int(slot0) or int(slot0) + kq + int(draft) > S:
+        bad(f"slots {slot0}..{int(slot0) + kq - 1} do not fit {S} slots per row (draft: {draft})")
+    if not 1 <= vocab <= min(logits.shape[1], SAMPLE_MAX_VOCAB):
+        bad(f"vocab must be in [1, min(ld = {logits.shape[1]}, {SAMPLE_MAX_VOCAB})], got {vocab}")
+    for name, t, dt in (("seeds", seeds, torch.int64), ("lens", lens, torch.int32)):
+        if t.dtype != dt or not t.is_contiguous() or t.numel() != B:
+            bad(f"{name} must be a contiguous {dt} tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if int(min_new) < 0:
+        bad(f"min_new must be >= 0, got {min_new}")
+    sup, n_sup = _id_list("sample_slots_", "suppress_ids", suppress_ids, SAMPLE_MAX_IDS)
+    _same_device("sample_slots_", logits.device, state.tensors() + (seeds, lens, suppress_ids))
+    _ck(_lib().adapcc_sample_slots(_ptr(logits), logits.stride(0), int(vocab), B, kq, S, int(slot0),
+                                   float(temperature), int(top_k), float(top_p), float(min_p), float(typical_p),
+                                   float(epsilon_cutoff), float(eta_cutoff), _ptr(seeds), _ptr(lens),
+                                   _ptr(state.emitted), _ptr(state.done), _ptr(state.nq), int(min_new), sup, n_sup,
+                                   None if draft else _ptr(state.g), _ptr(state.ids) if draft else None,
+                                   _ptr(state.d_in) if draft else None, _stream()), "sample_slots")
+
+
+def lookup_accept_drawn_(state: LookupState, lens: torch.Tensor, stop_ids: Optional[torch.Tensor] = None,
+                         count: bool = True, first: bool = False) -> None:
+    """``lookup_accept_``'s acceptance on the tokens ``state.g`` already holds (``sample_slots_``'s verify draws), with
+    no arg-max: the same kernel and rule. ``first``: one slot per row (the prefill's draw, ``state.nq`` all 1)."""
+    def bad(msg):
+        raise ValueError(f"lookup_accept_drawn_: {msg}")
+
+    if not isinstance(state, LookupState):
+        bad(f"state must be a LookupState, got {type(state).__name__}")
+    B, S = state.batch, state.k + 1
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
+        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    stop, n_stop = _id_list("lookup_accept_drawn_", "stop_ids", stop_ids, LOOKUP_MAX_IDS)
+    _same_device("lookup_accept_drawn_", lens.device, state.tensors() + (stop_ids,))
+    _ck(_lib().adapcc_lookup_accept_drawn(B, S, 1 if first else S, stop, n_stop, _ptr(state.g), _ptr(state.ids),
+                                          _ptr(state.nq), _ptr(state.seq), state.t_max, _ptr(lens),
+                                          _ptr(state.emitted), _ptr(state.done), _ptr(state.tokens), state.max_new,
+                                          _ptr(state.steps if count else None), _stream()), "lookup_accept_drawn")
+
+
+def assist_round_(state: AssistState, lens: torch.Tensor, d_lens: torch.Tensor, n_pos: int) -> None:
+    """The start of a round of assisted generation, from the target's state alone (``ops/assisted.py``): writes
+    ``state.ids`` (slot 0 the last token ``seq[b, lens[b]]``, 0 in the draft slots), ``state.pos`` (``lens[b] + j``
+    clamped to ``t_max - 1``), ``state.nq`` (``1 + min(k, max_new - emitted - 1)``, 0 for a done row), ``state.d_in``
+    (the last token), ``state.d_pos`` and the draft cache's lengths ``d_lens`` (int32 [B], set to ``lens``). No host
+    sync."""
+    def bad(msg):
+        raise ValueError(f"assist_round_: {msg}")
+
+    if not isinstance(state, AssistState):
+        bad(f"state must be an AssistState, got {type(state).__name__}")
+    B = state.batch
+    for name, t in (("lens", lens), ("d_lens", d_lens)):
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != B:
+            bad(f"{name} must be a contiguous int32 tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if int(n_pos) < 1:
+        bad(f"n_pos must be >= 1, got {n_pos}")
+    _same_device("assist_round_", lens.device, state.tensors() + (d_lens,))
+    _ck(_lib().adapcc_assist_round(_ptr(state.seq), state.t_max, B, state.k + 1, state.max_new, int(n_pos),
+                                   _ptr(lens), _ptr(state.emitted), _ptr(state.done), _ptr(state.ids), _ptr(state.pos),
+                                   _ptr(state.nq), _ptr(state.d_in), _ptr(d_lens), _ptr(state.d_pos), _stream()),
+        "assist_round")

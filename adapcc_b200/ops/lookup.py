@@ -113,25 +113,27 @@ def lookup_draft(seq: torch.Tensor, lens: torch.Tensor, emitted: torch.Tensor, d
 def lookup_accept(logits: torch.Tensor, vocab: int, ids: torch.Tensor, nq: torch.Tensor, seq: torch.Tensor,
                   lens: torch.Tensor, emitted: torch.Tensor, done: torch.Tensor, tokens: torch.Tensor,
                   steps: torch.Tensor = None, min_new: int = 0, suppress_ids: Sequence[int] = (),
-                  stop_ids: Sequence[int] = ()) -> None:
+                  stop_ids: Sequence[int] = (), drawn=None) -> None:
     """``lookup_accept_`` for a batch on the host, in place on the CPU tensors ``seq`` [B, t_max], ``lens``,
     ``emitted``, ``done`` [B], ``tokens`` [B, max_new] (-1 where nothing is written) and ``steps`` [B] (verify steps
     per live row; None: not counted). ``logits`` [B·ls, >= vocab] holds ``ls`` slots per row (1 for the prefill's
     logits, k + 1 for a verify step), ``ids`` [B·(k+1)] the step's input and ``nq`` [B] its real slots (at most
-    ``ls`` are used)."""
+    ``ls`` are used). ``drawn`` [B, ls] (``lookup_accept_drawn_``): the slots' tokens, already drawn
+    (``ops/assisted.py``), in place of the arg-maxes of ``logits`` (which may then be None)."""
     B, t_max = seq.shape
-    ls = logits.shape[0] // B
+    ls = logits.shape[0] // B if drawn is None else drawn.shape[1]
     S = ids.numel() // B
     max_new = tokens.shape[1]
     stop = set(int(s) for s in stop_ids)
-    rows = logits[:, :vocab].detach().float().cpu().numpy().reshape(B, ls, vocab)
+    rows = None if drawn is not None else logits[:, :vocab].detach().float().cpu().numpy().reshape(B, ls, vocab)
     ids = ids.cpu().reshape(B, S)
     for b in range(B):
         if done[b]:
             continue
         e, L = int(emitted[b]), int(lens[b])
         n = max(0, min(int(nq[b]), ls))
-        g = [greedy_token(rows[b, j], e + j, min_new, suppress_ids) for j in range(n)]
+        g = ([int(drawn[b, j]) for j in range(n)] if drawn is not None
+             else [greedy_token(rows[b, j], e + j, min_new, suppress_ids) for j in range(n)])
         out, fin = accept_row(g, ids[b, 1:n].tolist(), e, max_new, stop_ids)
         for i, t in enumerate(out):
             if L + 1 + i < t_max:

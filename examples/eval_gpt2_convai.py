@@ -59,6 +59,11 @@ def main():
     p.add_argument("--eta_cutoff", type=float, default=0.0,
                    help="f1: eta sampling, keep ids with probability at least min(eta, sqrt(eta) exp(-entropy)) "
                         "(0: off); replies go through the batched path")
+    p.add_argument("--assistant_checkpoint", default="",
+                   help="f1: a smaller model with the same vocabulary (a --checkpoint file) drafts tokens that the model "
+                        "verifies (assisted generation); the replies are those drawn without it, through the batched path")
+    p.add_argument("--num_assistant_tokens", type=int, default=4,
+                   help="f1 with --assistant_checkpoint: draft tokens per verify step")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -73,6 +78,10 @@ def main():
                   no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha,
                   prompt_lookup_num_tokens=a.prompt_lookup_num_tokens, min_p=a.min_p, typical_p=a.typical_p,
                   epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff)
+        if a.assistant_checkpoint:
+            kw["assistant_model"] = load_model_from_checkpoint(
+                a.assistant_checkpoint, a.device, torch.bfloat16 if a.device.startswith("cuda") else None)[0]
+            kw["num_assistant_tokens"] = a.num_assistant_tokens
     res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
                            a.batch_size, a.num_beams, **kw)
     print(json.dumps(res))
