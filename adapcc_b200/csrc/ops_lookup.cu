@@ -8,6 +8,8 @@
 //   lk_accept      : one thread per row: emits g_0, g_1, ... while the draft of the next slot equals the token just
 //                    emitted, stopping at a stop id (sets done, not written), at max_new tokens (sets done) or at the
 //                    first rejected draft; appends the emitted ids to the row's sequence, advances lens and emitted.
+//                    With per-slot accepted flags (rejection sampling, spec_slots_kernel in ops_sample.cu) it emits
+//                    the accepted drafts instead, then the token the slot of the first rejection holds.
 //   lk_draft       : one CTA per row: the earliest earlier occurrence of the sequence's last m tokens (m from the
 //                    n-gram size down to 1); the tokens after it are the drafts. Writes the next step's ids, positions
 //                    and real-slot count.
@@ -57,6 +59,8 @@ struct AcceptArgs {
   long long* tokens;           // [B, max_new]
   int max_new;
   int* steps;                  // [B]: verify steps per live row (null: not counted)
+  const int* acc;              // [B * kq] or null: draft j + 1 accepted (rejection sampling); g then holds the token a
+                               // round emits last if it ends at slot j
 };
 
 __device__ __forceinline__ int accept_slots(const AcceptArgs& a, int b) { return max(0, min(a.nq[b], a.ls)); }
@@ -95,7 +99,9 @@ __global__ void lk_accept_kernel(const __grid_constant__ AcceptArgs a) {
   int e = a.emitted[b], c = 0, done = 0;
   int* s = a.seq + (long long)b * a.t_max;
   for (int j = 0; j < nq; ++j) {
-    const int t = a.g[(long long)b * a.kq + j];
+    const long long o = (long long)b * a.kq + j;
+    const bool accepted = a.acc && j + 1 < nq && a.acc[o];
+    const int t = accepted ? (int)a.ids[o + 1] : a.g[o];
     if (L + 1 + c < a.t_max) s[L + 1 + c] = t;
     ++c;
     ++e;
@@ -110,7 +116,7 @@ __global__ void lk_accept_kernel(const __grid_constant__ AcceptArgs a) {
       done = 1;
       break;
     }
-    if (j + 1 < nq && a.ids[(long long)b * a.kq + j + 1] != t) break;   // draft j + 1 rejected
+    if (a.acc ? !accepted : j + 1 < nq && a.ids[o + 1] != t) break;   // draft j + 1 rejected
   }
   a.lens[b] = L + c;
   a.emitted_w[b] = e;
@@ -236,7 +242,7 @@ int adapcc_lookup_accept(const float* logits, int ld, int vocab, int B, int kq, 
   if (bits > 48 * 1024)
     CUDA_TRY(cudaFuncSetAttribute(lk_argmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bits));
   AcceptArgs a{logits, ld, vocab, B, kq, ls, emitted, min_new, suppress, n_suppress, g, ids, nq, seq, t_max, lens,
-               emitted, done, stop, n_stop, tokens, max_new, steps};
+               emitted, done, stop, n_stop, tokens, max_new, steps, nullptr};
   cudaStream_t s = (cudaStream_t)stream;
   lk_argmax_kernel<<<dim3(ls, B), kBeamThreads, bits, s>>>(a);
   CUDA_TRY(cudaGetLastError());
@@ -268,10 +274,12 @@ int adapcc_lookup_draft(const int* seq, int t_max, int B, int kq, int ngram, int
 }
 
 // lk_accept alone on g already drawn by adapcc_sample_slots: g int32, ids int64 [B * kq]; nq, lens, emitted, done
-// int32 [B]; seq int32 [B, t_max]; stop int32 list (null when empty); tokens int64 [B, max_new]; steps int32 [B] or null
+// int32 [B]; seq int32 [B, t_max]; stop int32 list (null when empty); tokens int64 [B, max_new]; steps int32 [B] or
+// null; acc int32 [B * kq] or null: the accepted flags and last tokens (g) of adapcc_spec_slots, null for the rule
+// that a draft is accepted when it equals the token just emitted
 int adapcc_lookup_accept_drawn(int B, int kq, int ls, const int* stop, int n_stop, const int* g, const long long* ids,
                                const int* nq, int* seq, int t_max, int* lens, int* emitted, int* done,
-                               long long* tokens, int max_new, int* steps, void* stream) {
+                               long long* tokens, int max_new, int* steps, const int* acc, void* stream) {
   if (B < 1 || B > 65535 || kq < 1 || kq > kLkMaxSlots || (ls != 1 && ls != kq) || t_max < 1 || max_new < 1) {
     set_error("lookup_accept_drawn: need 1 <= B <= 65535, 1 <= kq <= %d, ls in {1, kq}, t_max, max_new >= 1 (B=%d "
               "kq=%d ls=%d)", kLkMaxSlots, B, kq, ls);
@@ -286,7 +294,7 @@ int adapcc_lookup_accept_drawn(int B, int kq, int ls, const int* stop, int n_sto
     return -1;
   }
   AcceptArgs a{nullptr, 0, 0, B, kq, ls, emitted, 0, nullptr, 0, const_cast<int*>(g), ids, nq, seq, t_max, lens,
-               emitted, done, stop, n_stop, tokens, max_new, steps};
+               emitted, done, stop, n_stop, tokens, max_new, steps, acc};
   lk_accept_kernel<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();

@@ -11,7 +11,10 @@
 //             encoding of x (counts for top-k, masses for top-p), with no sort. The draw is an inclusive scan over the
 //             surviving weights in index order.
 //   slots   : the draws of assisted generation, one CTA per verify slot or draft (grid (slots, B)), through the same
-//             row body as `sample`, with a per-slot Philox counter and step (DESIGN.md §4a).
+//             row body as `sample`, with a per-slot Philox counter and step (DESIGN.md §4a). A draft draw can also
+//             write the draft's filtered weights, which rejection-sampling verification reads.
+//   spec    : rejection-sampling verification of a round, one CTA per verify slot (grid (k + 1, B)): the slot's draw,
+//             the acceptance of its draft and the residual draw, each from its own Philox word (DESIGN.md §4a).
 //
 // Every floating-point sum runs in fp32 in an order fixed by the thread layout (per-thread loops in index order,
 // shuffle trees, warp partials added in warp order), never by arrival. A row's token depends on its logits, its seed,
@@ -132,8 +135,10 @@ __device__ __forceinline__ float key2f(uint32_t k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
-// first output word of Philox4x32-10 (Salmon et al., SC'11) for counter (c0, 0, 0, 0) and key (k0, k1)
-__device__ __forceinline__ uint32_t philox_w0(uint32_t c0, uint32_t k0, uint32_t k1) {
+// the four output words of Philox4x32-10 (Salmon et al., SC'11) for counter (c0, 0, 0, 0) and key (k0, k1): the draw
+// uses word 0; rejection-sampling verification uses word 1 for the acceptance test and word 2 for the residual draw,
+// so neither depends on the draw that produced the draft
+__device__ __forceinline__ uint4 philox4(uint32_t c0, uint32_t k0, uint32_t k1) {
   uint32_t c1 = 0u, c2 = 0u, c3 = 0u;
 #pragma unroll
   for (int r = 0; r < 10; ++r) {
@@ -146,7 +151,7 @@ __device__ __forceinline__ uint32_t philox_w0(uint32_t c0, uint32_t k0, uint32_t
     k0 += 0x9E3779B9u;
     k1 += 0xBB67AE85u;
   }
-  return c0;
+  return make_uint4(c0, c1, c2, c3);
 }
 
 struct SampleSmem {
@@ -315,11 +320,90 @@ __device__ __noinline__ void filter_row(float* s_x, SampleSmem& sm, const Sample
   __syncthreads();                                  // the draw reads other threads' ids
 }
 
+__device__ __forceinline__ float philox_uniform(uint32_t w) { return (float)(w >> 8) * 0x1p-24f; }
+
+// The inverse-CDF pick over s_x[0, V) by the whole CTA: the ids with `counts(x)` count, with weight `weight(x)`. Returns the smallest counting i whose inclusive prefix of weights exceeds u Z' (Z', the total, goes to `zp`), or
+// the largest counting id when rounding leaves none, or -1 when no id counts. Thread t owns the contiguous ids
+// [t C, t C + C) (C odd, so a warp's reads hit 32 different banks); prefix = (sum of the lower threads' chunks, by a
+// shuffle scan and warp totals in order) + the running sum inside the chunk.
+template <class Counts, class Weight>
+__device__ __forceinline__ int scan_pick(const float* s_x, SampleSmem& sm, int V, Counts counts, Weight weight, float u,
+                                         float& zp) {
+  const int tid = threadIdx.x;
+  const int C = ((V + kSampleThreads - 1) / kSampleThreads) | 1;
+  const int i0 = min(tid * C, V), i1 = min(i0 + C, V);
+  float run = 0.f;
+  int last = -1;
+  for (int i = i0; i < i1; ++i) {
+    const float x = s_x[i];
+    if (counts(x)) {
+      run += weight(x);
+      last = i;
+    }
+  }
+  const int lane = tid & 31, warp = tid >> 5;
+  float inc = run;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float y = __shfl_up_sync(0xffffffffu, inc, o);
+    if (lane >= o) inc += y;
+  }
+  float excl = __shfl_up_sync(0xffffffffu, inc, 1);
+  if (lane == 0) excl = 0.f;
+  __syncthreads();
+  if (lane == 31) sm.f[warp] = inc;
+  __syncthreads();
+  // offset of this warp: an inclusive shuffle scan over the warp totals (lane w holds warp w's), the same in
+  // every warp; Z' is its last element
+  float tot = sm.f[lane];
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const float y = __shfl_up_sync(0xffffffffu, tot, o);
+    if (lane >= o) tot += y;
+  }
+  zp = __shfl_sync(0xffffffffu, tot, 31);
+  float off = __shfl_sync(0xffffffffu, tot, (warp + 31) & 31);
+  if (warp == 0) off = 0.f;
+  excl = off + excl;
+  const float target = u * zp;
+  int found = INT_MAX;
+  if (i0 < i1) {
+    float acc = 0.f;
+    for (int i = i0; i < i1; ++i) {
+      const float x = s_x[i];
+      if (counts(x)) {
+        acc += weight(x);
+        if (excl + acc > target) {
+          found = i;
+          break;
+        }
+      }
+    }
+  }
+  // the first crossing over the block; when rounding leaves none, the largest counting id
+  const unsigned long long first = 0xFFFFFFFFull - block_max(sm, 0xFFFFFFFFull - (unsigned long long)found);
+  return first != (unsigned long long)INT_MAX ? (int)first
+                                              : (int)block_max(sm, (unsigned long long)(last + 1)) - 1;
+}
+
+// What a draw decided from: the survivors are the ids with f2key(s_x[i]) >= tau, with weights expf(s_x[i] - m) and
+// total zp. No survivor (greedy, or no finite logit): tau above every key, zp = 0.
+struct RowCut {
+  uint32_t tau;
+  float m, zp;
+};
+
+__device__ __forceinline__ float cut_prob(float x, const RowCut& c) {
+  return f2key(x) >= c.tau ? expf(x - c.m) / c.zp : 0.f;
+}
+
 // One row of the definition (DESIGN.md §4a, steps 1-7) by the whole CTA: the logits row `l`, the tokens generated so
 // far `step` (the min-length rule), the Philox counter `pos` and the row's seed. Returns the token, the same in every
-// thread. sample_tokens_kernel and sample_slots_kernel both draw through it, so their tokens are the same bits.
+// thread. sample_tokens_kernel, sample_slots_kernel and spec_slots_kernel all draw through it, so their tokens are the
+// same bits. With `cut`, it also returns the survivors; s_x then still holds the row they are read from.
 __device__ __forceinline__ int draw_row(float* s_x, SampleSmem& sm, const SampleArgs& a, const float* l, int step,
-                                        int pos, long long seed) {
+                                        int pos, long long seed, RowCut* cut = nullptr) {
+  if (cut) *cut = RowCut{0xFFFFFFFFu, 0.f, 0.f};
   const int tid = threadIdx.x, V = a.vocab;
   const bool greedy = a.temperature == 0.f;
   for (int i = tid; i < V; i += kSampleThreads) s_x[i] = greedy ? l[i] : __fdiv_rn(l[i], a.temperature);
@@ -424,65 +508,13 @@ __device__ __forceinline__ int draw_row(float* s_x, SampleSmem& sm, const Sample
       filter_row(s_x, sm, a, tau, m, mkey);
       tau = kNegInfKey + 1;                         // the survivors are the finite ids
     }
-    // the draw:the smallest i whose inclusive prefix of surviving weights exceeds u Z'. Thread t owns the contiguous
-    // ids [t C, t C + C) (C odd, so a warp's reads hit 32 different banks); prefix = (sum of the lower threads' chunks,
-    // by a shuffle scan and warp totals in order) + the running sum inside the chunk.
-    const int C = ((V + kSampleThreads - 1) / kSampleThreads) | 1;
-    const int i0 = min(tid * C, V), i1 = min(i0 + C, V);
-    float run = 0.f;
-    int last = -1;
-    for (int i = i0; i < i1; ++i) {
-      const float x = s_x[i];
-      if (f2key(x) >= tau) {
-        run += expf(x - m);
-        last = i;
-      }
-    }
-    const int lane = tid & 31, warp = tid >> 5;
-    float inc = run;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const float y = __shfl_up_sync(0xffffffffu, inc, o);
-      if (lane >= o) inc += y;
-    }
-    float excl = __shfl_up_sync(0xffffffffu, inc, 1);
-    if (lane == 0) excl = 0.f;
-    __syncthreads();
-    if (lane == 31) sm.f[warp] = inc;
-    __syncthreads();
-    // offset of this warp: an inclusive shuffle scan over the warp totals (lane w holds warp w's), the same in
-    // every warp; Z' is its last element
-    float tot = sm.f[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const float y = __shfl_up_sync(0xffffffffu, tot, o);
-      if (lane >= o) tot += y;
-    }
-    const float zp = __shfl_sync(0xffffffffu, tot, 31);
-    float off = __shfl_sync(0xffffffffu, tot, (warp + 31) & 31);
-    if (warp == 0) off = 0.f;
-    excl = off + excl;
-    const uint32_t w0 = philox_w0((uint32_t)pos, (uint32_t)(unsigned long long)seed,
-                                  (uint32_t)((unsigned long long)seed >> 32));
-    const float target = (float)(w0 >> 8) * 0x1p-24f * zp;
-    int found = INT_MAX;
-    if (i0 < i1) {
-      float acc = 0.f;
-      for (int i = i0; i < i1; ++i) {
-        const float x = s_x[i];
-        if (f2key(x) >= tau) {
-          acc += expf(x - m);
-          if (excl + acc > target) {
-            found = i;
-            break;
-          }
-        }
-      }
-    }
-    // the first crossing over the block; when rounding leaves none, the largest surviving id
-    const unsigned long long first = 0xFFFFFFFFull - block_max(sm, 0xFFFFFFFFull - (unsigned long long)found);
-    token = first != (unsigned long long)INT_MAX ? (int)first
-                                                 : (int)block_max(sm, (unsigned long long)(last + 1)) - 1;
+    // the draw: the smallest i whose inclusive prefix of surviving weights exceeds u Z'
+    const uint32_t w0 = philox4((uint32_t)pos, (uint32_t)(unsigned long long)seed,
+                                (uint32_t)((unsigned long long)seed >> 32)).x;
+    float zp;
+    token = scan_pick(s_x, sm, V, [tau](float x) { return f2key(x) >= tau; }, [m](float x) { return expf(x - m); },
+                      philox_uniform(w0), zp);
+    if (cut) *cut = RowCut{tau, m, zp};
   }
   return token;
 }
@@ -524,6 +556,8 @@ struct SlotArgs {
   int* g;                    // verify: g[b * S + j] (slot j real iff j < nq)
   long long* ids;            // draft: ids[b * S + j + 1] and next[b] (draft j + 1 real iff j + 1 < nq; else 0)
   long long* next;
+  float* q;                  // draft, optional: the filtered weights of draft step j, q[(b * (S - 1) + j) * vocab + i]
+  float* zq;                 // ... (0 off the survivors) and their total zq[b * (S - 1) + j]
 };
 
 __global__ void __launch_bounds__(kSampleThreads, 1)
@@ -539,8 +573,9 @@ sample_slots_kernel(const __grid_constant__ SlotArgs a) {
     }
     return;
   }
+  RowCut cut;
   const int token = draw_row(s_x, sm, a.s, a.s.logits + ((long long)b * a.kq + x) * a.s.ld, a.emitted[b] + j,
-                             a.lens[b] + j + 1, a.s.seeds[b]);
+                             a.lens[b] + j + 1, a.s.seeds[b], &cut);
   if (threadIdx.x == 0) {
     if (draft) {
       a.ids[(long long)b * a.S + j + 1] = token;
@@ -549,6 +584,120 @@ sample_slots_kernel(const __grid_constant__ SlotArgs a) {
       a.g[(long long)b * a.S + j] = token;
     }
   }
+  if (a.q) {                                        // the draft's distribution at this step, for rejection sampling
+    const long long r = (long long)b * (a.S - 1) + j;
+    float* q = a.q + r * a.s.vocab;
+    for (int i = threadIdx.x; i < a.s.vocab; i += kSampleThreads) {
+      const float v = s_x[i];
+      q[i] = f2key(v) >= cut.tau ? expf(v - cut.m) : 0.f;
+    }
+    if (threadIdx.x == 0) a.zq[r] = cut.zp;
+  }
+}
+
+// ---- rejection-sampling verification (DESIGN.md §4a) ------------------------------------------------------------------
+struct SpecArgs {
+  SlotArgs t;                // the model's slots: logits [B * S, ld] (kq = S, slot0 = 0), g [B * S]; ids, q unused
+  const long long* ids;      // [B * S]: draft j + 1 in slot j + 1
+  const float* q;            // [B, S - 1, vocab] and [B, S - 1]: the draft's weights and totals (sample_slots_kernel)
+  const float* zq;
+  int* acc;                  // [B * S]: draft j + 1 accepted, for j < nq - 1
+  int* last;                 // [B * S]: the round's last token if it ends at slot j: t_j for j < nq - 1, else g_j
+};
+
+// CTA (j, b): draws g_j as sample_slots_kernel does; for a slot with a real draft d = d_{j+1} it also decides d
+// (accepted iff v Q_j(d) < P_j(d), v from Philox word 1 at lens + j + 1) and draws the residual t_j from
+// max(0, P_j - Q_j) with rho_d = 0 (word 2 at lens + j + 1; g_j when no weight is left). No slot depends on another.
+__global__ void __launch_bounds__(kSampleThreads, 1)
+spec_slots_kernel(const __grid_constant__ SpecArgs a) {
+  extern __shared__ float s_x[];                    // [vocab]
+  __shared__ SampleSmem sm;
+  const SlotArgs& t = a.t;
+  const int j = blockIdx.x, b = blockIdx.y, tid = threadIdx.x, V = t.s.vocab;
+  const int nq = t.nq[b];
+  if (t.done[b] || j >= nq) return;
+  const int L = t.lens[b];
+  const long long seed = t.s.seeds[b];
+  const long long o = (long long)b * t.S + j;
+  RowCut cut;
+  const int token = draw_row(s_x, sm, t.s, t.s.logits + o * t.s.ld, t.emitted[b] + j, L + j + 1, seed, &cut);
+  if (j + 1 >= nq) {                                // the last real slot: a round that gets here emits g_j
+    if (tid == 0) {
+      t.g[o] = token;
+      a.last[o] = token;
+    }
+    return;
+  }
+  const long long r = (long long)b * (t.S - 1) + j;
+  const float* wq = a.q + r * V;
+  const float zq = a.zq[r];
+  const long long dl = a.ids[o + 1];
+  const int d = dl >= 0 && dl < V ? (int)dl : -1;
+  const uint4 w = philox4((uint32_t)(L + j + 1), (uint32_t)(unsigned long long)seed,
+                          (uint32_t)((unsigned long long)seed >> 32));
+  if (tid == 0) {
+    const float pd = d >= 0 ? cut_prob(s_x[d], cut) : 0.f;
+    const float qd = d >= 0 && zq > 0.f ? wq[d] / zq : 0.f;
+    t.g[o] = token;
+    a.acc[o] = philox_uniform(w.y) * qd < pd;       // strict: an id with P = 0 is never accepted
+  }
+  __syncthreads();                                  // s_x[d] is read before the row becomes the residual
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const float p = cut_prob(s_x[i], cut), q = zq > 0.f ? wq[i] / zq : 0.f;
+    s_x[i] = i == d ? 0.f : fmaxf(0.f, p - q);
+  }
+  __syncthreads();
+  float zr;
+  const int res = scan_pick(s_x, sm, V, [](float x) { return x > 0.f; }, [](float x) { return x; },
+                            philox_uniform(w.z), zr);
+  if (tid == 0) a.last[o] = res >= 0 ? res : token;
+}
+
+// The checks and set-up shared by adapcc_sample_slots and adapcc_spec_slots; fills `s` or sets the error.
+static int slot_args(const char* who, const float* logits, int ld, int vocab, int B, int kq, int S, int slot0,
+                     bool draft, float temperature, int top_k, float top_p, float min_p, float typical_p,
+                     float epsilon, float eta, const long long* seeds, const int* lens, const int* emitted,
+                     const int* done, const int* nq, int min_new, const int* suppress, int n_suppress, SampleArgs& s) {
+  if (B < 1 || B > 65535 || S < 1 || S > kSlotMaxSlots || kq < 1 || (draft && kq != 1) || slot0 < 0 ||
+      slot0 + kq + (draft ? 1 : 0) > S || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab) {
+    set_error("%s: need 1 <= B <= 65535, 1 <= S <= %d, kq >= 1 (1 for drafts), 0 <= slot0, slot0 + kq (+ 1 for "
+              "drafts) <= S, 1 <= vocab <= %d, ld >= vocab (B=%d S=%d kq=%d slot0=%d vocab=%d ld=%d)", who,
+              kSlotMaxSlots, kSampleMaxVocab, B, S, kq, slot0, vocab, ld);
+    return -1;
+  }
+  if (!(temperature >= 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f) || !(min_p >= 0.f && min_p <= 1.f) ||
+      !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) || !(eta >= 0.f && eta < 1.f)) {
+    set_error("%s: need temperature >= 0, top_k >= 0, 0 < top_p <= 1, 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= "
+              "epsilon < 1, 0 <= eta < 1 (got %g, %d, %g, %g, %g, %g, %g)", who, temperature, top_k, top_p, min_p,
+              typical_p, epsilon, eta);
+    return -1;
+  }
+  if (n_suppress < 0 || n_suppress > kSampleMaxList || (n_suppress && !suppress)) {
+    set_error("%s: a suppress list of at most %d ids (got %d)", who, kSampleMaxList, n_suppress);
+    return -1;
+  }
+  if (!logits || !seeds || !lens || !emitted || !done || !nq) {
+    set_error("%s: null pointer", who);
+    return -1;
+  }
+  s = SampleArgs{logits, ld, vocab, temperature, top_p, top_k, seeds, nullptr, nullptr, min_new, suppress, n_suppress,
+                 nullptr, 0, nullptr, nullptr, nullptr, 1, min_p, typical_p, epsilon, eta,
+                 min_p > 0.f || typical_p < 1.f || epsilon > 0.f || eta > 0.f};
+  return 0;
+}
+
+// the row of a sampling kernel in shared memory, once per device
+template <class Kernel>
+static int allow_row_smem(const char* who, Kernel kernel, std::once_flag* once, cudaError_t* setup) {
+  int dev = 0;
+  CUDA_TRY(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= kOpsMaxDevices) { set_error("%s: device %d out of range", who, dev); return -1; }
+  std::call_once(once[dev], [&] {
+    setup[dev] = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                      kSampleMaxVocab * (int)sizeof(float));
+  });
+  CUDA_TRY(setup[dev]);
+  return 0;
 }
 
 }  // namespace adapcc
@@ -649,51 +798,60 @@ int adapcc_sample_tokens_filtered(const float* logits, int ld, int vocab, int B,
 }
 
 // logits fp32 [B * kq, ld]; seeds int64 [B]; lens, emitted, done, nq int32 [B]; suppress: int32 list (null when
-// empty). Verify draws: g int32 [B * S], ids = next = null. Draft draws (kq = 1: draft j + 1 needs draft j): ids int64
-// [B * S] and next int64 [B], g null.
+// empty). Verify draws: g int32 [B * S], ids = next = q = zq = null. Draft draws (kq = 1: draft j + 1 needs draft j):
+// ids int64 [B * S] and next int64 [B], g null; optionally (temperature > 0) the draft's weights q fp32
+// [B, S - 1, vocab] and totals zq fp32 [B, S - 1] of step slot0, both or neither.
 int adapcc_sample_slots(const float* logits, int ld, int vocab, int B, int kq, int S, int slot0, float temperature,
                         int top_k, float top_p, float min_p, float typical_p, float epsilon, float eta,
                         const long long* seeds, const int* lens, const int* emitted, const int* done, const int* nq,
                         int min_new, const int* suppress, int n_suppress, int* g, long long* ids, long long* next,
-                        void* stream) {
+                        float* q, float* zq, void* stream) {
   const bool draft = ids != nullptr;
-  if (B < 1 || B > 65535 || S < 1 || S > kSlotMaxSlots || kq < 1 || (draft && kq != 1) || slot0 < 0 ||
-      slot0 + kq + (draft ? 1 : 0) > S || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab) {
-    set_error("sample_slots: need 1 <= B <= 65535, 1 <= S <= %d, kq >= 1 (1 for drafts), 0 <= slot0, slot0 + kq (+ 1 "
-              "for drafts) <= S, 1 <= vocab <= %d, ld >= vocab (B=%d S=%d kq=%d slot0=%d vocab=%d ld=%d)", kSlotMaxSlots,
-              kSampleMaxVocab, B, S, kq, slot0, vocab, ld);
+  SampleArgs s;
+  if (slot_args("sample_slots", logits, ld, vocab, B, kq, S, slot0, draft, temperature, top_k, top_p, min_p,
+                typical_p, epsilon, eta, seeds, lens, emitted, done, nq, min_new, suppress, n_suppress, s))
     return -1;
-  }
-  if (!(temperature >= 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f) || !(min_p >= 0.f && min_p <= 1.f) ||
-      !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) || !(eta >= 0.f && eta < 1.f)) {
-    set_error("sample_slots: need temperature >= 0, top_k >= 0, 0 < top_p <= 1, 0 <= min_p <= 1, 0 < typical_p <= 1, "
-              "0 <= epsilon < 1, 0 <= eta < 1 (got %g, %d, %g, %g, %g, %g, %g)", temperature, top_k, top_p, min_p,
-              typical_p, epsilon, eta);
-    return -1;
-  }
-  if (n_suppress < 0 || n_suppress > kSampleMaxList || (n_suppress && !suppress)) {
-    set_error("sample_slots: a suppress list of at most %d ids (got %d)", kSampleMaxList, n_suppress);
-    return -1;
-  }
-  if (!logits || !seeds || !lens || !emitted || !done || !nq || (draft ? (!next || g) : (!g || next))) {
-    set_error("sample_slots: null pointer, or not exactly one of g and (ids, next)");
+  if ((draft ? (!next || g) : (!g || next)) || !q != !zq || (q && (!draft || !(temperature > 0.f)))) {
+    set_error("sample_slots: not exactly one of g and (ids, next), or q / zq without the other, or not with a draft "
+              "draw at temperature > 0");
     return -1;
   }
   static std::once_flag once[kOpsMaxDevices];
   static cudaError_t setup[kOpsMaxDevices];
-  int dev = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= kOpsMaxDevices) { set_error("sample_slots: device %d out of range", dev); return -1; }
-  std::call_once(once[dev], [&] {
-    setup[dev] = cudaFuncSetAttribute(sample_slots_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      kSampleMaxVocab * (int)sizeof(float));
-  });
-  CUDA_TRY(setup[dev]);
-  SampleArgs s{logits, ld, vocab, temperature, top_p, top_k, seeds, nullptr, nullptr, min_new, suppress, n_suppress,
-               nullptr, 0, nullptr, nullptr, nullptr, 1, min_p, typical_p, epsilon, eta,
-               min_p > 0.f || typical_p < 1.f || epsilon > 0.f || eta > 0.f};
-  SlotArgs a{s, B, kq, S, slot0, lens, emitted, done, nq, g, ids, next};
+  if (allow_row_smem("sample_slots", sample_slots_kernel, once, setup)) return -1;
+  SlotArgs a{s, B, kq, S, slot0, lens, emitted, done, nq, g, ids, next, q, zq};
   sample_slots_kernel<<<dim3(kq, B), kSampleThreads, (size_t)vocab * sizeof(float), (cudaStream_t)stream>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// Rejection-sampling verification of a round, one CTA per slot: logits fp32 [B * S, ld]; seeds int64 [B]; lens,
+// emitted, done, nq int32 [B]; suppress int32 list (null when empty); ids int64 [B * S] (the drafts); q fp32
+// [B, S - 1, vocab] and zq fp32 [B, S - 1] (sample_slots' draft weights); g, acc, last int32 [B * S]. temperature > 0.
+int adapcc_spec_slots(const float* logits, int ld, int vocab, int B, int S, float temperature, int top_k, float top_p,
+                      float min_p, float typical_p, float epsilon, float eta, const long long* seeds, const int* lens,
+                      const int* emitted, const int* done, const int* nq, int min_new, const int* suppress,
+                      int n_suppress, const long long* ids, const float* q, const float* zq, int* g, int* acc,
+                      int* last, void* stream) {
+  SampleArgs s;
+  if (slot_args("spec_slots", logits, ld, vocab, B, S, S, 0, false, temperature, top_k, top_p, min_p, typical_p,
+                epsilon, eta, seeds, lens, emitted, done, nq, min_new, suppress, n_suppress, s))
+    return -1;
+  if (S < 2 || !(temperature > 0.f)) {
+    set_error("spec_slots: need S >= 2 and temperature > 0 (got %d, %g)", S, temperature);
+    return -1;
+  }
+  if (!ids || !q || !zq || !g || !acc || !last) {
+    set_error("spec_slots: null pointer");
+    return -1;
+  }
+  static std::once_flag once[kOpsMaxDevices];
+  static cudaError_t setup[kOpsMaxDevices];
+  if (allow_row_smem("spec_slots", spec_slots_kernel, once, setup)) return -1;
+  SlotArgs t{s, B, S, S, 0, lens, emitted, done, nq, g, nullptr, nullptr, nullptr, nullptr};
+  SpecArgs a{t, ids, q, zq, acc, last};
+  spec_slots_kernel<<<dim3(S, B), kSampleThreads, (size_t)vocab * sizeof(float), (cudaStream_t)stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;

@@ -92,7 +92,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0,
                    penalty_alpha: float = 0.0, prompt_lookup_num_tokens: int = 0, min_p: float = 0.0,
                    typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
-                   assistant_model=None, num_assistant_tokens: int = 4) -> List[List[int]]:
+                   assistant_model=None, num_assistant_tokens: int = 4,
+                   assistant_verification: str = "coupled") -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -107,7 +108,10 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff`` go to ``generate`` (the truncation filters of the
     sampler, ``ops/sampling.py``). ``assistant_model`` (a draft model) and ``num_assistant_tokens`` go to ``generate``
     (assisted generation, ``ops/assisted.py``): the replies are the ones drawn without it; with ``num_beams`` or
-    ``penalty_alpha`` it is a ``ValueError``."""
+    ``penalty_alpha`` it is a ``ValueError``. ``assistant_verification="rejection"`` verifies the drafts by rejection
+    sampling instead: each reply token is still drawn from the model's distribution, but not the same draw."""
+    from ..ops.assisted import check_verification
+    check_verification("sample_replies", assistant_verification, assistant_model)
     if assistant_model is not None and (num_beams > 0 or penalty_alpha > 0):
         raise ValueError("sample_replies: assistant_model drafts for sampling and greedy generation only, not with "
                          f"num_beams > 0 or penalty_alpha > 0 (got {num_beams}, {penalty_alpha})")
@@ -138,7 +142,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, min_p=min_p,
                                    typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
                                    assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
-                                   **repeats)
+                                   assistant_verification=assistant_verification, **repeats)
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
 
 
@@ -228,7 +232,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      repetition_penalty: float = 1.0, no_repeat_ngram_size: int = 0, penalty_alpha: float = 0.0,
                      prompt_lookup_num_tokens: int = 0, min_p: float = 0.0, typical_p: float = 1.0,
                      epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model=None,
-                     num_assistant_tokens: int = 4, **sample_kw) -> Dict[str, float]:
+                     num_assistant_tokens: int = 4, assistant_verification: str = "coupled",
+                     **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -253,7 +258,10 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     filters of ``generate``'s sampler (``ops/sampling.py``), on that batched path.
 
     ``assistant_model`` (a draft model) with ``f1``: assisted generation with up to ``num_assistant_tokens`` drafts per
-    round (``ops/assisted.py``), on that batched path; the replies are those of the batched path without it."""
+    round (``ops/assisted.py``), on that batched path; the replies are those of the batched path without it, unless
+    ``assistant_verification="rejection"`` (rejection sampling: replies from the same distribution, other draws)."""
+    from ..ops.assisted import check_verification
+    check_verification("evaluate_dialogs", assistant_verification, assistant_model)
     repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
     lookup = prompt_lookup_num_tokens > 0
     filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
@@ -266,7 +274,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                                     no_repeat_ngram_size=no_repeat_ngram_size, penalty_alpha=penalty_alpha,
                                     prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters,
                                     assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
-                                    **sample_kw)
+                                    assistant_verification=assistant_verification, **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -581,7 +581,8 @@ class GPT2DoubleHeads(nn.Module):
                  no_repeat_ngram_size: int = 0, prompt_lookup_num_tokens: int = 0,
                  max_matching_ngram_size: int = 2, min_p: float = 0.0, typical_p: float = 1.0,
                  epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model: "GPT2DoubleHeads" = None,
-                 num_assistant_tokens: int = 4) -> Tuple[torch.Tensor, torch.Tensor]:
+                 num_assistant_tokens: int = 4,
+                 assistant_verification: str = "coupled") -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -623,12 +624,22 @@ class GPT2DoubleHeads(nn.Module):
         is in ``ops/assisted.py``. On the native path (``B·(k+1)`` at most 64 rows) a round replays one CUDA graph: the
         draft's k + 1 decode steps with k draws (``ops.sample_slots_``), the model on k + 1 slots per row, the LM head,
         the slots' draws and acceptance (``ops.lookup_accept_drawn_``; ``ops.lookup_accept_`` at temperature 0).
-        Afterwards ``self.assist_stats`` holds what ``lookup_stats`` holds for prompt lookup."""
+        Afterwards ``self.assist_stats`` holds what ``lookup_stats`` holds for prompt lookup.
+
+        ``assistant_verification`` is that rule, ``"coupled"``, or ``"rejection"``: HuggingFace's rejection sampling
+        (Leviathan et al. 2023), where a draft d is accepted with probability ``min(1, P(d) / Q(d))`` of the model's
+        and the draft's filtered distributions and a rejection is replaced by a draw from ``max(0, P - Q)``. Each
+        emitted token is then distributed as the model's, acceptance is their overlap rather than the agreement of
+        two draws, and the tokens depend on the draft. On the native path the draft draws also keep their weights and
+        the verify step runs ``ops.spec_slots_`` and ``ops.lookup_accept_drawn_(..., flagged=True)``. At temperature
+        0 both rules are the greedy one."""
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
         check_filter_args("generate", min_p, typical_p, epsilon_cutoff, eta_cutoff)
         filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
+        from ..ops.assisted import check_verification
+        check_verification("generate", assistant_verification, assistant_model)
         if assistant_model is not None:
             from ..ops import LOOKUP_MAX_TOKENS
             from ..ops.assisted import check_assist_args
@@ -636,7 +647,8 @@ class GPT2DoubleHeads(nn.Module):
                               prompt_lookup_num_tokens, repetition_penalty, no_repeat_ngram_size)
             return self._generate_assisted(assistant_model, int(num_assistant_tokens), input_ids, lengths,
                                            token_type_ids, reply_type, max_new_tokens, temperature, top_k, top_p,
-                                           stop_ids, suppress_ids, min_new_tokens, seed, filters)
+                                           stop_ids, suppress_ids, min_new_tokens, seed, filters,
+                                           assistant_verification == "rejection" and temperature > 0)
         K = prompt_lookup_num_tokens
         if K != 0:
             from ..ops import LOOKUP_MAX_NGRAM, LOOKUP_MAX_TOKENS
@@ -855,8 +867,9 @@ class GPT2DoubleHeads(nn.Module):
 
     def _generate_assisted(self, draft: "GPT2DoubleHeads", K: int, input_ids, lengths, token_type_ids, reply_type,
                            max_new_tokens, temperature, top_k, top_p, stop_ids, suppress_ids, min_new_tokens, seed,
-                           filters) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``generate`` with ``draft`` proposing up to ``K`` tokens per row and round (``ops/assisted.py``)."""
+                           filters, rejection: bool) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``generate`` with ``draft`` proposing up to ``K`` tokens per row and round (``ops/assisted.py``), verified
+        by coupled draws or, with ``rejection`` (temperature > 0), by rejection sampling."""
         B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens, 1.0, 0,
             num_beams=K + 1, rows_name="verify rows (batch x (num_assistant_tokens + 1))")
@@ -876,7 +889,7 @@ class GPT2DoubleHeads(nn.Module):
         dcache = KVCache(dc.n_layer, B, dc.n_head, t_max + K, dc.n_embd // dc.n_head, draft.wte.weight.dtype, dev)
         draft.hidden(input_ids, token_type_ids, cache=dcache, lengths=lengths)
         if not native:                              # CPU / not bf16: the definition on fp32 PyTorch logits
-            from ..ops.assisted import assist_round, draw_slots
+            from ..ops.assisted import assist_round, draw_slots, spec_slots
             from ..ops.lookup import lookup_accept
             head, dhead = weight.float(), draft.wte.weight.float()
             seq = torch.zeros(B, t_max, dtype=torch.int32)
@@ -894,26 +907,34 @@ class GPT2DoubleHeads(nn.Module):
                 ids, pos, nq, d_in, d_pos = assist_round(seq, lens, emitted, done, K, n, dc.n_positions)
                 dcache.lens.copy_(lens)
                 ids = ids.view(B, S)
+                qlogits = []
                 for j in range(S):
                     hd = draft._blocks(draft._embed(d_in.to(dev), tt_new, d_pos[j].to(dev)), dcache)
                     dcache.lens.add_(1)
                     if j < K:
-                        d = draw_slots(draft.lm_logits(hd, dhead), *scal, lens, emitted, done, nq, j, True, **kw)
+                        qlogits.append(draft.lm_logits(hd, dhead))
+                        d = draw_slots(qlogits[-1], *scal, lens, emitted, done, nq, j, True, **kw)
                         d_in = torch.from_numpy(d[:, 0]).clamp(min=0)
                         ids[:, j + 1] = d_in
                 ids = ids.reshape(-1)
                 cache.lens.copy_(lens)
                 hv = self._verify_hidden(ids.to(dev), pos.to(dev), tt_v, VerifyKV(cache, S, nq.to(dev)))
-                g = draw_slots(self.lm_logits(hv, head), *scal, lens, emitted, done, nq, **kw)
-                lookup_accept(None, V, ids, nq, seq, lens, emitted, done, tokens, steps, stop_ids=stop_ids, drawn=g)
+                acc = None
+                if rejection:
+                    _, acc, g = spec_slots(self.lm_logits(hv, head), torch.stack(qlogits, 1), *scal, lens, emitted,
+                                           done, nq, ids, **kw)
+                else:
+                    g = draw_slots(self.lm_logits(hv, head), *scal, lens, emitted, done, nq, **kw)
+                lookup_accept(None, V, ids, nq, seq, lens, emitted, done, tokens, steps, stop_ids=stop_ids, drawn=g,
+                              accepted=acc)
                 rounds += 1
             self.assist_stats = {"emitted": emitted, "steps": steps, "replays": rounds}
             return tokens.to(dev), (tokens >= 0).sum(1).to(dev)
 
         from ..ops import (AssistState, assist_round_, decode_attention_work_numel, lm_head_logits_, lookup_accept_,
-                           lookup_accept_drawn_, sample_slots_)
+                           lookup_accept_drawn_, sample_slots_, spec_slots_)
 
-        st = AssistState(B, K, n, t_max, dev)
+        st = AssistState(B, K, n, t_max, dev, V if rejection else 0)
         st.seq[:, :T] = input_ids
         dweight = draft.wte.weight
         logits = torch.empty(B * S, weight.shape[0], dtype=torch.float32, device=dev)
@@ -924,6 +945,9 @@ class GPT2DoubleHeads(nn.Module):
         def accept(lg, first=False):
             if temperature == 0:                    # greedy verification: the arg-max kernel of prompt lookup
                 lookup_accept_(lg, V, st, cache.lens, min_new_tokens, sup, stop, count=not first)
+            elif rejection and not first:
+                spec_slots_(lg, V, temperature, top_k, top_p, seeds, st, cache.lens, min_new_tokens, sup, **filters)
+                lookup_accept_drawn_(st, cache.lens, stop, flagged=True)
             else:
                 sample_slots_(lg, *draw, 0, min_new_tokens, sup, **filters)
                 lookup_accept_drawn_(st, cache.lens, stop, count=not first, first=first)
@@ -945,7 +969,8 @@ class GPT2DoubleHeads(nn.Module):
                     dcache.lens.add_(1)
                     if j < K:
                         lm_head_logits_(hd, dweight, dlogits)
-                        sample_slots_(dlogits, *draw, j, min_new_tokens, sup, draft=True, **filters)
+                        sample_slots_(dlogits, *draw, j, min_new_tokens, sup, draft=True, weights=rejection,
+                                      **filters)
                 return self._verify_hidden(st.ids, st.pos, tt_v, verify)
 
             def head_and_accept(hv):

@@ -72,9 +72,11 @@ def _lib():
                                              + [c_void_p] * 4 + [c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p])
         lib.adapcc_lookup_draft.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 7
         lib.adapcc_sample_slots.argtypes = ([c_void_p] + [c_int] * 6 + [c_float, c_int] + [c_float] * 5
-                                            + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 4)
+                                            + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 6)
+        lib.adapcc_spec_slots.argtypes = ([c_void_p] + [c_int] * 4 + [c_float, c_int] + [c_float] * 5
+                                          + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 7)
         lib.adapcc_lookup_accept_drawn.argtypes = ([c_int] * 3 + [c_void_p, c_int] + [c_void_p] * 4 + [c_int]
-                                                   + [c_void_p] * 4 + [c_int, c_void_p, c_void_p])
+                                                   + [c_void_p] * 4 + [c_int, c_void_p, c_void_p, c_void_p])
         lib.adapcc_assist_round.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 10
         _bound = True
     return lib
@@ -857,22 +859,36 @@ def lookup_draft_(state: LookupState, lens: torch.Tensor) -> None:
 class AssistState(LookupState):
     """A ``LookupState`` for assisted generation, where a draft model proposes the drafts (``ops/assisted.py``), plus
     the draft's input buffers: ``d_in`` int64 [B] the token the draft consumes next and ``d_pos`` int64 [k+1, B] its
-    positions at each of its k + 1 steps of a round (``lens[b] + j`` clamped to the model's ``n_positions - 1``)."""
+    positions at each of its k + 1 steps of a round (``lens[b] + j`` clamped to the model's ``n_positions - 1``).
 
-    def __init__(self, batch: int, k: int, max_new: int, t_max: int, device):
+    ``vocab > 0`` adds the buffers of rejection-sampling verification: ``q`` fp32 [B, k, vocab] and ``zq`` fp32 [B, k]
+    the draft's filtered weights at each draft step and their totals (``sample_slots_(..., weights=True)``), and
+    ``acc`` int32 [B·(k+1)] the accepted flags and ``last`` int32 [B·(k+1)] the round's last token if it ends at slot
+    j (``spec_slots_``). Otherwise they are None."""
+
+    def __init__(self, batch: int, k: int, max_new: int, t_max: int, device, vocab: int = 0):
         super().__init__(batch, k, max_new, t_max, 1, device)
         self.d_in = torch.zeros(self.batch, dtype=torch.int64, device=device)
         self.d_pos = torch.zeros(self.k + 1, self.batch, dtype=torch.int64, device=device)
+        self.q = self.zq = self.acc = self.last = None
+        if int(vocab) > 0:
+            B, K = self.batch, self.k
+            self.q = torch.zeros(B, K, int(vocab), dtype=torch.float32, device=device)
+            self.zq = torch.zeros(B, K, dtype=torch.float32, device=device)
+            self.acc = torch.zeros(B * (K + 1), dtype=torch.int32, device=device)
+            self.last = torch.zeros(B * (K + 1), dtype=torch.int32, device=device)
 
     def tensors(self):
-        """Every device tensor of the state, the draft's buffers included."""
-        return super().tensors() + (self.d_in, self.d_pos)
+        """Every device tensor of the state, the draft's and rejection sampling's buffers included."""
+        return super().tensors() + tuple(t for t in (self.d_in, self.d_pos, self.q, self.zq, self.acc, self.last)
+                                         if t is not None)
 
 
 def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int, top_p: float, seeds: torch.Tensor,
                   state: LookupState, lens: torch.Tensor, slot0: int = 0, min_new: int = 0,
                   suppress_ids: Optional[torch.Tensor] = None, draft: bool = False, min_p: float = 0.0,
-                  typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> None:
+                  typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
+                  weights: bool = False) -> None:
     """The draws of speculative decoding, one CTA per slot, on the device. ``logits`` fp32 [B·kq, ld] (the first
     ``vocab`` columns used) holds ``kq`` slots per row; its slot x of row b is slot ``j = slot0 + x``, drawn as
     ``sample_tokens_`` draws a row (the same bits) with the Philox counter ``lens[b] + j + 1`` (``lens`` int32 [B]) and
@@ -882,7 +898,9 @@ def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: i
     j]``; pad slots are left alone. Draft draws (``draft=True``, an ``AssistState``, one logits row per row): the token
     is draft j + 1, real iff
     ``j + 1 < state.nq[b]``; it goes to ``state.ids[b·(k+1) + j + 1]`` and ``state.d_in[b]`` (0 for a pad draft or a
-    done row). No host sync."""
+    done row). With ``weights`` (temperature > 0, an ``AssistState`` made with this ``vocab``), a real draft also
+    writes the weights ``exp(x_i - m)`` of the ids its draw kept (0 elsewhere) to ``state.q[b, j]`` and their total Z'
+    to ``state.zq[b, j]``; the tokens are the same bits either way. No host sync."""
     def bad(msg):
         raise ValueError(f"sample_slots_: {msg}")
 
@@ -901,13 +919,9 @@ def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: i
         bad(f"draft draws take one logits row per row (draft j + 1 depends on draft j), got {kq}")
     if not 0 <= int(slot0) or int(slot0) + kq + int(draft) > S:
         bad(f"slots {slot0}..{int(slot0) + kq - 1} do not fit {S} slots per row (draft: {draft})")
-    if not 1 <= vocab <= min(logits.shape[1], SAMPLE_MAX_VOCAB):
-        bad(f"vocab must be in [1, min(ld = {logits.shape[1]}, {SAMPLE_MAX_VOCAB})], got {vocab}")
-    for name, t, dt in (("seeds", seeds, torch.int64), ("lens", lens, torch.int32)):
-        if t.dtype != dt or not t.is_contiguous() or t.numel() != B:
-            bad(f"{name} must be a contiguous {dt} tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
-    if int(min_new) < 0:
-        bad(f"min_new must be >= 0, got {min_new}")
+    _check_slot_inputs(bad, logits, vocab, seeds, lens, B, min_new)
+    if weights and not (draft and temperature > 0 and state.q is not None and state.q.shape[2] == vocab):
+        bad(f"weights need a draft draw at temperature > 0 and an AssistState made with vocab = {vocab}")
     sup, n_sup = _id_list("sample_slots_", "suppress_ids", suppress_ids, SAMPLE_MAX_IDS)
     _same_device("sample_slots_", logits.device, state.tensors() + (seeds, lens, suppress_ids))
     _ck(_lib().adapcc_sample_slots(_ptr(logits), logits.stride(0), int(vocab), B, kq, S, int(slot0),
@@ -915,13 +929,67 @@ def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: i
                                    float(epsilon_cutoff), float(eta_cutoff), _ptr(seeds), _ptr(lens),
                                    _ptr(state.emitted), _ptr(state.done), _ptr(state.nq), int(min_new), sup, n_sup,
                                    None if draft else _ptr(state.g), _ptr(state.ids) if draft else None,
-                                   _ptr(state.d_in) if draft else None, _stream()), "sample_slots")
+                                   _ptr(state.d_in) if draft else None, _ptr(state.q if weights else None),
+                                   _ptr(state.zq if weights else None), _stream()), "sample_slots")
+
+
+def _check_slot_inputs(bad, logits: torch.Tensor, vocab: int, seeds: torch.Tensor, lens: torch.Tensor, B: int,
+                       min_new: int) -> None:
+    """The checks ``sample_slots_`` and ``spec_slots_`` share on their vocabulary, seeds, lengths and ``min_new``."""
+    if not 1 <= vocab <= min(logits.shape[1], SAMPLE_MAX_VOCAB):
+        bad(f"vocab must be in [1, min(ld = {logits.shape[1]}, {SAMPLE_MAX_VOCAB})], got {vocab}")
+    for name, t, dt in (("seeds", seeds, torch.int64), ("lens", lens, torch.int32)):
+        if t.dtype != dt or not t.is_contiguous() or t.numel() != B:
+            bad(f"{name} must be a contiguous {dt} tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if int(min_new) < 0:
+        bad(f"min_new must be >= 0, got {min_new}")
+
+
+def spec_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int, top_p: float, seeds: torch.Tensor,
+                state: AssistState, lens: torch.Tensor, min_new: int = 0, suppress_ids: Optional[torch.Tensor] = None,
+                min_p: float = 0.0, typical_p: float = 1.0, epsilon_cutoff: float = 0.0,
+                eta_cutoff: float = 0.0) -> None:
+    """Rejection-sampling verification of a round on the device (``ops/assisted.py``), one CTA per slot. ``logits``
+    fp32 [B·(k+1), ld] holds the model's slots; ``state`` is an ``AssistState`` made with this ``vocab``, whose
+    ``q`` / ``zq`` hold the round's draft weights (``sample_slots_(..., weights=True)``) and ``ids`` the drafts. For
+    every real slot j of a live row it writes ``state.g[b·(k+1) + j]``, the draw ``sample_slots_`` makes (the same
+    bits). For a slot with a real draft (``j + 1 < state.nq[b]``) it writes ``state.acc`` (draft j + 1 accepted: ``v
+    Q_j(d) < P_j(d)``) and ``state.last`` the residual draw t_j; for the last real slot ``state.last`` is g_j. Then
+    ``lookup_accept_drawn_(..., flagged=True)`` emits the round. Needs temperature > 0. No host sync."""
+    def bad(msg):
+        raise ValueError(f"spec_slots_: {msg}")
+
+    if not isinstance(state, AssistState) or state.q is None:
+        bad(f"state must be an AssistState made with a vocab, got {type(state).__name__}")
+    if not temperature > 0 or not top_k >= 0 or not 0 < top_p <= 1:
+        bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
+    from .sampling import check_filter_args
+
+    check_filter_args("spec_slots_", min_p, typical_p, epsilon_cutoff, eta_cutoff)
+    B, S = state.batch, state.k + 1
+    if (logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1
+            or logits.shape[0] != B * S):
+        bad(f"logits must be fp32 [{B * S}, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
+    _check_slot_inputs(bad, logits, vocab, seeds, lens, B, min_new)
+    if state.q.shape[2] != vocab:
+        bad(f"the state's draft weights have {state.q.shape[2]} columns, not vocab = {vocab}")
+    sup, n_sup = _id_list("spec_slots_", "suppress_ids", suppress_ids, SAMPLE_MAX_IDS)
+    _same_device("spec_slots_", logits.device, state.tensors() + (seeds, lens, suppress_ids))
+    _ck(_lib().adapcc_spec_slots(_ptr(logits), logits.stride(0), int(vocab), B, S, float(temperature), int(top_k),
+                                 float(top_p), float(min_p), float(typical_p), float(epsilon_cutoff),
+                                 float(eta_cutoff), _ptr(seeds), _ptr(lens), _ptr(state.emitted), _ptr(state.done),
+                                 _ptr(state.nq), int(min_new), sup, n_sup, _ptr(state.ids), _ptr(state.q),
+                                 _ptr(state.zq), _ptr(state.g), _ptr(state.acc), _ptr(state.last), _stream()),
+        "spec_slots")
 
 
 def lookup_accept_drawn_(state: LookupState, lens: torch.Tensor, stop_ids: Optional[torch.Tensor] = None,
-                         count: bool = True, first: bool = False) -> None:
+                         count: bool = True, first: bool = False, flagged: bool = False) -> None:
     """``lookup_accept_``'s acceptance on the tokens ``state.g`` already holds (``sample_slots_``'s verify draws), with
-    no arg-max: the same kernel and rule. ``first``: one slot per row (the prefill's draw, ``state.nq`` all 1)."""
+    no arg-max: the same kernel and rule. ``first``: one slot per row (the prefill's draw, ``state.nq`` all 1).
+    ``flagged`` (rejection sampling, after ``spec_slots_``): the row emits the drafts ``state.acc`` accepts, then
+    ``state.last`` at the first slot whose draft is rejected (or the last real slot), with the same stop and length
+    rules."""
     def bad(msg):
         raise ValueError(f"lookup_accept_drawn_: {msg}")
 
@@ -930,12 +998,16 @@ def lookup_accept_drawn_(state: LookupState, lens: torch.Tensor, stop_ids: Optio
     B, S = state.batch, state.k + 1
     if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
         bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
+    if flagged and (first or getattr(state, "acc", None) is None):
+        bad("flagged acceptance needs an AssistState made with a vocab, and not the first slot")
     stop, n_stop = _id_list("lookup_accept_drawn_", "stop_ids", stop_ids, LOOKUP_MAX_IDS)
     _same_device("lookup_accept_drawn_", lens.device, state.tensors() + (stop_ids,))
-    _ck(_lib().adapcc_lookup_accept_drawn(B, S, 1 if first else S, stop, n_stop, _ptr(state.g), _ptr(state.ids),
+    _ck(_lib().adapcc_lookup_accept_drawn(B, S, 1 if first else S, stop, n_stop,
+                                          _ptr(state.last if flagged else state.g), _ptr(state.ids),
                                           _ptr(state.nq), _ptr(state.seq), state.t_max, _ptr(lens),
                                           _ptr(state.emitted), _ptr(state.done), _ptr(state.tokens), state.max_new,
-                                          _ptr(state.steps if count else None), _stream()), "lookup_accept_drawn")
+                                          _ptr(state.steps if count else None), _ptr(state.acc if flagged else None),
+                                          _stream()), "lookup_accept_drawn")
 
 
 def assist_round_(state: AssistState, lens: torch.Tensor, d_lens: torch.Tensor, n_pos: int) -> None:

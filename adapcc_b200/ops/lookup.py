@@ -69,19 +69,22 @@ def greedy_token(logits, step: int, min_new: int = 0, suppress_ids: Sequence[int
 
 
 def accept_row(g: Sequence[int], drafts: Sequence[int], emitted: int, max_new: int,
-               stop_ids: Sequence[int] = ()) -> Tuple[List[int], bool]:
+               stop_ids: Sequence[int] = (), accepted: Sequence[bool] = None) -> Tuple[List[int], bool]:
     """Step 3 for one row: the slots' arg-maxes ``g`` (one per real slot) and the drafts (one fewer) -> the emitted ids
-    (a stop id included, as the last one) and whether the row is now done."""
+    (a stop id included, as the last one) and whether the row is now done. ``accepted`` (rejection sampling,
+    ``ops/assisted.py``): per draft whether it is accepted, in place of "equals the token just emitted"; the row emits
+    the leading accepted drafts, then ``g[a]`` (the token a round that ends at slot a emits)."""
     stop = set(int(s) for s in stop_ids)
     out: List[int] = []
     e = int(emitted)
     for j, t in enumerate(g):
-        t = int(t)
+        ok = accepted is not None and j + 1 < len(g) and bool(accepted[j])
+        t = int(drafts[j]) if ok else int(t)
         out.append(t)
         e += 1
         if t in stop or e >= max_new:
             return out, True
-        if j + 1 < len(g) and int(drafts[j]) != t:
+        if (not ok) if accepted is not None else (j + 1 < len(g) and int(drafts[j]) != t):
             break
     return out, False
 
@@ -113,13 +116,15 @@ def lookup_draft(seq: torch.Tensor, lens: torch.Tensor, emitted: torch.Tensor, d
 def lookup_accept(logits: torch.Tensor, vocab: int, ids: torch.Tensor, nq: torch.Tensor, seq: torch.Tensor,
                   lens: torch.Tensor, emitted: torch.Tensor, done: torch.Tensor, tokens: torch.Tensor,
                   steps: torch.Tensor = None, min_new: int = 0, suppress_ids: Sequence[int] = (),
-                  stop_ids: Sequence[int] = (), drawn=None) -> None:
+                  stop_ids: Sequence[int] = (), drawn=None, accepted=None) -> None:
     """``lookup_accept_`` for a batch on the host, in place on the CPU tensors ``seq`` [B, t_max], ``lens``,
     ``emitted``, ``done`` [B], ``tokens`` [B, max_new] (-1 where nothing is written) and ``steps`` [B] (verify steps
     per live row; None: not counted). ``logits`` [B·ls, >= vocab] holds ``ls`` slots per row (1 for the prefill's
     logits, k + 1 for a verify step), ``ids`` [B·(k+1)] the step's input and ``nq`` [B] its real slots (at most
     ``ls`` are used). ``drawn`` [B, ls] (``lookup_accept_drawn_``): the slots' tokens, already drawn
-    (``ops/assisted.py``), in place of the arg-maxes of ``logits`` (which may then be None)."""
+    (``ops/assisted.py``), in place of the arg-maxes of ``logits`` (which may then be None). ``accepted`` [B, ls]
+    (``lookup_accept_drawn_(..., flagged=True)``): per slot whether its draft is accepted (``accept_row``), with
+    ``drawn`` holding each slot's last token."""
     B, t_max = seq.shape
     ls = logits.shape[0] // B if drawn is None else drawn.shape[1]
     S = ids.numel() // B
@@ -134,7 +139,8 @@ def lookup_accept(logits: torch.Tensor, vocab: int, ids: torch.Tensor, nq: torch
         n = max(0, min(int(nq[b]), ls))
         g = ([int(drawn[b, j]) for j in range(n)] if drawn is not None
              else [greedy_token(rows[b, j], e + j, min_new, suppress_ids) for j in range(n)])
-        out, fin = accept_row(g, ids[b, 1:n].tolist(), e, max_new, stop_ids)
+        out, fin = accept_row(g, ids[b, 1:n].tolist(), e, max_new, stop_ids,
+                              None if accepted is None else [bool(accepted[b, j]) for j in range(n)])
         for i, t in enumerate(out):
             if L + 1 + i < t_max:
                 seq[b, L + 1 + i] = t

@@ -50,10 +50,11 @@ def philox4x32_10(counter: Sequence[int], key: Sequence[int]) -> Tuple[int, int,
     return c0, c1, c2, c3
 
 
-def uniform(seed: int, pos: int) -> float:
-    """The draw of a row: ``(w0 >> 8) * 2^-24`` (exact in fp32)."""
+def uniform(seed: int, pos: int, word: int = 0) -> float:
+    """``(w >> 8) * 2^-24`` (exact in fp32) for output word ``word`` of Philox4x32-10 at counter ``(pos, 0, 0, 0)``:
+    word 0 is the draw of a row; rejection-sampling verification (``ops/assisted.py``) uses words 1 and 2."""
     seed = int(seed) & 0xFFFFFFFFFFFFFFFF
-    return (philox4x32_10((pos, 0, 0, 0), (seed & _MASK, seed >> 32))[0] >> 8) * 2.0 ** -24
+    return (philox4x32_10((pos, 0, 0, 0), (seed & _MASK, seed >> 32))[word] >> 8) * 2.0 ** -24
 
 
 def top_filtering(logits: torch.Tensor, top_k: int = 0, top_p: float = 0.9, threshold: float = -float("inf")) -> torch.Tensor:

@@ -64,6 +64,9 @@ def main():
                         "verifies (assisted generation); the replies are those drawn without it, through the batched path")
     p.add_argument("--num_assistant_tokens", type=int, default=4,
                    help="f1 with --assistant_checkpoint: draft tokens per verify step")
+    p.add_argument("--assistant_verification", choices=("coupled", "rejection"), default="coupled",
+                   help="f1 with --assistant_checkpoint: coupled draws (the replies drawn without the draft) or "
+                        "rejection sampling (replies from the same distribution, more drafts accepted)")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -82,6 +85,7 @@ def main():
             kw["assistant_model"] = load_model_from_checkpoint(
                 a.assistant_checkpoint, a.device, torch.bfloat16 if a.device.startswith("cuda") else None)[0]
             kw["num_assistant_tokens"] = a.num_assistant_tokens
+            kw["assistant_verification"] = a.assistant_verification
     res = evaluate_dialogs(model, tok, raw["valid"], a.eval_type, a.max_history, a.max_examples, a.device, a.seed,
                            a.batch_size, a.num_beams, **kw)
     print(json.dumps(res))

@@ -15,8 +15,9 @@ the drafts bound it instead:
 * ``other``: an independently seeded two-block model, whose acceptance is about zero: the pure overhead.
 
 B = 1 / 8 rows, prompts of 128 / 512 random tokens, k = 2 / 4 / 7, greedy (temperature 0) and sampled (temperature 0.7,
-top-p 0.9). Plain and assisted calls are alternated in one process; medians of ``--reps`` calls after one warm-up call
-per configuration and length.
+top-p 0.9). Sampled assisted generation runs under both verification rules (``verification``: ``coupled`` draws or
+``rejection`` sampling); greedy rows are ``coupled`` (the rules agree at temperature 0). Plain and assisted calls are
+alternated in one process; medians of ``--reps`` calls after one warm-up call per configuration and length.
 
 Usage: ``python tools/assist_bench.py [--reps 3]``
 """
@@ -37,6 +38,7 @@ NEW_TOKENS = 64
 LONG_TOKENS = 192
 KS = (2, 4, 7)
 MODES = {"greedy": dict(temperature=0.0), "sampled": dict(temperature=0.7, top_p=0.9)}
+RULES = {"greedy": ("coupled",), "sampled": ("coupled", "rejection")}
 
 
 def _gpu_info():
@@ -82,12 +84,13 @@ def main():
         for T in (128, 512):
             prompt = torch.randint(0, model.cfg.vocab_size, (B, T), device="cuda", generator=g)
             for mode, kw in MODES.items():
-                cfgs = [None] + [(name, k) for name in drafts for k in KS]
+                cfgs = [None] + [(name, k, rule) for name in drafts for k in KS for rule in RULES[mode]]
                 times = {(c, m): [] for c in cfgs for m in (NEW_TOKENS, LONG_TOKENS)}
                 per_step = {c: [] for c in cfgs}
                 for rep in range(args.reps + 1):                 # rep 0 warms every configuration up
                     for c in cfgs:
-                        extra = {} if c is None else dict(assistant_model=drafts[c[0]], num_assistant_tokens=c[1])
+                        extra = {} if c is None else dict(assistant_model=drafts[c[0]], num_assistant_tokens=c[1],
+                                                          assistant_verification=c[2])
                         for m in (NEW_TOKENS, LONG_TOKENS):
                             ms = _timed(lambda: model.generate(prompt, max_new_tokens=m, seed=1, **kw, **extra))
                             if rep:
@@ -103,7 +106,7 @@ def main():
                 plain_e2e, plain_steady = cost(None)
                 for c in cfgs[1:]:
                     e2e, steady = cost(c)
-                    rows.append({"B": B, "T": T, "mode": mode, "draft": c[0], "k": c[1],
+                    rows.append({"B": B, "T": T, "mode": mode, "draft": c[0], "k": c[1], "verification": c[2],
                                  "plain_e2e_ms_per_token": round(plain_e2e, 4), "e2e_ms_per_token": round(e2e, 4),
                                  "plain_steady_ms_per_token": round(plain_steady, 4),
                                  "steady_ms_per_token": round(steady, 4),
