@@ -1,7 +1,10 @@
-// Prompt-lookup speculative decoding for greedy GPT-2 generation on the device, so a verify step is one CUDA graph
-// replay: the model on k + 1 slots per row, the LM head, then acceptance and the next drafts. The definition is in
-// ops/lookup.py and DESIGN.md §4a. The slots' attention is adapcc_verify_attn in ops_decode.cu; this file accepts
-// the drafts and finds the next ones.
+// Speculative decoding for GPT-2 generation on the device, so a verify step is one CUDA graph replay: the drafts, the
+// model on k + 1 slots per row, the LM head, then the slots' tokens and acceptance. The definitions are in
+// ops/lookup.py, ops/assisted.py and DESIGN.md §4a. The slots' attention is adapcc_verify_attn in ops_decode.cu; this
+// file finds prompt lookup's drafts, sets up a draft model's round, takes the arg-max of the slots (greedy
+// verification) and accepts the drafts. adapcc_lookup_argmax launches lk_argmax and adapcc_lookup_accept lk_accept, so
+// acceptance runs the same way on arg-maxes and on the draws of adapcc_sample_slots / adapcc_spec_slots
+// (ops_sample.cu).
 //
 //   lk_argmax      : grid (slots, B), 512 threads: each real slot's arg-max (topk_rows.cuh with N = 1, ties to the lower
 //                    id); suppress_ids are removed while emitted[b] + j < min_new.
@@ -16,8 +19,7 @@
 //   lk_round       : one thread per row, assisted generation (a draft model proposes the drafts, ops/assisted.py): the
 //                    start of a round from the target's state alone: slot 0, positions, real-slot count, the draft's
 //                    first input and positions, and the draft cache's lengths. The drafts are drawn by
-//                    sample_slots_kernel (ops_sample.cu), and adapcc_lookup_accept_drawn runs lk_accept on the slots'
-//                    tokens that kernel drew.
+//                    sample_slots_kernel (ops_sample.cu).
 //
 // Every grid depends on B, k and t_max only, so one capture serves every step. A row's results depend only on its own
 // logits, cache and sequence.
@@ -212,42 +214,34 @@ using namespace adapcc;
 
 extern "C" {
 
-// logits fp32 [B * ls, ld]; suppress / stop int32 lists (null when empty); g int32, ids int64 [B * kq]; nq, seq
-// [B, t_max], lens, emitted, done int32; tokens int64 [B, max_new]; steps int32 [B] or null
-int adapcc_lookup_accept(const float* logits, int ld, int vocab, int B, int kq, int ls, int min_new,
-                         const int* suppress, int n_suppress, const int* stop, int n_stop, int* g, const long long* ids,
-                         const int* nq, int* seq, int t_max, int* lens, int* emitted, int* done, long long* tokens,
-                         int max_new, int* steps, void* stream) {
-  if (B < 1 || B > 65535 || kq < 1 || kq > kLkMaxSlots || (ls != 1 && ls != kq) || vocab < 1 || ld < vocab ||
-      t_max < 1 || max_new < 1) {
-    set_error("lookup_accept: need 1 <= B <= 65535, 1 <= kq <= %d, ls in {1, kq}, 1 <= vocab <= ld, t_max, max_new "
-              ">= 1 (B=%d kq=%d ls=%d vocab=%d ld=%d)", kLkMaxSlots, B, kq, ls, vocab, ld);
+// lk_argmax alone: logits fp32 [B * ls, ld]; suppress int32 list (null when empty); g int32 [B * kq]; nq, emitted,
+// done int32 [B]
+int adapcc_lookup_argmax(const float* logits, int ld, int vocab, int B, int kq, int ls, int min_new,
+                         const int* suppress, int n_suppress, int* g, const int* nq, const int* emitted,
+                         const int* done, void* stream) {
+  if (B < 1 || B > 65535 || kq < 1 || kq > kLkMaxSlots || (ls != 1 && ls != kq) || vocab < 1 || ld < vocab) {
+    set_error("lookup_argmax: need 1 <= B <= 65535, 1 <= kq <= %d, ls in {1, kq}, 1 <= vocab <= ld (B=%d kq=%d ls=%d "
+              "vocab=%d ld=%d)", kLkMaxSlots, B, kq, ls, vocab, ld);
     return -1;
   }
-  if (n_suppress < 0 || n_suppress > kLkMaxIds || (n_suppress && !suppress) || n_stop < 0 || n_stop > kLkMaxIds ||
-      (n_stop && !stop)) {
-    set_error("lookup_accept: at most %d suppressed and %d stop ids (got %d, %d)", kLkMaxIds, kLkMaxIds, n_suppress,
-              n_stop);
+  if (n_suppress < 0 || n_suppress > kLkMaxIds || (n_suppress && !suppress)) {
+    set_error("lookup_argmax: at most %d suppressed ids (got %d)", kLkMaxIds, n_suppress);
     return -1;
   }
-  if (!logits || !g || !ids || !nq || !seq || !lens || !emitted || !done || !tokens) {
-    set_error("lookup_accept: null pointer");
+  if (!logits || !g || !nq || !emitted || !done) {
+    set_error("lookup_argmax: null pointer");
     return -1;
   }
   const size_t bits = n_suppress > 0 && min_new > 0 ? (size_t)(vocab + 31) / 32 * sizeof(uint32_t) : 0;
   if (bits > 200 * 1024) {
-    set_error("lookup_accept: suppression needs vocab <= %d (got %d)", 200 * 1024 * 8, vocab);
+    set_error("lookup_argmax: suppression needs vocab <= %d (got %d)", 200 * 1024 * 8, vocab);
     return -1;
   }
   if (bits > 48 * 1024)
     CUDA_TRY(cudaFuncSetAttribute(lk_argmax_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bits));
-  AcceptArgs a{logits, ld, vocab, B, kq, ls, emitted, min_new, suppress, n_suppress, g, ids, nq, seq, t_max, lens,
-               emitted, done, stop, n_stop, tokens, max_new, steps, nullptr};
-  cudaStream_t s = (cudaStream_t)stream;
-  lk_argmax_kernel<<<dim3(ls, B), kBeamThreads, bits, s>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  lk_accept_kernel<<<(B + 63) / 64, 64, 0, s>>>(a);
+  AcceptArgs a{logits, ld, vocab, B, kq, ls, emitted, min_new, suppress, n_suppress, g, nullptr, nq, nullptr, 0,
+               nullptr, nullptr, const_cast<int*>(done), nullptr, 0, nullptr, 0, nullptr, nullptr};
+  lk_argmax_kernel<<<dim3(ls, B), kBeamThreads, bits, (cudaStream_t)stream>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;
@@ -273,27 +267,27 @@ int adapcc_lookup_draft(const int* seq, int t_max, int B, int kq, int ngram, int
   return 0;
 }
 
-// lk_accept alone on g already drawn by adapcc_sample_slots: g int32, ids int64 [B * kq]; nq, lens, emitted, done
-// int32 [B]; seq int32 [B, t_max]; stop int32 list (null when empty); tokens int64 [B, max_new]; steps int32 [B] or
-// null; acc int32 [B * kq] or null: the accepted flags and last tokens (g) of adapcc_spec_slots, null for the rule
-// that a draft is accepted when it equals the token just emitted
-int adapcc_lookup_accept_drawn(int B, int kq, int ls, const int* stop, int n_stop, const int* g, const long long* ids,
-                               const int* nq, int* seq, int t_max, int* lens, int* emitted, int* done,
-                               long long* tokens, int max_new, int* steps, const int* acc, void* stream) {
-  if (B < 1 || B > 65535 || kq < 1 || kq > kLkMaxSlots || (ls != 1 && ls != kq) || t_max < 1 || max_new < 1) {
-    set_error("lookup_accept_drawn: need 1 <= B <= 65535, 1 <= kq <= %d, ls in {1, kq}, t_max, max_new >= 1 (B=%d "
-              "kq=%d ls=%d)", kLkMaxSlots, B, kq, ls);
+// lk_accept alone on the slots' tokens g (lk_argmax's arg-maxes, or adapcc_sample_slots' draws): g int32, ids int64
+// [B * kq]; nq, lens, emitted, done int32 [B]; seq int32 [B, t_max]; stop int32 list (null when empty); tokens int64
+// [B, max_new]; steps int32 [B] or null; acc int32 [B * kq] or null: the accepted flags and last tokens (g) of
+// adapcc_spec_slots, null for the rule that a draft is accepted when it equals the token just emitted
+int adapcc_lookup_accept(int B, int kq, const int* stop, int n_stop, const int* g, const long long* ids, const int* nq,
+                         int* seq, int t_max, int* lens, int* emitted, int* done, long long* tokens, int max_new,
+                         int* steps, const int* acc, void* stream) {
+  if (B < 1 || B > 65535 || kq < 1 || kq > kLkMaxSlots || t_max < 1 || max_new < 1) {
+    set_error("lookup_accept: need 1 <= B <= 65535, 1 <= kq <= %d, t_max, max_new >= 1 (B=%d kq=%d)", kLkMaxSlots, B,
+              kq);
     return -1;
   }
   if (n_stop < 0 || n_stop > kLkMaxIds || (n_stop && !stop)) {
-    set_error("lookup_accept_drawn: at most %d stop ids (got %d)", kLkMaxIds, n_stop);
+    set_error("lookup_accept: at most %d stop ids (got %d)", kLkMaxIds, n_stop);
     return -1;
   }
   if (!g || !ids || !nq || !seq || !lens || !emitted || !done || !tokens) {
-    set_error("lookup_accept_drawn: null pointer");
+    set_error("lookup_accept: null pointer");
     return -1;
   }
-  AcceptArgs a{nullptr, 0, 0, B, kq, ls, emitted, 0, nullptr, 0, const_cast<int*>(g), ids, nq, seq, t_max, lens,
+  AcceptArgs a{nullptr, 0, 0, B, kq, kq, emitted, 0, nullptr, 0, const_cast<int*>(g), ids, nq, seq, t_max, lens,
                emitted, done, stop, n_stop, tokens, max_new, steps, acc};
   lk_accept_kernel<<<(B + 63) / 64, 64, 0, (cudaStream_t)stream>>>(a);
   CUDA_TRY(cudaGetLastError());

@@ -611,10 +611,11 @@ class GPT2DoubleHeads(nn.Module):
         controls) verifies up to k draft tokens per row and step, copied from the row's own prompt and reply after the
         earliest earlier occurrence of its last ``max_matching_ngram_size`` (or fewer) tokens; the result is the greedy
         tokens. The definition is in ``ops/lookup.py``. On the native path (``B·(k+1)`` at most 64 rows) every verify
-        step replays one CUDA graph: the model on k + 1 slots per row (``ops.verify_attention_``), the LM head,
-        acceptance (``ops.lookup_accept_``) and the next drafts (``ops.lookup_draft_``); the host polls the done flags
-        every ``LOOKUP_POLL_PERIOD`` replays. Afterwards ``self.lookup_stats`` holds the rows' emitted tokens (a stop id
-        included) and verify steps, int32 [B], and the graph replays issued.
+        step replays one CUDA graph: the drafts (``ops.lookup_draft_``), the model on k + 1 slots per row
+        (``ops.verify_attention_``), the LM head, the slots' arg-maxes (``ops.lookup_argmax_``) and acceptance
+        (``ops.lookup_accept_``); the host polls the done flags every ``LOOKUP_POLL_PERIOD`` replays. Afterwards
+        ``self.lookup_stats`` holds the rows' emitted tokens (a stop id included) and verify steps, int32 [B], and the
+        graph replays issued.
 
         ``assistant_model`` (HuggingFace's assisted generation; a ``GPT2DoubleHeads`` with the same vocabulary, bf16 on
         the same device on the native path; not with prompt lookup or the repetition controls) drafts up to
@@ -623,15 +624,15 @@ class GPT2DoubleHeads(nn.Module):
         per-position logits the tokens are those of plain ``generate``; the draft changes only the speed. The definition
         is in ``ops/assisted.py``. On the native path (``B·(k+1)`` at most 64 rows) a round replays one CUDA graph: the
         draft's k + 1 decode steps with k draws (``ops.sample_slots_``), the model on k + 1 slots per row, the LM head,
-        the slots' draws and acceptance (``ops.lookup_accept_drawn_``; ``ops.lookup_accept_`` at temperature 0).
-        Afterwards ``self.assist_stats`` holds what ``lookup_stats`` holds for prompt lookup.
+        the slots' draws (arg-maxes at temperature 0) and acceptance (``ops.lookup_accept_``). Afterwards
+        ``self.assist_stats`` holds what ``lookup_stats`` holds for prompt lookup.
 
         ``assistant_verification`` is that rule, ``"coupled"``, or ``"rejection"``: HuggingFace's rejection sampling
         (Leviathan et al. 2023), where a draft d is accepted with probability ``min(1, P(d) / Q(d))`` of the model's
         and the draft's filtered distributions and a rejection is replaced by a draw from ``max(0, P - Q)``. Each
         emitted token is then distributed as the model's, acceptance is their overlap rather than the agreement of
         two draws, and the tokens depend on the draft. On the native path the draft draws also keep their weights and
-        the verify step runs ``ops.spec_slots_`` and ``ops.lookup_accept_drawn_(..., flagged=True)``. At temperature
+        the verify step runs ``ops.spec_slots_`` and ``ops.lookup_accept_(..., flagged=True)``. At temperature
         0 both rules are the greedy one."""
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
@@ -640,23 +641,22 @@ class GPT2DoubleHeads(nn.Module):
         filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
         from ..ops.assisted import check_verification
         check_verification("generate", assistant_verification, assistant_model)
-        if assistant_model is not None:
-            from ..ops import LOOKUP_MAX_TOKENS
-            from ..ops.assisted import check_assist_args
-            check_assist_args("generate", self, assistant_model, num_assistant_tokens, LOOKUP_MAX_TOKENS,
-                              prompt_lookup_num_tokens, repetition_penalty, no_repeat_ngram_size)
-            return self._generate_assisted(assistant_model, int(num_assistant_tokens), input_ids, lengths,
-                                           token_type_ids, reply_type, max_new_tokens, temperature, top_k, top_p,
-                                           stop_ids, suppress_ids, min_new_tokens, seed, filters,
-                                           assistant_verification == "rejection" and temperature > 0)
-        K = prompt_lookup_num_tokens
-        if K != 0:
+        if assistant_model is not None or prompt_lookup_num_tokens != 0:
             from ..ops import LOOKUP_MAX_NGRAM, LOOKUP_MAX_TOKENS
-            from ..ops.lookup import check_lookup_args
-            check_lookup_args("generate", K, max_matching_ngram_size, LOOKUP_MAX_TOKENS, LOOKUP_MAX_NGRAM, temperature,
-                              repetition_penalty, no_repeat_ngram_size)
-            return self._generate_lookup(input_ids, lengths, token_type_ids, reply_type, max_new_tokens, stop_ids,
-                                         suppress_ids, min_new_tokens, int(K), int(max_matching_ngram_size))
+            if assistant_model is not None:
+                from ..ops.assisted import check_assist_args
+                check_assist_args("generate", self, assistant_model, num_assistant_tokens, LOOKUP_MAX_TOKENS,
+                                  prompt_lookup_num_tokens, repetition_penalty, no_repeat_ngram_size)
+                K, ngram = num_assistant_tokens, 1
+            else:
+                from ..ops.lookup import check_lookup_args
+                check_lookup_args("generate", prompt_lookup_num_tokens, max_matching_ngram_size, LOOKUP_MAX_TOKENS,
+                                  LOOKUP_MAX_NGRAM, temperature, repetition_penalty, no_repeat_ngram_size)
+                K, ngram = prompt_lookup_num_tokens, max_matching_ngram_size
+            return self._generate_speculative(assistant_model, int(K), int(ngram), input_ids, lengths, token_type_ids,
+                                              reply_type, max_new_tokens, temperature, top_k, top_p, stop_ids,
+                                              suppress_ids, min_new_tokens, seed, filters,
+                                              assistant_verification == "rejection" and temperature > 0)
         B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size)
@@ -802,96 +802,40 @@ class GPT2DoubleHeads(nn.Module):
         hist_back = st.hist_back.view(n, B, K).cpu().numpy()
         return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n))
 
-    def _generate_lookup(self, input_ids, lengths, token_type_ids, reply_type, max_new_tokens, stop_ids, suppress_ids,
-                         min_new_tokens, K: int, ngram: int) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``generate`` at temperature 0 with prompt lookup of up to ``K`` drafts (``ops/lookup.py``)."""
+    def _generate_speculative(self, draft: Optional["GPT2DoubleHeads"], K: int, ngram: int, input_ids, lengths,
+                              token_type_ids, reply_type, max_new_tokens, temperature, top_k, top_p, stop_ids,
+                              suppress_ids, min_new_tokens, seed, filters,
+                              rejection: bool) -> Tuple[torch.Tensor, torch.Tensor]:
+        """``generate`` verifying up to ``K`` drafts per row and step. Without ``draft`` the drafts come from prompt
+        lookup of up to ``ngram`` tokens (``ops/lookup.py``, greedy only), with it from that model
+        (``ops/assisted.py``). The slots' tokens are arg-maxes at temperature 0, else coupled draws or, with
+        ``rejection``, rejection sampling; one acceptance follows. The stats go to ``self.lookup_stats`` or
+        ``self.assist_stats``."""
+        arg = "prompt_lookup_num_tokens" if draft is None else "num_assistant_tokens"
         B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens, 1.0, 0,
-            num_beams=K + 1, rows_name="verify rows (batch x (prompt_lookup_num_tokens + 1))")
-        cfg, dev, weight, V, S = self.cfg, input_ids.device, self.wte.weight, self.cfg.vocab_size, K + 1
-        tt_v = tt_new.repeat_interleave(S) if tt_new is not None else None
-        cache = self.new_cache(B, t_max)
-        h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
-        # the prompt's last token plays the row's last emitted token x_b, whose logits the prefill gave: lens = len - 1
-        cache.lens.sub_(1)
-        if not native:                              # CPU / not bf16: the definition on fp32 PyTorch logits
-            from ..ops.lookup import lookup_accept, lookup_draft
-            head = weight.float()
-            seq = torch.zeros(B, t_max, dtype=torch.int32)
-            seq[:, :T] = input_ids.cpu()
-            lens = cache.lens.cpu()
-            emitted, done, steps = (torch.zeros(B, dtype=torch.int32) for _ in range(3))
-            tokens = torch.full((B, n), -1, dtype=torch.int64)
-            ids, nq = torch.zeros(B * S, dtype=torch.int64), torch.ones(B, dtype=torch.int32)
-            lookup_accept(self.lm_logits(h, head), V, ids, nq, seq, lens, emitted, done, tokens, None, min_new_tokens,
-                          suppress_ids, stop_ids)
-            while not bool(done.all()):             # every live row emits at least one token per step
-                ids, pos, nq = lookup_draft(seq, lens, emitted, done, K, n, ngram)
-                cache.lens.copy_(lens)
-                hv = self._verify_hidden(ids.to(dev), pos.to(dev), tt_v, VerifyKV(cache, S, nq.to(dev)))
-                lookup_accept(self.lm_logits(hv, head), V, ids, nq, seq, lens, emitted, done, tokens, steps,
-                              min_new_tokens, suppress_ids, stop_ids)
-            self.lookup_stats = {"emitted": emitted, "steps": steps, "replays": int(steps.max())}
-            return tokens.to(dev), (tokens >= 0).sum(1).to(dev)
-
-        from ..ops import LookupState, decode_attention_work_numel, lm_head_logits_, lookup_accept_, lookup_draft_
-
-        st = LookupState(B, K, n, t_max, ngram, dev)
-        st.seq[:, :T] = input_ids
-        logits = torch.empty(B * S, weight.shape[0], dtype=torch.float32, device=dev)
-        sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
-        lm_head_logits_(h, weight, logits[:B])      # the first token, from the prefill's last positions
-        lookup_accept_(logits[:B], V, st, cache.lens, min_new_tokens, sup, stop, count=False)
-        lookup_draft_(st, cache.lens)
-        replays = 0
-        if n > 1:
-            H = cfg.n_head
-            work = torch.empty(decode_attention_work_numel(B * S, H, cfg.n_embd // H, t_max), dtype=torch.float32,
-                               device=dev)
-            verify = VerifyKV(cache, S, st.nq, work)
-
-            def accept_and_draft(hv):
-                lm_head_logits_(hv, weight, logits)
-                lookup_accept_(logits, V, st, cache.lens, min_new_tokens, sup, stop)
-                lookup_draft_(st, cache.lens)
-
-            # lookup_draft_ writes the next slots into the graph's own input buffers; lookup_accept_ advances the
-            # cache by the tokens it emits, up to k + 1 per replay, while the host counts one per replay. A live row
-            # emits at least one token per replay, so at most n - 1 replays follow the first token and the host's
-            # lengths stay at most max(lengths) + n - 1 < t_max: check_room never fires.
-            graph = DecodeGraph(self, cache, tt_v is not None, head=accept_and_draft, ids=st.ids, tt=tt_v,
-                                step=lambda ids, tt, c: self._verify_hidden(ids, st.pos, tt, verify))
-            replays = graph.run(n - 1, st.done, period=LOOKUP_POLL_PERIOD)
-        self.lookup_stats = {"emitted": st.emitted, "steps": st.steps, "replays": replays}
-        return st.tokens, (st.tokens >= 0).sum(1)
-
-    def _generate_assisted(self, draft: "GPT2DoubleHeads", K: int, input_ids, lengths, token_type_ids, reply_type,
-                           max_new_tokens, temperature, top_k, top_p, stop_ids, suppress_ids, min_new_tokens, seed,
-                           filters, rejection: bool) -> Tuple[torch.Tensor, torch.Tensor]:
-        """``generate`` with ``draft`` proposing up to ``K`` tokens per row and round (``ops/assisted.py``), verified
-        by coupled draws or, with ``rejection`` (temperature > 0), by rejection sampling."""
-        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
-            "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens, 1.0, 0,
-            num_beams=K + 1, rows_name="verify rows (batch x (num_assistant_tokens + 1))")
-        dc = draft.cfg
-        if t_max > dc.n_positions:
+            num_beams=K + 1, rows_name=f"verify rows (batch x ({arg} + 1))")
+        if draft is not None and t_max > draft.cfg.n_positions:
             raise ValueError(f"generate: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds the "
-                             f"assistant_model's n_positions = {dc.n_positions}")
+                             f"assistant_model's n_positions = {draft.cfg.n_positions}")
         cfg, dev, weight, V, S = self.cfg, input_ids.device, self.wte.weight, self.cfg.vocab_size, K + 1
-        seeds = _row_seeds(seed, B, dev)
+        seeds = _row_seeds(seed if draft is not None else 0, B, dev)     # prompt lookup is greedy and ignores seed
         tt_v = tt_new.repeat_interleave(S) if tt_new is not None else None
         cache = self.new_cache(B, t_max)
         h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
         # the prompt's last token plays the row's last emitted token x_b, whose logits the prefill gave: lens = len - 1
         cache.lens.sub_(1)
-        # The draft's cache has K more positions than the model's: a round runs all K + 1 draft steps, and those past a
-        # row's cap write there (their positions are clamped to n_positions - 1); nothing a real slot reads.
-        dcache = KVCache(dc.n_layer, B, dc.n_head, t_max + K, dc.n_embd // dc.n_head, draft.wte.weight.dtype, dev)
-        draft.hidden(input_ids, token_type_ids, cache=dcache, lengths=lengths)
+        stats = "lookup_stats" if draft is None else "assist_stats"
+        if draft is not None:
+            # The draft's cache has K more positions than the model's: a round runs all K + 1 draft steps, and those
+            # past a row's cap write there (their positions are clamped to n_positions - 1); nothing a real slot reads.
+            dc, dweight = draft.cfg, draft.wte.weight
+            dcache = KVCache(dc.n_layer, B, dc.n_head, t_max + K, dc.n_embd // dc.n_head, dweight.dtype, dev)
+            draft.hidden(input_ids, token_type_ids, cache=dcache, lengths=lengths)
         if not native:                              # CPU / not bf16: the definition on fp32 PyTorch logits
             from ..ops.assisted import assist_round, draw_slots, spec_slots
-            from ..ops.lookup import lookup_accept
-            head, dhead = weight.float(), draft.wte.weight.float()
+            from ..ops.lookup import lookup_accept, lookup_draft
+            head, dhead = weight.float(), dweight.float() if draft is not None else None
             seq = torch.zeros(B, t_max, dtype=torch.int32)
             seq[:, :T] = input_ids.cpu()
             lens = cache.lens.cpu()
@@ -900,23 +844,24 @@ class GPT2DoubleHeads(nn.Module):
             kw = dict(min_new=min_new_tokens, suppress_ids=suppress_ids, **filters)
             scal = (V, temperature, top_k, top_p, seeds.cpu().tolist())
             ids, nq = torch.zeros(B * S, dtype=torch.int64), torch.ones(B, dtype=torch.int32)
-            g = draw_slots(self.lm_logits(h, head), *scal, lens, emitted, done, nq, **kw)
+            g = draw_slots(self.lm_logits(h, head), *scal, lens, emitted, done, nq, **kw)   # greedy_token at T = 0
             lookup_accept(None, V, ids, nq, seq, lens, emitted, done, tokens, None, stop_ids=stop_ids, drawn=g)
             rounds = 0
             while not bool(done.all()):             # every live row emits at least one token per round
-                ids, pos, nq, d_in, d_pos = assist_round(seq, lens, emitted, done, K, n, dc.n_positions)
-                dcache.lens.copy_(lens)
-                ids = ids.view(B, S)
-                qlogits = []
-                for j in range(S):
-                    hd = draft._blocks(draft._embed(d_in.to(dev), tt_new, d_pos[j].to(dev)), dcache)
-                    dcache.lens.add_(1)
-                    if j < K:
-                        qlogits.append(draft.lm_logits(hd, dhead))
-                        d = draw_slots(qlogits[-1], *scal, lens, emitted, done, nq, j, True, **kw)
-                        d_in = torch.from_numpy(d[:, 0]).clamp(min=0)
-                        ids[:, j + 1] = d_in
-                ids = ids.reshape(-1)
+                if draft is None:
+                    ids, pos, nq = lookup_draft(seq, lens, emitted, done, K, n, ngram)
+                else:
+                    ids, pos, nq, d_in, d_pos = assist_round(seq, lens, emitted, done, K, n, dc.n_positions)
+                    dcache.lens.copy_(lens)
+                    qlogits = []
+                    for j in range(S):
+                        hd = draft._blocks(draft._embed(d_in.to(dev), tt_new, d_pos[j].to(dev)), dcache)
+                        dcache.lens.add_(1)
+                        if j < K:
+                            qlogits.append(draft.lm_logits(hd, dhead))
+                            d = draw_slots(qlogits[-1], *scal, lens, emitted, done, nq, j, True, **kw)
+                            d_in = torch.from_numpy(d[:, 0]).clamp(min=0)
+                            ids.view(B, S)[:, j + 1] = d_in
                 cache.lens.copy_(lens)
                 hv = self._verify_hidden(ids.to(dev), pos.to(dev), tt_v, VerifyKV(cache, S, nq.to(dev)))
                 acc = None
@@ -928,32 +873,33 @@ class GPT2DoubleHeads(nn.Module):
                 lookup_accept(None, V, ids, nq, seq, lens, emitted, done, tokens, steps, stop_ids=stop_ids, drawn=g,
                               accepted=acc)
                 rounds += 1
-            self.assist_stats = {"emitted": emitted, "steps": steps, "replays": rounds}
+            setattr(self, stats, {"emitted": emitted, "steps": steps, "replays": rounds})
             return tokens.to(dev), (tokens >= 0).sum(1).to(dev)
 
-        from ..ops import (AssistState, assist_round_, decode_attention_work_numel, lm_head_logits_, lookup_accept_,
-                           lookup_accept_drawn_, sample_slots_, spec_slots_)
+        from ..ops import (AssistState, LookupState, assist_round_, decode_attention_work_numel, lm_head_logits_,
+                           lookup_accept_, lookup_argmax_, lookup_draft_, sample_slots_, spec_slots_)
 
-        st = AssistState(B, K, n, t_max, dev, V if rejection else 0)
+        if draft is None:
+            st = LookupState(B, K, n, t_max, ngram, dev)
+        else:
+            st = AssistState(B, K, n, t_max, dev, V if rejection else 0)
+            dlogits = torch.empty(B, dweight.shape[0], dtype=torch.float32, device=dev)
         st.seq[:, :T] = input_ids
-        dweight = draft.wte.weight
         logits = torch.empty(B * S, weight.shape[0], dtype=torch.float32, device=dev)
-        dlogits = torch.empty(B, dweight.shape[0], dtype=torch.float32, device=dev)
         sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
         draw = (V, temperature, top_k, top_p, seeds, st, cache.lens)
 
-        def accept(lg, first=False):
-            if temperature == 0:                    # greedy verification: the arg-max kernel of prompt lookup
-                lookup_accept_(lg, V, st, cache.lens, min_new_tokens, sup, stop, count=not first)
-            elif rejection and not first:
-                spec_slots_(lg, V, temperature, top_k, top_p, seeds, st, cache.lens, min_new_tokens, sup, **filters)
-                lookup_accept_drawn_(st, cache.lens, stop, flagged=True)
+        def accept(lg, count=True):
+            if temperature == 0:
+                lookup_argmax_(lg, V, st, min_new_tokens, sup)
+            elif rejection and count:
+                spec_slots_(lg, *draw, min_new_tokens, sup, **filters)
             else:
                 sample_slots_(lg, *draw, 0, min_new_tokens, sup, **filters)
-                lookup_accept_drawn_(st, cache.lens, stop, count=not first, first=first)
+            lookup_accept_(st, cache.lens, stop, count=count, flagged=rejection and count)
 
         lm_head_logits_(h, weight, logits[:B])      # the first token, from the prefill's last positions
-        accept(logits[:B], first=True)
+        accept(logits[:B], count=False)
         replays = 0
         if n > 1:
             H = cfg.n_head
@@ -961,29 +907,34 @@ class GPT2DoubleHeads(nn.Module):
                                device=dev)
             verify = VerifyKV(cache, S, st.nq, work)
 
-            def round_step(ids, tt, c):
-                # a round depends on the model's state alone: its set-up also resets the draft cache's lengths
-                assist_round_(st, cache.lens, dcache.lens, dc.n_positions)
-                for j in range(S):
-                    hd = draft._blocks(draft._embed(st.d_in, tt_new, st.d_pos[j]), dcache)
-                    dcache.lens.add_(1)
-                    if j < K:
-                        lm_head_logits_(hd, dweight, dlogits)
-                        sample_slots_(dlogits, *draw, j, min_new_tokens, sup, draft=True, weights=rejection,
-                                      **filters)
+            def draft_and_verify(ids, tt, c):
+                # The drafts depend on the model's state alone (a round's set-up also resets the draft cache's
+                # lengths), so the warm-up step drafts for itself and leaves nothing behind.
+                if draft is None:
+                    lookup_draft_(st, cache.lens)
+                else:
+                    assist_round_(st, cache.lens, dcache.lens, dc.n_positions)
+                    for j in range(S):
+                        hd = draft._blocks(draft._embed(st.d_in, tt_new, st.d_pos[j]), dcache)
+                        dcache.lens.add_(1)
+                        if j < K:
+                            lm_head_logits_(hd, dweight, dlogits)
+                            sample_slots_(dlogits, *draw, j, min_new_tokens, sup, draft=True, weights=rejection,
+                                          **filters)
                 return self._verify_hidden(st.ids, st.pos, tt_v, verify)
 
             def head_and_accept(hv):
                 lm_head_logits_(hv, weight, logits)
                 accept(logits)
 
-            # lookup_accept_ advances the cache by the tokens it emits, up to k + 1 per replay, while the host counts
-            # one per replay; as for prompt lookup, at most n - 1 replays follow the first token, so check_room never
-            # fires
+            # The drafts go into the graph's own input buffers. lookup_accept_ advances the cache by the tokens it
+            # emits, up to k + 1 per replay, while the host counts one per replay. A live row emits at least one token
+            # per replay, so at most n - 1 replays follow the first token and the host's lengths stay at most
+            # max(lengths) + n - 1 < t_max: check_room never fires.
             graph = DecodeGraph(self, cache, tt_v is not None, head=head_and_accept, ids=st.ids, tt=tt_v,
-                                step=round_step)
+                                step=draft_and_verify)
             replays = graph.run(n - 1, st.done, period=LOOKUP_POLL_PERIOD)
-        self.assist_stats = {"emitted": st.emitted, "steps": st.steps, "replays": replays}
+        setattr(self, stats, {"emitted": st.emitted, "steps": st.steps, "replays": replays})
         return st.tokens, (st.tokens >= 0).sum(1)
 
     def _verify_hidden(self, ids: torch.Tensor, pos: torch.Tensor, tt: Optional[torch.Tensor],

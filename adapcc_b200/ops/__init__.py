@@ -68,15 +68,14 @@ def _lib():
         lib.adapcc_cs_context_init.argtypes = [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int,
                                                c_void_p]
         lib.adapcc_verify_attn.argtypes = [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]
-        lib.adapcc_lookup_accept.argtypes = ([c_void_p] + [c_int] * 6 + [c_void_p, c_int, c_void_p, c_int]
-                                             + [c_void_p] * 4 + [c_int] + [c_void_p] * 4 + [c_int, c_void_p, c_void_p])
+        lib.adapcc_lookup_argmax.argtypes = [c_void_p] + [c_int] * 6 + [c_void_p, c_int] + [c_void_p] * 5
+        lib.adapcc_lookup_accept.argtypes = ([c_int] * 2 + [c_void_p, c_int] + [c_void_p] * 4 + [c_int]
+                                             + [c_void_p] * 4 + [c_int, c_void_p, c_void_p, c_void_p])
         lib.adapcc_lookup_draft.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 7
         lib.adapcc_sample_slots.argtypes = ([c_void_p] + [c_int] * 6 + [c_float, c_int] + [c_float] * 5
                                             + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 6)
         lib.adapcc_spec_slots.argtypes = ([c_void_p] + [c_int] * 4 + [c_float, c_int] + [c_float] * 5
                                           + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 7)
-        lib.adapcc_lookup_accept_drawn.argtypes = ([c_int] * 3 + [c_void_p, c_int] + [c_void_p] * 4 + [c_int]
-                                                   + [c_void_p] * 4 + [c_int, c_void_p, c_void_p, c_void_p])
         lib.adapcc_assist_round.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 10
         _bound = True
     return lib
@@ -738,7 +737,7 @@ def contrastive_context_init_(h: torch.Tensor, lens: torch.Tensor, state: Contra
                                       state.t_max, _stream()), "cs_context_init")
 
 
-# ---- prompt-lookup speculative decoding: verify attention, acceptance, drafts (csrc/ops_lookup.cu) -----------------
+# ---- speculative decoding: verify attention, arg-max, acceptance, prompt-lookup drafts (csrc/ops_lookup.cu) --------
 LOOKUP_MAX_TOKENS = 15         # drafts per row: k + 1 <= 16 slots, each CTA of the verify attention runs them in turn
 LOOKUP_MAX_NGRAM = 16          # max_matching_ngram_size
 LOOKUP_MAX_IDS = 1024          # ids per suppress / stop list
@@ -766,14 +765,14 @@ def verify_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.T
 
 class LookupState:
     """Device state of a batched prompt-lookup generation of ``batch`` rows with up to ``k`` drafts each, up to
-    ``max_new`` tokens, a cache of ``t_max`` positions and n-grams of up to ``ngram`` tokens, as ``lookup_accept_`` and
-    ``lookup_draft_`` read and write it. Slot j of row b is row ``b·(k+1) + j``.
+    ``max_new`` tokens, a cache of ``t_max`` positions and n-grams of up to ``ngram`` tokens, as ``lookup_argmax_``,
+    ``lookup_accept_`` and ``lookup_draft_`` read and write it. Slot j of row b is row ``b·(k+1) + j``.
 
     ``ids`` int64 [B·(k+1)] the verify step's input (slot 0 the row's last token, then its drafts, 0 in a pad slot),
     ``pos`` int64 [B·(k+1)] their positions, ``nq`` int32 [B] the real slots (1 at the start: the prefill's logits);
     ``seq`` int32 [B, t_max] each row's sequence (the caller stores the prompts); ``emitted`` int32 [B] the tokens
     emitted (a stop id included); ``done`` int32 [B]; ``tokens`` int64 [B, max_new] the output (-1 where nothing was
-    emitted); ``steps`` int32 [B] verify steps per live row; ``g`` int32 [B·(k+1)] the slots' arg-maxes."""
+    emitted); ``steps`` int32 [B] verify steps per live row; ``g`` int32 [B·(k+1)] each real slot's token."""
 
     def __init__(self, batch: int, k: int, max_new: int, t_max: int, ngram: int, device):
         B, K, n = int(batch), int(k), int(max_new)
@@ -799,18 +798,14 @@ class LookupState:
         return (self.ids, self.pos, self.nq, self.seq, self.emitted, self.done, self.tokens, self.steps, self.g)
 
 
-def lookup_accept_(logits: torch.Tensor, vocab: int, state: LookupState, lens: torch.Tensor, min_new: int = 0,
-                   suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None,
-                   count: bool = True) -> None:
-    """Acceptance of every row, on the device (the definition in ``ops/lookup.py``). ``logits`` fp32 [B·ls, ld] (the
+def lookup_argmax_(logits: torch.Tensor, vocab: int, state: LookupState, min_new: int = 0,
+                   suppress_ids: Optional[torch.Tensor] = None) -> None:
+    """Greedy verification of every row, on the device (step 2 of ``ops/lookup.py``). ``logits`` fp32 [B·ls, ld] (the
     first ``vocab`` columns used) holds ``ls`` slots per row: k + 1 after a verify step, 1 for the prefill's logits
-    (with ``state.nq`` all 1 and ``lens`` one less than the prompt lengths). Each real slot's arg-max (ties to the
-    lower id; ``suppress_ids`` removed while ``emitted + j < min_new``) is emitted while the next slot's draft in
-    ``state.ids`` equals it; a stop id (not written) or ``state.max_new`` tokens end the row. Updates ``state.tokens``,
-    ``seq``, ``emitted``, ``done`` and, with ``count``, ``steps``, and advances ``lens`` (int32 [B]) by the number
-    emitted. No host sync."""
+    (with ``state.nq`` all 1). Each real slot's arg-max (ties to the lower id; ``suppress_ids`` removed while ``emitted
+    + j < min_new``) goes to ``state.g[b·(k+1) + j]``, for ``lookup_accept_``. No host sync."""
     def bad(msg):
-        raise ValueError(f"lookup_accept_: {msg}")
+        raise ValueError(f"lookup_argmax_: {msg}")
 
     if not isinstance(state, LookupState):
         bad(f"state must be a LookupState, got {type(state).__name__}")
@@ -823,16 +818,39 @@ def lookup_accept_(logits: torch.Tensor, vocab: int, state: LookupState, lens: t
         bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
     if int(min_new) < 0:
         bad(f"min_new must be >= 0, got {min_new}")
+    sup, n_sup = _id_list("lookup_argmax_", "suppress_ids", suppress_ids, LOOKUP_MAX_IDS)
+    _same_device("lookup_argmax_", logits.device, state.tensors() + (suppress_ids,))
+    _ck(_lib().adapcc_lookup_argmax(_ptr(logits), logits.stride(0), int(vocab), B, S, logits.shape[0] // B,
+                                    int(min_new), sup, n_sup, _ptr(state.g), _ptr(state.nq), _ptr(state.emitted),
+                                    _ptr(state.done), _stream()), "lookup_argmax")
+
+
+def lookup_accept_(state: LookupState, lens: torch.Tensor, stop_ids: Optional[torch.Tensor] = None,
+                   count: bool = True, flagged: bool = False) -> None:
+    """Acceptance of every row on the tokens ``state.g`` holds (``lookup_argmax_``'s arg-maxes, or the verify draws of
+    ``sample_slots_``), on the device (step 3 of ``ops/lookup.py``): slot j's token is emitted while the next slot's
+    draft in ``state.ids`` equals it; a stop id (not written) or ``state.max_new`` tokens end the row. ``flagged``
+    (rejection sampling, after ``spec_slots_``): the row emits the drafts ``state.acc`` accepts, then ``state.last`` at
+    the first slot whose draft is rejected (or the last real slot), with the same stop and length rules. Updates
+    ``state.tokens``, ``seq``, ``emitted``, ``done`` and, with ``count``, ``steps``, and advances ``lens`` (int32 [B])
+    by the number emitted. No host sync."""
+    def bad(msg):
+        raise ValueError(f"lookup_accept_: {msg}")
+
+    if not isinstance(state, LookupState):
+        bad(f"state must be a LookupState, got {type(state).__name__}")
+    B, S = state.batch, state.k + 1
     if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
         bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
-    sup, n_sup = _id_list("lookup_accept_", "suppress_ids", suppress_ids, LOOKUP_MAX_IDS)
+    if flagged and getattr(state, "acc", None) is None:
+        bad("flagged acceptance needs an AssistState made with a vocab")
     stop, n_stop = _id_list("lookup_accept_", "stop_ids", stop_ids, LOOKUP_MAX_IDS)
-    _same_device("lookup_accept_", logits.device, state.tensors() + (lens, suppress_ids, stop_ids))
-    _ck(_lib().adapcc_lookup_accept(_ptr(logits), logits.stride(0), int(vocab), B, S, logits.shape[0] // B,
-                                    int(min_new), sup, n_sup, stop, n_stop, _ptr(state.g), _ptr(state.ids),
+    _same_device("lookup_accept_", lens.device, state.tensors() + (stop_ids,))
+    _ck(_lib().adapcc_lookup_accept(B, S, stop, n_stop, _ptr(state.last if flagged else state.g), _ptr(state.ids),
                                     _ptr(state.nq), _ptr(state.seq), state.t_max, _ptr(lens), _ptr(state.emitted),
                                     _ptr(state.done), _ptr(state.tokens), state.max_new,
-                                    _ptr(state.steps if count else None), _stream()), "lookup_accept")
+                                    _ptr(state.steps if count else None), _ptr(state.acc if flagged else None),
+                                    _stream()), "lookup_accept")
 
 
 def lookup_draft_(state: LookupState, lens: torch.Tensor) -> None:
@@ -855,7 +873,7 @@ def lookup_draft_(state: LookupState, lens: torch.Tensor) -> None:
                                    _ptr(state.nq), _stream()), "lookup_draft")
 
 
-# ---- assisted generation: per-slot draws (csrc/ops_sample.cu), drawn acceptance and round set-up (ops_lookup.cu) ----
+# ---- assisted generation: per-slot draws (csrc/ops_sample.cu) and round set-up (ops_lookup.cu) ---------------------
 class AssistState(LookupState):
     """A ``LookupState`` for assisted generation, where a draft model proposes the drafts (``ops/assisted.py``), plus
     the draft's input buffers: ``d_in`` int64 [B] the token the draft consumes next and ``d_pos`` int64 [k+1, B] its
@@ -955,7 +973,7 @@ def spec_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int
     every real slot j of a live row it writes ``state.g[b·(k+1) + j]``, the draw ``sample_slots_`` makes (the same
     bits). For a slot with a real draft (``j + 1 < state.nq[b]``) it writes ``state.acc`` (draft j + 1 accepted: ``v
     Q_j(d) < P_j(d)``) and ``state.last`` the residual draw t_j; for the last real slot ``state.last`` is g_j. Then
-    ``lookup_accept_drawn_(..., flagged=True)`` emits the round. Needs temperature > 0. No host sync."""
+    ``lookup_accept_(..., flagged=True)`` emits the round. Needs temperature > 0. No host sync."""
     def bad(msg):
         raise ValueError(f"spec_slots_: {msg}")
 
@@ -981,33 +999,6 @@ def spec_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int
                                  _ptr(state.nq), int(min_new), sup, n_sup, _ptr(state.ids), _ptr(state.q),
                                  _ptr(state.zq), _ptr(state.g), _ptr(state.acc), _ptr(state.last), _stream()),
         "spec_slots")
-
-
-def lookup_accept_drawn_(state: LookupState, lens: torch.Tensor, stop_ids: Optional[torch.Tensor] = None,
-                         count: bool = True, first: bool = False, flagged: bool = False) -> None:
-    """``lookup_accept_``'s acceptance on the tokens ``state.g`` already holds (``sample_slots_``'s verify draws), with
-    no arg-max: the same kernel and rule. ``first``: one slot per row (the prefill's draw, ``state.nq`` all 1).
-    ``flagged`` (rejection sampling, after ``spec_slots_``): the row emits the drafts ``state.acc`` accepts, then
-    ``state.last`` at the first slot whose draft is rejected (or the last real slot), with the same stop and length
-    rules."""
-    def bad(msg):
-        raise ValueError(f"lookup_accept_drawn_: {msg}")
-
-    if not isinstance(state, LookupState):
-        bad(f"state must be a LookupState, got {type(state).__name__}")
-    B, S = state.batch, state.k + 1
-    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != B:
-        bad(f"lens must be a contiguous int32 tensor of {B} elements, got {lens.dtype} {tuple(lens.shape)}")
-    if flagged and (first or getattr(state, "acc", None) is None):
-        bad("flagged acceptance needs an AssistState made with a vocab, and not the first slot")
-    stop, n_stop = _id_list("lookup_accept_drawn_", "stop_ids", stop_ids, LOOKUP_MAX_IDS)
-    _same_device("lookup_accept_drawn_", lens.device, state.tensors() + (stop_ids,))
-    _ck(_lib().adapcc_lookup_accept_drawn(B, S, 1 if first else S, stop, n_stop,
-                                          _ptr(state.last if flagged else state.g), _ptr(state.ids),
-                                          _ptr(state.nq), _ptr(state.seq), state.t_max, _ptr(lens),
-                                          _ptr(state.emitted), _ptr(state.done), _ptr(state.tokens), state.max_new,
-                                          _ptr(state.steps if count else None), _ptr(state.acc if flagged else None),
-                                          _stream()), "lookup_accept_drawn")
 
 
 def assist_round_(state: AssistState, lens: torch.Tensor, d_lens: torch.Tensor, n_pos: int) -> None:

@@ -1,7 +1,7 @@
 """Assisted generation (HuggingFace's ``assistant_model``): a draft model proposes up to k tokens per row and the
 target verifies them in one step. This module is the CPU / non-bf16 path of ``GPT2DoubleHeads.generate(...,
 assistant_model=draft, num_assistant_tokens=k)`` and the reference the GPU tests compare ``sample_slots_``,
-``lookup_accept_drawn_`` and ``assist_round_`` against. It uses prompt lookup's conventions (``ops/lookup.py``): row b
+``lookup_accept_`` and ``assist_round_`` against. It uses prompt lookup's conventions (``ops/lookup.py``): row b
 has emitted ``e_b`` tokens, its last token ``x_b`` is not cached yet, ``lens[b] = len_b + e_b - 1``.
 
 One round of a live row, with ``r_b = min(k, max_new_tokens - e_b - 1)``:

@@ -1,6 +1,6 @@
 """Prompt-lookup speculative decoding for greedy generation (HuggingFace's ``prompt_lookup_num_tokens``): the CPU /
 non-bf16 path of ``GPT2DoubleHeads.generate(..., prompt_lookup_num_tokens=k)`` and the reference the GPU tests compare
-``lookup_accept_`` and ``lookup_draft_`` (csrc/ops_lookup.cu) against.
+``lookup_argmax_``, ``lookup_accept_`` and ``lookup_draft_`` (csrc/ops_lookup.cu) against.
 
 Row b has emitted ``e_b`` tokens. Its *sequence* ``s_b`` is its prompt without padding, then those tokens; the last
 one, ``x_b``, is not in the KV cache yet, so ``lens[b] = len_b + e_b - 1`` (DESIGN.md §4a). Before the first token
@@ -121,9 +121,9 @@ def lookup_accept(logits: torch.Tensor, vocab: int, ids: torch.Tensor, nq: torch
     ``emitted``, ``done`` [B], ``tokens`` [B, max_new] (-1 where nothing is written) and ``steps`` [B] (verify steps
     per live row; None: not counted). ``logits`` [B·ls, >= vocab] holds ``ls`` slots per row (1 for the prefill's
     logits, k + 1 for a verify step), ``ids`` [B·(k+1)] the step's input and ``nq`` [B] its real slots (at most
-    ``ls`` are used). ``drawn`` [B, ls] (``lookup_accept_drawn_``): the slots' tokens, already drawn
-    (``ops/assisted.py``), in place of the arg-maxes of ``logits`` (which may then be None). ``accepted`` [B, ls]
-    (``lookup_accept_drawn_(..., flagged=True)``): per slot whether its draft is accepted (``accept_row``), with
+    ``ls`` are used). ``drawn`` [B, ls]: the slots' tokens, already drawn (``ops/assisted.py``), in place of the
+    arg-maxes of ``logits`` (which may then be None). ``accepted`` [B, ls] (``lookup_accept_(..., flagged=True)``):
+    per slot whether its draft is accepted (``accept_row``), with
     ``drawn`` holding each slot's last token."""
     B, t_max = seq.shape
     ls = logits.shape[0] // B if drawn is None else drawn.shape[1]

@@ -1,8 +1,9 @@
 """Assisted generation on the GPU: ``sample_slots_`` bit for bit against ``sample_tokens_`` row by row,
-``assist_round_`` and ``lookup_accept_drawn_`` exactly against the definition (ops/assisted.py, ops/lookup.py), and
-``GPT2DoubleHeads.generate(..., assistant_model=draft)`` on GPT-2 small with random weights, with three drafts: greedy
-and sampled exactly against the definition evaluated eagerly with the same compute (host counters and acceptance, one
-``sample_tokens_`` call per slot), and greedy against plain ``generate`` up to near ties."""
+``assist_round_`` and ``lookup_accept_`` on drawn tokens exactly against the definition (ops/assisted.py,
+ops/lookup.py), and ``GPT2DoubleHeads.generate(..., assistant_model=draft)`` on GPT-2 small with random weights,
+with three drafts: greedy and sampled exactly against the definition evaluated eagerly with the same compute (host
+counters and acceptance, one ``sample_tokens_`` call per slot), and greedy against plain ``generate`` up to near
+ties."""
 import numpy as np
 import pytest
 import torch
@@ -97,8 +98,8 @@ def test_sample_slots_bit_exact_against_sample_tokens(dev, mode):
     print(f"mode {mode}: {drawn} slots drawn bit-exact")
 
 
-def test_round_and_drawn_acceptance_exact_against_the_definition(dev):
-    from adapcc_b200.ops import assist_round_, lookup_accept_drawn_, sample_slots_
+def test_round_and_accept_on_drawn_tokens_exact_against_the_definition(dev):
+    from adapcc_b200.ops import assist_round_, lookup_accept_, sample_slots_
     from adapcc_b200.ops.assisted import assist_round, draw_slots
     from adapcc_b200.ops.lookup import lookup_accept
 
@@ -138,7 +139,7 @@ def test_round_and_drawn_acceptance_exact_against_the_definition(dev):
     wl = lens.cpu().clone()
     lookup_accept(None, V, st.ids.cpu(), st.nq.cpu(), w["seq"], wl, w["emitted"], w["done"], w["tokens"],
                   w["steps"], stop_ids=stop, drawn=torch.from_numpy(host))
-    lookup_accept_drawn_(st, lens, torch.tensor(stop, dtype=torch.int32, device=dev))
+    lookup_accept_(st, lens, torch.tensor(stop, dtype=torch.int32, device=dev))
     torch.cuda.synchronize()
     for name in names:
         assert torch.equal(getattr(st, name).cpu(), w[name]), name

@@ -1,7 +1,7 @@
 """Prompt-lookup decoding on the GPU: ``verify_attention_`` bit for bit against sequential ``decode_attention_``
-launches, ``lookup_draft_`` and ``lookup_accept_`` exactly against the definition (ops/lookup.py), graph replay against
-eager launches, and ``GPT2DoubleHeads.generate(..., prompt_lookup_num_tokens=k)`` on GPT-2 small with random weights
-against plain greedy ``generate``, with a near-tie allowance calibrated in the test."""
+launches, ``lookup_draft_``, ``lookup_argmax_`` and ``lookup_accept_`` exactly against the definition (ops/lookup.py),
+graph replay against eager launches, and ``GPT2DoubleHeads.generate(..., prompt_lookup_num_tokens=k)`` on GPT-2
+small with random weights against plain greedy ``generate``, with a near-tie allowance calibrated in the test."""
 import numpy as np
 import pytest
 import torch
@@ -107,8 +107,8 @@ def test_lookup_draft_exact_against_the_definition(dev):
 
 
 @pytest.mark.parametrize("first", [False, True])
-def test_lookup_accept_exact_against_the_definition(dev, first):
-    from adapcc_b200.ops import lookup_accept_, lookup_draft_
+def test_lookup_argmax_and_accept_exact_against_the_definition(dev, first):
+    from adapcc_b200.ops import lookup_accept_, lookup_argmax_, lookup_draft_
     from adapcc_b200.ops.lookup import greedy_token, lookup_accept
 
     B, k, n, t_max, V, ld = 8, 4, 24, 120, 1000, 1024
@@ -145,9 +145,9 @@ def test_lookup_accept_exact_against_the_definition(dev, first):
     lookup_accept(torch.from_numpy(logits), V, st.ids.cpu(), st.nq.cpu(), want["seq"], wl, want["emitted"],
                   want["done"], want["tokens"], None if first else want["steps"], min_new, suppress, stop)
     dl = lens.clone()
-    lookup_accept_(torch.from_numpy(logits).to(dev), V, st, dl, min_new,
-                   torch.tensor(suppress, dtype=torch.int32, device=dev),
-                   torch.tensor(stop, dtype=torch.int32, device=dev), count=not first)
+    lookup_argmax_(torch.from_numpy(logits).to(dev), V, st, min_new,
+                   torch.tensor(suppress, dtype=torch.int32, device=dev))
+    lookup_accept_(st, dl, torch.tensor(stop, dtype=torch.int32, device=dev), count=not first)
     torch.cuda.synchronize()
     for name, t in want.items():
         assert torch.equal(getattr(st, name).cpu(), t), name

@@ -14,9 +14,9 @@ nothing about trained GPT-2; the step costs give the speed-up for any acceptance
 * ``steps``: one verify step (the model on B·(k+1) slots and the LM head on them) against one decode step (the model
   on B rows and the LM head), both replayed from CUDA graphs of 50 steps at 128 / 512 cached tokens.
 * ``kernels`` (one layer of GPT-2 small, 12 heads of 64, 8 rows, 128 / 512 cached tokens): ``verify_attention_``
-  against k + 1 sequential ``decode_attention_`` launches, and ``lookup_accept_`` + ``lookup_draft_`` after a verify
-  step (each launch also restores 8 lengths). 50 launches captured in a CUDA graph, timed with CUDA events over
-  ``--launches`` launches.
+  against k + 1 sequential ``decode_attention_`` launches, and ``lookup_argmax_`` + ``lookup_accept_`` +
+  ``lookup_draft_`` after a verify step (each launch also restores 8 lengths). 50 launches captured in a CUDA graph,
+  timed with CUDA events over ``--launches`` launches.
 
 Usage: ``python tools/lookup_bench.py [--reps 5] [--launches 1000]``
 """
@@ -170,7 +170,7 @@ def bench_steps(model, launches):
 
 def bench_kernels(model, launches):
     from adapcc_b200.ops import (LookupState, decode_attention_, decode_attention_work_numel, lookup_accept_,
-                                 lookup_draft_, verify_attention_)
+                                 lookup_argmax_, lookup_draft_, verify_attention_)
 
     cfg = model.cfg
     B, H, Dh, D, V = 8, cfg.n_head, cfg.n_embd // cfg.n_head, cfg.n_embd, cfg.vocab_size
@@ -206,7 +206,8 @@ def bench_kernels(model, launches):
 
             def accept_draft():
                 rl.copy_(lens)
-                lookup_accept_(logits, V, st, rl)
+                lookup_argmax_(logits, V, st)
+                lookup_accept_(st, rl)
                 lookup_draft_(st, rl)
 
             acc_us = _graph_us(accept_draft, launches)
