@@ -12,6 +12,17 @@
 //   kv_reorder  : cache[l, r, :, pos] = cache[l, parent[r], :, pos] for the generated positions, through a scratch
 //                 buffer (gather, then scatter), so cycles and many-to-one parent maps come out right.
 //
+// Beam sampling (HuggingFace's do_sample=True with num_beams > 1) replaces the first two:
+//   beam_sample_rows   : one 1024-thread CTA per beam row, the row's x_i = l_i / T in shared memory. m and log Z as
+//                        beam_rows computes them, then the sampler's top-k / top-p filter (sample_filter.cuh) with a
+//                        minimum keep count, then c_i = s + lp_i / T and the Gumbel key g_i = c_i + G_i of every kept
+//                        id, G_i from the item's Philox stream. The row's M best keys (a bisection for the M-th key,
+//                        then a rank sort) are kept, with their c next to them.
+//   beam_sample_select : one 512-thread CTA per item. Each key's place in the item's draw order is its place in its
+//                        row plus, per other row, a binary search for the larger keys; the first M form the sample.
+//                        The first K draws that finish are offered, and the K best-c draws that do not are the new
+//                        beams (DESIGN.md §4a).
+//
 // Every fp32 sum runs in an order fixed by the thread layout (per-thread loops in id order, shuffle trees, warp partials
 // added by a shuffle tree in warp order); an item's result depends only on its own rows. ops/beam.py evaluates the same
 // definition in fp64.
@@ -21,6 +32,7 @@
 #include <cstdint>
 
 #include "common.h"
+#include "sample_filter.cuh"
 #include "topk_rows.cuh"
 
 namespace adapcc {
@@ -29,6 +41,7 @@ constexpr int kBeamMaxK = 16;
 constexpr int kBeamMaxStop = 8;
 constexpr int kBeamMaxN = kBeamMaxK + kBeamMaxStop;   // candidates kept per row
 constexpr int kBeamMaxSuppress = 1024;
+constexpr int kBeamSampleMaxM = (kBeamMaxStop + 1) * kBeamMaxK;   // sampled candidates per item and per row
 constexpr int kReorderThreads = 256;
 
 struct BeamArgs {
@@ -216,6 +229,295 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const __grid_constant__
 
 __global__ void beam_step_incr_kernel(int* step) { *step += 1; }
 
+// ---- beam sampling ---------------------------------------------------------------------------------------------------
+struct BeamSampleArgs {
+  BeamArgs a;                  // a.N = M = min_keep * K; a.cand [B * K, M]: each row's M best Gumbel keys, best first
+  float temperature, top_p;
+  int top_k, min_keep;         // min_keep = max(2, 1 + n_stop)
+  const long long* seeds;      // [B]: the item's Philox key
+  float* cand_c;               // [B * K, M]: the candidate score c next to each key
+};
+
+// G = -log(-log u) for u = ((w >> 8) + 0.5) 2^-24: -log u is taken from u below 1/2 and from 1 - u above, and both
+// are exact in fp32, so G is finite for every word
+__device__ __forceinline__ float beam_gumbel(uint32_t w) {
+  const uint32_t k = w >> 8;
+  const float nlu = k < (1u << 23) ? -logf((float)(2u * k + 1u) * 0x1p-25f)
+                                   : -log1pf(-(float)((1u << 25) - 2u * k - 1u) * 0x1p-25f);
+  return -logf(nlu);
+}
+
+__global__ void __launch_bounds__(kSampleThreads, 1) beam_sample_rows_kernel(const __grid_constant__ BeamSampleArgs p) {
+  extern __shared__ float s_x[];                      // [vocab]: x_i = l_i / T, then g_i of the kept ids (-inf else)
+  __shared__ SampleSmem sm;
+  __shared__ float s_red[32];                         // beam_block_* with 1024 threads: warps 16-31 hold identities
+  __shared__ unsigned long long s_sel[kBeamSampleMaxM];
+  __shared__ int s_n;
+  const BeamArgs& a = p.a;
+  const int row = blockIdx.x, b = row / a.K, j = row - b * a.K, tid = threadIdx.x, V = a.vocab, M = a.N;
+  unsigned long long* out = a.cand + (long long)row * M;
+  float* out_c = p.cand_c + (long long)row * M;
+  const float s = a.scores[row];
+  if (a.done[b] || !(s > -INFINITY)) {                // a finished item or a dead beam offers nothing
+    for (int e = tid; e < M; e += kSampleThreads) out[e] = 0ull;
+    return;
+  }
+  const int step = *a.step;
+  const float* l = a.logits + (long long)row * a.ld;
+  for (int i = tid; i < V; i += kSampleThreads) s_x[i] = __fdiv_rn(__ldg(l + i), p.temperature);
+  __syncthreads();
+  if (step < a.min_new) {
+    for (int q = tid; q < a.n_suppress; q += kSampleThreads) {
+      const int id = a.suppress[q];
+      if (id >= 0 && id < V) s_x[id] = -INFINITY;
+    }
+    __syncthreads();
+  }
+  // m and log Z over the remaining ids, by the first 512 threads in beam_rows' order (the same bits)
+  float m = -INFINITY;
+  if (tid < kBeamThreads)
+    for (int i = tid; i < V; i += kBeamThreads)
+      if (s_x[i] != -INFINITY) m = fmaxf(m, __ldg(l + i));
+  m = beam_block_max(s_red, m);
+  if (!(m > -INFINITY)) {                             // every id removed or at -inf
+    for (int e = tid; e < M; e += kSampleThreads) out[e] = 0ull;
+    return;
+  }
+  float z = 0.f;
+  if (tid < kBeamThreads)
+    for (int i = tid; i < V; i += kBeamThreads)
+      if (s_x[i] != -INFINITY) z += expf(__ldg(l + i) - m);
+  z = beam_block_sum(s_red, z);
+  const float lz = logf(z);
+  auto cand_score = [&](int i) { return s + __fdiv_rn((__ldg(l + i) - m) - lz, p.temperature); };
+  // the sampler's filter on x, keeping at least min_keep values
+  unsigned long long best = 0;
+  int present = 0, z1 = 0, z2 = 0;
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const uint32_t k = f2key(s_x[i]);
+    if (k > kNegInfKey) {
+      ++present;
+      best = max(best, (unsigned long long)k);
+    }
+  }
+  best = block_max(sm, best);
+  float fz = 0.f;
+  block_sum(sm, fz, present, z1, z2);
+  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, p.min_keep, present, (uint32_t)best,
+                               key2f((uint32_t)best));
+  __syncthreads();                                    // every x is read before the row becomes the keys
+  // g_i = c_i + G_i; ids 4q..4q+3 take the four words of Philox at counter (q, j, step, 0)
+  const uint32_t k0 = (uint32_t)(unsigned long long)p.seeds[b], k1 = (uint32_t)((unsigned long long)p.seeds[b] >> 32);
+  for (int q = tid; q < (V + 3) / 4; q += kSampleThreads) {
+    bool kept[4], any = false;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int i = 4 * q + e;
+      kept[e] = i < V && f2key(s_x[i]) >= tau;
+      any |= kept[e];
+    }
+    uint4 w = make_uint4(0u, 0u, 0u, 0u);
+    if (any) w = philox4((uint32_t)q, (uint32_t)j, (uint32_t)step, 0u, k0, k1);
+    const uint32_t words[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int i = 4 * q + e;
+      if (i < V) s_x[i] = kept[e] ? cand_score(i) + beam_gumbel(words[e]) : -INFINITY;
+    }
+  }
+  __syncthreads();
+  // the M best keys (g bits, then the inverted id): all kept ids when there are at most M; else those above the M-th
+  // largest g, and of the ones equal to it the lowest ids
+  best = 0;
+  int cnt = 0;
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const uint32_t k = f2key(s_x[i]);
+    if (k > kNegInfKey) {
+      ++cnt;
+      best = max(best, (unsigned long long)k);
+    }
+  }
+  best = block_max(sm, best);
+  block_sum(sm, fz, cnt, z1, z2);
+  uint32_t thr = kNegInfKey;                          // taken: key > thr, or key == thr and id < cut
+  int cut = 0;
+  if (cnt > M) {
+    thr = kth_key(s_x, sm, V, M, (uint32_t)best);
+    int gt = 0, eq = 0, unused = 0;
+    for (int i = tid; i < V; i += kSampleThreads) {
+      const uint32_t k = f2key(s_x[i]);
+      gt += k > thr;
+      eq += k == thr;
+    }
+    block_sum(sm, fz, gt, eq, unused);
+    const int need = M - gt;
+    cut = V;
+    if (eq > need) {                                  // tied at the M-th key: the smallest cut with need ids below it
+      int lo = 0, hi = V;
+      while (hi - lo > 1) {
+        const int mid = lo + (hi - lo) / 2;
+        int c = 0, u0 = 0, u1 = 0;
+        for (int i = tid; i < mid; i += kSampleThreads) c += f2key(s_x[i]) == thr;
+        block_sum(sm, fz, c, u0, u1);
+        if (c >= need) hi = mid;
+        else lo = mid;
+      }
+      cut = hi;
+    }
+  }
+  if (tid == 0) s_n = 0;
+  __syncthreads();
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const uint32_t k = f2key(s_x[i]);
+    if (k > thr || (k == thr && i < cut)) s_sel[atomicAdd(&s_n, 1)] = ((unsigned long long)k << 32) |
+                                                                      (0xFFFFFFFFu - (uint32_t)i);
+  }
+  __syncthreads();
+  const int n = s_n;
+  // best first: a key's place is the number of larger keys (the keys are distinct)
+  for (int e = tid; e < M; e += kSampleThreads) {
+    if (e >= n) {
+      out[e] = 0ull;
+      continue;
+    }
+    const unsigned long long v = s_sel[e];
+    int r = 0;
+    for (int f = 0; f < n; ++f) r += s_sel[f] > v;
+    out[r] = v;
+    out_c[r] = cand_score((int)(0xFFFFFFFFu - (uint32_t)v));
+  }
+}
+
+__global__ void __launch_bounds__(kBeamThreads) beam_sample_select_kernel(const __grid_constant__ BeamSampleArgs p) {
+  __shared__ unsigned long long s_k[kBeamMaxK * kBeamSampleMaxM];   // the K rows' keys, re-keyed by the flat index
+  __shared__ float s_c[kBeamMaxK * kBeamSampleMaxM];
+  __shared__ int s_draw[kBeamSampleMaxM];             // draw d -> element j * M + place
+  __shared__ unsigned char s_fin[kBeamSampleMaxM];    // draw d finishes
+  __shared__ int s_beam[kBeamMaxK];                   // new beam k -> draw
+  __shared__ FinishedSet fs;
+  const BeamArgs& a = p.a;
+  const int b = blockIdx.x, tid = threadIdx.x, K = a.K, M = a.N, V = a.vocab, BK = a.B * a.K;
+  const int step = *a.step;
+  if (a.done[b] || step >= a.max_new) {               // nothing moves: every row keeps its own cache
+    if (tid < K) a.parent[b * K + tid] = b * K + tid;
+    return;
+  }
+  for (int e = tid; e < K * M; e += kBeamThreads) {
+    const int j = e / M;
+    const long long o = (long long)(b * K + j) * M + (e - j * M);
+    const unsigned long long v = a.cand[o];
+    const uint32_t flat = (uint32_t)j * (uint32_t)V + (0xFFFFFFFFu - (uint32_t)v);
+    s_k[e] = v ? (v & 0xFFFFFFFF00000000ull) | (0xFFFFFFFFu - flat) : 0ull;
+    s_c[e] = p.cand_c[o];
+  }
+  for (int d = tid; d < M; d += kBeamThreads) s_draw[d] = -1;
+  if (tid < K) s_beam[tid] = -1;
+  if (tid == 0) {
+    fs.K = K;
+    fs.count = a.fin_count[b];
+    for (int k = 0; k < K; ++k) {
+      fs.score[k] = a.fin_score[b * K + k];
+      fs.n[k] = a.fin_n[b * K + k];
+      fs.src[k] = a.fin_src[b * K + k];
+    }
+  }
+  __syncthreads();
+  // the draw order: a key's place in its (sorted) row plus the number of larger keys in each other row
+  for (int e = tid; e < K * M; e += kBeamThreads) {
+    const unsigned long long v = s_k[e];
+    if (!v) continue;
+    const int j = e / M;
+    int r = e - j * M;
+    for (int j2 = 0; j2 < K && r < M; ++j2) {
+      if (j2 == j) continue;
+      const unsigned long long* row = s_k + j2 * M;
+      int lo = 0, hi = M;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (row[mid] > v) lo = mid + 1;
+        else hi = mid;
+      }
+      r += lo;
+    }
+    if (r < M) s_draw[r] = e;
+  }
+  __syncthreads();
+  const bool last = step == a.max_new - 1;
+  auto token = [&](int e) { return (int)((0xFFFFFFFFu - (uint32_t)s_k[e]) - (uint32_t)(e / M) * (uint32_t)V); };
+  for (int d = tid; d < M; d += kBeamThreads) {
+    const int e = s_draw[d];
+    bool f = last;
+    if (e >= 0)
+      for (int q = 0; q < a.n_stop; ++q) f |= a.stop[q] == token(e);
+    s_fin[d] = f;
+  }
+  __syncthreads();
+  // the new beams: the K best c among the drawn candidates that do not finish, ties to the earlier draw
+  for (int d = tid; d < M; d += kBeamThreads) {
+    const int e = s_draw[d];
+    if (e < 0 || s_fin[d]) continue;
+    const float c = s_c[e];
+    int r = 0;
+    for (int d2 = 0; d2 < M && r < K; ++d2) {
+      const int e2 = s_draw[d2];
+      if (e2 < 0 || s_fin[d2]) continue;
+      const float c2 = s_c[e2];
+      r += c2 > c || (c2 == c && d2 < d);
+    }
+    if (r < K) s_beam[r] = d;
+  }
+  __syncthreads();
+  const int L = step + 1;                             // tokens of a hypothesis that ends at this step
+  if (tid == 0) {                                     // the first K draws that finish are offered, in draw order
+    for (int d = 0; d < K; ++d) {
+      const int e = s_draw[d];
+      if (e < 0) break;
+      if (!s_fin[d]) continue;
+      const int i = token(e);
+      bool is_stop = false;
+      for (int q = 0; q < a.n_stop; ++q) is_stop |= a.stop[q] == i;
+      if (is_stop) fs.offer(s_c[e] / a.pen[L], L - 1, e / M);
+      else fs.offer(s_c[e] / a.pen[a.max_new], a.max_new, d);
+    }
+  }
+  if (tid < K) {
+    const int r = b * K + tid;
+    const long long h = (long long)step * BK + r;
+    const int e = last ? s_draw[tid] : (s_beam[tid] >= 0 ? s_draw[s_beam[tid]] : -1);
+    // the last step has no live beams; its history slot k holds draw k, which an offer may point at
+    a.hist_tok[h] = e >= 0 ? token(e) : -1;
+    a.hist_back[h] = e >= 0 ? e / M : tid;
+    if (e >= 0 && !last) {
+      a.next_ids[r] = token(e);
+      a.parent[r] = b * K + e / M;
+      a.scores[r] = s_c[e];
+    } else {
+      a.next_ids[r] = 0;
+      a.parent[r] = r;
+      a.scores[r] = -INFINITY;
+    }
+  }
+  __syncthreads();
+  if (tid == 0) {
+    int done = 0;
+    if (last || s_beam[0] < 0) {
+      done = 1;
+    } else if (fs.count == K) {
+      // as in beam_select: a live sum can only fall, so the best reachable normalised score bounds every later offer
+      const float reach = s_c[s_draw[s_beam[0]]] / a.pen[a.alpha_pos ? a.max_new : L + 1];
+      done = !(reach > fs.score[K - 1]);
+    }
+    a.done[b] = done;
+    a.fin_count[b] = fs.count;
+  }
+  __syncthreads();
+  if (tid < K) {
+    a.fin_score[b * K + tid] = fs.score[tid];
+    a.fin_n[b * K + tid] = fs.n[tid];
+    a.fin_src[b * K + tid] = fs.src[tid];
+  }
+}
+
 // ---- KV-cache reordering -----------------------------------------------------------------------------------------
 struct ReorderArgs {
   __nv_bfloat16* k;            // [L, R, H, t_max, Dh]
@@ -301,6 +603,56 @@ int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, float
   CUDA_TRY(cudaGetLastError());
   count_launch();
   beam_select_kernel<<<B, 32, 0, s>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  beam_step_incr_kernel<<<1, 1, 0, s>>>(step);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// adapcc_beam_step's arguments, plus cand_c fp32 [B*K, M] next to cand uint64 [B*K, M] (M = max(2, 1 + n_stop) * K),
+// the sampling scalars (temperature > 0, top_k >= 0 with 0 off, 0 < top_p <= 1) and seeds int64 [B]; vocab <= 56 Ki
+int adapcc_beam_sample_step(const float* logits, int ld, int vocab, int B, int K, float* scores, int* step,
+                            int min_new, const int* suppress, int n_suppress, const int* stop, int n_stop,
+                            const float* pen, int alpha_pos, int max_new, int* done, void* cand, float* cand_c,
+                            long long* next_ids, int* parent, long long* hist_tok, int* hist_back, float* fin_score,
+                            int* fin_n, int* fin_src, int* fin_count, float temperature, int top_k, float top_p,
+                            const long long* seeds, void* stream) {
+  if (B < 1 || K < 1 || K > kBeamMaxK || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab || max_new < 1) {
+    set_error("beam_sample_step: need B >= 1, 1 <= K <= %d, 1 <= vocab <= %d, ld >= vocab, max_new >= 1 (B=%d K=%d "
+              "vocab=%d ld=%d max_new=%d)", kBeamMaxK, kSampleMaxVocab, B, K, vocab, ld, max_new);
+    return -1;
+  }
+  if (n_suppress < 0 || n_suppress > kBeamMaxSuppress || n_stop < 0 || n_stop > kBeamMaxStop ||
+      (n_suppress && !suppress) || (n_stop && !stop)) {
+    set_error("beam_sample_step: at most %d suppressed and %d stop ids (got %d, %d)", kBeamMaxSuppress, kBeamMaxStop,
+              n_suppress, n_stop);
+    return -1;
+  }
+  if (!(temperature > 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
+    set_error("beam_sample_step: need temperature > 0, top_k >= 0, 0 < top_p <= 1 (got %g, %d, %g)", temperature,
+              top_k, top_p);
+    return -1;
+  }
+  if (!logits || !scores || !step || !pen || !done || !cand || !cand_c || !next_ids || !parent || !hist_tok ||
+      !hist_back || !fin_score || !fin_n || !fin_src || !fin_count || !seeds) {
+    set_error("beam_sample_step: null pointer");
+    return -1;
+  }
+  const int min_keep = n_stop + 1 > 2 ? n_stop + 1 : 2;
+  const size_t smem = (size_t)vocab * sizeof(float);
+  if (smem > 48 * 1024)
+    CUDA_TRY(cudaFuncSetAttribute(beam_sample_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  BeamSampleArgs p{BeamArgs{logits, ld, vocab, B, K, min_keep * K, scores, step, min_new, suppress, n_suppress, stop,
+                            n_stop, pen, alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent,
+                            hist_tok, hist_back, fin_score, fin_n, fin_src, fin_count},
+                   temperature, top_p, top_k, min_keep, seeds, cand_c};
+  cudaStream_t s = (cudaStream_t)stream;
+  beam_sample_rows_kernel<<<B * K, kSampleThreads, smem, s>>>(p);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  beam_sample_select_kernel<<<B, kBeamThreads, 0, s>>>(p);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   beam_step_incr_kernel<<<1, 1, 0, s>>>(step);

@@ -7,9 +7,8 @@
 //             of d; each lane adds its chunks in order and a shuffle tree adds the lanes. The order depends on D only,
 //             so a row's bits do not depend on B, on the other rows or on which warp handles which rows of W.
 //   sample  : one CTA of 1024 threads per row; the row's x_i = l_i / temperature stay in shared memory for all passes.
-//             The top-k threshold and the top-p cut-off are found by bisection over the order-preserving integer
-//             encoding of x (counts for top-k, masses for top-p), with no sort. The draw is an inclusive scan over the
-//             surviving weights in index order.
+//             The top-k threshold, the top-p cut-off and the truncation filters are those of sample_filter.cuh (shared
+//             with sampled beam search). The draw is an inclusive scan over the surviving weights in index order.
 //   slots   : the draws of assisted generation, one CTA per verify slot or draft (grid (slots, B)), through the same
 //             row body as `sample`, with a per-slot Philox counter and step (DESIGN.md §4a). A draft draw can also
 //             write the draft's filtered weights, which rejection-sampling verification reads.
@@ -30,6 +29,7 @@
 
 #include "common.h"
 #include "device_prims.cuh"
+#include "sample_filter.cuh"
 
 namespace adapcc {
 
@@ -38,13 +38,9 @@ constexpr int kHeadRows = 4;                 // rows of W per warp and iteration
 constexpr int kHeadMaxChunks = 4;            // 8-element chunks of d per lane: D <= 32 * 8 * 4 = 1024
 constexpr int kHeadMaxD = 32 * 8 * kHeadMaxChunks;
 constexpr int kHeadMaxB = 64;                // h in shared memory: 64 x 1024 x 2 B = 128 KB at most
-constexpr int kSampleThreads = 1024;
-constexpr int kSampleWarps = kSampleThreads / 32;
-constexpr int kSampleMaxVocab = 56 * 1024;   // x of a row in shared memory: 224 KB
 constexpr int kSampleMaxList = 1024;
 constexpr int kOpsMaxDevices = 64;
 constexpr int kSlotMaxSlots = 16;            // verify slots per row (LOOKUP_MAX_TOKENS + 1)
-constexpr uint32_t kNegInfKey = 0x007FFFFFu; // key(-inf): ids at -inf (removed ones included) are never candidates
 
 __global__ void __launch_bounds__(kHeadThreads)
 lm_head_logits_kernel(const __nv_bfloat16* __restrict__ h, int ld_h, const __nv_bfloat16* __restrict__ W, int V, int D,
@@ -103,223 +99,6 @@ lm_head_logits_kernel(const __nv_bfloat16* __restrict__ h, int ld_h, const __nv_
 }
 
 // ---- sampling --------------------------------------------------------------------------------------------------------
-struct SampleArgs {
-  const float* logits;       // [B, ld], the first `vocab` columns used
-  int ld, vocab;
-  float temperature, top_p;
-  int top_k;
-  const long long* seeds;    // [B]
-  const int* pos;            // [B]: position of the token being drawn (the Philox counter)
-  int* step;                 // tokens generated so far (read here, incremented by step_incr_kernel)
-  int min_new;
-  const int* suppress;       // ids removed while *step < min_new
-  int n_suppress;
-  const int* stop;           // ids that end a row
-  int n_stop;
-  int* done;                 // [B]
-  long long* next_ids;       // [B]
-  long long* tokens;         // [B, max_new]
-  int max_new;
-  // truncation filters after top-p (DESIGN.md §4a); `filters` is set iff one of them is on
-  float min_p, typical_p, epsilon, eta;
-  bool filters;
-};
-
-// order-preserving: a < b (floats, no NaN) <=> key(a) < key(b)
-__device__ __forceinline__ uint32_t f2key(float f) {
-  const uint32_t u = __float_as_uint(f);
-  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
-__device__ __forceinline__ float key2f(uint32_t k) {
-  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
-// the four output words of Philox4x32-10 (Salmon et al., SC'11) for counter (c0, 0, 0, 0) and key (k0, k1): the draw
-// uses word 0; rejection-sampling verification uses word 1 for the acceptance test and word 2 for the residual draw,
-// so neither depends on the draw that produced the draft
-__device__ __forceinline__ uint4 philox4(uint32_t c0, uint32_t k0, uint32_t k1) {
-  uint32_t c1 = 0u, c2 = 0u, c3 = 0u;
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-    c0 = hi1 ^ c1 ^ k0;
-    c1 = lo1;
-    c2 = hi0 ^ c3 ^ k1;
-    c3 = lo0;
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-  return make_uint4(c0, c1, c2, c3);
-}
-
-struct SampleSmem {
-  float f[kSampleWarps];
-  float g[kSampleWarps];
-  int i[3][kSampleWarps];
-  unsigned long long u[kSampleWarps];
-};
-
-// every thread gets the block sums: a shuffle tree per warp, then each warp adds the 32 warp partials with the same
-// shuffle tree (lane w holds warp w's partial), so the order is fixed and every warp gets the same bits
-__device__ __forceinline__ void block_sum(SampleSmem& sm, float& f, int& a, int& b, int& c) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    f += __shfl_xor_sync(0xffffffffu, f, o);
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-    c += __shfl_xor_sync(0xffffffffu, c, o);
-  }
-  __syncthreads();                                  // the previous reduction's readers are done with the buffers
-  if (lane == 0) {
-    sm.f[warp] = f;
-    sm.i[0][warp] = a;
-    sm.i[1][warp] = b;
-    sm.i[2][warp] = c;
-  }
-  __syncthreads();
-  f = sm.f[lane];
-  a = sm.i[0][lane];
-  b = sm.i[1][lane];
-  c = sm.i[2][lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    f += __shfl_xor_sync(0xffffffffu, f, o);
-    a += __shfl_xor_sync(0xffffffffu, a, o);
-    b += __shfl_xor_sync(0xffffffffu, b, o);
-    c += __shfl_xor_sync(0xffffffffu, c, o);
-  }
-}
-
-// two fp32 block sums with the same fixed order as block_sum
-__device__ __forceinline__ void block_sum2(SampleSmem& sm, float& f, float& g) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    f += __shfl_xor_sync(0xffffffffu, f, o);
-    g += __shfl_xor_sync(0xffffffffu, g, o);
-  }
-  __syncthreads();
-  if (lane == 0) {
-    sm.f[warp] = f;
-    sm.g[warp] = g;
-  }
-  __syncthreads();
-  f = sm.f[lane];
-  g = sm.g[lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    f += __shfl_xor_sync(0xffffffffu, f, o);
-    g += __shfl_xor_sync(0xffffffffu, g, o);
-  }
-}
-
-__device__ __forceinline__ unsigned long long block_max(SampleSmem& sm, unsigned long long v) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if (lane == 0) sm.u[warp] = v;
-  __syncthreads();
-  v = sm.u[lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = max(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
-
-// z = sum of e_i = exp(x_i - m) and s1 = sum of e_i (x_i - m) over the finite ids, in block_sum's fixed order
-__device__ __forceinline__ void row_moments(const float* s_x, SampleSmem& sm, int V, float m, float& z, float& s1) {
-  z = 0.f;
-  s1 = 0.f;
-  for (int i = threadIdx.x; i < V; i += kSampleThreads) {
-    const float x = s_x[i];
-    if (x != -INFINITY) {
-      const float y = x - m, e = expf(y);
-      z += e;
-      s1 += e * y;
-    }
-  }
-  block_sum2(sm, z, s1);
-}
-
-// The truncation filters after top-p, in HuggingFace's order: min-p, typical, epsilon, eta. The kept set {key >= tau}
-// is first written into the row (-inf for every other id), and each filter removes ids the same way, so afterwards
-// the survivors are exactly the finite ids. A filter that is off costs nothing; p_i = e_i / Z over the current
-// survivors, with e_i = exp(x_i - m) and m the row maximum, which top-k, top-p and min-p always keep.
-__device__ __noinline__ void filter_row(float* s_x, SampleSmem& sm, const SampleArgs& a, uint32_t tau, float m,
-                                        uint32_t mkey) {
-  const int tid = threadIdx.x, V = a.vocab;
-  // materialise top-k / top-p; min-p keeps e_i >= min_p, i.e. p_i >= min_p p_max
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const float x = s_x[i];
-    if (f2key(x) < tau || (a.min_p > 0.f && expf(x - m) < a.min_p)) s_x[i] = -INFINITY;
-  }
-  uint32_t kmax = mkey;                             // key of the largest survivor: typical may remove the maximum
-  if (a.typical_p < 1.f) {
-    // H = log Z - mu with mu = sum p_i (x_i - m), so the deviation |-log p_i - H| is d_i = |(x_i - m) - mu|. The
-    // cut-off d* is the smallest d with G(d) = (mass of d_i <= d) >= p Z, found by bisection over the order-preserving
-    // keys of d. Invariant: G(lo) < p Z <= G(hi); G(lo) is carried and each pass adds the mass in (lo, mid]. Once no
-    // key lies strictly inside the half that holds d*, that half's upper end is d*. hi starts at key(+inf), so rounding
-    // that keeps every G below p Z keeps every id.
-    float z, s1;
-    row_moments(s_x, sm, V, m, z, s1);
-    const float mu = s1 / z, pz = a.typical_p * z;
-    uint32_t lo = f2key(0.f) - 1, hi = f2key(INFINITY);
-    float g_lo = 0.f;
-    while (hi - lo > 1) {
-      const uint32_t mid = lo + (hi - lo) / 2;
-      float s = 0.f;
-      int nl = 0, nh = 0, unused = 0;
-      for (int i = tid; i < V; i += kSampleThreads) {
-        const float x = s_x[i];
-        if (x != -INFINITY) {
-          const uint32_t k = f2key(fabsf((x - m) - mu));
-          if (k > lo && k <= hi) {
-            if (k <= mid) s += expf(x - m);
-            nl += k < mid;
-            nh += k > mid && k < hi;
-          }
-        }
-      }
-      block_sum(sm, s, nl, nh, unused);
-      const float g = g_lo + s;
-      if (g >= pz) {
-        hi = mid;
-        if (nl == 0) break;
-      } else {
-        lo = mid;
-        g_lo = g;
-        if (nh == 0) break;
-      }
-    }
-    unsigned long long best = 0;
-    for (int i = tid; i < V; i += kSampleThreads) {
-      const float x = s_x[i];
-      if (x != -INFINITY) {
-        if (f2key(fabsf((x - m) - mu)) > hi) s_x[i] = -INFINITY;
-        else best = max(best, (unsigned long long)f2key(x));
-      }
-    }
-    kmax = (uint32_t)block_max(sm, best);
-  }
-  // epsilon keeps p_i >= epsilon, eta keeps p_i >= min(eta, sqrt(eta) exp(-H)) with exp(-H) Z = exp(mu); both keep
-  // the largest survivors (ties together) as well, which only matters when no p_i reaches the threshold
-  for (int f = 0; f < 2; ++f) {
-    const float c = f == 0 ? a.epsilon : a.eta;
-    if (!(c > 0.f)) continue;
-    float z, s1;
-    row_moments(s_x, sm, V, m, z, s1);
-    const float t = f == 0 ? c * z : fminf(c * z, sqrtf(c) * expf(s1 / z));
-    for (int i = tid; i < V; i += kSampleThreads) {
-      const float x = s_x[i];
-      if (x != -INFINITY && expf(x - m) < t && f2key(x) != kmax) s_x[i] = -INFINITY;
-    }
-  }
-  __syncthreads();                                  // the draw reads other threads' ids
-}
-
 __device__ __forceinline__ float philox_uniform(uint32_t w) { return (float)(w >> 8) * 0x1p-24f; }
 
 // The inverse-CDF pick over s_x[0, V) by the whole CTA: the ids with `counts(x)` count, with weight `weight(x)`. Returns the smallest counting i whose inclusive prefix of weights exceeds u Z' (Z', the total, goes to `zp`), or
@@ -434,76 +213,7 @@ __device__ __forceinline__ int draw_row(float* s_x, SampleSmem& sm, const Sample
   } else if (present > 0) {
     const uint32_t mkey = (uint32_t)(best >> 32);
     const float m = key2f(mkey);
-    uint32_t tau = kNegInfKey + 1;                  // candidates are the ids with key >= tau
-    if (a.top_k > 0 && a.top_k < present) {
-      // tau = the k-th largest key counted with multiplicity. Invariant: count(key >= lo) >= k > count(key >= hi).
-      // Stops early once no key lies strictly between lo and hi: lo is then the k-th largest key.
-      uint32_t lo = kNegInfKey + 1, hi = mkey + 1;
-      int cnt_hi = 0;
-      while (hi - lo > 1) {
-        const uint32_t mid = lo + (hi - lo) / 2;
-        int c = 0, nl = 0, nh = 0;
-        for (int i = tid; i < V; i += kSampleThreads) {
-          const uint32_t k = f2key(s_x[i]);
-          if (k > lo && k < hi) {
-            c += k >= mid;
-            nl += k < mid;
-            nh += k > mid;
-          }
-        }
-        float f = 0.f;
-        block_sum(sm, f, c, nl, nh);
-        if (cnt_hi + c >= a.top_k) {
-          lo = mid;
-          if (nh == 0) break;
-        } else {
-          hi = mid;
-          cnt_hi += c;
-          if (nl == 0) break;
-        }
-      }
-      tau = lo;
-    }
-    float z = 0.f;
-    int u0 = 0, u1 = 0, u2 = 0;
-    for (int i = tid; i < V; i += kSampleThreads) {
-      const float x = s_x[i];
-      if (f2key(x) >= tau) z += expf(x - m);
-    }
-    block_sum(sm, z, u0, u1, u2);
-    const float pz = a.top_p * z;
-    if (a.top_p < 1.f && pz < z) {
-      // top-p: keep i iff F(key_i) <= p Z, F(t) = the mass of candidates with key > t (non-increasing in t).
-      // Invariant: F(lo) > p Z >= F(hi); F(hi) is carried, each pass adds the mass in (mid, hi]. Once no candidate key
-      // lies strictly between lo and hi, the kept set is key >= hi.
-      uint32_t lo = tau - 1, hi = mkey;
-      float f_hi = 0.f;
-      while (hi - lo > 1) {
-        const uint32_t mid = lo + (hi - lo) / 2;
-        float s = 0.f;
-        int nl = 0, nh = 0, unused = 0;
-        for (int i = tid; i < V; i += kSampleThreads) {
-          const float x = s_x[i];
-          const uint32_t k = f2key(x);
-          if (k > lo && k <= hi) {
-            if (k > mid) s += expf(x - m);
-            nl += k < mid;
-            nh += k > mid && k < hi;
-          }
-        }
-        block_sum(sm, s, nl, nh, unused);
-        const float f = f_hi + s;
-        if (f <= pz) {
-          hi = mid;
-          f_hi = f;
-          if (nl == 0) break;
-        } else {
-          lo = mid;
-          if (nh == 0) break;
-        }
-      }
-      tau = hi;
-    }
+    uint32_t tau = row_tau(s_x, sm, V, a.top_k, a.top_p, 1, present, mkey, m);
     if (a.filters) {
       filter_row(s_x, sm, a, tau, m, mkey);
       tau = kNegInfKey + 1;                         // the survivors are the finite ids

@@ -709,7 +709,9 @@ class GPT2DoubleHeads(nn.Module):
                     token_type_ids: Optional[torch.Tensor] = None, reply_type=None, num_beams: int = 4,
                     max_new_tokens: int = 20, length_penalty: float = 1.0, stop_ids: Sequence[int] = (),
                     suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
-                    no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    no_repeat_ngram_size: int = 0, do_sample: bool = False, temperature: float = 1.0,
+                    top_k: int = 0, top_p: float = 1.0, seed=0,
+                    num_return_sequences: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -722,22 +724,42 @@ class GPT2DoubleHeads(nn.Module):
         log-softmax, over its prompt and its own hypothesis (``ops/repeats.py``), so its log-probabilities are
         renormalised over the ids that remain.
 
-        Returns ``(tokens, n_new, scores)``: the best hypothesis of each item as int64 [B, max_new_tokens] (the stop
-        token excluded, padded with -1), its length int64 [B] and its normalised score fp32 [B].
+        ``do_sample=True`` is beam sampling (HuggingFace's ``generate(do_sample=True, num_beams=K)``; the definition is
+        ``ops.beam.BeamSampleReference``): each beam's ids are filtered by ``top_k`` (0: off) and ``top_p`` at
+        ``temperature`` > 0, keeping at least ``max(2, 1 + len(stop_ids))``, and the candidates are drawn without
+        replacement in proportion to ``exp(sum of log-probabilities / temperature)`` instead of ranked. ``seed``: an int
+        (item b uses ``seed + b``) or an int64 [B] tensor; an item's result depends on its prompt, its seed and the
+        scalars. With ``do_sample=False`` the sampling arguments are ignored.
+
+        Returns ``(tokens, n_new, scores)``: the ``num_return_sequences`` = r (``1 <= r <= num_beams``) best hypotheses
+        of each item, as rows ``b * r + q``, best first: int64 [B·r, max_new_tokens] (the stop token excluded, padded
+        with -1), their lengths int64 [B·r] and their normalised scores fp32 [B·r]. An item with fewer than r
+        finished hypotheses gets rows with no tokens, length 0 and score -inf.
 
         Each prompt is prefilled once and its keys and values copied to its ``num_beams`` rows of a cache of
         ``max(lengths) + max_new_tokens`` positions (more than ``n_positions`` is a ``ValueError``). On CUDA with bf16
         weights every token after the first replays one CUDA graph of decode step, LM head (``ops.lm_head_logits_``),
         the repetition controls when on (``ops.penalize_repeats_``), selection (``ops.beam_step_``) and cache
         reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the host reads the done flags once every 8
-        tokens, a period late. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
-        ``ops.repeats.penalize_repeats_reference``, ``ops.beam.BeamReference`` and torch indexing."""
-        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS
-        from ..ops.beam import BeamReference, best_hypotheses
+        tokens, a period late. Beam sampling takes a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids there, and
+        the items' seeds are a device input of the graph. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
+        ``ops.repeats.penalize_repeats_reference``, ``ops.beam.BeamReference`` (``BeamSampleReference``) and torch
+        indexing."""
+        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB
+        from ..ops.beam import BeamReference, BeamSampleReference, best_hypotheses
 
         K = int(num_beams)
         if not 1 <= K <= BEAM_MAX_BEAMS:
             raise ValueError(f"beam_search: num_beams must be in [1, {BEAM_MAX_BEAMS}], got {num_beams}")
+        R = int(num_return_sequences)
+        if not 1 <= R <= K:
+            raise ValueError(f"beam_search: num_return_sequences must be in [1, num_beams = {K}], got "
+                             f"{num_return_sequences}")
+        do_sample = bool(do_sample)
+        if do_sample and not temperature > 0:
+            raise ValueError(f"beam_search: do_sample=True needs temperature > 0, got {temperature}")
+        if do_sample and (int(top_k) < 0 or not 0 < top_p <= 1):
+            raise ValueError(f"beam_search: need top_k >= 0 and 0 < top_p <= 1, got {top_k}, {top_p}")
         if len(stop_ids) > BEAM_MAX_STOP or len(suppress_ids) > BEAM_MAX_SUPPRESS:
             raise ValueError(f"beam_search: at most {BEAM_MAX_STOP} stop ids and {BEAM_MAX_SUPPRESS} suppressed ids, "
                              f"got {len(stop_ids)} and {len(suppress_ids)}")
@@ -757,8 +779,14 @@ class GPT2DoubleHeads(nn.Module):
         del pre
         h = h.repeat_interleave(K, dim=0).contiguous()
         reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
+        seeds = _row_seeds(seed, B, dev) if do_sample else None
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
-            ref = BeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens)
+            if do_sample:
+                ref = BeamSampleReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
+                                          temperature=temperature, top_k=top_k, top_p=top_p,
+                                          seeds=seeds.cpu().tolist())
+            else:
+                ref = BeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens)
             head = weight.float()
             for i in range(n):
                 if i:
@@ -774,11 +802,15 @@ class GPT2DoubleHeads(nn.Module):
                     reps.reorder(rows)
                 if ref.done.all():
                     break
-            return tuple(t.to(dev) for t in ref.result())
+            return tuple(t.to(dev) for t in ref.result(R))
 
         from ..ops import BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
 
-        st = BeamState(B, K, n, length_penalty, dev)
+        if do_sample and V > SAMPLE_MAX_VOCAB:
+            raise ValueError(f"beam_search: do_sample=True needs a vocabulary of at most {SAMPLE_MAX_VOCAB} ids on the "
+                             f"native path, got {V}")
+        st = BeamState(B, K, n, length_penalty, dev, sample=do_sample)
+        scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds) if do_sample else {}
         logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
         sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
         prompt_len = cache.lens.clone()
@@ -788,7 +820,7 @@ class GPT2DoubleHeads(nn.Module):
             lm_head_logits_(hidden, weight, logits)
             if reps is not None:
                 reps.native(logits, cache.lens, st.step, st.next_ids, st.parent, K)
-            beam_step_(logits, V, st, min_new_tokens, sup, stop)
+            beam_step_(logits, V, st, min_new_tokens, sup, stop, **scalars)
             kv_reorder_(cache.k, cache.v, st.parent, prompt_len, cache.lens, n, scratch)
 
         select(h)                                   # the first selection, from the prefill's last positions
@@ -800,7 +832,7 @@ class GPT2DoubleHeads(nn.Module):
         fin = [list(zip(score[b], n_tok[b], src[b]))[:count[b]] for b in range(B)]
         hist_tok = st.hist_tok.view(n, B, K).cpu().numpy()
         hist_back = st.hist_back.view(n, B, K).cpu().numpy()
-        return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n))
+        return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n, R))
 
     def _generate_speculative(self, draft: Optional["GPT2DoubleHeads"], K: int, ngram: int, input_ids, lengths,
                               token_type_ids, reply_type, max_new_tokens, temperature, top_k, top_p, stop_ids,

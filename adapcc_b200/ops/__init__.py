@@ -53,6 +53,9 @@ def _lib():
         lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                          + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                          + [c_void_p] * 10 + [c_void_p])
+        lib.adapcc_beam_sample_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
+                                                + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
+                                                + [c_void_p] * 11 + [c_float, c_int, c_float, c_void_p, c_void_p])
         lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p,
                                                                                                 c_void_p]
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
@@ -437,9 +440,11 @@ class BeamState:
     each step's tokens and parent beams (0..K-1); the finished sets ``fin_score`` fp32, ``fin_n`` and ``fin_src`` int32
     [B, K] (best first: normalised score, tokens without the stop token, and the beam whose history at step
     ``fin_n - 1`` holds them) with ``fin_count`` int32 [B]; ``pen`` fp32 [max_new + 1], ``pen[L] = L ** length_penalty``
-    rounded to fp32 once on the host, so the kernel needs no ``powf``."""
+    rounded to fp32 once on the host, so the kernel needs no ``powf``. With ``sample`` (beam sampling) the candidate
+    scratch holds ``(BEAM_MAX_STOP + 1) · K`` keys per row, the most any sample draws, with ``cand_c`` fp32 beside it;
+    a step with M = ``max(2, 1 + n_stop) · K`` uses the first ``B·K·M`` entries of each as [B·K, M]."""
 
-    def __init__(self, batch: int, num_beams: int, max_new: int, length_penalty: float, device):
+    def __init__(self, batch: int, num_beams: int, max_new: int, length_penalty: float, device, sample: bool = False):
         B, K, n = int(batch), int(num_beams), int(max_new)
         if B < 1 or not 1 <= K <= BEAM_MAX_BEAMS or n < 1:
             raise ValueError(f"BeamState: need batch >= 1, 1 <= num_beams <= {BEAM_MAX_BEAMS} and max_new >= 1, got "
@@ -461,27 +466,47 @@ class BeamState:
         self.fin_count = torch.zeros(B, **i32)
         self.pen = torch.tensor([float(L) ** self.length_penalty if L else 1.0 for L in range(n + 1)],
                                 dtype=torch.float64).to(device=dev, dtype=torch.float32)
-        self.cand = torch.empty(B * K, K + BEAM_MAX_STOP, dtype=torch.int64, device=dev)
+        self.sample = bool(sample)
+        width = (BEAM_MAX_STOP + 1) * K if self.sample else K + BEAM_MAX_STOP
+        self.cand = torch.empty(B * K, width, dtype=torch.int64, device=dev)
+        self.cand_c = torch.empty(B * K, width, dtype=torch.float32, device=dev) if self.sample else None
 
     def tensors(self):
         """Every device tensor of the state (what ``beam_step_`` checks for one device)."""
         return (self.scores, self.step, self.done, self.next_ids, self.parent, self.hist_tok, self.hist_back,
-                self.fin_score, self.fin_n, self.fin_src, self.fin_count, self.pen, self.cand)
+                self.fin_score, self.fin_n, self.fin_src, self.fin_count, self.pen, self.cand, self.cand_c)
 
 
 def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int = 0,
-               suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None) -> None:
+               suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None,
+               temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
+               seeds: Optional[torch.Tensor] = None) -> None:
     """One beam-search selection for every item, on the device (the definition in ``ops/beam.py``, which computes the
     same in fp64). ``logits`` fp32 [B·K, ld] (the first ``vocab`` columns used) are the beams' next-token logits;
     ``suppress_ids`` (removed while ``state.step < min_new``) and ``stop_ids`` (at most 8; they finish a hypothesis)
     are int32 lists or None. Updates ``state``: the new beams' tokens go into ``state.next_ids``, their parents into
     ``state.parent`` (for ``kv_reorder_``), and ``state.step`` is incremented. No host sync, so it can be captured in a
-    CUDA graph."""
+    CUDA graph.
+
+    With ``seeds`` (int64 [B] on the device, each item's Philox key) the step is beam sampling
+    (``BeamSampleReference``): a ``BeamState(..., sample=True)``, ``temperature > 0``, ``top_k`` (0: off) and
+    ``top_p`` filter each beam's ids, and the candidates are drawn rather than ranked; vocab is at most
+    ``SAMPLE_MAX_VOCAB``. Without ``seeds`` the sampling scalars are ignored."""
     def bad(msg):
         raise ValueError(f"beam_step_: {msg}")
 
     if not isinstance(state, BeamState):
         bad(f"state must be a BeamState, got {type(state).__name__}")
+    if seeds is not None:
+        if not state.sample:
+            bad("sampling needs a BeamState(..., sample=True)")
+        if not temperature > 0 or not int(top_k) >= 0 or not 0 < top_p <= 1:
+            bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
+        if seeds.dtype != torch.int64 or not seeds.is_contiguous() or seeds.numel() != state.batch:
+            bad(f"seeds must be a contiguous int64 tensor of {state.batch} elements, got {seeds.dtype} "
+                f"{tuple(seeds.shape)}")
+        if vocab > SAMPLE_MAX_VOCAB:
+            bad(f"beam sampling needs vocab <= {SAMPLE_MAX_VOCAB}, got {vocab}")
     B, K = state.batch, state.num_beams
     if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1 or logits.shape[0] != B * K:
         bad(f"logits must be fp32 [{B * K}, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
@@ -491,7 +516,16 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
         bad(f"min_new must be >= 0, got {min_new}")
     sup, n_sup = _id_list("beam_step_", "suppress_ids", suppress_ids, BEAM_MAX_SUPPRESS)
     stop, n_stop = _id_list("beam_step_", "stop_ids", stop_ids, BEAM_MAX_STOP)
-    _same_device("beam_step_", logits.device, state.tensors() + (suppress_ids, stop_ids))
+    _same_device("beam_step_", logits.device, state.tensors() + (suppress_ids, stop_ids, seeds))
+    if seeds is not None:
+        _ck(_lib().adapcc_beam_sample_step(
+            _ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores), _ptr(state.step), int(min_new), sup,
+            n_sup, stop, n_stop, _ptr(state.pen), int(state.length_penalty > 0), state.max_new, _ptr(state.done),
+            _ptr(state.cand), _ptr(state.cand_c), _ptr(state.next_ids), _ptr(state.parent), _ptr(state.hist_tok),
+            _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_n), _ptr(state.fin_src),
+            _ptr(state.fin_count), float(temperature), int(top_k), float(top_p), _ptr(seeds), _stream()),
+            "beam_sample_step")
+        return
     _ck(_lib().adapcc_beam_step(_ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores),
                                 _ptr(state.step), int(min_new), sup, n_sup, stop, n_stop, _ptr(state.pen),
                                 int(state.length_penalty > 0), state.max_new, _ptr(state.done), _ptr(state.cand),

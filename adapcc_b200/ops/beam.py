@@ -25,6 +25,37 @@ is live. Per step, for every live beam row (DESIGN.md §4a):
    the normalised score.
 
 An item's result depends only on its prompt and the scalars, not on the other items.
+
+Beam sampling (``BeamSampleReference``, HuggingFace's ``_beam_search`` with ``do_sample=True``) keeps rules 1, 6 and
+7 and replaces 2-5 and 8. With ``n_stop`` stop ids, ``min_keep = max(2, 1 + n_stop)`` and ``M = min_keep · K``; per
+step, for every live beam row j of item b:
+
+S1. suppression is rule 1 (the repetition controls act before it, as in greedy mode); ``lp_i`` is rule 2's
+    log-softmax over the remaining ids;
+S2. the filter is the sampler's steps 3-6 (``ops/sampling.py``) with a minimum keep count: ``x_i = fl32(l_i / T)``;
+    top-k keeps the ``k' = max(k, min_keep)`` largest values (``k > 0``); top-p keeps i iff the weight of the kept
+    values strictly larger than ``x_i`` is ``<= p Z``, and always the ``min_keep`` largest values; tied values are
+    kept or dropped together (HuggingFace's warpers on ``lp / T`` with ``min_tokens_to_keep = min_keep``);
+S3. a kept id's candidate score is ``c = s_j + lp_i / T`` (the running sums are sums of warped log-probabilities);
+    every other id is at -inf;
+S4. the draw is an ordered sample without replacement of M candidates from the item's finite ``(j, i)`` with
+    probability proportional to ``exp(c)`` (HuggingFace's ``multinomial(softmax(c), M)`` over the flattened K·V
+    scores), by Gumbel-top-M: candidate ``(j, i)`` has the key ``g = c + G``, ``G = -log(-log u)``, ``u = ((w >> 8)
+    + 0.5) 2^-24`` with ``w`` word ``i & 3`` of Philox4x32-10 at counter ``(i >> 2, j, step, 0)`` and key ``(seed
+    mod 2^32, seed >> 32)`` of the item's seed; sorted by descending g, a tie to the lower flat index ``j·V + i``, the
+    sample is the first M (all finite ones if there are fewer). A row's own M best keys decide the sample, which is
+    what makes a bounded per-row selection exact, as in rule 5;
+S5. a candidate finishes if its token is a stop id or the step is the last (``max_new - 1``). The first K draws that
+    finish are offered in draw order: a stop id as in rule 6 (``c / L ** a``, L - 1 tokens, source beam j), otherwise
+    with ``L = max_new`` and ``max_new`` tokens, its token recorded as the last step's history slot d (its draw index)
+    with parent j. The new beams are the K largest-c (not g) drawn candidates that do not finish, in descending c,
+    ties to the earlier draw; missing beams are dead. The last step has none, so the item is done.
+
+Rules 6 and 7 are unchanged; the done rule stays exact because ``lp / T <= 0``. Item b's seed is ``seed + b`` for an
+int ``seed`` or ``seeds[b]``; its result depends on its prompt, its seed and the scalars only.
+
+``best_hypotheses(..., num_return_sequences=r)`` returns each item's first r finished hypotheses, best first, as rows
+``b · r + q`` (HuggingFace's flattening); rows past an item's count have no tokens, ``n_new`` 0 and score -inf.
 """
 from __future__ import annotations
 
@@ -144,26 +175,174 @@ class BeamReference:
         self.n_steps += 1
         return torch.from_numpy(nxt), torch.from_numpy(parent)
 
-    def result(self) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-        """``(tokens, n_new, scores)``: int64 [B, max_new] padded with -1, int64 [B], fp32 [B] of each item's best
-        hypothesis (no tokens and -inf when an item has none)."""
-        return best_hypotheses(self.fin, self.hist_tok, self.hist_back, self.max_new)
+    def result(self, num_return_sequences: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """``(tokens, n_new, scores)``: int64 [B·r, max_new] padded with -1, int64 [B·r], fp32 [B·r] of each item's r
+        best hypotheses (no tokens and -inf past an item's count)."""
+        return best_hypotheses(self.fin, self.hist_tok, self.hist_back, self.max_new, num_return_sequences)
 
 
-def best_hypotheses(fin, hist_tok, hist_back, max_new: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
-    """Each item's first finished hypothesis, its tokens followed back through the parent pointers. ``fin``: per item
-    a best-first list of ``(normalised score, n, source beam)``; ``hist_tok`` / ``hist_back`` [max_new, B, K]."""
-    B = len(fin)
-    tokens = torch.full((B, max_new), -1, dtype=torch.int64)
-    n_new = torch.zeros(B, dtype=torch.int64)
-    scores = torch.full((B,), float("-inf"), dtype=torch.float32)
+_MASK = np.uint64(0xFFFFFFFF)
+
+
+def philox_words(c0: np.ndarray, c1: int, c2: int, c3: int, seed: int) -> np.ndarray:
+    """Philox4x32-10 (``ops.sampling.philox4x32_10``) for the counters ``(c0[t], c1, c2, c3)`` and the key ``(seed mod
+    2^32, seed >> 32)``, vectorised: uint64 [len(c0), 4], the four output words of each counter."""
+    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    n = len(c0)
+    c = [np.asarray(c0, dtype=np.uint64) & _MASK] + [np.full(n, int(v) & 0xFFFFFFFF, dtype=np.uint64)
+                                                     for v in (c1, c2, c3)]
+    k0, k1 = np.uint64(seed & 0xFFFFFFFF), np.uint64(seed >> 32)
+    m0, m1 = np.uint64(0xD2511F53), np.uint64(0xCD9E8D57)
+    w0, w1, s32 = np.uint64(0x9E3779B9), np.uint64(0xBB67AE85), np.uint64(32)
+    for _ in range(10):
+        p0, p1 = m0 * c[0], m1 * c[2]
+        c = [(p1 >> s32) ^ c[1] ^ k0, p1 & _MASK, (p0 >> s32) ^ c[3] ^ k1, p0 & _MASK]
+        k0, k1 = (k0 + w0) & _MASK, (k1 + w1) & _MASK
+    return np.stack(c, axis=1)
+
+
+def gumbel(w: np.ndarray) -> np.ndarray:
+    """``G = -log(-log u)`` in fp64 for ``u = ((w >> 8) + 0.5) 2^-24`` (rule S4)."""
+    u = ((np.asarray(w, dtype=np.uint64) >> np.uint64(8)).astype(np.float64) + 0.5) * 2.0 ** -24
+    return -np.log(-np.log(u))
+
+
+def sample_keep(x: np.ndarray, top_k: int, top_p: float, min_keep: int) -> np.ndarray:
+    """Rule S2 on the fp32 values ``x = fl32(l / T)`` (-inf: removed): the bool mask of the kept ids, in fp64."""
+    cand = x > -np.inf
+    kept = cand.copy()
+    n = int(cand.sum())
+    if n == 0:
+        return kept
+    desc = np.sort(x[cand].astype(np.float64))[::-1]
+    k = max(int(top_k), min_keep) if top_k > 0 else 0
+    if 0 < k < n:
+        kept &= x >= desc[k - 1]
+    p = float(np.float32(top_p))
+    if p < 1.0:
+        xd = x.astype(np.float64)
+        m = xd[kept].max()
+        e = np.where(kept, np.exp(np.where(kept, xd - m, 0.0)), 0.0)
+        order = np.argsort(-xd[kept], kind="stable")
+        vals, csum = xd[kept][order], np.cumsum(e[kept][order])
+        first = np.searchsorted(-vals, -vals, side="left")    # the weight of the strictly larger values
+        tail = np.full(x.size, np.inf)
+        tail[np.flatnonzero(kept)[order]] = np.where(first > 0, csum[np.maximum(first - 1, 0)], 0.0)
+        keep_p = ~(tail > p * float(e.sum()))
+        keep_p |= x >= (desc[min_keep - 1] if min_keep < n else -np.inf)
+        kept &= keep_p
+    return kept
+
+
+class BeamSampleReference(BeamReference):
+    """Beam sampling (rules S1-S5 with 6 and 7, see the module docstring) for ``batch`` items in fp64, with the
+    interface of ``BeamReference``. ``seeds``: one int per item (its Philox key). ``temperature > 0`` and ``top_p`` are
+    rounded to fp32, as the kernel takes them; ``top_k = 0`` is off."""
+
+    def __init__(self, batch: int, num_beams: int, max_new: int, vocab: int, length_penalty: float = 1.0,
+                 stop_ids: Sequence[int] = (), suppress_ids: Sequence[int] = (), min_new: int = 0,
+                 early_stop: bool = True, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
+                 seeds: Sequence[int] = ()):
+        super().__init__(batch, num_beams, max_new, vocab, length_penalty, stop_ids, suppress_ids, min_new,
+                         early_stop)
+        if not temperature > 0 or int(top_k) < 0 or not 0 < top_p <= 1:
+            raise ValueError(f"BeamSampleReference: need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got "
+                             f"{temperature}, {top_k}, {top_p}")
+        self.seeds = [int(x) for x in seeds]
+        if len(self.seeds) != self.B:
+            raise ValueError(f"BeamSampleReference: need {self.B} seeds, got {len(self.seeds)}")
+        self.T = float(np.float32(temperature))
+        self.top_k, self.top_p = int(top_k), float(top_p)
+        self.min_keep = max(2, 1 + len(self.stop))
+        self.M = self.min_keep * self.K
+
+    def row_candidates(self, b: int, j: int, logits_row: np.ndarray, step: int):
+        """Rules S1-S4 for beam row j of item b: ``(ids, c, g)`` of its kept ids (fp64), in id order."""
+        s = self.scores[b, j]
+        x = np.array(logits_row[:self.vocab], dtype=np.float32)
+        if step < self.min_new and self.suppress.size:
+            x[self.suppress] = -np.inf
+        fin = x > -np.inf
+        if not np.isfinite(s) or not fin.any():
+            return np.zeros(0, dtype=np.int64), np.zeros(0), np.zeros(0)
+        xd = x.astype(np.float64)
+        m = xd[fin].max()
+        lp = (xd - m) - np.log(np.exp(xd[fin] - m).sum())
+        ids = np.flatnonzero(sample_keep((x / np.float32(self.T)).astype(np.float32), self.top_k, self.top_p,
+                                         self.min_keep))
+        c = s + lp[ids] / self.T
+        w = philox_words(ids >> 2, j, step, 0, self.seeds[b])[np.arange(ids.size), ids & 3]
+        return ids, c, c + gumbel(w)
+
+    def draws(self, b: int, logits: np.ndarray, step: int) -> List[Tuple[float, float, int, int]]:
+        """Item b's sample (rule S4): ``(g, c, j, i)`` in draw order, at most M."""
+        V = self.vocab
+        g, c, flat = [], [], []
+        for j in range(self.K):
+            ids, cj, gj = self.row_candidates(b, j, logits[b * self.K + j], step)
+            g.append(gj)
+            c.append(cj)
+            flat.append(j * V + ids)
+        g, c, flat = np.concatenate(g), np.concatenate(c), np.concatenate(flat)
+        order = np.lexsort((flat, -g))[:self.M]
+        return [(float(g[o]), float(c[o]), int(flat[o]) // V, int(flat[o]) % V) for o in order]
+
+    def step(self, logits) -> Tuple[torch.Tensor, torch.Tensor]:
+        """One step (rules S1-S5, 6 and 7) for every item that is not done."""
+        if isinstance(logits, torch.Tensor):
+            logits = logits.detach().float().cpu().numpy()
+        B, K = self.B, self.K
+        step = self.n_steps
+        if step >= self.max_new:
+            raise ValueError(f"BeamSampleReference: all {self.max_new} steps taken")
+        nxt = np.zeros(B * K, dtype=np.int64)
+        parent = np.arange(B * K, dtype=np.int64)
+        L, last = step + 1, step == self.max_new - 1
+        for b in range(B):
+            if self.done[b]:
+                continue
+            sample = self.draws(b, logits, step)
+            finishes = [last or i in self.stop for _, _, _, i in sample]
+            for d, (_, c, j, i) in enumerate(sample[:K]):
+                if i in self.stop:
+                    self.offer(b, c / self.penalty(L), L - 1, j)
+                elif last:
+                    self.offer(b, c / self.penalty(self.max_new), self.max_new, d)
+            live = sorted((d for d in range(len(sample)) if not finishes[d]), key=lambda d: (-sample[d][1], d))[:K]
+            new = np.full(K, -np.inf)
+            for k in range(K):
+                e = k if last else (live[k] if k < len(live) else -1)
+                if 0 <= e < len(sample):
+                    _, c, j, i = sample[e]
+                    self.hist_tok[step, b, k], self.hist_back[step, b, k] = i, j
+                    if not last:
+                        new[k], nxt[b * K + k], parent[b * K + k] = c, i, b * K + j
+                else:
+                    self.hist_tok[step, b, k], self.hist_back[step, b, k] = -1, k
+            self.scores[b] = new
+            if last or not live:
+                self.done[b] = True
+            elif self.early_stop and len(self.fin[b]) == K:
+                reach = new[0] / self.penalty(self.max_new if self.alpha > 0 else L + 1)
+                self.done[b] = not reach > self.fin[b][-1][0]
+        self.n_steps += 1
+        return torch.from_numpy(nxt), torch.from_numpy(parent)
+
+
+def best_hypotheses(fin, hist_tok, hist_back, max_new: int,
+                    num_return_sequences: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Each item's first ``num_return_sequences`` = r finished hypotheses, their tokens followed back through the
+    parent pointers, as rows ``b * r + q``. ``fin``: per item a best-first list of ``(normalised score, n, source
+    beam)``; ``hist_tok`` / ``hist_back`` [max_new, B, K]. Rows past an item's count: tokens -1, 0 and -inf."""
+    B, R = len(fin), int(num_return_sequences)
+    tokens = torch.full((B * R, max_new), -1, dtype=torch.int64)
+    n_new = torch.zeros(B * R, dtype=torch.int64)
+    scores = torch.full((B * R,), float("-inf"), dtype=torch.float32)
     for b in range(B):
-        if not fin[b]:
-            continue
-        score, n, src = fin[b][0]
-        r = int(src)
-        for u in range(int(n) - 1, -1, -1):
-            tokens[b, u] = int(hist_tok[u, b, r])
-            r = int(hist_back[u, b, r])
-        n_new[b], scores[b] = int(n), float(score)
+        for q, (score, n, src) in enumerate(fin[b][:R]):
+            row, r = b * R + q, int(src)
+            for u in range(int(n) - 1, -1, -1):
+                tokens[row, u] = int(hist_tok[u, b, r])
+                r = int(hist_back[u, b, r])
+            n_new[row], scores[row] = int(n), float(score)
     return tokens, n_new, scores

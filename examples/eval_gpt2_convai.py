@@ -38,6 +38,9 @@ def main():
                         "before filtering, so its F1 is a different sample")
     p.add_argument("--num_beams", type=int, default=0,
                    help="f1: decode the replies with GPT2DoubleHeads.beam_search and this many beams (0: sample)")
+    p.add_argument("--beam_sample", action="store_true",
+                   help="f1 with --num_beams: beam sampling, the beams' candidates drawn with --temperature, --top_k "
+                        "and --top_p instead of ranked")
     p.add_argument("--repetition_penalty", type=float, default=1.0,
                    help="f1: penalty on ids already in the prompt or reply (1: off); replies go through the batched path")
     p.add_argument("--no_repeat_ngram_size", type=int, default=0,
@@ -80,7 +83,7 @@ def main():
                   no_sample=a.no_sample, repetition_penalty=a.repetition_penalty,
                   no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha,
                   prompt_lookup_num_tokens=a.prompt_lookup_num_tokens, min_p=a.min_p, typical_p=a.typical_p,
-                  epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff)
+                  epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, beam_sample=a.beam_sample)
         if a.assistant_checkpoint:
             kw["assistant_model"] = load_model_from_checkpoint(
                 a.assistant_checkpoint, a.device, torch.bfloat16 if a.device.startswith("cuda") else None)[0]

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""GPT-2 small beam search: ``GPT2DoubleHeads.beam_search`` against greedy ``generate`` at the same number of rows, and
-the selection and cache-reordering kernels on their own.
+"""GPT-2 small beam search: ``GPT2DoubleHeads.beam_search`` against greedy ``generate`` at the same number of rows,
+beam sampling against beam search, and the selection and cache-reordering kernels on their own.
 
 Prints one JSON line with the device name and power limit read in the same run. Needs a CUDA device (there is no CPU
 fallback) and writes nothing into the repository.
@@ -13,7 +13,10 @@ fallback) and writes nothing into the repository.
 * ``kernels``: ``beam_step_`` (vocab 50257) and ``kv_reorder_`` (12 layers, 12 heads, Dh 64, every row taking another
   row's cache) at 64 rows (8 items x 8 beams) with 16 and 64 generated positions, 50 launches captured in a CUDA graph
   and timed with CUDA events over ``--launches`` launches. GB/s for the reorder counts the generated region read and
-  written twice (into the scratch and back).
+  written twice (into the scratch and back). Also the sampled ``beam_step_`` (temperature 1, no top-k, every id kept)
+  with top-p 1 and 0.9.
+* ``sampled``: ``beam_search(do_sample=True, top_k=50)`` against ``do_sample=False``, ms per generated token as in
+  ``search``, the two alternated run by run in this process (medians of ``--reps`` pairs after one warm-up each).
 
 Usage: ``python tools/beam_bench.py [--reps 3] [--launches 1000]``
 """
@@ -70,6 +73,34 @@ def bench_search(model, reps):
     return rows
 
 
+def bench_sampled(model, reps):
+    rows = []
+    g = torch.Generator(device="cuda").manual_seed(2)
+    for B in (1, 8):
+        for K in (4, 8):
+            for T in (128, 512):
+                prompt = torch.randint(0, model.cfg.vocab_size, (B, T), device="cuda", generator=g)
+                runs = {False: lambda: model.beam_search(prompt, num_beams=K, max_new_tokens=NEW_TOKENS),
+                        True: lambda: model.beam_search(prompt, num_beams=K, max_new_tokens=NEW_TOKENS,
+                                                        do_sample=True, temperature=1.0, top_k=50, seed=3)}
+                times = {False: [], True: []}
+                for sample in (False, True):
+                    runs[sample]()                                 # warm-up of this shape
+                for _ in range(reps):
+                    for sample in (False, True):
+                        torch.cuda.synchronize()
+                        t0 = time.perf_counter()
+                        runs[sample]()
+                        torch.cuda.synchronize()
+                        times[sample].append((time.perf_counter() - t0) * 1e3)
+                greedy, sampled = (statistics.median(times[x]) for x in (False, True))
+                rows.append({"batch": B, "beams": K, "prompt": T,
+                             "beam_search_ms_per_token": round(greedy / NEW_TOKENS, 3),
+                             "beam_sample_ms_per_token": round(sampled / NEW_TOKENS, 3),
+                             "sample_cost_ms_per_token": round((sampled - greedy) / NEW_TOKENS, 3)})
+    return rows
+
+
 def _graph_us(fn, launches):
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -108,6 +139,12 @@ def bench_kernels(model, launches):
     st.scores.zero_()
     step_us = _graph_us(lambda: beam_step_(logits, cfg.vocab_size, st), launches)
     out = {"rows": B * K, "lm_head_us": round(lm_us, 2), "beam_step_us": round(step_us, 2), "kv_reorder": []}
+    seeds = torch.arange(B, dtype=torch.int64, device="cuda")
+    for top_p in (1.0, 0.9):
+        st = BeamState(B, K, max_new, 1.0, "cuda", sample=True)
+        st.scores.zero_()
+        us = _graph_us(lambda: beam_step_(logits, cfg.vocab_size, st, top_p=top_p, seeds=seeds), launches)
+        out[f"beam_sample_step_top_p_{top_p}_us"] = round(us, 2)
     L, H, Dh, T = cfg.n_layer, cfg.n_head, cfg.n_embd // cfg.n_head, 512
     for gen in (16, 64):
         cache = model.new_cache(B * K, T + 64)
@@ -141,7 +178,7 @@ def main():
     torch.manual_seed(0)
     model = GPT2DoubleHeads(GPT2Config()).to(device="cuda", dtype=torch.bfloat16).eval()
     result = dict(info, new_tokens=NEW_TOKENS, kernels=bench_kernels(model, args.launches),
-                  search=bench_search(model, args.reps))
+                  search=bench_search(model, args.reps), sampled=bench_sampled(model, args.reps))
     print(json.dumps(result))
 
 
