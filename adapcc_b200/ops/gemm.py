@@ -38,8 +38,9 @@ def supported(x: torch.Tensor, weight: torch.Tensor) -> bool:
 def default_variant() -> int:
     """0: one output tile per CTA. 1: persistent CTAs. 2: two-CTA clusters that share the W slab by TMA multicast,
     one 256 x 256 tile per cluster. 3 (default): persistent two-CTA clusters, the only variant with the column-sum
-    output the MLP backward uses; shapes it does not cover (N % 256 != 0) go to variant 1. All four are checked against
-    fp32 references by the GPU tests (tests/test_gpu_tcgen05*.py; the file names predate the H100 port)."""
+    output the MLP backward uses; shapes it does not cover (N % 256 != 0) go to variant 1. All four are checked element by
+    element against fp64 references, and against each other bit for bit, by ``test_gemm_against_fp64``
+    (tests/test_gpu_kernels_reference.py), at shapes where a persistent CTA runs many tiles included."""
     return int(os.environ.get("ADAPCC_TCGEN05_VARIANT", "3"))
 
 

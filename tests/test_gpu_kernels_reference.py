@@ -113,17 +113,30 @@ def check_colsum(colsum, out):
 
 
 GEMM_M = [1, 8, 127, 129, 255, 257]
+# Shapes where a persistent CTA (132 of them) or CTA pair (66) computes many tiles one after the other, so the stage
+# ring's barrier parity, the epilogue staging ring and the aux prefetch all carry over from tile to tile:
+GEMM_MANY_TILES = [
+    (3072, 768, 8192),      # GPT-2's MLP up-projection: 384 pair tiles over 66 pairs, unevenly (5 or 6 each)
+    (768, 3072, 8192),      # ... and its down-projection: 96 pair tiles, 48 K slabs = 16 trips round the 3-stage ring
+    (3072, 768, 8193),      # odd number of row tiles: the last pair's second half is empty on all 12 column tiles
+    (1024, 64, 40000),      # one K slab per tile, 9 or 10 tiles per pair: each stage of the ring serves a different
+                            # tile on every use and its barrier parity goes 0, 1, 0 within one launch
+    (384, 768, 20000),      # 128-wide tiles (variants 0 / 1): 471 tiles over the persistent CTAs
+]
+GEMM_CASES = [(n, k, m) for n, k in ((256, 192), (384, 768)) for m in GEMM_M] + GEMM_MANY_TILES
 
 
 @gpu
-@pytest.mark.parametrize("m", GEMM_M)
-@pytest.mark.parametrize("n,k", [(256, 192), (384, 768)])
+@pytest.mark.parametrize("n,k,m", GEMM_CASES)
 def test_gemm_against_fp64(dev, m, n, k):
     """Every variant at ragged M (one row, below one tile, one past a tile, odd numbers of row tiles for the CTA-pair
     variants), 256-wide (N % 256 == 0) and 128-wide tiles, with and without bias; `pre` against the fp64 GEMM and `out`
-    against fp64 GELU of the kernel's own `pre`; the aux epilogues (dGELU, residual, column sums) at the same shapes.
+    against fp64 GELU of the kernel's own `pre`; the aux epilogues (dGELU, residual, column sums) at the same shapes,
+    their aux holding values up to +-40 where gelu' has saturated to 1 or 0.
     Variants differ only in which CTA computes a tile: the K-slab order, the wgmma sequence and the swizzled smem layout
-    (a multicast half lands exactly where a plain load would) are the same, so the bits must be identical."""
+    (a multicast half lands exactly where a plain load would) are the same, so the bits must be identical. Variant 0
+    launches one CTA per tile, so at the many-tile shapes this equality pins the persistent variants' tile-to-tile
+    state exactly."""
     from adapcc_b200.ops.gemm import linear_act
 
     torch.manual_seed(1000 * m + n + k)
@@ -142,7 +155,11 @@ def test_gemm_against_fp64(dev, m, n, k):
                 check_gelu(out, pre)
             for v in variants[1:]:
                 assert torch.equal(res[v][0], out) and torch.equal(res[v][1], pre), (act, bias is None, v)
-    aux = torch.randn(m, n, device=dev).bfloat16()
+    del res
+    aux = torch.randn(m, n, device=dev)
+    at = torch.arange(0, m * n, 97, device=dev)                     # 97 is coprime to every N here: all columns are hit
+    aux.view(-1)[at] = torch.tensor([3.0, -3.0, 6.0, -6.0, 12.0, -12.0, 40.0, -40.0], device=dev)[(at // 97) % 8]
+    aux = aux.bfloat16()
     dg, _ = linear_act(x, w, None, "dgelu", aux=aux, variant=0)
     check_dgelu(dg, x, w, aux)
     rs, _ = linear_act(x, w, b, "residual", aux=aux, variant=0)
@@ -362,6 +379,301 @@ def test_ln_checker_rejects_perturbed_reference():
         check_ln(y, mu[[1, 0] + list(range(2, 9))], rs, x, gamma, beta, 1e-5)   # one row's statistics swapped
     with pytest.raises(AssertionError):
         check_ln(y, mu, rs[[1, 0] + list(range(2, 9))], x, gamma, beta, 1e-5)
+
+
+# ---- fused add-LayerNorm forward -------------------------------------------------------------------------------------
+LN_WIDTHS = [256, 512, 768, 1024]
+# one row, one short of / exactly / one past a CTA's 8 rows, two unequal passes of the persistent grid at every
+# width (4099), and about ten passes with idle CTAs and a 3-row group in the last one (20011)
+LN_ROWS = [1, 7, 8, 9, 4099, 20011]
+NAN16 = 0x7FC0            # the bf16 quiet NaN torch.full writes: the bit pattern of untouched output
+
+
+def _same_bits(a, b):
+    return a.shape == b.shape and torch.equal(a.contiguous().view(torch.int16), b.contiguous().view(torch.int16))
+
+
+def _nan16(*shape, device):
+    return torch.full(shape, float("nan"), dtype=torch.bfloat16, device=device)
+
+
+def _untouched(t):
+    return bool((t.view(torch.int16) == NAN16).all())
+
+
+def _add_ln_fwd(x, res, gamma, beta, eps):
+    """adapcc_add_ln_fwd into NaN-filled outputs with one guard row past `rows` -> (sum_out, y, mean, rstd)."""
+    from adapcc_b200.ops.layers import _lib, _p, _s
+    from adapcc_b200.runtime.native import last_error
+
+    rows, d = x.shape
+    sum_out, y = _nan16(rows + 1, d, device=x.device), _nan16(rows + 1, d, device=x.device)
+    mean = torch.full((rows,), float("nan"), dtype=torch.float32, device=x.device)
+    rstd = torch.full((rows,), float("nan"), dtype=torch.float32, device=x.device)
+    rc = _lib().adapcc_add_ln_fwd(_p(x), _p(res), _p(gamma), _p(beta), _p(sum_out), _p(y), _p(mean), _p(rstd), rows, d,
+                                  eps, _s())
+    assert rc == 0, last_error()
+    assert _untouched(sum_out[rows]) and _untouched(y[rows]), "add_ln_fwd wrote past its last row"
+    return sum_out[:rows], y[:rows], mean, rstd
+
+
+def _add_ln_input(rows, d, kind, g):
+    """(x, res) whose sum is an `_ln_input` kind, nearly cancels, or is exactly constant on every other row."""
+    if kind == "cancel":
+        x = _ln_input(rows, d, "normal", g)
+        return x, (-x.float() + torch.randn(rows, d, generator=g) * 0.01).bfloat16()   # sum ~ 0.01, spacing of x ~ 0.01
+    if kind == "constsum":
+        x = torch.randint(-32, 33, (rows, d), generator=g).float()                     # small integers: exact in bf16
+        res = torch.randn(rows, d, generator=g)
+        res[::2] = 3.0 - x[::2]                                                         # x + res = 3 exactly: variance 0
+        return x.bfloat16(), res.bfloat16()
+    return _ln_input(rows, d, kind, g), (torch.randn(rows, d, generator=g) * 0.5).bfloat16()
+
+
+@gpu
+@pytest.mark.parametrize("d", LN_WIDTHS)
+@pytest.mark.parametrize("rows", LN_ROWS)
+@pytest.mark.parametrize("kind", ["normal", "offset", "cancel", "constsum"])
+def test_add_layernorm_forward_against_fp64(dev, d, rows, kind):
+    """The fused residual add: `sum_out` is the bf16 add bit for bit (one fp32 add, one rounding to nearest), and y,
+    mean, rstd are the LayerNorm of that ROUNDED sum, held to the bounds of `check_ln`."""
+    g = torch.Generator().manual_seed(3 * d + rows)
+    x, res = (t.to(dev) for t in _add_ln_input(rows, d, kind, g))
+    gamma = (torch.randn(d, generator=g) * 0.5 + 1).bfloat16().to(dev)
+    beta = (torch.randn(d, generator=g) * 0.1).bfloat16().to(dev)
+    s, y, mean, rstd = _add_ln_fwd(x, res, gamma, beta, 1e-5)
+    assert _same_bits(s, x + res)
+    if kind == "constsum":
+        assert torch.all(s[::2] == 3.0)
+    check_ln(y, mean, rstd, s, gamma, beta, 1e-5)
+
+
+@gpu
+def test_add_layernorm_forward_rejects_null_residual(dev):
+    """Without `res` or `sum_out` the entry point reports an error and launches nothing."""
+    from ctypes import c_void_p
+
+    from adapcc_b200.ops.layers import _lib, _p, _s
+    from adapcc_b200.runtime.native import last_error
+
+    lib = _lib()
+    rows, d = 9, 256
+    x = torch.randn(rows, d, device=dev).bfloat16()
+    gamma, beta = torch.ones(d, device=dev).bfloat16(), torch.zeros(d, device=dev).bfloat16()
+    s, y = _nan16(rows, d, device=dev), _nan16(rows, d, device=dev)
+    mean, rstd = torch.zeros(rows, device=dev), torch.zeros(rows, device=dev)
+    before = lib.adapcc_launch_count()
+    for res_p, sum_p in ((c_void_p(0), _p(s)), (_p(x), c_void_p(0))):
+        assert lib.adapcc_add_ln_fwd(_p(x), res_p, _p(gamma), _p(beta), sum_p, _p(y), _p(mean), _p(rstd), rows, d, 1e-5,
+                                     _s()) == -1
+        assert "res and sum_out" in last_error()
+    torch.cuda.synchronize()
+    assert lib.adapcc_launch_count() == before
+    assert _untouched(s) and _untouched(y)
+
+
+# ---- LayerNorm backward --------------------------------------------------------------------------------------------
+def _g(k):
+    """k successive fp32 roundings move a value by at most k u / (1 - k u), relatively."""
+    return k * U32 / (1 - k * U32)
+
+
+def _ln_bwd_terms(dy, x, gamma, mean, rstd):
+    """fp64 (xh, gy, c1, c2, rstd column) of the backward, from the fp32 statistics it is handed."""
+    rs = rstd.double()[:, None]
+    xh = (x.double() - mean.double()[:, None]) * rs
+    gy = dy.double() * gamma.double()
+    return xh, gy, gy.mean(1, keepdim=True), (gy * xh).mean(1, keepdim=True), rs
+
+
+def check_ln_bwd(dx, dgamma, dbeta, dy, x, gamma, mean, rstd, dres=None):
+    """dx = bf16(rstd (gy - c1 - xh c2) [+ dres]), dgamma = bf16(sum_rows dy xh), dbeta = bf16(sum_rows dy), with
+    xh = (x - mean) rstd, gy = dy gamma, c1 = mean_D(gy), c2 = mean_D(gy xh).
+
+    `mean` / `rstd` are the forward kernel's own fp32 outputs, taken as exact inputs here: `check_ln` bounds them
+    against fp64, so the two checks compose into one of the whole LayerNorm.
+
+    What the kernel rounds (fp32 unless said), each term of the bounds below in the same order:
+      xh    two roundings (the subtraction, the product); gy = dy gamma is exact (8 x 8 significant bits).
+      c1    a lane adds D / 32 values, 5 shuffle levels, the product with the rounded 1 / D: D / 32 + 6 roundings of
+            partial sums bounded by sum |gy|.
+      c2    the same tree over gy xh, whose terms carry xh's two roundings and the product's: D / 32 + 9, of
+            sum |gy xh|.
+      dx    gy and c1 go through gy - c1, the subtraction of xh c2 and the product with rstd (3 roundings); xh c2
+            through xh's two, its product and the same last two (5). With dres one more rounding of the sum. Then ONE
+            bf16 rounding. Everything is relative to rstd (|gy| + |c1| + |xh c2|), not to |dx|: the terms cancel.
+      dgamma, dbeta   fp32 sums of `rows` terms in whatever order the per-lane, per-CTA and finalising passes take
+            (rows + 64 roundings covers any order, as in `check_colsum_bf16`); a dgamma term also carries xh's two
+            roundings and the product's; then one bf16 rounding."""
+    xh, gy, c1, c2, rs = _ln_bwd_terms(dy, x, gamma, mean, rstd)
+    rows, d = xh.shape
+    depth = d / 32 + 6
+    dc1 = _g(depth) * gy.abs().mean(1, keepdim=True)
+    dc2 = _g(depth + 3) * (gy * xh).abs().mean(1, keepdim=True)
+    ref = rs * (gy - c1 - xh * c2)
+    e = rs * (dc1 + xh.abs() * dc2 + _g(3) * (gy.abs() + c1.abs() + dc1) + _g(5) * xh.abs() * (c2.abs() + dc2))
+    if dres is not None:
+        ref = ref + dres.double()
+        e = e + U32 * (ref.abs() + e)
+    assert_within(dx, ref, e + U16 * (ref.abs() + e), "layernorm dx")
+    for got, term, per_term, what in ((dgamma, dy.double() * xh, 3, "dgamma"), (dbeta, dy.double(), 0, "dbeta")):
+        want = term.sum(0)
+        e = _g(rows + 64 + per_term) * term.abs().sum(0)
+        assert_within(got, want, e + U16 * (want.abs() + e), f"layernorm {what}")
+
+
+def _ln_bwd_grid(rows, d):
+    """The backward's persistent grid (csrc/ops_norm.cu): 8 rows per CTA pass, at most 2 CTAs per SM (1 at D = 1024),
+    shrunk until every CTA runs the same number of passes but the last."""
+    groups = max(1, -(-rows // 8))
+    cap = torch.cuda.get_device_properties(0).multi_processor_count * (2 if d <= 768 else 1)
+    iters = -(-groups // cap)
+    return -(-groups // iters)
+
+
+def _sparse_rows(rows, grid):
+    """Row 0, the last row, and a row of the last 8-row group that the middle CTA of `grid` runs."""
+    groups, c = -(-rows // 8), grid // 2
+    last_group = c + (groups - 1 - c) // grid * grid
+    return sorted({0, rows - 1, min(last_group * 8 + 3, rows - 1)})
+
+
+def _ln_bwd_case(rows, d, xkind, dykind, keep, g, device):
+    """-> (x, dy, gamma). dykind "random": gamma has zeros and negative entries; "rowconst": dy constant along each row
+    and gamma constant, so gy = c1 and dx cancels to the rounding of c2; "sparse": "random" with dy zero outside the
+    rows `keep`, so every surviving term of dgamma / dbeta is visible at full precision."""
+    x = _ln_input(rows, d, xkind, g)
+    if dykind == "rowconst":
+        gamma = torch.full((d,), 1.5)
+        dy = (torch.randn(rows, 1, generator=g) * 2).expand(rows, d)
+    else:
+        gamma = torch.randn(d, generator=g) * 0.5 + 1
+        gamma[::5] = 0.0
+        gamma[1::7] *= -1.0
+        dy = torch.randn(rows, d, generator=g)
+        if dykind == "sparse":
+            mask = torch.zeros(rows, 1)
+            mask[keep] = 1.0
+            dy = dy * mask
+    return x.to(device), dy.bfloat16().contiguous().to(device), gamma.bfloat16().to(device)
+
+
+def _ln_bwd(dy, x, gamma, mean, rstd, dres=None, add=False):
+    """adapcc_ln_bwd (or adapcc_add_ln_bwd when `add`) into NaN-filled outputs -> (dx, dgamma, dbeta, part).
+
+    `part` is handed over at exactly 2 * adapcc_ln_partials(rows) * d floats, NaN-filled, with NaN guards behind it;
+    dx has one guard row. Neither guard may change."""
+    from ctypes import c_void_p
+
+    from adapcc_b200.ops.layers import _lib, _p, _s
+    from adapcc_b200.runtime.native import last_error
+
+    lib = _lib()
+    rows, d = x.shape
+    dx, dgamma, dbeta = _nan16(rows + 1, d, device=x.device), _nan16(d, device=x.device), _nan16(d, device=x.device)
+    n = 2 * lib.adapcc_ln_partials(rows) * d
+    scratch = torch.full((n + 1024,), float("nan"), dtype=torch.float32, device=x.device)
+    if add:
+        rc = lib.adapcc_add_ln_bwd(_p(dy), _p(x), _p(gamma), _p(mean), _p(rstd),
+                                   c_void_p(0) if dres is None else _p(dres), _p(dx), _p(dgamma), _p(dbeta),
+                                   _p(scratch), rows, d, _s())
+    else:
+        assert dres is None
+        rc = lib.adapcc_ln_bwd(_p(dy), _p(x), _p(gamma), _p(mean), _p(rstd), _p(dx), _p(dgamma), _p(dbeta),
+                               _p(scratch), rows, d, _s())
+    assert rc == 0, last_error()
+    assert _untouched(dx[rows]), "ln_bwd wrote past its last row"
+    assert bool(torch.isnan(scratch[n:]).all()), "ln_bwd wrote past its scratch"
+    return dx[:rows], dgamma, dbeta, scratch[:n]
+
+
+@gpu
+@pytest.mark.parametrize("d", LN_WIDTHS)
+@pytest.mark.parametrize("rows", LN_ROWS)
+@pytest.mark.parametrize("xkind", ["normal", "constant", "offset"])
+def test_layernorm_backward_against_fp64(dev, d, rows, xkind):
+    """Both entry points, with and without the residual-stream gradient, for every kind of dy. Constant rows of x have
+    xh = 0 and rstd = 1 / sqrt(eps): dx is rstd (gy - c1) alone, 316 times the usual scale.
+
+    Scratch layout: the dgamma partials are rows 0 .. grid - 1 of `part`, the dbeta partials start at grid * d (not
+    at the half-way point), and nothing past 2 * grid * d is written; at d = 1024 the grid is smaller than
+    adapcc_ln_partials(rows). The fp32 partials, summed in fp64, are held to dgamma's and dbeta's bounds WITHOUT the
+    output rounding.
+
+    Bits: the two entry points agree without dres; a second launch repeats dx, dgamma, dbeta; a row computed alone
+    (rows = 1) equals that row of the batch."""
+    from adapcc_b200.ops.layers import _lib
+
+    grid, partials = _ln_bwd_grid(rows, d), _lib().adapcc_ln_partials(rows)
+    assert grid == partials if d <= 768 else grid <= partials
+    keep = _sparse_rows(rows, grid)
+    g = torch.Generator().manual_seed(5 * d + rows)
+    for dykind in ("random", "rowconst", "sparse"):
+        x, dy, gamma = _ln_bwd_case(rows, d, xkind, dykind, keep, g, dev)
+        _, mean, rstd = _ln_fwd(x, gamma, torch.zeros_like(gamma), 1e-5)
+        dx, dgamma, dbeta, part = _ln_bwd(dy, x, gamma, mean, rstd)
+        check_ln_bwd(dx, dgamma, dbeta, dy, x, gamma, mean, rstd)
+        assert bool(torch.isfinite(part[:2 * grid * d]).all()), dykind
+        assert bool(torch.isnan(part[2 * grid * d:]).all()), dykind
+        xh, gy, c1, c2, rs = _ln_bwd_terms(dy, x, gamma, mean, rstd)
+        for p, term, per_term in ((part[:grid * d], dy.double() * xh, 3), (part[grid * d:2 * grid * d], dy.double(), 0)):
+            assert_within(p.view(grid, d).double().sum(0), term.sum(0), _g(rows + 64 + per_term) * term.abs().sum(0),
+                          f"layernorm backward partials ({dykind})")
+        again = _ln_bwd(dy, x, gamma, mean, rstd, add=True)
+        assert all(_same_bits(a, b) for a, b in zip(again[:3], (dx, dgamma, dbeta))), dykind
+        pre = rs * (gy - c1 - xh * c2)
+        del xh, gy
+        torch.manual_seed(rows + d)
+        # a random gradient on the residual stream, and one that cancels dx to the rounding error of its fp32 value:
+        # rounding before the add (bf16 twice) would then give exactly 0
+        for name, dres in (("random", torch.randn(rows, d, device=dev).bfloat16()), ("cancel", (-pre).bfloat16())):
+            dxr, dgr, dbr, _ = _ln_bwd(dy, x, gamma, mean, rstd, dres=dres, add=True)
+            check_ln_bwd(dxr, dgr, dbr, dy, x, gamma, mean, rstd, dres=dres)
+            assert _same_bits(dgr, dgamma) and _same_bits(dbr, dbeta), (dykind, name)
+            again = _ln_bwd(dy, x, gamma, mean, rstd, dres=dres, add=True)
+            assert all(_same_bits(a, b) for a, b in zip(again[:3], (dxr, dgr, dbr))), (dykind, name)
+            for r in keep:
+                alone = _ln_bwd(dy[r:r + 1], x[r:r + 1], gamma, mean[r:r + 1], rstd[r:r + 1], dres=dres[r:r + 1],
+                                add=True)[0]
+                assert _same_bits(alone[0], dxr[r]), (dykind, name, r)
+
+
+def test_ln_bwd_checker_rejects_perturbed_reference():
+    """The exact result passes; a backward without c1, without c2, with dres added after dx was rounded, with dgamma and
+    dbeta swapped, or with one row missing from dgamma does not."""
+    g = torch.Generator().manual_seed(0)
+    rows, d = 4099, 512
+    keep = _sparse_rows(rows, 257)
+
+    def case(dykind):
+        x, dy, gamma = _ln_bwd_case(rows, d, "normal", dykind, keep, g, "cpu")
+        x64 = x.double()
+        mu = x64.mean(1)
+        mean, rstd = mu.float(), (1.0 / torch.sqrt(((x64 - mu[:, None]) ** 2).mean(1) + 1e-5)).float()
+        return (dy, x, gamma, mean, rstd), _ln_bwd_terms(dy, x, gamma, mean, rstd)
+
+    args, (xh, gy, c1, c2, rs) = case("random")
+    pre = rs * (gy - c1 - xh * c2)
+    dg, db = (args[0].double() * xh).sum(0).bfloat16(), args[0].double().sum(0).bfloat16()
+    dres = (-pre).bfloat16()                                       # the sum is the rounding error of pre: a cancellation
+    check_ln_bwd(pre.bfloat16(), dg, db, *args)
+    check_ln_bwd((pre + dres.double()).bfloat16(), dg, db, *args, dres=dres)
+    with pytest.raises(AssertionError, match="dx"):
+        check_ln_bwd((rs * (gy - xh * c2)).bfloat16(), dg, db, *args)              # c1 dropped
+    with pytest.raises(AssertionError, match="dx"):
+        check_ln_bwd((rs * (gy - c1)).bfloat16(), dg, db, *args)                   # c2 dropped
+    with pytest.raises(AssertionError, match="dx"):
+        check_ln_bwd((pre.bfloat16().double() + dres.double()).bfloat16(), dg, db, *args, dres=dres)   # rounded twice
+    with pytest.raises(AssertionError, match="dgamma"):
+        check_ln_bwd(pre.bfloat16(), db, dg, *args)                                # swapped
+
+    args, (xh, gy, c1, c2, rs) = case("sparse")
+    pre = (rs * (gy - c1 - xh * c2)).bfloat16()
+    term = args[0].double() * xh
+    check_ln_bwd(pre, term.sum(0).bfloat16(), args[0].double().sum(0).bfloat16(), *args)
+    for r in keep:
+        with pytest.raises(AssertionError, match="dgamma"):
+            check_ln_bwd(pre, (term.sum(0) - term[r]).bfloat16(), args[0].double().sum(0).bfloat16(), *args)
 
 
 def check_colsum_bf16(out, a):
