@@ -345,8 +345,11 @@ class _ChunkedLMLoss(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, h, weight, labels, chunk, vocab, scale=None):
-        """``scale`` (1-element fp32 device tensor or None): the result is ``scale * sum of row losses`` and the
-        gradients produced here already contain it — the caller promises that the returned value enters the total
+        """-> (scaled, total): ``total`` is the sum of row losses (no gradient flows through it), ``scaled`` is
+        ``scale * total``, or ``total`` itself without a scale.
+
+        ``scale`` (1-element fp32 device tensor or None): the gradients produced here already contain it — the caller
+        promises that ``scaled`` enters the total
         loss with coefficient exactly 1 (GPT2DoubleHeads.forward does). That is what allows the weight gradient to be
         written straight into the engine's flat gradient buffer during the forward pass (``weight`` carries a grad sink,
         ops/layers.py::_sink): no 77 MB ``grad_w * g`` and no 77 MB accumulate kernel in the backward."""
@@ -393,8 +396,7 @@ class _ChunkedLMLoss(torch.autograd.Function):
                 grad_w = g.t() @ hs
             else:
                 grad_w.addmm_(g.t(), hs)
-        if scale is not None:
-            total = total * scale.reshape(())
+        scaled = total * scale.reshape(()) if scale is not None else total.clone()
         ctx.direct, ctx.weight = direct, weight
         if direct:
             ctx.save_for_backward(grad_h)
@@ -402,10 +404,11 @@ class _ChunkedLMLoss(torch.autograd.Function):
             if grad_w is None:
                 grad_w = torch.zeros_like(weight)
             ctx.save_for_backward(grad_h, grad_w)
-        return total
+        ctx.mark_non_differentiable(total)
+        return scaled, total
 
     @staticmethod
-    def backward(ctx, g):
+    def backward(ctx, g, _):
         if ctx.direct:                       # unit upstream gradient by contract; dW is already in weight.grad
             return ctx.saved_tensors[0], None, None, None, None, None
         grad_h, grad_w = ctx.saved_tensors
@@ -1092,7 +1095,8 @@ class GPT2DoubleHeads(nn.Module):
     def forward(self, input_ids, token_type_ids=None, mc_token_ids=None, lm_labels=None, mc_labels=None,
                 lm_coef: float = 1.0, mc_coef: float = 1.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """-> (loss, lm_loss, mc_loss). Shapes as in the reference: [B, C, T] ids/labels, [B, C]
-        mc_token_ids, [B] mc_labels; -100 labels are ignored."""
+        mc_token_ids, [B] mc_labels; -100 labels are ignored. ``lm_loss`` is the mean LM cross-entropy whatever
+        ``lm_coef`` is, reported without a gradient: the LM term reaches the parameters through ``loss`` only."""
         B, C, T = input_ids.shape
         ids = input_ids.reshape(B * C, T)
         tt = token_type_ids.reshape(B * C, T) if token_type_ids is not None else None
@@ -1114,10 +1118,11 @@ class GPT2DoubleHeads(nn.Module):
                 shift_l = shift_l.index_select(0, order)
             # the mean's 1/n and lm_coef travel INTO the fused CE kernel, so the LM term enters `loss` with
             # coefficient 1 (the contract of _ChunkedLMLoss's direct weight-gradient path)
-            scale = (lm_coef / n_valid.clamp(min=1).to(torch.float32)).reshape(1)
-            lm_term = _ChunkedLMLoss.apply(shift_h, self.wte.weight, shift_l, self.cfg.lm_chunk_rows,
-                                           self.cfg.vocab_size, scale)
-            lm_loss = lm_term / lm_coef if lm_coef != 0 else lm_term
+            n = n_valid.clamp(min=1).to(torch.float32)
+            scale = (lm_coef / n).reshape(1)
+            lm_term, lm_sum = _ChunkedLMLoss.apply(shift_h, self.wte.weight, shift_l, self.cfg.lm_chunk_rows,
+                                                   self.cfg.vocab_size, scale)
+            lm_loss = lm_sum / n                  # the mean itself, also when lm_coef is 0 and lm_term vanishes
             if compact:
                 # a batch with more scored rows than the capacity must not train silently on a subset
                 lm_loss = torch.where(n_valid > cap, torch.full_like(lm_loss, float("nan")), lm_loss)
