@@ -25,12 +25,20 @@
 //   (tests/test_gpu_kernels_reference.py checks it against an exact emulation of this arithmetic).
 //   Lookups that share a table (ids and token types both index wte) share owner slots, so a row hit through both is
 //   still committed exactly once.
+//
+// With dropout (DROP; dropout.cuh) the output row is drop(sum): the forward masks and scales the fp32 sum before the
+// one bf16 rounding, and the backward's dY entry is everywhere replaced by the fp32 value mask * scale * dY[t, c], the
+// mask recomputed from (seed, step, site, t, c >> 3). claim takes the row maximum of THOSE values and scatter converts
+// THOSE values, so the shift still bounds every integer that is added, and each lookup of token t still contributes one
+// integer per column that depends on (t, c) alone. The sum of integers is therefore still independent of arrival order
+// and of the hot / direct grouping: the repeatability argument above holds unchanged.
 #include <cuda_bf16.h>
 
 #include <climits>
 
 #include "common.h"
 #include "device_prims.cuh"
+#include "dropout.cuh"
 
 namespace adapcc {
 
@@ -49,11 +57,15 @@ struct EmbedBwdArgs {
   int K;
 };
 
-// y[t, :] = sum_k table_k[idx_k[t], :]; D % 8 == 0; one warp per row.
+// y[t, :] = [drop](sum_k table_k[idx_k[t], :]); D % 8 == 0; one warp per row.
+template <bool DROP>
 __global__ void __launch_bounds__(256)
-embed_sum_fwd_kernel(const __grid_constant__ EmbedFwdArgs a, int n, int D, __nv_bfloat16* __restrict__ out) {
+embed_sum_fwd_kernel(const __grid_constant__ EmbedFwdArgs a, int n, int D, __nv_bfloat16* __restrict__ out,
+                     const DropArgs drop) {
   const int warp = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (warp >= n) return;
+  DropKey dkey{};
+  if constexpr (DROP) dkey = drop_key(drop);
   const int nvec = D >> 3;
   const __nv_bfloat16* rows[kEmbedMaxLookups];
 #pragma unroll
@@ -72,22 +84,27 @@ embed_sum_fwd_kernel(const __grid_constant__ EmbedFwdArgs a, int n, int D, __nv_
         for (int i = 0; i < 8; ++i) acc[i] += f[i];
       }
     }
+    if constexpr (DROP) drop_apply(acc, drop_keep8(warp, c, drop, dkey), drop.scale);
     st16(out + (long long)warp * D + c * 8, pack<__nv_bfloat16>(acc));
   }
 }
 
 // one warp per lookup
+template <bool DROP>
 __global__ void __launch_bounds__(256)
 embed_bwd_claim_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, const __nv_bfloat16* __restrict__ dy,
-                       int* __restrict__ owner, unsigned int* __restrict__ maxbits) {
+                       int* __restrict__ owner, unsigned int* __restrict__ maxbits, const DropArgs drop) {
   const int i = (int)((blockIdx.x * (long long)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
   if (i >= a.K * n) return;
+  DropKey dkey{};
+  if constexpr (DROP) dkey = drop_key(drop);
   const int k = i / n, t = i - k * n;
   const int slot = a.owner_base[k] + (int)a.idx[k][t];
   unsigned int m = 0;
   for (int c = lane; c < (D >> 3); c += 32) {
     float f[8];
     unpack<__nv_bfloat16>(ld16(dy + (long long)t * D + c * 8), f);
+    if constexpr (DROP) drop_apply(f, drop_keep8(t, c, drop, dkey), drop.scale);
 #pragma unroll
     for (int e = 0; e < 8; ++e) m = max(m, __float_as_uint(fabsf(f[e])));      // NaN / inf order above every finite
   }
@@ -121,10 +138,11 @@ __device__ __forceinline__ void red_add_fixed(long long* p, long long q) {
 // order decides) does not change any bit of the result.
 constexpr int kEmbTile = 64, kEmbHot = 4, kEmbGroup = 128;       // 2 thread groups x 128 threads; group g: lookups j = g mod 2
 
+template <bool DROP>
 __global__ void __launch_bounds__(2 * kEmbGroup)
 embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, const __nv_bfloat16* __restrict__ dy,
                          const int* __restrict__ owner, const unsigned int* __restrict__ maxbits,
-                         long long* __restrict__ scratch, int lookup_bits) {
+                         long long* __restrict__ scratch, int lookup_bits, const DropArgs drop) {
   __shared__ int s_own[kEmbTile];
   __shared__ int s_row[kEmbTile];
   __shared__ int s_shift[kEmbTile];
@@ -176,6 +194,8 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
   __syncthreads();
   const int g = threadIdx.x / kEmbGroup, tg = threadIdx.x - g * kEmbGroup;
   const int nvec = D >> 3;
+  DropKey dkey{};
+  if constexpr (DROP) dkey = drop_key(drop);
   for (int c = tg; c < nvec; c += kEmbGroup) {
     long long acc[kEmbHot][8];
 #pragma unroll
@@ -187,6 +207,7 @@ embed_bwd_scatter_kernel(const __grid_constant__ EmbedBwdArgs a, int n, int D, c
       if (own < 0) continue;
       float f[8];
       unpack<__nv_bfloat16>(ld16(dy + (long long)s_row[jj] * D + c * 8), f);
+      if constexpr (DROP) drop_apply(f, drop_keep8(s_row[jj], c, drop, dkey), drop.scale);
       const int h = s_hot_of[jj];
       if (h < 0) {
         long long* dst = scratch + (long long)own * D + c * 8;
@@ -255,8 +276,9 @@ using namespace adapcc;
 
 extern "C" {
 
-// tables[k]: bf16 [rows_k, D]; idx[k]: int64 [n]; out: bf16 [n, D]
-int adapcc_embed_sum_fwd(void* const* tables, void* const* idx, int K, int n, int D, void* out, void* stream) {
+// tables[k]: bf16 [rows_k, D]; idx[k]: int64 [n]; out: bf16 [n, D]; drop: optional dropout of the sum
+static int embed_fwd_launch(void* const* tables, void* const* idx, int K, int n, int D, void* out, void* stream,
+                            const DropArgs* drop) {
   if (n <= 0) return 0;
   if (K < 1 || K > kEmbedMaxLookups || D % 8 != 0) { set_error("embed_sum_fwd: 1 <= K <= %d lookups, D %% 8 == 0", kEmbedMaxLookups); return -1; }
   EmbedFwdArgs a{};
@@ -267,17 +289,35 @@ int adapcc_embed_sum_fwd(void* const* tables, void* const* idx, int K, int n, in
     a.idx[k] = (const long long*)idx[k];
   }
   const int wpb = 8;
-  embed_sum_fwd_kernel<<<(n + wpb - 1) / wpb, wpb * 32, 0, (cudaStream_t)stream>>>(a, n, D, (__nv_bfloat16*)out);
+  const int grid = (n + wpb - 1) / wpb;
+  if (drop)
+    embed_sum_fwd_kernel<true><<<grid, wpb * 32, 0, (cudaStream_t)stream>>>(a, n, D, (__nv_bfloat16*)out, *drop);
+  else
+    embed_sum_fwd_kernel<false><<<grid, wpb * 32, 0, (cudaStream_t)stream>>>(a, n, D, (__nv_bfloat16*)out, DropArgs{});
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;
 }
 
+int adapcc_embed_sum_fwd(void* const* tables, void* const* idx, int K, int n, int D, void* out, void* stream) {
+  return embed_fwd_launch(tables, idx, K, n, D, out, stream, nullptr);
+}
+
+// The sum under dropout (dropout.cuh): seed int64 [1] and step int32 [1] on the device, site / thr / scale of the
+// definition; row t of the output is row t of the mask.
+int adapcc_embed_sum_drop_fwd(void* const* tables, void* const* idx, int K, int n, int D, void* out, const void* seed,
+                              const void* step, int site, unsigned int thr, float scale, void* stream) {
+  DropArgs d;
+  if (!drop_args("embed_sum_drop_fwd", seed, step, site, thr, scale, &d)) return -1;
+  return embed_fwd_launch(tables, idx, K, n, D, out, stream, &d);
+}
+
 // owner: int32 [sum of distinct table rows], all INT_MAX between calls; maxbits: uint32, same size, all zero between
 // calls; scratch: int64 [K * n, D], all zero between calls (adapcc_embed_bwd_reset establishes all three).
-// grads[k]: bf16 [rows_k, D], accumulated into.
-int adapcc_embed_sum_bwd(const void* dy, void* const* idx, void* const* grads, const int* owner_base, int K, int n,
-                         int D, int* owner, unsigned int* maxbits, long long* scratch, void* stream) {
+// grads[k]: bf16 [rows_k, D], accumulated into. drop: the forward's dropout, applied to dy as it is read.
+static int embed_bwd_launch(const void* dy, void* const* idx, void* const* grads, const int* owner_base, int K, int n,
+                            int D, int* owner, unsigned int* maxbits, long long* scratch, void* stream,
+                            const DropArgs* drop) {
   if (n <= 0) return 0;
   if (K < 1 || K > kEmbedMaxLookups || D % 8 != 0) { set_error("embed_sum_bwd: 1 <= K <= %d lookups, D %% 8 == 0", kEmbedMaxLookups); return -1; }
   if ((long long)K * n >= INT_MAX) { set_error("embed_sum_bwd: too many lookups"); return -1; }
@@ -294,13 +334,34 @@ int adapcc_embed_sum_bwd(const void* dy, void* const* idx, void* const* grads, c
   int lookup_bits = 0;                               // total <= 2^lookup_bits
   while ((1LL << lookup_bits) < (long long)total) ++lookup_bits;
   const int wpb = 8;
-  embed_bwd_claim_kernel<<<(total + wpb - 1) / wpb, wpb * 32, 0, s>>>(a, n, D, (const __nv_bfloat16*)dy, owner, maxbits);
-  embed_bwd_scatter_kernel<<<(total + kEmbTile - 1) / kEmbTile, 2 * kEmbGroup, 0, s>>>(a, n, D, (const __nv_bfloat16*)dy, owner,
-                                                                                   maxbits, scratch, lookup_bits);
+  const __nv_bfloat16* dyb = (const __nv_bfloat16*)dy;
+  const int cgrid = (total + wpb - 1) / wpb, sgrid = (total + kEmbTile - 1) / kEmbTile;
+  if (drop) {
+    embed_bwd_claim_kernel<true><<<cgrid, wpb * 32, 0, s>>>(a, n, D, dyb, owner, maxbits, *drop);
+    embed_bwd_scatter_kernel<true><<<sgrid, 2 * kEmbGroup, 0, s>>>(a, n, D, dyb, owner, maxbits, scratch, lookup_bits,
+                                                                   *drop);
+  } else {
+    embed_bwd_claim_kernel<false><<<cgrid, wpb * 32, 0, s>>>(a, n, D, dyb, owner, maxbits, DropArgs{});
+    embed_bwd_scatter_kernel<false><<<sgrid, 2 * kEmbGroup, 0, s>>>(a, n, D, dyb, owner, maxbits, scratch, lookup_bits,
+                                                                    DropArgs{});
+  }
   embed_bwd_commit_kernel<<<(total + wpb - 1) / wpb, wpb * 32, 0, s>>>(a, n, D, owner, maxbits, scratch, lookup_bits);
   CUDA_TRY(cudaGetLastError());
   count_launch(3);
   return 0;
+}
+
+int adapcc_embed_sum_bwd(const void* dy, void* const* idx, void* const* grads, const int* owner_base, int K, int n,
+                         int D, int* owner, unsigned int* maxbits, long long* scratch, void* stream) {
+  return embed_bwd_launch(dy, idx, grads, owner_base, K, n, D, owner, maxbits, scratch, stream, nullptr);
+}
+
+int adapcc_embed_sum_drop_bwd(const void* dy, void* const* idx, void* const* grads, const int* owner_base, int K, int n,
+                              int D, int* owner, unsigned int* maxbits, long long* scratch, const void* seed,
+                              const void* step, int site, unsigned int thr, float scale, void* stream) {
+  DropArgs d;
+  if (!drop_args("embed_sum_drop_bwd", seed, step, site, thr, scale, &d)) return -1;
+  return embed_bwd_launch(dy, idx, grads, owner_base, K, n, D, owner, maxbits, scratch, stream, &d);
 }
 
 int adapcc_embed_bwd_reset(int* owner, unsigned int* maxbits, long long n_owner, long long* scratch,

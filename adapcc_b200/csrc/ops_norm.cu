@@ -13,6 +13,7 @@
 
 #include "common.h"
 #include "device_prims.cuh"
+#include "dropout.cuh"
 
 namespace adapcc {
 
@@ -28,14 +29,19 @@ __device__ __forceinline__ float warp_sum(float v) {
 // RES: the row is x + res (the transformer's residual add); the bf16-rounded sum is written to
 // `sum_out` (the new residual stream) and normalised in the same pass, so the separate add kernel
 // and its re-read disappear.
-template <int VPL, bool RES>
+// DROP (with RES): the row is x + drop(res), the dropout of a transformer's residual branch (dropout.cuh): res is
+// masked and scaled in fp32 as it is read, the mask being recomputed from (seed, step, site, row, vector).
+template <int VPL, bool RES, bool DROP = false>
 __global__ void __launch_bounds__(kLnWarps * 32, VPL <= 3 ? 3 : 2)
 ln_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restrict__ res,
               const __nv_bfloat16* __restrict__ gamma, const __nv_bfloat16* __restrict__ beta,
               __nv_bfloat16* __restrict__ sum_out, __nv_bfloat16* __restrict__ y, float* __restrict__ mean,
-              float* __restrict__ rstd, int rows, float eps) {
+              float* __restrict__ rstd, int rows, float eps, const DropArgs drop) {
+  static_assert(RES || !DROP, "dropout acts on the residual branch");
   constexpr int D = VPL * 256;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  DropKey dkey{};
+  if constexpr (DROP) dkey = drop_key(drop);
   uint4 gp[VPL], bp[VPL];                       // packed; unpacked at use (registers buy occupancy here)
 #pragma unroll
   for (int v = 0; v < VPL; ++v) {
@@ -52,6 +58,7 @@ ln_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restri
       if constexpr (RES) {
         float fr[8];
         unpack<__nv_bfloat16>(ld16(reinterpret_cast<const uint4*>(res + (size_t)r * D) + lane + 32 * v), fr);
+        if constexpr (DROP) drop_apply(fr, drop_keep8(r, lane + 32 * v, drop, dkey), drop.scale);
 #pragma unroll
         for (int i = 0; i < 8; ++i) f[v][i] += fr[i];
         const uint4 packed = pack<__nv_bfloat16>(f[v]);      // statistics are taken of the ROUNDED sum,
@@ -83,12 +90,17 @@ ln_fwd_kernel(const __nv_bfloat16* __restrict__ x, const __nv_bfloat16* __restri
 }
 
 // RES: dx += dres (the gradient arriving on the residual stream), fused into the same pass.
-template <int VPL, bool RES>
+// DROP: the forward was s = x + drop(res), so the two inputs' gradients differ: dx as before, and a second output
+// ddrop = mask * scale * dx (taken of the fp32 dx, rounded to bf16 once) for the dropped branch, with the forward's mask.
+// A DROP instantiation is compiled on its own: which fp32 multiplies and adds become FFMAs can differ from the
+// DROP = false one, so its dx / dgamma / dbeta agree with it to rounding, not bit for bit. p = 0 runs DROP = false.
+template <int VPL, bool RES, bool DROP = false>
 __global__ void __launch_bounds__(kLnWarps * 32, VPL <= 3 ? 2 : 1)
 ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restrict__ x,
               const __nv_bfloat16* __restrict__ gamma, const float* __restrict__ mean, const float* __restrict__ rstd,
               const __nv_bfloat16* __restrict__ dres, __nv_bfloat16* __restrict__ dx,
-              float* __restrict__ part_dgamma, float* __restrict__ part_dbeta, int rows) {
+              float* __restrict__ part_dgamma, float* __restrict__ part_dbeta, int rows,
+              __nv_bfloat16* __restrict__ ddrop, const DropArgs drop) {
   constexpr int D = VPL * 256;
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   // gamma stays packed (bf16x8 per register quad) and is unpacked at use: 12 instead of 24 registers
@@ -126,6 +138,8 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restr
     c1 = warp_sum(c1) * (1.f / D);
     c2 = warp_sum(c2) * (1.f / D);
     uint4* ox = reinterpret_cast<uint4*>(dx + (size_t)r * D);
+    DropKey dkey{};                               // read per row: held across the loop it would cost the registers
+    if constexpr (DROP) dkey = drop_key(drop);    // that keep two CTAs on an SM at D = 768
 #pragma unroll
     for (int v = 0; v < VPL; ++v) {
       float o[8];
@@ -138,6 +152,10 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const __nv_bfloat16* __restr
         for (int i = 0; i < 8; ++i) o[i] += fr[i];
       }
       st16(ox + lane + 32 * v, pack<__nv_bfloat16>(o));
+      if constexpr (DROP) {
+        drop_apply(o, drop_keep8(r, lane + 32 * v, drop, dkey), drop.scale);
+        st16(reinterpret_cast<uint4*>(ddrop + (size_t)r * D) + lane + 32 * v, pack<__nv_bfloat16>(o));
+      }
     }
   }
   // CTA reduction of the per-warp column accumulators -> one partial row per CTA
@@ -270,21 +288,27 @@ static int ln_bwd_ctas_per_sm(int d) { return d <= 768 ? 2 : 1; }
 int adapcc_ln_partials(int rows) { return ln_grid(rows, 2); }       // upper bound of the backward grid
 
 // y = LayerNorm(x [+ res]); when res != nullptr the bf16 sum x + res is also written to sum_out.
+// drop (with res): the sum is x + drop(res).
 static int ln_fwd_launch(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
-                         float* mean, float* rstd, int rows, int d, float eps, void* stream) {
+                         float* mean, float* rstd, int rows, int d, float eps, void* stream,
+                         const DropArgs* drop = nullptr) {
   cudaStream_t s = (cudaStream_t)stream;
   if (rows <= 0) return 0;
   const int grid = ln_grid(rows, ln_fwd_ctas_per_sm(d));
 #define LN_FWD(V)                                                                                                  \
   do {                                                                                                             \
-    if (res)                                                                                                       \
+    if (drop)                                                                                                      \
+      ln_fwd_kernel<V, true, true><<<grid, kLnWarps * 32, 0, s>>>((const __nv_bfloat16*)x,                         \
+          (const __nv_bfloat16*)res, (const __nv_bfloat16*)gamma, (const __nv_bfloat16*)beta,                      \
+          (__nv_bfloat16*)sum_out, (__nv_bfloat16*)y, mean, rstd, rows, eps, *drop);                               \
+    else if (res)                                                                                                  \
       ln_fwd_kernel<V, true><<<grid, kLnWarps * 32, 0, s>>>((const __nv_bfloat16*)x, (const __nv_bfloat16*)res,    \
           (const __nv_bfloat16*)gamma, (const __nv_bfloat16*)beta, (__nv_bfloat16*)sum_out, (__nv_bfloat16*)y,     \
-          mean, rstd, rows, eps);                                                                                  \
+          mean, rstd, rows, eps, DropArgs{});                                                                      \
     else                                                                                                           \
       ln_fwd_kernel<V, false><<<grid, kLnWarps * 32, 0, s>>>((const __nv_bfloat16*)x, nullptr,                     \
           (const __nv_bfloat16*)gamma, (const __nv_bfloat16*)beta, nullptr, (__nv_bfloat16*)y, mean, rstd, rows,   \
-          eps);                                                                                                    \
+          eps, DropArgs{});                                                                                        \
   } while (0)
   switch (d) {
     case 256: LN_FWD(1); break;
@@ -312,9 +336,10 @@ int adapcc_add_ln_fwd(const void* x, const void* res, const void* gamma, const v
 
 // part: fp32 scratch of 2 * adapcc_ln_partials(rows) * d floats. dgamma/dbeta: bf16 [d].
 // dres (optional, bf16 [rows, d]): gradient of the residual stream, added to dx in the same pass.
+// drop (optional): ddrop (bf16 [rows, d]) = mask * scale * dx is written as well.
 static int ln_bwd_launch(const void* dy, const void* x, const void* gamma, const float* mean, const float* rstd,
                          const void* dres, void* dx, void* dgamma, void* dbeta, float* part, int rows, int d,
-                         void* stream) {
+                         void* stream, void* ddrop = nullptr, const DropArgs* drop = nullptr) {
   cudaStream_t s = (cudaStream_t)stream;
   if (rows <= 0) return 0;
   const int grid = ln_grid(rows, ln_bwd_ctas_per_sm(d));
@@ -322,12 +347,21 @@ static int ln_bwd_launch(const void* dy, const void* x, const void* gamma, const
   float* pb = part + (size_t)grid * d;
 #define LN_BWD(V)                                                                                                  \
   do {                                                                                                             \
-    if (dres)                                                                                                      \
-      ln_bwd_kernel<V, true><<<grid, kLnWarps * 32, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,     \
-          (const __nv_bfloat16*)gamma, mean, rstd, (const __nv_bfloat16*)dres, (__nv_bfloat16*)dx, pg, pb, rows);  \
+    const __nv_bfloat16 *dy_ = (const __nv_bfloat16*)dy, *x_ = (const __nv_bfloat16*)x;                            \
+    const __nv_bfloat16 *g_ = (const __nv_bfloat16*)gamma, *dr_ = (const __nv_bfloat16*)dres;                      \
+    __nv_bfloat16 *dx_ = (__nv_bfloat16*)dx, *dd_ = (__nv_bfloat16*)ddrop;                                         \
+    if (drop && dres)                                                                                              \
+      ln_bwd_kernel<V, true, true><<<grid, kLnWarps * 32, 0, s>>>(dy_, x_, g_, mean, rstd, dr_, dx_, pg, pb, rows, \
+                                                                  dd_, *drop);                                     \
+    else if (drop)                                                                                                 \
+      ln_bwd_kernel<V, false, true><<<grid, kLnWarps * 32, 0, s>>>(dy_, x_, g_, mean, rstd, nullptr, dx_, pg, pb,  \
+                                                                   rows, dd_, *drop);                              \
+    else if (dres)                                                                                                 \
+      ln_bwd_kernel<V, true><<<grid, kLnWarps * 32, 0, s>>>(dy_, x_, g_, mean, rstd, dr_, dx_, pg, pb, rows,       \
+                                                            nullptr, DropArgs{});                                  \
     else                                                                                                           \
-      ln_bwd_kernel<V, false><<<grid, kLnWarps * 32, 0, s>>>((const __nv_bfloat16*)dy, (const __nv_bfloat16*)x,    \
-          (const __nv_bfloat16*)gamma, mean, rstd, nullptr, (__nv_bfloat16*)dx, pg, pb, rows);                     \
+      ln_bwd_kernel<V, false><<<grid, kLnWarps * 32, 0, s>>>(dy_, x_, g_, mean, rstd, nullptr, dx_, pg, pb, rows,  \
+                                                             nullptr, DropArgs{});                                 \
   } while (0)
   switch (d) {
     case 256: LN_BWD(1); break;
@@ -354,6 +388,29 @@ int adapcc_add_ln_bwd(const void* dy, const void* x, const void* gamma, const fl
                       const void* dres, void* dx, void* dgamma, void* dbeta, float* part, int rows, int d,
                       void* stream) {
   return ln_bwd_launch(dy, x, gamma, mean, rstd, dres, dx, dgamma, dbeta, part, rows, d, stream);
+}
+
+// The residual branch under dropout (dropout.cuh): seed int64 [1] and step int32 [1] on the device, site / thr / scale
+// of the definition. thr == 0 (p = 0) keeps everything with scale 1: the bits of adapcc_add_ln_fwd / _bwd.
+// sum_out = x + drop(res), y = LayerNorm(sum_out)
+int adapcc_add_ln_drop_fwd(const void* x, const void* res, const void* gamma, const void* beta, void* sum_out, void* y,
+                           float* mean, float* rstd, int rows, int d, float eps, const void* seed, const void* step,
+                           int site, unsigned int thr, float scale, void* stream) {
+  DropArgs a;
+  if (!res || !sum_out) { set_error("add_ln_drop_fwd: res and sum_out are required"); return -1; }
+  if (!drop_args("add_ln_drop_fwd", seed, step, site, thr, scale, &a)) return -1;
+  return ln_fwd_launch(x, res, gamma, beta, sum_out, y, mean, rstd, rows, d, eps, stream, &a);
+}
+
+// dx = LayerNorm backward [+ dsum], ddrop = mask * scale * dx: the gradients of x and of res
+int adapcc_add_ln_drop_bwd(const void* dy, const void* x, const void* gamma, const float* mean, const float* rstd,
+                           const void* dsum, void* dx, void* ddrop, void* dgamma, void* dbeta, float* part, int rows,
+                           int d, const void* seed, const void* step, int site, unsigned int thr, float scale,
+                           void* stream) {
+  DropArgs a;
+  if (!ddrop) { set_error("add_ln_drop_bwd: ddrop is required"); return -1; }
+  if (!drop_args("add_ln_drop_bwd", seed, step, site, thr, scale, &a)) return -1;
+  return ln_bwd_launch(dy, x, gamma, mean, rstd, dsum, dx, dgamma, dbeta, part, rows, d, stream, ddrop, &a);
 }
 
 int adapcc_colsum_splits(int rows) { return std::max(1, std::min(64, rows / 64)); }

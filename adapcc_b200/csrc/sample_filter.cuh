@@ -1,13 +1,16 @@
 // The row filter of the on-device sampler (ops_sample.cu) and of sampled beam search (ops_beam.cu): one CTA of 1024
 // threads holds a row's values x_i in shared memory. The top-k threshold and the top-p cut-off are found by bisection
 // over the order-preserving integer encoding of x (counts for top-k, masses for top-p), with no sort; the truncation
-// filters after top-p (min-p, typical, epsilon, eta) remove ids from the row in place. Also the Philox4x32-10
-// generator both samplers draw from, and the block reductions in their fixed order (per-thread loops in index order,
-// shuffle trees, the 32 warp partials added by the same shuffle tree in warp order).
+// filters after top-p (min-p, typical, epsilon, eta) remove ids from the row in place. Also the counter convention
+// of the Philox4x32-10 draws both samplers make (the generator is philox.cuh), and the block reductions in their
+// fixed order (per-thread loops in index order, shuffle trees, the 32 warp partials added by the same shuffle tree in
+// warp order).
 #pragma once
 
 #include <cmath>
 #include <cstdint>
+
+#include "philox.cuh"
 
 namespace adapcc {
 
@@ -46,23 +49,6 @@ __device__ __forceinline__ uint32_t f2key(float f) {
 
 __device__ __forceinline__ float key2f(uint32_t k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
-// the four output words of Philox4x32-10 (Salmon et al., SC'11) for counter (c0, c1, c2, c3) and key (k0, k1)
-__device__ __forceinline__ uint4 philox4(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0,
-                                         uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-    const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-    c0 = hi1 ^ c1 ^ k0;
-    c1 = lo1;
-    c2 = hi0 ^ c3 ^ k1;
-    c3 = lo0;
-    k0 += 0x9E3779B9u;
-    k1 += 0xBB67AE85u;
-  }
-  return make_uint4(c0, c1, c2, c3);
 }
 
 // counter (c0, 0, 0, 0): a token draw uses word 0; rejection-sampling verification uses word 1 for the acceptance

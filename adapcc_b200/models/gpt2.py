@@ -29,6 +29,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..ops.dropout import DropoutState, check_p, dropout, site_attn, site_embed, site_mlp, site_summary
 from ..ops.layers import FusedLayerNorm, FusedLinear
 from ..ops.repeats import check_repeat_args, penalize_repeats_reference
 from ..ops.sampling import check_filter_args, sample_reference, top_filtering
@@ -48,6 +49,13 @@ class GPT2Config:
     initializer_range: float = 0.02
     lm_chunk_rows: int = 8192            # rows of the fused LM-head/CE evaluated at a time (bf16 logits of one
                                          # chunk: 8192 x 50304 x 2 B = 0.8 GB; measured 2 % faster per step than 2048)
+    # Dropout of the embedding sum, of every block's attention and MLP output, and of the multiple-choice head's
+    # summary input, where HF GPT-2 applies it (whose GPT2Config() defaults are 0.1 each); masks as ops/dropout.py
+    # defines them. 0: off, and the step is the one without these fields. Attention-probability dropout (HF's
+    # attn_pdrop) does not exist here: see ROADMAP.md.
+    embd_pdrop: float = 0.0
+    resid_pdrop: float = 0.0
+    summary_first_dropout: float = 0.0
 
     @classmethod
     def tiny(cls) -> "GPT2Config":
@@ -317,20 +325,24 @@ class Block(nn.Module):
         return self.c_proj(a.transpose(1, 2).reshape(B, T, D))
 
     def forward_deferred(self, x: torch.Tensor, delta: Optional[torch.Tensor], cache: Optional["KVCache"] = None,
-                         layer: int = 0):
+                         layer: int = 0, drop=None):
         """Same block with every residual add fused into the LayerNorm that follows it: takes the
         residual stream ``x`` and the previous block's not-yet-added MLP output ``delta``, returns
-        (stream, this block's not-yet-added MLP output)."""
+        (stream, this block's not-yet-added MLP output). ``drop = (p, state)``: residual dropout, applied to each
+        branch inside the add-LayerNorm that adds it (``delta`` is block ``layer - 1``'s MLP output)."""
         if delta is None:
             h = self.ln_1(x)
         else:
-            x, h = self.ln_1.forward_add(x, delta)
-        x, h = self.ln_2.forward_add(x, self._attn(h, cache, layer))
+            x, h = self.ln_1.forward_add(x, delta, drop and (*drop, site_mlp(layer - 1)))
+        x, h = self.ln_2.forward_add(x, self._attn(h, cache, layer), drop and (*drop, site_attn(layer)))
         return x, self._mlp(h)
 
-    def forward(self, x: torch.Tensor, cache: Optional["KVCache"] = None, layer: int = 0) -> torch.Tensor:
-        x = x + self._attn(self.ln_1(x), cache, layer)
-        return x + self._mlp(self.ln_2(x))
+    def forward(self, x: torch.Tensor, cache: Optional["KVCache"] = None, layer: int = 0, drop=None) -> torch.Tensor:
+        if drop is None:
+            x = x + self._attn(self.ln_1(x), cache, layer)
+            return x + self._mlp(self.ln_2(x))
+        x = x + dropout(self._attn(self.ln_1(x), cache, layer), *drop, site_attn(layer))
+        return x + dropout(self._mlp(self.ln_2(x)), *drop, site_mlp(layer))
 
 
 def use_sink(p) -> bool:
@@ -451,6 +463,15 @@ class GPT2DoubleHeads(nn.Module):
             self.wte.weight._adapcc_embed_table = True
             self.wpe.weight._adapcc_embed_table = True
         self._pos_cache = {}
+        for name, p in (("embd_pdrop", cfg.embd_pdrop), ("resid_pdrop", cfg.resid_pdrop),
+                        ("summary_first_dropout", cfg.summary_first_dropout)):
+            check_p(f"GPT2Config.{name}", p)
+        # The arguments of every dropout mask (ops/dropout.py), on the model's device so that a captured step reads
+        # the current values. Plain attributes that _apply moves with the module, NOT buffers: state_dict() keeps its
+        # keys (the engine checkpoints them), and DistributedDataParallel, which broadcasts rank 0's buffers at
+        # construction and before every forward, neither overwrites the per-rank seeds nor gains a collective per step.
+        self.dropout_seed = torch.zeros(1, dtype=torch.int64)
+        self.dropout_step = torch.zeros(1, dtype=torch.int32)
         self.apply(self._init)
         for blk in self.h:                                  # GPT-2 residual-projection scaling
             for lin in (blk.c_proj, blk.c_proj2):
@@ -462,23 +483,69 @@ class GPT2DoubleHeads(nn.Module):
             if isinstance(m, nn.Linear) and m.bias is not None:
                 nn.init.zeros_(m.bias)
 
+    def _apply(self, fn, *args, **kwargs):
+        """``.to`` / ``.cuda`` / ``.bfloat16`` ...: the dropout state follows the parameters' device (a conversion of
+        the floating-point dtype leaves the two integer tensors as they are, as it would leave integer buffers)."""
+        super()._apply(fn, *args, **kwargs)
+        self.dropout_seed, self.dropout_step = fn(self.dropout_seed), fn(self.dropout_step)
+        return self
+
     def num_parameters(self) -> int:
         return sum(p.numel() for p in self.parameters())
 
+    @property
+    def has_dropout(self) -> bool:
+        """Whether any dropout probability of the configuration is non-zero."""
+        cfg = self.cfg
+        return cfg.embd_pdrop > 0 or cfg.resid_pdrop > 0 or cfg.summary_first_dropout > 0
+
+    def set_dropout(self, seed: int, step: int = 0) -> None:
+        """The seed of the dropout masks and the number of training forwards already run (in place: a captured step
+        keeps reading the same tensors). Two models with equal parameters, seed and step train alike bit for bit.
+        The state is per process: data-parallel ranks that should draw different masks get different seeds, and
+        DistributedDataParallel does not synchronise it."""
+        fresh = DropoutState.create(seed, step)
+        self.dropout_seed.copy_(fresh.seed)
+        self.dropout_step.copy_(fresh.step)
+
+    def dropout_state(self) -> DropoutState:
+        """The model's seed and step buffers as the ``DropoutState`` the ops take (views, not copies)."""
+        return DropoutState(self.dropout_seed, self.dropout_step)
+
+    def _begin_dropout(self) -> Optional[DropoutState]:
+        """The state of an active training forward, its step counter advanced; None when nothing drops.
+
+        The counter advances HERE, before the first mask of the step is drawn, and nowhere else: the backward
+        recomputes its masks from the counter, so it must read the value the forward read, and the next forward the
+        next one. Advancing at the end of the forward would hand the backward the next step's masks."""
+        if not (self.training and self.has_dropout):
+            return None
+        state = self.dropout_state()
+        state.advance()
+        return state
+
     def hidden(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], cache: Optional["KVCache"] = None,
-               lengths: Optional[Sequence[int]] = None) -> torch.Tensor:
+               lengths: Optional[Sequence[int]] = None, drop: Optional[DropoutState] = None) -> torch.Tensor:
         """Final-LayerNorm hidden states [N, T, D]. With ``cache`` this is also the prefill of incremental decoding:
         every layer's keys and values of positions 0..T-1 go into the cache and its lengths become ``lengths`` (the real
         length of each right-padded row; default T for all). Causal attention makes the padding invisible to the real
-        tokens, and ``decode_step`` overwrites the padded slots."""
+        tokens, and ``decode_step`` overwrites the padded slots. ``drop``: the state of an active training forward
+        (``forward`` passes it; never together with a cache, so no decoding path drops whatever the mode)."""
         N, T = input_ids.shape
         if cache is not None:
+            if drop is not None:
+                raise ValueError("hidden: dropout and a KV cache exclude each other")
             cache.reset(lengths if lengths is not None else [T] * N, T)
-        return self._blocks(self._embed(input_ids, token_type_ids), cache)
+        cfg = self.cfg
+        embd = (cfg.embd_pdrop, drop, site_embed()) if drop is not None and cfg.embd_pdrop > 0 else None
+        resid = (cfg.resid_pdrop, drop) if drop is not None and cfg.resid_pdrop > 0 else None
+        return self._blocks(self._embed(input_ids, token_type_ids, drop=embd), cache, resid)
 
-    def _embed(self, ids: torch.Tensor, tt: Optional[torch.Tensor], pos: Optional[torch.Tensor] = None) -> torch.Tensor:
+    def _embed(self, ids: torch.Tensor, tt: Optional[torch.Tensor], pos: Optional[torch.Tensor] = None,
+               drop=None) -> torch.Tensor:
         """wte[ids] + wpe[pos] (+ wte[tt]), added in that order: [*ids.shape, D]; ``pos`` defaults to 0..T-1 in every
-        row of ids [N, T]. One ``fused_embedding_sum`` for bf16 CUDA tables if ``fused_embed``."""
+        row of ids [N, T]. One ``fused_embedding_sum`` for bf16 CUDA tables if ``fused_embed``. ``drop = (p, state,
+        site)``: dropout of the sum."""
         if (self.fused_embed and ids.is_cuda and self.wte.weight.dtype == torch.bfloat16
                 and self.wpe.weight.dtype == torch.bfloat16):
             from ..ops import fused_embedding_sum
@@ -488,12 +555,12 @@ class GPT2DoubleHeads(nn.Module):
                 if pos is None:
                     pos = self._pos_cache[(N, T, ids.device)] = torch.arange(T, device=ids.device).repeat(N)
             lookups = [(0, ids), (1, pos)] + ([(0, tt)] if tt is not None else [])
-            return fused_embedding_sum([self.wte.weight, self.wpe.weight], lookups).view(*ids.shape, -1)
+            return fused_embedding_sum([self.wte.weight, self.wpe.weight], lookups, drop).view(*ids.shape, -1)
         # the default positions broadcast over the rows, so wpe's gradient is summed over them before the lookup
         x = self.wte(ids) + self.wpe(torch.arange(ids.shape[-1], device=ids.device) if pos is None else pos)
         if tt is not None:
             x = x + self.wte(tt)
-        return x
+        return x if drop is None else dropout(x, *drop)
 
     def lm_logits(self, h: torch.Tensor, head: Optional[torch.Tensor] = None) -> torch.Tensor:
         """fp32 logits [..., vocab_size] of ``h`` [..., D] through the tied head; ``head``: a kept fp32 ``wte.weight``."""
@@ -501,14 +568,15 @@ class GPT2DoubleHeads(nn.Module):
             head = self.wte.weight.float()
         return (h.float() @ head.t())[..., :self.cfg.vocab_size]
 
-    def _blocks(self, x: torch.Tensor, cache: Optional["KVCache"]) -> torch.Tensor:
+    def _blocks(self, x: torch.Tensor, cache: Optional["KVCache"], drop=None) -> torch.Tensor:
+        """``drop = (p, state)``: residual dropout; the final add-LayerNorm carries the last block's MLP site."""
         if self.fuse_add_ln:
             delta = None
             for i, blk in enumerate(self.h):
-                x, delta = blk.forward_deferred(x, delta, cache, i)
-            return self.ln_f.forward_add(x, delta)[1]
+                x, delta = blk.forward_deferred(x, delta, cache, i, drop)
+            return self.ln_f.forward_add(x, delta, drop and (*drop, site_mlp(len(self.h) - 1)))[1]
         for i, blk in enumerate(self.h):
-            x = blk(x, cache, i)
+            x = blk(x, cache, i, drop)
         return self.ln_f(x)
 
     def new_cache(self, batch: int, t_max: Optional[int] = None) -> "KVCache":
@@ -1100,7 +1168,8 @@ class GPT2DoubleHeads(nn.Module):
         B, C, T = input_ids.shape
         ids = input_ids.reshape(B * C, T)
         tt = token_type_ids.reshape(B * C, T) if token_type_ids is not None else None
-        h = self.hidden(ids, tt)                                              # [B*C, T, D]
+        drop = self._begin_dropout()
+        h = self.hidden(ids, tt, drop=drop)                                   # [B*C, T, D]
         zero = torch.zeros((), dtype=torch.float32, device=h.device)
         lm_loss, mc_loss = zero, zero
         if lm_labels is not None:
@@ -1130,6 +1199,8 @@ class GPT2DoubleHeads(nn.Module):
         if mc_token_ids is not None and mc_labels is not None:
             idx = mc_token_ids.reshape(B * C, 1, 1).expand(-1, 1, h.shape[-1])
             cls_h = h.gather(1, idx).squeeze(1)                               # [B*C, D]
+            if drop is not None and self.cfg.summary_first_dropout > 0:
+                cls_h = dropout(cls_h, self.cfg.summary_first_dropout, drop, site_summary(self.cfg.n_layer))
             mc_logits = self.mc_head(cls_h).view(B, C).float()
             mc_loss = F.cross_entropy(mc_logits, mc_labels)
         loss = (lm_term if lm_labels is not None else zero) + mc_coef * mc_loss

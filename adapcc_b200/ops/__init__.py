@@ -6,7 +6,7 @@ from __future__ import annotations
 
 import ctypes
 import math
-from ctypes import c_float, c_int, c_longlong, c_void_p
+from ctypes import c_float, c_int, c_longlong, c_uint, c_void_p
 from typing import Optional
 
 import torch
@@ -38,6 +38,10 @@ def _lib():
         lib.adapcc_embed_sum_fwd.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]
         lib.adapcc_embed_sum_bwd.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                              c_void_p, c_void_p, c_void_p]
+        drop = [c_void_p, c_void_p, c_int, c_uint, c_float]            # seed, step, site, thr, scale
+        lib.adapcc_embed_sum_drop_fwd.argtypes = [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p] + drop + [c_void_p]
+        lib.adapcc_embed_sum_drop_bwd.argtypes = ([c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
+                                                   c_void_p, c_void_p] + drop + [c_void_p])
         lib.adapcc_embed_bwd_reset.argtypes = [c_void_p, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p]
         lib.adapcc_decode_attn.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_void_p]
         lib.adapcc_decode_attn_work.argtypes = [c_int] * 4
@@ -227,16 +231,26 @@ def _ptr_array(tensors):
 
 
 class _EmbedSumFn(torch.autograd.Function):
-    """y[t] = sum_k tables[spec[k]][idx_k[t]] (bf16, fp32 sum); args: spec, K index tensors, then the tables."""
+    """y[t] = sum_k tables[spec[k]][idx_k[t]] (bf16, fp32 sum); args: spec, drop, K index tensors, then the tables.
+    ``drop`` = (p, state, site) or None: y[t] = dropout(sum) with row t of the mask (ops/dropout.py), applied to the
+    fp32 sum forward and to dY backward, recomputed both times."""
 
     @staticmethod
-    def forward(ctx, spec, *args):
+    def forward(ctx, spec, drop, *args):
         K = len(spec)
         idx, tables = args[:K], args[K:]
         n, D = idx[0].numel(), tables[0].shape[1]
         out = torch.empty(n, D, dtype=tables[0].dtype, device=tables[0].device)
-        _ck(_lib().adapcc_embed_sum_fwd(_ptr_array([tables[j] for j in spec]), _ptr_array(idx), K, n, D,
-                                        c_void_p(out.data_ptr()), _stream()), "embed_sum_fwd")
+        ctx.drop = None
+        if drop is None:
+            _ck(_lib().adapcc_embed_sum_fwd(_ptr_array([tables[j] for j in spec]), _ptr_array(idx), K, n, D,
+                                            c_void_p(out.data_ptr()), _stream()), "embed_sum_fwd")
+        else:
+            from .dropout import drop_tail
+            ctx.drop = drop_tail("fused_embedding_sum", *drop, out.device)
+            ctx.state = drop[1]                            # owns the tensors ctx.drop points at
+            _ck(_lib().adapcc_embed_sum_drop_fwd(_ptr_array([tables[j] for j in spec]), _ptr_array(idx), K, n, D,
+                                                 c_void_p(out.data_ptr()), *ctx.drop, _stream()), "embed_sum_drop_fwd")
         ctx.spec, ctx.idx, ctx.tables, ctx.n, ctx.D = spec, idx, tables, n, D
         return out
 
@@ -263,20 +277,27 @@ class _EmbedSumFn(torch.autograd.Function):
                 grads.append(g)
                 ret.append(g)
         ob = (c_int * K)(*[base[j] for j in spec])
-        _ck(_lib().adapcc_embed_sum_bwd(c_void_p(dy.data_ptr()), _ptr_array(idx), _ptr_array([grads[j] for j in spec]),
-                                        ob, K, n, D, c_void_p(owner.data_ptr()), c_void_p(maxbits.data_ptr()),
-                                        c_void_p(scratch.data_ptr()), _stream()), "embed_sum_bwd")
+        work = (c_void_p(owner.data_ptr()), c_void_p(maxbits.data_ptr()), c_void_p(scratch.data_ptr()))
+        if ctx.drop is None:
+            _ck(_lib().adapcc_embed_sum_bwd(c_void_p(dy.data_ptr()), _ptr_array(idx),
+                                            _ptr_array([grads[j] for j in spec]), ob, K, n, D, *work, _stream()),
+                "embed_sum_bwd")
+        else:
+            _ck(_lib().adapcc_embed_sum_drop_bwd(c_void_p(dy.data_ptr()), _ptr_array(idx),
+                                                 _ptr_array([grads[j] for j in spec]), ob, K, n, D, *work, *ctx.drop,
+                                                 _stream()), "embed_sum_drop_bwd")
         for s in sinks:
             if s is not None:
                 s.done()
-        return (None,) + (None,) * K + tuple(ret)
+        return (None, None) + (None,) * K + tuple(ret)
 
 
-def fused_embedding_sum(tables, lookups) -> torch.Tensor:
+def fused_embedding_sum(tables, lookups, drop=None) -> torch.Tensor:
     """``sum_k tables[j_k][idx_k]`` for ``lookups = [(j_k, idx_k), ...]`` (idx_k: int64, all the same number of
     elements n) -> [n, D]. bf16 CUDA tables with int64 CUDA indices: one forward kernel and a sort-free three-launch
     backward that accumulates duplicate rows in 64-bit fixed point (csrc/ops_embed.cu). Anything else: plain
-    ``F.embedding`` sums."""
+    ``F.embedding`` sums. ``drop = (p, state, site)``: dropout of the sum (``ops/dropout.py``), inside the same kernels
+    on the fused path and through ``dropout`` otherwise."""
     t0 = tables[0]
     fused = (t0.is_cuda and all(t.dtype == torch.bfloat16 and t.is_contiguous() and t.shape[1] == t0.shape[1]
                                 for t in tables) and t0.shape[1] % 8 == 0 and 1 <= len(lookups) <= 4
@@ -286,10 +307,13 @@ def fused_embedding_sum(tables, lookups) -> torch.Tensor:
         for j, ix in lookups:
             e = torch.nn.functional.embedding(ix.reshape(-1), tables[j])
             out = e if out is None else out + e
+        if drop is not None:
+            from .dropout import dropout
+            out = dropout(out, *drop)
         return out
     spec = tuple(int(j) for j, _ in lookups)
     idx = tuple(ix.reshape(-1).contiguous() for _, ix in lookups)
-    return _EmbedSumFn.apply(spec, *idx, *tables)
+    return _EmbedSumFn.apply(spec, drop, *idx, *tables)
 
 
 # ---- decode attention over a KV cache (csrc/ops_decode.cu) -------------------------------------------------------

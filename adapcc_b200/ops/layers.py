@@ -4,13 +4,13 @@
   dbeta reduced in the same pass). Falls back to ``F.layer_norm`` for CPU tensors, non-bf16 dtypes
   or widths other than 256/512/768/1024.
   ``forward_add(x, res)`` also fuses the preceding residual add (and, backward, the residual-stream
-  gradient add).
+  gradient add); with ``drop`` the residual branch passes through dropout (ops/dropout.py) in the same kernels.
 * ``FusedLinear`` — ``F.linear`` (cuBLASLt, bias epilogue) whose backward computes the bias gradient
   with the column-sum kernel instead of ATen's generic reduction.
 """
 from __future__ import annotations
 
-from ctypes import c_float, c_int, c_void_p
+from ctypes import c_float, c_int, c_uint, c_void_p
 
 import torch
 import torch.nn as nn
@@ -31,6 +31,9 @@ def _lib():
         lib.adapcc_ln_bwd.argtypes = [c_void_p] * 9 + [c_int, c_int, c_void_p]
         lib.adapcc_add_ln_fwd.argtypes = [c_void_p] * 8 + [c_int, c_int, c_float, c_void_p]
         lib.adapcc_add_ln_bwd.argtypes = [c_void_p] * 10 + [c_int, c_int, c_void_p]
+        drop = [c_void_p, c_void_p, c_int, c_uint, c_float]            # seed, step, site, thr, scale
+        lib.adapcc_add_ln_drop_fwd.argtypes = [c_void_p] * 8 + [c_int, c_int, c_float] + drop + [c_void_p]
+        lib.adapcc_add_ln_drop_bwd.argtypes = [c_void_p] * 11 + [c_int, c_int] + drop + [c_void_p]
         lib.adapcc_ln_partials.argtypes = [c_int]
         lib.adapcc_colsum.argtypes = [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]
         lib.adapcc_colsum_splits.argtypes = [c_int]
@@ -148,6 +151,55 @@ class _AddLayerNormFn(torch.autograd.Function):
         return (dx, dx) + finish() + (None,)
 
 
+class _AddLayerNormDropFn(torch.autograd.Function):
+    """(x, res) -> (s = x + drop(res), LayerNorm(s)) in one pass, the mask recomputed from ``(p, state, site)``
+    (ops/dropout.py). The two inputs' gradients differ, so the backward kernel writes both: dx (LayerNorm input
+    gradient plus the gradient arriving on ``s``) and dres = mask * scale * dx."""
+
+    @staticmethod
+    def forward(ctx, x, res, gamma, beta, eps, p, state, site):
+        from .dropout import drop_tail
+
+        lib = _lib()
+        d = x.shape[-1]
+        x2 = x.reshape(-1, d).contiguous()
+        r2 = res.reshape(-1, d).contiguous()
+        rows = x2.shape[0]
+        ssum = torch.empty_like(x2)
+        y = torch.empty_like(x2)
+        mean = torch.empty(rows, dtype=torch.float32, device=x.device)
+        rstd = torch.empty(rows, dtype=torch.float32, device=x.device)
+        ctx.drop = drop_tail("forward_add", p, state, site, x.device)
+        if lib.adapcc_add_ln_drop_fwd(_p(x2), _p(r2), _p(gamma), _p(beta), _p(ssum), _p(y), _p(mean), _p(rstd), rows,
+                                      d, eps, *ctx.drop, _s()) != 0:
+            raise NativeError(f"add_ln_drop_fwd failed: {last_error()}")
+        ctx.save_for_backward(ssum, gamma, mean, rstd)
+        ctx.params = (gamma, beta)
+        ctx.p, ctx.state = p, state                   # the state owns the tensors ctx.drop points at
+        ctx.set_materialize_grads(False)
+        return ssum.view(x.shape), y.view(x.shape)
+
+    @staticmethod
+    def backward(ctx, dsum, dy):
+        lib = _lib()
+        s2, gamma, mean, rstd = ctx.saved_tensors
+        rows, d = s2.shape
+        if dy is None:                                # only the sum was used downstream
+            from .dropout import dropout
+            return (dsum, dropout(dsum, ctx.p, ctx.state, ctx.drop[2])) + (None,) * 6
+        dy2 = dy.reshape(rows, d).contiguous()
+        ds2 = None if dsum is None else dsum.reshape(rows, d).contiguous()   # keep alive past the launch
+        dx = torch.empty_like(s2)
+        dres = torch.empty_like(s2)
+        dgamma, dbeta, finish = _ln_param_grads(ctx.params)
+        part = torch.empty(2 * lib.adapcc_ln_partials(rows) * d, dtype=torch.float32, device=s2.device)
+        if lib.adapcc_add_ln_drop_bwd(_p(dy2), _p(s2), _p(gamma), _p(mean), _p(rstd),
+                                      c_void_p(0) if ds2 is None else _p(ds2), _p(dx), _p(dres), _p(dgamma), _p(dbeta),
+                                      _p(part), rows, d, *ctx.drop, _s()) != 0:
+            raise NativeError(f"add_ln_drop_bwd failed: {last_error()}")
+        return (dx.view(dy.shape), dres.view(dy.shape)) + finish() + (None,) * 4
+
+
 class FusedLayerNorm(nn.LayerNorm):
     """``nn.LayerNorm`` whose bf16 CUDA forward / backward are single kernels (csrc/ops_norm.cu; optional residual add
     fused in: ``forward_add``); under the flat engine the backward writes d(gamma) / d(beta) straight into the flat
@@ -162,10 +214,17 @@ class FusedLayerNorm(nn.LayerNorm):
             return _LayerNormFn.apply(x, self.weight, self.bias, self.eps)
         return F.layer_norm(x, self.normalized_shape, self.weight, self.bias, self.eps)
 
-    def forward_add(self, x, res):
-        """-> (x + res, LayerNorm(x + res)): the residual add of a pre-LN transformer block fused into
-        the normalisation that follows it (one kernel forward, one backward)."""
-        if self._fusable(x) and res.shape == x.shape and res.dtype == x.dtype:
+    def forward_add(self, x, res, drop=None):
+        """-> (s, LayerNorm(s)) with s = x + res: the residual add of a pre-LN transformer block fused into
+        the normalisation that follows it (one kernel forward, one backward). ``drop = (p, state, site)``: s = x +
+        dropout(res) with the mask of ops/dropout.py, in the same kernels; None is the path without dropout."""
+        fusable = self._fusable(x) and res.shape == x.shape and res.dtype == x.dtype
+        if drop is not None:
+            if fusable:
+                return _AddLayerNormDropFn.apply(x, res, self.weight, self.bias, self.eps, *drop)
+            from .dropout import dropout
+            res = dropout(res, *drop)
+        elif fusable:
             return _AddLayerNormFn.apply(x, res, self.weight, self.bias, self.eps)
         s = x + res
         return s, F.layer_norm(s, self.normalized_shape, self.weight, self.bias, self.eps)

@@ -20,6 +20,7 @@ mean over the active ranks, clip + AdamW — but lays memory out for the hardwar
 from __future__ import annotations
 
 import os
+import warnings
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Sequence
 
@@ -75,7 +76,7 @@ class FlatDataParallel:
                  weight_decay: float = 0.01, max_norm: float = 1.0, optimizer: str = "adamw",
                  param_dtype: torch.dtype = torch.bfloat16, algo: str = "auto", active: Optional[Sequence[int]] = None,
                  comm_fn: Optional[Callable] = None, direct_grads: Optional[bool] = None,
-                 zero1: Optional[bool] = None):
+                 zero1: Optional[bool] = None, dropout_seed: Optional[int] = None):
         """``comm``: a :class:`~adapcc_b200.runtime.native.NativeComm` (or None for one GPU).
         ``comm_fn(flat_slice)``: alternative collective (e.g. an NCCL all-reduce) for baselines.
         ``direct_grads``: FusedLinear / FusedLayerNorm backward kernels write their parameter gradients
@@ -83,12 +84,20 @@ class FlatDataParallel:
         be applied once per step; default on (``ADAPCC_DIRECT_GRADS=0`` turns it off).
         ``zero1`` (default: on when eligible, see below): shard the optimizer over the ranks — buckets are
         reduce-SCATTERED during backward, every rank runs AdamW on its 1/N slices only and the updated parameters are
-        broadcast by the same kernel through the NVSwitch multicast alias (csrc/zero.cu)."""
+        broadcast by the same kernel through the NVSwitch multicast alias (csrc/zero.cu).
+        ``dropout_seed``: ``model.set_dropout(dropout_seed + rank)``, so the ranks draw different masks (a model with
+        dropout, see ``GPT2Config``); the captured step needs no new input, the state being on the device. Without it
+        the model keeps the seed it has, and at world size > 1 a warning says that the ranks may share their masks."""
         self.model, self.comm, self.world_size, self.rank = model, comm, world_size, rank
         self.lr, self.betas, self.eps, self.weight_decay, self.max_norm = lr, betas, eps, weight_decay, max_norm
         self.optimizer, self.algo, self.comm_fn = optimizer, algo, comm_fn
         self.active = list(active) if active is not None else list(range(world_size))
         self.device = next(model.parameters()).device
+        if dropout_seed is not None:
+            model.set_dropout(int(dropout_seed) + rank)
+        elif world_size > 1 and getattr(model, "has_dropout", False):
+            warnings.warn("FlatDataParallel: the model has dropout and no dropout_seed was given: every rank keeps the "
+                          "model's own seed, so ranks whose seeds are equal draw the same masks")
         params = [p for p in model.parameters() if p.requires_grad]
         self.params = params
         total = sum((p.numel() + 7) // 8 * 8 for p in params)       # every view 16-byte aligned
@@ -387,9 +396,14 @@ class FlatDataParallel:
             per[names[id(p)]] = {"master": self.master[off:off + n].detach().cpu().clone().view(p.shape),
                                  "exp_avg": self.exp_avg[off:off + n].detach().cpu().clone().view(p.shape),
                                  "exp_avg_sq": self.exp_avg_sq[off:off + n].detach().cpu().clone().view(p.shape)}
-        return {"format": 1, "steps_done": int(self.steps_done), "step_t": int(self.step_t.item()),
-                "hyper": {"lr": self.lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay,
-                          "max_norm": self.max_norm, "optimizer": self.optimizer}, "params": per}
+        sd = {"format": 1, "steps_done": int(self.steps_done), "step_t": int(self.step_t.item()),
+              "hyper": {"lr": self.lr, "betas": tuple(self.betas), "eps": self.eps, "weight_decay": self.weight_decay,
+                        "max_norm": self.max_norm, "optimizer": self.optimizer}, "params": per}
+        if getattr(self.model, "has_dropout", False):      # the mask sequence: a resumed run continues it. The seed is the
+            # base seed (this rank's minus its rank), so that whichever rank writes the file, rank r resumes seed + r
+            sd["dropout"] = {"seed": int(self.model.dropout_seed.item()) - self.rank,
+                             "step": int(self.model.dropout_step.item())}
+        return sd
 
     def load_state_dict(self, sd: Dict[str, object], strict: bool = True) -> None:
         """In place (buffer addresses — and therefore a captured CUDA graph — stay valid): fp32 state from the
@@ -415,6 +429,14 @@ class FlatDataParallel:
         self.step_t.fill_(int(sd.get("step_t", self.steps_done)))
         h = sd.get("hyper", {})
         self.set_lr(h.get("lr", self.lr))
+        has = getattr(self.model, "has_dropout", False)
+        if "dropout" in sd and has:
+            self.model.set_dropout(sd["dropout"]["seed"] + self.rank, sd["dropout"]["step"])
+        elif "dropout" in sd:
+            warnings.warn("load_state_dict: the checkpoint carries a dropout state and the model has no dropout: ignored")
+        elif has:
+            warnings.warn("load_state_dict: the checkpoint carries no dropout state: the model keeps its seed and step, "
+                          "so the mask sequence does not continue the checkpointed run's")
 
     def close(self) -> None:
         for h in self._hooks:

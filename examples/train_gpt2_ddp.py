@@ -53,6 +53,9 @@ def main():
     p.add_argument("--fuse_add_ln", action="store_true", help="residual adds fused into the following LayerNorm")
     p.add_argument("--lm_rows", default="all", choices=["all", "scored"],
                    help="scored: LM head only on rows with a label (same loss/gradients, ~1/8 of the rows)")
+    p.add_argument("--dropout", type=float, default=0.0,
+                   help="embedding, residual and summary dropout probability (HF GPT-2's default is 0.1); 0: off")
+    p.add_argument("--dropout_seed", type=int, default=0, help="seed of the dropout masks (rank r uses seed + r)")
     a = p.parse_args()
 
     rank, world, local = (int(os.environ.get(k, d)) for k, d in (("RANK", 0), ("WORLD_SIZE", 1), ("LOCAL_RANK", 0)))
@@ -62,6 +65,7 @@ def main():
     os.environ.setdefault("MASTER_PORT", "1234")
     dist.init_process_group("nccl", rank=rank, world_size=world, device_id=dev)
     cfg = GPT2Config.tiny() if a.tiny else GPT2Config()
+    cfg.embd_pdrop = cfg.resid_pdrop = cfg.summary_first_dropout = a.dropout
     torch.manual_seed(0)
     model = GPT2DoubleHeads(cfg).to(dev)
     a.heap_mb = (model.num_parameters() * 2 >> 20) + 64
@@ -77,7 +81,7 @@ def main():
         model.lm_row_capacity = max(lm_rows_needed(b["lm_labels"].cpu()) for b in batches)
     if a.engine == "flat":
         eng = FlatDataParallel(model, comm.native if world > 1 else None, world_size=world, rank=rank, lr=a.lr,
-                               max_norm=a.max_norm)
+                               max_norm=a.max_norm, dropout_seed=a.dropout_seed)
         if a.checkpoint and os.path.exists(a.checkpoint):            # before capture: the lr is baked into the graph
             eng.load_state_dict(torch.load(a.checkpoint, map_location="cpu", weights_only=False))
             if rank == 0:
@@ -87,6 +91,7 @@ def main():
         step = (lambda b: eng.step_graph(b)) if a.graph else (lambda b: eng.step(b))
     else:
         model = model.bfloat16()
+        model.set_dropout(a.dropout_seed + rank)
         ddp = wrap_ddp(model, comm, local, bucket_cap_mb=25)
         opt = torch.optim.AdamW(ddp.parameters(), lr=a.lr, fused=True)
 

@@ -81,6 +81,9 @@ def main():
     p.add_argument("--parallel_degree", type=int, default=4)
     p.add_argument("--profile_freq", type=int, default=0)
     p.add_argument("--seed", type=int, default=0)
+    p.add_argument("--dropout", type=float, default=0.0,
+                   help="embedding, residual and summary dropout probability (HF GPT-2's default is 0.1); 0: off")
+    p.add_argument("--dropout_seed", type=int, default=0, help="seed of the dropout masks (rank r uses seed + r)")
     a = p.parse_args()
     a.synthetic = dict(n_train=a.synthetic_dialogs, n_valid=max(8, a.synthetic_dialogs // 8), n_candidates=4, seed=a.seed)
 
@@ -97,6 +100,7 @@ def main():
         dist.init_process_group("gloo", rank=rank, world_size=world)
 
     cfg = GPT2Config.tiny() if a.tiny else GPT2Config()
+    cfg.embd_pdrop = cfg.resid_pdrop = cfg.summary_first_dropout = a.dropout
     if a.tiny:
         cfg.n_positions = 128
     tok = build_tokenizer(a, cfg, rank)
@@ -125,7 +129,7 @@ def main():
         from adapcc_b200.parallel.engine import FlatDataParallel
 
         eng = FlatDataParallel(model, comm.native if world > 1 else None, world_size=world, rank=rank, lr=a.lr,
-                               max_norm=a.max_norm, weight_decay=0.0)
+                               max_norm=a.max_norm, weight_decay=0.0, dropout_seed=a.dropout_seed)
         if a.checkpoint and os.path.exists(a.checkpoint):
             ck = torch.load(a.checkpoint, map_location="cpu", weights_only=False)
             eng.load_state_dict(ck["engine"])
@@ -133,11 +137,14 @@ def main():
     else:
         from adapcc_b200.parallel.ddp import wrap_ddp
 
+        model.set_dropout(a.dropout_seed + rank)
         ddp = wrap_ddp(model, comm, local, zero_copy=False) if world > 1 else model
         opt = torch.optim.AdamW(model.parameters(), lr=a.lr, weight_decay=0.0)
         if a.checkpoint and os.path.exists(a.checkpoint):
             ck = torch.load(a.checkpoint, map_location="cpu", weights_only=False)
             model.load_state_dict(ck["model"])
+            if "dropout" in ck:                           # continue the mask sequence (the flat engine does it itself)
+                model.set_dropout(ck["dropout"]["seed"] + rank, ck["dropout"]["step"])
             start_epoch = int(ck.get("epoch", -1)) + 1
 
     def validate(tag):
@@ -197,7 +204,10 @@ def main():
             print(f"epoch {epoch}: {seen * world / dt:,.0f} tokens/s ({dt:.1f} s)", flush=True)
         validate(f"epoch {epoch}")
         if a.checkpoint:
-            ck = pack_checkpoint(model, os.path.abspath(a.tokenizer), eng, {"epoch": epoch})   # collective under ZeRO-1
+            extra = {"epoch": epoch}
+            if eng is None and model.has_dropout:         # rank 0's seed is the base seed; every rank has run as many steps
+                extra["dropout"] = {"seed": int(model.dropout_seed) - rank, "step": int(model.dropout_step)}
+            ck = pack_checkpoint(model, os.path.abspath(a.tokenizer), eng, extra)   # collective under ZeRO-1
             if rank == 0:
                 torch.save(ck, a.checkpoint + ".tmp")
                 os.replace(a.checkpoint + ".tmp", a.checkpoint)
