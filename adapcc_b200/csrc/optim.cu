@@ -5,7 +5,9 @@
 // AdamW + clip_grad_norm_ 1.0). With all parameters and (all-reduced) gradients living in two flat
 // buffers the whole update is two launches: a sum-of-squares reduction (global grad norm, no host
 // sync) and one AdamW pass that applies the clip coefficient, updates fp32 master / m / v and
-// writes the bf16 parameters back — memory bound, 128-bit accesses, graph capturable.
+// writes the bf16 parameters back — memory bound, 128-bit accesses, graph capturable. With gradient accumulation two
+// more passes per bucket, both launched from the engine's bucket-ready events: accumulate a micro-batch's gradient into
+// an fp32 buffer, and fold the last one in with the 1/M mean before the bucket's collective.
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 
@@ -150,6 +152,84 @@ sgd_kernel(P* __restrict__ param, const G* __restrict__ grad, float* __restrict_
   }
 }
 
+// ---- gradient accumulation over micro-batches ---------------------------------------------------------------------
+// The engine's fp32 accumulator acc of the micro-batch gradients g_1..g_M (bf16 or fp32, whatever the flat buffer
+// holds): acc = f32(g_1), acc = f32(acc + f32(g_m)), and on the last micro-batch g = round(f32(f32(acc + f32(g_M)) *
+// scale)) with scale = f32(1/M). Every add and multiply is rounded on its own (__fadd_rn / __fmul_rn: never contracted
+// into an FMA), so the result is the same bits as that definition in torch. One thread per 8 elements per iteration:
+// 16-byte loads and stores, no atomics. n % 8 == 0 and 16-byte aligned pointers (checked by the entry points).
+template <typename T> struct Vec8;
+template <> struct Vec8<__nv_bfloat16> {
+  static __device__ __forceinline__ void load(const __nv_bfloat16* p, long long i, float (&f)[8]) {
+    const uint4 q = reinterpret_cast<const uint4*>(p)[i];
+    const __nv_bfloat162* h = reinterpret_cast<const __nv_bfloat162*>(&q);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { const float2 t = __bfloat1622float2(h[k]); f[2 * k] = t.x; f[2 * k + 1] = t.y; }
+  }
+  static __device__ __forceinline__ void store(__nv_bfloat16* p, long long i, const float (&f)[8]) {
+    uint4 q;
+    __nv_bfloat162* h = reinterpret_cast<__nv_bfloat162*>(&q);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) h[k] = __floats2bfloat162_rn(f[2 * k], f[2 * k + 1]);
+    reinterpret_cast<uint4*>(p)[i] = q;
+  }
+};
+template <> struct Vec8<float> {
+  static __device__ __forceinline__ void load(const float* p, long long i, float (&f)[8]) {
+    const float4 a = reinterpret_cast<const float4*>(p)[2 * i], b = reinterpret_cast<const float4*>(p)[2 * i + 1];
+    f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
+  }
+  static __device__ __forceinline__ void store(float* p, long long i, const float (&f)[8]) {
+    reinterpret_cast<float4*>(p)[2 * i] = make_float4(f[0], f[1], f[2], f[3]);
+    reinterpret_cast<float4*>(p)[2 * i + 1] = make_float4(f[4], f[5], f[6], f[7]);
+  }
+};
+
+// acc = f32(g) (FIRST) or acc = acc + f32(g)
+template <typename T, bool FIRST>
+__global__ void __launch_bounds__(256) grad_accum_kernel(const T* __restrict__ g, float* __restrict__ acc, long long nv) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += stride) {
+    float f[8];
+    Vec8<T>::load(g, i, f);
+    if (!FIRST) {
+      float a[8];
+      Vec8<float>::load(acc, i, a);
+#pragma unroll
+      for (int k = 0; k < 8; ++k) f[k] = __fadd_rn(a[k], f[k]);
+    }
+    Vec8<float>::store(acc, i, f);
+  }
+}
+
+// g = round(f32(acc + f32(g)) * scale)
+template <typename T>
+__global__ void __launch_bounds__(256) grad_fold_kernel(T* __restrict__ g, const float* __restrict__ acc, long long nv,
+                                                        float scale) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nv; i += stride) {
+    float f[8], a[8];
+    Vec8<T>::load(g, i, f);
+    Vec8<float>::load(acc, i, a);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) f[k] = __fmul_rn(__fadd_rn(a[k], f[k]), scale);
+    Vec8<T>::store(g, i, f);
+  }
+}
+
+// blocks of 256 threads for n / 8 vectors: at most 8 resident blocks on each of the H100's 132 SMs
+inline unsigned grad_accum_grid(long long n) { return (unsigned)std::min<long long>(132 * 8, (n / 8 + 255) / 256); }
+
+inline bool grad_accum_args(const char* who, const void* g, const float* acc, long long n, int dtype) {
+  if (dtype != BF16 && dtype != F32) { set_error("%s: gradient dtype must be bf16 or fp32, got %d", who, dtype); return false; }
+  if (n % 8 != 0) { set_error("%s: n = %lld must be a multiple of 8", who, n); return false; }
+  if ((reinterpret_cast<uintptr_t>(g) | reinterpret_cast<uintptr_t>(acc)) & 15) {
+    set_error("%s: gradient and accumulator must be 16-byte aligned", who);
+    return false;
+  }
+  return true;
+}
+
 }  // namespace adapcc
 
 using namespace adapcc;
@@ -213,6 +293,38 @@ int adapcc_fused_adamw_lr(void* param, const void* grad, float* master, float* m
   else if (param_dtype == F32 && grad_dtype == BF16)
     adamw_kernel<float, __nv_bfloat16><<<blocks, 512, 0, s>>>((float*)param, (const __nv_bfloat16*)grad, master, m, v, n, a, sumsq, step_ptr, lr_ptr);
   else { set_error("adamw: unsupported dtypes %d/%d", param_dtype, grad_dtype); return -1; }
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// Micro-batch accumulate: acc = f32(g) when `first`, else acc = f32(acc + f32(g)). g: n elements of `dtype` (F32 or
+// BF16), acc: n fp32; both 16-byte aligned, n % 8 == 0.
+int adapcc_grad_accum(const void* g, float* acc, long long n, int dtype, int first, void* stream) {
+  if (!grad_accum_args("grad_accum", g, acc, n, dtype)) return -1;
+  if (n <= 0) return 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  const unsigned grid = grad_accum_grid(n);
+  if (dtype == BF16) {
+    if (first) grad_accum_kernel<__nv_bfloat16, true><<<grid, 256, 0, s>>>((const __nv_bfloat16*)g, acc, n / 8);
+    else grad_accum_kernel<__nv_bfloat16, false><<<grid, 256, 0, s>>>((const __nv_bfloat16*)g, acc, n / 8);
+  } else {
+    if (first) grad_accum_kernel<float, true><<<grid, 256, 0, s>>>((const float*)g, acc, n / 8);
+    else grad_accum_kernel<float, false><<<grid, 256, 0, s>>>((const float*)g, acc, n / 8);
+  }
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// Last micro-batch: g = round(f32(f32(acc + f32(g)) * scale)), in place; scale is 1/M.
+int adapcc_grad_fold(void* g, const float* acc, long long n, int dtype, float scale, void* stream) {
+  if (!grad_accum_args("grad_fold", g, acc, n, dtype)) return -1;
+  if (n <= 0) return 0;
+  cudaStream_t s = (cudaStream_t)stream;
+  const unsigned grid = grad_accum_grid(n);
+  if (dtype == BF16) grad_fold_kernel<__nv_bfloat16><<<grid, 256, 0, s>>>((__nv_bfloat16*)g, acc, n / 8, scale);
+  else grad_fold_kernel<float><<<grid, 256, 0, s>>>((float*)g, acc, n / 8, scale);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;

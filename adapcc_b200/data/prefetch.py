@@ -9,7 +9,7 @@ replay (``static_out``) and the copy of batch *k+1* overlaps the compute of batc
 """
 from __future__ import annotations
 
-from typing import Dict, Iterable, Iterator, Optional
+from typing import Dict, Iterable, Iterator, List, Optional
 
 import torch
 
@@ -91,3 +91,18 @@ class PinnedPrefetcher:
             yield out
             if not more:
                 return
+
+
+def micro_batch_groups(loader: Iterable[Dict[str, torch.Tensor]], device, M: int) -> Iterator[List[Dict[str, torch.Tensor]]]:
+    """The loader's batches on ``device`` in groups of ``M`` consecutive ones, in order (an incomplete last group is
+    dropped): the micro-batches of one optimizer step under gradient accumulation. The prefetcher ring holds M + 1
+    slots, so every batch of a group is still the loader's batch when the group is yielded and until the next group is
+    requested (with fewer slots the next batch's upload would already overwrite the first ones of the group)."""
+    if int(M) < 1:
+        raise ValueError(f"micro_batch_groups: M must be >= 1, got {M}")
+    group: List[Dict[str, torch.Tensor]] = []
+    for batch in PinnedPrefetcher(loader, device, depth=int(M) + 1):
+        group.append(batch)
+        if len(group) == M:
+            yield group
+            group = []

@@ -22,6 +22,8 @@ def _lib():
     lib = load_library()
     if not _bound:
         lib.adapcc_sumsq.argtypes = [c_void_p, c_longlong, c_int, c_void_p, c_void_p]
+        lib.adapcc_grad_accum.argtypes = [c_void_p, c_void_p, c_longlong, c_int, c_int, c_void_p]
+        lib.adapcc_grad_fold.argtypes = [c_void_p, c_void_p, c_longlong, c_int, c_float, c_void_p]
         lib.adapcc_fused_adamw.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_longlong, c_int, c_int,
                                            c_float, c_float, c_float, c_float, c_float, c_int, c_float, c_float,
                                            c_void_p, c_void_p, c_void_p]
@@ -127,6 +129,30 @@ def sumsq_(grad: torch.Tensor, out: torch.Tensor) -> torch.Tensor:
     _ck(_lib().adapcc_sumsq(c_void_p(grad.data_ptr()), grad.numel(), _dt(grad), c_void_p(out.data_ptr()), _stream()),
         "sumsq")
     return out
+
+
+def _check_accum(who: str, grad: torch.Tensor, acc: torch.Tensor) -> None:
+    if acc.dtype != torch.float32 or acc.numel() != grad.numel() or not (grad.is_contiguous() and acc.is_contiguous()):
+        raise ValueError(f"{who}: acc must be a contiguous fp32 tensor of grad's {grad.numel()} elements, got {acc.dtype} "
+                         f"{tuple(acc.shape)} (grad {grad.dtype} {tuple(grad.shape)})")
+
+
+def grad_accum_(grad: torch.Tensor, acc: torch.Tensor, first: bool) -> torch.Tensor:
+    """acc = f32(grad) when ``first``, else acc = f32(acc + f32(grad)): one micro-batch's (bf16 or fp32) gradient into
+    the fp32 accumulator, each add rounded on its own. Both 16-byte aligned, numel a multiple of 8."""
+    _check_accum("grad_accum", grad, acc)
+    _ck(_lib().adapcc_grad_accum(c_void_p(grad.data_ptr()), c_void_p(acc.data_ptr()), grad.numel(), _dt(grad),
+                                 int(bool(first)), _stream()), "grad_accum")
+    return acc
+
+
+def grad_fold_(grad: torch.Tensor, acc: torch.Tensor, scale: float) -> torch.Tensor:
+    """In place: grad = round(f32(f32(acc + f32(grad)) * f32(scale))), the last micro-batch's gradient folded into the
+    accumulator and scaled (by 1/M for the mean over M micro-batches), each add and multiply rounded on its own."""
+    _check_accum("grad_fold", grad, acc)
+    _ck(_lib().adapcc_grad_fold(c_void_p(grad.data_ptr()), c_void_p(acc.data_ptr()), grad.numel(), _dt(grad),
+                                float(scale), _stream()), "grad_fold")
+    return grad
 
 
 def fused_adamw_(param: torch.Tensor, grad: torch.Tensor, master: torch.Tensor, m: torch.Tensor, v: torch.Tensor, *,

@@ -47,3 +47,21 @@ def rebuild_buckets(ddp, communicator) -> bool:
         return False
     with symmetric_allocations(communicator):
         return bool(reducer._rebuild_buckets())
+
+
+def ddp_accumulate(ddp, micro, **kwargs) -> torch.Tensor:
+    """Forward and backward of one optimizer step's micro-batches (dicts of model inputs, ``kwargs`` added to each
+    call) through DistributedDataParallel, or a bare module at world size 1, into the parameters' ``.grad``: ``no_sync``
+    for all but the last, so the gradients are all-reduced once per step, and each loss (the model output's first
+    element) times 1/M, so the gradient is that of the mean of the M micro-batch losses, the objective of
+    ``FlatDataParallel(gradient_accumulation_steps=M)``. M = 1 is a plain forward and backward. -> that mean, detached."""
+    M = len(micro)
+    total = None
+    for i, b in enumerate(micro):
+        last = i == M - 1 or not hasattr(ddp, "no_sync")
+        with contextlib.nullcontext() if last else ddp.no_sync():
+            out = ddp(**b, **kwargs)
+            loss = out[0] if isinstance(out, (tuple, list)) else out
+            (loss * (1.0 / M) if M > 1 else loss).backward()
+        total = loss.detach() if total is None else total + loss.detach()
+    return total / M if M > 1 else total

@@ -21,6 +21,7 @@ from __future__ import annotations
 
 import os
 import warnings
+from collections.abc import Mapping
 from dataclasses import dataclass
 from typing import Callable, Dict, List, Optional, Sequence
 
@@ -76,7 +77,8 @@ class FlatDataParallel:
                  weight_decay: float = 0.01, max_norm: float = 1.0, optimizer: str = "adamw",
                  param_dtype: torch.dtype = torch.bfloat16, algo: str = "auto", active: Optional[Sequence[int]] = None,
                  comm_fn: Optional[Callable] = None, direct_grads: Optional[bool] = None,
-                 zero1: Optional[bool] = None, dropout_seed: Optional[int] = None):
+                 zero1: Optional[bool] = None, dropout_seed: Optional[int] = None,
+                 gradient_accumulation_steps: int = 1):
         """``comm``: a :class:`~adapcc_b200.runtime.native.NativeComm` (or None for one GPU).
         ``comm_fn(flat_slice)``: alternative collective (e.g. an NCCL all-reduce) for baselines.
         ``direct_grads``: FusedLinear / FusedLayerNorm backward kernels write their parameter gradients
@@ -87,7 +89,27 @@ class FlatDataParallel:
         broadcast by the same kernel through the NVSwitch multicast alias (csrc/zero.cu).
         ``dropout_seed``: ``model.set_dropout(dropout_seed + rank)``, so the ranks draw different masks (a model with
         dropout, see ``GPT2Config``); the captured step needs no new input, the state being on the device. Without it
-        the model keeps the seed it has, and at world size > 1 a warning says that the ranks may share their masks."""
+        the model keeps the seed it has, and at world size > 1 a warning says that the ranks may share their masks.
+
+        ``gradient_accumulation_steps`` M (default 1): one optimizer step runs M micro-batches in order, and ``step`` /
+        ``step_graph`` / ``capture`` take a sequence of M batch dicts of equal shapes (a plain dict when M = 1). Each
+        micro-batch runs as a step without accumulation does (``flat_grad`` zeroed, forward, backward with the fused ops'
+        direct gradient writes; its loss is NOT scaled by 1/M) and leaves its bf16 gradient g_m. An fp32 buffer
+        ``grad_acc`` of ``total`` elements, allocated only when M > 1, holds acc_1 = f32(g_1), acc_m = f32(acc_{m-1} +
+        f32(g_m)); on the last micro-batch each bucket is folded, ``flat_grad = bf16(f32(f32(acc_{M-1} + f32(g_M)) *
+        f32(1/M)))``, every add and multiply rounded on its own. Each bucket's accumulate (micro-batches 1..M-1) or fold
+        (micro-batch M) runs on the collective stream as soon as the bucket's gradients are ready, overlapping the rest
+        of the backward; after the fold the bucket's collective runs as it does without accumulation, so the gradient is
+        sent once per step and not once per micro-batch. Everything after (ZeRO-1, the norm, clipping, AdamW / SGD) sees
+        the folded ``flat_grad``. The loss returned is f32(sum_m loss_m) * f32(1/M), the mean of the micro-batch losses
+        (HuggingFace's accumulation objective), which differs from the mean over the whole batch when the micro-batches
+        score different numbers of labels. Each micro-batch's forward advances the dropout counter (M per step).
+        ``steps_done``, ``step_t``, ``set_lr`` and checkpoints count optimizer steps; the accumulator is empty between
+        steps, so a checkpoint does not depend on M. M = 1 is the engine without accumulation, launch for launch."""
+        if (isinstance(gradient_accumulation_steps, bool) or not isinstance(gradient_accumulation_steps, int)
+                or gradient_accumulation_steps < 1):
+            raise ValueError(f"gradient_accumulation_steps must be an int >= 1, got {gradient_accumulation_steps!r}")
+        self.grad_accum_steps = gradient_accumulation_steps
         self.model, self.comm, self.world_size, self.rank = model, comm, world_size, rank
         self.lr, self.betas, self.eps, self.weight_decay, self.max_norm = lr, betas, eps, weight_decay, max_norm
         self.optimizer, self.algo, self.comm_fn = optimizer, algo, comm_fn
@@ -134,6 +156,9 @@ class FlatDataParallel:
             self.zero_copy = True
         else:
             self.flat_grad = torch.zeros(total, dtype=param_dtype, device=dev)
+        # micro-batch gradient sums (gradient_accumulation_steps > 1): written before it is read in every step
+        self.grad_acc = torch.empty(total, dtype=torch.float32, device=dev) if self.grad_accum_steps > 1 else None
+        self._inv_m = torch.full((), 1.0 / self.grad_accum_steps, dtype=torch.float32, device=dev)
         self.master = torch.zeros(total, dtype=torch.float32, device=dev)
         self.exp_avg = torch.zeros(total, dtype=torch.float32, device=dev)
         self.exp_avg_sq = torch.zeros(total, dtype=torch.float32, device=dev)
@@ -214,9 +239,10 @@ class FlatDataParallel:
         self.direct_grads = bool(self._sinks)
         self._debug = os.environ.get("ADAPCC_ENGINE_DEBUG", "0") == "1"
         self._ready: List[bool] = [False] * len(params)
+        self._micro = 1                                   # 1-based index of the micro-batch in flight
         self.comm_stream = torch.cuda.Stream(device=dev, priority=-1) if dev.type == "cuda" else None
         self._graph = None
-        self._static: Dict[str, torch.Tensor] = {}
+        self._static_batches: List[Dict[str, torch.Tensor]] = []
         self._static_loss = None
         self.steps_done = 0
         self.native_launches_per_step = 0
@@ -247,13 +273,27 @@ class FlatDataParallel:
         return hook
 
     def _launch_bucket(self, b: _Bucket) -> None:
-        if self.world_size <= 1 or (self.comm is None and self.comm_fn is None):
+        """Bucket ``b``'s gradients of the current micro-batch are final: on the collective stream, add them to the
+        accumulator (micro-batches 1..M-1), or fold them into it (micro-batch M) and run the bucket's collective."""
+        collective = self.world_size > 1 and (self.comm is not None or self.comm_fn is not None)
+        M = self.grad_accum_steps
+        if M == 1 and not collective:
             return
         cur = torch.cuda.current_stream(self.device)
         self.comm_stream.wait_stream(cur)
         self._forked = True
         with torch.cuda.stream(self.comm_stream):
             seg = self.flat_grad[b.start:b.end]
+            if M > 1:
+                from ..ops import grad_accum_, grad_fold_
+
+                acc = self.grad_acc[b.start:b.end]
+                if self._micro < M:
+                    grad_accum_(seg, acc, first=self._micro == 1)
+                    return
+                grad_fold_(seg, acc, 1.0 / M)
+                if not collective:
+                    return
             if self.comm_fn is not None:
                 self.comm_fn(seg)
             elif self.zero1:
@@ -264,9 +304,9 @@ class FlatDataParallel:
                 self.comm.all_reduce(seg, op="avg", algo=self.algo, active=self.active)
 
     # -- one training step -------------------------------------------------------------------------
-    def _step_body(self, batch: Dict[str, torch.Tensor]) -> torch.Tensor:
-        from ..ops import fused_adamw_, fused_sgd_, incr_, sumsq_
-
+    def _micro_step(self, batch: Dict[str, torch.Tensor]) -> torch.Tensor:
+        """Forward and backward of one micro-batch into the zeroed ``flat_grad``; the buckets' accumulate / fold /
+        collective launches happen from the gradient-ready events. Returns the (device) loss."""
         self.flat_grad.zero_()
         self._forked = False
         self._ready = [False] * len(self.params)
@@ -282,8 +322,20 @@ class FlatDataParallel:
                 b.pending = 0                         # their zeros still travel, or the bucket's other gradients
                 self._launch_bucket(b)                # would stay un-averaged (same parameters on every rank, as in DDP)
         cur = torch.cuda.current_stream(self.device)
-        if self._forked:                            # join the collective stream (also under capture)
-            cur.wait_stream(self.comm_stream)
+        if self._forked:                            # join the collective stream (also under capture); the next
+            cur.wait_stream(self.comm_stream)       # micro-batch's zero_() must not overtake this one's accumulates
+        return loss.detach()
+
+    def _step_body(self, batches: List[Dict[str, torch.Tensor]]) -> torch.Tensor:
+        from ..ops import fused_adamw_, fused_sgd_, incr_, sumsq_
+
+        loss = None
+        for m, batch in enumerate(batches, 1):
+            self._micro = m
+            lm = self._micro_step(batch)
+            loss = lm if loss is None else loss + lm                  # fp32, in micro-batch order
+        if len(batches) > 1:
+            loss = loss.float() * self._inv_m
         incr_(self.step_t)
         if self.zero1:
             self._zero1_update()
@@ -298,7 +350,7 @@ class FlatDataParallel:
                          max_norm=self.max_norm or 0.0, sumsq=sumsq, step_tensor=self.step_t, lr_tensor=self.lr_t)
         else:
             fused_sgd_(self.flat_param, self.flat_grad, self.master, lr=self.lr)
-        return loss.detach()
+        return loss
 
     def set_lr(self, lr: float) -> None:
         """Change the learning rate (e.g. from a scheduler, once per step). The optimizer kernel reads it from a device
@@ -327,24 +379,53 @@ class FlatDataParallel:
                                   sumsq=self.sumsq if clip else None, step_tensor=self.step_t)
         self.comm.device_barrier(self.active)
 
-    def step(self, batch: Dict[str, torch.Tensor]) -> torch.Tensor:
-        """Eager step on device-resident inputs. Returns the (device) loss."""
-        loss = self._step_body(batch)
+    def _micro_batches(self, batches, who: str, like: Optional[List[Dict[str, torch.Tensor]]] = None):
+        """``batches`` as a list of the step's M micro-batch dicts; ``ValueError`` unless it is a sequence of M dicts
+        (or one dict when M = 1) whose keys and tensor shapes agree with each other and with ``like``'s."""
+        M = self.grad_accum_steps
+        if isinstance(batches, Mapping):
+            if M != 1:
+                raise ValueError(f"{who}: gradient_accumulation_steps = {M} takes a sequence of {M} micro-batch dicts, "
+                                 "got one dict")
+            batches = [batches]
+        elif isinstance(batches, (list, tuple)):
+            batches = list(batches)
+        else:
+            raise ValueError(f"{who}: expected a batch dict or a sequence of them, got {type(batches).__name__}")
+        if len(batches) != M or not all(isinstance(b, Mapping) for b in batches):
+            raise ValueError(f"{who}: gradient_accumulation_steps = {M} takes {M} micro-batch dicts, got "
+                             f"{len(batches)} items")
+
+        def shapes(b):
+            return {k: tuple(v.shape) if torch.is_tensor(v) else None for k, v in b.items()}
+
+        want = shapes(like[0] if like else batches[0])
+        for m, b in enumerate(batches):
+            if shapes(b) != want:
+                raise ValueError(f"{who}: micro-batch {m} has shapes {shapes(b)}, "
+                                 f"{'the captured step' if like else 'micro-batch 0'} has {want}")
+        return batches
+
+    def step(self, batch) -> torch.Tensor:
+        """Eager optimizer step on device-resident inputs: one batch dict, or a sequence of
+        ``gradient_accumulation_steps`` micro-batch dicts. Returns the (device) loss, the mean over the micro-batches."""
+        loss = self._step_body(self._micro_batches(batch, "step"))
         self.steps_done += 1
         return loss
 
     # -- CUDA graph ---------------------------------------------------------------------------------
-    def capture(self, example_batch: Dict[str, torch.Tensor], warmup: int = 2) -> None:
-        """Capture one full step. ``example_batch`` fixes the shapes; later steps copy their inputs
-        into the static buffers (``step_graph``)."""
+    def capture(self, example_batch, warmup: int = 2) -> None:
+        """Capture one full optimizer step, all its micro-batches in one graph. ``example_batch`` (one batch dict, or the
+        sequence of ``gradient_accumulation_steps`` micro-batch dicts ``step`` takes) fixes the shapes; later steps
+        copy their inputs into the static buffers, one dict per micro-batch (``step_graph``)."""
         from ..runtime.native import load_library
 
-        self._static = {k: v.clone() for k, v in example_batch.items()}
+        self._static_batches = [{k: v.clone() for k, v in b.items()} for b in self._micro_batches(example_batch, "capture")]
         s = torch.cuda.Stream(device=self.device)
         s.wait_stream(torch.cuda.current_stream(self.device))
         with torch.cuda.stream(s):
             for _ in range(warmup):                       # allocator + cuBLAS workspaces settle
-                self._step_body(self._static)
+                self._step_body(self._static_batches)
                 self.steps_done += 1
         torch.cuda.current_stream(self.device).wait_stream(s)
         torch.cuda.synchronize(self.device)
@@ -352,13 +433,16 @@ class FlatDataParallel:
         c0 = lib.adapcc_launch_count() if hasattr(lib, "adapcc_launch_count") else 0
         self._graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(self._graph):
-            self._static_loss = self._step_body(self._static)
+            self._static_loss = self._step_body(self._static_batches)
         self.native_launches_per_step = (lib.adapcc_launch_count() - c0) if hasattr(lib, "adapcc_launch_count") else 0
 
-    def step_graph(self, batch: Dict[str, torch.Tensor]) -> torch.Tensor:
-        """Copy ``batch`` (pinned host or device tensors) into the static inputs and replay."""
-        for k, v in batch.items():
-            self._static[k].copy_(v, non_blocking=True)
+    def step_graph(self, batch) -> torch.Tensor:
+        """Copy ``batch`` (pinned host or device tensors; the form ``step`` takes) into the static inputs and
+        replay. Every micro-batch dict must have the captured keys and shapes (``ValueError`` otherwise, also at M = 1:
+        a key left out would replay the previous step's tensor)."""
+        for static, batch in zip(self._static_batches, self._micro_batches(batch, "step_graph", self._static_batches)):
+            for k, v in batch.items():
+                static[k].copy_(v, non_blocking=True)
         self._graph.replay()
         self.steps_done += 1
         return self._static_loss

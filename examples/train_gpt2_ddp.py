@@ -22,7 +22,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from adapcc_b200 import ALLREDUCE  # noqa: E402
 from adapcc_b200.adapcc import AdapCC  # noqa: E402
 from adapcc_b200.models.gpt2 import GPT2Config, GPT2DoubleHeads, lm_rows_needed, synthetic_batch  # noqa: E402
-from adapcc_b200.parallel.ddp import rebuild_buckets, wrap_ddp  # noqa: E402
+from adapcc_b200.parallel.ddp import ddp_accumulate, rebuild_buckets, wrap_ddp  # noqa: E402
 from adapcc_b200.parallel.engine import FlatDataParallel  # noqa: E402
 
 
@@ -56,7 +56,12 @@ def main():
     p.add_argument("--dropout", type=float, default=0.0,
                    help="embedding, residual and summary dropout probability (HF GPT-2's default is 0.1); 0: off")
     p.add_argument("--dropout_seed", type=int, default=0, help="seed of the dropout masks (rank r uses seed + r)")
+    p.add_argument("--gradient_accumulation_steps", type=int, default=1,
+                   help="micro-batches (of --train_batch_size each) per optimizer step; --steps counts optimizer steps")
     a = p.parse_args()
+    M = a.gradient_accumulation_steps
+    if M < 1:
+        raise SystemExit("--gradient_accumulation_steps must be >= 1")
 
     rank, world, local = (int(os.environ.get(k, d)) for k, d in (("RANK", 0), ("WORLD_SIZE", 1), ("LOCAL_RANK", 0)))
     torch.cuda.set_device(local)
@@ -81,13 +86,13 @@ def main():
         model.lm_row_capacity = max(lm_rows_needed(b["lm_labels"].cpu()) for b in batches)
     if a.engine == "flat":
         eng = FlatDataParallel(model, comm.native if world > 1 else None, world_size=world, rank=rank, lr=a.lr,
-                               max_norm=a.max_norm, dropout_seed=a.dropout_seed)
+                               max_norm=a.max_norm, dropout_seed=a.dropout_seed, gradient_accumulation_steps=M)
         if a.checkpoint and os.path.exists(a.checkpoint):            # before capture: the lr is baked into the graph
             eng.load_state_dict(torch.load(a.checkpoint, map_location="cpu", weights_only=False))
             if rank == 0:
                 print("resumed from %s at step %d" % (a.checkpoint, eng.steps_done), flush=True)
         if a.graph:
-            eng.capture(batches[0])
+            eng.capture([batches[j % len(batches)] for j in range(M)] if M > 1 else batches[0])
         step = (lambda b: eng.step_graph(b)) if a.graph else (lambda b: eng.step(b))
     else:
         model = model.bfloat16()
@@ -95,17 +100,16 @@ def main():
         ddp = wrap_ddp(model, comm, local, bucket_cap_mb=25)
         opt = torch.optim.AdamW(ddp.parameters(), lr=a.lr, fused=True)
 
-        def step(b, _i=[0]):
+        def step(micro, _i=[0]):
             comm.update_relay(step=_i[0])
-            loss = ddp(**b, lm_coef=a.lm_coef, mc_coef=a.mc_coef)[0]
             opt.zero_grad(set_to_none=False)
-            loss.backward()
+            loss = ddp_accumulate(ddp, micro if M > 1 else [micro], lm_coef=a.lm_coef, mc_coef=a.mc_coef)
             torch.nn.utils.clip_grad_norm_(ddp.parameters(), a.max_norm)
             opt.step()
             if _i[0] == 0:
                 rebuild_buckets(ddp, comm)
             _i[0] += 1
-            return loss.detach()
+            return loss
 
     for i in range(a.steps):
         if i and AdapCC.profile_freq and i % AdapCC.profile_freq == 0 and a.engine == "ddp":
@@ -113,7 +117,7 @@ def main():
         t0 = time.time()
         if a.linear_decay and a.engine == "flat":
             eng.set_lr(a.lr * max(0.0, 1.0 - i / max(1, a.steps)))
-        loss = step(batches[i % len(batches)])
+        loss = step([batches[(i * M + j) % len(batches)] for j in range(M)] if M > 1 else batches[i % len(batches)])
         torch.cuda.synchronize()
         if rank == 0:
             print("step %d loss %.4f computation time: %.3f" % (i, loss.item(), time.time() - t0), flush=True)

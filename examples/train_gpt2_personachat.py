@@ -24,10 +24,11 @@ import torch.distributed as dist
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from adapcc_b200 import ALLREDUCE  # noqa: E402
 from adapcc_b200.adapcc import AdapCC  # noqa: E402
-from adapcc_b200.data import (DialogTokenizer, PinnedPrefetcher, corpus_of, get_data_loaders,  # noqa: E402
+from adapcc_b200.data import (DialogTokenizer, corpus_of, get_data_loaders, micro_batch_groups,  # noqa: E402
                               synthetic_personachat)
 from adapcc_b200.eval import evaluate_tensors, pack_checkpoint  # noqa: E402
 from adapcc_b200.models.gpt2 import GPT2Config, GPT2DoubleHeads  # noqa: E402
+from adapcc_b200.parallel.ddp import ddp_accumulate  # noqa: E402
 
 
 def build_tokenizer(a, cfg, rank):
@@ -84,7 +85,12 @@ def main():
     p.add_argument("--dropout", type=float, default=0.0,
                    help="embedding, residual and summary dropout probability (HF GPT-2's default is 0.1); 0: off")
     p.add_argument("--dropout_seed", type=int, default=0, help="seed of the dropout masks (rank r uses seed + r)")
+    p.add_argument("--gradient_accumulation_steps", type=int, default=1,
+                   help="micro-batches (of --train_batch_size each) per optimizer step; steps count optimizer steps")
     a = p.parse_args()
+    M = a.gradient_accumulation_steps
+    if M < 1:
+        raise SystemExit("--gradient_accumulation_steps must be >= 1")
     a.synthetic = dict(n_train=a.synthetic_dialogs, n_valid=max(8, a.synthetic_dialogs // 8), n_candidates=4, seed=a.seed)
 
     rank, world, local = (int(os.environ.get(k, d)) for k, d in (("RANK", 0), ("WORLD_SIZE", 1), ("LOCAL_RANK", 0)))
@@ -109,11 +115,13 @@ def main():
     T = train_loader.dataset.tensors["input_ids"].shape[-1]
     if T > cfg.n_positions:
         raise SystemExit(f"inputs are {T} tokens long, the model has {cfg.n_positions} positions: pass --seq_len")
-    steps_per_epoch = len(train_loader)
+    steps_per_epoch = len(train_loader) // M                      # optimizer steps; a partial last group is skipped
+    if steps_per_epoch == 0:
+        raise SystemExit(f"{len(train_loader)} batches per epoch are fewer than --gradient_accumulation_steps {M}")
     total_steps = a.n_epochs * steps_per_epoch if not a.max_steps else min(a.max_steps, a.n_epochs * steps_per_epoch)
     if rank == 0:
         print(f"train {tuple(train_loader.dataset.tensors['input_ids'].shape)} valid "
-              f"{tuple(valid_loader.dataset.tensors['input_ids'].shape)} (N, candidates, T); {steps_per_epoch} steps/epoch/rank; "
+              f"{tuple(valid_loader.dataset.tensors['input_ids'].shape)} (N, candidates, T); {steps_per_epoch} steps/epoch/rank of {M} micro-batch(es); "
               f"vocab {tok.base_vocab} + 5 special of {cfg.vocab_size}", flush=True)
 
     torch.manual_seed(a.seed)
@@ -129,7 +137,8 @@ def main():
         from adapcc_b200.parallel.engine import FlatDataParallel
 
         eng = FlatDataParallel(model, comm.native if world > 1 else None, world_size=world, rank=rank, lr=a.lr,
-                               max_norm=a.max_norm, weight_decay=0.0, dropout_seed=a.dropout_seed)
+                               max_norm=a.max_norm, weight_decay=0.0, dropout_seed=a.dropout_seed,
+                               gradient_accumulation_steps=M)
         if a.checkpoint and os.path.exists(a.checkpoint):
             ck = torch.load(a.checkpoint, map_location="cpu", weights_only=False)
             eng.load_state_dict(ck["engine"])
@@ -170,28 +179,27 @@ def main():
         if train_sampler is not None:
             train_sampler.set_epoch(epoch)
         t0, seen, run_loss = time.time(), 0, None
-        for batch in PinnedPrefetcher(train_loader, dev):
+        for micro in micro_batch_groups(train_loader, dev, M):
             if step >= total_steps:
                 break
             lr = a.lr * max(0.0, 1.0 - step / max(1, total_steps))            # PiecewiseLinear(lr -> 0)
             if eng is not None:
                 eng.set_lr(lr)
+                inputs = micro if M > 1 else micro[0]
                 if a.graph and not captured:
-                    eng.capture(batch)
+                    eng.capture(inputs)
                     captured = True
-                loss = eng.step_graph(batch) if a.graph else eng.step(batch)
+                loss = eng.step_graph(inputs) if a.graph else eng.step(inputs)
             else:
                 for g in opt.param_groups:
                     g["lr"] = lr
                 comm.update_relay(step)
-                loss = ddp(**batch, lm_coef=a.lm_coef, mc_coef=a.mc_coef)[0]
                 opt.zero_grad(set_to_none=False)
-                loss.backward()
+                loss = ddp_accumulate(ddp, micro, lm_coef=a.lm_coef, mc_coef=a.mc_coef)
                 torch.nn.utils.clip_grad_norm_(model.parameters(), a.max_norm)
                 opt.step()
-                loss = loss.detach()
             step += 1
-            seen += batch["input_ids"].numel()
+            seen += sum(b["input_ids"].numel() for b in micro)
             if step % 10 == 0 or step == total_steps:
                 v = float(loss)                                                # one device→host read per 10 steps
                 run_loss = v if run_loss is None else 0.98 * run_loss + 0.02 * v
