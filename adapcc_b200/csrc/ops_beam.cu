@@ -9,6 +9,9 @@
 //   beam_select : one warp per item. The K rows' N best, re-keyed by the flat index j * V + i, are walked in rank order
 //                 (rounds of a warp maximum): the first K non-stop candidates become the new beams, stop candidates
 //                 ranked before the K-th are offered to the finished set, and the done rule is applied (DESIGN.md §4a).
+//   beam_group_select : diverse (group) beam search's beam_select, one warp per item: the groups in order, each one's
+//                 candidates re-keyed with the Hamming penalty of the earlier groups' new tokens, then walked as in
+//                 beam_select with the group's own finished set and done flag (DESIGN.md §4a).
 //   kv_reorder  : cache[l, r, :, pos] = cache[l, parent[r], :, pos] for the generated positions, through a scratch
 //                 buffer (gather, then scatter), so cycles and many-to-one parent maps come out right.
 //
@@ -228,6 +231,133 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const __grid_constant__
 }
 
 __global__ void beam_step_incr_kernel(int* step) { *step += 1; }
+
+// ---- diverse (group) beam search ----------------------------------------------------------------------------------
+struct BeamGroupArgs {
+  BeamArgs a;                  // a.fin_* [B, K] read as [B, G, Kg]; a.fin_count [B * G]; a.done [B] the item flags
+  int G;                       // groups; group g owns the item's beams g * Kg .. (g + 1) * Kg - 1, Kg = K / G
+  int* group_done;             // [B * G]
+  float lambda;                // diversity penalty
+};
+
+// One warp per item; the groups in order g = 0 .. G-1. A candidate whose token the earlier groups' new beams of this
+// step took n > 0 times is re-keyed with c' = fl32(c - fl32(lambda * n)); n = 0 keeps c's key, so group 0 is beam_select
+// with K = Kg. The walk, the offers (to the group's own finished set of Kg) and the done rule are beam_select's, per
+// group. The rows' N = K + n_stop unpenalised best suffice: at most K - Kg tokens are penalised (DESIGN.md §4a).
+__global__ void __launch_bounds__(32) beam_group_select_kernel(const __grid_constant__ BeamGroupArgs p) {
+  __shared__ unsigned long long s_c[kBeamMaxK * kBeamMaxN];
+  __shared__ FinishedSet fs;
+  __shared__ int s_tok[kBeamMaxK], s_par[kBeamMaxK], s_taken[kBeamMaxK];
+  __shared__ float s_sc[kBeamMaxK];
+  const BeamArgs& a = p.a;
+  const int b = blockIdx.x, lane = threadIdx.x, K = a.K, N = a.N, V = a.vocab, BK = a.B * a.K, G = p.G, Kg = K / G;
+  const int step = *a.step;
+  if (a.done[b] || step >= a.max_new) {               // nothing moves: every row keeps its own cache
+    if (lane < K) a.parent[b * K + lane] = b * K + lane;
+    return;
+  }
+  const int L = step + 1;                             // tokens of a hypothesis that ends at this step
+  int n_taken = 0, all_done = 1;
+  for (int g = 0; g < G; ++g) {
+    const int j0 = g * Kg, fo = b * K + j0, gi = b * G + g;
+    if (p.group_done[gi]) {                           // a done group: dead rows that keep their own cache
+      if (lane < Kg) a.parent[fo + lane] = fo + lane;
+      continue;
+    }
+    for (int e = lane; e < Kg * N; e += 32) {
+      const int j = j0 + e / N;
+      const unsigned long long v = a.cand[(long long)(b * K + j) * N + (e - (j - j0) * N)];
+      const uint32_t i = 0xFFFFFFFFu - (uint32_t)v, flat = (uint32_t)j * (uint32_t)V + i;
+      uint32_t hi = (uint32_t)(v >> 32);
+      int n = 0;
+      for (int t = 0; t < n_taken; ++t) n += s_taken[t] == (int)i;
+      if (v && n) {
+        const float cp = __fsub_rn(beam_key2f(hi), __fmul_rn(p.lambda, (float)n));
+        hi = cp > -INFINITY ? beam_f2key(cp) : 0u;
+      }
+      s_c[e] = v && hi ? ((unsigned long long)hi << 32) | (0xFFFFFFFFu - flat) : 0ull;
+    }
+    if (lane == 0) {
+      fs.K = Kg;
+      fs.count = a.fin_count[gi];
+      for (int k = 0; k < Kg; ++k) {
+        fs.score[k] = a.fin_score[fo + k];
+        fs.n[k] = a.fin_n[fo + k];
+        fs.src[k] = a.fin_src[fo + k];
+      }
+    }
+    __syncwarp();
+    int nb = 0;
+    unsigned long long bound = ~0ull;
+    while (nb < Kg) {
+      unsigned long long best = 0ull;
+      for (int e = lane; e < Kg * N; e += 32) {
+        const unsigned long long v = s_c[e];
+        if (v < bound && v > best) best = v;
+      }
+      best = warp_max_u64(best);
+      if (best == 0ull) break;
+      bound = best;
+      const uint32_t flat = 0xFFFFFFFFu - (uint32_t)best;
+      const int j = (int)(flat / (uint32_t)V), i = (int)(flat - (uint32_t)j * (uint32_t)V);
+      const float c = beam_key2f((uint32_t)(best >> 32));
+      bool is_stop = false;
+      for (int q = 0; q < a.n_stop; ++q) is_stop |= a.stop[q] == i;
+      if (lane == 0) {
+        if (is_stop) {
+          fs.offer(c / a.pen[L], L - 1, j);
+        } else {
+          s_tok[nb] = i;
+          s_par[nb] = j;
+          s_sc[nb] = c;
+        }
+      }
+      nb += !is_stop;
+    }
+    __syncwarp();
+    int done = 0;
+    if (lane == 0) {
+      if (step == a.max_new - 1) {
+        for (int k = 0; k < nb; ++k) fs.offer(s_sc[k] / a.pen[a.max_new], a.max_new, j0 + k);
+        done = 1;
+      } else if (nb == 0) {
+        done = 1;
+      } else if (fs.count == Kg) {
+        const float reach = s_sc[0] / a.pen[a.alpha_pos ? a.max_new : L + 1];
+        done = !(reach > fs.score[Kg - 1]);
+      }
+      p.group_done[gi] = done;
+      a.fin_count[gi] = fs.count;
+      for (int k = 0; k < nb; ++k) s_taken[n_taken + k] = s_tok[k];
+    }
+    done = __shfl_sync(0xffffffffu, done, 0);
+    all_done &= done;
+    n_taken += nb;                                    // this step's new beams count, even if the group is now done
+    __syncwarp();
+    if (lane < Kg) {
+      const int r = fo + lane;
+      const long long h = (long long)step * BK + r;
+      if (lane < nb) {
+        a.next_ids[r] = s_tok[lane];
+        a.parent[r] = b * K + s_par[lane];
+        a.scores[r] = done ? -INFINITY : s_sc[lane];  // a done group's beams are dead from now on
+        a.hist_tok[h] = s_tok[lane];
+        a.hist_back[h] = s_par[lane];
+      } else {
+        a.next_ids[r] = 0;
+        a.parent[r] = r;
+        a.scores[r] = -INFINITY;
+        a.hist_tok[h] = -1;
+        a.hist_back[h] = j0 + lane;
+      }
+      a.fin_score[r] = fs.score[lane];
+      a.fin_n[r] = fs.n[lane];
+      a.fin_src[r] = fs.src[lane];
+    }
+    __syncwarp();
+  }
+  if (lane == 0) a.done[b] = all_done;
+}
 
 // ---- beam sampling ---------------------------------------------------------------------------------------------------
 struct BeamSampleArgs {
@@ -603,6 +733,58 @@ int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, float
   CUDA_TRY(cudaGetLastError());
   count_launch();
   beam_select_kernel<<<B, 32, 0, s>>>(a);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  beam_step_incr_kernel<<<1, 1, 0, s>>>(step);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// adapcc_beam_step's arguments with the groups G (K % G == 0), group_done int32 [B*G], fin_count int32 [B*G] and the
+// diversity penalty lambda (finite, >= 0)
+int adapcc_beam_group_step(const float* logits, int ld, int vocab, int B, int K, int G, float* scores, int* step,
+                           int min_new, const int* suppress, int n_suppress, const int* stop, int n_stop,
+                           const float* pen, int alpha_pos, int max_new, int* done, int* group_done, void* cand,
+                           long long* next_ids, int* parent, long long* hist_tok, int* hist_back, float* fin_score,
+                           int* fin_n, int* fin_src, int* fin_count, float lambda, void* stream) {
+  if (B < 1 || K < 1 || K > kBeamMaxK || G < 1 || K % G != 0 || vocab < 1 || ld < vocab || max_new < 1 ||
+      (unsigned long long)K * (unsigned long long)vocab > 0xFFFFFFFFull) {
+    set_error("beam_group_step: need B >= 1, 1 <= K <= %d, G >= 1 dividing K, vocab >= 1, ld >= vocab, K * vocab < "
+              "2^32, max_new >= 1 (B=%d K=%d G=%d vocab=%d ld=%d max_new=%d)", kBeamMaxK, B, K, G, vocab, ld, max_new);
+    return -1;
+  }
+  if (n_suppress < 0 || n_suppress > kBeamMaxSuppress || n_stop < 0 || n_stop > kBeamMaxStop ||
+      (n_suppress && !suppress) || (n_stop && !stop)) {
+    set_error("beam_group_step: at most %d suppressed and %d stop ids (got %d, %d)", kBeamMaxSuppress, kBeamMaxStop,
+              n_suppress, n_stop);
+    return -1;
+  }
+  if (!(lambda >= 0.f && lambda < INFINITY)) {
+    set_error("beam_group_step: the diversity penalty must be finite and >= 0 (got %g)", lambda);
+    return -1;
+  }
+  if (!logits || !scores || !step || !pen || !done || !group_done || !cand || !next_ids || !parent || !hist_tok ||
+      !hist_back || !fin_score || !fin_n || !fin_src || !fin_count) {
+    set_error("beam_group_step: null pointer");
+    return -1;
+  }
+  const size_t bits = n_suppress > 0 && min_new > 0 ? (size_t)(vocab + 31) / 32 * sizeof(uint32_t) : 0;
+  if (bits > 200 * 1024) {
+    set_error("beam_group_step: suppression needs vocab <= %d (got %d)", 200 * 1024 * 8, vocab);
+    return -1;
+  }
+  if (bits > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(beam_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                                      (int)bits));
+  BeamGroupArgs p{BeamArgs{logits, ld, vocab, B, K, K + n_stop, scores, step, min_new, suppress, n_suppress, stop,
+                           n_stop, pen, alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
+                           hist_back, fin_score, fin_n, fin_src, fin_count},
+                  G, group_done, lambda};
+  cudaStream_t s = (cudaStream_t)stream;
+  beam_rows_kernel<<<B * K, kBeamThreads, bits, s>>>(p.a);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  beam_group_select_kernel<<<B, 32, 0, s>>>(p);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   beam_step_incr_kernel<<<1, 1, 0, s>>>(step);

@@ -93,7 +93,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    penalty_alpha: float = 0.0, prompt_lookup_num_tokens: int = 0, min_p: float = 0.0,
                    typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
                    assistant_model=None, num_assistant_tokens: int = 4,
-                   assistant_verification: str = "coupled", beam_sample: bool = False) -> List[List[int]]:
+                   assistant_verification: str = "coupled", beam_sample: bool = False, num_beam_groups: int = 1,
+                   diversity_penalty: float = 0.0) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -111,7 +112,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     ``penalty_alpha`` it is a ``ValueError``. ``assistant_verification="rejection"`` verifies the drafts by rejection
     sampling instead: each reply token is still drawn from the model's distribution, but not the same draw.
     ``beam_sample`` with ``num_beams > 0``: beam sampling (``beam_search(do_sample=True)``) with ``temperature``,
-    ``top_k``, ``top_p`` and the seeds."""
+    ``top_k``, ``top_p`` and the seeds. ``num_beam_groups`` and ``diversity_penalty`` go to ``beam_search`` (diverse
+    beam search, ``ops/beam.py``)."""
     from ..ops.assisted import check_verification
     check_verification("sample_replies", assistant_verification, assistant_model)
     if assistant_model is not None and (num_beams > 0 or penalty_alpha > 0):
@@ -133,7 +135,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
             else {}
         tokens, n_new, _ = model.beam_search(ids, lengths, tt, reply_type, num_beams=num_beams,
                                              max_new_tokens=max_length, stop_ids=special, suppress_ids=special,
-                                             min_new_tokens=min_length, **repeats, **sampled)
+                                             min_new_tokens=min_length, num_beam_groups=num_beam_groups,
+                                             diversity_penalty=diversity_penalty, **repeats, **sampled)
         return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
     if penalty_alpha > 0:
         tokens, n_new = model.contrastive_search(ids, lengths, tt, reply_type, top_k=top_k, penalty_alpha=penalty_alpha,
@@ -237,7 +240,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      prompt_lookup_num_tokens: int = 0, min_p: float = 0.0, typical_p: float = 1.0,
                      epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model=None,
                      num_assistant_tokens: int = 4, assistant_verification: str = "coupled",
-                     beam_sample: bool = False, **sample_kw) -> Dict[str, float]:
+                     beam_sample: bool = False, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
+                     **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -248,7 +252,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
 
     ``num_beams > 0`` with ``f1``: the replies are decoded by beam search instead (:func:`sample_replies`), on that
     batched path (one example at a time when ``batch_size`` is 0); with ``beam_sample`` by beam sampling, with the
-    sampling arguments and the batched path's seeds.
+    sampling arguments and the batched path's seeds; with ``num_beam_groups`` > 1 by diverse beam search with
+    ``diversity_penalty``.
 
     ``repetition_penalty != 1`` or ``no_repeat_ngram_size > 0`` with ``f1``: the repetition controls of
     ``generate`` / ``beam_search`` (``ops/repeats.py``), also on that batched path.
@@ -280,7 +285,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                                     prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters,
                                     assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
                                     assistant_verification=assistant_verification, beam_sample=beam_sample,
-                                    **sample_kw)
+                                    num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty, **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -782,7 +782,8 @@ class GPT2DoubleHeads(nn.Module):
                     suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
                     no_repeat_ngram_size: int = 0, do_sample: bool = False, temperature: float = 1.0,
                     top_k: int = 0, top_p: float = 1.0, seed=0,
-                    num_return_sequences: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    num_return_sequences: int = 1, num_beam_groups: int = 1,
+                    diversity_penalty: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -802,6 +803,13 @@ class GPT2DoubleHeads(nn.Module):
         (item b uses ``seed + b``) or an int64 [B] tensor; an item's result depends on its prompt, its seed and the
         scalars. With ``do_sample=False`` the sampling arguments are ignored.
 
+        ``num_beam_groups`` = G > 1 is diverse beam search (HuggingFace 4.x's ``num_beam_groups`` /
+        ``diversity_penalty``; the definition is ``ops.beam.GroupBeamReference``): the beams form G groups of
+        ``num_beams / G`` that select in order each step, a candidate's score lowered by ``diversity_penalty`` (finite,
+        > 0) for each new beam of an earlier group of the item with the same token; each group keeps its own
+        ``num_beams / G`` finished hypotheses and the results are their union, best first. G must divide
+        ``num_beams``, cannot be combined with ``do_sample`` and, for G = 1, ``diversity_penalty`` must be 0.
+
         Returns ``(tokens, n_new, scores)``: the ``num_return_sequences`` = r (``1 <= r <= num_beams``) best hypotheses
         of each item, as rows ``b * r + q``, best first: int64 [B·r, max_new_tokens] (the stop token excluded, padded
         with -1), their lengths int64 [B·r] and their normalised scores fp32 [B·r]. An item with fewer than r
@@ -814,10 +822,11 @@ class GPT2DoubleHeads(nn.Module):
         reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the host reads the done flags once every 8
         tokens, a period late. Beam sampling takes a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids there, and
         the items' seeds are a device input of the graph. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
-        ``ops.repeats.penalize_repeats_reference``, ``ops.beam.BeamReference`` (``BeamSampleReference``) and torch
-        indexing."""
+        ``ops.repeats.penalize_repeats_reference``, ``ops.beam.BeamReference`` (``BeamSampleReference``,
+        ``GroupBeamReference``) and torch indexing."""
         from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB
-        from ..ops.beam import BeamReference, BeamSampleReference, best_hypotheses
+        from ..ops.beam import (BeamReference, BeamSampleReference, GroupBeamReference, best_hypotheses,
+                                merge_finished_sets)
 
         K = int(num_beams)
         if not 1 <= K <= BEAM_MAX_BEAMS:
@@ -827,6 +836,14 @@ class GPT2DoubleHeads(nn.Module):
             raise ValueError(f"beam_search: num_return_sequences must be in [1, num_beams = {K}], got "
                              f"{num_return_sequences}")
         do_sample = bool(do_sample)
+        G, lam = int(num_beam_groups), float(diversity_penalty)
+        if not 1 <= G <= K or K % G != 0:
+            raise ValueError(f"beam_search: num_beam_groups must divide num_beams = {K}, got {num_beam_groups}")
+        if G > 1 and (do_sample or not (math.isfinite(lam) and lam > 0)):
+            raise ValueError(f"beam_search: num_beam_groups > 1 needs do_sample=False and a finite diversity_penalty "
+                             f"> 0, got do_sample={do_sample}, diversity_penalty={diversity_penalty}")
+        if G == 1 and lam != 0:
+            raise ValueError(f"beam_search: diversity_penalty needs num_beam_groups > 1, got {diversity_penalty}")
         if do_sample and not temperature > 0:
             raise ValueError(f"beam_search: do_sample=True needs temperature > 0, got {temperature}")
         if do_sample and (int(top_k) < 0 or not 0 < top_p <= 1):
@@ -856,6 +873,9 @@ class GPT2DoubleHeads(nn.Module):
                 ref = BeamSampleReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
                                           temperature=temperature, top_k=top_k, top_p=top_p,
                                           seeds=seeds.cpu().tolist())
+            elif G > 1:
+                ref = GroupBeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
+                                         num_beam_groups=G, diversity_penalty=lam)
             else:
                 ref = BeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens)
             head = weight.float()
@@ -880,8 +900,10 @@ class GPT2DoubleHeads(nn.Module):
         if do_sample and V > SAMPLE_MAX_VOCAB:
             raise ValueError(f"beam_search: do_sample=True needs a vocabulary of at most {SAMPLE_MAX_VOCAB} ids on the "
                              f"native path, got {V}")
-        st = BeamState(B, K, n, length_penalty, dev, sample=do_sample)
+        st = BeamState(B, K, n, length_penalty, dev, sample=do_sample, groups=G)
         scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds) if do_sample else {}
+        if G > 1:
+            scalars = dict(diversity_penalty=lam)
         logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
         sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
         prompt_len = cache.lens.clone()
@@ -898,9 +920,10 @@ class GPT2DoubleHeads(nn.Module):
         if n > 1:
             # beam_step_ writes the new beams' tokens into the graph's own input buffer
             DecodeGraph(self, cache, tt_new is not None, head=select, ids=st.next_ids, tt=tt_new).run(n - 1, st.done)
-        count = st.fin_count.cpu().tolist()
+        count, Kg = st.fin_count.cpu().tolist(), K // G
         score, n_tok, src = st.fin_score.cpu().tolist(), st.fin_n.cpu().tolist(), st.fin_src.cpu().tolist()
-        fin = [list(zip(score[b], n_tok[b], src[b]))[:count[b]] for b in range(B)]
+        fin = [merge_finished_sets([list(zip(score[b], n_tok[b], src[b]))[g * Kg:g * Kg + count[b * G + g]]
+                                    for g in range(G)]) for b in range(B)]
         hist_tok = st.hist_tok.view(n, B, K).cpu().numpy()
         hist_back = st.hist_back.view(n, B, K).cpu().numpy()
         return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n, R))

@@ -59,6 +59,9 @@ def _lib():
         lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                          + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                          + [c_void_p] * 10 + [c_void_p])
+        lib.adapcc_beam_group_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
+                                               + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
+                                               + [c_void_p] * 11 + [c_float, c_void_p])
         lib.adapcc_beam_sample_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                                 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                                 + [c_void_p] * 11 + [c_float, c_int, c_float, c_void_p, c_void_p])
@@ -492,17 +495,27 @@ class BeamState:
     ``fin_n - 1`` holds them) with ``fin_count`` int32 [B]; ``pen`` fp32 [max_new + 1], ``pen[L] = L ** length_penalty``
     rounded to fp32 once on the host, so the kernel needs no ``powf``. With ``sample`` (beam sampling) the candidate
     scratch holds ``(BEAM_MAX_STOP + 1) · K`` keys per row, the most any sample draws, with ``cand_c`` fp32 beside it;
-    a step with M = ``max(2, 1 + n_stop) · K`` uses the first ``B·K·M`` entries of each as [B·K, M]."""
+    a step with M = ``max(2, 1 + n_stop) · K`` uses the first ``B·K·M`` entries of each as [B·K, M].
 
-    def __init__(self, batch: int, num_beams: int, max_new: int, length_penalty: float, device, sample: bool = False):
-        B, K, n = int(batch), int(num_beams), int(max_new)
+    ``groups`` = G > 1 (diverse beam search, ``ops.beam.GroupBeamReference``; G divides K, not with ``sample``): group g
+    owns beams ``g·K/G .. (g+1)·K/G - 1``, each group's beam 0 starts at 0, the finished arrays [B, K] are read as
+    [B, G, K/G] (one set per group), ``fin_count`` and ``group_done`` are int32 [B·G], and ``done`` stays the item
+    flag [B]: all of the item's groups are done."""
+
+    def __init__(self, batch: int, num_beams: int, max_new: int, length_penalty: float, device, sample: bool = False,
+                 groups: int = 1):
+        B, K, n, G = int(batch), int(num_beams), int(max_new), int(groups)
         if B < 1 or not 1 <= K <= BEAM_MAX_BEAMS or n < 1:
             raise ValueError(f"BeamState: need batch >= 1, 1 <= num_beams <= {BEAM_MAX_BEAMS} and max_new >= 1, got "
                              f"{batch}, {num_beams}, {max_new}")
+        if not 1 <= G <= K or K % G != 0 or (G > 1 and sample):
+            raise ValueError(f"BeamState: groups must divide num_beams = {K} and cannot be combined with sample, got "
+                             f"{groups} (sample={sample})")
         self.batch, self.num_beams, self.max_new, self.length_penalty = B, K, n, float(length_penalty)
+        self.groups = G
         i32, dev = dict(dtype=torch.int32, device=device), device
         self.scores = torch.full((B, K), float("-inf"), dtype=torch.float32, device=dev)
-        self.scores[:, 0] = 0.0
+        self.scores[:, ::K // G] = 0.0
         self.scores = self.scores.reshape(B * K)
         self.step = torch.zeros(1, **i32)
         self.done = torch.zeros(B, **i32)
@@ -513,7 +526,8 @@ class BeamState:
         self.fin_score = torch.full((B, K), float("-inf"), dtype=torch.float32, device=dev)
         self.fin_n = torch.zeros(B, K, **i32)
         self.fin_src = torch.zeros(B, K, **i32)
-        self.fin_count = torch.zeros(B, **i32)
+        self.fin_count = torch.zeros(B * G, **i32)
+        self.group_done = torch.zeros(B * G, **i32)
         self.pen = torch.tensor([float(L) ** self.length_penalty if L else 1.0 for L in range(n + 1)],
                                 dtype=torch.float64).to(device=dev, dtype=torch.float32)
         self.sample = bool(sample)
@@ -524,13 +538,14 @@ class BeamState:
     def tensors(self):
         """Every device tensor of the state (what ``beam_step_`` checks for one device)."""
         return (self.scores, self.step, self.done, self.next_ids, self.parent, self.hist_tok, self.hist_back,
-                self.fin_score, self.fin_n, self.fin_src, self.fin_count, self.pen, self.cand, self.cand_c)
+                self.fin_score, self.fin_n, self.fin_src, self.fin_count, self.group_done, self.pen, self.cand,
+                self.cand_c)
 
 
 def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int = 0,
                suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None,
                temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
-               seeds: Optional[torch.Tensor] = None) -> None:
+               seeds: Optional[torch.Tensor] = None, diversity_penalty: float = 0.0) -> None:
     """One beam-search selection for every item, on the device (the definition in ``ops/beam.py``, which computes the
     same in fp64). ``logits`` fp32 [B·K, ld] (the first ``vocab`` columns used) are the beams' next-token logits;
     ``suppress_ids`` (removed while ``state.step < min_new``) and ``stop_ids`` (at most 8; they finish a hypothesis)
@@ -541,12 +556,21 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
     With ``seeds`` (int64 [B] on the device, each item's Philox key) the step is beam sampling
     (``BeamSampleReference``): a ``BeamState(..., sample=True)``, ``temperature > 0``, ``top_k`` (0: off) and
     ``top_p`` filter each beam's ids, and the candidates are drawn rather than ranked; vocab is at most
-    ``SAMPLE_MAX_VOCAB``. Without ``seeds`` the sampling scalars are ignored."""
+    ``SAMPLE_MAX_VOCAB``. Without ``seeds`` the sampling scalars are ignored.
+
+    A state with ``groups`` > 1 is diverse beam search (``GroupBeamReference``): the groups select in order, a
+    candidate's score lowered by ``diversity_penalty`` (finite, > 0; 0 for one group) per new beam of an earlier group
+    of the item that took its token this step."""
     def bad(msg):
         raise ValueError(f"beam_step_: {msg}")
 
     if not isinstance(state, BeamState):
         bad(f"state must be a BeamState, got {type(state).__name__}")
+    lam = float(diversity_penalty)
+    if state.groups > 1 and not (math.isfinite(lam) and lam > 0):
+        bad(f"a BeamState with {state.groups} groups needs a finite diversity_penalty > 0, got {diversity_penalty}")
+    if state.groups == 1 and lam != 0:
+        bad(f"diversity_penalty needs a BeamState with groups > 1, got {diversity_penalty}")
     if seeds is not None:
         if not state.sample:
             bad("sampling needs a BeamState(..., sample=True)")
@@ -575,6 +599,14 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
             _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_n), _ptr(state.fin_src),
             _ptr(state.fin_count), float(temperature), int(top_k), float(top_p), _ptr(seeds), _stream()),
             "beam_sample_step")
+        return
+    if state.groups > 1:
+        _ck(_lib().adapcc_beam_group_step(
+            _ptr(logits), logits.stride(0), int(vocab), B, K, state.groups, _ptr(state.scores), _ptr(state.step),
+            int(min_new), sup, n_sup, stop, n_stop, _ptr(state.pen), int(state.length_penalty > 0), state.max_new,
+            _ptr(state.done), _ptr(state.group_done), _ptr(state.cand), _ptr(state.next_ids), _ptr(state.parent),
+            _ptr(state.hist_tok), _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_n),
+            _ptr(state.fin_src), _ptr(state.fin_count), lam, _stream()), "beam_group_step")
         return
     _ck(_lib().adapcc_beam_step(_ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores),
                                 _ptr(state.step), int(min_new), sup, n_sup, stop, n_stop, _ptr(state.pen),

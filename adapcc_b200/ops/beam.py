@@ -54,6 +54,32 @@ S5. a candidate finishes if its token is a stop id or the step is the last (``ma
 Rules 6 and 7 are unchanged; the done rule stays exact because ``lp / T <= 0``. Item b's seed is ``seed + b`` for an
 int ``seed`` or ``seeds[b]``; its result depends on its prompt, its seed and the scalars only.
 
+Diverse (group) beam search (``GroupBeamReference``, Vijayakumar et al. 2016; HuggingFace 4.x's
+``_group_beam_search`` with ``HammingDiversityLogitsProcessor``) splits an item's K beams into G = ``num_beam_groups``
+groups of ``K_g = K / G``: group g owns beams ``g·K_g .. (g+1)·K_g - 1`` (rows ``b·K + j``), and each group's first
+beam starts at 0, the others at -inf. With ``λ = fl32(diversity_penalty)``, per step the groups of an item that is not
+done are processed in order g = 0 .. G-1, skipping done groups:
+
+G1. rules 1 and 2 are unchanged (the repetition controls act before them);
+G2. ``n_i`` is the number of this step's new beams of groups 0..g-1 of the item whose token is i (stop candidates,
+    dead beams and groups done before this step count for nothing; a group that becomes done this step counts); a
+    candidate scores ``c = s_j + lp_i - λ·n_i``, so the running sums and the finished scores include the penalty;
+G3. rules 3-5 within the group, with K_g for K: its candidates only are ranked, its first K_g non-stop candidates
+    become its beams in rank order, and a stop candidate ranked before the K_g-th non-stop one is offered to the
+    group's finished set;
+G4. rule 6 per (item, group): each set holds at most K_g hypotheses;
+G5. rule 7 per group: a group is done when its set is full and its best live beam cannot beat its worst hypothesis
+    (exact, because λ >= 0 only lowers sums); a done group's beams are dead; an item is done when all its groups are;
+    rule 8 applies per group at ``max_new``;
+G6. an item's hypotheses are the union of its groups' sets by descending normalised score, a tie to the lower group,
+    then to the group's own order (``merge_finished_sets``).
+
+G = 1 is the beam search above. Group 0 evolves exactly as a beam search of K_g beams on its rows. Per row the
+best ``K + n_stop`` unpenalised candidates still decide the selection: at most ``g·K_g <= K - K_g`` tokens are
+penalised, so a candidate past them ranks below at least ``K_g + n_stop`` of its row's candidates. Deliberate
+differences from HuggingFace 4.x: the repetition controls act before the log-softmax, the done rule is the exact one,
+and done groups add no pad tokens to the Hamming counts.
+
 ``best_hypotheses(..., num_return_sequences=r)`` returns each item's first r finished hypotheses, best first, as rows
 ``b · r + q`` (HuggingFace's flattening); rows past an item's count have no tokens, ``n_new`` 0 and score -inf.
 """
@@ -96,14 +122,7 @@ class BeamReference:
     def offer(self, b: int, score: float, n: int, src: int) -> None:
         """Rule 6: offer item b's finished set a hypothesis of normalised score ``score``, ``n`` tokens (without its
         stop token) and source beam ``src``."""
-        fin = self.fin[b]
-        if len(fin) == self.K and not score > fin[-1][0]:
-            return
-        p = len(fin)
-        while p > 0 and fin[p - 1][0] < score:
-            p -= 1
-        fin.insert(p, (score, n, src))
-        del fin[self.K:]
+        offer_finished(self.fin[b], self.K, score, n, src)
 
     def candidates(self, logits_row: np.ndarray, s: float, step: int) -> np.ndarray:
         """fp64 scores ``c_i = s + lp_i`` of one beam row (-inf for removed ids)."""
@@ -119,18 +138,21 @@ class BeamReference:
     def ranking(self, b: int, logits: np.ndarray, step: int) -> List[Tuple[float, int, int]]:
         """Item b's finite candidates ``(c, j, i)`` in rank order, the best ``K + n_stop`` of each row (rule 5: the
         walk never reaches further into a row)."""
-        K, V = self.K, self.vocab
-        keep = K + len(self.stop)
-        rows = []
-        for j in range(K):
-            c = self.candidates(logits[b * K + j], self.scores[b, j], step)
-            ids = np.flatnonzero(c > -np.inf)
-            if ids.size > keep:                                  # every id tied with the keep-th best stays in
-                ids = ids[c[ids] >= np.partition(c[ids], ids.size - keep)[ids.size - keep]]
-            ids = ids[np.lexsort((ids, -c[ids]))][:keep]
-            rows.extend((float(c[i]), j * V + int(i)) for i in ids)
+        V = self.vocab
+        rows = [(c, j * V + i) for j in range(self.K) for c, i in self.row_best(b, j, logits, step)]
         rows.sort(key=lambda t: (-t[0], t[1]))
         return [(c, f // V, f % V) for c, f in rows]
+
+    def row_best(self, b: int, j: int, logits: np.ndarray, step: int) -> List[Tuple[float, int]]:
+        """Beam row j of item b: its best ``K + n_stop`` finite candidates ``(c, i)``, best first, ties to the lower
+        id."""
+        keep = self.K + len(self.stop)
+        c = self.candidates(logits[b * self.K + j], self.scores[b, j], step)
+        ids = np.flatnonzero(c > -np.inf)
+        if ids.size > keep:                                      # every id tied with the keep-th best stays in
+            ids = ids[c[ids] >= np.partition(c[ids], ids.size - keep)[ids.size - keep]]
+        ids = ids[np.lexsort((ids, -c[ids]))][:keep]
+        return [(float(c[i]), int(i)) for i in ids]
 
     def step(self, logits) -> Tuple[torch.Tensor, torch.Tensor]:
         """One selection (rules 1-8) for every item that is not done; see the class docstring."""
@@ -179,6 +201,116 @@ class BeamReference:
         """``(tokens, n_new, scores)``: int64 [B·r, max_new] padded with -1, int64 [B·r], fp32 [B·r] of each item's r
         best hypotheses (no tokens and -inf past an item's count)."""
         return best_hypotheses(self.fin, self.hist_tok, self.hist_back, self.max_new, num_return_sequences)
+
+
+def offer_finished(fin: List[Tuple[float, int, int]], cap: int, score: float, n: int, src: int) -> None:
+    """Rule 6 on one finished set ``fin`` (best first) of at most ``cap`` hypotheses: ``(score, n, src)`` goes in
+    after every entry with a score >= its own, unless the set is full and it does not beat the worst."""
+    if len(fin) == cap and not score > fin[-1][0]:
+        return
+    p = len(fin)
+    while p > 0 and fin[p - 1][0] < score:
+        p -= 1
+    fin.insert(p, (score, n, src))
+    del fin[cap:]
+
+
+def merge_finished_sets(sets: Sequence[Sequence[Tuple[float, int, int]]]) -> List[Tuple[float, int, int]]:
+    """Rule G6: one item's finished hypotheses from its groups' sets (each best first, in group order) as one
+    best-first list; a tie goes to the lower group, then to the group's own order. One set is returned as it is."""
+    return sorted((h for fin in sets for h in fin), key=lambda h: -h[0])
+
+
+class GroupBeamReference(BeamReference):
+    """Diverse (group) beam search (rules G1-G6, see the module docstring) for ``batch`` items in fp64, with the
+    interface of ``BeamReference``. ``fin[b][g]`` is group g's finished set, ``group_done`` [B, G] the groups' done
+    flags (rule 7 per group) and ``result`` merges the sets (``merge_finished_sets``). ``early_stop=False`` keeps a
+    done group selecting, its beams still counting for nothing in the Hamming counts: the results must not change."""
+
+    def __init__(self, batch: int, num_beams: int, max_new: int, vocab: int, length_penalty: float = 1.0,
+                 stop_ids: Sequence[int] = (), suppress_ids: Sequence[int] = (), min_new: int = 0,
+                 early_stop: bool = True, num_beam_groups: int = 1, diversity_penalty: float = 0.0):
+        super().__init__(batch, num_beams, max_new, vocab, length_penalty, stop_ids, suppress_ids, min_new,
+                         early_stop)
+        G, lam = int(num_beam_groups), float(diversity_penalty)
+        if not 1 <= G <= self.K or self.K % G != 0 or not (np.isfinite(lam) and lam >= 0):
+            raise ValueError(f"GroupBeamReference: need num_beam_groups dividing num_beams = {self.K} and a finite "
+                             f"diversity_penalty >= 0, got {num_beam_groups}, {diversity_penalty}")
+        self.G, self.Kg, self.lam = G, self.K // G, float(np.float32(lam))
+        self.scores[:, ::self.Kg] = 0.0
+        self.fin = [[[] for _ in range(G)] for _ in range(self.B)]
+        self.group_done = np.zeros((self.B, G), dtype=bool)
+        self.stopped = np.zeros((self.B, G), dtype=bool)   # the group selects no more (group_done with early_stop)
+
+    def group_ranking(self, b: int, g: int, logits: np.ndarray, step: int,
+                      taken: Sequence[int]) -> List[Tuple[float, int, int]]:
+        """Group g of item b's candidates ``(c, j, i)`` in rank order (rule G2), ``taken``: the tokens of this step's
+        counted new beams of the earlier groups."""
+        V = self.vocab
+        rows = []
+        for j in range(g * self.Kg, (g + 1) * self.Kg):
+            for c, i in self.row_best(b, j, logits, step):
+                n = sum(t == i for t in taken)
+                rows.append((c - self.lam * n if n else c, j * V + i))
+        rows.sort(key=lambda t: (-t[0], t[1]))
+        return [(c, f // V, f % V) for c, f in rows]
+
+    def step(self, logits) -> Tuple[torch.Tensor, torch.Tensor]:
+        """One step (rules G1-G5) for every item that is not done."""
+        if isinstance(logits, torch.Tensor):
+            logits = logits.detach().float().cpu().numpy()
+        B, K, Kg = self.B, self.K, self.Kg
+        step = self.n_steps
+        if step >= self.max_new:
+            raise ValueError(f"GroupBeamReference: all {self.max_new} steps taken")
+        nxt = np.zeros(B * K, dtype=np.int64)
+        parent = np.arange(B * K, dtype=np.int64)
+        L, last = step + 1, step == self.max_new - 1
+        for b in range(B):
+            if self.done[b]:
+                continue
+            taken: List[int] = []
+            for g in range(self.G):
+                if self.stopped[b, g]:
+                    continue
+                j0, fin, counted = g * Kg, self.fin[b][g], not self.group_done[b, g]
+                beams = []
+                for c, j, i in self.group_ranking(b, g, logits, step, taken):
+                    if len(beams) == Kg:
+                        break
+                    if i in self.stop:
+                        offer_finished(fin, Kg, c / self.penalty(L), L - 1, j)
+                    else:
+                        beams.append((c, j, i))
+                new = np.full(Kg, -np.inf)
+                for k in range(Kg):
+                    if k < len(beams):
+                        c, j, i = beams[k]
+                        new[k], nxt[b * K + j0 + k], parent[b * K + j0 + k] = c, i, b * K + j
+                        self.hist_tok[step, b, j0 + k], self.hist_back[step, b, j0 + k] = i, j
+                    else:
+                        self.hist_tok[step, b, j0 + k], self.hist_back[step, b, j0 + k] = -1, j0 + k
+                if last:
+                    for k in range(len(beams)):
+                        offer_finished(fin, Kg, new[k] / self.penalty(self.max_new), self.max_new, j0 + k)
+                    self.group_done[b, g] = self.stopped[b, g] = True
+                elif not beams:
+                    self.group_done[b, g] = self.stopped[b, g] = True
+                elif len(fin) == Kg:
+                    reach = new[0] / self.penalty(self.max_new if self.alpha > 0 else L + 1)
+                    self.group_done[b, g] |= not reach > fin[-1][0]
+                    self.stopped[b, g] |= self.early_stop and self.group_done[b, g]
+                if counted:                                      # this step's new beams count, even if now done
+                    taken.extend(i for _, _, i in beams)
+                self.scores[b, j0:j0 + Kg] = -np.inf if self.stopped[b, g] else new
+            self.done[b] = bool(self.stopped[b].all())
+        self.n_steps += 1
+        return torch.from_numpy(nxt), torch.from_numpy(parent)
+
+    def result(self, num_return_sequences: int = 1) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """``BeamReference.result`` of the merged finished sets (rule G6)."""
+        return best_hypotheses([merge_finished_sets(f) for f in self.fin], self.hist_tok, self.hist_back,
+                               self.max_new, num_return_sequences)
 
 
 _MASK = np.uint64(0xFFFFFFFF)

@@ -41,6 +41,11 @@ def main():
     p.add_argument("--beam_sample", action="store_true",
                    help="f1 with --num_beams: beam sampling, the beams' candidates drawn with --temperature, --top_k "
                         "and --top_p instead of ranked")
+    p.add_argument("--num_beam_groups", type=int, default=1,
+                   help="f1 with --num_beams: diverse beam search with this many groups of beams (1: off); needs "
+                        "--diversity_penalty > 0")
+    p.add_argument("--diversity_penalty", type=float, default=0.0,
+                   help="f1 with --num_beam_groups > 1: score lowered per earlier group's beam with the same token")
     p.add_argument("--repetition_penalty", type=float, default=1.0,
                    help="f1: penalty on ids already in the prompt or reply (1: off); replies go through the batched path")
     p.add_argument("--no_repeat_ngram_size", type=int, default=0,
@@ -83,7 +88,8 @@ def main():
                   no_sample=a.no_sample, repetition_penalty=a.repetition_penalty,
                   no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha,
                   prompt_lookup_num_tokens=a.prompt_lookup_num_tokens, min_p=a.min_p, typical_p=a.typical_p,
-                  epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, beam_sample=a.beam_sample)
+                  epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, beam_sample=a.beam_sample,
+                  num_beam_groups=a.num_beam_groups, diversity_penalty=a.diversity_penalty)
         if a.assistant_checkpoint:
             kw["assistant_model"] = load_model_from_checkpoint(
                 a.assistant_checkpoint, a.device, torch.bfloat16 if a.device.startswith("cuda") else None)[0]

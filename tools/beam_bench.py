@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """GPT-2 small beam search: ``GPT2DoubleHeads.beam_search`` against greedy ``generate`` at the same number of rows,
-beam sampling against beam search, and the selection and cache-reordering kernels on their own.
+beam sampling against beam search, diverse beam search by group count, and the selection and cache-reordering
+kernels on their own.
 
 Prints one JSON line with the device name and power limit read in the same run. Needs a CUDA device (there is no CPU
 fallback) and writes nothing into the repository.
@@ -17,6 +18,10 @@ fallback) and writes nothing into the repository.
   with top-p 1 and 0.9.
 * ``sampled``: ``beam_search(do_sample=True, top_k=50)`` against ``do_sample=False``, ms per generated token as in
   ``search``, the two alternated run by run in this process (medians of ``--reps`` pairs after one warm-up each).
+* ``groups``: diverse beam search, ``beam_search(num_beam_groups=G, diversity_penalty=0.5)`` for B = 8 items, K = 8
+  beams, G = 1 / 2 / 4 / 8 and 128-token prompts, ms per generated token as in ``search`` (no stop ids, so every call
+  runs all 64 tokens), the four alternated run by run; and ``beam_step_`` alone at 64 rows (vocab 50257) with G = 1
+  against G = 8, timed as in ``kernels``.
 
 Usage: ``python tools/beam_bench.py [--reps 3] [--launches 1000]``
 """
@@ -101,6 +106,41 @@ def bench_sampled(model, reps):
     return rows
 
 
+def bench_groups(model, reps, launches):
+    from adapcc_b200.ops import BeamState, beam_step_
+
+    B, K, lam = 8, 8, 0.5
+    g = torch.Generator(device="cuda").manual_seed(5)
+    prompt = torch.randint(0, model.cfg.vocab_size, (B, 128), device="cuda", generator=g)
+    groups = (1, 2, 4, 8)
+
+    def run(G):
+        return model.beam_search(prompt, num_beams=K, max_new_tokens=NEW_TOKENS, num_beam_groups=G,
+                                 diversity_penalty=lam if G > 1 else 0.0)
+
+    times = {G: [] for G in groups}
+    for G in groups:
+        run(G)                                                     # warm-up of this shape
+    for _ in range(reps):
+        for G in groups:
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            run(G)
+            torch.cuda.synchronize()
+            times[G].append((time.perf_counter() - t0) * 1e3)
+    out = {"batch": B, "beams": K, "prompt": 128, "diversity_penalty": lam,
+           "ms_per_token": {str(G): round(statistics.median(times[G]) / NEW_TOKENS, 3) for G in groups}}
+    logits = torch.randn(B * K, model.wte.weight.shape[0], device="cuda", generator=g) * 3
+    max_new = launches + 4 * GRAPH_LAUNCHES
+    for G in (1, 8):
+        st = BeamState(B, K, max_new, 1.0, "cuda", groups=G)
+        st.scores.zero_()
+        kw = dict(diversity_penalty=lam) if G > 1 else {}
+        out[f"beam_step_G{G}_us"] = round(_graph_us(lambda: beam_step_(logits, model.cfg.vocab_size, st, **kw),
+                                                    launches), 2)
+    return out
+
+
 def _graph_us(fn, launches):
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -178,7 +218,8 @@ def main():
     torch.manual_seed(0)
     model = GPT2DoubleHeads(GPT2Config()).to(device="cuda", dtype=torch.bfloat16).eval()
     result = dict(info, new_tokens=NEW_TOKENS, kernels=bench_kernels(model, args.launches),
-                  search=bench_search(model, args.reps), sampled=bench_sampled(model, args.reps))
+                  search=bench_search(model, args.reps), sampled=bench_sampled(model, args.reps),
+                  groups=bench_groups(model, args.reps, args.launches))
     print(json.dumps(result))
 
 
