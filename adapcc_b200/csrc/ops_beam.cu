@@ -6,12 +6,11 @@
 //                 c_i = s + ((l_i - m) - logf(Z)) as a 64-bit key (order-preserving float bits, then the inverted id, so
 //                 a tie goes to the lower id), of which the row's N = K + n_stop best are kept (topk_rows.cuh, shared
 //                 with contrastive search).
-//   beam_select : one warp per item. The K rows' N best, re-keyed by the flat index j * V + i, are walked in rank order
-//                 (rounds of a warp maximum): the first K non-stop candidates become the new beams, stop candidates
-//                 ranked before the K-th are offered to the finished set, and the done rule is applied (DESIGN.md §4a).
-//   beam_group_select : diverse (group) beam search's beam_select, one warp per item: the groups in order, each one's
-//                 candidates re-keyed with the Hamming penalty of the earlier groups' new tokens, then walked as in
-//                 beam_select with the group's own finished set and done flag (DESIGN.md §4a).
+//   beam_select : one warp per item, its G groups of Kg = K / G beams in order (G = 1: plain beam search). A group's
+//                 Kg rows' N best, re-keyed by the flat index j * V + i and by the Hamming penalty of the earlier
+//                 groups' new tokens, are walked in rank order (rounds of a warp maximum): the first Kg non-stop
+//                 candidates become the group's new beams, stop candidates ranked before the Kg-th are offered to the
+//                 group's finished set, and the done rule is applied per group (DESIGN.md §4a).
 //   kv_reorder  : cache[l, r, :, pos] = cache[l, parent[r], :, pos] for the generated positions, through a scratch
 //                 buffer (gather, then scatter), so cycles and many-to-one parent maps come out right.
 //
@@ -66,10 +65,13 @@ struct BeamArgs {
   int* parent;                 // [B * K]: row the new beam continues (absolute row index)
   long long* hist_tok;         // [max_new, B * K]: token of beam k at each step
   int* hist_back;              // [max_new, B * K]: its parent beam (0..K-1) at the previous step
-  float* fin_score;            // [B, K] finished set, best first: normalised score
-  int* fin_n;                  // [B, K] tokens of the hypothesis (the stop token excluded)
-  int* fin_src;                // [B, K] beam whose history at step fin_n - 1 holds those tokens
-  int* fin_count;              // [B]
+  float* fin_score;            // [B, G, Kg] finished sets, best first: normalised score
+  int* fin_n;                  // [B, G, Kg] tokens of the hypothesis (the stop token excluded)
+  int* fin_src;                // [B, G, Kg] beam whose history at step fin_n - 1 holds those tokens
+  int* fin_count;              // [B * G]
+  int G;                       // groups; group g owns the item's beams g * Kg .. (g + 1) * Kg - 1, Kg = K / G
+  int* group_done;             // [B * G] (beam_select only)
+  float lambda;                // diversity penalty (beam_select only)
 };
 
 __global__ void __launch_bounds__(kBeamThreads, 1) beam_rows_kernel(const __grid_constant__ BeamArgs a) {
@@ -117,6 +119,28 @@ struct FinishedSet {
   float score[kBeamMaxK];
   int n[kBeamMaxK], src[kBeamMaxK];
   int count, K;
+  // the set of K = cap entries at fin_*[base ..] with its count at fin_count[ci]: thread t < cap loads entry t,
+  // thread 0 the count as well
+  __device__ void load(const BeamArgs& a, int base, int ci, int cap, int t) {
+    if (t < cap) {
+      score[t] = a.fin_score[base + t];
+      n[t] = a.fin_n[base + t];
+      src[t] = a.fin_src[base + t];
+    }
+    if (t == 0) {
+      K = cap;
+      count = a.fin_count[ci];
+    }
+  }
+  // thread t < K stores entry t, thread 0 the count as well
+  __device__ void store(const BeamArgs& a, int base, int ci, int t) const {
+    if (t < K) {
+      a.fin_score[base + t] = score[t];
+      a.fin_n[base + t] = n[t];
+      a.fin_src[base + t] = src[t];
+    }
+    if (t == 0) a.fin_count[ci] = count;
+  }
   // keeps the K best by score; on a tie the earlier entry stays ahead
   __device__ void offer(float sh, int nn, int sc) {
     if (count == K && !(sh > score[K - 1])) return;
@@ -131,127 +155,27 @@ struct FinishedSet {
     src[p] = sc;
     if (count < K) ++count;
   }
-};
-
-__global__ void __launch_bounds__(32) beam_select_kernel(const __grid_constant__ BeamArgs a) {
-  __shared__ unsigned long long s_c[kBeamMaxK * kBeamMaxN];
-  __shared__ FinishedSet fs;
-  __shared__ int s_tok[kBeamMaxK], s_par[kBeamMaxK];
-  __shared__ float s_sc[kBeamMaxK];
-  const int b = blockIdx.x, lane = threadIdx.x, K = a.K, N = a.N, V = a.vocab, BK = a.B * a.K;
-  const int step = *a.step;
-  if (a.done[b] || step >= a.max_new) {               // nothing moves: every row keeps its own cache
-    if (lane < K) a.parent[b * K + lane] = b * K + lane;
-    return;
+  // the done rule after a step that is not the last, for the best live sum s of L = step + 1 tokens: the set is full
+  // and s cannot reach its worst entry. A live sum can only fall, so its best reachable normalised score is
+  // s / L_max^a (a > 0) or s / (L + 1)^a.
+  __device__ bool done_rule(const BeamArgs& a, float s, int L) const {
+    return count == K && !(s / a.pen[a.alpha_pos ? a.max_new : L + 1] > score[K - 1]);
   }
-  for (int e = lane; e < K * N; e += 32) {
-    const int j = e / N;
-    const unsigned long long v = a.cand[(long long)(b * K + j) * N + (e - j * N)];
-    const uint32_t flat = (uint32_t)j * (uint32_t)V + (0xFFFFFFFFu - (uint32_t)v);
-    s_c[e] = v ? (v & 0xFFFFFFFF00000000ull) | (0xFFFFFFFFu - flat) : 0ull;
-  }
-  if (lane == 0) {
-    fs.K = K;
-    fs.count = a.fin_count[b];
-    for (int k = 0; k < K; ++k) {
-      fs.score[k] = a.fin_score[b * K + k];
-      fs.n[k] = a.fin_n[b * K + k];
-      fs.src[k] = a.fin_src[b * K + k];
-    }
-  }
-  __syncwarp();
-  // the walk: candidates in rank order until K non-stop ones are taken
-  const int L = step + 1;                             // tokens of a hypothesis that ends at this step
-  int nb = 0;
-  unsigned long long bound = ~0ull;
-  while (nb < K) {
-    unsigned long long best = 0ull;
-    for (int e = lane; e < K * N; e += 32) {
-      const unsigned long long v = s_c[e];
-      if (v < bound && v > best) best = v;
-    }
-    best = warp_max_u64(best);
-    if (best == 0ull) break;
-    bound = best;
-    const uint32_t flat = 0xFFFFFFFFu - (uint32_t)best;
-    const int j = (int)(flat / (uint32_t)V), i = (int)(flat - (uint32_t)j * (uint32_t)V);
-    const float c = beam_key2f((uint32_t)(best >> 32));
-    bool is_stop = false;
-    for (int q = 0; q < a.n_stop; ++q) is_stop |= a.stop[q] == i;
-    if (lane == 0) {
-      if (is_stop) {
-        fs.offer(c / a.pen[L], L - 1, j);
-      } else {
-        s_tok[nb] = i;
-        s_par[nb] = j;
-        s_sc[nb] = c;
-      }
-    }
-    nb += !is_stop;
-  }
-  __syncwarp();
-  if (lane < K) {
-    const int r = b * K + lane;
-    const long long h = (long long)step * BK + r;
-    if (lane < nb) {
-      a.next_ids[r] = s_tok[lane];
-      a.parent[r] = b * K + s_par[lane];
-      a.scores[r] = s_sc[lane];
-      a.hist_tok[h] = s_tok[lane];
-      a.hist_back[h] = s_par[lane];
-    } else {                                          // fewer than K finite non-stop candidates: a dead beam
-      a.next_ids[r] = 0;
-      a.parent[r] = r;
-      a.scores[r] = -INFINITY;
-      a.hist_tok[h] = -1;
-      a.hist_back[h] = lane;
-    }
-  }
-  if (lane == 0) {
-    int done = 0;
-    if (step == a.max_new - 1) {                      // the last step: the live beams are offered in beam order
-      for (int k = 0; k < nb; ++k) fs.offer(s_sc[k] / a.pen[a.max_new], a.max_new, k);
-      done = 1;
-    } else if (nb == 0) {
-      done = 1;
-    } else if (fs.count == K) {
-      // a live sum can only fall: its best reachable normalised score is s / L_max^a (a > 0) or s / (L + 1)^a
-      const float reach = s_sc[0] / a.pen[a.alpha_pos ? a.max_new : L + 1];
-      done = !(reach > fs.score[K - 1]);
-    }
-    a.done[b] = done;
-    a.fin_count[b] = fs.count;
-  }
-  __syncwarp();
-  if (lane < K) {
-    a.fin_score[b * K + lane] = fs.score[lane];
-    a.fin_n[b * K + lane] = fs.n[lane];
-    a.fin_src[b * K + lane] = fs.src[lane];
-  }
-}
-
-__global__ void beam_step_incr_kernel(int* step) { *step += 1; }
-
-// ---- diverse (group) beam search ----------------------------------------------------------------------------------
-struct BeamGroupArgs {
-  BeamArgs a;                  // a.fin_* [B, K] read as [B, G, Kg]; a.fin_count [B * G]; a.done [B] the item flags
-  int G;                       // groups; group g owns the item's beams g * Kg .. (g + 1) * Kg - 1, Kg = K / G
-  int* group_done;             // [B * G]
-  float lambda;                // diversity penalty
 };
 
 // One warp per item; the groups in order g = 0 .. G-1. A candidate whose token the earlier groups' new beams of this
-// step took n > 0 times is re-keyed with c' = fl32(c - fl32(lambda * n)); n = 0 keeps c's key, so group 0 is beam_select
-// with K = Kg. The walk, the offers (to the group's own finished set of Kg) and the done rule are beam_select's, per
-// group. The rows' N = K + n_stop unpenalised best suffice: at most K - Kg tokens are penalised (DESIGN.md §4a).
-__global__ void __launch_bounds__(32) beam_group_select_kernel(const __grid_constant__ BeamGroupArgs p) {
+// step took n > 0 times is re-keyed with c' = fl32(c - fl32(lambda * n)); n = 0 keeps c's key, so group 0 selects as
+// plain beam search with K = Kg. The rows' N = K + n_stop unpenalised best suffice: at most K - Kg tokens are
+// penalised (DESIGN.md §4a).
+__global__ void __launch_bounds__(32) beam_select_kernel(const __grid_constant__ BeamArgs a) {
   __shared__ unsigned long long s_c[kBeamMaxK * kBeamMaxN];
   __shared__ FinishedSet fs;
   __shared__ int s_tok[kBeamMaxK], s_par[kBeamMaxK], s_taken[kBeamMaxK];
   __shared__ float s_sc[kBeamMaxK];
-  const BeamArgs& a = p.a;
-  const int b = blockIdx.x, lane = threadIdx.x, K = a.K, N = a.N, V = a.vocab, BK = a.B * a.K, G = p.G, Kg = K / G;
+  const int b = blockIdx.x, lane = threadIdx.x, K = a.K, N = a.N, V = a.vocab, BK = a.B * a.K, G = a.G, Kg = K / G;
   const int step = *a.step;
+  // the done groups, one bit each, read next to the item's flag so that the loads overlap
+  const unsigned g_done = __ballot_sync(0xffffffffu, lane < G && a.group_done[b * G + lane]);
   if (a.done[b] || step >= a.max_new) {               // nothing moves: every row keeps its own cache
     if (lane < K) a.parent[b * K + lane] = b * K + lane;
     return;
@@ -260,7 +184,7 @@ __global__ void __launch_bounds__(32) beam_group_select_kernel(const __grid_cons
   int n_taken = 0, all_done = 1;
   for (int g = 0; g < G; ++g) {
     const int j0 = g * Kg, fo = b * K + j0, gi = b * G + g;
-    if (p.group_done[gi]) {                           // a done group: dead rows that keep their own cache
+    if (g_done >> g & 1u) {                           // a done group: dead rows that keep their own cache
       if (lane < Kg) a.parent[fo + lane] = fo + lane;
       continue;
     }
@@ -272,21 +196,14 @@ __global__ void __launch_bounds__(32) beam_group_select_kernel(const __grid_cons
       int n = 0;
       for (int t = 0; t < n_taken; ++t) n += s_taken[t] == (int)i;
       if (v && n) {
-        const float cp = __fsub_rn(beam_key2f(hi), __fmul_rn(p.lambda, (float)n));
+        const float cp = __fsub_rn(beam_key2f(hi), __fmul_rn(a.lambda, (float)n));
         hi = cp > -INFINITY ? beam_f2key(cp) : 0u;
       }
       s_c[e] = v && hi ? ((unsigned long long)hi << 32) | (0xFFFFFFFFu - flat) : 0ull;
     }
-    if (lane == 0) {
-      fs.K = Kg;
-      fs.count = a.fin_count[gi];
-      for (int k = 0; k < Kg; ++k) {
-        fs.score[k] = a.fin_score[fo + k];
-        fs.n[k] = a.fin_n[fo + k];
-        fs.src[k] = a.fin_src[fo + k];
-      }
-    }
+    fs.load(a, fo, gi, Kg, lane);
     __syncwarp();
+    // the walk: candidates in rank order until Kg non-stop ones are taken
     int nb = 0;
     unsigned long long bound = ~0ull;
     while (nb < Kg) {
@@ -310,54 +227,50 @@ __global__ void __launch_bounds__(32) beam_group_select_kernel(const __grid_cons
           s_tok[nb] = i;
           s_par[nb] = j;
           s_sc[nb] = c;
+          s_taken[n_taken + nb] = i;
         }
       }
       nb += !is_stop;
     }
     __syncwarp();
-    int done = 0;
+    int done = 1;
     if (lane == 0) {
-      if (step == a.max_new - 1) {
+      if (step == a.max_new - 1) {                    // the last step: the live beams are offered in beam order
         for (int k = 0; k < nb; ++k) fs.offer(s_sc[k] / a.pen[a.max_new], a.max_new, j0 + k);
-        done = 1;
-      } else if (nb == 0) {
-        done = 1;
-      } else if (fs.count == Kg) {
-        const float reach = s_sc[0] / a.pen[a.alpha_pos ? a.max_new : L + 1];
-        done = !(reach > fs.score[Kg - 1]);
+      } else {
+        done = nb == 0 || fs.done_rule(a, s_sc[0], L);
       }
-      p.group_done[gi] = done;
-      a.fin_count[gi] = fs.count;
-      for (int k = 0; k < nb; ++k) s_taken[n_taken + k] = s_tok[k];
+      if (G > 1) a.group_done[gi] = done;             // one group: a.done[b] is its flag
     }
     done = __shfl_sync(0xffffffffu, done, 0);
     all_done &= done;
     n_taken += nb;                                    // this step's new beams count, even if the group is now done
     __syncwarp();
+    fs.store(a, fo, gi, lane);
     if (lane < Kg) {
       const int r = fo + lane;
       const long long h = (long long)step * BK + r;
       if (lane < nb) {
         a.next_ids[r] = s_tok[lane];
         a.parent[r] = b * K + s_par[lane];
-        a.scores[r] = done ? -INFINITY : s_sc[lane];  // a done group's beams are dead from now on
+        // a done group's beams are dead from now on; with one group the item's done flag stops beam_rows_kernel
+        a.scores[r] = done && G > 1 ? -INFINITY : s_sc[lane];
         a.hist_tok[h] = s_tok[lane];
         a.hist_back[h] = s_par[lane];
-      } else {
+      } else {                                        // fewer than Kg finite non-stop candidates: a dead beam
         a.next_ids[r] = 0;
         a.parent[r] = r;
         a.scores[r] = -INFINITY;
         a.hist_tok[h] = -1;
         a.hist_back[h] = j0 + lane;
       }
-      a.fin_score[r] = fs.score[lane];
-      a.fin_n[r] = fs.n[lane];
-      a.fin_src[r] = fs.src[lane];
     }
     __syncwarp();
   }
   if (lane == 0) a.done[b] = all_done;
 }
+
+__global__ void beam_step_incr_kernel(int* step) { *step += 1; }
 
 // ---- beam sampling ---------------------------------------------------------------------------------------------------
 struct BeamSampleArgs {
@@ -542,15 +455,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_sample_select_kernel(const 
   }
   for (int d = tid; d < M; d += kBeamThreads) s_draw[d] = -1;
   if (tid < K) s_beam[tid] = -1;
-  if (tid == 0) {
-    fs.K = K;
-    fs.count = a.fin_count[b];
-    for (int k = 0; k < K; ++k) {
-      fs.score[k] = a.fin_score[b * K + k];
-      fs.n[k] = a.fin_n[b * K + k];
-      fs.src[k] = a.fin_src[b * K + k];
-    }
-  }
+  fs.load(a, b * K, b, K, tid);
   __syncthreads();
   // the draw order: a key's place in its (sorted) row plus the number of larger keys in each other row
   for (int e = tid; e < K * M; e += kBeamThreads) {
@@ -628,24 +533,8 @@ __global__ void __launch_bounds__(kBeamThreads) beam_sample_select_kernel(const 
     }
   }
   __syncthreads();
-  if (tid == 0) {
-    int done = 0;
-    if (last || s_beam[0] < 0) {
-      done = 1;
-    } else if (fs.count == K) {
-      // as in beam_select: a live sum can only fall, so the best reachable normalised score bounds every later offer
-      const float reach = s_c[s_draw[s_beam[0]]] / a.pen[a.alpha_pos ? a.max_new : L + 1];
-      done = !(reach > fs.score[K - 1]);
-    }
-    a.done[b] = done;
-    a.fin_count[b] = fs.count;
-  }
-  __syncthreads();
-  if (tid < K) {
-    a.fin_score[b * K + tid] = fs.score[tid];
-    a.fin_n[b * K + tid] = fs.n[tid];
-    a.fin_src[b * K + tid] = fs.src[tid];
-  }
+  if (tid == 0) a.done[b] = last || s_beam[0] < 0 || fs.done_rule(a, s_c[s_draw[s_beam[0]]], L);
+  fs.store(a, b * K, b, tid);
 }
 
 // ---- KV-cache reordering -----------------------------------------------------------------------------------------
@@ -687,6 +576,27 @@ __global__ void __launch_bounds__(kReorderThreads) kv_reorder_kernel(const __gri
   }
 }
 
+// the checks both step entry points make; each then checks its own mode's arguments and sets a.N from n_stop
+static int check_beam_args(const char* who, const BeamArgs& a) {
+  if (a.B < 1 || a.K < 1 || a.K > kBeamMaxK || a.vocab < 1 || a.ld < a.vocab || a.max_new < 1) {
+    set_error("%s: need B >= 1, 1 <= K <= %d, vocab >= 1, ld >= vocab, max_new >= 1 (B=%d K=%d vocab=%d ld=%d "
+              "max_new=%d)", who, kBeamMaxK, a.B, a.K, a.vocab, a.ld, a.max_new);
+    return -1;
+  }
+  if (a.n_suppress < 0 || a.n_suppress > kBeamMaxSuppress || a.n_stop < 0 || a.n_stop > kBeamMaxStop ||
+      (a.n_suppress && !a.suppress) || (a.n_stop && !a.stop)) {
+    set_error("%s: at most %d suppressed and %d stop ids (got %d, %d)", who, kBeamMaxSuppress, kBeamMaxStop,
+              a.n_suppress, a.n_stop);
+    return -1;
+  }
+  if (!a.logits || !a.scores || !a.step || !a.pen || !a.done || !a.cand || !a.next_ids || !a.parent || !a.hist_tok ||
+      !a.hist_back || !a.fin_score || !a.fin_n || !a.fin_src || !a.fin_count) {
+    set_error("%s: null pointer", who);
+    return -1;
+  }
+  return 0;
+}
+
 }  // namespace adapcc
 
 using namespace adapcc;
@@ -694,30 +604,26 @@ using namespace adapcc;
 extern "C" {
 
 // logits fp32 [B*K, ld]; scores fp32 [B*K]; step int32 [1]; suppress / stop int32 lists (may be null when empty);
-// pen fp32 [max_new + 1]; done int32 [B]; cand uint64 [B*K, K + n_stop]; next_ids int64 [B*K]; parent int32 [B*K];
-// hist_tok int64 [max_new, B*K]; hist_back int32 [max_new, B*K]; fin_score fp32 / fin_n, fin_src int32 [B, K];
-// fin_count int32 [B]
-int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, float* scores, int* step, int min_new,
+// pen fp32 [max_new + 1]; done int32 [B]; group_done int32 [B*G] with the groups G dividing K (1: plain beam search);
+// cand uint64 [B*K, K + n_stop]; next_ids int64 [B*K]; parent int32 [B*K]; hist_tok int64 / hist_back int32
+// [max_new, B*K]; fin_score fp32 / fin_n, fin_src int32 [B, K]; fin_count int32 [B*G]; the diversity penalty lambda
+// finite and >= 0
+int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, int G, float* scores, int* step, int min_new,
                      const int* suppress, int n_suppress, const int* stop, int n_stop, const float* pen, int alpha_pos,
-                     int max_new, int* done, void* cand, long long* next_ids, int* parent, long long* hist_tok,
-                     int* hist_back, float* fin_score, int* fin_n, int* fin_src, int* fin_count, void* stream) {
-  if (B < 1 || K < 1 || K > kBeamMaxK || vocab < 1 || ld < vocab || max_new < 1 ||
-      (unsigned long long)K * (unsigned long long)vocab > 0xFFFFFFFFull) {
-    set_error("beam_step: need B >= 1, 1 <= K <= %d, vocab >= 1, ld >= vocab, K * vocab < 2^32, max_new >= 1 (B=%d "
-              "K=%d vocab=%d ld=%d max_new=%d)", kBeamMaxK, B, K, vocab, ld, max_new);
+                     int max_new, int* done, int* group_done, void* cand, long long* next_ids, int* parent,
+                     long long* hist_tok, int* hist_back, float* fin_score, int* fin_n, int* fin_src, int* fin_count,
+                     float lambda, void* stream) {
+  BeamArgs a{logits, ld, vocab, B, K, 0, scores, step, min_new, suppress, n_suppress, stop, n_stop, pen, alpha_pos,
+             max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok, hist_back, fin_score, fin_n,
+             fin_src, fin_count, G, group_done, lambda};
+  if (check_beam_args("beam_step", a)) return -1;
+  if (G < 1 || K % G != 0 || (unsigned long long)K * (unsigned long long)vocab > 0xFFFFFFFFull || !group_done ||
+      !(lambda >= 0.f && lambda < INFINITY)) {
+    set_error("beam_step: need G >= 1 dividing K, K * vocab < 2^32, a finite diversity penalty >= 0 and group_done "
+              "(K=%d G=%d vocab=%d lambda=%g)", K, G, vocab, lambda);
     return -1;
   }
-  if (n_suppress < 0 || n_suppress > kBeamMaxSuppress || n_stop < 0 || n_stop > kBeamMaxStop ||
-      (n_suppress && !suppress) || (n_stop && !stop)) {
-    set_error("beam_step: at most %d suppressed and %d stop ids (got %d, %d)", kBeamMaxSuppress, kBeamMaxStop,
-              n_suppress, n_stop);
-    return -1;
-  }
-  if (!logits || !scores || !step || !pen || !done || !cand || !next_ids || !parent || !hist_tok || !hist_back ||
-      !fin_score || !fin_n || !fin_src || !fin_count) {
-    set_error("beam_step: null pointer");
-    return -1;
-  }
+  a.N = K + n_stop;
   const size_t bits = n_suppress > 0 && min_new > 0 ? (size_t)(vocab + 31) / 32 * sizeof(uint32_t) : 0;
   if (bits > 200 * 1024) {
     set_error("beam_step: suppression needs vocab <= %d (got %d)", 200 * 1024 * 8, vocab);
@@ -725,9 +631,6 @@ int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, float
   }
   if (bits > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(beam_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                                       (int)bits));
-  BeamArgs a{logits, ld, vocab, B, K, K + n_stop, scores, step, min_new, suppress, n_suppress, stop, n_stop, pen,
-             alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok, hist_back, fin_score,
-             fin_n, fin_src, fin_count};
   cudaStream_t s = (cudaStream_t)stream;
   beam_rows_kernel<<<B * K, kBeamThreads, bits, s>>>(a);
   CUDA_TRY(cudaGetLastError());
@@ -741,95 +644,34 @@ int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, float
   return 0;
 }
 
-// adapcc_beam_step's arguments with the groups G (K % G == 0), group_done int32 [B*G], fin_count int32 [B*G] and the
-// diversity penalty lambda (finite, >= 0)
-int adapcc_beam_group_step(const float* logits, int ld, int vocab, int B, int K, int G, float* scores, int* step,
-                           int min_new, const int* suppress, int n_suppress, const int* stop, int n_stop,
-                           const float* pen, int alpha_pos, int max_new, int* done, int* group_done, void* cand,
-                           long long* next_ids, int* parent, long long* hist_tok, int* hist_back, float* fin_score,
-                           int* fin_n, int* fin_src, int* fin_count, float lambda, void* stream) {
-  if (B < 1 || K < 1 || K > kBeamMaxK || G < 1 || K % G != 0 || vocab < 1 || ld < vocab || max_new < 1 ||
-      (unsigned long long)K * (unsigned long long)vocab > 0xFFFFFFFFull) {
-    set_error("beam_group_step: need B >= 1, 1 <= K <= %d, G >= 1 dividing K, vocab >= 1, ld >= vocab, K * vocab < "
-              "2^32, max_new >= 1 (B=%d K=%d G=%d vocab=%d ld=%d max_new=%d)", kBeamMaxK, B, K, G, vocab, ld, max_new);
-    return -1;
-  }
-  if (n_suppress < 0 || n_suppress > kBeamMaxSuppress || n_stop < 0 || n_stop > kBeamMaxStop ||
-      (n_suppress && !suppress) || (n_stop && !stop)) {
-    set_error("beam_group_step: at most %d suppressed and %d stop ids (got %d, %d)", kBeamMaxSuppress, kBeamMaxStop,
-              n_suppress, n_stop);
-    return -1;
-  }
-  if (!(lambda >= 0.f && lambda < INFINITY)) {
-    set_error("beam_group_step: the diversity penalty must be finite and >= 0 (got %g)", lambda);
-    return -1;
-  }
-  if (!logits || !scores || !step || !pen || !done || !group_done || !cand || !next_ids || !parent || !hist_tok ||
-      !hist_back || !fin_score || !fin_n || !fin_src || !fin_count) {
-    set_error("beam_group_step: null pointer");
-    return -1;
-  }
-  const size_t bits = n_suppress > 0 && min_new > 0 ? (size_t)(vocab + 31) / 32 * sizeof(uint32_t) : 0;
-  if (bits > 200 * 1024) {
-    set_error("beam_group_step: suppression needs vocab <= %d (got %d)", 200 * 1024 * 8, vocab);
-    return -1;
-  }
-  if (bits > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(beam_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                      (int)bits));
-  BeamGroupArgs p{BeamArgs{logits, ld, vocab, B, K, K + n_stop, scores, step, min_new, suppress, n_suppress, stop,
-                           n_stop, pen, alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
-                           hist_back, fin_score, fin_n, fin_src, fin_count},
-                  G, group_done, lambda};
-  cudaStream_t s = (cudaStream_t)stream;
-  beam_rows_kernel<<<B * K, kBeamThreads, bits, s>>>(p.a);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_group_select_kernel<<<B, 32, 0, s>>>(p);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_step_incr_kernel<<<1, 1, 0, s>>>(step);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  return 0;
-}
-
-// adapcc_beam_step's arguments, plus cand_c fp32 [B*K, M] next to cand uint64 [B*K, M] (M = max(2, 1 + n_stop) * K),
-// the sampling scalars (temperature > 0, top_k >= 0 with 0 off, 0 < top_p <= 1) and seeds int64 [B]; vocab <= 56 Ki
+// adapcc_beam_step's arguments for one group (no G, group_done or lambda; fin_count int32 [B]), plus cand_c fp32
+// [B*K, M] next to cand uint64 [B*K, M] (M = max(2, 1 + n_stop) * K), the sampling scalars (temperature > 0,
+// top_k >= 0 with 0 off, 0 < top_p <= 1) and seeds int64 [B]; vocab <= 56 Ki
 int adapcc_beam_sample_step(const float* logits, int ld, int vocab, int B, int K, float* scores, int* step,
                             int min_new, const int* suppress, int n_suppress, const int* stop, int n_stop,
                             const float* pen, int alpha_pos, int max_new, int* done, void* cand, float* cand_c,
                             long long* next_ids, int* parent, long long* hist_tok, int* hist_back, float* fin_score,
                             int* fin_n, int* fin_src, int* fin_count, float temperature, int top_k, float top_p,
                             const long long* seeds, void* stream) {
-  if (B < 1 || K < 1 || K > kBeamMaxK || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab || max_new < 1) {
-    set_error("beam_sample_step: need B >= 1, 1 <= K <= %d, 1 <= vocab <= %d, ld >= vocab, max_new >= 1 (B=%d K=%d "
-              "vocab=%d ld=%d max_new=%d)", kBeamMaxK, kSampleMaxVocab, B, K, vocab, ld, max_new);
+  BeamSampleArgs p{BeamArgs{logits, ld, vocab, B, K, 0, scores, step, min_new, suppress, n_suppress, stop, n_stop,
+                            pen, alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
+                            hist_back, fin_score, fin_n, fin_src, fin_count, 1, nullptr, 0.f},
+                   temperature, top_p, top_k, 0, seeds, cand_c};
+  if (check_beam_args("beam_sample_step", p.a)) return -1;
+  if (vocab > kSampleMaxVocab || !(temperature > 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
+    set_error("beam_sample_step: need vocab <= %d, temperature > 0, top_k >= 0, 0 < top_p <= 1 (got %d, %g, %d, %g)",
+              kSampleMaxVocab, vocab, temperature, top_k, top_p);
     return -1;
   }
-  if (n_suppress < 0 || n_suppress > kBeamMaxSuppress || n_stop < 0 || n_stop > kBeamMaxStop ||
-      (n_suppress && !suppress) || (n_stop && !stop)) {
-    set_error("beam_sample_step: at most %d suppressed and %d stop ids (got %d, %d)", kBeamMaxSuppress, kBeamMaxStop,
-              n_suppress, n_stop);
-    return -1;
-  }
-  if (!(temperature > 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
-    set_error("beam_sample_step: need temperature > 0, top_k >= 0, 0 < top_p <= 1 (got %g, %d, %g)", temperature,
-              top_k, top_p);
-    return -1;
-  }
-  if (!logits || !scores || !step || !pen || !done || !cand || !cand_c || !next_ids || !parent || !hist_tok ||
-      !hist_back || !fin_score || !fin_n || !fin_src || !fin_count || !seeds) {
+  if (!cand_c || !seeds) {
     set_error("beam_sample_step: null pointer");
     return -1;
   }
-  const int min_keep = n_stop + 1 > 2 ? n_stop + 1 : 2;
+  p.min_keep = n_stop + 1 > 2 ? n_stop + 1 : 2;
+  p.a.N = p.min_keep * K;
   const size_t smem = (size_t)vocab * sizeof(float);
   if (smem > 48 * 1024)
     CUDA_TRY(cudaFuncSetAttribute(beam_sample_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  BeamSampleArgs p{BeamArgs{logits, ld, vocab, B, K, min_keep * K, scores, step, min_new, suppress, n_suppress, stop,
-                            n_stop, pen, alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent,
-                            hist_tok, hist_back, fin_score, fin_n, fin_src, fin_count},
-                   temperature, top_p, top_k, min_keep, seeds, cand_c};
   cudaStream_t s = (cudaStream_t)stream;
   beam_sample_rows_kernel<<<B * K, kSampleThreads, smem, s>>>(p);
   CUDA_TRY(cudaGetLastError());

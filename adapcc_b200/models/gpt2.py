@@ -822,11 +822,10 @@ class GPT2DoubleHeads(nn.Module):
         reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the host reads the done flags once every 8
         tokens, a period late. Beam sampling takes a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids there, and
         the items' seeds are a device input of the graph. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
-        ``ops.repeats.penalize_repeats_reference``, ``ops.beam.BeamReference`` (``BeamSampleReference``,
-        ``GroupBeamReference``) and torch indexing."""
+        ``ops.repeats.penalize_repeats_reference``, ``ops.beam.GroupBeamReference`` (``BeamSampleReference`` with
+        ``do_sample``) and torch indexing."""
         from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB
-        from ..ops.beam import (BeamReference, BeamSampleReference, GroupBeamReference, best_hypotheses,
-                                merge_finished_sets)
+        from ..ops.beam import BeamSampleReference, GroupBeamReference, best_hypotheses, merge_finished_sets
 
         K = int(num_beams)
         if not 1 <= K <= BEAM_MAX_BEAMS:
@@ -873,11 +872,9 @@ class GPT2DoubleHeads(nn.Module):
                 ref = BeamSampleReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
                                           temperature=temperature, top_k=top_k, top_p=top_p,
                                           seeds=seeds.cpu().tolist())
-            elif G > 1:
+            else:
                 ref = GroupBeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
                                          num_beam_groups=G, diversity_penalty=lam)
-            else:
-                ref = BeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens)
             head = weight.float()
             for i in range(n):
                 if i:
@@ -901,9 +898,8 @@ class GPT2DoubleHeads(nn.Module):
             raise ValueError(f"beam_search: do_sample=True needs a vocabulary of at most {SAMPLE_MAX_VOCAB} ids on the "
                              f"native path, got {V}")
         st = BeamState(B, K, n, length_penalty, dev, sample=do_sample, groups=G)
-        scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds) if do_sample else {}
-        if G > 1:
-            scalars = dict(diversity_penalty=lam)
+        scalars = (dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds) if do_sample
+                   else dict(diversity_penalty=lam))
         logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
         sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
         prompt_len = cache.lens.clone()

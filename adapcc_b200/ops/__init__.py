@@ -56,12 +56,9 @@ def _lib():
                                                       + [c_float] * 5 + [c_void_p] * 3
                                                       + [c_int, c_void_p, c_int, c_void_p, c_int]
                                                       + [c_void_p] * 3 + [c_int, c_void_p])
-        lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
+        lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                          + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
-                                         + [c_void_p] * 10 + [c_void_p])
-        lib.adapcc_beam_group_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
-                                               + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
-                                               + [c_void_p] * 11 + [c_float, c_void_p])
+                                         + [c_void_p] * 11 + [c_float, c_void_p])
         lib.adapcc_beam_sample_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                                 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                                 + [c_void_p] * 11 + [c_float, c_int, c_float, c_void_p, c_void_p])
@@ -600,20 +597,12 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
             _ptr(state.fin_count), float(temperature), int(top_k), float(top_p), _ptr(seeds), _stream()),
             "beam_sample_step")
         return
-    if state.groups > 1:
-        _ck(_lib().adapcc_beam_group_step(
-            _ptr(logits), logits.stride(0), int(vocab), B, K, state.groups, _ptr(state.scores), _ptr(state.step),
-            int(min_new), sup, n_sup, stop, n_stop, _ptr(state.pen), int(state.length_penalty > 0), state.max_new,
-            _ptr(state.done), _ptr(state.group_done), _ptr(state.cand), _ptr(state.next_ids), _ptr(state.parent),
-            _ptr(state.hist_tok), _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_n),
-            _ptr(state.fin_src), _ptr(state.fin_count), lam, _stream()), "beam_group_step")
-        return
-    _ck(_lib().adapcc_beam_step(_ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores),
-                                _ptr(state.step), int(min_new), sup, n_sup, stop, n_stop, _ptr(state.pen),
-                                int(state.length_penalty > 0), state.max_new, _ptr(state.done), _ptr(state.cand),
-                                _ptr(state.next_ids), _ptr(state.parent), _ptr(state.hist_tok), _ptr(state.hist_back),
-                                _ptr(state.fin_score), _ptr(state.fin_n), _ptr(state.fin_src), _ptr(state.fin_count),
-                                _stream()), "beam_step")
+    _ck(_lib().adapcc_beam_step(
+        _ptr(logits), logits.stride(0), int(vocab), B, K, state.groups, _ptr(state.scores), _ptr(state.step),
+        int(min_new), sup, n_sup, stop, n_stop, _ptr(state.pen), int(state.length_penalty > 0), state.max_new,
+        _ptr(state.done), _ptr(state.group_done), _ptr(state.cand), _ptr(state.next_ids), _ptr(state.parent),
+        _ptr(state.hist_tok), _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_n), _ptr(state.fin_src),
+        _ptr(state.fin_count), lam, _stream()), "beam_step")
 
 
 def kv_reorder_scratch_numel(k_cache: torch.Tensor, max_new: int) -> int:
