@@ -94,7 +94,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
                    assistant_model=None, num_assistant_tokens: int = 4,
                    assistant_verification: str = "coupled", beam_sample: bool = False, num_beam_groups: int = 1,
-                   diversity_penalty: float = 0.0) -> List[List[int]]:
+                   diversity_penalty: float = 0.0, guidance_scale: float = 1.0,
+                   guidance_negative: str = "last_token") -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -113,19 +114,43 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     sampling instead: each reply token is still drawn from the model's distribution, but not the same draw.
     ``beam_sample`` with ``num_beams > 0``: beam sampling (``beam_search(do_sample=True)``) with ``temperature``,
     ``top_k``, ``top_p`` and the seeds. ``num_beam_groups`` and ``diversity_penalty`` go to ``beam_search`` (diverse
-    beam search, ``ops/beam.py``)."""
+    beam search, ``ops/beam.py``). ``guidance_scale`` != 1 goes to ``generate`` (classifier-free guidance,
+    ``ops/guidance.py``) with each dialogue's negative prompt: ``guidance_negative="last_token"`` is the prompt's last
+    token (HuggingFace's default), ``"no_persona"`` the same dialogue without the persona (built and truncated as the
+    prompt is), so guidance pushes each reply towards its persona. Guidance with ``num_beams``, ``penalty_alpha``,
+    prompt lookup or an assistant is a ``ValueError``."""
     from ..ops.assisted import check_verification
     check_verification("sample_replies", assistant_verification, assistant_model)
     if assistant_model is not None and (num_beams > 0 or penalty_alpha > 0):
         raise ValueError("sample_replies: assistant_model drafts for sampling and greedy generation only, not with "
                          f"num_beams > 0 or penalty_alpha > 0 (got {num_beams}, {penalty_alpha})")
-    insts = [build_input_from_segments(persona, history, [], tokenizer, with_eos=False,
-                                       max_len=model.cfg.n_positions - max_length) for persona, history in dialogs]
-    lengths = [len(i.input_ids) for i in insts]
-    T = max(lengths)
+    if guidance_negative not in ("last_token", "no_persona"):
+        raise ValueError(f"sample_replies: guidance_negative must be 'last_token' or 'no_persona', got "
+                         f"{guidance_negative!r}")
+    if guidance_scale != 1.0 and (num_beams > 0 or penalty_alpha > 0 or prompt_lookup_num_tokens > 0
+                                  or assistant_model is not None):
+        raise ValueError("sample_replies: guidance_scale != 1 works with sampling and greedy generation only, not with "
+                         "num_beams > 0, penalty_alpha > 0, prompt_lookup_num_tokens > 0 or assistant_model (got "
+                         f"{num_beams}, {penalty_alpha}, {prompt_lookup_num_tokens}, "
+                         f"{type(assistant_model).__name__})")
     pad = tokenizer.special_ids[-1]
-    ids = torch.tensor([i.input_ids + [pad] * (T - len(i.input_ids)) for i in insts], device=device)
-    tt = torch.tensor([i.token_type_ids + [pad] * (T - len(i.token_type_ids)) for i in insts], device=device)
+
+    def padded(persona_of):
+        insts = [build_input_from_segments(persona_of(persona), history, [], tokenizer, with_eos=False,
+                                           max_len=model.cfg.n_positions - max_length) for persona, history in dialogs]
+        lengths = [len(i.input_ids) for i in insts]
+        T = max(lengths)
+        ids = torch.tensor([i.input_ids + [pad] * (T - len(i.input_ids)) for i in insts], device=device)
+        tt = torch.tensor([i.token_type_ids + [pad] * (T - len(i.token_type_ids)) for i in insts], device=device)
+        return insts, lengths, ids, tt
+
+    insts, lengths, ids, tt = padded(lambda persona: persona)
+    guidance = {}
+    if guidance_scale != 1.0:
+        guidance = dict(guidance_scale=guidance_scale)
+        if guidance_negative == "no_persona":
+            _, n_lengths, n_ids, n_tt = padded(lambda persona: [])
+            guidance.update(negative_prompt_ids=n_ids, negative_lengths=n_lengths, negative_token_type_ids=n_tt)
     reply_type = torch.tensor([i.token_type_ids[-1] for i in insts], device=device)
     seed = torch.tensor(list(seeds) if seeds is not None else range(len(insts)), dtype=torch.int64)
     special = list(tokenizer.special_ids)
@@ -149,7 +174,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, min_p=min_p,
                                    typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
                                    assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
-                                   assistant_verification=assistant_verification, **repeats)
+                                   assistant_verification=assistant_verification, **repeats, **guidance)
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
 
 
@@ -241,6 +266,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model=None,
                      num_assistant_tokens: int = 4, assistant_verification: str = "coupled",
                      beam_sample: bool = False, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
+                     guidance_scale: float = 1.0, guidance_negative: str = "last_token",
                      **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
@@ -269,7 +295,10 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
 
     ``assistant_model`` (a draft model) with ``f1``: assisted generation with up to ``num_assistant_tokens`` drafts per
     round (``ops/assisted.py``), on that batched path; the replies are those of the batched path without it, unless
-    ``assistant_verification="rejection"`` (rejection sampling: replies from the same distribution, other draws)."""
+    ``assistant_verification="rejection"`` (rejection sampling: replies from the same distribution, other draws).
+
+    ``guidance_scale != 1`` with ``f1``: classifier-free guidance against ``guidance_negative`` (``"last_token"`` or
+    ``"no_persona"``, see :func:`sample_replies`), on that batched path."""
     from ..ops.assisted import check_verification
     check_verification("evaluate_dialogs", assistant_verification, assistant_model)
     repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
@@ -278,14 +307,15 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0
     assisted = assistant_model is not None
     if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup or filtered
-            or assisted) and eval_type == "f1":
+            or assisted or guidance_scale != 1.0) and eval_type == "f1":
         return _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples, device, seed,
                                     max(batch_size, 1), num_beams=num_beams, repetition_penalty=repetition_penalty,
                                     no_repeat_ngram_size=no_repeat_ngram_size, penalty_alpha=penalty_alpha,
                                     prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters,
                                     assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
                                     assistant_verification=assistant_verification, beam_sample=beam_sample,
-                                    num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty, **sample_kw)
+                                    num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty,
+                                    guidance_scale=guidance_scale, guidance_negative=guidance_negative, **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

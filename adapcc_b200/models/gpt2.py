@@ -30,6 +30,7 @@ import torch.nn as nn
 import torch.nn.functional as F
 
 from ..ops.dropout import DropoutState, check_p, dropout, site_attn, site_embed, site_mlp, site_summary
+from ..ops.guidance import check_guidance_args, guided_scores_reference
 from ..ops.layers import FusedLayerNorm, FusedLinear
 from ..ops.repeats import check_repeat_args, penalize_repeats_reference
 from ..ops.sampling import check_filter_args, sample_reference, top_filtering
@@ -232,29 +233,33 @@ class VerifyKV:
 
 
 class _Repeats:
-    """The repetition controls of a batched decoder over the R rows of its cache: ``seq`` int32 [R, t_max] each row's
-    sequence (its prompt, then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the penalty and the
-    n-gram size. ``create`` returns None when both controls are off, so then nothing is allocated or launched."""
+    """The repetition controls of a batched decoder over the first R rows of its cache (``rows``; default all of them,
+    ``generate`` with guidance passes its B prompt rows): ``seq`` int32 [R, t_max] each row's sequence (its prompt,
+    then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the penalty and the n-gram size.
+    ``create`` returns None when both controls are off, so then nothing is allocated or launched."""
 
-    def __init__(self, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int):
+    def __init__(self, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
+                 rows: Optional[int] = None):
         B, T = input_ids.shape
-        self.seq = torch.zeros(cache.batch, cache.t_max, dtype=torch.int32, device=input_ids.device)
-        self.seq[:, :T] = input_ids.repeat_interleave(cache.batch // B, dim=0)
-        self.prompt_len = cache.lens.clone()
+        self.rows = cache.batch if rows is None else int(rows)
+        self.seq = torch.zeros(self.rows, cache.t_max, dtype=torch.int32, device=input_ids.device)
+        self.seq[:, :T] = input_ids.repeat_interleave(self.rows // B, dim=0)
+        self.prompt_len = cache.lens[:self.rows].clone()
         self.vocab, self.penalty, self.ngram = vocab, penalty, ngram
 
     @classmethod
-    def create(cls, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float,
-               ngram: int) -> Optional["_Repeats"]:
-        return cls(input_ids, cache, vocab, penalty, ngram) if penalty != 1.0 or ngram > 0 else None
+    def create(cls, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
+               rows: Optional[int] = None) -> Optional["_Repeats"]:
+        return cls(input_ids, cache, vocab, penalty, ngram, rows) if penalty != 1.0 or ngram > 0 else None
 
     def eager(self, logits: torch.Tensor, cache: KVCache, consumed: Optional[torch.Tensor]) -> torch.Tensor:
         """``penalize_repeats_reference`` over every row's sequence, after storing ``consumed`` [R] (the tokens the last
         decode step consumed; None before the first one) at ``lens - 1``."""
+        R = self.rows
         if consumed is not None:
             dev = self.seq.device
-            self.seq[torch.arange(cache.batch, device=dev), cache.lens.long() - 1] = consumed.to(dev, torch.int32)
-        return penalize_repeats_reference(logits, [self.seq[r, :x] for r, x in enumerate(cache.host_lens)],
+            self.seq[torch.arange(R, device=dev), cache.lens[:R].long() - 1] = consumed.to(dev, torch.int32)
+        return penalize_repeats_reference(logits, [self.seq[r, :x] for r, x in enumerate(cache.host_lens[:R])],
                                           self.vocab, self.penalty, self.ngram)
 
     def reorder(self, rows: torch.Tensor) -> None:
@@ -644,6 +649,32 @@ class GPT2DoubleHeads(nn.Module):
             tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
         return B, T, lengths, n, t_max, last, tt_new, native
 
+    def _guidance_rows(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], lengths: List[int],
+                       last: torch.Tensor, tt_new: Optional[torch.Tensor], negative_prompt_ids: Optional[torch.Tensor],
+                       neg_lengths: List[int], negative_token_type_ids: Optional[torch.Tensor]):
+        """``generate``'s 2B prefill rows with guidance: the prompts, then the negative prompts (each row's last prompt
+        token when ``negative_prompt_ids`` is None), right-padded to one width. Returns ``(ids, token types or None,
+        lengths, token types of new tokens [2B] or None)``."""
+        B, T = input_ids.shape
+        dev = input_ids.device
+        rows = torch.arange(B, device=dev)
+        if negative_prompt_ids is None:
+            neg, neg_tt = input_ids[rows, last][:, None], None
+            if token_type_ids is not None:
+                neg_tt = token_type_ids[rows, last][:, None]
+        else:
+            neg, neg_tt = negative_prompt_ids.to(dev), negative_token_type_ids
+            if neg_tt is None and token_type_ids is not None:
+                neg_tt = tt_new[:, None].expand(neg.shape)
+        Tn = neg.shape[1]
+        ids = torch.zeros(2 * B, max(T, Tn), dtype=input_ids.dtype, device=dev)
+        ids[:B, :T], ids[B:, :Tn] = input_ids, neg
+        tt = None
+        if token_type_ids is not None:
+            tt = torch.zeros_like(ids, dtype=token_type_ids.dtype)
+            tt[:B, :T], tt[B:, :Tn] = token_type_ids, neg_tt.to(dev)
+        return ids, tt, list(lengths) + list(neg_lengths), None if tt_new is None else tt_new.repeat(2)
+
     @torch.no_grad()
     def generate(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
                  token_type_ids: Optional[torch.Tensor] = None, reply_type=None, max_new_tokens: int = 20,
@@ -653,7 +684,9 @@ class GPT2DoubleHeads(nn.Module):
                  max_matching_ngram_size: int = 2, min_p: float = 0.0, typical_p: float = 1.0,
                  epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model: "GPT2DoubleHeads" = None,
                  num_assistant_tokens: int = 4,
-                 assistant_verification: str = "coupled") -> Tuple[torch.Tensor, torch.Tensor]:
+                 assistant_verification: str = "coupled", guidance_scale: float = 1.0,
+                 negative_prompt_ids: Optional[torch.Tensor] = None, negative_lengths: Optional[Sequence[int]] = None,
+                 negative_token_type_ids: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -704,7 +737,19 @@ class GPT2DoubleHeads(nn.Module):
         emitted token is then distributed as the model's, acceptance is their overlap rather than the agreement of
         two draws, and the tokens depend on the draft. On the native path the draft draws also keep their weights and
         the verify step runs ``ops.spec_slots_`` and ``ops.lookup_accept_(..., flagged=True)``. At temperature
-        0 both rules are the greedy one."""
+        0 both rules are the greedy one.
+
+        ``guidance_scale`` = g != 1 is HuggingFace's classifier-free guidance (``UnbatchedClassifierFreeGuidance
+        LogitsProcessor``; the definition is in ``ops/guidance.py``; any finite g, 1: off). Each row also decodes a
+        negative prompt, ``negative_prompt_ids`` [B, Tn] right-padded to ``negative_lengths`` (default Tn), by default
+        the row's last prompt token alone with its token type; the negative rows consume the tokens the prompt rows
+        draw. Each token's scores become ``g * (lc - lu) + lu`` of the two rows' log-softmaxes, before the repetition
+        controls (which see the prompt rows' sequences only) and the sampler. When the prompts have
+        ``token_type_ids``, negative prompts take ``negative_token_type_ids``, else the type of the new tokens; new
+        tokens take the same type in both rows. Not with prompt lookup or an assistant. The cache then holds 2B rows, prompts
+        first (at most ``LM_HEAD_MAX_ROWS`` on the native path), prefilled together; on the native path each graph
+        replay runs the decode step and LM head on all of them and ``ops.guidance_mix_`` after the head. Prompt rows
+        draw from the same seeds and positions as without guidance."""
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
@@ -712,6 +757,13 @@ class GPT2DoubleHeads(nn.Module):
         filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
         from ..ops.assisted import check_verification
         check_verification("generate", assistant_verification, assistant_model)
+        B0 = input_ids.shape[0] if input_ids.dim() == 2 else 0
+        neg_lengths = check_guidance_args("generate", guidance_scale, B0, negative_prompt_ids, negative_lengths,
+                                          negative_token_type_ids, token_type_ids, max_new_tokens, self.cfg.n_positions)
+        guided = neg_lengths is not None
+        if guided and (assistant_model is not None or prompt_lookup_num_tokens != 0):
+            raise ValueError("generate: guidance_scale != 1 cannot be combined with prompt_lookup_num_tokens or "
+                             f"assistant_model (got {prompt_lookup_num_tokens}, {type(assistant_model).__name__})")
         if assistant_model is not None or prompt_lookup_num_tokens != 0:
             from ..ops import LOOKUP_MAX_NGRAM, LOOKUP_MAX_TOKENS
             if assistant_model is not None:
@@ -730,44 +782,62 @@ class GPT2DoubleHeads(nn.Module):
                                               assistant_verification == "rejection" and temperature > 0)
         B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
-            repetition_penalty, no_repeat_ngram_size)
+            repetition_penalty, no_repeat_ngram_size, num_beams=2 if guided else 1,
+            rows_name="rows with guidance (batch x 2)")
         dev, V = input_ids.device, self.cfg.vocab_size
         seeds = _row_seeds(seed, B, dev)
-        cache = self.new_cache(B, t_max)
-        h = self.hidden(input_ids, token_type_ids, cache=cache, lengths=lengths)[torch.arange(B, device=dev), last]
+        if guided:                                  # rows [0, B): the prompts, rows [B, 2B): the negative prompts
+            ids_all, tt_all, lengths_all, tt_new = self._guidance_rows(
+                input_ids, token_type_ids, lengths, last, tt_new, negative_prompt_ids, neg_lengths,
+                negative_token_type_ids)
+            t_max = max(lengths_all) + n
+            last = torch.tensor(lengths_all, device=dev) - 1
+        else:
+            ids_all, tt_all, lengths_all = input_ids, token_type_ids, lengths
+        R = len(lengths_all)
+        cache = self.new_cache(R, t_max)
+        h = self.hidden(ids_all, tt_all, cache=cache, lengths=lengths_all)[torch.arange(R, device=dev), last]
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
-        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
+        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, B)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = self.wte.weight.float()
             done = torch.zeros(B, dtype=torch.int32)
             for i in range(n):
                 if i:
-                    h = self.decode_step(nxt.to(dev), tt_new, cache)
+                    h = self.decode_step(nxt.to(dev).repeat(R // B), tt_new, cache)
                 logits = self.lm_logits(h, head)
+                if guided:
+                    logits = guided_scores_reference(logits[:B], logits[B:], V, guidance_scale).float()
                 if reps is not None:
                     logits = reps.eager(logits, cache, nxt if i else None)
-                nxt, tok, done = sample_reference(logits, V, temperature, top_k, top_p, seeds, cache.lens, i,
+                nxt, tok, done = sample_reference(logits, V, temperature, top_k, top_p, seeds, cache.lens[:B], i,
                                                   min_new_tokens, suppress_ids, stop_ids, done, **filters)
                 tokens[:, i] = tok.to(dev)
                 if bool(done.all()):
                     break
             return tokens, (tokens >= 0).sum(1)
 
-        from ..ops import lm_head_logits_, sample_tokens_
+        from ..ops import guidance_mix_, lm_head_logits_, sample_tokens_
 
         weight = self.wte.weight
-        logits = torch.empty(B, weight.shape[0], dtype=torch.float32, device=dev)
-        next_ids = torch.zeros(B, dtype=torch.int64, device=dev)
+        logits = torch.empty(R, weight.shape[0], dtype=torch.float32, device=dev)
+        next_ids = torch.zeros(R, dtype=torch.int64, device=dev)
         done = torch.zeros(B, dtype=torch.int32, device=dev)
         step = torch.zeros(1, dtype=torch.int32, device=dev)
         sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
+        # the prompt rows (all rows without guidance)
+        lg, lens, ids = logits[:B], cache.lens[:B], next_ids[:B]
 
         def head_and_sample(hidden):
             lm_head_logits_(hidden, weight, logits)
+            if guided:
+                guidance_mix_(logits, V, B, guidance_scale)
             if reps is not None:
-                reps.native(logits, cache.lens, step, next_ids)
-            sample_tokens_(logits, V, temperature, top_k, top_p, seeds, cache.lens, step,
-                           min_new_tokens, sup, stop, done, next_ids, tokens, **filters)
+                reps.native(lg, lens, step, ids)
+            sample_tokens_(lg, V, temperature, top_k, top_p, seeds, lens, step,
+                           min_new_tokens, sup, stop, done, ids, tokens, **filters)
+            if guided:                              # the negative rows consume the prompt rows' tokens
+                next_ids[B:].copy_(ids)
 
         head_and_sample(h)                          # the first token, from the prefill's last positions
         if n > 1:

@@ -66,6 +66,7 @@ def _lib():
                                                                                                 c_void_p]
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
                                                 + [c_int, c_float, c_int, c_void_p])
+        lib.adapcc_guidance_mix.argtypes = [c_void_p, c_int, c_int, c_int, c_float, c_void_p]
         lib.adapcc_cs_sim_numel.argtypes = [c_int] * 3
         lib.adapcc_cs_sim_numel.restype = c_longlong
         lib.adapcc_cand_attn.argtypes = [c_void_p] * 7 + [c_int] * 6 + [c_void_p, c_void_p]
@@ -686,6 +687,33 @@ def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, promp
     _ck(_lib().adapcc_penalize_repeats(_ptr(logits), logits.stride(0), int(vocab), R, _ptr(seq), seq.shape[1],
                                        _ptr(prompt_len), _ptr(lens), _ptr(step), _ptr(ids), _ptr(parent), int(group),
                                        float(penalty), int(ngram), _stream()), "penalize_repeats")
+
+
+# ---- classifier-free guidance (csrc/ops_guidance.cu) ---------------------------------------------------------------
+def guidance_mix_(logits: torch.Tensor, vocab: int, B: int, scale: float) -> torch.Tensor:
+    """Classifier-free guidance in place, on the device (the definition in ``ops/guidance.py``, which computes the same
+    in fp64): ``logits`` fp32 [2B, ld] hold the prompts' rows, then the negative prompts' rows. Row b's first ``vocab``
+    columns become ``scale * (lc - lu) + lu``, ``lc`` / ``lu`` the log-softmaxes of rows b and B + b; the other
+    columns and rows [B, 2B) are not written. fp32 sums in an order fixed by the thread layout, so a row's bits depend
+    on its two input rows, ``vocab`` and ``scale`` only. No host sync."""
+    def bad(msg):
+        raise ValueError(f"guidance_mix_: {msg}")
+
+    from .guidance import FP32_MAX
+
+    if not (math.isfinite(scale) and abs(scale) <= FP32_MAX):
+        bad(f"need a finite fp32 scale, got {scale}")
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
+        bad(f"logits must be fp32 [2B, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)} stride "
+            f"{logits.stride()}")
+    if int(B) < 1 or logits.shape[0] != 2 * int(B):
+        bad(f"logits must have 2B rows for B >= 1, got {logits.shape[0]} rows and B = {B}")
+    if not 1 <= vocab <= logits.shape[1]:
+        bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
+    _same_device("guidance_mix_", logits.device, ())
+    _ck(_lib().adapcc_guidance_mix(_ptr(logits), logits.stride(0), int(vocab), int(B), float(scale), _stream()),
+        "guidance_mix")
+    return logits
 
 
 # ---- contrastive search: candidate attention, selection, re-rank and commit (csrc/ops_contrastive.cu) ---------------

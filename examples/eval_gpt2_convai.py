@@ -75,6 +75,11 @@ def main():
     p.add_argument("--assistant_verification", choices=("coupled", "rejection"), default="coupled",
                    help="f1 with --assistant_checkpoint: coupled draws (the replies drawn without the draft) or "
                         "rejection sampling (replies from the same distribution, more drafts accepted)")
+    p.add_argument("--guidance_scale", type=float, default=1.0,
+                   help="f1: classifier-free guidance scale (1: off); replies go through the batched path")
+    p.add_argument("--guidance_negative", choices=("last_token", "no_persona"), default="last_token",
+                   help="f1 with --guidance_scale: the negative prompt, the prompt's last token or the dialogue "
+                        "without the persona")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -89,7 +94,8 @@ def main():
                   no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha,
                   prompt_lookup_num_tokens=a.prompt_lookup_num_tokens, min_p=a.min_p, typical_p=a.typical_p,
                   epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, beam_sample=a.beam_sample,
-                  num_beam_groups=a.num_beam_groups, diversity_penalty=a.diversity_penalty)
+                  num_beam_groups=a.num_beam_groups, diversity_penalty=a.diversity_penalty,
+                  guidance_scale=a.guidance_scale, guidance_negative=a.guidance_negative)
         if a.assistant_checkpoint:
             kw["assistant_model"] = load_model_from_checkpoint(
                 a.assistant_checkpoint, a.device, torch.bfloat16 if a.device.startswith("cuda") else None)[0]

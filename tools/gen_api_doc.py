@@ -30,6 +30,7 @@ MODULES = [
     ("adapcc_b200.ops.assisted", ["check_assist_args", "draw_slot", "assist_round", "draw_slots", "check_verification",
                                   "filtered_probs", "spec_slot", "spec_slots"]),
     ("adapcc_b200.ops.repeats", ["penalize_repeats_reference", "banned_ngram_ids", "check_repeat_args"]),
+    ("adapcc_b200.ops.guidance", ["check_guidance_args", "guided_scores_reference"]),
     ("adapcc_b200.ops.layers", ["FusedLayerNorm", "FusedLinear", "linear_backward"]),
     ("adapcc_b200.ops.gemm", ["linear_act", "linear_gelu", "supported", "default_variant"]),
     ("adapcc_b200.strategy.trees", ["Tree", "Strategy"]),
