@@ -25,6 +25,14 @@
 //                        The first K draws that finish are offered, and the K best-c draws that do not are the new
 //                        beams (DESIGN.md §4a).
 //
+// Stochastic beam search (Kool et al. 2019; rules R1-R8 of ops/beam.py) replaces them too:
+//   beam_stochastic_rows   : one 1024-thread CTA per beam row, x_i = l_i / T in shared memory. The sampler's filter
+//                            (min_keep 1), log Z over the kept ids, then phi_i = phi + lp'_i and Gphi_i = phi_i + G_i
+//                            of every kept id; the K + 1 best Gphi (row_best_keys, shared with beam_sample_rows) are
+//                            offered with their keys truncated at the beam's key G and their phi.
+//   beam_stochastic_select : one 512-thread CTA per item. Every entry of the pool (finished set, offered children) is
+//                            ranked by counting; the K first survive, entry K + 1 raises kappa.
+//
 // Every fp32 sum runs in an order fixed by the thread layout (per-thread loops in id order, shuffle trees, warp partials
 // added by a shuffle tree in warp order); an item's result depends only on its own rows. ops/beam.py evaluates the same
 // definition in fp64.
@@ -290,6 +298,74 @@ __device__ __forceinline__ float beam_gumbel(uint32_t w) {
   return -logf(nlu);
 }
 
+// The M best keys f2key(s_x[i]) of a row of 1024 threads (all finite ones when there are at most M; else those above
+// the M-th largest key, and of the ones equal to it the lowest ids) as (key << 32) | ~i, best first: emit(r, v) for
+// r < M, v = 0 past the count. s_sel holds M entries. Returns the largest key.
+template <class Emit>
+__device__ __forceinline__ uint32_t row_best_keys(const float* s_x, SampleSmem& sm, int V, int M,
+                                                  unsigned long long* s_sel, int* s_n, Emit emit) {
+  const int tid = threadIdx.x;
+  unsigned long long best = 0;
+  int cnt = 0, z1 = 0, z2 = 0;
+  float fz = 0.f;
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const uint32_t k = f2key(s_x[i]);
+    if (k > kNegInfKey) {
+      ++cnt;
+      best = max(best, (unsigned long long)k);
+    }
+  }
+  best = block_max(sm, best);
+  block_sum(sm, fz, cnt, z1, z2);
+  uint32_t thr = kNegInfKey;                          // taken: key > thr, or key == thr and id < cut
+  int cut = 0;
+  if (cnt > M) {
+    thr = kth_key(s_x, sm, V, M, (uint32_t)best);
+    int gt = 0, eq = 0, unused = 0;
+    for (int i = tid; i < V; i += kSampleThreads) {
+      const uint32_t k = f2key(s_x[i]);
+      gt += k > thr;
+      eq += k == thr;
+    }
+    block_sum(sm, fz, gt, eq, unused);
+    const int need = M - gt;
+    cut = V;
+    if (eq > need) {                                  // tied at the M-th key: the smallest cut with need ids below it
+      int lo = 0, hi = V;
+      while (hi - lo > 1) {
+        const int mid = lo + (hi - lo) / 2;
+        int c = 0, u0 = 0, u1 = 0;
+        for (int i = tid; i < mid; i += kSampleThreads) c += f2key(s_x[i]) == thr;
+        block_sum(sm, fz, c, u0, u1);
+        if (c >= need) hi = mid;
+        else lo = mid;
+      }
+      cut = hi;
+    }
+  }
+  if (tid == 0) *s_n = 0;
+  __syncthreads();
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const uint32_t k = f2key(s_x[i]);
+    if (k > thr || (k == thr && i < cut)) s_sel[atomicAdd(s_n, 1)] = ((unsigned long long)k << 32) |
+                                                                     (0xFFFFFFFFu - (uint32_t)i);
+  }
+  __syncthreads();
+  const int n = *s_n;
+  // best first: a key's place is the number of larger keys (the keys are distinct)
+  for (int e = tid; e < M; e += kSampleThreads) {
+    if (e >= n) {
+      emit(e, 0ull);
+      continue;
+    }
+    const unsigned long long v = s_sel[e];
+    int r = 0;
+    for (int f = 0; f < n; ++f) r += s_sel[f] > v;
+    emit(r, v);
+  }
+  return (uint32_t)best;
+}
+
 __global__ void __launch_bounds__(kSampleThreads, 1) beam_sample_rows_kernel(const __grid_constant__ BeamSampleArgs p) {
   extern __shared__ float s_x[];                      // [vocab]: x_i = l_i / T, then g_i of the kept ids (-inf else)
   __shared__ SampleSmem sm;
@@ -369,66 +445,10 @@ __global__ void __launch_bounds__(kSampleThreads, 1) beam_sample_rows_kernel(con
     }
   }
   __syncthreads();
-  // the M best keys (g bits, then the inverted id): all kept ids when there are at most M; else those above the M-th
-  // largest g, and of the ones equal to it the lowest ids
-  best = 0;
-  int cnt = 0;
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const uint32_t k = f2key(s_x[i]);
-    if (k > kNegInfKey) {
-      ++cnt;
-      best = max(best, (unsigned long long)k);
-    }
-  }
-  best = block_max(sm, best);
-  block_sum(sm, fz, cnt, z1, z2);
-  uint32_t thr = kNegInfKey;                          // taken: key > thr, or key == thr and id < cut
-  int cut = 0;
-  if (cnt > M) {
-    thr = kth_key(s_x, sm, V, M, (uint32_t)best);
-    int gt = 0, eq = 0, unused = 0;
-    for (int i = tid; i < V; i += kSampleThreads) {
-      const uint32_t k = f2key(s_x[i]);
-      gt += k > thr;
-      eq += k == thr;
-    }
-    block_sum(sm, fz, gt, eq, unused);
-    const int need = M - gt;
-    cut = V;
-    if (eq > need) {                                  // tied at the M-th key: the smallest cut with need ids below it
-      int lo = 0, hi = V;
-      while (hi - lo > 1) {
-        const int mid = lo + (hi - lo) / 2;
-        int c = 0, u0 = 0, u1 = 0;
-        for (int i = tid; i < mid; i += kSampleThreads) c += f2key(s_x[i]) == thr;
-        block_sum(sm, fz, c, u0, u1);
-        if (c >= need) hi = mid;
-        else lo = mid;
-      }
-      cut = hi;
-    }
-  }
-  if (tid == 0) s_n = 0;
-  __syncthreads();
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const uint32_t k = f2key(s_x[i]);
-    if (k > thr || (k == thr && i < cut)) s_sel[atomicAdd(&s_n, 1)] = ((unsigned long long)k << 32) |
-                                                                      (0xFFFFFFFFu - (uint32_t)i);
-  }
-  __syncthreads();
-  const int n = s_n;
-  // best first: a key's place is the number of larger keys (the keys are distinct)
-  for (int e = tid; e < M; e += kSampleThreads) {
-    if (e >= n) {
-      out[e] = 0ull;
-      continue;
-    }
-    const unsigned long long v = s_sel[e];
-    int r = 0;
-    for (int f = 0; f < n; ++f) r += s_sel[f] > v;
+  row_best_keys(s_x, sm, V, M, s_sel, &s_n, [&](int r, unsigned long long v) {
     out[r] = v;
-    out_c[r] = cand_score((int)(0xFFFFFFFFu - (uint32_t)v));
-  }
+    if (v) out_c[r] = cand_score((int)(0xFFFFFFFFu - (uint32_t)v));
+  });
 }
 
 __global__ void __launch_bounds__(kBeamThreads) beam_sample_select_kernel(const __grid_constant__ BeamSampleArgs p) {
@@ -537,6 +557,233 @@ __global__ void __launch_bounds__(kBeamThreads) beam_sample_select_kernel(const 
   fs.store(a, b * K, b, tid);
 }
 
+// ---- stochastic beam search ------------------------------------------------------------------------------------------
+struct BeamStochasticArgs {
+  BeamArgs a;                  // a.N = K + 1; a.scores: the live beams' log-probabilities phi (-inf: dead); a.fin_score
+                               // the finished entries' keys; a.cand [B * K, K + 1]: each row's offered children
+  float temperature, top_p;
+  int top_k;
+  const long long* seeds;      // [B]: the item's Philox key
+  float* keys;                 // [B * K]: the live beams' keys G
+  float* cand_key;             // [B * K, K + 1]: the truncated key of the child next to each cand entry
+  float* cand_phi;             // [B * K, K + 1]: its log-probability phi
+  float* fin_phi;              // [B, K]: the finished entries' log-probabilities
+  float* kappa;                // [B]: the largest key pruned so far
+};
+
+// log(1 - exp(x)) for x <= 0 without cancellation on either side of -ln 2; -inf at x = 0
+__device__ __forceinline__ float log1mexp(float x) {
+  return x > -0.693147182f ? logf(-expm1f(x)) : log1pf(-expf(x));
+}
+
+__global__ void __launch_bounds__(kSampleThreads, 1)
+beam_stochastic_rows_kernel(const __grid_constant__ BeamStochasticArgs p) {
+  extern __shared__ float s_x[];                      // [vocab]: x_i = l_i / T, then Gphi_i of the kept ids (-inf else)
+  __shared__ SampleSmem sm;
+  __shared__ unsigned long long s_sel[kBeamMaxK + 1], s_ord[kBeamMaxK + 1];
+  __shared__ int s_n;
+  __shared__ float s_z;
+  const BeamArgs& a = p.a;
+  const int row = blockIdx.x, b = row / a.K, j = row - b * a.K, tid = threadIdx.x, V = a.vocab, N = a.N;
+  unsigned long long* out = a.cand + (long long)row * N;
+  const float phi = a.scores[row];
+  if (a.done[b] || !(phi > -INFINITY)) {              // a finished item or a dead beam offers nothing
+    if (tid < N) out[tid] = 0ull;
+    return;
+  }
+  const int step = *a.step;
+  const float* l = a.logits + (long long)row * a.ld;
+  for (int i = tid; i < V; i += kSampleThreads) s_x[i] = __fdiv_rn(__ldg(l + i), p.temperature);
+  __syncthreads();
+  if (step < a.min_new) {
+    for (int q = tid; q < a.n_suppress; q += kSampleThreads) {
+      const int id = a.suppress[q];
+      if (id >= 0 && id < V) s_x[id] = -INFINITY;
+    }
+    __syncthreads();
+  }
+  unsigned long long best = 0;
+  int present = 0, z1 = 0, z2 = 0;
+  float fz = 0.f;
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const uint32_t k = f2key(s_x[i]);
+    if (k > kNegInfKey) {
+      ++present;
+      best = max(best, (unsigned long long)k);
+    }
+  }
+  best = block_max(sm, best);
+  block_sum(sm, fz, present, z1, z2);
+  if (present == 0) {                                 // every id removed or at -inf
+    if (tid < N) out[tid] = 0ull;
+    return;
+  }
+  // the sampler's filter (min_keep 1), then log Z over the kept ids: lp'_i = (x_i - m) - log Z
+  const float m = key2f((uint32_t)best);
+  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, 1, present, (uint32_t)best, m);
+  float z = 0.f;
+  int u0 = 0, u1 = 0, u2 = 0;
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const float x = s_x[i];
+    if (f2key(x) >= tau) z += expf(x - m);
+  }
+  block_sum(sm, z, u0, u1, u2);                       // its barriers order every read of x before the writes below
+  const float lz = logf(z);
+  auto child_phi = [&](int i) { return phi + ((__fdiv_rn(__ldg(l + i), p.temperature) - m) - lz); };
+  // Gphi_i = phi_i + G_i; ids 4q..4q+3 take the four words of Philox at counter (q, j, step, 1)
+  const uint32_t k0 = (uint32_t)(unsigned long long)p.seeds[b], k1 = (uint32_t)((unsigned long long)p.seeds[b] >> 32);
+  for (int q = tid; q < (V + 3) / 4; q += kSampleThreads) {
+    bool kept[4], any = false;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int i = 4 * q + e;
+      kept[e] = i < V && f2key(s_x[i]) >= tau;
+      any |= kept[e];
+    }
+    uint4 w = make_uint4(0u, 0u, 0u, 0u);
+    if (any) w = philox4((uint32_t)q, (uint32_t)j, (uint32_t)step, 1u, k0, k1);
+    const uint32_t words[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int i = 4 * q + e;
+      if (i < V) s_x[i] = kept[e] ? child_phi(i) + beam_gumbel(words[e]) : -INFINITY;
+    }
+  }
+  __syncthreads();
+  // the K + 1 best children by Gphi, each with its key truncated at G: G - softplus(v),
+  // v = G - Gphi + log1mexp(Gphi - Zj), Zj the row's largest Gphi (its child keeps G exactly)
+  const float G = p.keys[row];
+  float* out_key = p.cand_key + (long long)row * N;
+  float* out_phi = p.cand_phi + (long long)row * N;
+  const uint32_t zkey = row_best_keys(s_x, sm, V, N, s_sel, &s_n, [&](int r, unsigned long long v) {
+    out[r] = v;
+    s_ord[r] = v;
+  });
+  if (tid == 0) s_z = key2f(zkey);
+  __syncthreads();
+  if (tid < N && s_ord[tid]) {
+    const unsigned long long v = s_ord[tid];
+    const int i = (int)(0xFFFFFFFFu - (uint32_t)v);
+    const float gphi = key2f((uint32_t)(v >> 32));
+    const float u = (G - gphi) + log1mexp(gphi - s_z);
+    out_key[tid] = (G - fmaxf(u, 0.f)) - log1pf(expf(-fabsf(u)));
+    out_phi[tid] = child_phi(i);
+  }
+}
+
+// One 512-thread CTA per item. The pool is the finished set (entries 0..K-1) and the rows' offered children; each
+// entry's rank is the number of entries before it (descending key, then finished before children, the set's order,
+// the lower flat index j * V + i), so the K + 1 first are known without a sort.
+__global__ void __launch_bounds__(kBeamThreads) beam_stochastic_select_kernel(
+    const __grid_constant__ BeamStochasticArgs p) {
+  constexpr int kPool = kBeamMaxK + kBeamMaxK * (kBeamMaxK + 1);
+  __shared__ unsigned long long s_k[kPool];           // (key bits << 32) | inverted order; 0: no entry
+  __shared__ int s_at[kBeamMaxK + 1];                 // rank -> entry
+  __shared__ FinishedSet old, nw;
+  __shared__ float s_ophi[kBeamMaxK], s_nphi[kBeamMaxK];
+  __shared__ int s_tok[kBeamMaxK], s_par[kBeamMaxK];
+  __shared__ float s_phi[kBeamMaxK], s_key[kBeamMaxK];
+  __shared__ int s_nb;
+  const BeamArgs& a = p.a;
+  const int b = blockIdx.x, tid = threadIdx.x, K = a.K, N = a.N, V = a.vocab, BK = a.B * a.K, P = K + K * N;
+  const int step = *a.step;
+  if (a.done[b] || step >= a.max_new) {               // nothing moves: every row keeps its own cache
+    if (tid < K) a.parent[b * K + tid] = b * K + tid;
+    return;
+  }
+  old.load(a, b * K, b, K, tid);
+  if (tid < K) {
+    s_ophi[tid] = p.fin_phi[b * K + tid];
+    nw.score[tid] = -INFINITY;
+    nw.n[tid] = 0;
+    nw.src[tid] = 0;
+    s_nphi[tid] = -INFINITY;
+  }
+  if (tid <= K) s_at[tid] = -1;
+  for (int e = tid; e < K * N; e += kBeamThreads) {
+    const int j = e / N;
+    const long long o = (long long)(b * K + j) * N + (e - j * N);
+    const unsigned long long v = a.cand[o];
+    const uint32_t key = v ? f2key(p.cand_key[o]) : 0u;
+    const uint32_t flat = (uint32_t)j * (uint32_t)V + (0xFFFFFFFFu - (uint32_t)v);
+    s_k[K + e] = key > kNegInfKey ? ((unsigned long long)key << 32) | (0xFFFFFFFFu - kBeamMaxK - flat) : 0ull;
+  }
+  __syncthreads();
+  if (tid < K) {
+    const uint32_t key = tid < old.count ? f2key(old.score[tid]) : 0u;
+    s_k[tid] = key > kNegInfKey ? ((unsigned long long)key << 32) | (0xFFFFFFFFu - (uint32_t)tid) : 0ull;
+  }
+  __syncthreads();
+  for (int e = tid; e < P; e += kBeamThreads) {
+    const unsigned long long v = s_k[e];
+    if (!v) continue;
+    int r = 0;
+    for (int f = 0; f < P && r <= K; ++f) r += s_k[f] > v;
+    if (r <= K) s_at[r] = e;
+  }
+  __syncthreads();
+  const bool last = step == a.max_new - 1;
+  const int L = step + 1;                             // tokens of a hypothesis that ends at this step
+  if (tid == 0) {                                     // the K first survive, in rank order
+    nw.K = K;
+    nw.count = 0;
+    int nb = 0;
+    auto finish = [&](float key, int n, int src, float ph) {
+      nw.score[nw.count] = key;
+      nw.n[nw.count] = n;
+      nw.src[nw.count] = src;
+      s_nphi[nw.count++] = ph;
+    };
+    for (int r = 0; r < K && s_at[r] >= 0; ++r) {
+      const int e = s_at[r];
+      const float key = key2f((uint32_t)(s_k[e] >> 32));
+      if (e < K) {
+        finish(key, old.n[e], old.src[e], s_ophi[e]);
+        continue;
+      }
+      const int j = (e - K) / N;
+      const long long o = (long long)(b * K + j) * N + (e - K - j * N);
+      const int i = (int)(0xFFFFFFFFu - (uint32_t)a.cand[o]);
+      bool is_stop = false;
+      for (int q = 0; q < a.n_stop; ++q) is_stop |= a.stop[q] == i;
+      if (is_stop) {
+        finish(key, L - 1, j, p.cand_phi[o]);
+        continue;
+      }
+      // a new beam takes history slot nb; at the last step it finishes there
+      s_tok[nb] = i;
+      s_par[nb] = j;
+      s_phi[nb] = p.cand_phi[o];
+      s_key[nb] = key;
+      if (last) finish(key, a.max_new, nb, p.cand_phi[o]);
+      ++nb;
+    }
+    if (s_at[K] >= 0) p.kappa[b] = fmaxf(p.kappa[b], key2f((uint32_t)(s_k[s_at[K]] >> 32)));
+    s_nb = nb;
+    a.done[b] = last || nb == 0;
+  }
+  __syncthreads();
+  nw.store(a, b * K, b, tid);
+  if (tid < K) {
+    p.fin_phi[b * K + tid] = s_nphi[tid];
+    const int r = b * K + tid, nb = s_nb;
+    const long long h = (long long)step * BK + r;
+    a.hist_tok[h] = tid < nb ? s_tok[tid] : -1;
+    a.hist_back[h] = tid < nb ? s_par[tid] : tid;
+    if (tid < nb && !last) {
+      a.next_ids[r] = s_tok[tid];
+      a.parent[r] = b * K + s_par[tid];
+      a.scores[r] = s_phi[tid];
+      p.keys[r] = s_key[tid];
+    } else {
+      a.next_ids[r] = 0;
+      a.parent[r] = r;
+      a.scores[r] = -INFINITY;
+      p.keys[r] = -INFINITY;
+    }
+  }
+}
+
 // ---- KV-cache reordering -----------------------------------------------------------------------------------------
 struct ReorderArgs {
   __nv_bfloat16* k;            // [L, R, H, t_max, Dh]
@@ -576,7 +823,8 @@ __global__ void __launch_bounds__(kReorderThreads) kv_reorder_kernel(const __gri
   }
 }
 
-// the checks both step entry points make; each then checks its own mode's arguments and sets a.N from n_stop
+// the checks every step entry point makes; each then checks its own mode's arguments and sets a.N. alpha_pos < 0: no
+// length penalty (stochastic beam search), so no pen
 static int check_beam_args(const char* who, const BeamArgs& a) {
   if (a.B < 1 || a.K < 1 || a.K > kBeamMaxK || a.vocab < 1 || a.ld < a.vocab || a.max_new < 1) {
     set_error("%s: need B >= 1, 1 <= K <= %d, vocab >= 1, ld >= vocab, max_new >= 1 (B=%d K=%d vocab=%d ld=%d "
@@ -589,7 +837,7 @@ static int check_beam_args(const char* who, const BeamArgs& a) {
               a.n_suppress, a.n_stop);
     return -1;
   }
-  if (!a.logits || !a.scores || !a.step || !a.pen || !a.done || !a.cand || !a.next_ids || !a.parent || !a.hist_tok ||
+  if (!a.logits || !a.scores || !a.step || (a.alpha_pos >= 0 && !a.pen) || !a.done || !a.cand || !a.next_ids || !a.parent || !a.hist_tok ||
       !a.hist_back || !a.fin_score || !a.fin_n || !a.fin_src || !a.fin_count) {
     set_error("%s: null pointer", who);
     return -1;
@@ -677,6 +925,48 @@ int adapcc_beam_sample_step(const float* logits, int ld, int vocab, int B, int K
   CUDA_TRY(cudaGetLastError());
   count_launch();
   beam_sample_select_kernel<<<B, kBeamThreads, 0, s>>>(p);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  beam_step_incr_kernel<<<1, 1, 0, s>>>(step);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// stochastic beam search: adapcc_beam_sample_step's arguments without the length penalty, with scores the live beams'
+// log-probabilities, keys fp32 [B*K] their keys, cand uint64 / cand_key, cand_phi fp32 [B*K, K + 1] the offered
+// children, fin_score the finished entries' keys and fin_phi fp32 [B, K] their log-probabilities, kappa fp32 [B]
+int adapcc_beam_stochastic_step(const float* logits, int ld, int vocab, int B, int K, float* scores, float* keys,
+                                int* step, int min_new, const int* suppress, int n_suppress, const int* stop, int n_stop,
+                                int max_new, int* done, void* cand, float* cand_key, float* cand_phi,
+                                long long* next_ids, int* parent, long long* hist_tok, int* hist_back,
+                                float* fin_score, float* fin_phi, int* fin_n, int* fin_src, int* fin_count,
+                                float* kappa, float temperature, int top_k, float top_p, const long long* seeds,
+                                void* stream) {
+  BeamStochasticArgs p{BeamArgs{logits, ld, vocab, B, K, 0, scores, step, min_new, suppress, n_suppress, stop, n_stop,
+                                nullptr, -1, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
+                                hist_back, fin_score, fin_n, fin_src, fin_count, 1, nullptr, 0.f},
+                       temperature, top_p, top_k, seeds, keys, cand_key, cand_phi, fin_phi, kappa};
+  if (check_beam_args("beam_stochastic_step", p.a)) return -1;
+  if (vocab > kSampleMaxVocab || !(temperature > 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
+    set_error("beam_stochastic_step: need vocab <= %d, temperature > 0, top_k >= 0, 0 < top_p <= 1 (got %d, %g, %d, "
+              "%g)", kSampleMaxVocab, vocab, temperature, top_k, top_p);
+    return -1;
+  }
+  if (!keys || !cand_key || !cand_phi || !fin_phi || !kappa || !seeds) {
+    set_error("beam_stochastic_step: null pointer");
+    return -1;
+  }
+  p.a.N = K + 1;
+  const size_t smem = (size_t)vocab * sizeof(float);
+  if (smem > 48 * 1024)
+    CUDA_TRY(cudaFuncSetAttribute(beam_stochastic_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                  (int)smem));
+  cudaStream_t s = (cudaStream_t)stream;
+  beam_stochastic_rows_kernel<<<B * K, kSampleThreads, smem, s>>>(p);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  beam_stochastic_select_kernel<<<B, kBeamThreads, 0, s>>>(p);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   beam_step_incr_kernel<<<1, 1, 0, s>>>(step);

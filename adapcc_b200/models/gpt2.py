@@ -894,7 +894,7 @@ class GPT2DoubleHeads(nn.Module):
         the items' seeds are a device input of the graph. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
         ``ops.repeats.penalize_repeats_reference``, ``ops.beam.GroupBeamReference`` (``BeamSampleReference`` with
         ``do_sample``) and torch indexing."""
-        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB
+        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB, BeamState
         from ..ops.beam import BeamSampleReference, GroupBeamReference, best_hypotheses, merge_finished_sets
 
         K = int(num_beams)
@@ -920,10 +920,122 @@ class GPT2DoubleHeads(nn.Module):
         if len(stop_ids) > BEAM_MAX_STOP or len(suppress_ids) > BEAM_MAX_SUPPRESS:
             raise ValueError(f"beam_search: at most {BEAM_MAX_STOP} stop ids and {BEAM_MAX_SUPPRESS} suppressed ids, "
                              f"got {len(stop_ids)} and {len(suppress_ids)}")
+        def start(B, n, V, dev, native):
+            seeds = _row_seeds(seed, B, dev) if do_sample else None
+            if not native:                          # CPU / not bf16: the fp64 definition
+                if do_sample:
+                    return BeamSampleReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
+                                               temperature=temperature, top_k=top_k, top_p=top_p,
+                                               seeds=seeds.cpu().tolist())
+                return GroupBeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
+                                          num_beam_groups=G, diversity_penalty=lam)
+            if do_sample and V > SAMPLE_MAX_VOCAB:
+                raise ValueError(f"beam_search: do_sample=True needs a vocabulary of at most {SAMPLE_MAX_VOCAB} ids "
+                                 f"on the native path, got {V}")
+            st = BeamState(B, K, n, length_penalty, dev, sample=do_sample, groups=G)
+            return st, (dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds) if do_sample
+                         else dict(diversity_penalty=lam))
+
+        sel = self._beam_decode("beam_search", input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
+                                min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start)
+        dev, B, n = input_ids.device, input_ids.shape[0], int(max_new_tokens)
+        if not isinstance(sel, tuple):
+            return tuple(t.to(dev) for t in sel.result(R))
+        st = sel[0]
+        count, Kg = st.fin_count.cpu().tolist(), K // G
+        score, n_tok, src = st.fin_score.cpu().tolist(), st.fin_n.cpu().tolist(), st.fin_src.cpu().tolist()
+        fin = [merge_finished_sets([list(zip(score[b], n_tok[b], src[b]))[g * Kg:g * Kg + count[b * G + g]]
+                                    for g in range(G)]) for b in range(B)]
+        hist_tok = st.hist_tok.view(n, B, K).cpu().numpy()
+        hist_back = st.hist_back.view(n, B, K).cpu().numpy()
+        return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n, R))
+
+    @torch.no_grad()
+    def stochastic_beam_search(self, input_ids: torch.Tensor, lengths: Optional[Sequence[int]] = None,
+                               token_type_ids: Optional[torch.Tensor] = None, reply_type=None, num_beams: int = 4,
+                               max_new_tokens: int = 20, temperature: float = 1.0, top_k: int = 0,
+                               top_p: float = 1.0, stop_ids: Sequence[int] = (), suppress_ids: Sequence[int] = (),
+                               min_new_tokens: int = 0, repetition_penalty: float = 1.0,
+                               no_repeat_ngram_size: int = 0, seed=0):
+        """Stochastic beam search (Kool, van Hoof and Welling 2019): ``num_beams`` = K distinct replies per prompt,
+        drawn without replacement from the law ``generate`` samples from with the same ``temperature``, ``top_k``,
+        ``top_p``, stop / suppress / ``min_new_tokens``, repetition settings and ``max_new_tokens``; the definition
+        (rules R1-R8, properties P1-P4) is ``ops.beam.StochasticBeamReference``. The first reply of an item is itself
+        an exact sample of that law. ``seed``: an int (item b uses ``seed + b``) or an int64 [B] tensor; an item's
+        result depends on its prompt, its seed and the scalars only. The other arguments work as in ``beam_search``.
+
+        Returns ``(tokens, n_new, log_probs, keys, kappa)``: rows ``b·K + q``, the largest key first, of int64 [B·K,
+        max_new_tokens] (the stop token excluded, padded with -1), int64 [B·K] lengths, fp32 [B·K] log-probabilities
+        under the law and fp32 [B·K] perturbed keys (rows past an item's count have no tokens, length 0 and -inf),
+        and the thresholds ``kappa`` fp32 [B]. With them ``ops.beam.sbs_estimate(f, log_probs, kappa)`` is an
+        unbiased estimate of the expectation of any f of the reply (exact when kappa is -inf: then the K replies are
+        the whole support).
+
+        The decode loop is ``beam_search``'s: on CUDA with bf16 weights every token after the first replays one CUDA
+        graph of decode step, LM head, the repetition controls when on, ``ops.beam_step_`` on a stochastic
+        ``ops.BeamState`` and ``ops.kv_reorder_``; there a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids and at
+        most 64 beam rows per call. Elsewhere the same loop runs eagerly through ``StochasticBeamReference``. Bad
+        arguments raise ``ValueError`` naming them before anything is launched."""
+        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB, BeamState
+        from ..ops.beam import StochasticBeamReference, stochastic_results
+
+        who = "stochastic_beam_search"
+        K = int(num_beams)
+        if not 1 <= K <= BEAM_MAX_BEAMS:
+            raise ValueError(f"{who}: num_beams must be in [1, {BEAM_MAX_BEAMS}], got {num_beams}")
+        if not temperature > 0:
+            raise ValueError(f"{who}: temperature must be > 0, got {temperature}")
+        if int(top_k) < 0:
+            raise ValueError(f"{who}: top_k must be >= 0, got {top_k}")
+        if not 0 < top_p <= 1:
+            raise ValueError(f"{who}: top_p must be in (0, 1], got {top_p}")
+        if len(stop_ids) > BEAM_MAX_STOP:
+            raise ValueError(f"{who}: at most {BEAM_MAX_STOP} stop_ids, got {len(stop_ids)}")
+        if len(suppress_ids) > BEAM_MAX_SUPPRESS:
+            raise ValueError(f"{who}: at most {BEAM_MAX_SUPPRESS} suppress_ids, got {len(suppress_ids)}")
+        scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p)
+
+        def start(B, n, V, dev, native):
+            seeds = _row_seeds(seed, B, dev)
+            if not native:
+                return StochasticBeamReference(B, K, n, V, stop_ids, suppress_ids, min_new_tokens,
+                                               seeds=seeds.cpu().tolist(), **scalars)
+            if V > SAMPLE_MAX_VOCAB:
+                raise ValueError(f"{who}: the vocabulary (vocab_size = {V}) must be at most {SAMPLE_MAX_VOCAB} ids on "
+                                 f"the native path")
+            return BeamState(B, K, n, 1.0, dev, seeds=seeds), scalars
+
+        sel = self._beam_decode(who, input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
+                                min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start)
+        dev = input_ids.device
+        if not isinstance(sel, tuple):
+            return tuple(t.to(dev) for t in sel.result())
+        st = sel[0]
+        B, n = st.batch, st.max_new
+        count = st.fin_count.cpu().tolist()
+        cols = [x.cpu().tolist() for x in (st.fin_score, st.fin_n, st.fin_src, st.fin_phi)]
+        fin = [list(zip(*(c[b] for c in cols)))[:count[b]] for b in range(B)]
+        out = stochastic_results(fin, st.hist_tok.view(n, B, K).cpu().numpy(), st.hist_back.view(n, B, K).cpu().numpy(),
+                                 n, K, st.kappa.cpu().numpy())
+        return tuple(t.to(dev) for t in out)
+
+    def _beam_decode(self, who: str, input_ids: torch.Tensor, lengths, token_type_ids, reply_type, K: int,
+                     max_new_tokens: int, min_new_tokens: int, repetition_penalty: float, no_repeat_ngram_size: int,
+                     stop_ids: Sequence[int], suppress_ids: Sequence[int], start):
+        """The decode loop of the beam decoders. ``start(B, n, V, device, native)`` is called after the argument checks
+        and before anything is launched; it returns the selector: on the native path ``(BeamState, keyword arguments
+        of beam_step_)``, elsewhere a reference with ``step(logits) -> (next_ids, parent)`` and ``done``. Each prompt
+        is prefilled once and its keys and values copied to its K rows; every token then takes the LM head, the
+        repetition controls when on, the selection and the cache reordering. On the native path every token after
+        the first replays one CUDA graph of them and the host reads the done flags once every 8 tokens; elsewhere
+        the same loop runs eagerly with fp32 PyTorch logits and torch indexing. Returns the selector."""
+        from ..ops import beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
+
         B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
-            "beam_search", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
+            who, input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, num_beams=K)
         dev, V, weight = input_ids.device, self.cfg.vocab_size, self.wte.weight
+        sel = start(B, n, V, dev, native)
         if tt_new is not None:
             tt_new = tt_new.repeat_interleave(K)
         # one prefill per prompt, its keys and values copied to the prompt's K rows (the beams share that region)
@@ -936,15 +1048,7 @@ class GPT2DoubleHeads(nn.Module):
         del pre
         h = h.repeat_interleave(K, dim=0).contiguous()
         reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
-        seeds = _row_seeds(seed, B, dev) if do_sample else None
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
-            if do_sample:
-                ref = BeamSampleReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
-                                          temperature=temperature, top_k=top_k, top_p=top_p,
-                                          seeds=seeds.cpu().tolist())
-            else:
-                ref = GroupBeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
-                                         num_beam_groups=G, diversity_penalty=lam)
             head = weight.float()
             for i in range(n):
                 if i:
@@ -952,24 +1056,17 @@ class GPT2DoubleHeads(nn.Module):
                 logits = self.lm_logits(h, head)
                 if reps is not None:
                     logits = reps.eager(logits, cache, nxt if i else None)
-                nxt, parent = ref.step(logits)
+                nxt, parent = sel.step(logits)
                 rows = parent.to(dev)
                 cache.k.copy_(cache.k[:, rows])
                 cache.v.copy_(cache.v[:, rows])
                 if reps is not None:
                     reps.reorder(rows)
-                if ref.done.all():
+                if sel.done.all():
                     break
-            return tuple(t.to(dev) for t in ref.result(R))
+            return sel
 
-        from ..ops import BeamState, beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
-
-        if do_sample and V > SAMPLE_MAX_VOCAB:
-            raise ValueError(f"beam_search: do_sample=True needs a vocabulary of at most {SAMPLE_MAX_VOCAB} ids on the "
-                             f"native path, got {V}")
-        st = BeamState(B, K, n, length_penalty, dev, sample=do_sample, groups=G)
-        scalars = (dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds) if do_sample
-                   else dict(diversity_penalty=lam))
+        st, scalars = sel
         logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
         sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
         prompt_len = cache.lens.clone()
@@ -986,13 +1083,7 @@ class GPT2DoubleHeads(nn.Module):
         if n > 1:
             # beam_step_ writes the new beams' tokens into the graph's own input buffer
             DecodeGraph(self, cache, tt_new is not None, head=select, ids=st.next_ids, tt=tt_new).run(n - 1, st.done)
-        count, Kg = st.fin_count.cpu().tolist(), K // G
-        score, n_tok, src = st.fin_score.cpu().tolist(), st.fin_n.cpu().tolist(), st.fin_src.cpu().tolist()
-        fin = [merge_finished_sets([list(zip(score[b], n_tok[b], src[b]))[g * Kg:g * Kg + count[b * G + g]]
-                                    for g in range(G)]) for b in range(B)]
-        hist_tok = st.hist_tok.view(n, B, K).cpu().numpy()
-        hist_back = st.hist_back.view(n, B, K).cpu().numpy()
-        return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n, R))
+        return sel
 
     def _generate_speculative(self, draft: Optional["GPT2DoubleHeads"], K: int, ngram: int, input_ids, lengths,
                               token_type_ids, reply_type, max_new_tokens, temperature, top_k, top_p, stop_ids,

@@ -62,6 +62,9 @@ def _lib():
         lib.adapcc_beam_sample_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                                 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                                 + [c_void_p] * 11 + [c_float, c_int, c_float, c_void_p, c_void_p])
+        lib.adapcc_beam_stochastic_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                                     c_int, c_void_p, c_int, c_void_p, c_int, c_int]
+                                                    + [c_void_p] * 14 + [c_float, c_int, c_float, c_void_p, c_void_p])
         lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p,
                                                                                                 c_void_p]
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
@@ -498,10 +501,17 @@ class BeamState:
     ``groups`` = G > 1 (diverse beam search, ``ops.beam.GroupBeamReference``; G divides K, not with ``sample``): group g
     owns beams ``g·K/G .. (g+1)·K/G - 1``, each group's beam 0 starts at 0, the finished arrays [B, K] are read as
     [B, G, K/G] (one set per group), ``fin_count`` and ``group_done`` are int32 [B·G], and ``done`` stays the item
-    flag [B]: all of the item's groups are done."""
+    flag [B]: all of the item's groups are done.
+
+    ``seeds`` (int64 [B], each item's Philox key; not with ``sample`` or ``groups``) makes the state stochastic beam
+    search (``ops.beam.StochasticBeamReference``, rules R1-R8): ``scores`` are the live beams' log-probabilities φ,
+    ``keys`` fp32 [B·K] their perturbed keys (beam 0 starts at the Gumbel of rule R1's start, rounded to fp32),
+    ``fin_score`` holds the finished entries' keys and ``fin_phi`` fp32 [B, K] their log-probabilities, ``kappa`` fp32
+    [B] the largest key pruned so far (-inf at the start), and ``cand_key`` / ``cand_phi`` fp32 [B·K, K + 1] the
+    children each row offers, next to the first K + 1 entries of each ``cand`` row. ``length_penalty`` is unused."""
 
     def __init__(self, batch: int, num_beams: int, max_new: int, length_penalty: float, device, sample: bool = False,
-                 groups: int = 1):
+                 groups: int = 1, seeds: Optional[torch.Tensor] = None):
         B, K, n, G = int(batch), int(num_beams), int(max_new), int(groups)
         if B < 1 or not 1 <= K <= BEAM_MAX_BEAMS or n < 1:
             raise ValueError(f"BeamState: need batch >= 1, 1 <= num_beams <= {BEAM_MAX_BEAMS} and max_new >= 1, got "
@@ -509,6 +519,10 @@ class BeamState:
         if not 1 <= G <= K or K % G != 0 or (G > 1 and sample):
             raise ValueError(f"BeamState: groups must divide num_beams = {K} and cannot be combined with sample, got "
                              f"{groups} (sample={sample})")
+        if seeds is not None and (sample or G > 1 or seeds.dtype != torch.int64 or seeds.numel() != B):
+            raise ValueError(f"BeamState: seeds (stochastic beam search) must be int64 with {B} elements and cannot "
+                             f"be combined with sample or groups, got {seeds.dtype} {tuple(seeds.shape)} "
+                             f"(sample={sample}, groups={groups})")
         self.batch, self.num_beams, self.max_new, self.length_penalty = B, K, n, float(length_penalty)
         self.groups = G
         i32, dev = dict(dtype=torch.int32, device=device), device
@@ -532,12 +546,23 @@ class BeamState:
         width = (BEAM_MAX_STOP + 1) * K if self.sample else K + BEAM_MAX_STOP
         self.cand = torch.empty(B * K, width, dtype=torch.int64, device=dev)
         self.cand_c = torch.empty(B * K, width, dtype=torch.float32, device=dev) if self.sample else None
+        self.seeds = self.keys = self.fin_phi = self.kappa = self.cand_key = self.cand_phi = None
+        if seeds is not None:
+            from .beam import start_keys
+            self.seeds = seeds.reshape(B).to(dev).contiguous()
+            self.keys = torch.full((B, K), float("-inf"), dtype=torch.float32, device=dev)
+            self.keys[:, 0] = torch.from_numpy(start_keys(self.seeds.cpu().tolist())).to(dev, torch.float32)
+            self.keys = self.keys.reshape(B * K)
+            self.fin_phi = torch.full((B, K), float("-inf"), dtype=torch.float32, device=dev)
+            self.kappa = torch.full((B,), float("-inf"), dtype=torch.float32, device=dev)
+            self.cand_key = torch.empty(B * K, K + 1, dtype=torch.float32, device=dev)
+            self.cand_phi = torch.empty(B * K, K + 1, dtype=torch.float32, device=dev)
 
     def tensors(self):
         """Every device tensor of the state (what ``beam_step_`` checks for one device)."""
         return (self.scores, self.step, self.done, self.next_ids, self.parent, self.hist_tok, self.hist_back,
                 self.fin_score, self.fin_n, self.fin_src, self.fin_count, self.group_done, self.pen, self.cand,
-                self.cand_c)
+                self.cand_c, self.seeds, self.keys, self.fin_phi, self.kappa, self.cand_key, self.cand_phi)
 
 
 def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int = 0,
@@ -558,7 +583,11 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
 
     A state with ``groups`` > 1 is diverse beam search (``GroupBeamReference``): the groups select in order, a
     candidate's score lowered by ``diversity_penalty`` (finite, > 0; 0 for one group) per new beam of an earlier group
-    of the item that took its token this step."""
+    of the item that took its token this step.
+
+    A state with ``seeds`` is stochastic beam search (``StochasticBeamReference``): ``temperature > 0``, ``top_k`` and
+    ``top_p`` filter each beam's ids as ``generate``'s sampler does, the state's own seeds drive the draws (``seeds``
+    must be None) and vocab is at most ``SAMPLE_MAX_VOCAB``."""
     def bad(msg):
         raise ValueError(f"beam_step_: {msg}")
 
@@ -569,6 +598,13 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
         bad(f"a BeamState with {state.groups} groups needs a finite diversity_penalty > 0, got {diversity_penalty}")
     if state.groups == 1 and lam != 0:
         bad(f"diversity_penalty needs a BeamState with groups > 1, got {diversity_penalty}")
+    if state.seeds is not None:
+        if seeds is not None:
+            bad("a stochastic BeamState carries its items' seeds; pass seeds=None")
+        if not temperature > 0 or not int(top_k) >= 0 or not 0 < top_p <= 1:
+            bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
+        if vocab > SAMPLE_MAX_VOCAB:
+            bad(f"stochastic beam search needs vocab <= {SAMPLE_MAX_VOCAB}, got {vocab}")
     if seeds is not None:
         if not state.sample:
             bad("sampling needs a BeamState(..., sample=True)")
@@ -589,6 +625,15 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
     sup, n_sup = _id_list("beam_step_", "suppress_ids", suppress_ids, BEAM_MAX_SUPPRESS)
     stop, n_stop = _id_list("beam_step_", "stop_ids", stop_ids, BEAM_MAX_STOP)
     _same_device("beam_step_", logits.device, state.tensors() + (suppress_ids, stop_ids, seeds))
+    if state.seeds is not None:
+        _ck(_lib().adapcc_beam_stochastic_step(
+            _ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores), _ptr(state.keys), _ptr(state.step),
+            int(min_new), sup, n_sup, stop, n_stop, state.max_new, _ptr(state.done), _ptr(state.cand),
+            _ptr(state.cand_key), _ptr(state.cand_phi), _ptr(state.next_ids), _ptr(state.parent),
+            _ptr(state.hist_tok), _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_phi),
+            _ptr(state.fin_n), _ptr(state.fin_src), _ptr(state.fin_count), _ptr(state.kappa), float(temperature),
+            int(top_k), float(top_p), _ptr(state.seeds), _stream()), "beam_stochastic_step")
+        return
     if seeds is not None:
         _ck(_lib().adapcc_beam_sample_step(
             _ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores), _ptr(state.step), int(min_new), sup,

@@ -80,6 +80,48 @@ penalised, so a candidate past them ranks below at least ``K_g + n_stop`` of its
 differences from HuggingFace 4.x: the repetition controls act before the log-softmax, the done rule is the exact one,
 and done groups add no pad tokens to the Hamming counts.
 
+Stochastic beam search (``StochasticBeamReference``; Kool, van Hoof and Welling, ICML 2019, "Stochastic Beams and
+Where to Find Them") draws K distinct replies without replacement from the law ``generate`` samples from. Per item b
+there are K slots; a live slot j carries φ_j, the log-probability of its prefix, and G_j, its perturbed key. The item
+also keeps a finished set of at most K entries ``(key, φ, n, src)`` and a threshold κ_b, which starts at -inf. At the
+start slot 0 is live with φ = 0 and G_0 = the Gumbel (rule S4's transform) of word 0 of Philox4x32-10 at counter
+``(0, 0, 0, 2)`` under the item's key; the other slots are dead. At step t (L = t + 1), for every live slot j:
+
+R1. suppression below ``min_new`` is rule 1; the repetition controls act on the logits before it, as in ``generate``;
+R2. ``x_i = fl32(l_i / T)``; the kept set is the sampler's top-k, then top-p (``ops/sampling.py`` steps 4 and 6),
+    with min_keep 1: ``sample_keep(x, top_k, top_p, 1)``, the filter ``generate`` draws from;
+R3. for a kept i, ``lp'_i = (x_i - m) - log sum_kept exp(x_k - m)`` with m the largest kept x, and the child's
+    log-probability is ``φ_ji = φ_j + lp'_i``: the per-step law is ``generate``'s, renormalised over the kept ids (beam
+    sampling's ``s + lp / T`` is not renormalised; this rule differs on purpose);
+R4. ``Gφ_ji = φ_ji + Gumbel(w)``, w word ``i & 3`` of Philox at counter ``(i >> 2, j, t, 1)`` (the last counter word
+    separates this stream from beam sampling's);
+R5. ``Z_j`` = the largest Gφ_ji over the kept i; the child's key is its Gumbel truncated at G_j:
+    ``G̃_ji = G_j - max(v, 0) - log1p(exp(-|v|))`` with ``v = G_j - Gφ_ji + log1mexp(Gφ_ji - Z_j)``,
+    ``log1mexp(a) = log(-expm1(a))`` for ``a > -ln 2`` and ``log1p(-exp(a))`` otherwise. ``log1mexp(0) = -inf``, so
+    the row's best child keeps G_j exactly; in exact arithmetic ``G̃ = -log(exp(-G_j) - exp(-Z_j) + exp(-Gφ))``;
+R6. each row offers its K + 1 best children by Gφ, a tie to the lower id; G̃ is monotone in Gφ within a row, so no
+    child it does not offer could survive or be entry K + 1 of rule R7;
+R7. the item's pool is its finished set and every row's offered children, ranked by descending key; on a tie a
+    finished entry goes first, finished entries keep their set order and children go by the lower flat index
+    ``j·V + i``. The first K survive, in rank order: a surviving child whose token is a stop id enters the finished
+    set with ``n = L - 1`` tokens, φ including the stop token's lp' and ``src = j``; at ``t = max_new - 1`` every
+    other surviving child takes history slot k in rank order, as a new beam would, and enters the set with ``n =
+    max_new`` and ``src = k``; otherwise the other survivors become the new live beams in rank order (beam 0 the
+    best). ``κ_b = max(κ_b, key of pool entry K + 1)`` when it exists: by R6 this is the largest key ever pruned, since
+    a pruned node's largest descendant key is its own;
+R8. the item is done when it has no live beam. Its results are its finished set, best (largest key) first.
+
+Properties (``tests/test_stochastic_beam_cpu.py`` checks them):
+
+P1. an item's first result is distributed exactly as the reply ``generate`` draws with the same temperature, top_k,
+    top_p, stop / suppress / min_new, repetition settings and ``max_new_tokens`` (the same law, another random stream);
+P2. its results are ``min(K, |support|)`` distinct sequences, a Gumbel-top-K sample without replacement from that law;
+P3. κ = -inf if and only if the support holds at most K sequences;
+P4. ``sum over results of f · exp(φ) / q``, ``q = -expm1(-exp(φ - κ))``, is unbiased for E[f] (priority sampling;
+    Kool et al. §4); with κ = -inf, q = 1 and the sum is exact (``sbs_estimate``).
+
+An item's result depends on its prompt, its seed and the scalars only.
+
 ``best_hypotheses(..., num_return_sequences=r)`` returns each item's first r finished hypotheses, best first, as rows
 ``b · r + q`` (HuggingFace's flattening); rows past an item's count have no tokens, ``n_new`` 0 and score -inf.
 """
@@ -203,15 +245,15 @@ class BeamReference:
         return best_hypotheses(self.fin, self.hist_tok, self.hist_back, self.max_new, num_return_sequences)
 
 
-def offer_finished(fin: List[Tuple[float, int, int]], cap: int, score: float, n: int, src: int) -> None:
-    """Rule 6 on one finished set ``fin`` (best first) of at most ``cap`` hypotheses: ``(score, n, src)`` goes in
-    after every entry with a score >= its own, unless the set is full and it does not beat the worst."""
+def offer_finished(fin: List[Tuple[float, int, int]], cap: int, score: float, n: int, src: int, *extra) -> None:
+    """Rule 6 on one finished set ``fin`` (best first) of at most ``cap`` hypotheses: ``(score, n, src, *extra)`` goes
+    in after every entry with a score >= its own, unless the set is full and it does not beat the worst."""
     if len(fin) == cap and not score > fin[-1][0]:
         return
     p = len(fin)
     while p > 0 and fin[p - 1][0] < score:
         p -= 1
-    fin.insert(p, (score, n, src))
+    fin.insert(p, (score, n, src) + extra)
     del fin[cap:]
 
 
@@ -478,3 +520,136 @@ def best_hypotheses(fin, hist_tok, hist_back, max_new: int,
                 r = int(hist_back[u, b, r])
             n_new[row], scores[row] = int(n), float(score)
     return tokens, n_new, scores
+
+
+def start_keys(seeds: Sequence[int]) -> np.ndarray:
+    """Rule R1's start: each item's G_0, the Gumbel of word 0 of Philox at counter ``(0, 0, 0, 2)``, in fp64."""
+    return np.array([gumbel(philox_words(np.zeros(1, dtype=np.int64), 0, 0, 2, s)[0, 0]) for s in seeds])
+
+
+def truncated_gumbel(G: float, gphi: np.ndarray, Z: float) -> np.ndarray:
+    """Rule R5 in fp64: the keys of children with perturbed log-probabilities ``gphi`` (their largest ``Z``) of a beam
+    with key ``G``."""
+    a = np.asarray(gphi, dtype=np.float64) - Z
+    with np.errstate(divide="ignore", invalid="ignore"):
+        l1m = np.where(a > -np.log(2.0), np.log(-np.expm1(a)), np.log1p(-np.exp(a)))
+    v = G - gphi + l1m
+    return G - np.maximum(v, 0.0) - np.log1p(np.exp(-np.abs(v)))
+
+
+class StochasticBeamReference(BeamReference):
+    """Stochastic beam search (rules R1-R8, see the module docstring) for ``batch`` items in fp64, with the interface of
+    ``BeamReference``. ``scores`` [B, K] are the live beams' φ, ``keys`` [B, K] their keys G, ``fin[b]`` item b's
+    finished set as ``(key, n, src, φ)``, best first, and ``kappa`` [B] the thresholds. ``seeds``: one int per item;
+    ``temperature > 0`` and ``top_p`` are rounded to fp32, as the kernels take them; ``top_k = 0`` is off."""
+
+    def __init__(self, batch: int, num_beams: int, max_new: int, vocab: int, stop_ids: Sequence[int] = (),
+                 suppress_ids: Sequence[int] = (), min_new: int = 0, temperature: float = 1.0, top_k: int = 0,
+                 top_p: float = 1.0, seeds: Sequence[int] = ()):
+        super().__init__(batch, num_beams, max_new, vocab, 1.0, stop_ids, suppress_ids, min_new)
+        if not temperature > 0 or int(top_k) < 0 or not 0 < top_p <= 1:
+            raise ValueError(f"StochasticBeamReference: need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got "
+                             f"{temperature}, {top_k}, {top_p}")
+        self.seeds = [int(x) for x in seeds]
+        if len(self.seeds) != self.B:
+            raise ValueError(f"StochasticBeamReference: need {self.B} seeds, got {len(self.seeds)}")
+        self.T = float(np.float32(temperature))
+        self.top_k, self.top_p = int(top_k), float(top_p)
+        self.keys = np.full((self.B, self.K), -np.inf)
+        self.keys[:, 0] = start_keys(self.seeds)
+        self.kappa = np.full(self.B, -np.inf)
+
+    def children(self, b: int, j: int, logits_row: np.ndarray, step: int):
+        """Rules R1-R6 for beam row j of item b: ``(ids, phi, gphi, key)`` of the children it offers, by descending
+        Gφ (a tie to the lower id); empty for a dead beam."""
+        empty = np.zeros(0, dtype=np.int64), np.zeros(0), np.zeros(0), np.zeros(0)
+        x = (np.array(logits_row[:self.vocab], dtype=np.float32) / np.float32(self.T)).astype(np.float32)
+        if step < self.min_new and self.suppress.size:
+            x[self.suppress] = -np.inf
+        if not np.isfinite(self.scores[b, j]) or not (x > -np.inf).any():
+            return empty
+        ids = np.flatnonzero(sample_keep(x, self.top_k, self.top_p, 1))
+        xd = x[ids].astype(np.float64)
+        m = xd.max()
+        phi = self.scores[b, j] + ((xd - m) - np.log(np.exp(xd - m).sum()))
+        w = philox_words(ids >> 2, j, step, 1, self.seeds[b])[np.arange(ids.size), ids & 3]
+        gphi = phi + gumbel(w)
+        order = np.lexsort((ids, -gphi))[:self.K + 1]
+        return ids[order], phi[order], gphi[order], truncated_gumbel(self.keys[b, j], gphi[order], gphi.max())
+
+    def step(self, logits) -> Tuple[torch.Tensor, torch.Tensor]:
+        """One step (rules R1-R8) for every item that is not done."""
+        if isinstance(logits, torch.Tensor):
+            logits = logits.detach().float().cpu().numpy()
+        B, K, V = self.B, self.K, self.vocab
+        step = self.n_steps
+        if step >= self.max_new:
+            raise ValueError(f"StochasticBeamReference: all {self.max_new} steps taken")
+        nxt = np.zeros(B * K, dtype=np.int64)
+        parent = np.arange(B * K, dtype=np.int64)
+        L, last = step + 1, step == self.max_new - 1
+        for b in range(B):
+            if self.done[b]:
+                continue
+            # pool entries (key, tie order, payload): finished entries first on a tie, then children by flat index
+            pool = [(f[0], q, f) for q, f in enumerate(self.fin[b])]
+            for j in range(K):
+                ids, phi, _, key = self.children(b, j, logits[b * K + j], step)
+                pool += [(float(key[e]), K + j * V + int(ids[e]), (j, int(ids[e]), float(phi[e])))
+                         for e in range(ids.size)]
+            pool.sort(key=lambda t: (-t[0], t[1]))
+            if len(pool) > K:
+                self.kappa[b] = max(self.kappa[b], pool[K][0])
+            fin, beams = [], []
+            for key, order, payload in pool[:K]:
+                if order < K:
+                    offer_finished(fin, K, *payload)
+                    continue
+                j, i, phi = payload
+                if i in self.stop:
+                    offer_finished(fin, K, key, L - 1, j, phi)
+                    continue
+                if last:
+                    offer_finished(fin, K, key, self.max_new, len(beams), phi)
+                beams.append((key, j, i, phi))
+            self.fin[b] = fin
+            self.scores[b], self.keys[b] = -np.inf, -np.inf
+            for k in range(K):
+                if k < len(beams):
+                    key, j, i, phi = beams[k]
+                    self.hist_tok[step, b, k], self.hist_back[step, b, k] = i, j
+                    if not last:
+                        self.scores[b, k], self.keys[b, k] = phi, key
+                        nxt[b * K + k], parent[b * K + k] = i, b * K + j
+                else:
+                    self.hist_tok[step, b, k], self.hist_back[step, b, k] = -1, k
+            self.done[b] = last or not beams
+        self.n_steps += 1
+        return torch.from_numpy(nxt), torch.from_numpy(parent)
+
+    def result(self):
+        """``stochastic_results`` of the finished sets: ``(tokens, n_new, log_probs, keys, kappa)``."""
+        return stochastic_results(self.fin, self.hist_tok, self.hist_back, self.max_new, self.K, self.kappa)
+
+
+def stochastic_results(fin, hist_tok, hist_back, max_new: int, K: int, kappa):
+    """Each item's finished set ``(key, n, src, φ)`` (best first) as ``(tokens, n_new, log_probs, keys, kappa)``: rows
+    ``b·K + q`` of int64 [B·K, max_new] padded with -1, int64 [B·K], fp32 [B·K] twice (rows past an item's count: no
+    tokens, 0 and -inf), and fp32 [B]."""
+    tokens, n_new, keys = best_hypotheses([[f[:3] for f in fb] for fb in fin], hist_tok, hist_back, max_new, K)
+    _, _, log_probs = best_hypotheses([[(f[3], f[1], f[2]) for f in fb] for fb in fin], hist_tok, hist_back, max_new,
+                                      K)
+    return tokens, n_new, log_probs, keys, torch.as_tensor(np.asarray(kappa, dtype=np.float32))
+
+
+def sbs_estimate(values: torch.Tensor, log_probs: torch.Tensor, kappa: torch.Tensor) -> torch.Tensor:
+    """Property P4: per item, ``sum_q f_q · exp(φ_q) / q_q`` with ``q = -expm1(-exp(φ - κ))``, an unbiased estimate of
+    E[f] under the reply law (exact when κ = -inf). ``values`` and ``log_probs`` are [B·K] (or [B, K]) in the row order
+    of ``stochastic_beam_search``, ``kappa`` [B]; rows with φ = -inf count for nothing. Returns fp64 [B]."""
+    kappa = kappa.double().reshape(-1)
+    phi = log_probs.double().reshape(kappa.numel(), -1)
+    f = values.double().reshape(phi.shape)
+    live = phi > float("-inf")
+    q = -torch.expm1(-torch.exp(phi - kappa[:, None]))
+    w = torch.where(live, torch.exp(phi) / torch.where(live, q, torch.ones_like(q)), torch.zeros_like(q))
+    return (torch.where(live, f, torch.zeros_like(f)) * w).sum(1)

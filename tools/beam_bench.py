@@ -22,6 +22,10 @@ fallback) and writes nothing into the repository.
   beams, G = 1 / 2 / 4 / 8 and 128-token prompts, ms per generated token as in ``search`` (no stop ids, so every call
   runs all 64 tokens), the four alternated run by run; and ``beam_step_`` alone at 64 rows (vocab 50257) with G = 1
   against G = 8, timed as in ``kernels``.
+* ``stochastic``: ``stochastic_beam_search(top_k=50)`` against ``beam_search(do_sample=True, top_k=50)`` for B = 8
+  items, K = 8 beams and 128-token prompts, ms per generated token as in ``sampled`` (no stop ids, 64 new tokens),
+  the two alternated run by run; and the stochastic ``beam_step_`` (its rows and select kernels, temperature 1, no
+  top-k) alone at 64 rows (vocab 50257), timed as in ``kernels``.
 
 Usage: ``python tools/beam_bench.py [--reps 3] [--launches 1000]``
 """
@@ -141,6 +145,37 @@ def bench_groups(model, reps, launches):
     return out
 
 
+def bench_stochastic(model, reps, launches):
+    from adapcc_b200.ops import BeamState, beam_step_
+
+    B, K, T = 8, 8, 128
+    g = torch.Generator(device="cuda").manual_seed(7)
+    prompt = torch.randint(0, model.cfg.vocab_size, (B, T), device="cuda", generator=g)
+    runs = {"stochastic": lambda: model.stochastic_beam_search(prompt, num_beams=K, max_new_tokens=NEW_TOKENS,
+                                                                top_k=50, seed=3),
+            "beam_sample": lambda: model.beam_search(prompt, num_beams=K, max_new_tokens=NEW_TOKENS, do_sample=True,
+                                                     temperature=1.0, top_k=50, seed=3)}
+    times = {k: [] for k in runs}
+    for fn in runs.values():
+        fn()                                                       # warm-up of this shape
+    for _ in range(reps):
+        for k, fn in runs.items():
+            torch.cuda.synchronize()
+            t0 = time.perf_counter()
+            fn()
+            torch.cuda.synchronize()
+            times[k].append((time.perf_counter() - t0) * 1e3)
+    out = {"batch": B, "beams": K, "prompt": T, "top_k": 50,
+           "ms_per_token": {k: round(statistics.median(v) / NEW_TOKENS, 3) for k, v in times.items()}}
+    V = 50257
+    logits = torch.randn(B * K, model.wte.weight.shape[0], device="cuda", generator=g) * 3
+    st = BeamState(B, K, launches + 4 * GRAPH_LAUNCHES, 1.0, "cuda", seeds=torch.arange(B, dtype=torch.int64))
+    st.scores.zero_()                                              # every beam live, so no item finishes
+    st.keys.zero_()
+    out["stochastic_step_us"] = round(_graph_us(lambda: beam_step_(logits, V, st), launches), 2)
+    return out
+
+
 def _graph_us(fn, launches):
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
@@ -219,7 +254,8 @@ def main():
     model = GPT2DoubleHeads(GPT2Config()).to(device="cuda", dtype=torch.bfloat16).eval()
     result = dict(info, new_tokens=NEW_TOKENS, kernels=bench_kernels(model, args.launches),
                   search=bench_search(model, args.reps), sampled=bench_sampled(model, args.reps),
-                  groups=bench_groups(model, args.reps, args.launches))
+                  groups=bench_groups(model, args.reps, args.launches),
+                  stochastic=bench_stochastic(model, args.reps, args.launches))
     print(json.dumps(result))
 
 

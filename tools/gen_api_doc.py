@@ -22,7 +22,9 @@ MODULES = [
                                   "check_filter_args"]),
     ("adapcc_b200.ops.dropout", ["DropoutState", "dropout", "dropout_mask", "dropout_reference", "threshold"]),
     ("adapcc_b200.ops.beam", ["BeamReference", "BeamSampleReference", "GroupBeamReference", "best_hypotheses",
-                              "merge_finished_sets", "offer_finished", "sample_keep", "philox_words", "gumbel"]),
+                              "merge_finished_sets", "offer_finished", "sample_keep", "philox_words", "gumbel",
+                              "StochasticBeamReference", "stochastic_results", "sbs_estimate", "truncated_gumbel",
+                              "start_keys"]),
     ("adapcc_b200.ops.contrastive", ["candidates_row", "max_cosine", "rerank_row", "select_candidates",
                                      "check_contrastive_args"]),
     ("adapcc_b200.ops.lookup", ["draft_row", "greedy_token", "accept_row", "lookup_draft", "lookup_accept",
