@@ -15,23 +15,27 @@
 //                 buffer (gather, then scatter), so cycles and many-to-one parent maps come out right.
 //
 // Beam sampling (HuggingFace's do_sample=True with num_beams > 1) replaces the first two:
-//   beam_sample_rows   : one 1024-thread CTA per beam row, the row's x_i = l_i / T in shared memory. m and log Z as
-//                        beam_rows computes them, then the sampler's top-k / top-p filter (sample_filter.cuh) with a
-//                        minimum keep count, then c_i = s + lp_i / T and the Gumbel key g_i = c_i + G_i of every kept
-//                        id, G_i from the item's Philox stream. The row's M best keys (a bisection for the M-th key,
-//                        then a rank sort) are kept, with their c next to them.
+//   beam_sample_rows   : one 1024-thread CTA per beam row, the row's x_i = l_i / T in shared memory (the sampler's
+//                        row_prologue, sample_filter.cuh). m and log Z as beam_rows computes them, then the sampler's
+//                        top-k / top-p filter with a minimum keep count, then c_i = s + lp_i / T and the Gumbel key
+//                        g_i = c_i + G_i of every kept id, G_i from the item's Philox stream (gumbel_row). The row's M
+//                        best keys (a bisection for the M-th key, then a rank sort) are kept, with their c next to them.
 //   beam_sample_select : one 512-thread CTA per item. Each key's place in the item's draw order is its place in its
 //                        row plus, per other row, a binary search for the larger keys; the first M form the sample.
 //                        The first K draws that finish are offered, and the K best-c draws that do not are the new
 //                        beams (DESIGN.md §4a).
 //
 // Stochastic beam search (Kool et al. 2019; rules R1-R8 of ops/beam.py) replaces them too:
-//   beam_stochastic_rows   : one 1024-thread CTA per beam row, x_i = l_i / T in shared memory. The sampler's filter
-//                            (min_keep 1), log Z over the kept ids, then phi_i = phi + lp'_i and Gphi_i = phi_i + G_i
-//                            of every kept id; the K + 1 best Gphi (row_best_keys, shared with beam_sample_rows) are
-//                            offered with their keys truncated at the beam's key G and their phi.
+//   beam_stochastic_rows   : one 1024-thread CTA per beam row, x_i = l_i / T in shared memory (row_prologue). The
+//                            sampler's filter (min_keep 1), log Z over the kept ids, then phi_i = phi + lp'_i and
+//                            Gphi_i = phi_i + G_i of every kept id (gumbel_row, its own Philox counter word); the K + 1
+//                            best Gphi (row_best_keys, shared with beam_sample_rows) are offered with their keys
+//                            truncated at the beam's key G and their phi.
 //   beam_stochastic_select : one 512-thread CTA per item. Every entry of the pool (finished set, offered children) is
 //                            ranked by counting; the K first survive, entry K + 1 raises kappa.
+//
+// The three select kernels write their rows' outputs through one write_beam, and the three step entry points make
+// their launches through one launch_beam_step.
 //
 // Every fp32 sum runs in an order fixed by the thread layout (per-thread loops in id order, shuffle trees, warp partials
 // added by a shuffle tree in warp order); an item's result depends only on its own rows. ops/beam.py evaluates the same
@@ -171,6 +175,20 @@ struct FinishedSet {
   }
 };
 
+// Beam k of item b at this step. With `hist` its history slot records token tok from beam par (0..K-1), else -1 and
+// the beam itself. With `live` (implies hist) the row continues beam par with tok and the score sc; else it is dead:
+// token 0, its own cache, -inf.
+__device__ __forceinline__ void write_beam(const BeamArgs& a, int b, int k, int step, bool hist, bool live, int tok,
+                                           int par, float sc) {
+  const int r = b * a.K + k;
+  const long long h = (long long)step * (a.B * a.K) + r;
+  a.hist_tok[h] = hist ? tok : -1;
+  a.hist_back[h] = hist ? par : k;
+  a.next_ids[r] = live ? tok : 0;
+  a.parent[r] = live ? b * a.K + par : r;
+  a.scores[r] = live ? sc : -INFINITY;
+}
+
 // One warp per item; the groups in order g = 0 .. G-1. A candidate whose token the earlier groups' new beams of this
 // step took n > 0 times is re-keyed with c' = fl32(c - fl32(lambda * n)); n = 0 keeps c's key, so group 0 selects as
 // plain beam search with K = Kg. The rows' N = K + n_stop unpenalised best suffice: at most K - Kg tokens are
@@ -180,7 +198,7 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const __grid_constant__
   __shared__ FinishedSet fs;
   __shared__ int s_tok[kBeamMaxK], s_par[kBeamMaxK], s_taken[kBeamMaxK];
   __shared__ float s_sc[kBeamMaxK];
-  const int b = blockIdx.x, lane = threadIdx.x, K = a.K, N = a.N, V = a.vocab, BK = a.B * a.K, G = a.G, Kg = K / G;
+  const int b = blockIdx.x, lane = threadIdx.x, K = a.K, N = a.N, V = a.vocab, G = a.G, Kg = K / G;
   const int step = *a.step;
   // the done groups, one bit each, read next to the item's flag so that the loads overlap
   const unsigned g_done = __ballot_sync(0xffffffffu, lane < G && a.group_done[b * G + lane]);
@@ -255,24 +273,11 @@ __global__ void __launch_bounds__(32) beam_select_kernel(const __grid_constant__
     n_taken += nb;                                    // this step's new beams count, even if the group is now done
     __syncwarp();
     fs.store(a, fo, gi, lane);
-    if (lane < Kg) {
-      const int r = fo + lane;
-      const long long h = (long long)step * BK + r;
-      if (lane < nb) {
-        a.next_ids[r] = s_tok[lane];
-        a.parent[r] = b * K + s_par[lane];
-        // a done group's beams are dead from now on; with one group the item's done flag stops beam_rows_kernel
-        a.scores[r] = done && G > 1 ? -INFINITY : s_sc[lane];
-        a.hist_tok[h] = s_tok[lane];
-        a.hist_back[h] = s_par[lane];
-      } else {                                        // fewer than Kg finite non-stop candidates: a dead beam
-        a.next_ids[r] = 0;
-        a.parent[r] = r;
-        a.scores[r] = -INFINITY;
-        a.hist_tok[h] = -1;
-        a.hist_back[h] = j0 + lane;
-      }
-    }
+    // fewer than Kg finite non-stop candidates leave dead beams; a done group's beams are dead from now on, and with
+    // one group the item's done flag stops beam_rows_kernel
+    if (lane < Kg)
+      write_beam(a, b, j0 + lane, step, lane < nb, lane < nb, s_tok[lane], s_par[lane],
+                 done && G > 1 ? -INFINITY : s_sc[lane]);
     __syncwarp();
   }
   if (lane == 0) a.done[b] = all_done;
@@ -296,6 +301,34 @@ __device__ __forceinline__ float beam_gumbel(uint32_t w) {
   const float nlu = k < (1u << 23) ? -logf((float)(2u * k + 1u) * 0x1p-25f)
                                    : -log1pf(-(float)((1u << 25) - 2u * k - 1u) * 0x1p-25f);
   return -logf(nlu);
+}
+
+// The Gumbel pass of the sampled row kernels over the row x in s_x: each kept id (f2key(x_i) >= tau) becomes
+// score(i) + G_i, every other id -inf. Ids 4q..4q+3 take the four words of Philox at counter (q, j, step, c3) under
+// the item's seed, one call per four ids of which one is kept; c3 is 0 for beam sampling, 1 for stochastic beam
+// search. Every x is read before the call; the row is complete for every thread after it.
+template <class Score>
+__device__ __forceinline__ void gumbel_row(float* s_x, int V, uint32_t tau, long long seed, int j, int step,
+                                           uint32_t c3, Score score) {
+  const uint32_t k0 = (uint32_t)(unsigned long long)seed, k1 = (uint32_t)((unsigned long long)seed >> 32);
+  for (int q = threadIdx.x; q < (V + 3) / 4; q += kSampleThreads) {
+    bool kept[4], any = false;
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int i = 4 * q + e;
+      kept[e] = i < V && f2key(s_x[i]) >= tau;
+      any |= kept[e];
+    }
+    uint4 w = make_uint4(0u, 0u, 0u, 0u);
+    if (any) w = philox4((uint32_t)q, (uint32_t)j, (uint32_t)step, c3, k0, k1);
+    const uint32_t words[4] = {w.x, w.y, w.z, w.w};
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+      const int i = 4 * q + e;
+      if (i < V) s_x[i] = kept[e] ? score(i) + beam_gumbel(words[e]) : -INFINITY;
+    }
+  }
+  __syncthreads();
 }
 
 // The M best keys f2key(s_x[i]) of a row of 1024 threads (all finite ones when there are at most M; else those above
@@ -383,15 +416,8 @@ __global__ void __launch_bounds__(kSampleThreads, 1) beam_sample_rows_kernel(con
   }
   const int step = *a.step;
   const float* l = a.logits + (long long)row * a.ld;
-  for (int i = tid; i < V; i += kSampleThreads) s_x[i] = __fdiv_rn(__ldg(l + i), p.temperature);
-  __syncthreads();
-  if (step < a.min_new) {
-    for (int q = tid; q < a.n_suppress; q += kSampleThreads) {
-      const int id = a.suppress[q];
-      if (id >= 0 && id < V) s_x[id] = -INFINITY;
-    }
-    __syncthreads();
-  }
+  unsigned long long best;
+  const int present = row_prologue(s_x, sm, l, V, p.temperature, step, a.min_new, a.suppress, a.n_suppress, best);
   // m and log Z over the remaining ids, by the first 512 threads in beam_rows' order (the same bits)
   float m = -INFINITY;
   if (tid < kBeamThreads)
@@ -404,47 +430,17 @@ __global__ void __launch_bounds__(kSampleThreads, 1) beam_sample_rows_kernel(con
   }
   float z = 0.f;
   if (tid < kBeamThreads)
+#pragma unroll 2                                      // the prologue's count and maximum stay live: 4 costs 2 registers
     for (int i = tid; i < V; i += kBeamThreads)
       if (s_x[i] != -INFINITY) z += expf(__ldg(l + i) - m);
   z = beam_block_sum(s_red, z);
   const float lz = logf(z);
   auto cand_score = [&](int i) { return s + __fdiv_rn((__ldg(l + i) - m) - lz, p.temperature); };
   // the sampler's filter on x, keeping at least min_keep values
-  unsigned long long best = 0;
-  int present = 0, z1 = 0, z2 = 0;
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const uint32_t k = f2key(s_x[i]);
-    if (k > kNegInfKey) {
-      ++present;
-      best = max(best, (unsigned long long)k);
-    }
-  }
-  best = block_max(sm, best);
-  float fz = 0.f;
-  block_sum(sm, fz, present, z1, z2);
-  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, p.min_keep, present, (uint32_t)best,
-                               key2f((uint32_t)best));
+  const uint32_t mkey = (uint32_t)(best >> 32);
+  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, p.min_keep, present, mkey, key2f(mkey));
   __syncthreads();                                    // every x is read before the row becomes the keys
-  // g_i = c_i + G_i; ids 4q..4q+3 take the four words of Philox at counter (q, j, step, 0)
-  const uint32_t k0 = (uint32_t)(unsigned long long)p.seeds[b], k1 = (uint32_t)((unsigned long long)p.seeds[b] >> 32);
-  for (int q = tid; q < (V + 3) / 4; q += kSampleThreads) {
-    bool kept[4], any = false;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int i = 4 * q + e;
-      kept[e] = i < V && f2key(s_x[i]) >= tau;
-      any |= kept[e];
-    }
-    uint4 w = make_uint4(0u, 0u, 0u, 0u);
-    if (any) w = philox4((uint32_t)q, (uint32_t)j, (uint32_t)step, 0u, k0, k1);
-    const uint32_t words[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int i = 4 * q + e;
-      if (i < V) s_x[i] = kept[e] ? cand_score(i) + beam_gumbel(words[e]) : -INFINITY;
-    }
-  }
-  __syncthreads();
+  gumbel_row(s_x, V, tau, p.seeds[b], j, step, 0u, cand_score);   // g_i = c_i + G_i
   row_best_keys(s_x, sm, V, M, s_sel, &s_n, [&](int r, unsigned long long v) {
     out[r] = v;
     if (v) out_c[r] = cand_score((int)(0xFFFFFFFFu - (uint32_t)v));
@@ -459,7 +455,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_sample_select_kernel(const 
   __shared__ int s_beam[kBeamMaxK];                   // new beam k -> draw
   __shared__ FinishedSet fs;
   const BeamArgs& a = p.a;
-  const int b = blockIdx.x, tid = threadIdx.x, K = a.K, M = a.N, V = a.vocab, BK = a.B * a.K;
+  const int b = blockIdx.x, tid = threadIdx.x, K = a.K, M = a.N, V = a.vocab;
   const int step = *a.step;
   if (a.done[b] || step >= a.max_new) {               // nothing moves: every row keeps its own cache
     if (tid < K) a.parent[b * K + tid] = b * K + tid;
@@ -536,21 +532,10 @@ __global__ void __launch_bounds__(kBeamThreads) beam_sample_select_kernel(const 
     }
   }
   if (tid < K) {
-    const int r = b * K + tid;
-    const long long h = (long long)step * BK + r;
     const int e = last ? s_draw[tid] : (s_beam[tid] >= 0 ? s_draw[s_beam[tid]] : -1);
     // the last step has no live beams; its history slot k holds draw k, which an offer may point at
-    a.hist_tok[h] = e >= 0 ? token(e) : -1;
-    a.hist_back[h] = e >= 0 ? e / M : tid;
-    if (e >= 0 && !last) {
-      a.next_ids[r] = token(e);
-      a.parent[r] = b * K + e / M;
-      a.scores[r] = s_c[e];
-    } else {
-      a.next_ids[r] = 0;
-      a.parent[r] = r;
-      a.scores[r] = -INFINITY;
-    }
+    if (e >= 0) write_beam(a, b, tid, step, true, !last, token(e), e / M, s_c[e]);
+    else write_beam(a, b, tid, step, false, false, 0, 0, 0.f);
   }
   __syncthreads();
   if (tid == 0) a.done[b] = last || s_beam[0] < 0 || fs.done_rule(a, s_c[s_draw[s_beam[0]]], L);
@@ -593,34 +578,16 @@ beam_stochastic_rows_kernel(const __grid_constant__ BeamStochasticArgs p) {
   }
   const int step = *a.step;
   const float* l = a.logits + (long long)row * a.ld;
-  for (int i = tid; i < V; i += kSampleThreads) s_x[i] = __fdiv_rn(__ldg(l + i), p.temperature);
-  __syncthreads();
-  if (step < a.min_new) {
-    for (int q = tid; q < a.n_suppress; q += kSampleThreads) {
-      const int id = a.suppress[q];
-      if (id >= 0 && id < V) s_x[id] = -INFINITY;
-    }
-    __syncthreads();
-  }
-  unsigned long long best = 0;
-  int present = 0, z1 = 0, z2 = 0;
-  float fz = 0.f;
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const uint32_t k = f2key(s_x[i]);
-    if (k > kNegInfKey) {
-      ++present;
-      best = max(best, (unsigned long long)k);
-    }
-  }
-  best = block_max(sm, best);
-  block_sum(sm, fz, present, z1, z2);
+  unsigned long long best;
+  const int present = row_prologue(s_x, sm, l, V, p.temperature, step, a.min_new, a.suppress, a.n_suppress, best);
   if (present == 0) {                                 // every id removed or at -inf
     if (tid < N) out[tid] = 0ull;
     return;
   }
   // the sampler's filter (min_keep 1), then log Z over the kept ids: lp'_i = (x_i - m) - log Z
-  const float m = key2f((uint32_t)best);
-  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, 1, present, (uint32_t)best, m);
+  const uint32_t mkey = (uint32_t)(best >> 32);
+  const float m = key2f(mkey);
+  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, 1, present, mkey, m);
   float z = 0.f;
   int u0 = 0, u1 = 0, u2 = 0;
   for (int i = tid; i < V; i += kSampleThreads) {
@@ -630,26 +597,7 @@ beam_stochastic_rows_kernel(const __grid_constant__ BeamStochasticArgs p) {
   block_sum(sm, z, u0, u1, u2);                       // its barriers order every read of x before the writes below
   const float lz = logf(z);
   auto child_phi = [&](int i) { return phi + ((__fdiv_rn(__ldg(l + i), p.temperature) - m) - lz); };
-  // Gphi_i = phi_i + G_i; ids 4q..4q+3 take the four words of Philox at counter (q, j, step, 1)
-  const uint32_t k0 = (uint32_t)(unsigned long long)p.seeds[b], k1 = (uint32_t)((unsigned long long)p.seeds[b] >> 32);
-  for (int q = tid; q < (V + 3) / 4; q += kSampleThreads) {
-    bool kept[4], any = false;
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int i = 4 * q + e;
-      kept[e] = i < V && f2key(s_x[i]) >= tau;
-      any |= kept[e];
-    }
-    uint4 w = make_uint4(0u, 0u, 0u, 0u);
-    if (any) w = philox4((uint32_t)q, (uint32_t)j, (uint32_t)step, 1u, k0, k1);
-    const uint32_t words[4] = {w.x, w.y, w.z, w.w};
-#pragma unroll
-    for (int e = 0; e < 4; ++e) {
-      const int i = 4 * q + e;
-      if (i < V) s_x[i] = kept[e] ? child_phi(i) + beam_gumbel(words[e]) : -INFINITY;
-    }
-  }
-  __syncthreads();
+  gumbel_row(s_x, V, tau, p.seeds[b], j, step, 1u, child_phi);    // Gphi_i = phi_i + G_i
   // the K + 1 best children by Gphi, each with its key truncated at G: G - softplus(v),
   // v = G - Gphi + log1mexp(Gphi - Zj), Zj the row's largest Gphi (its child keeps G exactly)
   const float G = p.keys[row];
@@ -685,7 +633,7 @@ __global__ void __launch_bounds__(kBeamThreads) beam_stochastic_select_kernel(
   __shared__ float s_phi[kBeamMaxK], s_key[kBeamMaxK];
   __shared__ int s_nb;
   const BeamArgs& a = p.a;
-  const int b = blockIdx.x, tid = threadIdx.x, K = a.K, N = a.N, V = a.vocab, BK = a.B * a.K, P = K + K * N;
+  const int b = blockIdx.x, tid = threadIdx.x, K = a.K, N = a.N, V = a.vocab, P = K + K * N;
   const int step = *a.step;
   if (a.done[b] || step >= a.max_new) {               // nothing moves: every row keeps its own cache
     if (tid < K) a.parent[b * K + tid] = b * K + tid;
@@ -766,21 +714,9 @@ __global__ void __launch_bounds__(kBeamThreads) beam_stochastic_select_kernel(
   nw.store(a, b * K, b, tid);
   if (tid < K) {
     p.fin_phi[b * K + tid] = s_nphi[tid];
-    const int r = b * K + tid, nb = s_nb;
-    const long long h = (long long)step * BK + r;
-    a.hist_tok[h] = tid < nb ? s_tok[tid] : -1;
-    a.hist_back[h] = tid < nb ? s_par[tid] : tid;
-    if (tid < nb && !last) {
-      a.next_ids[r] = s_tok[tid];
-      a.parent[r] = b * K + s_par[tid];
-      a.scores[r] = s_phi[tid];
-      p.keys[r] = s_key[tid];
-    } else {
-      a.next_ids[r] = 0;
-      a.parent[r] = r;
-      a.scores[r] = -INFINITY;
-      p.keys[r] = -INFINITY;
-    }
+    const bool live = tid < s_nb && !last;
+    write_beam(a, b, tid, step, tid < s_nb, live, s_tok[tid], s_par[tid], s_phi[tid]);
+    p.keys[b * K + tid] = live ? s_key[tid] : -INFINITY;
   }
 }
 
@@ -845,6 +781,36 @@ static int check_beam_args(const char* who, const BeamArgs& a) {
   return 0;
 }
 
+// the sampled modes' scalars, and the vocabulary their row kernels hold in shared memory
+static int check_sampling_args(const char* who, int vocab, float temperature, int top_k, float top_p) {
+  if (vocab > kSampleMaxVocab || !(temperature > 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
+    set_error("%s: need vocab <= %d, temperature > 0, top_k >= 0, 0 < top_p <= 1 (got %d, %g, %d, %g)", who,
+              kSampleMaxVocab, vocab, temperature, top_k, top_p);
+    return -1;
+  }
+  return 0;
+}
+
+// One step on the stream: `rows` with a CTA of `rows_threads` per beam row and `smem` bytes of dynamic shared memory
+// (opted in above the default 48 KB), `select` with a CTA of `select_threads` per item, then the step increment.
+template <class Args>
+static int launch_beam_step(const BeamArgs& a, const Args& p, void (*rows)(Args), int rows_threads, size_t smem,
+                            void (*select)(Args), int select_threads, void* stream) {
+  if (smem > 48 * 1024)
+    CUDA_TRY(cudaFuncSetAttribute(rows, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  cudaStream_t s = (cudaStream_t)stream;
+  rows<<<a.B * a.K, rows_threads, smem, s>>>(p);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  select<<<a.B, select_threads, 0, s>>>(p);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  beam_step_incr_kernel<<<1, 1, 0, s>>>(a.step);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
 }  // namespace adapcc
 
 using namespace adapcc;
@@ -877,19 +843,7 @@ int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, int G
     set_error("beam_step: suppression needs vocab <= %d (got %d)", 200 * 1024 * 8, vocab);
     return -1;
   }
-  if (bits > 48 * 1024) CUDA_TRY(cudaFuncSetAttribute(beam_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                                      (int)bits));
-  cudaStream_t s = (cudaStream_t)stream;
-  beam_rows_kernel<<<B * K, kBeamThreads, bits, s>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_select_kernel<<<B, 32, 0, s>>>(a);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_step_incr_kernel<<<1, 1, 0, s>>>(step);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  return 0;
+  return launch_beam_step(a, a, beam_rows_kernel, kBeamThreads, bits, beam_select_kernel, 32, stream);
 }
 
 // adapcc_beam_step's arguments for one group (no G, group_done or lambda; fin_count int32 [B]), plus cand_c fp32
@@ -905,32 +859,17 @@ int adapcc_beam_sample_step(const float* logits, int ld, int vocab, int B, int K
                             pen, alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
                             hist_back, fin_score, fin_n, fin_src, fin_count, 1, nullptr, 0.f},
                    temperature, top_p, top_k, 0, seeds, cand_c};
-  if (check_beam_args("beam_sample_step", p.a)) return -1;
-  if (vocab > kSampleMaxVocab || !(temperature > 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
-    set_error("beam_sample_step: need vocab <= %d, temperature > 0, top_k >= 0, 0 < top_p <= 1 (got %d, %g, %d, %g)",
-              kSampleMaxVocab, vocab, temperature, top_k, top_p);
+  if (check_beam_args("beam_sample_step", p.a) ||
+      check_sampling_args("beam_sample_step", vocab, temperature, top_k, top_p))
     return -1;
-  }
   if (!cand_c || !seeds) {
     set_error("beam_sample_step: null pointer");
     return -1;
   }
   p.min_keep = n_stop + 1 > 2 ? n_stop + 1 : 2;
   p.a.N = p.min_keep * K;
-  const size_t smem = (size_t)vocab * sizeof(float);
-  if (smem > 48 * 1024)
-    CUDA_TRY(cudaFuncSetAttribute(beam_sample_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  cudaStream_t s = (cudaStream_t)stream;
-  beam_sample_rows_kernel<<<B * K, kSampleThreads, smem, s>>>(p);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_sample_select_kernel<<<B, kBeamThreads, 0, s>>>(p);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_step_incr_kernel<<<1, 1, 0, s>>>(step);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  return 0;
+  return launch_beam_step(p.a, p, beam_sample_rows_kernel, kSampleThreads, (size_t)vocab * sizeof(float),
+                          beam_sample_select_kernel, kBeamThreads, stream);
 }
 
 // stochastic beam search: adapcc_beam_sample_step's arguments without the length penalty, with scores the live beams'
@@ -947,32 +886,16 @@ int adapcc_beam_stochastic_step(const float* logits, int ld, int vocab, int B, i
                                 nullptr, -1, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
                                 hist_back, fin_score, fin_n, fin_src, fin_count, 1, nullptr, 0.f},
                        temperature, top_p, top_k, seeds, keys, cand_key, cand_phi, fin_phi, kappa};
-  if (check_beam_args("beam_stochastic_step", p.a)) return -1;
-  if (vocab > kSampleMaxVocab || !(temperature > 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
-    set_error("beam_stochastic_step: need vocab <= %d, temperature > 0, top_k >= 0, 0 < top_p <= 1 (got %d, %g, %d, "
-              "%g)", kSampleMaxVocab, vocab, temperature, top_k, top_p);
+  if (check_beam_args("beam_stochastic_step", p.a) ||
+      check_sampling_args("beam_stochastic_step", vocab, temperature, top_k, top_p))
     return -1;
-  }
   if (!keys || !cand_key || !cand_phi || !fin_phi || !kappa || !seeds) {
     set_error("beam_stochastic_step: null pointer");
     return -1;
   }
   p.a.N = K + 1;
-  const size_t smem = (size_t)vocab * sizeof(float);
-  if (smem > 48 * 1024)
-    CUDA_TRY(cudaFuncSetAttribute(beam_stochastic_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  (int)smem));
-  cudaStream_t s = (cudaStream_t)stream;
-  beam_stochastic_rows_kernel<<<B * K, kSampleThreads, smem, s>>>(p);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_stochastic_select_kernel<<<B, kBeamThreads, 0, s>>>(p);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  beam_step_incr_kernel<<<1, 1, 0, s>>>(step);
-  CUDA_TRY(cudaGetLastError());
-  count_launch();
-  return 0;
+  return launch_beam_step(p.a, p, beam_stochastic_rows_kernel, kSampleThreads, (size_t)vocab * sizeof(float),
+                          beam_stochastic_select_kernel, kBeamThreads, stream);
 }
 
 // k / v bf16 [L, R, H, t_max, Dh] contiguous; parent, prompt_len, lens int32 [R]; scratch at least

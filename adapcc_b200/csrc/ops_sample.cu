@@ -183,32 +183,11 @@ __device__ __forceinline__ float cut_prob(float x, const RowCut& c) {
 __device__ __forceinline__ int draw_row(float* s_x, SampleSmem& sm, const SampleArgs& a, const float* l, int step,
                                         int pos, long long seed, RowCut* cut = nullptr) {
   if (cut) *cut = RowCut{0xFFFFFFFFu, 0.f, 0.f};
-  const int tid = threadIdx.x, V = a.vocab;
-  const bool greedy = a.temperature == 0.f;
-  for (int i = tid; i < V; i += kSampleThreads) s_x[i] = greedy ? l[i] : __fdiv_rn(l[i], a.temperature);
-  __syncthreads();
-  if (step < a.min_new) {                           // the min-length rule comes before any filtering
-    for (int j = tid; j < a.n_suppress; j += kSampleThreads) {
-      const int id = a.suppress[j];
-      if (id >= 0 && id < V) s_x[id] = -INFINITY;
-    }
-    __syncthreads();
-  }
-  // the maximum (lowest index on a tie) and the number of candidates
-  unsigned long long best = 0;
-  int present = 0, z1 = 0, z2 = 0;
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const uint32_t k = f2key(s_x[i]);
-    if (k > kNegInfKey) {
-      ++present;
-      best = max(best, ((unsigned long long)k << 32) | (0xFFFFFFFFu - (uint32_t)i));
-    }
-  }
-  best = block_max(sm, best);
-  float fz = 0.f;
-  block_sum(sm, fz, present, z1, z2);
+  const int V = a.vocab;
+  unsigned long long best;
+  const int present = row_prologue(s_x, sm, l, V, a.temperature, step, a.min_new, a.suppress, a.n_suppress, best);
   int token = 0;                                    // a row without a finite logit draws id 0
-  if (present > 0 && greedy) {
+  if (present > 0 && a.temperature == 0.f) {
     token = (int)(0xFFFFFFFFu - (uint32_t)best);
   } else if (present > 0) {
     const uint32_t mkey = (uint32_t)(best >> 32);

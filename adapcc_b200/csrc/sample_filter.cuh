@@ -1,5 +1,5 @@
-// The row filter of the on-device sampler (ops_sample.cu) and of sampled beam search (ops_beam.cu): one CTA of 1024
-// threads holds a row's values x_i in shared memory. The top-k threshold and the top-p cut-off are found by bisection
+// The row prologue and filter of the on-device sampler (ops_sample.cu) and of sampled beam search (ops_beam.cu): one
+// CTA of 1024 threads holds a row's values x_i in shared memory. The top-k threshold and the top-p cut-off are found by bisection
 // over the order-preserving integer encoding of x (counts for top-k, masses for top-p), with no sort; the truncation
 // filters after top-p (min-p, typical, epsilon, eta) remove ids from the row in place. Also the counter convention
 // of the Philox4x32-10 draws both samplers make (the generator is philox.cuh), and the block reductions in their
@@ -145,6 +145,38 @@ __device__ __forceinline__ void row_moments(const float* s_x, SampleSmem& sm, in
     }
   }
   block_sum2(sm, z, s1);
+}
+
+// The start of every sampled row, by the whole CTA: s_x[i] = x_i = l_i / T for the logits row l (l_i itself at T = 0),
+// then, while step < min_new, the suppressed ids at -inf (the min-length rule comes before any filtering). Returns the
+// number of finite ids; `best` gets their block maximum (key << 32) | ~i, a tie to the lower id. The sampler's draw_row
+// and sampled beam search's row kernels all begin here, so their rows are the same bits.
+__device__ __forceinline__ int row_prologue(float* s_x, SampleSmem& sm, const float* l, int V, float T, int step,
+                                            int min_new, const int* suppress, int n_suppress,
+                                            unsigned long long& best) {
+  const int tid = threadIdx.x;
+  for (int i = tid; i < V; i += kSampleThreads) s_x[i] = T == 0.f ? l[i] : __fdiv_rn(l[i], T);
+  __syncthreads();
+  if (step < min_new) {
+    for (int j = tid; j < n_suppress; j += kSampleThreads) {
+      const int id = suppress[j];
+      if (id >= 0 && id < V) s_x[id] = -INFINITY;
+    }
+    __syncthreads();
+  }
+  best = 0;
+  int present = 0, z1 = 0, z2 = 0;
+  for (int i = tid; i < V; i += kSampleThreads) {
+    const uint32_t k = f2key(s_x[i]);
+    if (k > kNegInfKey) {
+      ++present;
+      best = max(best, ((unsigned long long)k << 32) | (0xFFFFFFFFu - (uint32_t)i));
+    }
+  }
+  best = block_max(sm, best);
+  float fz = 0.f;
+  block_sum(sm, fz, present, z1, z2);
+  return present;
 }
 
 // The k-th largest key f2key(s_x[i]) counted with multiplicity, for 0 < k < (number of finite ids); mkey is the

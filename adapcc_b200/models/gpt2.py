@@ -649,6 +649,28 @@ class GPT2DoubleHeads(nn.Module):
             tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
         return B, T, lengths, n, t_max, last, tt_new, native
 
+    @staticmethod
+    def _beam_args(who: str, num_beams: int, stop_ids: Sequence[int], suppress_ids: Sequence[int], sample: bool,
+                   temperature: float, top_k: int, top_p: float) -> int:
+        """The argument checks the beam decoders share, before anything is launched: ``num_beams``, the stop and
+        suppress list sizes and, with ``sample``, the sampling scalars. Returns K. Errors name ``who``."""
+        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS
+
+        K = int(num_beams)
+        if not 1 <= K <= BEAM_MAX_BEAMS:
+            raise ValueError(f"{who}: num_beams must be in [1, {BEAM_MAX_BEAMS}], got {num_beams}")
+        if len(stop_ids) > BEAM_MAX_STOP:
+            raise ValueError(f"{who}: at most {BEAM_MAX_STOP} stop_ids, got {len(stop_ids)}")
+        if len(suppress_ids) > BEAM_MAX_SUPPRESS:
+            raise ValueError(f"{who}: at most {BEAM_MAX_SUPPRESS} suppress_ids, got {len(suppress_ids)}")
+        if sample and not temperature > 0:
+            raise ValueError(f"{who}: sampling needs temperature > 0, got {temperature}")
+        if sample and int(top_k) < 0:
+            raise ValueError(f"{who}: top_k must be >= 0, got {top_k}")
+        if sample and not 0 < top_p <= 1:
+            raise ValueError(f"{who}: top_p must be in (0, 1], got {top_p}")
+        return K
+
     def _guidance_rows(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], lengths: List[int],
                        last: torch.Tensor, tt_new: Optional[torch.Tensor], negative_prompt_ids: Optional[torch.Tensor],
                        neg_lengths: List[int], negative_token_type_ids: Optional[torch.Tensor]):
@@ -894,17 +916,15 @@ class GPT2DoubleHeads(nn.Module):
         the items' seeds are a device input of the graph. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
         ``ops.repeats.penalize_repeats_reference``, ``ops.beam.GroupBeamReference`` (``BeamSampleReference`` with
         ``do_sample``) and torch indexing."""
-        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB, BeamState
+        from ..ops import SAMPLE_MAX_VOCAB, BeamState
         from ..ops.beam import BeamSampleReference, GroupBeamReference, best_hypotheses, merge_finished_sets
 
-        K = int(num_beams)
-        if not 1 <= K <= BEAM_MAX_BEAMS:
-            raise ValueError(f"beam_search: num_beams must be in [1, {BEAM_MAX_BEAMS}], got {num_beams}")
+        do_sample = bool(do_sample)
+        K = self._beam_args("beam_search", num_beams, stop_ids, suppress_ids, do_sample, temperature, top_k, top_p)
         R = int(num_return_sequences)
         if not 1 <= R <= K:
             raise ValueError(f"beam_search: num_return_sequences must be in [1, num_beams = {K}], got "
                              f"{num_return_sequences}")
-        do_sample = bool(do_sample)
         G, lam = int(num_beam_groups), float(diversity_penalty)
         if not 1 <= G <= K or K % G != 0:
             raise ValueError(f"beam_search: num_beam_groups must divide num_beams = {K}, got {num_beam_groups}")
@@ -913,13 +933,7 @@ class GPT2DoubleHeads(nn.Module):
                              f"> 0, got do_sample={do_sample}, diversity_penalty={diversity_penalty}")
         if G == 1 and lam != 0:
             raise ValueError(f"beam_search: diversity_penalty needs num_beam_groups > 1, got {diversity_penalty}")
-        if do_sample and not temperature > 0:
-            raise ValueError(f"beam_search: do_sample=True needs temperature > 0, got {temperature}")
-        if do_sample and (int(top_k) < 0 or not 0 < top_p <= 1):
-            raise ValueError(f"beam_search: need top_k >= 0 and 0 < top_p <= 1, got {top_k}, {top_p}")
-        if len(stop_ids) > BEAM_MAX_STOP or len(suppress_ids) > BEAM_MAX_SUPPRESS:
-            raise ValueError(f"beam_search: at most {BEAM_MAX_STOP} stop ids and {BEAM_MAX_SUPPRESS} suppressed ids, "
-                             f"got {len(stop_ids)} and {len(suppress_ids)}")
+
         def start(B, n, V, dev, native):
             seeds = _row_seeds(seed, B, dev) if do_sample else None
             if not native:                          # CPU / not bf16: the fp64 definition
@@ -942,10 +956,7 @@ class GPT2DoubleHeads(nn.Module):
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result(R))
         st = sel[0]
-        count, Kg = st.fin_count.cpu().tolist(), K // G
-        score, n_tok, src = st.fin_score.cpu().tolist(), st.fin_n.cpu().tolist(), st.fin_src.cpu().tolist()
-        fin = [merge_finished_sets([list(zip(score[b], n_tok[b], src[b]))[g * Kg:g * Kg + count[b * G + g]]
-                                    for g in range(G)]) for b in range(B)]
+        fin = [merge_finished_sets(sets) for sets in st.finished()]
         hist_tok = st.hist_tok.view(n, B, K).cpu().numpy()
         hist_back = st.hist_back.view(n, B, K).cpu().numpy()
         return tuple(t.to(dev) for t in best_hypotheses(fin, hist_tok, hist_back, n, R))
@@ -976,23 +987,11 @@ class GPT2DoubleHeads(nn.Module):
         ``ops.BeamState`` and ``ops.kv_reorder_``; there a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids and at
         most 64 beam rows per call. Elsewhere the same loop runs eagerly through ``StochasticBeamReference``. Bad
         arguments raise ``ValueError`` naming them before anything is launched."""
-        from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS, SAMPLE_MAX_VOCAB, BeamState
+        from ..ops import SAMPLE_MAX_VOCAB, BeamState
         from ..ops.beam import StochasticBeamReference, stochastic_results
 
         who = "stochastic_beam_search"
-        K = int(num_beams)
-        if not 1 <= K <= BEAM_MAX_BEAMS:
-            raise ValueError(f"{who}: num_beams must be in [1, {BEAM_MAX_BEAMS}], got {num_beams}")
-        if not temperature > 0:
-            raise ValueError(f"{who}: temperature must be > 0, got {temperature}")
-        if int(top_k) < 0:
-            raise ValueError(f"{who}: top_k must be >= 0, got {top_k}")
-        if not 0 < top_p <= 1:
-            raise ValueError(f"{who}: top_p must be in (0, 1], got {top_p}")
-        if len(stop_ids) > BEAM_MAX_STOP:
-            raise ValueError(f"{who}: at most {BEAM_MAX_STOP} stop_ids, got {len(stop_ids)}")
-        if len(suppress_ids) > BEAM_MAX_SUPPRESS:
-            raise ValueError(f"{who}: at most {BEAM_MAX_SUPPRESS} suppress_ids, got {len(suppress_ids)}")
+        K = self._beam_args(who, num_beams, stop_ids, suppress_ids, True, temperature, top_k, top_p)
         scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p)
 
         def start(B, n, V, dev, native):
@@ -1012,9 +1011,7 @@ class GPT2DoubleHeads(nn.Module):
             return tuple(t.to(dev) for t in sel.result())
         st = sel[0]
         B, n = st.batch, st.max_new
-        count = st.fin_count.cpu().tolist()
-        cols = [x.cpu().tolist() for x in (st.fin_score, st.fin_n, st.fin_src, st.fin_phi)]
-        fin = [list(zip(*(c[b] for c in cols)))[:count[b]] for b in range(B)]
+        fin = [sets[0] for sets in st.finished()]
         out = stochastic_results(fin, st.hist_tok.view(n, B, K).cpu().numpy(), st.hist_back.view(n, B, K).cpu().numpy(),
                                  n, K, st.kappa.cpu().numpy())
         return tuple(t.to(dev) for t in out)

@@ -564,6 +564,15 @@ class BeamState:
                 self.fin_score, self.fin_n, self.fin_src, self.fin_count, self.group_done, self.pen, self.cand,
                 self.cand_c, self.seeds, self.keys, self.fin_phi, self.kappa, self.cand_key, self.cand_phi)
 
+    def finished(self):
+        """The finished sets on the host: per item, per group, its ``(score, n, src)`` entries best first, with the
+        log-probability φ as a fourth field in a stochastic state."""
+        B, G, Kg = self.batch, self.groups, self.num_beams // self.groups
+        count = self.fin_count.cpu().tolist()
+        cols = [x.cpu().tolist() for x in (self.fin_score, self.fin_n, self.fin_src, self.fin_phi) if x is not None]
+        return [[list(zip(*(c[b] for c in cols)))[g * Kg:g * Kg + count[b * G + g]] for g in range(G)]
+                for b in range(B)]
+
 
 def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int = 0,
                suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None,
@@ -598,23 +607,20 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
         bad(f"a BeamState with {state.groups} groups needs a finite diversity_penalty > 0, got {diversity_penalty}")
     if state.groups == 1 and lam != 0:
         bad(f"diversity_penalty needs a BeamState with groups > 1, got {diversity_penalty}")
-    if state.seeds is not None:
-        if seeds is not None:
-            bad("a stochastic BeamState carries its items' seeds; pass seeds=None")
-        if not temperature > 0 or not int(top_k) >= 0 or not 0 < top_p <= 1:
-            bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
-        if vocab > SAMPLE_MAX_VOCAB:
-            bad(f"stochastic beam search needs vocab <= {SAMPLE_MAX_VOCAB}, got {vocab}")
+    if state.seeds is not None and seeds is not None:
+        bad("a stochastic BeamState carries its items' seeds; pass seeds=None")
     if seeds is not None:
         if not state.sample:
             bad("sampling needs a BeamState(..., sample=True)")
-        if not temperature > 0 or not int(top_k) >= 0 or not 0 < top_p <= 1:
-            bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
         if seeds.dtype != torch.int64 or not seeds.is_contiguous() or seeds.numel() != state.batch:
             bad(f"seeds must be a contiguous int64 tensor of {state.batch} elements, got {seeds.dtype} "
                 f"{tuple(seeds.shape)}")
+    if state.seeds is not None or seeds is not None:
+        mode = "stochastic beam search" if state.seeds is not None else "beam sampling"
+        if not temperature > 0 or not int(top_k) >= 0 or not 0 < top_p <= 1:
+            bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
         if vocab > SAMPLE_MAX_VOCAB:
-            bad(f"beam sampling needs vocab <= {SAMPLE_MAX_VOCAB}, got {vocab}")
+            bad(f"{mode} needs vocab <= {SAMPLE_MAX_VOCAB}, got {vocab}")
     B, K = state.batch, state.num_beams
     if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1 or logits.shape[0] != B * K:
         bad(f"logits must be fp32 [{B * K}, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")

@@ -248,7 +248,8 @@ def test_build_log_shows_beam_kernels_for_sm90a_without_spills():
     __graft_entry__.build()
     log = open(os.path.join(ROOT, "adapcc_b200", "_C", "build.log")).read()
     assert re.search(r"-gencode arch=compute_90a,code=sm_90a \S.*ops_beam\.cu", log)
-    for kernel in ("beam_rows_kernel", "beam_select_kernel", "kv_reorder_kernel"):
+    for kernel in ("beam_rows_kernel", "beam_select_kernel", "beam_sample_rows_kernel", "beam_sample_select_kernel",
+                   "beam_stochastic_rows_kernel", "beam_stochastic_select_kernel", "kv_reorder_kernel"):
         hits = re.findall(r"Compiling entry function '(\w*%s\w*)' for 'sm_90a'" % kernel, log)
         assert hits, kernel
         for name in hits:

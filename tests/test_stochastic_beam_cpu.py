@@ -3,7 +3,6 @@ autoregressive logit table and on the tiny GPT-2, against the reply law of ``gen
 ``ops/sampling.py`` (chi-square tests with fixed seeds), the truncated Gumbel, the estimator, the edge cases, the
 argument errors and the build of the kernels (nvcc only, no device)."""
 import os
-import re
 import sys
 from itertools import product
 
@@ -267,17 +266,3 @@ def test_bad_arguments_name_the_argument(tiny):
     with pytest.raises(ValueError):
         StochasticBeamReference(2, 2, 3, 5, seeds=[0])
 
-
-def test_build_log_shows_stochastic_beam_kernels_for_sm90a_without_spills():
-    import __graft_entry__
-
-    __graft_entry__.build()
-    log = open(os.path.join(ROOT, "adapcc_b200", "_C", "build.log")).read()
-    assert re.search(r"-gencode arch=compute_90a,code=sm_90a \S.*ops_beam\.cu", log)
-    for kernel in ("beam_stochastic_rows_kernel", "beam_stochastic_select_kernel"):
-        hits = re.findall(r"Compiling entry function '(\w*%s\w*)' for 'sm_90a'" % kernel, log)
-        assert hits, kernel
-        for name in hits:
-            props = re.search(r"Function properties for %s\s+(\d+) bytes stack frame, (\d+) bytes spill stores, "
-                              r"(\d+) bytes spill loads" % name, log)
-            assert props and props.group(2) == "0" and props.group(3) == "0", (name, props and props.group(0))
