@@ -95,7 +95,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    assistant_model=None, num_assistant_tokens: int = 4,
                    assistant_verification: str = "coupled", beam_sample: bool = False, num_beam_groups: int = 1,
                    diversity_penalty: float = 0.0, guidance_scale: float = 1.0,
-                   guidance_negative: str = "last_token") -> List[List[int]]:
+                   guidance_negative: str = "last_token", sequence_bias=None,
+                   bad_words_ids=None) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -118,7 +119,9 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     ``ops/guidance.py``) with each dialogue's negative prompt: ``guidance_negative="last_token"`` is the prompt's last
     token (HuggingFace's default), ``"no_persona"`` the same dialogue without the persona (built and truncated as the
     prompt is), so guidance pushes each reply towards its persona. Guidance with ``num_beams``, ``penalty_alpha``,
-    prompt lookup or an assistant is a ``ValueError``."""
+    prompt lookup or an assistant is a ``ValueError``. ``sequence_bias`` and ``bad_words_ids`` (HuggingFace's; token
+    ids of the dialogue tokenizer) go to ``generate`` / ``beam_search`` / ``contrastive_search`` (``ops/repeats.py``);
+    with prompt lookup or an assistant they are a ``ValueError``."""
     from ..ops.assisted import check_verification
     check_verification("sample_replies", assistant_verification, assistant_model)
     if assistant_model is not None and (num_beams > 0 or penalty_alpha > 0):
@@ -155,6 +158,10 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     seed = torch.tensor(list(seeds) if seeds is not None else range(len(insts)), dtype=torch.int64)
     special = list(tokenizer.special_ids)
     repeats = dict(repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
+    if sequence_bias is not None:
+        repeats["sequence_bias"] = sequence_bias
+    if bad_words_ids is not None:
+        repeats["bad_words_ids"] = bad_words_ids
     if num_beams > 0:
         sampled = dict(do_sample=True, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed) if beam_sample \
             else {}
@@ -176,6 +183,19 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                                    assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
                                    assistant_verification=assistant_verification, **repeats, **guidance)
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
+
+
+def bad_word_ids(tokenizer, words: Sequence[str]) -> List[List[int]]:
+    """``bad_words_ids`` banning each of ``words`` (surrounding blanks stripped, empty ones skipped) as the dialogue
+    tokenizer encodes it both at the start of a text and after a space, each distinct encoding once."""
+    out: List[List[int]] = []
+    for w in words:
+        w = w.strip()
+        for text in (w, " " + w) if w else ():
+            ids = list(tokenizer.encode(text))
+            if ids and ids not in out:
+                out.append(ids)
+    return out
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -266,8 +286,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, assistant_model=None,
                      num_assistant_tokens: int = 4, assistant_verification: str = "coupled",
                      beam_sample: bool = False, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
-                     guidance_scale: float = 1.0, guidance_negative: str = "last_token",
-                     **sample_kw) -> Dict[str, float]:
+                     guidance_scale: float = 1.0, guidance_negative: str = "last_token", sequence_bias=None,
+                     bad_words_ids=None, **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -282,7 +302,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``diversity_penalty``.
 
     ``repetition_penalty != 1`` or ``no_repeat_ngram_size > 0`` with ``f1``: the repetition controls of
-    ``generate`` / ``beam_search`` (``ops/repeats.py``), also on that batched path.
+    ``generate`` / ``beam_search`` (``ops/repeats.py``), also on that batched path; so do ``sequence_bias`` and
+    ``bad_words_ids``.
 
     ``penalty_alpha > 0`` with ``f1``: the replies are decoded by contrastive search with ``top_k`` candidates
     (:func:`sample_replies`), on that batched path.
@@ -301,7 +322,9 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``"no_persona"``, see :func:`sample_replies`), on that batched path."""
     from ..ops.assisted import check_verification
     check_verification("evaluate_dialogs", assistant_verification, assistant_model)
-    repeats = repetition_penalty != 1.0 or no_repeat_ngram_size > 0
+    repeats = (repetition_penalty != 1.0 or no_repeat_ngram_size > 0 or bool(sequence_bias)
+               or bool(bad_words_ids))
+    bias = {k: v for k, v in (("sequence_bias", sequence_bias), ("bad_words_ids", bad_words_ids)) if v is not None}
     lookup = prompt_lookup_num_tokens > 0
     filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
     filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0
@@ -315,7 +338,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                                     assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
                                     assistant_verification=assistant_verification, beam_sample=beam_sample,
                                     num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty,
-                                    guidance_scale=guidance_scale, guidance_negative=guidance_negative, **sample_kw)
+                                    guidance_scale=guidance_scale, guidance_negative=guidance_negative, **bias,
+                                    **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

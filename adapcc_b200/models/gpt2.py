@@ -32,7 +32,7 @@ import torch.nn.functional as F
 from ..ops.dropout import DropoutState, check_p, dropout, site_attn, site_embed, site_mlp, site_summary
 from ..ops.guidance import check_guidance_args, guided_scores_reference
 from ..ops.layers import FusedLayerNorm, FusedLinear
-from ..ops.repeats import check_repeat_args, penalize_repeats_reference
+from ..ops.repeats import check_repeat_args, check_sequence_bias_args, penalize_repeats_reference
 from ..ops.sampling import check_filter_args, sample_reference, top_filtering
 
 
@@ -235,22 +235,26 @@ class VerifyKV:
 class _Repeats:
     """The repetition controls of a batched decoder over the first R rows of its cache (``rows``; default all of them,
     ``generate`` with guidance passes its B prompt rows): ``seq`` int32 [R, t_max] each row's sequence (its prompt,
-    then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the penalty and the n-gram size.
-    ``create`` returns None when both controls are off, so then nothing is allocated or launched."""
+    then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the sequence-bias table
+    (``ops.repeats.SequenceBias`` or None), the penalty and the n-gram size. ``create`` returns None when all of them
+    are off, so then nothing is allocated or launched."""
 
     def __init__(self, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
-                 rows: Optional[int] = None):
+                 rows: Optional[int] = None, bias=None):
         B, T = input_ids.shape
         self.rows = cache.batch if rows is None else int(rows)
         self.seq = torch.zeros(self.rows, cache.t_max, dtype=torch.int32, device=input_ids.device)
         self.seq[:, :T] = input_ids.repeat_interleave(self.rows // B, dim=0)
         self.prompt_len = cache.lens[:self.rows].clone()
-        self.vocab, self.penalty, self.ngram = vocab, penalty, ngram
+        self.vocab, self.penalty, self.ngram, self.bias = vocab, penalty, ngram, bias
+        if bias is not None and input_ids.is_cuda:
+            bias.device_tensors(input_ids.device)       # before any capture: the graph keeps these pointers
 
     @classmethod
     def create(cls, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
-               rows: Optional[int] = None) -> Optional["_Repeats"]:
-        return cls(input_ids, cache, vocab, penalty, ngram, rows) if penalty != 1.0 or ngram > 0 else None
+               rows: Optional[int] = None, bias=None) -> Optional["_Repeats"]:
+        on = penalty != 1.0 or ngram > 0 or bias is not None
+        return cls(input_ids, cache, vocab, penalty, ngram, rows, bias) if on else None
 
     def eager(self, logits: torch.Tensor, cache: KVCache, consumed: Optional[torch.Tensor]) -> torch.Tensor:
         """``penalize_repeats_reference`` over every row's sequence, after storing ``consumed`` [R] (the tokens the last
@@ -260,7 +264,7 @@ class _Repeats:
             dev = self.seq.device
             self.seq[torch.arange(R, device=dev), cache.lens[:R].long() - 1] = consumed.to(dev, torch.int32)
         return penalize_repeats_reference(logits, [self.seq[r, :x] for r, x in enumerate(cache.host_lens[:R])],
-                                          self.vocab, self.penalty, self.ngram)
+                                          self.vocab, self.penalty, self.ngram, self.bias)
 
     def reorder(self, rows: torch.Tensor) -> None:
         """Row r continues row ``rows[r]`` (a beam its parent)."""
@@ -271,7 +275,7 @@ class _Repeats:
         """``ops.penalize_repeats_`` on ``logits`` in place; it also stores ``ids`` and follows ``parent``."""
         from ..ops import penalize_repeats_
         penalize_repeats_(logits, self.vocab, self.seq, self.prompt_len, lens, step, ids, parent, group,
-                          self.penalty, self.ngram)
+                          self.penalty, self.ngram, self.bias)
 
 
 def _row_seeds(seed, B: int, dev) -> torch.Tensor:
@@ -612,12 +616,14 @@ class GPT2DoubleHeads(nn.Module):
     def _decode_setup(self, who: str, input_ids: torch.Tensor, lengths: Optional[Sequence[int]],
                       token_type_ids: Optional[torch.Tensor], reply_type, max_new_tokens: int, min_new_tokens: int,
                       repetition_penalty: float, no_repeat_ngram_size: int, num_beams: int = 1,
-                      rows_name: str = "beam rows (batch x num_beams)"):
+                      rows_name: str = "beam rows (batch x num_beams)", sequence_bias=None, bad_words_ids=None,
+                      stop_ids: Sequence[int] = ()):
         """The checks and prompt quantities the batched decoders share, before anything is launched:
-        ``(B, T, lengths, n, t_max, last, tt_new, native)``. ``last`` [B] is each prompt's last position, ``tt_new`` [B]
-        the token type of new tokens (None without token types), and ``native`` says whether the bf16 CUDA kernels
-        run; they take at most ``LM_HEAD_MAX_ROWS`` rows, ``num_beams`` per prompt (called ``rows_name`` in the error
-        when more than one). Errors name ``who``."""
+        ``(B, T, lengths, n, t_max, last, tt_new, native, bias)``. ``last`` [B] is each prompt's last position,
+        ``tt_new`` [B] the token type of new tokens (None without token types), ``native`` says whether the bf16 CUDA
+        kernels run; they take at most ``LM_HEAD_MAX_ROWS`` rows, ``num_beams`` per prompt (called ``rows_name`` in
+        the error when more than one). ``bias`` is the table of ``sequence_bias`` and ``bad_words_ids``
+        (``ops.repeats.check_sequence_bias_args``; None when both are off). Errors name ``who``."""
         from ..ops import LM_HEAD_MAX_ROWS
 
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
@@ -632,6 +638,7 @@ class GPT2DoubleHeads(nn.Module):
             raise ValueError(f"{who}: need max_new_tokens >= 1 and min_new_tokens >= 0, got {max_new_tokens}, "
                              f"{min_new_tokens}")
         check_repeat_args(who, repetition_penalty, no_repeat_ngram_size)
+        bias = check_sequence_bias_args(who, sequence_bias, bad_words_ids, self.cfg.vocab_size, stop_ids)
         t_max = max(lengths) + n
         if t_max > self.cfg.n_positions:
             raise ValueError(f"{who}: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds "
@@ -647,7 +654,7 @@ class GPT2DoubleHeads(nn.Module):
             tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
         elif token_type_ids is not None:
             tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
-        return B, T, lengths, n, t_max, last, tt_new, native
+        return B, T, lengths, n, t_max, last, tt_new, native, bias
 
     @staticmethod
     def _beam_args(who: str, num_beams: int, stop_ids: Sequence[int], suppress_ids: Sequence[int], sample: bool,
@@ -708,7 +715,8 @@ class GPT2DoubleHeads(nn.Module):
                  num_assistant_tokens: int = 4,
                  assistant_verification: str = "coupled", guidance_scale: float = 1.0,
                  negative_prompt_ids: Optional[torch.Tensor] = None, negative_lengths: Optional[Sequence[int]] = None,
-                 negative_token_type_ids: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                 negative_token_type_ids: Optional[torch.Tensor] = None, sequence_bias=None,
+                 bad_words_ids=None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -718,7 +726,12 @@ class GPT2DoubleHeads(nn.Module):
         ``stop_ids`` ends its row. ``temperature == 0`` is greedy. The draw of each token is defined in
         ``ops/sampling.py``: a row's tokens depend on its prompt, its seed and the scalars, not on the other rows.
         ``repetition_penalty`` (1: off) and ``no_repeat_ngram_size`` (0: off) act on each row's logits first, over its
-        prompt and the tokens generated so far (``ops/repeats.py``). ``min_p`` (0: off), ``typical_p`` (1: off),
+        prompt and the tokens generated so far (``ops/repeats.py``). Before them, ``sequence_bias`` (HuggingFace's:
+        a dict ``{tuple(ids): bias}`` or a list of ``[ids, bias]`` pairs, finite biases) adds each bias to the logit
+        of a sequence's last id when the row's prompt and tokens end with the sequence's other ids, and
+        ``bad_words_ids`` (a list of id lists; a one-token list in ``stop_ids`` is dropped) does the same with -inf,
+        so no listed sequence is ever produced; at most ``ops.repeats.BIAS_MAX_ENTRIES`` entries of at most
+        ``BIAS_MAX_LEN`` ids in all, one table for every row. ``min_p`` (0: off), ``typical_p`` (1: off),
         ``epsilon_cutoff`` (0: off) and ``eta_cutoff`` (0: off) are HuggingFace's truncation samplers: at temperature
         > 0 they filter, in that order, the ids that top-k and top-p kept, just before the draw (inside
         ``ops.sample_tokens_`` on the native path); at temperature 0 they have no effect.
@@ -729,7 +742,7 @@ class GPT2DoubleHeads(nn.Module):
         exceeds ``n_positions``: there is no sliding window here, ``sample_sequence`` has one). On CUDA with bf16
         weights the LM head and the sampler are native kernels (``ops.lm_head_logits_``, ``ops.sample_tokens_``) and
         every token after the first replays one CUDA graph of decode step, LM head (``ops.penalize_repeats_`` when a
-        repetition control is on) and sampler, which feeds the drawn ids back into its own input; the host reads the
+        repetition control or sequence bias is on) and sampler, which feeds the drawn ids back into its own input; the host reads the
         done flags once every 8 tokens, a step late, to stop early. Elsewhere the same loop runs eagerly with fp32
         PyTorch logits, ``ops.repeats.penalize_repeats_reference`` and ``ops.sampling.sample_reference``.
 
@@ -766,7 +779,7 @@ class GPT2DoubleHeads(nn.Module):
         negative prompt, ``negative_prompt_ids`` [B, Tn] right-padded to ``negative_lengths`` (default Tn), by default
         the row's last prompt token alone with its token type; the negative rows consume the tokens the prompt rows
         draw. Each token's scores become ``g * (lc - lu) + lu`` of the two rows' log-softmaxes, before the repetition
-        controls (which see the prompt rows' sequences only) and the sampler. When the prompts have
+        controls and sequence bias (which see the prompt rows' sequences only) and the sampler. When the prompts have
         ``token_type_ids``, negative prompts take ``negative_token_type_ids``, else the type of the new tokens; new
         tokens take the same type in both rows. Not with prompt lookup or an assistant. The cache then holds 2B rows, prompts
         first (at most ``LM_HEAD_MAX_ROWS`` on the native path), prefilled together; on the native path each graph
@@ -783,6 +796,11 @@ class GPT2DoubleHeads(nn.Module):
         neg_lengths = check_guidance_args("generate", guidance_scale, B0, negative_prompt_ids, negative_lengths,
                                           negative_token_type_ids, token_type_ids, max_new_tokens, self.cfg.n_positions)
         guided = neg_lengths is not None
+        speculative = assistant_model is not None or prompt_lookup_num_tokens != 0
+        if speculative and (sequence_bias or bad_words_ids):
+            raise ValueError("generate: sequence_bias and bad_words_ids cannot be combined with "
+                             f"prompt_lookup_num_tokens or assistant_model (got {prompt_lookup_num_tokens}, "
+                             f"{type(assistant_model).__name__})")
         if guided and (assistant_model is not None or prompt_lookup_num_tokens != 0):
             raise ValueError("generate: guidance_scale != 1 cannot be combined with prompt_lookup_num_tokens or "
                              f"assistant_model (got {prompt_lookup_num_tokens}, {type(assistant_model).__name__})")
@@ -802,10 +820,11 @@ class GPT2DoubleHeads(nn.Module):
                                               reply_type, max_new_tokens, temperature, top_k, top_p, stop_ids,
                                               suppress_ids, min_new_tokens, seed, filters,
                                               assistant_verification == "rejection" and temperature > 0)
-        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+        B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, num_beams=2 if guided else 1,
-            rows_name="rows with guidance (batch x 2)")
+            rows_name="rows with guidance (batch x 2)", sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
+            stop_ids=stop_ids)
         dev, V = input_ids.device, self.cfg.vocab_size
         seeds = _row_seeds(seed, B, dev)
         if guided:                                  # rows [0, B): the prompts, rows [B, 2B): the negative prompts
@@ -820,7 +839,7 @@ class GPT2DoubleHeads(nn.Module):
         cache = self.new_cache(R, t_max)
         h = self.hidden(ids_all, tt_all, cache=cache, lengths=lengths_all)[torch.arange(R, device=dev), last]
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
-        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, B)
+        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, B, bias)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = self.wte.weight.float()
             done = torch.zeros(B, dtype=torch.int32)
@@ -874,8 +893,8 @@ class GPT2DoubleHeads(nn.Module):
                     suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
                     no_repeat_ngram_size: int = 0, do_sample: bool = False, temperature: float = 1.0,
                     top_k: int = 0, top_p: float = 1.0, seed=0,
-                    num_return_sequences: int = 1, num_beam_groups: int = 1,
-                    diversity_penalty: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    num_return_sequences: int = 1, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
+                    sequence_bias=None, bad_words_ids=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -886,7 +905,9 @@ class GPT2DoubleHeads(nn.Module):
         changes its result. An item's result depends on its prompt and the scalars only, not on the other items.
         ``repetition_penalty`` (1: off) and ``no_repeat_ngram_size`` (0: off) act on each beam's logits before the
         log-softmax, over its prompt and its own hypothesis (``ops/repeats.py``), so its log-probabilities are
-        renormalised over the ids that remain.
+        renormalised over the ids that remain. So do ``sequence_bias`` and ``bad_words_ids`` (as in ``generate``),
+        applied first: a biased beam's log-probabilities are renormalised too, where HuggingFace adds the bias to the
+        log-probabilities after normalisation.
 
         ``do_sample=True`` is beam sampling (HuggingFace's ``generate(do_sample=True, num_beams=K)``; the definition is
         ``ops.beam.BeamSampleReference``): each beam's ids are filtered by ``top_k`` (0: off) and ``top_p`` at
@@ -910,7 +931,7 @@ class GPT2DoubleHeads(nn.Module):
         Each prompt is prefilled once and its keys and values copied to its ``num_beams`` rows of a cache of
         ``max(lengths) + max_new_tokens`` positions (more than ``n_positions`` is a ``ValueError``). On CUDA with bf16
         weights every token after the first replays one CUDA graph of decode step, LM head (``ops.lm_head_logits_``),
-        the repetition controls when on (``ops.penalize_repeats_``), selection (``ops.beam_step_``) and cache
+        the repetition controls and sequence bias when on (``ops.penalize_repeats_``), selection (``ops.beam_step_``) and cache
         reordering (``ops.kv_reorder_``), at most 64 beam rows per call; the host reads the done flags once every 8
         tokens, a period late. Beam sampling takes a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids there, and
         the items' seeds are a device input of the graph. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
@@ -951,7 +972,8 @@ class GPT2DoubleHeads(nn.Module):
                          else dict(diversity_penalty=lam))
 
         sel = self._beam_decode("beam_search", input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
-                                min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start)
+                                min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
+                                sequence_bias, bad_words_ids)
         dev, B, n = input_ids.device, input_ids.shape[0], int(max_new_tokens)
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result(R))
@@ -967,10 +989,11 @@ class GPT2DoubleHeads(nn.Module):
                                max_new_tokens: int = 20, temperature: float = 1.0, top_k: int = 0,
                                top_p: float = 1.0, stop_ids: Sequence[int] = (), suppress_ids: Sequence[int] = (),
                                min_new_tokens: int = 0, repetition_penalty: float = 1.0,
-                               no_repeat_ngram_size: int = 0, seed=0):
+                               no_repeat_ngram_size: int = 0, seed=0, sequence_bias=None, bad_words_ids=None):
         """Stochastic beam search (Kool, van Hoof and Welling 2019): ``num_beams`` = K distinct replies per prompt,
         drawn without replacement from the law ``generate`` samples from with the same ``temperature``, ``top_k``,
-        ``top_p``, stop / suppress / ``min_new_tokens``, repetition settings and ``max_new_tokens``; the definition
+        ``top_p``, stop / suppress / ``min_new_tokens``, repetition settings, ``sequence_bias`` and ``bad_words_ids``
+        and ``max_new_tokens``; the definition
         (rules R1-R8, properties P1-P4) is ``ops.beam.StochasticBeamReference``. The first reply of an item is itself
         an exact sample of that law. ``seed``: an int (item b uses ``seed + b``) or an int64 [B] tensor; an item's
         result depends on its prompt, its seed and the scalars only. The other arguments work as in ``beam_search``.
@@ -983,7 +1006,8 @@ class GPT2DoubleHeads(nn.Module):
         the whole support).
 
         The decode loop is ``beam_search``'s: on CUDA with bf16 weights every token after the first replays one CUDA
-        graph of decode step, LM head, the repetition controls when on, ``ops.beam_step_`` on a stochastic
+        graph of decode step, LM head, the repetition controls and sequence bias when on, ``ops.beam_step_`` on a
+        stochastic
         ``ops.BeamState`` and ``ops.kv_reorder_``; there a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids and at
         most 64 beam rows per call. Elsewhere the same loop runs eagerly through ``StochasticBeamReference``. Bad
         arguments raise ``ValueError`` naming them before anything is launched."""
@@ -1005,7 +1029,8 @@ class GPT2DoubleHeads(nn.Module):
             return BeamState(B, K, n, 1.0, dev, seeds=seeds), scalars
 
         sel = self._beam_decode(who, input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
-                                min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start)
+                                min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
+                                sequence_bias, bad_words_ids)
         dev = input_ids.device
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result())
@@ -1018,19 +1043,21 @@ class GPT2DoubleHeads(nn.Module):
 
     def _beam_decode(self, who: str, input_ids: torch.Tensor, lengths, token_type_ids, reply_type, K: int,
                      max_new_tokens: int, min_new_tokens: int, repetition_penalty: float, no_repeat_ngram_size: int,
-                     stop_ids: Sequence[int], suppress_ids: Sequence[int], start):
+                     stop_ids: Sequence[int], suppress_ids: Sequence[int], start, sequence_bias=None,
+                     bad_words_ids=None):
         """The decode loop of the beam decoders. ``start(B, n, V, device, native)`` is called after the argument checks
         and before anything is launched; it returns the selector: on the native path ``(BeamState, keyword arguments
         of beam_step_)``, elsewhere a reference with ``step(logits) -> (next_ids, parent)`` and ``done``. Each prompt
         is prefilled once and its keys and values copied to its K rows; every token then takes the LM head, the
-        repetition controls when on, the selection and the cache reordering. On the native path every token after
+        repetition controls and sequence bias when on, the selection and the cache reordering. On the native path every token after
         the first replays one CUDA graph of them and the host reads the done flags once every 8 tokens; elsewhere
         the same loop runs eagerly with fp32 PyTorch logits and torch indexing. Returns the selector."""
         from ..ops import beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
 
-        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+        B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(
             who, input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
-            repetition_penalty, no_repeat_ngram_size, num_beams=K)
+            repetition_penalty, no_repeat_ngram_size, num_beams=K, sequence_bias=sequence_bias,
+            bad_words_ids=bad_words_ids, stop_ids=stop_ids)
         dev, V, weight = input_ids.device, self.cfg.vocab_size, self.wte.weight
         sel = start(B, n, V, dev, native)
         if tt_new is not None:
@@ -1044,7 +1071,7 @@ class GPT2DoubleHeads(nn.Module):
         cache.v[:, :, :, :T].copy_(pre.v.repeat_interleave(K, dim=1))
         del pre
         h = h.repeat_interleave(K, dim=0).contiguous()
-        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
+        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, bias=bias)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = weight.float()
             for i in range(n):
@@ -1092,7 +1119,7 @@ class GPT2DoubleHeads(nn.Module):
         ``rejection``, rejection sampling; one acceptance follows. The stats go to ``self.lookup_stats`` or
         ``self.assist_stats``."""
         arg = "prompt_lookup_num_tokens" if draft is None else "num_assistant_tokens"
-        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+        B, T, lengths, n, t_max, last, tt_new, native, _ = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens, 1.0, 0,
             num_beams=K + 1, rows_name=f"verify rows (batch x ({arg} + 1))")
         if draft is not None and t_max > draft.cfg.n_positions:
@@ -1236,7 +1263,8 @@ class GPT2DoubleHeads(nn.Module):
                            token_type_ids: Optional[torch.Tensor] = None, reply_type=None, top_k: int = 4,
                            penalty_alpha: float = 0.6, max_new_tokens: int = 20, stop_ids: Sequence[int] = (),
                            suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
-                           no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+                           no_repeat_ngram_size: int = 0, sequence_bias=None,
+                           bad_words_ids=None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched contrastive search (Su et al., 2022; HuggingFace's ``penalty_alpha`` + ``top_k``); the definition is
         in ``ops/contrastive.py``.
 
@@ -1245,13 +1273,15 @@ class GPT2DoubleHeads(nn.Module):
         between the candidate's final hidden state and the hidden states of the row's sequence so far (its prompt
         without padding, then its emitted tokens). ``penalty_alpha = 0`` or ``top_k = 1`` is greedy decoding.
         ``input_ids``, ``lengths``, ``reply_type``, token types, ``stop_ids``, ``suppress_ids``, ``min_new_tokens``,
-        the repetition controls and the return value ``(tokens, n_new)`` work as in ``generate``.
+        the repetition controls, ``sequence_bias``, ``bad_words_ids`` (applied to the logits before the candidates
+        are taken) and the return value ``(tokens, n_new)`` work as in ``generate``.
 
         The prompts are prefilled into a KV cache of ``max(lengths) + max_new_tokens`` positions (more than
         ``n_positions`` is a ``ValueError``) and the context is taken from the prefill's hidden states. On CUDA with
         bf16 weights (at most 64 rows) every token replays one CUDA graph: the candidate step (``ops.cand_attention_``
         attends for all k candidates over the shared cache), re-rank and commit (``ops.contrastive_rerank_``), the LM
-        head on the winners, ``ops.penalize_repeats_`` when on, and the next candidates (``ops.contrastive_select_``);
+        head on the winners, ``ops.penalize_repeats_`` when a repetition control or sequence bias is on, and the
+        next candidates (``ops.contrastive_select_``);
         the host reads the done flags once every 8 tokens, a period late. Elsewhere the same loop runs eagerly:
         candidates decode through ``decode_attention`` on a k-fold copy of the rows and the selection runs in fp64
         (``ops/contrastive.py``)."""
@@ -1260,9 +1290,10 @@ class GPT2DoubleHeads(nn.Module):
 
         check_contrastive_args("contrastive_search", top_k, penalty_alpha, CONTRASTIVE_MAX_K)
         K, alpha = int(top_k), float(penalty_alpha)
-        B, T, lengths, n, t_max, last, tt_new, native = self._decode_setup(
+        B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(
             "contrastive_search", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
-            repetition_penalty, no_repeat_ngram_size)
+            repetition_penalty, no_repeat_ngram_size, sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
+            stop_ids=stop_ids)
         cfg, dev, weight = self.cfg, input_ids.device, self.wte.weight
         tt_cand = tt_new.repeat_interleave(K) if tt_new is not None else None
         cache = self.new_cache(B, t_max)
@@ -1270,7 +1301,7 @@ class GPT2DoubleHeads(nn.Module):
         h = hs[torch.arange(B, device=dev), last].contiguous()
         V, L, H = cfg.vocab_size, cfg.n_layer, cfg.n_head
         D = cfg.n_embd
-        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size)
+        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, bias=bias)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = weight.float()
             cand = CandidateKV(cache, K, torch.zeros(L, 2, B * K, D, dtype=weight.dtype, device=dev))

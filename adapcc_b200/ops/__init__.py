@@ -68,7 +68,7 @@ def _lib():
         lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p,
                                                                                                 c_void_p]
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
-                                                + [c_int, c_float, c_int, c_void_p])
+                                                + [c_int, c_float, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p])
         lib.adapcc_guidance_mix.argtypes = [c_void_p, c_int, c_int, c_int, c_float, c_void_p]
         lib.adapcc_cs_sim_numel.argtypes = [c_int] * 3
         lib.adapcc_cs_sim_numel.restype = c_longlong
@@ -694,16 +694,16 @@ def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tens
                                  _ptr(lens), int(max_new), _ptr(scratch), _stream()), "kv_reorder")
 
 
-# ---- repetition penalty and no-repeat n-gram blocking (csrc/ops_repeats.cu) ----------------------------------------
+# ---- sequence bias, repetition penalty and no-repeat n-gram blocking (csrc/ops_repeats.cu) -------------------------
 REPEATS_MAX_GROUP = 16         # rows per parent group (beams per item)
 REPEATS_MAX_LEN = 1024         # sequence positions per row (GPT-2's n_positions)
 
 
 def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, prompt_len: torch.Tensor,
                       lens: torch.Tensor, step: torch.Tensor, ids: torch.Tensor, parent: Optional[torch.Tensor],
-                      group: int, penalty: float, ngram: int) -> None:
-    """The repetition penalty and no-repeat n-gram blocking of every row, in place, on the device (the definition in
-    ``ops/repeats.py``, which this kernel equals bit for bit). ``logits`` fp32 [R, ld] (the first ``vocab`` columns
+                      group: int, penalty: float, ngram: int, bias=None) -> None:
+    """The sequence bias, repetition penalty and no-repeat n-gram blocking of every row, in place, on the device (the
+    definition in ``ops/repeats.py``, which this kernel equals bit for bit). ``logits`` fp32 [R, ld] (the first ``vocab`` columns
     used); ``seq`` int32 [R, t_max] the rows' sequences, kept up to date here; ``prompt_len`` and ``lens`` int32 [R];
     ``step`` int32 [1] (the counter of ``generate`` / ``BeamState``); ``ids`` int64 [R] the tokens the decode step just
     consumed; ``parent`` int32 [R] or None, each row's parent inside its group of ``group`` consecutive rows.
@@ -711,13 +711,19 @@ def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, promp
     With ``*step > 0`` the sequences first advance: a row with a parent takes the parent's generated region
     ``seq[parent[r], prompt_len[r]:lens[r] - 1]`` (cycles and many-to-one maps come out right), then
     ``seq[r, lens[r] - 1] = ids[r]``. With ``*step == 0`` the sequence is the prompt as stored. Row r's sequence is then
-    ``seq[r, :lens[r]]``; ``penalty`` (1: off) and ``ngram`` (0: off) are applied to it. The grid depends on R and
-    ``group`` only and there is no host sync, so one capture serves every token."""
+    ``seq[r, :lens[r]]``; ``bias`` (an ``ops.repeats.SequenceBias`` from ``check_sequence_bias_args``, None: off),
+    ``penalty`` (1: off) and ``ngram`` (0: off) are applied to it. The table goes to the device once per table and
+    device and keeps its pointers, so a graph may capture it. The grid depends on R and ``group`` only and there is no
+    host sync, so one capture serves every token."""
+    from .repeats import SequenceBias
+
     def bad(msg):
         raise ValueError(f"penalize_repeats_: {msg}")
 
     if not (math.isfinite(penalty) and penalty > 0) or int(ngram) < 0:
         bad(f"need a finite penalty > 0 and ngram >= 0, got {penalty}, {ngram}")
+    if bias is not None and not isinstance(bias, SequenceBias):
+        bad(f"bias must be an ops.repeats.SequenceBias or None, got {type(bias).__name__}")
     if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
         bad(f"logits must be fp32 [R, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
     R = logits.shape[0]
@@ -734,10 +740,15 @@ def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, promp
                            ("parent", parent, torch.int32, R)):
         if t is not None and (t.dtype != dt or not t.is_contiguous() or t.numel() != n):
             bad(f"{name} must be a contiguous {dt} tensor of {n} elements, got {t.dtype} {tuple(t.shape)}")
+    if bias is not None and bias.max_id >= vocab:
+        bad(f"the bias table holds id {bias.max_id}, outside [0, vocab = {vocab})")
     _same_device("penalize_repeats_", logits.device, (seq, prompt_len, lens, step, ids, parent))
+    tab, val = bias.device_tensors(logits.device) if bias is not None else (None, None)
     _ck(_lib().adapcc_penalize_repeats(_ptr(logits), logits.stride(0), int(vocab), R, _ptr(seq), seq.shape[1],
                                        _ptr(prompt_len), _ptr(lens), _ptr(step), _ptr(ids), _ptr(parent), int(group),
-                                       float(penalty), int(ngram), _stream()), "penalize_repeats")
+                                       float(penalty), int(ngram), _ptr(tab), _ptr(val),
+                                       bias.num_targets if bias is not None else 0,
+                                       bias.num_entries if bias is not None else 0, _stream()), "penalize_repeats")
 
 
 # ---- classifier-free guidance (csrc/ops_guidance.cu) ---------------------------------------------------------------

@@ -87,7 +87,8 @@ also keeps a finished set of at most K entries ``(key, φ, n, src)`` and a thres
 start slot 0 is live with φ = 0 and G_0 = the Gumbel (rule S4's transform) of word 0 of Philox4x32-10 at counter
 ``(0, 0, 0, 2)`` under the item's key; the other slots are dead. At step t (L = t + 1), for every live slot j:
 
-R1. suppression below ``min_new`` is rule 1; the repetition controls act on the logits before it, as in ``generate``;
+R1. suppression below ``min_new`` is rule 1; the repetition controls and sequence bias act on the logits before it,
+    as in ``generate``;
 R2. ``x_i = fl32(l_i / T)``; the kept set is the sampler's top-k, then top-p (``ops/sampling.py`` steps 4 and 6),
     with min_keep 1: ``sample_keep(x, top_k, top_p, 1)``, the filter ``generate`` draws from;
 R3. for a kept i, ``lp'_i = (x_i - m) - log sum_kept exp(x_k - m)`` with m the largest kept x, and the child's
@@ -114,7 +115,8 @@ R8. the item is done when it has no live beam. Its results are its finished set,
 Properties (``tests/test_stochastic_beam_cpu.py`` checks them):
 
 P1. an item's first result is distributed exactly as the reply ``generate`` draws with the same temperature, top_k,
-    top_p, stop / suppress / min_new, repetition settings and ``max_new_tokens`` (the same law, another random stream);
+    top_p, stop / suppress / min_new, repetition settings, sequence bias and bad words and ``max_new_tokens`` (the
+    same law, another random stream);
 P2. its results are ``min(K, |support|)`` distinct sequences, a Gumbel-top-K sample without replacement from that law;
 P3. κ = -inf if and only if the support holds at most K sequences;
 P4. ``sum over results of f · exp(φ) / q``, ``q = -expm1(-exp(φ - κ))``, is unbiased for E[f] (priority sampling;

@@ -8,7 +8,7 @@ hidden state at every position of that sequence (the prompt's from the prefill, 
 is never part of the context, so a row's result does not depend on the other prompts of the batch. At each step, on the
 fp32 logits ``l`` of the row's last position (DESIGN.md §4a):
 
-1. the repetition controls, when on, are applied as in ``generate`` (``ops/repeats.py``); then, while
+1. the sequence bias and repetition controls, when on, are applied as in ``generate`` (``ops/repeats.py``); then, while
    ``step < min_new_tokens``, the ids in ``suppress_ids`` are removed;
 2. the candidates are the ``top_k`` ids with the largest remaining logits, ranked by descending logit, ties to the
    lower id; ids at -inf are never candidates, and if fewer than ``top_k`` remain the missing slots are invalid;

@@ -14,6 +14,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from adapcc_b200.data import synthetic_personachat  # noqa: E402
 from adapcc_b200.eval import evaluate_dialogs, load_model_from_checkpoint  # noqa: E402
+from adapcc_b200.eval.convai import bad_word_ids  # noqa: E402
 
 
 def main():
@@ -80,6 +81,9 @@ def main():
     p.add_argument("--guidance_negative", choices=("last_token", "no_persona"), default="last_token",
                    help="f1 with --guidance_scale: the negative prompt, the prompt's last token or the dialogue "
                         "without the persona")
+    p.add_argument("--bad_words", default="",
+                   help="f1: comma-separated words the replies may never contain, each banned as encoded with and "
+                        "without a leading space; replies go through the batched path")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -96,6 +100,8 @@ def main():
                   epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, beam_sample=a.beam_sample,
                   num_beam_groups=a.num_beam_groups, diversity_penalty=a.diversity_penalty,
                   guidance_scale=a.guidance_scale, guidance_negative=a.guidance_negative)
+        if a.bad_words:
+            kw["bad_words_ids"] = bad_word_ids(tok, a.bad_words.split(","))
         if a.assistant_checkpoint:
             kw["assistant_model"] = load_model_from_checkpoint(
                 a.assistant_checkpoint, a.device, torch.bfloat16 if a.device.startswith("cuda") else None)[0]

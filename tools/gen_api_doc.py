@@ -31,7 +31,8 @@ MODULES = [
                                 "check_lookup_args", "mean_tokens_per_step"]),
     ("adapcc_b200.ops.assisted", ["check_assist_args", "draw_slot", "assist_round", "draw_slots", "check_verification",
                                   "filtered_probs", "spec_slot", "spec_slots"]),
-    ("adapcc_b200.ops.repeats", ["penalize_repeats_reference", "banned_ngram_ids", "check_repeat_args"]),
+    ("adapcc_b200.ops.repeats", ["penalize_repeats_reference", "banned_ngram_ids", "check_repeat_args",
+                                 "check_sequence_bias_args", "SequenceBias"]),
     ("adapcc_b200.ops.guidance", ["check_guidance_args", "guided_scores_reference"]),
     ("adapcc_b200.ops.layers", ["FusedLayerNorm", "FusedLinear", "linear_backward"]),
     ("adapcc_b200.ops.gemm", ["linear_act", "linear_gelu", "supported", "default_variant"]),
@@ -59,7 +60,7 @@ MODULES = [
                                        "get_data_loaders"]),
     ("adapcc_b200.data.prefetch", ["PinnedPrefetcher", "micro_batch_groups"]),
     ("adapcc_b200.eval.convai", ["mc_scores", "sample_reply", "sample_replies", "evaluate_tensors", "f1_score",
-                                  "next_word_probability", "evaluate_dialogs"]),
+                                  "next_word_probability", "evaluate_dialogs", "bad_word_ids"]),
     ("adapcc_b200.eval", ["pack_checkpoint", "load_model_from_checkpoint"]),
     ("adapcc_b200.synth.plan", None),
 ]
