@@ -16,8 +16,9 @@
 //
 // Beam sampling (HuggingFace's do_sample=True with num_beams > 1) replaces the first two:
 //   beam_sample_rows   : one 1024-thread CTA per beam row, the row's x_i = l_i / T in shared memory (the sampler's
-//                        row_prologue, sample_filter.cuh). m and log Z as beam_rows computes them, then the sampler's
-//                        top-k / top-p filter with a minimum keep count, then c_i = s + lp_i / T and the Gumbel key
+//                        row_prologue, sample_filter.cuh). m and log Z of the unfiltered row as beam_rows computes
+//                        them, then the sampler's top-h, top-k / top-p and truncation filters with a minimum keep
+//                        count, then c_i = s + lp_i / T and the Gumbel key
 //                        g_i = c_i + G_i of every kept id, G_i from the item's Philox stream (gumbel_row). The row's M
 //                        best keys (a bisection for the M-th key, then a rank sort) are kept, with their c next to them.
 //   beam_sample_select : one 512-thread CTA per item. Each key's place in the item's draw order is its place in its
@@ -27,7 +28,7 @@
 //
 // Stochastic beam search (Kool et al. 2019; rules R1-R8 of ops/beam.py) replaces them too:
 //   beam_stochastic_rows   : one 1024-thread CTA per beam row, x_i = l_i / T in shared memory (row_prologue). The
-//                            sampler's filter (min_keep 1), log Z over the kept ids, then phi_i = phi + lp'_i and
+//                            sampler's filters (min_keep 1), log Z over the kept ids, then phi_i = phi + lp'_i and
 //                            Gphi_i = phi_i + G_i of every kept id (gumbel_row, its own Philox counter word); the K + 1
 //                            best Gphi (row_best_keys, shared with beam_sample_rows) are offered with their keys
 //                            truncated at the beam's key G and their phi.
@@ -289,9 +290,11 @@ __global__ void beam_step_incr_kernel(int* step) { *step += 1; }
 struct BeamSampleArgs {
   BeamArgs a;                  // a.N = M = min_keep * K; a.cand [B * K, M]: each row's M best Gumbel keys, best first
   float temperature, top_p;
-  int top_k, min_keep;         // min_keep = max(2, 1 + n_stop)
+  int top_k;
   const long long* seeds;      // [B]: the item's Philox key
   float* cand_c;               // [B * K, M]: the candidate score c next to each key
+  float top_h;                 // 0: off
+  FilterArgs f;                // f.min_keep = max(2, 1 + n_stop), for every filter
 };
 
 // G = -log(-log u) for u = ((w >> 8) + 0.5) 2^-24: -log u is taken from u below 1/2 and from 1 - u above, and both
@@ -331,80 +334,13 @@ __device__ __forceinline__ void gumbel_row(float* s_x, int V, uint32_t tau, long
   __syncthreads();
 }
 
-// The M best keys f2key(s_x[i]) of a row of 1024 threads (all finite ones when there are at most M; else those above
-// the M-th largest key, and of the ones equal to it the lowest ids) as (key << 32) | ~i, best first: emit(r, v) for
-// r < M, v = 0 past the count. s_sel holds M entries. Returns the largest key.
-template <class Emit>
-__device__ __forceinline__ uint32_t row_best_keys(const float* s_x, SampleSmem& sm, int V, int M,
-                                                  unsigned long long* s_sel, int* s_n, Emit emit) {
-  const int tid = threadIdx.x;
-  unsigned long long best = 0;
-  int cnt = 0, z1 = 0, z2 = 0;
-  float fz = 0.f;
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const uint32_t k = f2key(s_x[i]);
-    if (k > kNegInfKey) {
-      ++cnt;
-      best = max(best, (unsigned long long)k);
-    }
-  }
-  best = block_max(sm, best);
-  block_sum(sm, fz, cnt, z1, z2);
-  uint32_t thr = kNegInfKey;                          // taken: key > thr, or key == thr and id < cut
-  int cut = 0;
-  if (cnt > M) {
-    thr = kth_key(s_x, sm, V, M, (uint32_t)best);
-    int gt = 0, eq = 0, unused = 0;
-    for (int i = tid; i < V; i += kSampleThreads) {
-      const uint32_t k = f2key(s_x[i]);
-      gt += k > thr;
-      eq += k == thr;
-    }
-    block_sum(sm, fz, gt, eq, unused);
-    const int need = M - gt;
-    cut = V;
-    if (eq > need) {                                  // tied at the M-th key: the smallest cut with need ids below it
-      int lo = 0, hi = V;
-      while (hi - lo > 1) {
-        const int mid = lo + (hi - lo) / 2;
-        int c = 0, u0 = 0, u1 = 0;
-        for (int i = tid; i < mid; i += kSampleThreads) c += f2key(s_x[i]) == thr;
-        block_sum(sm, fz, c, u0, u1);
-        if (c >= need) hi = mid;
-        else lo = mid;
-      }
-      cut = hi;
-    }
-  }
-  if (tid == 0) *s_n = 0;
-  __syncthreads();
-  for (int i = tid; i < V; i += kSampleThreads) {
-    const uint32_t k = f2key(s_x[i]);
-    if (k > thr || (k == thr && i < cut)) s_sel[atomicAdd(s_n, 1)] = ((unsigned long long)k << 32) |
-                                                                     (0xFFFFFFFFu - (uint32_t)i);
-  }
-  __syncthreads();
-  const int n = *s_n;
-  // best first: a key's place is the number of larger keys (the keys are distinct)
-  for (int e = tid; e < M; e += kSampleThreads) {
-    if (e >= n) {
-      emit(e, 0ull);
-      continue;
-    }
-    const unsigned long long v = s_sel[e];
-    int r = 0;
-    for (int f = 0; f < n; ++f) r += s_sel[f] > v;
-    emit(r, v);
-  }
-  return (uint32_t)best;
-}
-
 __global__ void __launch_bounds__(kSampleThreads, 1) beam_sample_rows_kernel(const __grid_constant__ BeamSampleArgs p) {
   extern __shared__ float s_x[];                      // [vocab]: x_i = l_i / T, then g_i of the kept ids (-inf else)
   __shared__ SampleSmem sm;
   __shared__ float s_red[32];                         // beam_block_* with 1024 threads: warps 16-31 hold identities
-  __shared__ unsigned long long s_sel[kBeamSampleMaxM];
+  __shared__ unsigned long long s_sel[kBeamSampleMaxM];   // also top-h's kTopHN entries
   __shared__ int s_n;
+  static_assert(kBeamSampleMaxM >= kTopHN, "top-h shares s_sel");
   const BeamArgs& a = p.a;
   const int row = blockIdx.x, b = row / a.K, j = row - b * a.K, tid = threadIdx.x, V = a.vocab, M = a.N;
   unsigned long long* out = a.cand + (long long)row * M;
@@ -436,9 +372,16 @@ __global__ void __launch_bounds__(kSampleThreads, 1) beam_sample_rows_kernel(con
   z = beam_block_sum(s_red, z);
   const float lz = logf(z);
   auto cand_score = [&](int i) { return s + __fdiv_rn((__ldg(l + i) - m) - lz, p.temperature); };
-  // the sampler's filter on x, keeping at least min_keep values
+  // the sampler's filters on x, each keeping at least min_keep values; log Z above is the unfiltered row's
   const uint32_t mkey = (uint32_t)(best >> 32);
-  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, p.min_keep, present, mkey, key2f(mkey));
+  const float mx = key2f(mkey);
+  int kept = present;
+  if (p.top_h > 0.f) kept = top_h_row(s_x, sm, V, present, mx, p.top_h, p.f.min_keep, s_sel, &s_n);
+  uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, p.f.min_keep, kept, mkey, mx);
+  if (p.f.on()) {
+    filter_row(s_x, sm, V, p.f, tau, mx, mkey);
+    tau = kNegInfKey + 1;                             // the survivors are the finite ids
+  }
   __syncthreads();                                    // every x is read before the row becomes the keys
   gumbel_row(s_x, V, tau, p.seeds[b], j, step, 0u, cand_score);   // g_i = c_i + G_i
   row_best_keys(s_x, sm, V, M, s_sel, &s_n, [&](int r, unsigned long long v) {
@@ -549,6 +492,8 @@ struct BeamStochasticArgs {
   float temperature, top_p;
   int top_k;
   const long long* seeds;      // [B]: the item's Philox key
+  float top_h;                 // 0: off
+  FilterArgs f;                // min_keep 1, as in the sampler
   float* keys;                 // [B * K]: the live beams' keys G
   float* cand_key;             // [B * K, K + 1]: the truncated key of the child next to each cand entry
   float* cand_phi;             // [B * K, K + 1]: its log-probability phi
@@ -565,7 +510,8 @@ __global__ void __launch_bounds__(kSampleThreads, 1)
 beam_stochastic_rows_kernel(const __grid_constant__ BeamStochasticArgs p) {
   extern __shared__ float s_x[];                      // [vocab]: x_i = l_i / T, then Gphi_i of the kept ids (-inf else)
   __shared__ SampleSmem sm;
-  __shared__ unsigned long long s_sel[kBeamMaxK + 1], s_ord[kBeamMaxK + 1];
+  __shared__ unsigned long long s_sel[kTopHN > kBeamMaxK + 1 ? kTopHN : kBeamMaxK + 1];   // top-h's too
+  __shared__ unsigned long long s_ord[kBeamMaxK + 1];
   __shared__ int s_n;
   __shared__ float s_z;
   const BeamArgs& a = p.a;
@@ -584,10 +530,16 @@ beam_stochastic_rows_kernel(const __grid_constant__ BeamStochasticArgs p) {
     if (tid < N) out[tid] = 0ull;
     return;
   }
-  // the sampler's filter (min_keep 1), then log Z over the kept ids: lp'_i = (x_i - m) - log Z
+  // the sampler's filters (min_keep 1), then log Z over the kept ids: lp'_i = (x_i - m) - log Z
   const uint32_t mkey = (uint32_t)(best >> 32);
   const float m = key2f(mkey);
-  const uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, 1, present, mkey, m);
+  int kept = present;
+  if (p.top_h > 0.f) kept = top_h_row(s_x, sm, V, present, m, p.top_h, 1, s_sel, &s_n);
+  uint32_t tau = row_tau(s_x, sm, V, p.top_k, p.top_p, 1, kept, mkey, m);
+  if (p.f.on()) {
+    filter_row(s_x, sm, V, p.f, tau, m, mkey);
+    tau = kNegInfKey + 1;
+  }
   float z = 0.f;
   int u0 = 0, u1 = 0, u2 = 0;
   for (int i = tid; i < V; i += kSampleThreads) {
@@ -791,6 +743,17 @@ static int check_sampling_args(const char* who, int vocab, float temperature, in
   return 0;
 }
 
+// the truncation filters of the sampled modes, each off at its neutral value
+static int check_filter_args(const char* who, float min_p, float typical_p, float epsilon, float eta, float top_h) {
+  if (!(min_p >= 0.f && min_p <= 1.f) || !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) ||
+      !(eta >= 0.f && eta < 1.f) || !(top_h >= 0.f && top_h <= 1.f)) {
+    set_error("%s: need 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= epsilon < 1, 0 <= eta < 1, 0 <= top_h <= 1 (got "
+              "%g, %g, %g, %g, %g)", who, min_p, typical_p, epsilon, eta, top_h);
+    return -1;
+  }
+  return 0;
+}
+
 // One step on the stream: `rows` with a CTA of `rows_threads` per beam row and `smem` bytes of dynamic shared memory
 // (opted in above the default 48 KB), `select` with a CTA of `select_threads` per item, then the step increment.
 template <class Args>
@@ -848,46 +811,52 @@ int adapcc_beam_step(const float* logits, int ld, int vocab, int B, int K, int G
 
 // adapcc_beam_step's arguments for one group (no G, group_done or lambda; fin_count int32 [B]), plus cand_c fp32
 // [B*K, M] next to cand uint64 [B*K, M] (M = max(2, 1 + n_stop) * K), the sampling scalars (temperature > 0,
-// top_k >= 0 with 0 off, 0 < top_p <= 1) and seeds int64 [B]; vocab <= 56 Ki
+// top_k >= 0 with 0 off, 0 < top_p <= 1), seeds int64 [B] and the truncation filters (off at min_p = 0,
+// typical_p = 1, epsilon = 0, eta = 0, top_h = 0); vocab <= 56 Ki
 int adapcc_beam_sample_step(const float* logits, int ld, int vocab, int B, int K, float* scores, int* step,
                             int min_new, const int* suppress, int n_suppress, const int* stop, int n_stop,
                             const float* pen, int alpha_pos, int max_new, int* done, void* cand, float* cand_c,
                             long long* next_ids, int* parent, long long* hist_tok, int* hist_back, float* fin_score,
                             int* fin_n, int* fin_src, int* fin_count, float temperature, int top_k, float top_p,
-                            const long long* seeds, void* stream) {
+                            const long long* seeds, float min_p, float typical_p, float epsilon, float eta,
+                            float top_h, void* stream) {
   BeamSampleArgs p{BeamArgs{logits, ld, vocab, B, K, 0, scores, step, min_new, suppress, n_suppress, stop, n_stop,
                             pen, alpha_pos, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
                             hist_back, fin_score, fin_n, fin_src, fin_count, 1, nullptr, 0.f},
-                   temperature, top_p, top_k, 0, seeds, cand_c};
+                   temperature, top_p, top_k, seeds, cand_c, top_h, FilterArgs{min_p, typical_p, epsilon, eta, 0}};
   if (check_beam_args("beam_sample_step", p.a) ||
-      check_sampling_args("beam_sample_step", vocab, temperature, top_k, top_p))
+      check_sampling_args("beam_sample_step", vocab, temperature, top_k, top_p) ||
+      check_filter_args("beam_sample_step", min_p, typical_p, epsilon, eta, top_h))
     return -1;
   if (!cand_c || !seeds) {
     set_error("beam_sample_step: null pointer");
     return -1;
   }
-  p.min_keep = n_stop + 1 > 2 ? n_stop + 1 : 2;
-  p.a.N = p.min_keep * K;
+  p.f.min_keep = n_stop + 1 > 2 ? n_stop + 1 : 2;
+  p.a.N = p.f.min_keep * K;
   return launch_beam_step(p.a, p, beam_sample_rows_kernel, kSampleThreads, (size_t)vocab * sizeof(float),
                           beam_sample_select_kernel, kBeamThreads, stream);
 }
 
 // stochastic beam search: adapcc_beam_sample_step's arguments without the length penalty, with scores the live beams'
 // log-probabilities, keys fp32 [B*K] their keys, cand uint64 / cand_key, cand_phi fp32 [B*K, K + 1] the offered
-// children, fin_score the finished entries' keys and fin_phi fp32 [B, K] their log-probabilities, kappa fp32 [B]
+// children, fin_score the finished entries' keys and fin_phi fp32 [B, K] their log-probabilities, kappa fp32 [B],
+// then adapcc_beam_sample_step's truncation filters
 int adapcc_beam_stochastic_step(const float* logits, int ld, int vocab, int B, int K, float* scores, float* keys,
                                 int* step, int min_new, const int* suppress, int n_suppress, const int* stop, int n_stop,
                                 int max_new, int* done, void* cand, float* cand_key, float* cand_phi,
                                 long long* next_ids, int* parent, long long* hist_tok, int* hist_back,
                                 float* fin_score, float* fin_phi, int* fin_n, int* fin_src, int* fin_count,
                                 float* kappa, float temperature, int top_k, float top_p, const long long* seeds,
-                                void* stream) {
+                                float min_p, float typical_p, float epsilon, float eta, float top_h, void* stream) {
   BeamStochasticArgs p{BeamArgs{logits, ld, vocab, B, K, 0, scores, step, min_new, suppress, n_suppress, stop, n_stop,
                                 nullptr, -1, max_new, done, (unsigned long long*)cand, next_ids, parent, hist_tok,
                                 hist_back, fin_score, fin_n, fin_src, fin_count, 1, nullptr, 0.f},
-                       temperature, top_p, top_k, seeds, keys, cand_key, cand_phi, fin_phi, kappa};
+                       temperature, top_p, top_k, seeds, top_h, FilterArgs{min_p, typical_p, epsilon, eta, 1}, keys,
+                       cand_key, cand_phi, fin_phi, kappa};
   if (check_beam_args("beam_stochastic_step", p.a) ||
-      check_sampling_args("beam_stochastic_step", vocab, temperature, top_k, top_p))
+      check_sampling_args("beam_stochastic_step", vocab, temperature, top_k, top_p) ||
+      check_filter_args("beam_stochastic_step", min_p, typical_p, epsilon, eta, top_h))
     return -1;
   if (!keys || !cand_key || !cand_phi || !fin_phi || !kappa || !seeds) {
     set_error("beam_stochastic_step: null pointer");

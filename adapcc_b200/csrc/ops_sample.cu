@@ -7,8 +7,9 @@
 //             of d; each lane adds its chunks in order and a shuffle tree adds the lanes. The order depends on D only,
 //             so a row's bits do not depend on B, on the other rows or on which warp handles which rows of W.
 //   sample  : one CTA of 1024 threads per row; the row's x_i = l_i / temperature stay in shared memory for all passes.
-//             The top-k threshold, the top-p cut-off and the truncation filters are those of sample_filter.cuh (shared
-//             with sampled beam search). The draw is an inclusive scan over the surviving weights in index order.
+//             Top-h, the top-k threshold, the top-p cut-off and the truncation filters are those of sample_filter.cuh
+//             (shared with sampled beam search). The draw is an inclusive scan over the surviving weights in index
+//             order.
 //   slots   : the draws of assisted generation, one CTA per verify slot or draft (grid (slots, B)), through the same
 //             row body as `sample`, with a per-slot Philox counter and step (DESIGN.md §4a). A draft draw can also
 //             write the draft's filtered weights, which rejection-sampling verification reads.
@@ -192,9 +193,15 @@ __device__ __forceinline__ int draw_row(float* s_x, SampleSmem& sm, const Sample
   } else if (present > 0) {
     const uint32_t mkey = (uint32_t)(best >> 32);
     const float m = key2f(mkey);
-    uint32_t tau = row_tau(s_x, sm, V, a.top_k, a.top_p, 1, present, mkey, m);
-    if (a.filters) {
-      filter_row(s_x, sm, a, tau, m, mkey);
+    int kept = present;
+    if (a.top_h > 0.f) {
+      __shared__ unsigned long long s_sel[kTopHN];
+      __shared__ int s_n;
+      kept = top_h_row(s_x, sm, V, present, m, a.top_h, 1, s_sel, &s_n);
+    }
+    uint32_t tau = row_tau(s_x, sm, V, a.top_k, a.top_p, 1, kept, mkey, m);
+    if (a.f.on()) {
+      filter_row(s_x, sm, V, a.f, tau, m, mkey);
       tau = kNegInfKey + 1;                         // the survivors are the finite ids
     }
     // the draw: the smallest i whose inclusive prefix of surviving weights exceeds u Z'
@@ -345,7 +352,7 @@ spec_slots_kernel(const __grid_constant__ SpecArgs a) {
 // The checks and set-up shared by adapcc_sample_slots and adapcc_spec_slots; fills `s` or sets the error.
 static int slot_args(const char* who, const float* logits, int ld, int vocab, int B, int kq, int S, int slot0,
                      bool draft, float temperature, int top_k, float top_p, float min_p, float typical_p,
-                     float epsilon, float eta, const long long* seeds, const int* lens, const int* emitted,
+                     float epsilon, float eta, float top_h, const long long* seeds, const int* lens, const int* emitted,
                      const int* done, const int* nq, int min_new, const int* suppress, int n_suppress, SampleArgs& s) {
   if (B < 1 || B > 65535 || S < 1 || S > kSlotMaxSlots || kq < 1 || (draft && kq != 1) || slot0 < 0 ||
       slot0 + kq + (draft ? 1 : 0) > S || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab) {
@@ -355,10 +362,11 @@ static int slot_args(const char* who, const float* logits, int ld, int vocab, in
     return -1;
   }
   if (!(temperature >= 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f) || !(min_p >= 0.f && min_p <= 1.f) ||
-      !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) || !(eta >= 0.f && eta < 1.f)) {
+      !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) || !(eta >= 0.f && eta < 1.f) ||
+      !(top_h >= 0.f && top_h <= 1.f)) {
     set_error("%s: need temperature >= 0, top_k >= 0, 0 < top_p <= 1, 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= "
-              "epsilon < 1, 0 <= eta < 1 (got %g, %d, %g, %g, %g, %g, %g)", who, temperature, top_k, top_p, min_p,
-              typical_p, epsilon, eta);
+              "epsilon < 1, 0 <= eta < 1, 0 <= top_h <= 1 (got %g, %d, %g, %g, %g, %g, %g, %g)", who, temperature,
+              top_k, top_p, min_p, typical_p, epsilon, eta, top_h);
     return -1;
   }
   if (n_suppress < 0 || n_suppress > kSampleMaxList || (n_suppress && !suppress)) {
@@ -370,8 +378,7 @@ static int slot_args(const char* who, const float* logits, int ld, int vocab, in
     return -1;
   }
   s = SampleArgs{logits, ld, vocab, temperature, top_p, top_k, seeds, nullptr, nullptr, min_new, suppress, n_suppress,
-                 nullptr, 0, nullptr, nullptr, nullptr, 1, min_p, typical_p, epsilon, eta,
-                 min_p > 0.f || typical_p < 1.f || epsilon > 0.f || eta > 0.f};
+                 nullptr, 0, nullptr, nullptr, nullptr, 1, top_h, FilterArgs{min_p, typical_p, epsilon, eta, 1}};
   return 0;
 }
 
@@ -432,12 +439,12 @@ int adapcc_lm_head_logits(const void* h, int ld_h, const void* w, int V, int D, 
 
 // logits: fp32 [B, ld]; seeds int64 [B]; pos int32 [B]; step: int32 [1] on the device; suppress / stop: int32 lists
 // on the device (may be null when empty); done int32 [B]; next_ids int64 [B]; tokens int64 [B, max_new]; the
-// filters are off at min_p = 0, typical_p = 1, epsilon = 0 and eta = 0
+// filters are off at min_p = 0, typical_p = 1, epsilon = 0, eta = 0 and top_h = 0
 int adapcc_sample_tokens_filtered(const float* logits, int ld, int vocab, int B, float temperature, int top_k,
                                   float top_p, float min_p, float typical_p, float epsilon, float eta,
                                   const long long* seeds, const int* pos, int* step, int min_new, const int* suppress,
                                   int n_suppress, const int* stop, int n_stop, int* done, long long* next_ids,
-                                  long long* tokens, int max_new, void* stream) {
+                                  long long* tokens, int max_new, float top_h, void* stream) {
   if (B < 1 || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab || max_new < 1) {
     set_error("sample_tokens: need B >= 1, 1 <= vocab <= %d, ld >= vocab, max_new >= 1 (B=%d vocab=%d ld=%d "
               "max_new=%d)", kSampleMaxVocab, B, vocab, ld, max_new);
@@ -449,9 +456,9 @@ int adapcc_sample_tokens_filtered(const float* logits, int ld, int vocab, int B,
     return -1;
   }
   if (!(min_p >= 0.f && min_p <= 1.f) || !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) ||
-      !(eta >= 0.f && eta < 1.f)) {
-    set_error("sample_tokens: need 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= epsilon < 1, 0 <= eta < 1 (got %g, %g, "
-              "%g, %g)", min_p, typical_p, epsilon, eta);
+      !(eta >= 0.f && eta < 1.f) || !(top_h >= 0.f && top_h <= 1.f)) {
+    set_error("sample_tokens: need 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= epsilon < 1, 0 <= eta < 1, 0 <= top_h "
+              "<= 1 (got %g, %g, %g, %g, %g)", min_p, typical_p, epsilon, eta, top_h);
     return -1;
   }
   if (n_suppress < 0 || n_stop < 0 || n_suppress > kSampleMaxList || n_stop > kSampleMaxList ||
@@ -474,8 +481,7 @@ int adapcc_sample_tokens_filtered(const float* logits, int ld, int vocab, int B,
   });
   CUDA_TRY(setup[dev]);
   SampleArgs a{logits, ld, vocab, temperature, top_p, top_k, seeds, pos, step, min_new, suppress, n_suppress,
-               stop, n_stop, done, next_ids, tokens, max_new, min_p, typical_p, epsilon, eta,
-               min_p > 0.f || typical_p < 1.f || epsilon > 0.f || eta > 0.f};
+               stop, n_stop, done, next_ids, tokens, max_new, top_h, FilterArgs{min_p, typical_p, epsilon, eta, 1}};
   cudaStream_t s = (cudaStream_t)stream;
   sample_tokens_kernel<<<B, kSampleThreads, (size_t)vocab * sizeof(float), s>>>(a);
   CUDA_TRY(cudaGetLastError());
@@ -494,11 +500,11 @@ int adapcc_sample_slots(const float* logits, int ld, int vocab, int B, int kq, i
                         int top_k, float top_p, float min_p, float typical_p, float epsilon, float eta,
                         const long long* seeds, const int* lens, const int* emitted, const int* done, const int* nq,
                         int min_new, const int* suppress, int n_suppress, int* g, long long* ids, long long* next,
-                        float* q, float* zq, void* stream) {
+                        float* q, float* zq, float top_h, void* stream) {
   const bool draft = ids != nullptr;
   SampleArgs s;
   if (slot_args("sample_slots", logits, ld, vocab, B, kq, S, slot0, draft, temperature, top_k, top_p, min_p,
-                typical_p, epsilon, eta, seeds, lens, emitted, done, nq, min_new, suppress, n_suppress, s))
+                typical_p, epsilon, eta, top_h, seeds, lens, emitted, done, nq, min_new, suppress, n_suppress, s))
     return -1;
   if ((draft ? (!next || g) : (!g || next)) || !q != !zq || (q && (!draft || !(temperature > 0.f)))) {
     set_error("sample_slots: not exactly one of g and (ids, next), or q / zq without the other, or not with a draft "
@@ -522,10 +528,10 @@ int adapcc_spec_slots(const float* logits, int ld, int vocab, int B, int S, floa
                       float min_p, float typical_p, float epsilon, float eta, const long long* seeds, const int* lens,
                       const int* emitted, const int* done, const int* nq, int min_new, const int* suppress,
                       int n_suppress, const long long* ids, const float* q, const float* zq, int* g, int* acc,
-                      int* last, void* stream) {
+                      int* last, float top_h, void* stream) {
   SampleArgs s;
   if (slot_args("spec_slots", logits, ld, vocab, B, S, S, 0, false, temperature, top_k, top_p, min_p, typical_p,
-                epsilon, eta, seeds, lens, emitted, done, nq, min_new, suppress, n_suppress, s))
+                epsilon, eta, top_h, seeds, lens, emitted, done, nq, min_new, suppress, n_suppress, s))
     return -1;
   if (S < 2 || !(temperature > 0.f)) {
     set_error("spec_slots: need S >= 2 and temperature > 0 (got %d, %g)", S, temperature);
@@ -553,7 +559,7 @@ int adapcc_sample_tokens(const float* logits, int ld, int vocab, int B, float te
                          int max_new, void* stream) {
   return adapcc_sample_tokens_filtered(logits, ld, vocab, B, temperature, top_k, top_p, 0.f, 1.f, 0.f, 0.f, seeds, pos,
                                        step, min_new, suppress, n_suppress, stop, n_stop, done, next_ids, tokens,
-                                       max_new, stream);
+                                       max_new, 0.f, stream);
 }
 
 }  // extern "C"

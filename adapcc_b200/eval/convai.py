@@ -96,7 +96,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    assistant_verification: str = "coupled", beam_sample: bool = False, num_beam_groups: int = 1,
                    diversity_penalty: float = 0.0, guidance_scale: float = 1.0,
                    guidance_negative: str = "last_token", sequence_bias=None,
-                   bad_words_ids=None) -> List[List[int]]:
+                   bad_words_ids=None, top_h: float = 0.0) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -108,14 +108,14 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     ``generate`` / ``beam_search`` / ``contrastive_search`` (``ops/repeats.py``); the prompt counts as part of each
     reply's sequence. ``prompt_lookup_num_tokens`` > 0 (with ``no_sample``) verifies up to that many draft tokens per
     step, copied from the prompt and the reply so far; the replies are the greedy ones (``ops/lookup.py``).
-    ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff`` go to ``generate`` (the truncation filters of the
-    sampler, ``ops/sampling.py``). ``assistant_model`` (a draft model) and ``num_assistant_tokens`` go to ``generate``
-    (assisted generation, ``ops/assisted.py``): the replies are the ones drawn without it; with ``num_beams`` or
+    ``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff`` and ``top_h`` go to ``generate`` (the truncation
+    filters of the sampler, ``ops/sampling.py``), and to ``beam_search`` with ``beam_sample``. ``assistant_model`` (a
+    draft model) and ``num_assistant_tokens`` go to ``generate`` (assisted generation, ``ops/assisted.py``): the replies are the ones drawn without it; with ``num_beams`` or
     ``penalty_alpha`` it is a ``ValueError``. ``assistant_verification="rejection"`` verifies the drafts by rejection
     sampling instead: each reply token is still drawn from the model's distribution, but not the same draw.
     ``beam_sample`` with ``num_beams > 0``: beam sampling (``beam_search(do_sample=True)``) with ``temperature``,
-    ``top_k``, ``top_p`` and the seeds. ``num_beam_groups`` and ``diversity_penalty`` go to ``beam_search`` (diverse
-    beam search, ``ops/beam.py``). ``guidance_scale`` != 1 goes to ``generate`` (classifier-free guidance,
+    ``top_k``, ``top_p``, the truncation filters and the seeds. ``num_beam_groups`` and ``diversity_penalty`` go to
+    ``beam_search`` (diverse beam search, ``ops/beam.py``). ``guidance_scale`` != 1 goes to ``generate`` (classifier-free guidance,
     ``ops/guidance.py``) with each dialogue's negative prompt: ``guidance_negative="last_token"`` is the prompt's last
     token (HuggingFace's default), ``"no_persona"`` the same dialogue without the persona (built and truncated as the
     prompt is), so guidance pushes each reply towards its persona. Guidance with ``num_beams``, ``penalty_alpha``,
@@ -158,13 +158,14 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     seed = torch.tensor(list(seeds) if seeds is not None else range(len(insts)), dtype=torch.int64)
     special = list(tokenizer.special_ids)
     repeats = dict(repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
+    filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff, top_h=top_h)
     if sequence_bias is not None:
         repeats["sequence_bias"] = sequence_bias
     if bad_words_ids is not None:
         repeats["bad_words_ids"] = bad_words_ids
     if num_beams > 0:
-        sampled = dict(do_sample=True, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed) if beam_sample \
-            else {}
+        sampled = dict(do_sample=True, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
+                       **filters) if beam_sample else {}
         tokens, n_new, _ = model.beam_search(ids, lengths, tt, reply_type, num_beams=num_beams,
                                              max_new_tokens=max_length, stop_ids=special, suppress_ids=special,
                                              min_new_tokens=min_length, num_beam_groups=num_beam_groups,
@@ -178,8 +179,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     tokens, n_new = model.generate(ids, lengths, tt, reply_type, max_new_tokens=max_length,
                                    temperature=0.0 if no_sample else temperature, top_k=top_k, top_p=top_p,
                                    stop_ids=special, suppress_ids=special, min_new_tokens=min_length, seed=seed,
-                                   prompt_lookup_num_tokens=prompt_lookup_num_tokens, min_p=min_p,
-                                   typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                                   prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters,
                                    assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
                                    assistant_verification=assistant_verification, **repeats, **guidance)
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
@@ -287,7 +287,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      num_assistant_tokens: int = 4, assistant_verification: str = "coupled",
                      beam_sample: bool = False, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
                      guidance_scale: float = 1.0, guidance_negative: str = "last_token", sequence_bias=None,
-                     bad_words_ids=None, **sample_kw) -> Dict[str, float]:
+                     bad_words_ids=None, top_h: float = 0.0, **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -311,8 +311,9 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``prompt_lookup_num_tokens > 0`` with ``f1`` and ``no_sample``: greedy replies with prompt lookup decoding
     (:func:`sample_replies`), on that batched path.
 
-    ``min_p > 0``, ``typical_p < 1``, ``epsilon_cutoff > 0`` or ``eta_cutoff > 0`` with ``f1``: the truncation
-    filters of ``generate``'s sampler (``ops/sampling.py``), on that batched path.
+    ``min_p > 0``, ``typical_p < 1``, ``epsilon_cutoff > 0``, ``eta_cutoff > 0`` or ``top_h > 0`` with ``f1``: the
+    truncation filters of ``generate``'s sampler (``ops/sampling.py``), on that batched path; with ``beam_sample``
+    they filter the beams too.
 
     ``assistant_model`` (a draft model) with ``f1``: assisted generation with up to ``num_assistant_tokens`` drafts per
     round (``ops/assisted.py``), on that batched path; the replies are those of the batched path without it, unless
@@ -326,8 +327,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                or bool(bad_words_ids))
     bias = {k: v for k, v in (("sequence_bias", sequence_bias), ("bad_words_ids", bad_words_ids)) if v is not None}
     lookup = prompt_lookup_num_tokens > 0
-    filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
-    filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0
+    filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff, top_h=top_h)
+    filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0 or top_h > 0
     assisted = assistant_model is not None
     if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup or filtered
             or assisted or guidance_scale != 1.0) and eval_type == "f1":

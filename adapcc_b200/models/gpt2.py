@@ -658,9 +658,10 @@ class GPT2DoubleHeads(nn.Module):
 
     @staticmethod
     def _beam_args(who: str, num_beams: int, stop_ids: Sequence[int], suppress_ids: Sequence[int], sample: bool,
-                   temperature: float, top_k: int, top_p: float) -> int:
+                   temperature: float, top_k: int, top_p: float, filters: Optional[dict] = None) -> int:
         """The argument checks the beam decoders share, before anything is launched: ``num_beams``, the stop and
-        suppress list sizes and, with ``sample``, the sampling scalars. Returns K. Errors name ``who``."""
+        suppress list sizes and, with ``sample``, the sampling scalars and the truncation ``filters`` (keyword
+        arguments of ``check_filter_args``). Returns K. Errors name ``who``."""
         from ..ops import BEAM_MAX_BEAMS, BEAM_MAX_STOP, BEAM_MAX_SUPPRESS
 
         K = int(num_beams)
@@ -676,6 +677,8 @@ class GPT2DoubleHeads(nn.Module):
             raise ValueError(f"{who}: top_k must be >= 0, got {top_k}")
         if sample and not 0 < top_p <= 1:
             raise ValueError(f"{who}: top_p must be in (0, 1], got {top_p}")
+        if sample and filters:
+            check_filter_args(who, **filters)
         return K
 
     def _guidance_rows(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], lengths: List[int],
@@ -716,7 +719,7 @@ class GPT2DoubleHeads(nn.Module):
                  assistant_verification: str = "coupled", guidance_scale: float = 1.0,
                  negative_prompt_ids: Optional[torch.Tensor] = None, negative_lengths: Optional[Sequence[int]] = None,
                  negative_token_type_ids: Optional[torch.Tensor] = None, sequence_bias=None,
-                 bad_words_ids=None) -> Tuple[torch.Tensor, torch.Tensor]:
+                 bad_words_ids=None, top_h: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -734,7 +737,10 @@ class GPT2DoubleHeads(nn.Module):
         ``BIAS_MAX_LEN`` ids in all, one table for every row. ``min_p`` (0: off), ``typical_p`` (1: off),
         ``epsilon_cutoff`` (0: off) and ``eta_cutoff`` (0: off) are HuggingFace's truncation samplers: at temperature
         > 0 they filter, in that order, the ids that top-k and top-p kept, just before the draw (inside
-        ``ops.sample_tokens_`` on the native path); at temperature 0 they have no effect.
+        ``ops.sample_tokens_`` on the native path). ``top_h`` (in (0, 1]; 0: off; 1 is on) is HuggingFace's
+        entropy-bounded top-h: of the row's 100 largest values it keeps the longest prefix, by value, whose partial
+        entropy stays within ``top_h`` times their entropy; it acts before top-k. At temperature 0 no filter has an
+        effect.
 
         Returns ``(tokens, n_new)``: int64 [B, max_new_tokens] (-1 after a row stopped) and the tokens per row.
 
@@ -788,8 +794,9 @@ class GPT2DoubleHeads(nn.Module):
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
-        check_filter_args("generate", min_p, typical_p, epsilon_cutoff, eta_cutoff)
-        filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
+        check_filter_args("generate", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
+        filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                       top_h=top_h)
         from ..ops.assisted import check_verification
         check_verification("generate", assistant_verification, assistant_model)
         B0 = input_ids.shape[0] if input_ids.dim() == 2 else 0
@@ -894,7 +901,9 @@ class GPT2DoubleHeads(nn.Module):
                     no_repeat_ngram_size: int = 0, do_sample: bool = False, temperature: float = 1.0,
                     top_k: int = 0, top_p: float = 1.0, seed=0,
                     num_return_sequences: int = 1, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
-                    sequence_bias=None, bad_words_ids=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    sequence_bias=None, bad_words_ids=None, min_p: float = 0.0, typical_p: float = 1.0,
+                    epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
+                    top_h: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -911,10 +920,13 @@ class GPT2DoubleHeads(nn.Module):
 
         ``do_sample=True`` is beam sampling (HuggingFace's ``generate(do_sample=True, num_beams=K)``; the definition is
         ``ops.beam.BeamSampleReference``): each beam's ids are filtered by ``top_k`` (0: off) and ``top_p`` at
-        ``temperature`` > 0, keeping at least ``max(2, 1 + len(stop_ids))``, and the candidates are drawn without
-        replacement in proportion to ``exp(sum of log-probabilities / temperature)`` instead of ranked. ``seed``: an int
-        (item b uses ``seed + b``) or an int64 [B] tensor; an item's result depends on its prompt, its seed and the
-        scalars. With ``do_sample=False`` the sampling arguments are ignored.
+        ``temperature`` > 0, then by ``generate``'s truncation filters ``min_p``, ``typical_p``, ``epsilon_cutoff``
+        and ``eta_cutoff``, with ``top_h`` before top-k, each keeping at least ``max(2, 1 + len(stop_ids))`` ids
+        (HuggingFace's ``min_tokens_to_keep``; its top-h has none), and the candidates are drawn without replacement in
+        proportion to ``exp(sum of log-probabilities / temperature)`` instead of ranked; the log-probabilities are
+        those of the unfiltered row, as in HuggingFace. ``seed``: an int (item b uses ``seed + b``) or an int64 [B]
+        tensor; an item's result depends on its prompt, its seed and the scalars. With ``do_sample=False`` the sampling
+        arguments and the filters are ignored.
 
         ``num_beam_groups`` = G > 1 is diverse beam search (HuggingFace 4.x's ``num_beam_groups`` /
         ``diversity_penalty``; the definition is ``ops.beam.GroupBeamReference``): the beams form G groups of
@@ -941,7 +953,10 @@ class GPT2DoubleHeads(nn.Module):
         from ..ops.beam import BeamSampleReference, GroupBeamReference, best_hypotheses, merge_finished_sets
 
         do_sample = bool(do_sample)
-        K = self._beam_args("beam_search", num_beams, stop_ids, suppress_ids, do_sample, temperature, top_k, top_p)
+        filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                       top_h=top_h)
+        K = self._beam_args("beam_search", num_beams, stop_ids, suppress_ids, do_sample, temperature, top_k, top_p,
+                            filters)
         R = int(num_return_sequences)
         if not 1 <= R <= K:
             raise ValueError(f"beam_search: num_return_sequences must be in [1, num_beams = {K}], got "
@@ -961,14 +976,14 @@ class GPT2DoubleHeads(nn.Module):
                 if do_sample:
                     return BeamSampleReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
                                                temperature=temperature, top_k=top_k, top_p=top_p,
-                                               seeds=seeds.cpu().tolist())
+                                               seeds=seeds.cpu().tolist(), **filters)
                 return GroupBeamReference(B, K, n, V, length_penalty, stop_ids, suppress_ids, min_new_tokens,
                                           num_beam_groups=G, diversity_penalty=lam)
             if do_sample and V > SAMPLE_MAX_VOCAB:
                 raise ValueError(f"beam_search: do_sample=True needs a vocabulary of at most {SAMPLE_MAX_VOCAB} ids "
                                  f"on the native path, got {V}")
             st = BeamState(B, K, n, length_penalty, dev, sample=do_sample, groups=G)
-            return st, (dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds) if do_sample
+            return st, (dict(temperature=temperature, top_k=top_k, top_p=top_p, seeds=seeds, **filters) if do_sample
                          else dict(diversity_penalty=lam))
 
         sel = self._beam_decode("beam_search", input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
@@ -989,10 +1004,13 @@ class GPT2DoubleHeads(nn.Module):
                                max_new_tokens: int = 20, temperature: float = 1.0, top_k: int = 0,
                                top_p: float = 1.0, stop_ids: Sequence[int] = (), suppress_ids: Sequence[int] = (),
                                min_new_tokens: int = 0, repetition_penalty: float = 1.0,
-                               no_repeat_ngram_size: int = 0, seed=0, sequence_bias=None, bad_words_ids=None):
+                               no_repeat_ngram_size: int = 0, seed=0, sequence_bias=None, bad_words_ids=None,
+                               min_p: float = 0.0, typical_p: float = 1.0, epsilon_cutoff: float = 0.0,
+                               eta_cutoff: float = 0.0, top_h: float = 0.0):
         """Stochastic beam search (Kool, van Hoof and Welling 2019): ``num_beams`` = K distinct replies per prompt,
         drawn without replacement from the law ``generate`` samples from with the same ``temperature``, ``top_k``,
-        ``top_p``, stop / suppress / ``min_new_tokens``, repetition settings, ``sequence_bias`` and ``bad_words_ids``
+        ``top_p``, truncation filters (``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff``, ``top_h``), stop /
+        suppress / ``min_new_tokens``, repetition settings, ``sequence_bias`` and ``bad_words_ids``
         and ``max_new_tokens``; the definition
         (rules R1-R8, properties P1-P4) is ``ops.beam.StochasticBeamReference``. The first reply of an item is itself
         an exact sample of that law. ``seed``: an int (item b uses ``seed + b``) or an int64 [B] tensor; an item's
@@ -1015,8 +1033,10 @@ class GPT2DoubleHeads(nn.Module):
         from ..ops.beam import StochasticBeamReference, stochastic_results
 
         who = "stochastic_beam_search"
-        K = self._beam_args(who, num_beams, stop_ids, suppress_ids, True, temperature, top_k, top_p)
-        scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p)
+        filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                       top_h=top_h)
+        K = self._beam_args(who, num_beams, stop_ids, suppress_ids, True, temperature, top_k, top_p, filters)
+        scalars = dict(temperature=temperature, top_k=top_k, top_p=top_p, **filters)
 
         def start(B, n, V, dev, native):
             seeds = _row_seeds(seed, B, dev)

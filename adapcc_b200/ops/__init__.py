@@ -55,16 +55,18 @@ def _lib():
         lib.adapcc_sample_tokens_filtered.argtypes = ([c_void_p, c_int, c_int, c_int, c_float, c_int]
                                                       + [c_float] * 5 + [c_void_p] * 3
                                                       + [c_int, c_void_p, c_int, c_void_p, c_int]
-                                                      + [c_void_p] * 3 + [c_int, c_void_p])
+                                                      + [c_void_p] * 3 + [c_int, c_float, c_void_p])
         lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                          + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                          + [c_void_p] * 11 + [c_float, c_void_p])
         lib.adapcc_beam_sample_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                                 + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
-                                                + [c_void_p] * 11 + [c_float, c_int, c_float, c_void_p, c_void_p])
+                                                + [c_void_p] * 11 + [c_float, c_int, c_float, c_void_p]
+                                                + [c_float] * 5 + [c_void_p])
         lib.adapcc_beam_stochastic_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                                      c_int, c_void_p, c_int, c_void_p, c_int, c_int]
-                                                    + [c_void_p] * 14 + [c_float, c_int, c_float, c_void_p, c_void_p])
+                                                    + [c_void_p] * 14 + [c_float, c_int, c_float, c_void_p]
+                                                    + [c_float] * 5 + [c_void_p])
         lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p,
                                                                                                 c_void_p]
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
@@ -86,9 +88,11 @@ def _lib():
                                              + [c_void_p] * 4 + [c_int, c_void_p, c_void_p, c_void_p])
         lib.adapcc_lookup_draft.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 7
         lib.adapcc_sample_slots.argtypes = ([c_void_p] + [c_int] * 6 + [c_float, c_int] + [c_float] * 5
-                                            + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 6)
+                                            + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 5
+                                            + [c_float, c_void_p])
         lib.adapcc_spec_slots.argtypes = ([c_void_p] + [c_int] * 4 + [c_float, c_int] + [c_float] * 5
-                                          + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 7)
+                                          + [c_void_p] * 5 + [c_int, c_void_p, c_int] + [c_void_p] * 6
+                                          + [c_float, c_void_p])
         lib.adapcc_assist_round.argtypes = [c_void_p] + [c_int] * 5 + [c_void_p] * 10
         _bound = True
     return lib
@@ -436,7 +440,7 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
                    seeds: torch.Tensor, pos: torch.Tensor, step: torch.Tensor, min_new: int,
                    suppress_ids: Optional[torch.Tensor], stop_ids: Optional[torch.Tensor], done: torch.Tensor,
                    next_ids: torch.Tensor, tokens: torch.Tensor, min_p: float = 0.0, typical_p: float = 1.0,
-                   epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> None:
+                   epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0) -> None:
     """One seeded top-k / top-p draw per row, on the device (the definition in ``ops/sampling.py``, which computes the
     same in fp64). ``logits`` fp32 [B, ld] (the first ``vocab`` columns used), ``seeds`` int64 [B], ``pos`` int32 [B]
     (position of the drawn token: the Philox counter), ``step`` int32 [1] (tokens generated so far; incremented),
@@ -445,7 +449,8 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
     a stop id. ``temperature == 0`` is greedy. No host sync, so it can be captured in a CUDA graph.
 
     ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff`` (HuggingFace's truncation samplers; off at 0, 1,
-    0 and 0) filter the ids that top-p kept, in that order, before the draw; they have no effect at temperature 0."""
+    0 and 0) filter the ids that top-p kept, in that order, before the draw; ``top_h`` (HuggingFace's entropy-bounded
+    top-h, in (0, 1]; 0: off) filters the row before top-k. None has an effect at temperature 0."""
     def bad(msg):
         raise ValueError(f"sample_tokens_: {msg}")
 
@@ -453,7 +458,7 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
         bad(f"need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
     from .sampling import check_filter_args
 
-    check_filter_args("sample_tokens_", min_p, typical_p, epsilon_cutoff, eta_cutoff)
+    check_filter_args("sample_tokens_", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
     if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
         bad(f"logits must be fp32 [B, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
     B = logits.shape[0]
@@ -474,7 +479,7 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
                                              int(top_k), float(top_p), float(min_p), float(typical_p),
                                              float(epsilon_cutoff), float(eta_cutoff), _ptr(seeds), _ptr(pos),
                                              _ptr(step), int(min_new), sup, n_sup, stop, n_stop, _ptr(done),
-                                             _ptr(next_ids), _ptr(tokens), tokens.shape[1], _stream()),
+                                             _ptr(next_ids), _ptr(tokens), tokens.shape[1], float(top_h), _stream()),
         "sample_tokens")
 
 
@@ -577,7 +582,9 @@ class BeamState:
 def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int = 0,
                suppress_ids: Optional[torch.Tensor] = None, stop_ids: Optional[torch.Tensor] = None,
                temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
-               seeds: Optional[torch.Tensor] = None, diversity_penalty: float = 0.0) -> None:
+               seeds: Optional[torch.Tensor] = None, diversity_penalty: float = 0.0, min_p: float = 0.0,
+               typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
+               top_h: float = 0.0) -> None:
     """One beam-search selection for every item, on the device (the definition in ``ops/beam.py``, which computes the
     same in fp64). ``logits`` fp32 [B·K, ld] (the first ``vocab`` columns used) are the beams' next-token logits;
     ``suppress_ids`` (removed while ``state.step < min_new``) and ``stop_ids`` (at most 8; they finish a hypothesis)
@@ -588,7 +595,9 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
     With ``seeds`` (int64 [B] on the device, each item's Philox key) the step is beam sampling
     (``BeamSampleReference``): a ``BeamState(..., sample=True)``, ``temperature > 0``, ``top_k`` (0: off) and
     ``top_p`` filter each beam's ids, and the candidates are drawn rather than ranked; vocab is at most
-    ``SAMPLE_MAX_VOCAB``. Without ``seeds`` the sampling scalars are ignored.
+    ``SAMPLE_MAX_VOCAB``. Without ``seeds`` the sampling scalars are ignored. The truncation filters ``min_p``,
+    ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff`` and ``top_h`` (off at 0, 1, 0, 0 and 0) act in both sampled
+    modes, as in ``sample_tokens_``; beam sampling keeps at least ``max(2, 1 + n_stop)`` ids in each.
 
     A state with ``groups`` > 1 is diverse beam search (``GroupBeamReference``): the groups select in order, a
     candidate's score lowered by ``diversity_penalty`` (finite, > 0; 0 for one group) per new beam of an earlier group
@@ -619,6 +628,9 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
         mode = "stochastic beam search" if state.seeds is not None else "beam sampling"
         if not temperature > 0 or not int(top_k) >= 0 or not 0 < top_p <= 1:
             bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
+        from .sampling import check_filter_args
+
+        check_filter_args("beam_step_", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
         if vocab > SAMPLE_MAX_VOCAB:
             bad(f"{mode} needs vocab <= {SAMPLE_MAX_VOCAB}, got {vocab}")
     B, K = state.batch, state.num_beams
@@ -631,6 +643,7 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
     sup, n_sup = _id_list("beam_step_", "suppress_ids", suppress_ids, BEAM_MAX_SUPPRESS)
     stop, n_stop = _id_list("beam_step_", "stop_ids", stop_ids, BEAM_MAX_STOP)
     _same_device("beam_step_", logits.device, state.tensors() + (suppress_ids, stop_ids, seeds))
+    filters = [float(v) for v in (min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)]
     if state.seeds is not None:
         _ck(_lib().adapcc_beam_stochastic_step(
             _ptr(logits), logits.stride(0), int(vocab), B, K, _ptr(state.scores), _ptr(state.keys), _ptr(state.step),
@@ -638,7 +651,7 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
             _ptr(state.cand_key), _ptr(state.cand_phi), _ptr(state.next_ids), _ptr(state.parent),
             _ptr(state.hist_tok), _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_phi),
             _ptr(state.fin_n), _ptr(state.fin_src), _ptr(state.fin_count), _ptr(state.kappa), float(temperature),
-            int(top_k), float(top_p), _ptr(state.seeds), _stream()), "beam_stochastic_step")
+            int(top_k), float(top_p), _ptr(state.seeds), *filters, _stream()), "beam_stochastic_step")
         return
     if seeds is not None:
         _ck(_lib().adapcc_beam_sample_step(
@@ -646,7 +659,7 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
             n_sup, stop, n_stop, _ptr(state.pen), int(state.length_penalty > 0), state.max_new, _ptr(state.done),
             _ptr(state.cand), _ptr(state.cand_c), _ptr(state.next_ids), _ptr(state.parent), _ptr(state.hist_tok),
             _ptr(state.hist_back), _ptr(state.fin_score), _ptr(state.fin_n), _ptr(state.fin_src),
-            _ptr(state.fin_count), float(temperature), int(top_k), float(top_p), _ptr(seeds), _stream()),
+            _ptr(state.fin_count), float(temperature), int(top_k), float(top_p), _ptr(seeds), *filters, _stream()),
             "beam_sample_step")
         return
     _ck(_lib().adapcc_beam_step(
@@ -1101,7 +1114,7 @@ def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: i
                   state: LookupState, lens: torch.Tensor, slot0: int = 0, min_new: int = 0,
                   suppress_ids: Optional[torch.Tensor] = None, draft: bool = False, min_p: float = 0.0,
                   typical_p: float = 1.0, epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
-                  weights: bool = False) -> None:
+                  weights: bool = False, top_h: float = 0.0) -> None:
     """The draws of speculative decoding, one CTA per slot, on the device. ``logits`` fp32 [B·kq, ld] (the first
     ``vocab`` columns used) holds ``kq`` slots per row; its slot x of row b is slot ``j = slot0 + x``, drawn as
     ``sample_tokens_`` draws a row (the same bits) with the Philox counter ``lens[b] + j + 1`` (``lens`` int32 [B]) and
@@ -1123,7 +1136,7 @@ def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: i
         bad(f"need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
     from .sampling import check_filter_args
 
-    check_filter_args("sample_slots_", min_p, typical_p, epsilon_cutoff, eta_cutoff)
+    check_filter_args("sample_slots_", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
     B, S = state.batch, state.k + 1
     if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1 or logits.shape[0] % B:
         bad(f"logits must be fp32 [{B}·kq, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
@@ -1143,7 +1156,7 @@ def sample_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: i
                                    _ptr(state.emitted), _ptr(state.done), _ptr(state.nq), int(min_new), sup, n_sup,
                                    None if draft else _ptr(state.g), _ptr(state.ids) if draft else None,
                                    _ptr(state.d_in) if draft else None, _ptr(state.q if weights else None),
-                                   _ptr(state.zq if weights else None), _stream()), "sample_slots")
+                                   _ptr(state.zq if weights else None), float(top_h), _stream()), "sample_slots")
 
 
 def _check_slot_inputs(bad, logits: torch.Tensor, vocab: int, seeds: torch.Tensor, lens: torch.Tensor, B: int,
@@ -1161,7 +1174,7 @@ def _check_slot_inputs(bad, logits: torch.Tensor, vocab: int, seeds: torch.Tenso
 def spec_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int, top_p: float, seeds: torch.Tensor,
                 state: AssistState, lens: torch.Tensor, min_new: int = 0, suppress_ids: Optional[torch.Tensor] = None,
                 min_p: float = 0.0, typical_p: float = 1.0, epsilon_cutoff: float = 0.0,
-                eta_cutoff: float = 0.0) -> None:
+                eta_cutoff: float = 0.0, top_h: float = 0.0) -> None:
     """Rejection-sampling verification of a round on the device (``ops/assisted.py``), one CTA per slot. ``logits``
     fp32 [B·(k+1), ld] holds the model's slots; ``state`` is an ``AssistState`` made with this ``vocab``, whose
     ``q`` / ``zq`` hold the round's draft weights (``sample_slots_(..., weights=True)``) and ``ids`` the drafts. For
@@ -1178,7 +1191,7 @@ def spec_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int
         bad(f"need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, {top_k}, {top_p}")
     from .sampling import check_filter_args
 
-    check_filter_args("spec_slots_", min_p, typical_p, epsilon_cutoff, eta_cutoff)
+    check_filter_args("spec_slots_", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
     B, S = state.batch, state.k + 1
     if (logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1
             or logits.shape[0] != B * S):
@@ -1192,7 +1205,8 @@ def spec_slots_(logits: torch.Tensor, vocab: int, temperature: float, top_k: int
                                  float(top_p), float(min_p), float(typical_p), float(epsilon_cutoff),
                                  float(eta_cutoff), _ptr(seeds), _ptr(lens), _ptr(state.emitted), _ptr(state.done),
                                  _ptr(state.nq), int(min_new), sup, n_sup, _ptr(state.ids), _ptr(state.q),
-                                 _ptr(state.zq), _ptr(state.g), _ptr(state.acc), _ptr(state.last), _stream()),
+                                 _ptr(state.zq), _ptr(state.g), _ptr(state.acc), _ptr(state.last), float(top_h),
+                                 _stream()),
         "spec_slots")
 
 

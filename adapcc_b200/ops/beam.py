@@ -32,10 +32,13 @@ step, for every live beam row j of item b:
 
 S1. suppression is rule 1 (the repetition controls act before it, as in greedy mode); ``lp_i`` is rule 2's
     log-softmax over the remaining ids;
-S2. the filter is the sampler's steps 3-6 (``ops/sampling.py``) with a minimum keep count: ``x_i = fl32(l_i / T)``;
-    top-k keeps the ``k' = max(k, min_keep)`` largest values (``k > 0``); top-p keeps i iff the weight of the kept
-    values strictly larger than ``x_i`` is ``<= p Z``, and always the ``min_keep`` largest values; tied values are
-    kept or dropped together (HuggingFace's warpers on ``lp / T`` with ``min_tokens_to_keep = min_keep``);
+S2. the filter is the sampler's steps 3-6a (``ops/sampling.py``'s ``keep``) with a minimum keep count: ``x_i =
+    fl32(l_i / T)``; top-h keeps at least its ``min_keep`` first entries; top-k keeps the ``k' = max(k, min_keep)``
+    largest values (``k > 0``); top-p keeps i iff the weight of the kept values strictly larger than ``x_i`` is ``<=
+    p Z``, and always the ``min_keep`` largest values; min-p, typical, epsilon and eta each keep ``min_keep`` ids as
+    well; tied values are kept or dropped together, except at top-h's cut (HuggingFace's warpers on ``lp / T`` with
+    ``min_tokens_to_keep = min_keep``; HuggingFace's top-h has no keep count, and without one a step could offer
+    fewer than M candidates);
 S3. a kept id's candidate score is ``c = s_j + lp_i / T`` (the running sums are sums of warped log-probabilities);
     every other id is at -inf;
 S4. the draw is an ordered sample without replacement of M candidates from the item's finite ``(j, i)`` with
@@ -89,8 +92,9 @@ start slot 0 is live with φ = 0 and G_0 = the Gumbel (rule S4's transform) of w
 
 R1. suppression below ``min_new`` is rule 1; the repetition controls and sequence bias act on the logits before it,
     as in ``generate``;
-R2. ``x_i = fl32(l_i / T)``; the kept set is the sampler's top-k, then top-p (``ops/sampling.py`` steps 4 and 6),
-    with min_keep 1: ``sample_keep(x, top_k, top_p, 1)``, the filter ``generate`` draws from;
+R2. ``x_i = fl32(l_i / T)``; the kept set is the sampler's (``ops/sampling.py`` steps 3a-6a: top-h, top-k, top-p,
+    min-p, typical, epsilon, eta) with min_keep 1: ``keep(x, top_k, top_p, 1, ...)``, the filter ``generate`` draws
+    from;
 R3. for a kept i, ``lp'_i = (x_i - m) - log sum_kept exp(x_k - m)`` with m the largest kept x, and the child's
     log-probability is ``φ_ji = φ_j + lp'_i``: the per-step law is ``generate``'s, renormalised over the kept ids (beam
     sampling's ``s + lp / T`` is not renormalised; this rule differs on purpose);
@@ -115,8 +119,8 @@ R8. the item is done when it has no live beam. Its results are its finished set,
 Properties (``tests/test_stochastic_beam_cpu.py`` checks them):
 
 P1. an item's first result is distributed exactly as the reply ``generate`` draws with the same temperature, top_k,
-    top_p, stop / suppress / min_new, repetition settings, sequence bias and bad words and ``max_new_tokens`` (the
-    same law, another random stream);
+    top_p, truncation filters, stop / suppress / min_new, repetition settings, sequence bias and bad words and
+    ``max_new_tokens`` (the same law, another random stream);
 P2. its results are ``min(K, |support|)`` distinct sequences, a Gumbel-top-K sample without replacement from that law;
 P3. κ = -inf if and only if the support holds at most K sequences;
 P4. ``sum over results of f · exp(φ) / q``, ``q = -expm1(-exp(φ - κ))``, is unbiased for E[f] (priority sampling;
@@ -133,6 +137,8 @@ from typing import List, Sequence, Tuple
 
 import numpy as np
 import torch
+
+from .sampling import check_filter_args, keep
 
 
 class BeamReference:
@@ -384,46 +390,30 @@ def gumbel(w: np.ndarray) -> np.ndarray:
 
 
 def sample_keep(x: np.ndarray, top_k: int, top_p: float, min_keep: int) -> np.ndarray:
-    """Rule S2 on the fp32 values ``x = fl32(l / T)`` (-inf: removed): the bool mask of the kept ids, in fp64."""
-    cand = x > -np.inf
-    kept = cand.copy()
-    n = int(cand.sum())
-    if n == 0:
-        return kept
-    desc = np.sort(x[cand].astype(np.float64))[::-1]
-    k = max(int(top_k), min_keep) if top_k > 0 else 0
-    if 0 < k < n:
-        kept &= x >= desc[k - 1]
-    p = float(np.float32(top_p))
-    if p < 1.0:
-        xd = x.astype(np.float64)
-        m = xd[kept].max()
-        e = np.where(kept, np.exp(np.where(kept, xd - m, 0.0)), 0.0)
-        order = np.argsort(-xd[kept], kind="stable")
-        vals, csum = xd[kept][order], np.cumsum(e[kept][order])
-        first = np.searchsorted(-vals, -vals, side="left")    # the weight of the strictly larger values
-        tail = np.full(x.size, np.inf)
-        tail[np.flatnonzero(kept)[order]] = np.where(first > 0, csum[np.maximum(first - 1, 0)], 0.0)
-        keep_p = ~(tail > p * float(e.sum()))
-        keep_p |= x >= (desc[min_keep - 1] if min_keep < n else -np.inf)
-        kept &= keep_p
-    return kept
+    """Rule S2's top-k / top-p on the fp32 values ``x = fl32(l / T)`` (-inf: removed): the bool mask of the kept ids,
+    ``ops.sampling.keep`` with the truncation filters off."""
+    return keep(x, top_k, top_p, min_keep)[0]
 
 
 class BeamSampleReference(BeamReference):
     """Beam sampling (rules S1-S5 with 6 and 7, see the module docstring) for ``batch`` items in fp64, with the
-    interface of ``BeamReference``. ``seeds``: one int per item (its Philox key). ``temperature > 0`` and ``top_p`` are
-    rounded to fp32, as the kernel takes them; ``top_k = 0`` is off."""
+    interface of ``BeamReference``. ``seeds``: one int per item (its Philox key). ``temperature > 0``, ``top_p`` and
+    the truncation filters (``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff``, ``top_h``; off at 0, 1, 0,
+    0 and 0) are rounded to fp32, as the kernel takes them; ``top_k = 0`` is off."""
 
     def __init__(self, batch: int, num_beams: int, max_new: int, vocab: int, length_penalty: float = 1.0,
                  stop_ids: Sequence[int] = (), suppress_ids: Sequence[int] = (), min_new: int = 0,
                  early_stop: bool = True, temperature: float = 1.0, top_k: int = 0, top_p: float = 1.0,
-                 seeds: Sequence[int] = ()):
+                 seeds: Sequence[int] = (), min_p: float = 0.0, typical_p: float = 1.0, epsilon_cutoff: float = 0.0,
+                 eta_cutoff: float = 0.0, top_h: float = 0.0):
         super().__init__(batch, num_beams, max_new, vocab, length_penalty, stop_ids, suppress_ids, min_new,
                          early_stop)
         if not temperature > 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"BeamSampleReference: need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got "
                              f"{temperature}, {top_k}, {top_p}")
+        check_filter_args("BeamSampleReference", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
+        self.filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                            top_h=top_h)
         self.seeds = [int(x) for x in seeds]
         if len(self.seeds) != self.B:
             raise ValueError(f"BeamSampleReference: need {self.B} seeds, got {len(self.seeds)}")
@@ -444,8 +434,8 @@ class BeamSampleReference(BeamReference):
         xd = x.astype(np.float64)
         m = xd[fin].max()
         lp = (xd - m) - np.log(np.exp(xd[fin] - m).sum())
-        ids = np.flatnonzero(sample_keep((x / np.float32(self.T)).astype(np.float32), self.top_k, self.top_p,
-                                         self.min_keep))
+        ids = np.flatnonzero(keep((x / np.float32(self.T)).astype(np.float32), self.top_k, self.top_p,
+                                  self.min_keep, **self.filters)[0])
         c = s + lp[ids] / self.T
         w = philox_words(ids >> 2, j, step, 0, self.seeds[b])[np.arange(ids.size), ids & 3]
         return ids, c, c + gumbel(w)
@@ -543,15 +533,20 @@ class StochasticBeamReference(BeamReference):
     """Stochastic beam search (rules R1-R8, see the module docstring) for ``batch`` items in fp64, with the interface of
     ``BeamReference``. ``scores`` [B, K] are the live beams' φ, ``keys`` [B, K] their keys G, ``fin[b]`` item b's
     finished set as ``(key, n, src, φ)``, best first, and ``kappa`` [B] the thresholds. ``seeds``: one int per item;
-    ``temperature > 0`` and ``top_p`` are rounded to fp32, as the kernels take them; ``top_k = 0`` is off."""
+    ``temperature > 0``, ``top_p`` and the truncation filters are rounded to fp32, as the kernels take them;
+    ``top_k = 0`` is off."""
 
     def __init__(self, batch: int, num_beams: int, max_new: int, vocab: int, stop_ids: Sequence[int] = (),
                  suppress_ids: Sequence[int] = (), min_new: int = 0, temperature: float = 1.0, top_k: int = 0,
-                 top_p: float = 1.0, seeds: Sequence[int] = ()):
+                 top_p: float = 1.0, seeds: Sequence[int] = (), min_p: float = 0.0, typical_p: float = 1.0,
+                 epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0):
         super().__init__(batch, num_beams, max_new, vocab, 1.0, stop_ids, suppress_ids, min_new)
         if not temperature > 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"StochasticBeamReference: need temperature > 0, top_k >= 0 and 0 < top_p <= 1, got "
                              f"{temperature}, {top_k}, {top_p}")
+        check_filter_args("StochasticBeamReference", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
+        self.filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                            top_h=top_h)
         self.seeds = [int(x) for x in seeds]
         if len(self.seeds) != self.B:
             raise ValueError(f"StochasticBeamReference: need {self.B} seeds, got {len(self.seeds)}")
@@ -570,7 +565,7 @@ class StochasticBeamReference(BeamReference):
             x[self.suppress] = -np.inf
         if not np.isfinite(self.scores[b, j]) or not (x > -np.inf).any():
             return empty
-        ids = np.flatnonzero(sample_keep(x, self.top_k, self.top_p, 1))
+        ids = np.flatnonzero(keep(x, self.top_k, self.top_p, 1, **self.filters)[0])
         xd = x[ids].astype(np.float64)
         m = xd.max()
         phi = self.scores[b, j] + ((xd - m) - np.log(np.exp(xd - m).sum()))

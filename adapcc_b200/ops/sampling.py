@@ -6,6 +6,10 @@ For each row (DESIGN.md §4a):
 1. while ``step < min_new`` the ids in ``suppress_ids`` are removed (set to -inf) before anything else;
 2. ``temperature == 0``: the token is the arg-max over the remaining ids, the lowest index on a tie;
 3. otherwise ``x_i = fl32(l_i / temperature)`` (correctly rounded);
+3a. top-h (``top_h > 0``; HuggingFace's ``TopHLogitsWarper``): the n = min(100, number of candidates) largest values,
+   ordered by value descending with ties to the lower id, have ``p_r = e_r / Z_n`` over those n and
+   ``H = -sum p_r log p_r``; the longest prefix whose running sum of ``-p_r log p_r`` is ``<= top_h H`` is kept, and
+   always the first ``min(min_keep, n)`` entries. Every later step works on the ids it keeps;
 4. top-k (0 < k < number of candidates): keep ``x_i >= tau``, tau the k-th largest value counted with multiplicity;
 5. ``m`` = max of the kept values, ``e_i = exp(x_i - m)`` for kept ids, ``Z = sum e_i``;
 6. top-p (p < 1): keep i iff the weight of the kept ids with a strictly larger value is ``<= p Z`` (tied values are
@@ -17,7 +21,10 @@ For each row (DESIGN.md §4a):
    ``typical_p Z`` of the weight (tied deviations kept or dropped together; it may drop the maximum);
    epsilon (``epsilon_cutoff > 0``) keeps ``p_i >= epsilon_cutoff``; eta (``eta_cutoff > 0``) keeps
    ``p_i >= min(eta, sqrt(eta) exp(-H))``; epsilon and eta also keep the largest values of K (ties together), which
-   matters only when no id reaches the threshold. Each scalar is rounded to fp32 first, as ``top_p`` is;
+   matters only when no id reaches the threshold. Each scalar is rounded to fp32 first, as ``top_p`` is. With a
+   minimum keep count (``min_keep``, HuggingFace's ``min_tokens_to_keep``; 1 here, ``max(2, 1 + n_stop)`` in beam
+   sampling), top-k keeps ``max(k, min_keep)`` values, and top-p, min-p, epsilon and eta also keep the ``min_keep``
+   largest values of K, typical the ``min_keep`` smallest deviations, ties together (``keep``);
 7. ``u = (w0 >> 8) 2^-24`` with ``w0`` the first word of Philox4x32-10 at counter ``(pos, 0, 0, 0)`` and key
    ``(seed mod 2^32, seed >> 32)``; the token is the smallest kept i whose prefix sum of surviving weights exceeds
    ``u Z'`` (Z' = their total), or the largest kept id if there is none;
@@ -74,13 +81,16 @@ def top_filtering(logits: torch.Tensor, top_k: int = 0, top_p: float = 0.9, thre
     return logits
 
 
-def check_filter_args(who: str, min_p: float, typical_p: float, epsilon_cutoff: float, eta_cutoff: float) -> None:
+def check_filter_args(who: str, min_p: float, typical_p: float, epsilon_cutoff: float, eta_cutoff: float,
+                      top_h: float = 0.0) -> None:
     """``ValueError`` naming the argument unless ``0 <= min_p <= 1``, ``0 < typical_p <= 1``, ``0 <= epsilon_cutoff <
-    1`` and ``0 <= eta_cutoff < 1`` (each filter is off at 0, 1, 0 and 0 respectively)."""
+    1``, ``0 <= eta_cutoff < 1`` and ``0 <= top_h <= 1`` (each filter is off at 0, 1, 0, 0 and 0 respectively; top-h
+    at 1 is on)."""
     for name, v, ok, rng in (("min_p", min_p, lambda f: 0 <= f <= 1, "[0, 1]"),
                              ("typical_p", typical_p, lambda f: 0 < f <= 1, "(0, 1]"),
                              ("epsilon_cutoff", epsilon_cutoff, lambda f: 0 <= f < 1, "[0, 1)"),
-                             ("eta_cutoff", eta_cutoff, lambda f: 0 <= f < 1, "[0, 1)")):
+                             ("eta_cutoff", eta_cutoff, lambda f: 0 <= f < 1, "[0, 1)"),
+                             ("top_h", top_h, lambda f: 0 <= f <= 1, "[0, 1]")):
         try:
             f = float(v)
         except (TypeError, ValueError):
@@ -89,18 +99,40 @@ def check_filter_args(who: str, min_p: float, typical_p: float, epsilon_cutoff: 
             raise ValueError(f"{who}: {name} must be in {rng}, got {v!r}")
 
 
+def _floor(x: np.ndarray, kept: np.ndarray, k: int) -> float:
+    """The k-th largest value of ``x`` over ``kept`` (counted with multiplicity), or -inf when K holds at most k."""
+    v = x[kept]
+    return float(np.sort(v)[::-1][k - 1]) if k < v.size else -np.inf
+
+
+def _top_h(x: np.ndarray, kept: np.ndarray, top_h: float, min_keep: int) -> Dict[str, object]:
+    """Step 3a on ``kept`` in place. Returns the running sums ``cum`` of ``-p_r log p_r`` in the entries' order, the
+    threshold ``thr`` (``top_h H``) and the number ``c`` of entries kept."""
+    ids = np.flatnonzero(kept)
+    order = ids[np.lexsort((ids, -x[ids]))][:100]
+    y = x[order] - x[order[0]]
+    Z = float(np.exp(y).sum())
+    p = np.exp(y) / Z
+    h = p * (np.log(Z) - y)                                   # -p log p without log(0)
+    cum, thr = np.cumsum(h), top_h * float(h.sum())
+    c = max(int((cum <= thr).sum()), min(max(min_keep, 1), order.size))
+    kept[:] = False
+    kept[order[:c]] = True
+    return dict(cum=cum, thr=thr, c=c)
+
+
 def _filter(x: np.ndarray, e: np.ndarray, m: float, kept: np.ndarray, min_p: float, typical_p: float,
-            epsilon_cutoff: float, eta_cutoff: float) -> Dict[str, Dict[str, object]]:
+            epsilon_cutoff: float, eta_cutoff: float, min_keep: int = 1) -> Dict[str, Dict[str, object]]:
     """Step 6a on ``kept`` in place. Returns, per filter that is on, the quantity it compared (``q``, NaN outside K)
     and its threshold (``thr``); typical, epsilon and eta also give ``Z`` and ``mu`` (= sum p_i (x_i - m)) of the K
     they saw, and typical the weight ``G`` of ``{d_i <= d}`` at each distinct deviation of K in ascending order and
-    ``pZ``, the weight G must reach."""
+    ``pZ``, the weight G must reach. ``thr`` is the filter's own threshold; the ``min_keep`` floor comes on top."""
     out: Dict[str, Dict[str, object]] = {}
     mp, tp, ep, et = (float(np.float32(v)) for v in (min_p, typical_p, epsilon_cutoff, eta_cutoff))
     y = x - m
     if mp > 0:
         out["min_p"] = dict(q=np.where(kept, e, np.nan), thr=mp)
-        kept &= e >= mp
+        kept &= (e >= mp) | (x >= _floor(x, kept, min_keep))
     if tp < 1:
         Z = float(e[kept].sum())
         mu = float((e[kept] * y[kept]).sum()) / Z
@@ -111,7 +143,7 @@ def _filter(x: np.ndarray, e: np.ndarray, m: float, kept: np.ndarray, min_p: flo
         hit = np.flatnonzero(G >= tp * Z)
         dstar = float(ds[hit[0]] if hit.size else ds[-1])
         out["typical"] = dict(q=d, thr=dstar, G=G, pZ=tp * Z, Z=Z, mu=mu)
-        kept &= d <= dstar
+        kept &= d <= max(dstar, float(ds[min(min_keep, ds.size) - 1]))
     for name, c in (("epsilon", ep), ("eta", et)):
         if c > 0:
             Z = float(e[kept].sum())
@@ -120,18 +152,62 @@ def _filter(x: np.ndarray, e: np.ndarray, m: float, kept: np.ndarray, min_p: flo
             if name == "eta":
                 thr = min(c, np.sqrt(c) * np.exp(mu - np.log(Z)))        # exp(-H), H = log Z - mu
             out[name] = dict(q=p, thr=float(thr), Z=Z, mu=mu)
-            kept &= (p >= thr) | (x == x[kept].max())
+            kept &= (p >= thr) | (x >= _floor(x, kept, min_keep))
     return out
+
+
+def keep(x, top_k: int = 0, top_p: float = 1.0, min_keep: int = 1, min_p: float = 0.0, typical_p: float = 1.0,
+         epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0) -> Tuple[np.ndarray, Dict]:
+    """The kept set of one row, in fp64: steps 3a-6a on the fp32 values ``x = fl32(l / T)`` (-inf: removed), in
+    HuggingFace's order (top-h, top-k, top-p, min-p, typical, epsilon, eta), each filter keeping at least
+    ``min_keep`` ids. The sampler, stochastic beam search (``min_keep = 1``) and beam sampling (``max(2, 1 +
+    n_stop)``) all filter through it. Returns the bool mask of the kept ids and what it was decided from: ``m`` (the
+    largest value top-k kept), ``e`` (fp64 weights ``exp(x_i - m)`` of the ids kept by top-k), ``Z``, ``pZ``,
+    ``tail`` (for each top-k survivor, the weight of the larger values: the quantity top-p compares with pZ),
+    ``top_h`` (see ``_top_h``; present when top-h is on) and ``filters`` (see ``_filter``). ``top_p`` and
+    ``top_h`` are rounded to fp32 first."""
+    x = np.asarray(x, dtype=np.float32).reshape(-1)
+    kept = x > -np.inf
+    info: Dict[str, object] = {}
+    if not kept.any():
+        return kept, info
+    xd = x.astype(np.float64)
+    th = float(np.float32(top_h))
+    if th > 0:
+        info["top_h"] = _top_h(xd, kept, th, min_keep)
+    n = int(kept.sum())
+    k = max(int(top_k), min_keep) if top_k > 0 else 0
+    if 0 < k < n:
+        kept &= xd >= _floor(xd, kept, k)
+    m = xd[kept].max()
+    e = np.where(kept, np.exp(np.where(kept, xd - m, 0.0)), 0.0)
+    Z = float(e.sum())
+    p = float(np.float32(top_p))
+    pZ = p * Z
+    order = np.argsort(-xd[kept], kind="stable")
+    vals = xd[kept][order]
+    csum = np.cumsum(e[kept][order])
+    # weight of the values strictly larger than each kept value: the sum before the first of its ties
+    first = np.searchsorted(-vals, -vals, side="left")
+    above = np.where(first > 0, csum[np.maximum(first - 1, 0)], 0.0)
+    tail = np.full(x.size, np.nan)
+    tail[np.flatnonzero(kept)[order]] = above
+    if p < 1.0:
+        kept &= ~(tail > pZ) | (xd >= _floor(xd, kept, min_keep))
+    info.update(m=m, e=e, Z=Z, pZ=pZ, tail=tail,
+                filters=_filter(xd, e, m, kept, min_p, typical_p, epsilon_cutoff, eta_cutoff, min_keep))
+    return kept, info
 
 
 def reference_row(logits, temperature: float, top_k: int, top_p: float, seed: int, pos: int, step: int = 0,
                   min_new: int = 0, suppress_ids: Sequence[int] = (), min_p: float = 0.0, typical_p: float = 1.0,
-                  epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0) -> Dict[str, object]:
+                  epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0) -> Dict[str, object]:
     """One row of the definition (steps 1-7) in fp64. ``logits``: the row's ``vocab`` fp32 values. Returns the token
     and what it was decided from: ``kept`` (bool mask of the surviving ids), ``e`` (fp64 weights of the ids kept by
     top-k), ``Z``, ``pZ``, ``Zp`` (Z'), ``target`` (u Z'), ``cum`` (inclusive prefix sums of the surviving weights),
     ``tail`` (for each top-k survivor, the weight of the larger values: the quantity top-p compares with pZ) and
-    ``filters`` (per truncation filter that is on, what it compared with which threshold: see ``_filter``)."""
+    ``filters`` (per truncation filter that is on, what it compared with which threshold: see ``_filter``) and, with
+    top-h on, ``top_h`` (see ``_top_h``). The kept set is ``keep``'s with ``min_keep = 1``."""
     x = np.array(logits, dtype=np.float32).reshape(-1)
     if step < min_new:
         ids = np.array([i for i in suppress_ids if 0 <= i < x.size], dtype=np.int64)
@@ -145,33 +221,17 @@ def reference_row(logits, temperature: float, top_k: int, top_p: float, seed: in
         out["kept"] = np.arange(x.size) == out["token"]
         return out
     x = (x / np.float32(temperature)).astype(np.float32)
-    kept = cand.copy()
-    if 0 < top_k < int(cand.sum()):
-        tau = np.sort(x[cand])[::-1][top_k - 1]
-        kept &= x >= tau
-    xd = x.astype(np.float64)
-    m = xd[kept].max()
-    e = np.where(kept, np.exp(np.where(kept, xd - m, 0.0)), 0.0)
-    Z = float(e.sum())
-    pZ = float(np.float32(top_p)) * Z
-    order = np.argsort(-xd[kept], kind="stable")
-    vals = xd[kept][order]
-    csum = np.cumsum(e[kept][order])
-    # weight of the values strictly larger than each kept value: the sum before the first of its ties
-    first = np.searchsorted(-vals, -vals, side="left")
-    above = np.where(first > 0, csum[np.maximum(first - 1, 0)], 0.0)
-    tail = np.full(x.size, np.nan)
-    tail[np.flatnonzero(kept)[order]] = above
-    if float(np.float32(top_p)) < 1.0:
-        kept &= ~(tail > pZ)
-    filters = _filter(xd, e, m, kept, min_p, typical_p, epsilon_cutoff, eta_cutoff)
+    kept, info = keep(x, top_k, top_p, 1, min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
+    e = info["e"]
     w = np.where(kept, e, 0.0)
     cum = np.cumsum(w)
     Zp = float(cum[-1])
     target = uniform(seed, pos) * Zp
     hit = np.flatnonzero(kept & (cum > target))
-    out.update(token=int(hit[0]) if hit.size else int(np.flatnonzero(kept)[-1]), kept=kept, e=e, Z=Z, pZ=pZ, Zp=Zp,
-               target=target, cum=cum, tail=tail, filters=filters)
+    out.update(token=int(hit[0]) if hit.size else int(np.flatnonzero(kept)[-1]), kept=kept, e=e, Z=info["Z"],
+               pZ=info["pZ"], Zp=Zp, target=target, cum=cum, tail=info["tail"], filters=info["filters"])
+    if "top_h" in info:
+        out["top_h"] = info["top_h"]
     return out
 
 
@@ -179,8 +239,8 @@ def sample_reference(logits: torch.Tensor, vocab: int, temperature: float, top_k
                      seeds: torch.Tensor, pos: torch.Tensor, step: int, min_new: int = 0,
                      suppress_ids: Sequence[int] = (), stop_ids: Sequence[int] = (),
                      done: torch.Tensor = None, min_p: float = 0.0, typical_p: float = 1.0,
-                     epsilon_cutoff: float = 0.0,
-                     eta_cutoff: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                     epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
+                     top_h: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """``sample_tokens_`` for a batch, in fp64 on the host: ``logits`` [B, >= vocab] (fp32 values), ``seeds`` [B],
     ``pos`` [B], the scalar ``step``, ``done`` [B] (default: no row done). Returns ``(next_ids, tokens, done)``: int64
     [B] the ids fed to the next step, int64 [B] this step's reply column (-1 for stopped or finished rows), and the
@@ -188,8 +248,9 @@ def sample_reference(logits: torch.Tensor, vocab: int, temperature: float, top_k
     if temperature < 0 or top_k < 0 or not 0 < top_p <= 1:
         raise ValueError(f"sample_reference: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got "
                          f"{temperature}, {top_k}, {top_p}")
-    check_filter_args("sample_reference", min_p, typical_p, epsilon_cutoff, eta_cutoff)
-    filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff)
+    check_filter_args("sample_reference", min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
+    filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
+                   top_h=top_h)
     B = logits.shape[0]
     rows = logits[:, :vocab].detach().float().cpu().numpy()
     seeds, pos = seeds.cpu().tolist(), pos.cpu().tolist()

@@ -68,6 +68,9 @@ def main():
     p.add_argument("--eta_cutoff", type=float, default=0.0,
                    help="f1: eta sampling, keep ids with probability at least min(eta, sqrt(eta) exp(-entropy)) "
                         "(0: off); replies go through the batched path")
+    p.add_argument("--top_h", type=float, default=0.0,
+                   help="f1: top-h, keep the most probable ids whose partial entropy stays within this fraction of the "
+                        "entropy of the 100 most probable (0: off); replies go through the batched path")
     p.add_argument("--assistant_checkpoint", default="",
                    help="f1: a smaller model with the same vocabulary (a --checkpoint file) drafts tokens that the model "
                         "verifies (assisted generation); the replies are those drawn without it, through the batched path")
@@ -97,7 +100,7 @@ def main():
                   no_sample=a.no_sample, repetition_penalty=a.repetition_penalty,
                   no_repeat_ngram_size=a.no_repeat_ngram_size, penalty_alpha=a.penalty_alpha,
                   prompt_lookup_num_tokens=a.prompt_lookup_num_tokens, min_p=a.min_p, typical_p=a.typical_p,
-                  epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, beam_sample=a.beam_sample,
+                  epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, top_h=a.top_h, beam_sample=a.beam_sample,
                   num_beam_groups=a.num_beam_groups, diversity_penalty=a.diversity_penalty,
                   guidance_scale=a.guidance_scale, guidance_negative=a.guidance_negative)
         if a.bad_words:

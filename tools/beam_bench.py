@@ -26,8 +26,11 @@ fallback) and writes nothing into the repository.
   items, K = 8 beams and 128-token prompts, ms per generated token as in ``sampled`` (no stop ids, 64 new tokens),
   the two alternated run by run; and the stochastic ``beam_step_`` (its rows and select kernels, temperature 1, no
   top-k) alone at 64 rows (vocab 50257), timed as in ``kernels``.
+* ``filters``: the sampled ``beam_step_`` of beam sampling and of stochastic beam search (temperature 0.7, no top-k,
+  top-p 1, two stop ids, so beam sampling keeps 3 ids in every filter) at 64 rows (vocab 50257), timed as in
+  ``kernels``, with the truncation filters off and with each one on: top-h, min-p, typical, epsilon and eta.
 
-Usage: ``python tools/beam_bench.py [--reps 3] [--launches 1000]``
+Usage: ``python tools/beam_bench.py [--reps 3] [--launches 1000] [--sections kernels,filters,...]``
 """
 import argparse
 import json
@@ -237,11 +240,42 @@ def bench_kernels(model, launches):
     return out
 
 
+FILTERS = [("off", {}), ("top_h=0.9", dict(top_h=0.9)), ("min_p=0.05", dict(min_p=0.05)),
+           ("typical_p=0.9", dict(typical_p=0.9)), ("epsilon_cutoff=3e-4", dict(epsilon_cutoff=3e-4)),
+           ("eta_cutoff=3e-4", dict(eta_cutoff=3e-4))]
+
+
+def bench_filters(model, launches):
+    from adapcc_b200.ops import BeamState, beam_step_
+
+    B, K, V = 8, 8, 50257
+    g = torch.Generator(device="cuda").manual_seed(9)
+    logits = torch.randn(B * K, model.wte.weight.shape[0], device="cuda", generator=g) * 3
+    stop = torch.tensor([11, 13], dtype=torch.int32, device="cuda")
+    seeds = torch.arange(B, dtype=torch.int64, device="cuda")
+    max_new = launches + 4 * GRAPH_LAUNCHES
+    out = {"rows": B * K, "temperature": 0.7, "beam_sample_step_us": {}, "stochastic_step_us": {}}
+    for name, f in FILTERS:
+        st = BeamState(B, K, max_new, 1.0, "cuda", sample=True)
+        st.scores.zero_()
+        us = _graph_us(lambda: beam_step_(logits, V, st, 0, None, stop, temperature=0.7, seeds=seeds, **f), launches)
+        out["beam_sample_step_us"][name] = round(us, 2)
+        st = BeamState(B, K, max_new, 1.0, "cuda", seeds=seeds.cpu())
+        st.scores.zero_()
+        st.keys.zero_()
+        us = _graph_us(lambda: beam_step_(logits, V, st, 0, None, stop, temperature=0.7, **f), launches)
+        out["stochastic_step_us"][name] = round(us, 2)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--reps", type=int, default=3)
     ap.add_argument("--launches", type=int, default=1000)
+    ap.add_argument("--sections", default="kernels,search,sampled,groups,stochastic,filters",
+                    help="comma-separated sections to run (default: all)")
     args = ap.parse_args()
+    sections = set(args.sections.split(","))
     if not torch.cuda.is_available():
         sys.exit("beam_bench: needs a CUDA device")
     from adapcc_b200.models.gpt2 import GPT2Config, GPT2DoubleHeads
@@ -252,10 +286,12 @@ def main():
     info = _gpu_info()
     torch.manual_seed(0)
     model = GPT2DoubleHeads(GPT2Config()).to(device="cuda", dtype=torch.bfloat16).eval()
-    result = dict(info, new_tokens=NEW_TOKENS, kernels=bench_kernels(model, args.launches),
-                  search=bench_search(model, args.reps), sampled=bench_sampled(model, args.reps),
-                  groups=bench_groups(model, args.reps, args.launches),
-                  stochastic=bench_stochastic(model, args.reps, args.launches))
+    runs = dict(kernels=lambda: bench_kernels(model, args.launches), search=lambda: bench_search(model, args.reps),
+                sampled=lambda: bench_sampled(model, args.reps),
+                groups=lambda: bench_groups(model, args.reps, args.launches),
+                stochastic=lambda: bench_stochastic(model, args.reps, args.launches),
+                filters=lambda: bench_filters(model, args.launches))
+    result = dict(info, new_tokens=NEW_TOKENS, **{k: fn() for k, fn in runs.items() if k in sections})
     print(json.dumps(result))
 
 

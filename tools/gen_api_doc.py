@@ -18,8 +18,8 @@ MODULES = [
     ("adapcc_b200.parallel.ddp", None),
     ("adapcc_b200.parallel.expert_parallel", ["ExpertExchange"]),
     ("adapcc_b200.ops", None),
-    ("adapcc_b200.ops.sampling", ["top_filtering", "philox4x32_10", "uniform", "reference_row", "sample_reference",
-                                  "check_filter_args"]),
+    ("adapcc_b200.ops.sampling", ["top_filtering", "philox4x32_10", "uniform", "keep", "reference_row",
+                                  "sample_reference", "check_filter_args"]),
     ("adapcc_b200.ops.dropout", ["DropoutState", "dropout", "dropout_mask", "dropout_reference", "threshold"]),
     ("adapcc_b200.ops.beam", ["BeamReference", "BeamSampleReference", "GroupBeamReference", "best_hypotheses",
                               "merge_finished_sets", "offer_finished", "sample_keep", "philox_words", "gumbel",

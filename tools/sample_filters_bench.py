@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""The cost of the sampler's truncation filters (min-p, typical, epsilon, eta) on GPT-2's vocabulary.
+"""The cost of the sampler's truncation filters (min-p, typical, epsilon, eta, top-h) on GPT-2's vocabulary.
 
 Prints one JSON line. Needs a CUDA device (there is no CPU fallback) and writes nothing into the repository.
 
 * ``kernels``: ``sample_tokens_`` alone at B = 1 / 8 / 64 and vocab 50262, temperature 0.7, ``top_p = 0.9``, on
-  ``randn * 3`` logits, with every filter off and with each filter on (and all four together). 50 launches are
+  ``randn * 3`` logits, with every filter off and with each filter on (and min-p to eta together). 50 launches are
   captured in a CUDA graph and timed with CUDA events over ``--launches`` launches; the configurations are alternated
   and each figure is the median over ``--rounds`` rounds. ``--baseline-lib`` times another build of ``libadapcc.so``
   (for example the one before the filters existed) through its ``adapcc_sample_tokens`` in the same rounds, so the
@@ -34,7 +34,8 @@ GRAPH_LAUNCHES = 50
 NEW_TOKENS = 64
 FILTERS = [("off", {}), ("min_p=0.05", dict(min_p=0.05)), ("typical_p=0.9", dict(typical_p=0.9)),
            ("epsilon_cutoff=3e-4", dict(epsilon_cutoff=3e-4)), ("eta_cutoff=3e-4", dict(eta_cutoff=3e-4)),
-           ("all four", dict(min_p=0.05, typical_p=0.9, epsilon_cutoff=3e-4, eta_cutoff=3e-4))]
+           ("all four", dict(min_p=0.05, typical_p=0.9, epsilon_cutoff=3e-4, eta_cutoff=3e-4)),
+           ("top_h=0.9", dict(top_h=0.9))]
 
 
 def _gpu_info():
