@@ -45,6 +45,7 @@
 
 #include <cmath>
 #include <cstdint>
+#include <type_traits>
 
 #include "common.h"
 #include "sample_filter.cuh"
@@ -680,19 +681,23 @@ struct ReorderArgs {
   const int* parent;           // [R]
   const int* prompt_len;       // [R]: first generated position
   const int* lens;             // [R]: positions held
-  uint4* scratch;              // [R, max_new, L, 2, H, Dh / 8]
+  uint4* scratch;              // [R, max_new, L, 2, H, Dh / 8]; fp8: [R, max_new, L, 2, H, Dh / 16], then the scales
+  float* k_scale;              // fp8 cache (k / v then hold e4m3 bytes): [L, R, H, t_max]; else null
+  float* v_scale;
 };
 
 // one CTA per (generated position t, row r): every layer, k and v, every head. A row that keeps its own parent, a
-// parent out of range and positions at or past lens[r] are skipped.
-template <bool kGather>
+// parent out of range and positions at or past lens[r] are skipped. kFp8: k / v are e4m3 bytes, and the scales move
+// through float [R, max_new, L, 2, H] after the bytes in scratch.
+template <bool kGather, bool kFp8>
 __global__ void __launch_bounds__(kReorderThreads) kv_reorder_kernel(const __grid_constant__ ReorderArgs a) {
+  using T = typename std::conditional<kFp8, uint8_t, __nv_bfloat16>::type;
   const int t = blockIdx.x, r = blockIdx.y;
   const int p = a.parent[r];
   if (p == r || p < 0 || p >= a.R) return;
   const int pos = a.prompt_len[r] + t;
   if (pos < 0 || pos >= a.lens[r] || pos >= a.t_max) return;
-  const int nv = a.Dh / 8;
+  const int nv = a.Dh / (16 / sizeof(T));
   const int per = a.L * 2 * a.H * nv;
   uint4* scr = a.scratch + ((long long)r * a.max_new + t) * per;
   const int src_row = kGather ? p : r;
@@ -702,12 +707,25 @@ __global__ void __launch_bounds__(kReorderThreads) kv_reorder_kernel(const __gri
     const int h = rest % a.H;
     rest /= a.H;
     const int kv = rest & 1, l = rest >> 1;
-    __nv_bfloat16* base = kv ? a.v : a.k;
+    T* base = reinterpret_cast<T*>(kv ? a.v : a.k);
     uint4* cell = reinterpret_cast<uint4*>(base + ((((long long)l * a.R + src_row) * a.H + h) * a.t_max + pos) * a.Dh) + d;
     if (kGather)
       scr[e] = *cell;
     else
       *cell = scr[e];
+  }
+  if constexpr (kFp8) {
+    const int ns = a.L * 2 * a.H;
+    float* sscr = reinterpret_cast<float*>(a.scratch + (long long)a.R * a.max_new * per) +
+                  ((long long)r * a.max_new + t) * ns;
+    for (int e = threadIdx.x; e < ns; e += kReorderThreads) {
+      const int h = e % a.H, kv = (e / a.H) & 1, l = e / (2 * a.H);
+      float* cell = (kv ? a.v_scale : a.k_scale) + (((long long)l * a.R + src_row) * a.H + h) * a.t_max + pos;
+      if (kGather)
+        sscr[e] = *cell;
+      else
+        *cell = sscr[e];
+    }
   }
 }
 
@@ -868,12 +886,20 @@ int adapcc_beam_stochastic_step(const float* logits, int ld, int vocab, int B, i
 }
 
 // k / v bf16 [L, R, H, t_max, Dh] contiguous; parent, prompt_len, lens int32 [R]; scratch at least
-// R * max_new * L * 2 * H * Dh bf16, 16-byte aligned
+// R * max_new * L * 2 * H * Dh bf16, 16-byte aligned. k_scale / v_scale: null for a bf16 cache; with an fp8 cache (k / v
+// e4m3 bytes [L, R, H, t_max, Dh], Dh a multiple of 16) fp32 [L, R, H, t_max], and scratch at least
+// R * max_new * L * 2 * H * (Dh + 4) bytes
 int adapcc_kv_reorder(void* k, void* v, int L, int R, int H, int t_max, int Dh, const int* parent,
-                      const int* prompt_len, const int* lens, int max_new, void* scratch, void* stream) {
+                      const int* prompt_len, const int* lens, int max_new, void* scratch, void* k_scale, void* v_scale,
+                      void* stream) {
   if (L < 1 || R < 1 || R > 65535 || H < 1 || t_max < 1 || Dh < 8 || Dh % 8 != 0 || max_new < 1) {
     set_error("kv_reorder: need L, H, t_max, max_new >= 1, 1 <= R <= 65535, Dh a positive multiple of 8 (L=%d R=%d "
               "H=%d t_max=%d Dh=%d max_new=%d)", L, R, H, t_max, Dh, max_new);
+    return -1;
+  }
+  if (!k_scale != !v_scale || (k_scale && Dh % 16 != 0) || ((uintptr_t)k_scale | (uintptr_t)v_scale) & 3) {
+    set_error("kv_reorder: k_scale and v_scale must both be null, or both 4-byte aligned with Dh a multiple of 16 "
+              "(Dh=%d)", Dh);
     return -1;
   }
   if (!k || !v || !parent || !prompt_len || !lens || !scratch) {
@@ -885,13 +911,19 @@ int adapcc_kv_reorder(void* k, void* v, int L, int R, int H, int t_max, int Dh, 
     return -1;
   }
   ReorderArgs a{(__nv_bfloat16*)k, (__nv_bfloat16*)v, L, R, H, t_max, Dh, max_new, parent, prompt_len, lens,
-                (uint4*)scratch};
+                (uint4*)scratch, (float*)k_scale, (float*)v_scale};
   cudaStream_t s = (cudaStream_t)stream;
   const dim3 grid(max_new, R);
-  kv_reorder_kernel<true><<<grid, kReorderThreads, 0, s>>>(a);
+  if (k_scale)
+    kv_reorder_kernel<true, true><<<grid, kReorderThreads, 0, s>>>(a);
+  else
+    kv_reorder_kernel<true, false><<<grid, kReorderThreads, 0, s>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
-  kv_reorder_kernel<false><<<grid, kReorderThreads, 0, s>>>(a);
+  if (k_scale)
+    kv_reorder_kernel<false, true><<<grid, kReorderThreads, 0, s>>>(a);
+  else
+    kv_reorder_kernel<false, false><<<grid, kReorderThreads, 0, s>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   return 0;

@@ -29,10 +29,18 @@
 // never by arrival: a query's output bits depend on its q, the keys and values it attends and P only, not on B, kq,
 // the other queries, the staging or graph replay versus eager launch. So a candidate or a verify slot is
 // bit-identical to decode_attn at the same keys. lens and nq are only read here.
+//
+// fp8 cache (decode_attn with k_scale / v_scale): every cached key and value vector is Dh e4m3 bytes q and an fp32
+// power-of-two scale 2^e, read as fl32(q) * 2^e (ops/kvcache.py, DESIGN.md §4a). Scaling by a power of two commutes
+// with every fp32 product and sum, so the kernel multiplies a key's dot product by its scale once and folds the value's
+// scale into its weight p, and gives the bits of the bf16 kernel on a bf16 cache holding the dequantized values. The
+// new token attends to its own k / v unquantized (from qkv); the CTA that stores them quantizes them.
 #include <cuda_bf16.h>
+#include <cuda_fp8.h>
 
 #include <cmath>
 #include <cstdint>
+#include <type_traits>
 
 #include "common.h"
 #include "device_prims.cuh"
@@ -59,7 +67,49 @@ struct DecodeArgs {
   __nv_bfloat16* side_k;      // [B * kq, H * Dh]: each query's new key (null: it goes into the cache)
   __nv_bfloat16* side_v;
   int kq, chain, H, Dh, t_max, qkv_stride, n_splits;
+  float* k_scale;             // [B, H, t_max]: with an fp8 cache (k_cache / v_cache then hold e4m3 bytes); else null
+  float* v_scale;
 };
+
+// fl32 of 8 e4m3 bytes (exact: e4m3 -> f16 -> f32)
+__device__ __forceinline__ void unpack_fp8(uint2 v, float* f) {
+  const uint32_t w[2] = {v.x, v.y};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const __half2_raw h = __nv_cvt_fp8x2_to_halfraw2((__nv_fp8x2_storage_t)(w[i >> 1] >> (16 * (i & 1))), __NV_E4M3);
+    const float2 t = __half22float2(__half2(h));
+    f[2 * i] = t.x;
+    f[2 * i + 1] = t.y;
+  }
+}
+
+// Quantizes one bf16 vector of 8 * nvec elements (ops/kvcache.py): lane c < nvec of the 16-lane group holds elements
+// 8c .. 8c + 7 in x (own) and writes their bytes to q + 8c; lane 0 writes the scale. Every lane of the warp calls it
+// (the group's max is a shuffle). amax is the largest |x| as bits: NaN > inf > any finite value, so the max is exact
+// in any order and a non-finite vector is seen whatever its other elements are.
+__device__ __forceinline__ void quantize_fp8(const uint4 x4, bool own, int c, uint8_t* q, float* scale) {
+  float x[8];
+  unpack<__nv_bfloat16>(x4, x);
+  unsigned m = 0;
+  if (own) {
+#pragma unroll
+    for (int e = 0; e < 8; ++e) m = max(m, __float_as_uint(fabsf(x[e])));
+  }
+#pragma unroll
+  for (int o = 8; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+  const float amax = __uint_as_float(m);
+  const bool finite = amax <= 3.402823466e38f;
+  const int ex = finite && amax > 0.f ? ilogbf(amax) - 7 : 0;       // amax * 2^-ex in [128, 256)
+  if (!own) return;
+  uint32_t w[4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 t = make_float2(ldexpf(x[2 * i], -ex), ldexpf(x[2 * i + 1], -ex));
+    w[i] = finite ? (uint32_t)__nv_cvt_float2_to_fp8x2(t, __NV_SATFINITE, __NV_E4M3) : 0u;
+  }
+  *reinterpret_cast<uint2*>(q + c * 8) = make_uint2(w[0] | (w[1] << 16), w[2] | (w[3] << 16));
+  if (c == 0) *scale = finite ? ldexpf(1.f, ex) : __int_as_float(0x7fc00000);
+}
 
 // real queries of cache row b, whose length is L
 __device__ __forceinline__ int decode_queries(const DecodeArgs& a, int b, int L) {
@@ -70,8 +120,11 @@ __device__ __forceinline__ int decode_queries(const DecodeArgs& a, int b, int L)
 // kStaged is chosen at launch: staging the tile costs 37 KB of shared memory and more than twice the registers, which
 // only pays when several queries read it. The unstaged kernel runs one query and stores into the cache; keeping side
 // buffers out of it keeps it at 32 registers (36 with them, which cost decode up to 3 % at 96 (row, head) pairs).
-template <bool kStaged>
+// T is the cache element: __nv_bfloat16, or uint8_t for an fp8 cache (unstaged only).
+template <bool kStaged, typename T>
 __global__ void __launch_bounds__(kDecodeThreads) decode_attn_split_kernel(const __grid_constant__ DecodeArgs a) {
+  constexpr bool kFp8 = std::is_same<T, uint8_t>::value;
+  static_assert(!(kStaged && kFp8), "the staged variant reads a bf16 cache only");
   constexpr int S = kDecodeSplit;
   __shared__ float s_p[S];                          // scores, then exp(score - max)
   __shared__ float s_acc[kDecodeThreads * 8];       // per key group: its partial P.V
@@ -87,10 +140,11 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_attn_split_kernel(const
   const int tid = threadIdx.x, c = tid & (G - 1), grp = tid / G, ngrp = kDecodeThreads / G;
   const bool act = c < nvec;
   const long long head = ((long long)b * a.H + h) * a.t_max * Dh;
-  __nv_bfloat16* kc = a.k_cache + head;
-  __nv_bfloat16* vc = a.v_cache + head;
-  const __nv_bfloat16* tk = kc + (long long)j0 * Dh;   // the split's cached keys and values: key jj at jj * Dh
-  const __nv_bfloat16* tv = vc + (long long)j0 * Dh;
+  T* kc = reinterpret_cast<T*>(a.k_cache) + head;
+  T* vc = reinterpret_cast<T*>(a.v_cache) + head;
+  const T* tk = kc + (long long)j0 * Dh;             // the split's cached keys and values: key jj at jj * Dh
+  const T* tv = vc + (long long)j0 * Dh;
+  const long long sh = ((long long)b * a.H + h) * a.t_max + j0;     // fp8: the scale of key jj at sh + jj
   if constexpr (kStaged) {
     __shared__ __align__(16) __nv_bfloat16 s_k[S * kDecodeMaxDh];
     __shared__ __align__(16) __nv_bfloat16 s_v[S * kDecodeMaxDh];
@@ -125,14 +179,25 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_attn_split_kernel(const
       float d = 0.f;
       if (act && jj < n) {
         float k[8];
-        unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(
-            j >= L ? (kStaged ? qnew + (long long)(j - L) * a.qkv_stride : qrow) + D + c * 8
-                   : tk + jj * Dh + c * 8), k);
+        if constexpr (kFp8) {
+          if (j < L)
+            unpack_fp8(*reinterpret_cast<const uint2*>(tk + jj * Dh + c * 8), k);
+          else
+            unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(qrow + D + c * 8), k);
+        } else {
+          unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(
+              j >= L ? (kStaged ? qnew + (long long)(j - L) * a.qkv_stride : qrow) + D + c * 8
+                     : tk + jj * Dh + c * 8), k);
+        }
 #pragma unroll
         for (int e = 0; e < 8; ++e) d = fmaf(q[e], k[e], d);
       }
       for (int o = G >> 1; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-      if (c == 0 && jj < n) s_p[jj] = d * scale;
+      if constexpr (kFp8) {
+        if (c == 0 && jj < n) s_p[jj] = (j < L ? d * a.k_scale[sh + jj] : d) * scale;
+      } else {
+        if (c == 0 && jj < n) s_p[jj] = d * scale;
+      }
     }
     __syncthreads();
     // 2. max and sum of exp over the split (max is exact in any order; the sum's order is fixed by the layout)
@@ -165,10 +230,19 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_attn_split_kernel(const
       for (int jj = grp; jj < n; jj += ngrp) {
         const int j = j0 + jj;
         float v[8];
-        unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(
-            j >= L ? (kStaged ? qnew + (long long)(j - L) * a.qkv_stride : qrow) + 2 * D + c * 8
-                   : tv + jj * Dh + c * 8), v);
-        const float p = s_p[jj];
+        float p = s_p[jj];
+        if constexpr (kFp8) {
+          if (j < L) {
+            unpack_fp8(*reinterpret_cast<const uint2*>(tv + jj * Dh + c * 8), v);
+            p *= a.v_scale[sh + jj];
+          } else {
+            unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(qrow + 2 * D + c * 8), v);
+          }
+        } else {
+          unpack<__nv_bfloat16>(*reinterpret_cast<const uint4*>(
+              j >= L ? (kStaged ? qnew + (long long)(j - L) * a.qkv_stride : qrow) + 2 * D + c * 8
+                     : tv + jj * Dh + c * 8), v);
+        }
 #pragma unroll
         for (int e = 0; e < 8; ++e) acc[e] = fmaf(p, v[e], acc[e]);
       }
@@ -184,7 +258,17 @@ __global__ void __launch_bounds__(kDecodeThreads) decode_attn_split_kernel(const
     }
     // the query's new k / v are stored last: this CTA read them from qkv above, and no CTA reads position P from the
     // cache
-    if (P < j0 + S && tid < nvec) {
+    if constexpr (kFp8) {
+      if (P < j0 + S && tid < 32) {                 // warp 0: lanes 0 .. nvec - 1 hold the vector
+        const long long ps = ((long long)b * a.H + h) * a.t_max + P;
+        const bool own = tid < nvec;
+        const int c8 = own ? tid * 8 : 0;
+        quantize_fp8(*reinterpret_cast<const uint4*>(qrow + D + c8), own, tid, kc + (long long)P * Dh,
+                     a.k_scale + ps);
+        quantize_fp8(*reinterpret_cast<const uint4*>(qrow + 2 * D + c8), own, tid, vc + (long long)P * Dh,
+                     a.v_scale + ps);
+      }
+    } else if (P < j0 + S && tid < nvec) {
       const bool side = kStaged && a.side_k;
       __nv_bfloat16* nk = side ? a.side_k + bq * D + h * Dh : kc + (long long)P * Dh;
       __nv_bfloat16* nv = side ? a.side_v + bq * D + h * Dh : vc + (long long)P * Dh;
@@ -233,6 +317,27 @@ __global__ void __launch_bounds__(kDecodeMaxDh) decode_attn_combine_kernel(const
   o[t] = __float2bfloat16_rn(acc / l);
 }
 
+// Prefill of an fp8 cache: positions [0, T) of one layer from the c_attn output kv [B, T, 3 * H * Dh] (k at H * Dh,
+// v at 2 * H * Dh), read in place. One CTA per (position t, row b); each 16-lane group quantizes one vector (the k
+// and v of every head in turn), so the grid depends on the shapes only. 2H vectors and an even number of groups per
+// CTA keep the loop bound uniform across each warp, as the shuffles need.
+constexpr int kQuantThreads = 256;
+
+__global__ void __launch_bounds__(kQuantThreads) kv_quantize_kernel(const __nv_bfloat16* kv, uint8_t* k, uint8_t* v,
+                                                                    float* k_scale, float* v_scale, int H, int Dh,
+                                                                    int T, int t_max) {
+  const int t = blockIdx.x, b = blockIdx.y, D = H * Dh;
+  const int c = threadIdx.x & 15;
+  const bool own = c < (Dh >> 3);
+  const __nv_bfloat16* row = kv + ((long long)b * T + t) * 3 * D;
+  for (int g = threadIdx.x >> 4; g < 2 * H; g += kQuantThreads / 16) {
+    const int h = g >> 1, isv = g & 1;
+    const uint4 x = own ? *reinterpret_cast<const uint4*>(row + (1 + isv) * D + h * Dh + c * 8) : make_uint4(0, 0, 0, 0);
+    const long long cell = ((long long)b * H + h) * t_max + t;
+    quantize_fp8(x, own, c, (isv ? v : k) + cell * Dh, (isv ? v_scale : k_scale) + cell);
+  }
+}
+
 inline int decode_splits(int t_max) { return (t_max + kDecodeSplit - 1) / kDecodeSplit; }
 
 // Checks the arguments of the C entry point `who` (the prefix of its errors), whose rows hold 1..max_kq queries, and
@@ -261,13 +366,21 @@ static int decode_attn_launch(const char* who, int max_kq, DecodeArgs a, int B, 
     set_error("%s: lens and work must be non-null, and lens, nq and work 4-byte aligned", who);
     return -1;
   }
+  if (!a.k_scale != !a.v_scale || ((uintptr_t)a.k_scale | (uintptr_t)a.v_scale) & 3 ||
+      (a.k_scale && (kq != 1 || a.side_k))) {
+    set_error("%s: k_scale and v_scale must both be null or both 4-byte aligned, and an fp8 cache takes one query per "
+              "row and no side buffers", who);
+    return -1;
+  }
   a.n_splits = decode_splits(t_max);
   cudaStream_t s = (cudaStream_t)stream;
   const dim3 grid(a.n_splits, H, B);
-  if (kq == 1 && !a.side_k)
-    decode_attn_split_kernel<false><<<grid, kDecodeThreads, 0, s>>>(a);
+  if (a.k_scale)
+    decode_attn_split_kernel<false, uint8_t><<<grid, kDecodeThreads, 0, s>>>(a);
+  else if (kq == 1 && !a.side_k)
+    decode_attn_split_kernel<false, __nv_bfloat16><<<grid, kDecodeThreads, 0, s>>>(a);
   else
-    decode_attn_split_kernel<true><<<grid, kDecodeThreads, 0, s>>>(a);
+    decode_attn_split_kernel<true, __nv_bfloat16><<<grid, kDecodeThreads, 0, s>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
   decode_attn_combine_kernel<<<dim3(H, kq, B), kDecodeMaxDh, 0, s>>>(a);
@@ -289,13 +402,42 @@ long long adapcc_decode_attn_work(int B, int H, int Dh, int t_max) {
 }
 
 // qkv: bf16 [B, qkv_stride] (q | k | v of the new token, H * Dh each); k_cache / v_cache: bf16 [B, H, t_max, Dh];
-// lens: int32 [B] (keys already cached; read only); out: bf16 [B, H * Dh]; work: fp32, adapcc_decode_attn_work elements
+// lens: int32 [B] (keys already cached; read only); out: bf16 [B, H * Dh]; work: fp32, adapcc_decode_attn_work elements.
+// k_scale / v_scale: null for a bf16 cache; with an fp8 cache (k_cache / v_cache e4m3 bytes [B, H, t_max, Dh]) fp32
+// [B, H, t_max], the scale of each cached vector
 int adapcc_decode_attn(const void* qkv, void* k_cache, void* v_cache, const int* lens, void* out, int B, int H, int Dh,
-                       int t_max, int qkv_stride, void* work, void* stream) {
-  const DecodeArgs a{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, lens, nullptr,
-                     (float*)work, (__nv_bfloat16*)out, nullptr, nullptr, /*kq=*/1, /*chain=*/0, H, Dh, t_max,
-                     qkv_stride};
+                       int t_max, int qkv_stride, void* work, void* k_scale, void* v_scale, void* stream) {
+  DecodeArgs a{(const __nv_bfloat16*)qkv, (__nv_bfloat16*)k_cache, (__nv_bfloat16*)v_cache, lens, nullptr,
+               (float*)work, (__nv_bfloat16*)out, nullptr, nullptr, /*kq=*/1, /*chain=*/0, H, Dh, t_max, qkv_stride};
+  a.k_scale = (float*)k_scale;
+  a.v_scale = (float*)v_scale;
   return decode_attn_launch("decode_attn", 1, a, B, stream);
+}
+
+// Prefill of one layer's fp8 cache: positions [0, T) of every row. kv: bf16 [B, T, 3 * H * Dh] contiguous (the c_attn
+// output); k_cache / v_cache: e4m3 bytes [B, H, t_max, Dh]; k_scale / v_scale: fp32 [B, H, t_max]
+int adapcc_kv_quantize(const void* kv, void* k_cache, void* v_cache, void* k_scale, void* v_scale, int B, int T, int H,
+                       int Dh, int t_max, void* stream) {
+  if (B < 1 || B > 65535 || H < 1 || T < 1 || T > t_max || Dh < 8 || Dh > kDecodeMaxDh || Dh % 8 != 0) {
+    set_error("kv_quantize: need 1 <= B <= 65535, H >= 1, 1 <= T <= t_max and Dh a multiple of 8 in [8, %d] (B=%d "
+              "T=%d H=%d Dh=%d t_max=%d)", kDecodeMaxDh, B, T, H, Dh, t_max);
+    return -1;
+  }
+  if (!kv || !k_cache || !v_cache || !k_scale || !v_scale) {
+    set_error("kv_quantize: null pointer");
+    return -1;
+  }
+  if (((uintptr_t)kv & 15) || (((uintptr_t)k_cache | (uintptr_t)v_cache) & 7) ||
+      (((uintptr_t)k_scale | (uintptr_t)v_scale) & 3)) {
+    set_error("kv_quantize: kv must be 16-byte, the caches 8-byte and the scales 4-byte aligned");
+    return -1;
+  }
+  kv_quantize_kernel<<<dim3(T, B), kQuantThreads, 0, (cudaStream_t)stream>>>(
+      (const __nv_bfloat16*)kv, (uint8_t*)k_cache, (uint8_t*)v_cache, (float*)k_scale, (float*)v_scale, H, Dh, T,
+      t_max);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
 }
 
 // Contrastive-search candidates: kq queries per row, all at position lens[b]. qkv: bf16 [B * kq, qkv_stride];

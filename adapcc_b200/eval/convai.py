@@ -96,7 +96,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    assistant_verification: str = "coupled", beam_sample: bool = False, num_beam_groups: int = 1,
                    diversity_penalty: float = 0.0, guidance_scale: float = 1.0,
                    guidance_negative: str = "last_token", sequence_bias=None,
-                   bad_words_ids=None, top_h: float = 0.0) -> List[List[int]]:
+                   bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -121,7 +121,9 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     prompt is), so guidance pushes each reply towards its persona. Guidance with ``num_beams``, ``penalty_alpha``,
     prompt lookup or an assistant is a ``ValueError``. ``sequence_bias`` and ``bad_words_ids`` (HuggingFace's; token
     ids of the dialogue tokenizer) go to ``generate`` / ``beam_search`` / ``contrastive_search`` (``ops/repeats.py``);
-    with prompt lookup or an assistant they are a ``ValueError``."""
+    with prompt lookup or an assistant they are a ``ValueError``. ``kv_cache_dtype`` (``"fp8_e4m3"``: an fp8 KV
+    cache, ``ops/kvcache.py``) goes to ``generate`` / ``beam_search``; with ``penalty_alpha``, prompt lookup or an
+    assistant it is a ``ValueError``."""
     from ..ops.assisted import check_verification
     check_verification("sample_replies", assistant_verification, assistant_model)
     if assistant_model is not None and (num_beams > 0 or penalty_alpha > 0):
@@ -157,7 +159,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     reply_type = torch.tensor([i.token_type_ids[-1] for i in insts], device=device)
     seed = torch.tensor(list(seeds) if seeds is not None else range(len(insts)), dtype=torch.int64)
     special = list(tokenizer.special_ids)
-    repeats = dict(repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size)
+    repeats = dict(repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
+                   kv_cache_dtype=kv_cache_dtype)
     filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff, top_h=top_h)
     if sequence_bias is not None:
         repeats["sequence_bias"] = sequence_bias
@@ -287,7 +290,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      num_assistant_tokens: int = 4, assistant_verification: str = "coupled",
                      beam_sample: bool = False, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
                      guidance_scale: float = 1.0, guidance_negative: str = "last_token", sequence_bias=None,
-                     bad_words_ids=None, top_h: float = 0.0, **sample_kw) -> Dict[str, float]:
+                     bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
+                     **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -320,7 +324,10 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``assistant_verification="rejection"`` (rejection sampling: replies from the same distribution, other draws).
 
     ``guidance_scale != 1`` with ``f1``: classifier-free guidance against ``guidance_negative`` (``"last_token"`` or
-    ``"no_persona"``, see :func:`sample_replies`), on that batched path."""
+    ``"no_persona"``, see :func:`sample_replies`), on that batched path.
+
+    ``kv_cache_dtype="fp8_e4m3"`` with ``f1``: the replies are decoded with an fp8 KV cache (``ops/kvcache.py``), on
+    that batched path; comparing F1 with and without it measures what the quantization costs."""
     from ..ops.assisted import check_verification
     check_verification("evaluate_dialogs", assistant_verification, assistant_model)
     repeats = (repetition_penalty != 1.0 or no_repeat_ngram_size > 0 or bool(sequence_bias)
@@ -331,7 +338,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0 or top_h > 0
     assisted = assistant_model is not None
     if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup or filtered
-            or assisted or guidance_scale != 1.0) and eval_type == "f1":
+            or assisted or guidance_scale != 1.0 or kv_cache_dtype is not None) and eval_type == "f1":
         return _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples, device, seed,
                                     max(batch_size, 1), num_beams=num_beams, repetition_penalty=repetition_penalty,
                                     no_repeat_ngram_size=no_repeat_ngram_size, penalty_alpha=penalty_alpha,
@@ -340,7 +347,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                                     assistant_verification=assistant_verification, beam_sample=beam_sample,
                                     num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty,
                                     guidance_scale=guidance_scale, guidance_negative=guidance_negative, **bias,
-                                    **sample_kw)
+                                    kv_cache_dtype=kv_cache_dtype, **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -31,6 +31,7 @@ import torch.nn.functional as F
 
 from ..ops.dropout import DropoutState, check_p, dropout, site_attn, site_embed, site_mlp, site_summary
 from ..ops.guidance import check_guidance_args, guided_scores_reference
+from ..ops.kvcache import check_kv_cache_dtype
 from ..ops.layers import FusedLayerNorm, FusedLinear
 from ..ops.repeats import check_repeat_args, check_sequence_bias_args, penalize_repeats_reference
 from ..ops.sampling import check_filter_args, sample_reference, top_filtering
@@ -117,12 +118,24 @@ class KVCache:
     [L, B, H, t_max, Dh] in the model's dtype, ``lens`` (int32 [B] on the device: tokens cached per row, what the
     kernels read), ``host_lens`` (the same numbers on the host, which issues every step and so always knows them) and
     ``work``, the split-partials workspace of the native decode-attention kernel (bf16 on CUDA; None otherwise),
-    allocated once so a captured step reuses it."""
+    allocated once so a captured step reuses it.
 
-    def __init__(self, n_layer: int, batch: int, n_head: int, t_max: int, head_dim: int, dtype: torch.dtype, device):
+    ``kv_cache_dtype="fp8_e4m3"``: ``k`` / ``v`` hold e4m3 bytes (uint8) and ``k_scale`` / ``v_scale`` (fp32
+    [L, B, H, t_max]) the power-of-two scale of each vector, as ``ops/kvcache.py`` defines; every cached position is
+    quantized, the prompt's included. Otherwise the scales are None."""
+
+    def __init__(self, n_layer: int, batch: int, n_head: int, t_max: int, head_dim: int, dtype: torch.dtype, device,
+                 kv_cache_dtype: Optional[str] = None):
         self.batch, self.t_max = int(batch), int(t_max)
-        self.k = torch.zeros(n_layer, batch, n_head, t_max, head_dim, dtype=dtype, device=device)
+        self.kv_cache_dtype = check_kv_cache_dtype("KVCache", kv_cache_dtype)
+        fp8 = kv_cache_dtype is not None
+        self.k = torch.zeros(n_layer, batch, n_head, t_max, head_dim, dtype=torch.uint8 if fp8 else dtype,
+                             device=device)
         self.v = torch.zeros_like(self.k)
+        self.k_scale = self.v_scale = None
+        if fp8:
+            self.k_scale = torch.zeros(n_layer, batch, n_head, t_max, dtype=torch.float32, device=self.k.device)
+            self.v_scale = torch.zeros_like(self.k_scale)
         self.lens = torch.zeros(batch, dtype=torch.int32, device=self.k.device)
         self.host_lens: List[int] = [0] * self.batch
         self.work = None
@@ -130,6 +143,18 @@ class KVCache:
             from ..ops import decode_attention_work_numel
             self.work = torch.empty(decode_attention_work_numel(batch, n_head, head_dim, t_max), dtype=torch.float32,
                                     device=self.k.device)
+
+    @property
+    def parts(self) -> List[torch.Tensor]:
+        """Every per-position tensor: ``k``, ``v`` and, with an fp8 cache, ``k_scale`` and ``v_scale`` (each indexed
+        [layer, row, head, position, ...])."""
+        return [self.k, self.v] + ([self.k_scale, self.v_scale] if self.k_scale is not None else [])
+
+    def scales(self, layer: int):
+        """``(k_scale, v_scale)`` of layer ``layer``; (None, None) for a cache in the model's dtype."""
+        if self.k_scale is None:
+            return None, None
+        return self.k_scale[layer], self.v_scale[layer]
 
     def reset(self, lengths: Sequence[int], T: int) -> None:
         """Lengths after a prefill of T (right-padded) positions."""
@@ -154,25 +179,37 @@ class KVCache:
 
 
 def decode_attention(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
-                     work: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     work: Optional[torch.Tensor] = None, k_scale: Optional[torch.Tensor] = None,
+                     v_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """One layer of decode attention: ``qkv`` [B, 3·H·Dh] (q | k | v of each row's new token), caches [B, H, t_max, Dh],
     ``lens`` int32 [B]. Stores the new k / v at position ``lens[b]`` and returns softmax(q·K[0..lens[b]]ᵀ/√Dh)·V [B, H·Dh]
     with an fp32 softmax. With ``work`` (bf16 CUDA caches) this is the native kernel (``ops.decode_attention_``);
-    otherwise the same computation in PyTorch, the reference the CPU tests use."""
+    otherwise the same computation in PyTorch, the reference the CPU tests use. With ``k_scale`` / ``v_scale`` (fp32
+    [B, H, t_max]) the caches are fp8 (``ops/kvcache.py``): the new k / v are stored quantized, and the new token
+    attends to them unquantized and to the dequantized cache before ``lens[b]``."""
     B, H, t_max, Dh = k_cache.shape
     if work is not None:
         from ..ops import decode_attention_
         out = torch.empty(B, H * Dh, dtype=qkv.dtype, device=qkv.device)
-        return decode_attention_(qkv, k_cache, v_cache, lens, out, work)
+        return decode_attention_(qkv, k_cache, v_cache, lens, out, work, k_scale=k_scale, v_scale=v_scale)
     q, k, v = qkv.reshape(B, 3, H, Dh).unbind(1)
     pos = lens.long()
     rows = torch.arange(B, device=qkv.device)
-    k_cache[rows, :, pos] = k
-    v_cache[rows, :, pos] = v
-    s = torch.einsum("bhd,bhtd->bht", q.float(), k_cache.float()) / math.sqrt(Dh)
+    if k_scale is not None:
+        from ..ops.kvcache import dequantize, quantize
+        keys, values = dequantize(k_cache, k_scale), dequantize(v_cache, v_scale)
+        keys[rows, :, pos] = k.float()
+        values[rows, :, pos] = v.float()
+        for x, qc, sc in ((k, k_cache, k_scale), (v, v_cache, v_scale)):
+            qc[rows, :, pos], sc[rows, :, pos] = quantize(x)
+    else:
+        k_cache[rows, :, pos] = k
+        v_cache[rows, :, pos] = v
+        keys, values = k_cache.float(), v_cache.float()
+    s = torch.einsum("bhd,bhtd->bht", q.float(), keys) / math.sqrt(Dh)
     s = s.masked_fill(torch.arange(t_max, device=qkv.device) > pos[:, None, None], float("-inf"))
     p = torch.softmax(s, dim=-1)
-    return torch.einsum("bht,bhtd->bhd", p, v_cache.float()).to(qkv.dtype).reshape(B, H * Dh)
+    return torch.einsum("bht,bhtd->bhd", p, values).to(qkv.dtype).reshape(B, H * Dh)
 
 
 class CandidateKV:
@@ -322,12 +359,23 @@ class Block(nn.Module):
         if isinstance(cache, (CandidateKV, VerifyKV)):   # contrastive search / prompt lookup: k + 1 slots per row
             return self.c_proj(cache.attend(self.c_attn(h), layer))
         if cache is not None and h.dim() == 2:       # decode: one new token per row [B, D] against the cache
-            return self.c_proj(decode_attention(self.c_attn(h), cache.k[layer], cache.v[layer], cache.lens, cache.work))
+            return self.c_proj(decode_attention(self.c_attn(h), cache.k[layer], cache.v[layer], cache.lens, cache.work,
+                                                *cache.scales(layer)))
         B, T, D = h.shape
         # split along the feature dim (views; measured 6 % faster fwd+bwd than the packed permute:
         # the backward writes dq/dk/dv straight into one [B, T, 3D] buffer layout-wise)
-        q, k, v = (t.view(B, T, self.n_head, D // self.n_head).transpose(1, 2) for t in self.c_attn(h).split(D, dim=-1))
-        if cache is not None:                         # prefill: keep this layer's keys and values
+        qkv = self.c_attn(h)
+        q, k, v = (t.view(B, T, self.n_head, D // self.n_head).transpose(1, 2) for t in qkv.split(D, dim=-1))
+        if cache is not None and cache.k_scale is not None:     # prefill of an fp8 cache: quantize every position
+            ks, vs = cache.scales(layer)
+            if cache.work is not None:
+                from ..ops import kv_quantize_
+                kv_quantize_(qkv.detach(), cache.k[layer], cache.v[layer], ks, vs)
+            else:
+                from ..ops.kvcache import store_
+                store_(k.detach(), cache.k[layer, :, :, :T], ks[:, :, :T])
+                store_(v.detach(), cache.v[layer, :, :, :T], vs[:, :, :T])
+        elif cache is not None:                       # prefill: keep this layer's keys and values
             cache.k[layer, :, :, :T].copy_(k.detach())
             cache.v[layer, :, :, :T].copy_(v.detach())
         a = causal_attention(q, k, v)
@@ -588,15 +636,16 @@ class GPT2DoubleHeads(nn.Module):
             x = blk(x, cache, i, drop)
         return self.ln_f(x)
 
-    def new_cache(self, batch: int, t_max: Optional[int] = None) -> "KVCache":
+    def new_cache(self, batch: int, t_max: Optional[int] = None, kv_cache_dtype: Optional[str] = None) -> "KVCache":
         """An empty KV cache for ``batch`` rows of up to ``t_max`` (default ``n_positions``) tokens, on the model's
-        device and in its dtype."""
+        device and in its dtype, or in fp8 with ``kv_cache_dtype="fp8_e4m3"`` (``ops/kvcache.py``)."""
         cfg = self.cfg
         t_max = cfg.n_positions if t_max is None else int(t_max)
         if not 1 <= t_max <= cfg.n_positions:
             raise ValueError(f"new_cache: t_max must be in [1, {cfg.n_positions}], got {t_max}")
         w = self.wte.weight
-        return KVCache(cfg.n_layer, batch, cfg.n_head, t_max, cfg.n_embd // cfg.n_head, w.dtype, w.device)
+        return KVCache(cfg.n_layer, batch, cfg.n_head, t_max, cfg.n_embd // cfg.n_head, w.dtype, w.device,
+                       kv_cache_dtype)
 
     @torch.no_grad()
     def decode_step(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], cache: "KVCache") -> torch.Tensor:
@@ -617,13 +666,14 @@ class GPT2DoubleHeads(nn.Module):
                       token_type_ids: Optional[torch.Tensor], reply_type, max_new_tokens: int, min_new_tokens: int,
                       repetition_penalty: float, no_repeat_ngram_size: int, num_beams: int = 1,
                       rows_name: str = "beam rows (batch x num_beams)", sequence_bias=None, bad_words_ids=None,
-                      stop_ids: Sequence[int] = ()):
+                      stop_ids: Sequence[int] = (), kv_cache_dtype: Optional[str] = None):
         """The checks and prompt quantities the batched decoders share, before anything is launched:
         ``(B, T, lengths, n, t_max, last, tt_new, native, bias)``. ``last`` [B] is each prompt's last position,
         ``tt_new`` [B] the token type of new tokens (None without token types), ``native`` says whether the bf16 CUDA
         kernels run; they take at most ``LM_HEAD_MAX_ROWS`` rows, ``num_beams`` per prompt (called ``rows_name`` in
         the error when more than one). ``bias`` is the table of ``sequence_bias`` and ``bad_words_ids``
-        (``ops.repeats.check_sequence_bias_args``; None when both are off). Errors name ``who``."""
+        (``ops.repeats.check_sequence_bias_args``; None when both are off). ``kv_cache_dtype`` must be None or one of
+        ``ops.kvcache.KV_CACHE_DTYPES``. Errors name ``who``."""
         from ..ops import LM_HEAD_MAX_ROWS
 
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
@@ -638,6 +688,7 @@ class GPT2DoubleHeads(nn.Module):
             raise ValueError(f"{who}: need max_new_tokens >= 1 and min_new_tokens >= 0, got {max_new_tokens}, "
                              f"{min_new_tokens}")
         check_repeat_args(who, repetition_penalty, no_repeat_ngram_size)
+        check_kv_cache_dtype(who, kv_cache_dtype)
         bias = check_sequence_bias_args(who, sequence_bias, bad_words_ids, self.cfg.vocab_size, stop_ids)
         t_max = max(lengths) + n
         if t_max > self.cfg.n_positions:
@@ -719,7 +770,8 @@ class GPT2DoubleHeads(nn.Module):
                  assistant_verification: str = "coupled", guidance_scale: float = 1.0,
                  negative_prompt_ids: Optional[torch.Tensor] = None, negative_lengths: Optional[Sequence[int]] = None,
                  negative_token_type_ids: Optional[torch.Tensor] = None, sequence_bias=None,
-                 bad_words_ids=None, top_h: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor]:
+                 bad_words_ids=None, top_h: float = 0.0,
+                 kv_cache_dtype: Optional[str] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -790,7 +842,13 @@ class GPT2DoubleHeads(nn.Module):
         tokens take the same type in both rows. Not with prompt lookup or an assistant. The cache then holds 2B rows, prompts
         first (at most ``LM_HEAD_MAX_ROWS`` on the native path), prefilled together; on the native path each graph
         replay runs the decode step and LM head on all of them and ``ops.guidance_mix_`` after the head. Prompt rows
-        draw from the same seeds and positions as without guidance."""
+        draw from the same seeds and positions as without guidance.
+
+        ``kv_cache_dtype="fp8_e4m3"`` keeps the KV cache in fp8 (``ops/kvcache.py``): each cached key and value vector
+        as e4m3 bytes with a power-of-two scale, half the bytes of bf16 for every decode step to read. Every cached
+        position is quantized, the prompt's included; the prefill attends to the unquantized keys and values, and each
+        new token to its own. On the native path the prefill quantizes through ``ops.kv_quantize_`` and every step
+        runs the fp8 ``ops.decode_attention_``. Not with prompt lookup or an assistant (``ValueError``)."""
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
@@ -804,6 +862,10 @@ class GPT2DoubleHeads(nn.Module):
                                           negative_token_type_ids, token_type_ids, max_new_tokens, self.cfg.n_positions)
         guided = neg_lengths is not None
         speculative = assistant_model is not None or prompt_lookup_num_tokens != 0
+        if speculative and kv_cache_dtype is not None:
+            raise ValueError("generate: kv_cache_dtype cannot be combined with prompt_lookup_num_tokens or "
+                             f"assistant_model (got {kv_cache_dtype!r}, {prompt_lookup_num_tokens}, "
+                             f"{type(assistant_model).__name__})")
         if speculative and (sequence_bias or bad_words_ids):
             raise ValueError("generate: sequence_bias and bad_words_ids cannot be combined with "
                              f"prompt_lookup_num_tokens or assistant_model (got {prompt_lookup_num_tokens}, "
@@ -831,7 +893,7 @@ class GPT2DoubleHeads(nn.Module):
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, num_beams=2 if guided else 1,
             rows_name="rows with guidance (batch x 2)", sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
-            stop_ids=stop_ids)
+            stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype)
         dev, V = input_ids.device, self.cfg.vocab_size
         seeds = _row_seeds(seed, B, dev)
         if guided:                                  # rows [0, B): the prompts, rows [B, 2B): the negative prompts
@@ -843,7 +905,7 @@ class GPT2DoubleHeads(nn.Module):
         else:
             ids_all, tt_all, lengths_all = input_ids, token_type_ids, lengths
         R = len(lengths_all)
-        cache = self.new_cache(R, t_max)
+        cache = self.new_cache(R, t_max, kv_cache_dtype)
         h = self.hidden(ids_all, tt_all, cache=cache, lengths=lengths_all)[torch.arange(R, device=dev), last]
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
         reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, B, bias)
@@ -902,8 +964,8 @@ class GPT2DoubleHeads(nn.Module):
                     top_k: int = 0, top_p: float = 1.0, seed=0,
                     num_return_sequences: int = 1, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
                     sequence_bias=None, bad_words_ids=None, min_p: float = 0.0, typical_p: float = 1.0,
-                    epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
-                    top_h: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0,
+                    kv_cache_dtype: Optional[str] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -948,7 +1010,10 @@ class GPT2DoubleHeads(nn.Module):
         tokens, a period late. Beam sampling takes a vocabulary of at most ``ops.SAMPLE_MAX_VOCAB`` ids there, and
         the items' seeds are a device input of the graph. Elsewhere the same loop runs eagerly with fp32 PyTorch logits,
         ``ops.repeats.penalize_repeats_reference``, ``ops.beam.GroupBeamReference`` (``BeamSampleReference`` with
-        ``do_sample``) and torch indexing."""
+        ``do_sample``) and torch indexing.
+
+        ``kv_cache_dtype="fp8_e4m3"`` keeps the KV cache in fp8 as in ``generate``; the cache reordering then moves
+        the bytes and the scales."""
         from ..ops import SAMPLE_MAX_VOCAB, BeamState
         from ..ops.beam import BeamSampleReference, GroupBeamReference, best_hypotheses, merge_finished_sets
 
@@ -988,7 +1053,7 @@ class GPT2DoubleHeads(nn.Module):
 
         sel = self._beam_decode("beam_search", input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
                                 min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
-                                sequence_bias, bad_words_ids)
+                                sequence_bias, bad_words_ids, kv_cache_dtype)
         dev, B, n = input_ids.device, input_ids.shape[0], int(max_new_tokens)
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result(R))
@@ -1006,7 +1071,7 @@ class GPT2DoubleHeads(nn.Module):
                                min_new_tokens: int = 0, repetition_penalty: float = 1.0,
                                no_repeat_ngram_size: int = 0, seed=0, sequence_bias=None, bad_words_ids=None,
                                min_p: float = 0.0, typical_p: float = 1.0, epsilon_cutoff: float = 0.0,
-                               eta_cutoff: float = 0.0, top_h: float = 0.0):
+                               eta_cutoff: float = 0.0, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None):
         """Stochastic beam search (Kool, van Hoof and Welling 2019): ``num_beams`` = K distinct replies per prompt,
         drawn without replacement from the law ``generate`` samples from with the same ``temperature``, ``top_k``,
         ``top_p``, truncation filters (``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff``, ``top_h``), stop /
@@ -1014,7 +1079,8 @@ class GPT2DoubleHeads(nn.Module):
         and ``max_new_tokens``; the definition
         (rules R1-R8, properties P1-P4) is ``ops.beam.StochasticBeamReference``. The first reply of an item is itself
         an exact sample of that law. ``seed``: an int (item b uses ``seed + b``) or an int64 [B] tensor; an item's
-        result depends on its prompt, its seed and the scalars only. The other arguments work as in ``beam_search``.
+        result depends on its prompt, its seed and the scalars only. The other arguments work as in ``beam_search``,
+        ``kv_cache_dtype`` included.
 
         Returns ``(tokens, n_new, log_probs, keys, kappa)``: rows ``b·K + q``, the largest key first, of int64 [B·K,
         max_new_tokens] (the stop token excluded, padded with -1), int64 [B·K] lengths, fp32 [B·K] log-probabilities
@@ -1050,7 +1116,7 @@ class GPT2DoubleHeads(nn.Module):
 
         sel = self._beam_decode(who, input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
                                 min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
-                                sequence_bias, bad_words_ids)
+                                sequence_bias, bad_words_ids, kv_cache_dtype)
         dev = input_ids.device
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result())
@@ -1064,7 +1130,7 @@ class GPT2DoubleHeads(nn.Module):
     def _beam_decode(self, who: str, input_ids: torch.Tensor, lengths, token_type_ids, reply_type, K: int,
                      max_new_tokens: int, min_new_tokens: int, repetition_penalty: float, no_repeat_ngram_size: int,
                      stop_ids: Sequence[int], suppress_ids: Sequence[int], start, sequence_bias=None,
-                     bad_words_ids=None):
+                     bad_words_ids=None, kv_cache_dtype: Optional[str] = None):
         """The decode loop of the beam decoders. ``start(B, n, V, device, native)`` is called after the argument checks
         and before anything is launched; it returns the selector: on the native path ``(BeamState, keyword arguments
         of beam_step_)``, elsewhere a reference with ``step(logits) -> (next_ids, parent)`` and ``done``. Each prompt
@@ -1077,18 +1143,18 @@ class GPT2DoubleHeads(nn.Module):
         B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(
             who, input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, num_beams=K, sequence_bias=sequence_bias,
-            bad_words_ids=bad_words_ids, stop_ids=stop_ids)
+            bad_words_ids=bad_words_ids, stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype)
         dev, V, weight = input_ids.device, self.cfg.vocab_size, self.wte.weight
         sel = start(B, n, V, dev, native)
         if tt_new is not None:
             tt_new = tt_new.repeat_interleave(K)
         # one prefill per prompt, its keys and values copied to the prompt's K rows (the beams share that region)
-        pre = self.new_cache(B, T)
+        pre = self.new_cache(B, T, kv_cache_dtype)
         h = self.hidden(input_ids, token_type_ids, cache=pre, lengths=lengths)[torch.arange(B, device=dev), last]
-        cache = self.new_cache(B * K, t_max)
+        cache = self.new_cache(B * K, t_max, kv_cache_dtype)
         cache.reset([x for x in lengths for _ in range(K)], T)
-        cache.k[:, :, :, :T].copy_(pre.k.repeat_interleave(K, dim=1))
-        cache.v[:, :, :, :T].copy_(pre.v.repeat_interleave(K, dim=1))
+        for dst, src in zip(cache.parts, pre.parts):
+            dst[:, :, :, :T].copy_(src.repeat_interleave(K, dim=1))
         del pre
         h = h.repeat_interleave(K, dim=0).contiguous()
         reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, bias=bias)
@@ -1102,8 +1168,8 @@ class GPT2DoubleHeads(nn.Module):
                     logits = reps.eager(logits, cache, nxt if i else None)
                 nxt, parent = sel.step(logits)
                 rows = parent.to(dev)
-                cache.k.copy_(cache.k[:, rows])
-                cache.v.copy_(cache.v[:, rows])
+                for t in cache.parts:
+                    t.copy_(t[:, rows])
                 if reps is not None:
                     reps.reorder(rows)
                 if sel.done.all():
@@ -1114,14 +1180,16 @@ class GPT2DoubleHeads(nn.Module):
         logits = torch.empty(B * K, weight.shape[0], dtype=torch.float32, device=dev)
         sup, stop = (torch.tensor(list(x), dtype=torch.int32, device=dev) for x in (suppress_ids, stop_ids))
         prompt_len = cache.lens.clone()
-        scratch = torch.empty(kv_reorder_scratch_numel(cache.k, n), dtype=cache.k.dtype, device=dev)
+        fp8 = cache.k_scale is not None
+        scratch = torch.empty(kv_reorder_scratch_numel(cache.k, n, fp8=fp8), dtype=cache.k.dtype, device=dev)
 
         def select(hidden):
             lm_head_logits_(hidden, weight, logits)
             if reps is not None:
                 reps.native(logits, cache.lens, st.step, st.next_ids, st.parent, K)
             beam_step_(logits, V, st, min_new_tokens, sup, stop, **scalars)
-            kv_reorder_(cache.k, cache.v, st.parent, prompt_len, cache.lens, n, scratch)
+            kv_reorder_(cache.k, cache.v, st.parent, prompt_len, cache.lens, n, scratch, k_scale=cache.k_scale,
+                        v_scale=cache.v_scale)
 
         select(h)                                   # the first selection, from the prefill's last positions
         if n > 1:
@@ -1283,8 +1351,8 @@ class GPT2DoubleHeads(nn.Module):
                            token_type_ids: Optional[torch.Tensor] = None, reply_type=None, top_k: int = 4,
                            penalty_alpha: float = 0.6, max_new_tokens: int = 20, stop_ids: Sequence[int] = (),
                            suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
-                           no_repeat_ngram_size: int = 0, sequence_bias=None,
-                           bad_words_ids=None) -> Tuple[torch.Tensor, torch.Tensor]:
+                           no_repeat_ngram_size: int = 0, sequence_bias=None, bad_words_ids=None,
+                           kv_cache_dtype: Optional[str] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched contrastive search (Su et al., 2022; HuggingFace's ``penalty_alpha`` + ``top_k``); the definition is
         in ``ops/contrastive.py``.
 
@@ -1304,10 +1372,14 @@ class GPT2DoubleHeads(nn.Module):
         next candidates (``ops.contrastive_select_``);
         the host reads the done flags once every 8 tokens, a period late. Elsewhere the same loop runs eagerly:
         candidates decode through ``decode_attention`` on a k-fold copy of the rows and the selection runs in fp64
-        (``ops/contrastive.py``)."""
+        (``ops/contrastive.py``). The cache is in the model's dtype: ``kv_cache_dtype`` other than None is a
+        ``ValueError``."""
         from ..ops import CONTRASTIVE_MAX_K
         from ..ops.contrastive import check_contrastive_args, rerank_row, select_candidates
 
+        if kv_cache_dtype is not None:
+            raise ValueError(f"contrastive_search: kv_cache_dtype must be None (an fp8 cache is not supported), got "
+                             f"{kv_cache_dtype!r}")
         check_contrastive_args("contrastive_search", top_k, penalty_alpha, CONTRASTIVE_MAX_K)
         K, alpha = int(top_k), float(penalty_alpha)
         B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(

@@ -45,7 +45,8 @@ def _lib():
         lib.adapcc_embed_sum_drop_bwd.argtypes = ([c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p,
                                                    c_void_p, c_void_p] + drop + [c_void_p])
         lib.adapcc_embed_bwd_reset.argtypes = [c_void_p, c_void_p, c_longlong, c_void_p, c_longlong, c_void_p]
-        lib.adapcc_decode_attn.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p, c_void_p]
+        lib.adapcc_decode_attn.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p] * 4
+        lib.adapcc_kv_quantize.argtypes = [c_void_p] * 5 + [c_int] * 5 + [c_void_p]
         lib.adapcc_decode_attn_work.argtypes = [c_int] * 4
         lib.adapcc_decode_attn_work.restype = c_longlong
         lib.adapcc_lm_head_logits.argtypes = [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_int, c_void_p]
@@ -67,8 +68,7 @@ def _lib():
                                                      c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                                     + [c_void_p] * 14 + [c_float, c_int, c_float, c_void_p]
                                                     + [c_float] * 5 + [c_void_p])
-        lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int, c_void_p,
-                                                                                                c_void_p]
+        lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int] + [c_void_p] * 4
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
                                                 + [c_int, c_float, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p])
         lib.adapcc_guidance_mix.argtypes = [c_void_p, c_int, c_int, c_int, c_float, c_void_p]
@@ -356,16 +356,26 @@ def decode_attention_work_numel(batch: int, n_head: int, head_dim: int, t_max: i
     return int(_lib().adapcc_decode_attn_work(batch, n_head, head_dim, t_max))
 
 
-def _check_decode_attn(who: str, kq: int, qkv, k_cache, v_cache, lens, out, work, nq=None, side_k=None, side_v=None):
+def _check_decode_attn(who: str, kq: int, qkv, k_cache, v_cache, lens, out, work, nq=None, side_k=None, side_v=None,
+                       k_scale=None, v_scale=None):
     """``ValueError`` (prefixed ``who``) unless the tensors fit a decode-style attention of ``kq`` queries per cache row
-    (``csrc/ops_decode.cu``); returns the cache shape (B, H, t_max, Dh)."""
+    (``csrc/ops_decode.cu``); returns the cache shape (B, H, t_max, Dh). With ``k_scale`` / ``v_scale`` the caches are
+    fp8 (uint8 bytes, ``ops/kvcache.py``)."""
     def bad(msg):
         raise ValueError(f"{who}: {msg}")
 
+    fp8 = k_scale is not None or v_scale is not None
     rows = [(name, t) for name, t in (("out", out), ("side_k", side_k), ("side_v", side_v)) if t is not None]
-    for name, t in [("qkv", qkv), ("k_cache", k_cache), ("v_cache", v_cache)] + rows:
+    caches = [("k_cache", k_cache), ("v_cache", v_cache)]
+    for name, t in [("qkv", qkv)] + ([] if fp8 else caches) + rows:
         if t.dtype != torch.bfloat16:
             bad(f"{name} must be bf16, got {t.dtype}")
+    if fp8:
+        if k_scale is None or v_scale is None:
+            bad("an fp8 cache needs both k_scale and v_scale")
+        for name, t in caches:
+            if t.dtype != torch.uint8:
+                bad(f"{name} must be uint8 (fp8 e4m3 bytes) with scales, got {t.dtype}")
     if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
         bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} "
             f"and {tuple(v_cache.shape)}")
@@ -381,7 +391,10 @@ def _check_decode_attn(who: str, kq: int, qkv, k_cache, v_cache, lens, out, work
             bad(f"{name} must be a contiguous int32 tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
     if work.dtype != torch.float32 or not work.is_contiguous():
         bad(f"work must be a contiguous fp32 tensor, got {work.dtype}")
-    _same_device(who, k_cache.device, (qkv, v_cache, lens, nq, out, side_k, side_v, work))
+    for name, t in (("k_scale", k_scale), ("v_scale", v_scale)):
+        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() or t.shape != (B, H, t_max)):
+            bad(f"{name} must be a contiguous fp32 [{B}, {H}, {t_max}] tensor, got {t.dtype} {tuple(t.shape)}")
+    _same_device(who, k_cache.device, (qkv, v_cache, lens, nq, out, side_k, side_v, work, k_scale, v_scale))
     need = decode_attention_work_numel(R, H, Dh, t_max)
     if work.numel() < need:
         bad(f"work holds {work.numel()} elements, {need} needed")
@@ -389,17 +402,50 @@ def _check_decode_attn(who: str, kq: int, qkv, k_cache, v_cache, lens, out, work
 
 
 def decode_attention_(qkv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, lens: torch.Tensor,
-                      out: torch.Tensor, work: torch.Tensor) -> torch.Tensor:
+                      out: torch.Tensor, work: torch.Tensor, *, k_scale: Optional[torch.Tensor] = None,
+                      v_scale: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Attention of one new token per row over a KV cache, in place. ``qkv`` bf16 [B, 3·H·Dh] (q | k | v of the new
     token; rows may be strided), ``k_cache`` / ``v_cache`` bf16 [B, H, t_max, Dh], ``lens`` int32 [B] (tokens already
     cached per row; read, never written). Stores the new k / v at position ``lens[b]`` and writes
     ``out[b] = softmax(q·K[0..lens[b]]ᵀ / √Dh)·V[0..lens[b]]`` (bf16 [B, H·Dh], fp32 softmax and accumulation). A row
     with ``lens[b]`` outside [0, t_max) is left alone and its output is zero. ``work``: fp32, at least
-    ``decode_attention_work_numel`` elements. Repeatable bit for bit; no host sync, so it can be captured in a graph."""
-    B, H, t_max, Dh = _check_decode_attn("decode_attention_", 1, qkv, k_cache, v_cache, lens, out, work)
+    ``decode_attention_work_numel`` elements. Repeatable bit for bit; no host sync, so it can be captured in a graph.
+
+    With ``k_scale`` / ``v_scale`` (fp32 [B, H, t_max]) the caches are fp8: uint8 e4m3 bytes [B, H, t_max, Dh], read
+    and stored as ``ops/kvcache.py`` defines. The new token attends to its own k / v unquantized and stores them
+    quantized; the output has the bits of the bf16 op on a bf16 cache holding the dequantized values."""
+    B, H, t_max, Dh = _check_decode_attn("decode_attention_", 1, qkv, k_cache, v_cache, lens, out, work,
+                                         k_scale=k_scale, v_scale=v_scale)
     _ck(_lib().adapcc_decode_attn(_ptr(qkv), _ptr(k_cache), _ptr(v_cache), _ptr(lens), _ptr(out), B, H, Dh, t_max,
-                                  qkv.stride(0), _ptr(work), _stream()), "decode_attn")
+                                  qkv.stride(0), _ptr(work), _ptr(k_scale), _ptr(v_scale), _stream()), "decode_attn")
     return out
+
+
+def kv_quantize_(kv: torch.Tensor, k_cache: torch.Tensor, v_cache: torch.Tensor, k_scale: torch.Tensor,
+                 v_scale: torch.Tensor) -> None:
+    """The prefill of one layer's fp8 cache: quantizes positions [0, T) of every row in place, as ``ops/kvcache.py``
+    defines. ``kv`` is the c_attn output, contiguous bf16 [B, T, 3·H·Dh] (q | k | v), read in place; ``k_cache`` /
+    ``v_cache`` uint8 [B, H, t_max, Dh] and ``k_scale`` / ``v_scale`` fp32 [B, H, t_max]. Positions >= T are not
+    touched. The grid depends on the shapes only; no host sync."""
+    def bad(msg):
+        raise ValueError(f"kv_quantize_: {msg}")
+
+    if k_cache.dtype != torch.uint8 or v_cache.dtype != torch.uint8:
+        bad(f"k_cache / v_cache must be uint8 (fp8 e4m3 bytes), got {k_cache.dtype}, {v_cache.dtype}")
+    if k_cache.dim() != 4 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape or not v_cache.is_contiguous():
+        bad(f"k_cache / v_cache must be contiguous [B, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} and "
+            f"{tuple(v_cache.shape)}")
+    B, H, t_max, Dh = k_cache.shape
+    for name, t in (("k_scale", k_scale), ("v_scale", v_scale)):
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.shape != (B, H, t_max):
+            bad(f"{name} must be a contiguous fp32 [{B}, {H}, {t_max}] tensor, got {t.dtype} {tuple(t.shape)}")
+    if kv.dtype != torch.bfloat16 or kv.dim() != 3 or not kv.is_contiguous() or kv.shape[0] != B or \
+            kv.shape[2] != 3 * H * Dh or not 1 <= kv.shape[1] <= t_max:
+        bad(f"kv must be a contiguous bf16 [{B}, T, {3 * H * Dh}] tensor with 1 <= T <= {t_max}, got {kv.dtype} "
+            f"{tuple(kv.shape)}")
+    _same_device("kv_quantize_", k_cache.device, (kv, v_cache, k_scale, v_scale))
+    _ck(_lib().adapcc_kv_quantize(_ptr(kv), _ptr(k_cache), _ptr(v_cache), _ptr(k_scale), _ptr(v_scale), B,
+                                  kv.shape[1], H, Dh, t_max, _stream()), "kv_quantize")
 
 
 # ---- LM head and token sampling for generation (csrc/ops_sample.cu) ------------------------------------------------
@@ -670,25 +716,34 @@ def beam_step_(logits: torch.Tensor, vocab: int, state: BeamState, min_new: int 
         _ptr(state.fin_count), lam, _stream()), "beam_step")
 
 
-def kv_reorder_scratch_numel(k_cache: torch.Tensor, max_new: int) -> int:
-    """bf16 elements of the scratch ``kv_reorder_`` needs for caches shaped like ``k_cache`` [L, R, H, t_max, Dh]."""
+def kv_reorder_scratch_numel(k_cache: torch.Tensor, max_new: int, *, fp8: bool = False) -> int:
+    """bf16 elements of the scratch ``kv_reorder_`` needs for caches shaped like ``k_cache`` [L, R, H, t_max, Dh];
+    with ``fp8``, bytes (uint8) for an fp8 cache and its scales."""
     L, R, H, _, Dh = k_cache.shape
-    return R * int(max_new) * L * 2 * H * Dh
+    return R * int(max_new) * L * 2 * H * (Dh + 4 if fp8 else Dh)
 
 
 def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tensor, prompt_len: torch.Tensor,
-                lens: torch.Tensor, max_new: int, scratch: torch.Tensor) -> None:
+                lens: torch.Tensor, max_new: int, scratch: torch.Tensor, *, k_scale: Optional[torch.Tensor] = None,
+                v_scale: Optional[torch.Tensor] = None) -> None:
     """In place, for every layer l and row r with ``parent[r] != r``: ``k[l, r, :, pos] = k[l, parent[r], :, pos]`` and
     the same for ``v``, over the generated positions ``pos = prompt_len[r] + t``, ``0 <= t < max_new``, ``pos <
     lens[r]``. The caches are bf16 [L, R, H, t_max, Dh]; ``parent``, ``prompt_len`` and ``lens`` int32 [R]. Every
     source is read into ``scratch`` (bf16, ``kv_reorder_scratch_numel`` elements) before anything is written, so cycles
     and many-to-one maps come out right. The grid follows ``max_new``, not the lengths, so one capture serves every
-    step. No host sync."""
+    step. No host sync.
+
+    With ``k_scale`` / ``v_scale`` (fp32 [L, R, H, t_max]) the caches are fp8 (uint8 bytes, ``ops/kvcache.py``; Dh a
+    multiple of 16): the bytes and the scales move, and ``scratch`` is uint8 of ``kv_reorder_scratch_numel(...,
+    fp8=True)`` bytes."""
     def bad(msg):
         raise ValueError(f"kv_reorder_: {msg}")
 
-    if k_cache.dtype != torch.bfloat16 or v_cache.dtype != torch.bfloat16 or scratch.dtype != torch.bfloat16:
-        bad(f"k_cache, v_cache and scratch must be bf16, got {k_cache.dtype}, {v_cache.dtype}, {scratch.dtype}")
+    fp8 = k_scale is not None or v_scale is not None
+    dt = torch.uint8 if fp8 else torch.bfloat16
+    if k_cache.dtype != dt or v_cache.dtype != dt or scratch.dtype != dt:
+        bad(f"k_cache, v_cache and scratch must be {'uint8 with scales' if fp8 else 'bf16'}, got {k_cache.dtype}, "
+            f"{v_cache.dtype}, {scratch.dtype}")
     if (k_cache.dim() != 5 or not k_cache.is_contiguous() or v_cache.shape != k_cache.shape
             or not v_cache.is_contiguous()):
         bad(f"k_cache / v_cache must be contiguous [L, R, H, t_max, Dh] of one shape, got {tuple(k_cache.shape)} and "
@@ -699,12 +754,20 @@ def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tens
     for name, t in (("parent", parent), ("prompt_len", prompt_len), ("lens", lens)):
         if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != R:
             bad(f"{name} must be a contiguous int32 tensor of {R} elements, got {t.dtype} {tuple(t.shape)}")
-    need = kv_reorder_scratch_numel(k_cache, max_new)
+    if fp8:
+        if Dh % 16 != 0:
+            bad(f"an fp8 cache needs Dh a multiple of 16, got {Dh}")
+        for name, t in (("k_scale", k_scale), ("v_scale", v_scale)):
+            if t is None or t.dtype != torch.float32 or not t.is_contiguous() or t.shape != (L, R, H, t_max):
+                bad(f"{name} must be a contiguous fp32 [{L}, {R}, {H}, {t_max}] tensor, got "
+                    f"{None if t is None else (t.dtype, tuple(t.shape))}")
+    need = kv_reorder_scratch_numel(k_cache, max_new, fp8=fp8)
     if not scratch.is_contiguous() or scratch.numel() < need:
         bad(f"scratch must be contiguous with at least {need} elements, got {scratch.numel()}")
-    _same_device("kv_reorder_", k_cache.device, (v_cache, parent, prompt_len, lens, scratch))
+    _same_device("kv_reorder_", k_cache.device, (v_cache, parent, prompt_len, lens, scratch, k_scale, v_scale))
     _ck(_lib().adapcc_kv_reorder(_ptr(k_cache), _ptr(v_cache), L, R, H, t_max, Dh, _ptr(parent), _ptr(prompt_len),
-                                 _ptr(lens), int(max_new), _ptr(scratch), _stream()), "kv_reorder")
+                                 _ptr(lens), int(max_new), _ptr(scratch), _ptr(k_scale), _ptr(v_scale), _stream()),
+        "kv_reorder")
 
 
 # ---- sequence bias, repetition penalty and no-repeat n-gram blocking (csrc/ops_repeats.cu) -------------------------

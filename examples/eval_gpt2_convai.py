@@ -87,6 +87,9 @@ def main():
     p.add_argument("--bad_words", default="",
                    help="f1: comma-separated words the replies may never contain, each banned as encoded with and "
                         "without a leading space; replies go through the batched path")
+    p.add_argument("--kv_cache_dtype", choices=("fp8_e4m3",), default=None,
+                   help="f1: keep the KV cache in fp8 (e4m3 bytes with a power-of-two scale per vector; default: the "
+                        "model's dtype); replies go through the batched path")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -102,7 +105,8 @@ def main():
                   prompt_lookup_num_tokens=a.prompt_lookup_num_tokens, min_p=a.min_p, typical_p=a.typical_p,
                   epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, top_h=a.top_h, beam_sample=a.beam_sample,
                   num_beam_groups=a.num_beam_groups, diversity_penalty=a.diversity_penalty,
-                  guidance_scale=a.guidance_scale, guidance_negative=a.guidance_negative)
+                  guidance_scale=a.guidance_scale, guidance_negative=a.guidance_negative,
+                  kv_cache_dtype=a.kv_cache_dtype)
         if a.bad_words:
             kw["bad_words_ids"] = bad_word_ids(tok, a.bad_words.split(","))
         if a.assistant_checkpoint:

@@ -34,6 +34,7 @@ MODULES = [
     ("adapcc_b200.ops.repeats", ["penalize_repeats_reference", "banned_ngram_ids", "check_repeat_args",
                                  "check_sequence_bias_args", "SequenceBias"]),
     ("adapcc_b200.ops.guidance", ["check_guidance_args", "guided_scores_reference"]),
+    ("adapcc_b200.ops.kvcache", ["quantize", "dequantize", "store_", "check_kv_cache_dtype"]),
     ("adapcc_b200.ops.layers", ["FusedLayerNorm", "FusedLinear", "linear_backward"]),
     ("adapcc_b200.ops.gemm", ["linear_act", "linear_gelu", "supported", "default_variant"]),
     ("adapcc_b200.strategy.trees", ["Tree", "Strategy"]),
