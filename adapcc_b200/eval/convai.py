@@ -96,7 +96,9 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    assistant_verification: str = "coupled", beam_sample: bool = False, num_beam_groups: int = 1,
                    diversity_penalty: float = 0.0, guidance_scale: float = 1.0,
                    guidance_negative: str = "last_token", sequence_bias=None,
-                   bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None) -> List[List[int]]:
+                   bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
+                   frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
+                   context_no_repeat_ngram_size: int = 0) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -121,7 +123,9 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     prompt is), so guidance pushes each reply towards its persona. Guidance with ``num_beams``, ``penalty_alpha``,
     prompt lookup or an assistant is a ``ValueError``. ``sequence_bias`` and ``bad_words_ids`` (HuggingFace's; token
     ids of the dialogue tokenizer) go to ``generate`` / ``beam_search`` / ``contrastive_search`` (``ops/repeats.py``);
-    with prompt lookup or an assistant they are a ``ValueError``. ``kv_cache_dtype`` (``"fp8_e4m3"``: an fp8 KV
+    with prompt lookup or an assistant they are a ``ValueError``. So do ``frequency_penalty`` and
+    ``presence_penalty`` (over each reply's own tokens) and ``context_no_repeat_ngram_size`` (no n-gram of the persona
+    and history copied into the reply). ``kv_cache_dtype`` (``"fp8_e4m3"``: an fp8 KV
     cache, ``ops/kvcache.py``) goes to ``generate`` / ``beam_search``; with ``penalty_alpha``, prompt lookup or an
     assistant it is a ``ValueError``."""
     from ..ops.assisted import check_verification
@@ -160,7 +164,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     seed = torch.tensor(list(seeds) if seeds is not None else range(len(insts)), dtype=torch.int64)
     special = list(tokenizer.special_ids)
     repeats = dict(repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
-                   kv_cache_dtype=kv_cache_dtype)
+                   kv_cache_dtype=kv_cache_dtype, frequency_penalty=frequency_penalty,
+                   presence_penalty=presence_penalty, context_no_repeat_ngram_size=context_no_repeat_ngram_size)
     filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff, top_h=top_h)
     if sequence_bias is not None:
         repeats["sequence_bias"] = sequence_bias
@@ -291,7 +296,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      beam_sample: bool = False, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
                      guidance_scale: float = 1.0, guidance_negative: str = "last_token", sequence_bias=None,
                      bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
-                     **sample_kw) -> Dict[str, float]:
+                     frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
+                     context_no_repeat_ngram_size: int = 0, **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -306,8 +312,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``diversity_penalty``.
 
     ``repetition_penalty != 1`` or ``no_repeat_ngram_size > 0`` with ``f1``: the repetition controls of
-    ``generate`` / ``beam_search`` (``ops/repeats.py``), also on that batched path; so do ``sequence_bias`` and
-    ``bad_words_ids``.
+    ``generate`` / ``beam_search`` (``ops/repeats.py``), also on that batched path; so do ``sequence_bias``,
+    ``bad_words_ids``, ``frequency_penalty``, ``presence_penalty`` and ``context_no_repeat_ngram_size``.
 
     ``penalty_alpha > 0`` with ``f1``: the replies are decoded by contrastive search with ``top_k`` candidates
     (:func:`sample_replies`), on that batched path.
@@ -331,8 +337,11 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     from ..ops.assisted import check_verification
     check_verification("evaluate_dialogs", assistant_verification, assistant_model)
     repeats = (repetition_penalty != 1.0 or no_repeat_ngram_size > 0 or bool(sequence_bias)
-               or bool(bad_words_ids))
+               or bool(bad_words_ids) or frequency_penalty != 0 or presence_penalty != 0
+               or context_no_repeat_ngram_size > 0)
     bias = {k: v for k, v in (("sequence_bias", sequence_bias), ("bad_words_ids", bad_words_ids)) if v is not None}
+    counts = dict(frequency_penalty=frequency_penalty, presence_penalty=presence_penalty,
+                  context_no_repeat_ngram_size=context_no_repeat_ngram_size)
     lookup = prompt_lookup_num_tokens > 0
     filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff, top_h=top_h)
     filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0 or top_h > 0
@@ -347,7 +356,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                                     assistant_verification=assistant_verification, beam_sample=beam_sample,
                                     num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty,
                                     guidance_scale=guidance_scale, guidance_negative=guidance_negative, **bias,
-                                    kv_cache_dtype=kv_cache_dtype, **sample_kw)
+                                    kv_cache_dtype=kv_cache_dtype, **counts, **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -273,25 +273,32 @@ class _Repeats:
     """The repetition controls of a batched decoder over the first R rows of its cache (``rows``; default all of them,
     ``generate`` with guidance passes its B prompt rows): ``seq`` int32 [R, t_max] each row's sequence (its prompt,
     then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the sequence-bias table
-    (``ops.repeats.SequenceBias`` or None), the penalty and the n-gram size. ``create`` returns None when all of them
-    are off, so then nothing is allocated or launched."""
+    (``ops.repeats.SequenceBias`` or None), the repetition penalty, the n-gram size, the frequency and presence
+    penalties and the context n-gram size (the keyword arguments ``GPT2DoubleHeads._decode_setup`` returns).
+    ``create`` returns None when all of them are off, so then nothing is allocated or launched."""
 
     def __init__(self, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
-                 rows: Optional[int] = None, bias=None):
+                 rows: Optional[int] = None, bias=None, frequency: float = 0.0, presence: float = 0.0,
+                 context_ngram: int = 0):
         B, T = input_ids.shape
         self.rows = cache.batch if rows is None else int(rows)
         self.seq = torch.zeros(self.rows, cache.t_max, dtype=torch.int32, device=input_ids.device)
         self.seq[:, :T] = input_ids.repeat_interleave(self.rows // B, dim=0)
         self.prompt_len = cache.lens[:self.rows].clone()
+        self.host_prompt_len = list(cache.host_lens[:self.rows])
         self.vocab, self.penalty, self.ngram, self.bias = vocab, penalty, ngram, bias
+        self.counts = dict(frequency=float(frequency), presence=float(presence), context_ngram=int(context_ngram))
         if bias is not None and input_ids.is_cuda:
             bias.device_tensors(input_ids.device)       # before any capture: the graph keeps these pointers
 
     @classmethod
     def create(cls, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
-               rows: Optional[int] = None, bias=None) -> Optional["_Repeats"]:
-        on = penalty != 1.0 or ngram > 0 or bias is not None
-        return cls(input_ids, cache, vocab, penalty, ngram, rows, bias) if on else None
+               rows: Optional[int] = None, bias=None, frequency: float = 0.0, presence: float = 0.0,
+               context_ngram: int = 0) -> Optional["_Repeats"]:
+        on = (penalty != 1.0 or ngram > 0 or bias is not None or frequency != 0 or presence != 0
+              or context_ngram > 0)
+        return cls(input_ids, cache, vocab, penalty, ngram, rows, bias, frequency, presence,
+                   context_ngram) if on else None
 
     def eager(self, logits: torch.Tensor, cache: KVCache, consumed: Optional[torch.Tensor]) -> torch.Tensor:
         """``penalize_repeats_reference`` over every row's sequence, after storing ``consumed`` [R] (the tokens the last
@@ -301,7 +308,8 @@ class _Repeats:
             dev = self.seq.device
             self.seq[torch.arange(R, device=dev), cache.lens[:R].long() - 1] = consumed.to(dev, torch.int32)
         return penalize_repeats_reference(logits, [self.seq[r, :x] for r, x in enumerate(cache.host_lens[:R])],
-                                          self.vocab, self.penalty, self.ngram, self.bias)
+                                          self.vocab, self.penalty, self.ngram, self.bias,
+                                          prompt_lens=self.host_prompt_len, **self.counts)
 
     def reorder(self, rows: torch.Tensor) -> None:
         """Row r continues row ``rows[r]`` (a beam its parent)."""
@@ -312,7 +320,7 @@ class _Repeats:
         """``ops.penalize_repeats_`` on ``logits`` in place; it also stores ``ids`` and follows ``parent``."""
         from ..ops import penalize_repeats_
         penalize_repeats_(logits, self.vocab, self.seq, self.prompt_len, lens, step, ids, parent, group,
-                          self.penalty, self.ngram, self.bias)
+                          self.penalty, self.ngram, self.bias, **self.counts)
 
 
 def _row_seeds(seed, B: int, dev) -> torch.Tensor:
@@ -666,13 +674,17 @@ class GPT2DoubleHeads(nn.Module):
                       token_type_ids: Optional[torch.Tensor], reply_type, max_new_tokens: int, min_new_tokens: int,
                       repetition_penalty: float, no_repeat_ngram_size: int, num_beams: int = 1,
                       rows_name: str = "beam rows (batch x num_beams)", sequence_bias=None, bad_words_ids=None,
-                      stop_ids: Sequence[int] = (), kv_cache_dtype: Optional[str] = None):
+                      stop_ids: Sequence[int] = (), kv_cache_dtype: Optional[str] = None,
+                      frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
+                      context_no_repeat_ngram_size: int = 0):
         """The checks and prompt quantities the batched decoders share, before anything is launched:
-        ``(B, T, lengths, n, t_max, last, tt_new, native, bias)``. ``last`` [B] is each prompt's last position,
+        ``(B, T, lengths, n, t_max, last, tt_new, native, controls)``. ``last`` [B] is each prompt's last position,
         ``tt_new`` [B] the token type of new tokens (None without token types), ``native`` says whether the bf16 CUDA
         kernels run; they take at most ``LM_HEAD_MAX_ROWS`` rows, ``num_beams`` per prompt (called ``rows_name`` in
-        the error when more than one). ``bias`` is the table of ``sequence_bias`` and ``bad_words_ids``
-        (``ops.repeats.check_sequence_bias_args``; None when both are off). ``kv_cache_dtype`` must be None or one of
+        the error when more than one). ``controls`` are the keyword arguments of ``_Repeats.create`` after the
+        decoder's own: the repetition penalty and n-gram size, ``bias`` the table of ``sequence_bias`` and
+        ``bad_words_ids`` (``ops.repeats.check_sequence_bias_args``; None when both are off), and the frequency,
+        presence and context n-gram settings. ``kv_cache_dtype`` must be None or one of
         ``ops.kvcache.KV_CACHE_DTYPES``. Errors name ``who``."""
         from ..ops import LM_HEAD_MAX_ROWS
 
@@ -687,7 +699,8 @@ class GPT2DoubleHeads(nn.Module):
         if n < 1 or int(min_new_tokens) < 0:
             raise ValueError(f"{who}: need max_new_tokens >= 1 and min_new_tokens >= 0, got {max_new_tokens}, "
                              f"{min_new_tokens}")
-        check_repeat_args(who, repetition_penalty, no_repeat_ngram_size)
+        check_repeat_args(who, repetition_penalty, no_repeat_ngram_size, frequency_penalty, presence_penalty,
+                          context_no_repeat_ngram_size)
         check_kv_cache_dtype(who, kv_cache_dtype)
         bias = check_sequence_bias_args(who, sequence_bias, bad_words_ids, self.cfg.vocab_size, stop_ids)
         t_max = max(lengths) + n
@@ -705,7 +718,10 @@ class GPT2DoubleHeads(nn.Module):
             tt_new = torch.as_tensor(reply_type, dtype=torch.int64).to(dev).expand(B).contiguous()
         elif token_type_ids is not None:
             tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
-        return B, T, lengths, n, t_max, last, tt_new, native, bias
+        controls = dict(penalty=repetition_penalty, ngram=no_repeat_ngram_size, bias=bias,
+                        frequency=float(frequency_penalty), presence=float(presence_penalty),
+                        context_ngram=int(context_no_repeat_ngram_size))
+        return B, T, lengths, n, t_max, last, tt_new, native, controls
 
     @staticmethod
     def _beam_args(who: str, num_beams: int, stop_ids: Sequence[int], suppress_ids: Sequence[int], sample: bool,
@@ -771,7 +787,9 @@ class GPT2DoubleHeads(nn.Module):
                  negative_prompt_ids: Optional[torch.Tensor] = None, negative_lengths: Optional[Sequence[int]] = None,
                  negative_token_type_ids: Optional[torch.Tensor] = None, sequence_bias=None,
                  bad_words_ids=None, top_h: float = 0.0,
-                 kv_cache_dtype: Optional[str] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                 kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
+                 presence_penalty: float = 0.0,
+                 context_no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -786,7 +804,12 @@ class GPT2DoubleHeads(nn.Module):
         of a sequence's last id when the row's prompt and tokens end with the sequence's other ids, and
         ``bad_words_ids`` (a list of id lists; a one-token list in ``stop_ids`` is dropped) does the same with -inf,
         so no listed sequence is ever produced; at most ``ops.repeats.BIAS_MAX_ENTRIES`` entries of at most
-        ``BIAS_MAX_LEN`` ids in all, one table for every row. ``min_p`` (0: off), ``typical_p`` (1: off),
+        ``BIAS_MAX_LEN`` ids in all, one table for every row. ``frequency_penalty`` and ``presence_penalty`` (the
+        OpenAI / vLLM penalties; any finite values, 0: off) act after the repetition penalty: each id that occurs c
+        times among the row's generated tokens (the prompt does not count) loses ``c * frequency_penalty``, then
+        ``presence_penalty``. ``context_no_repeat_ngram_size`` = m (0: off; ParlAI's ``beam_context_block_ngram``)
+        bans, after ``no_repeat_ngram_size``, every id that would complete an m-gram found inside the row's prompt;
+        m = 1 bans every prompt id. ``min_p`` (0: off), ``typical_p`` (1: off),
         ``epsilon_cutoff`` (0: off) and ``eta_cutoff`` (0: off) are HuggingFace's truncation samplers: at temperature
         > 0 they filter, in that order, the ids that top-k and top-p kept, just before the draw (inside
         ``ops.sample_tokens_`` on the native path). ``top_h`` (in (0, 1]; 0: off; 1 is on) is HuggingFace's
@@ -800,15 +823,16 @@ class GPT2DoubleHeads(nn.Module):
         exceeds ``n_positions``: there is no sliding window here, ``sample_sequence`` has one). On CUDA with bf16
         weights the LM head and the sampler are native kernels (``ops.lm_head_logits_``, ``ops.sample_tokens_``) and
         every token after the first replays one CUDA graph of decode step, LM head (``ops.penalize_repeats_`` when a
-        repetition control or sequence bias is on) and sampler, which feeds the drawn ids back into its own input; the host reads the
-        done flags once every 8 tokens, a step late, to stop early. Elsewhere the same loop runs eagerly with fp32
-        PyTorch logits, ``ops.repeats.penalize_repeats_reference`` and ``ops.sampling.sample_reference``.
+        repetition control, penalty or sequence bias is on) and sampler, which feeds the drawn ids back into its own
+        input; the host reads the done flags once every 8 tokens, a step late, to stop early. Elsewhere the same loop
+        runs eagerly with fp32 PyTorch logits, ``ops.repeats.penalize_repeats_reference`` and
+        ``ops.sampling.sample_reference``.
 
         ``prompt_lookup_num_tokens`` = k > 0 (HuggingFace's prompt lookup decoding; greedy only, without the repetition
-        controls) verifies up to k draft tokens per row and step, copied from the row's own prompt and reply after the
-        earliest earlier occurrence of its last ``max_matching_ngram_size`` (or fewer) tokens; the result is the greedy
-        tokens. The definition is in ``ops/lookup.py``. On the native path (``B·(k+1)`` at most 64 rows) every verify
-        step replays one CUDA graph: the drafts (``ops.lookup_draft_``), the model on k + 1 slots per row
+        controls, the penalties or the sequence bias) verifies up to k draft tokens per row and step, copied from the
+        row's own prompt and reply after the earliest earlier occurrence of its last ``max_matching_ngram_size`` (or
+        fewer) tokens; the result is the greedy tokens. The definition is in ``ops/lookup.py``. On the native path
+        (``B·(k+1)`` at most 64 rows) every verify step replays one CUDA graph: the drafts (``ops.lookup_draft_``), the model on k + 1 slots per row
         (``ops.verify_attention_``), the LM head, the slots' arg-maxes (``ops.lookup_argmax_``) and acceptance
         (``ops.lookup_accept_``); the host polls the done flags every ``LOOKUP_POLL_PERIOD`` replays. Afterwards
         ``self.lookup_stats`` holds the rows' emitted tokens (a stop id included) and verify steps, int32 [B], and the
@@ -870,6 +894,11 @@ class GPT2DoubleHeads(nn.Module):
             raise ValueError("generate: sequence_bias and bad_words_ids cannot be combined with "
                              f"prompt_lookup_num_tokens or assistant_model (got {prompt_lookup_num_tokens}, "
                              f"{type(assistant_model).__name__})")
+        if speculative and (frequency_penalty != 0 or presence_penalty != 0 or context_no_repeat_ngram_size != 0):
+            raise ValueError("generate: frequency_penalty, presence_penalty and context_no_repeat_ngram_size cannot be "
+                             f"combined with prompt_lookup_num_tokens or assistant_model (got {frequency_penalty}, "
+                             f"{presence_penalty}, {context_no_repeat_ngram_size}, {prompt_lookup_num_tokens}, "
+                             f"{type(assistant_model).__name__})")
         if guided and (assistant_model is not None or prompt_lookup_num_tokens != 0):
             raise ValueError("generate: guidance_scale != 1 cannot be combined with prompt_lookup_num_tokens or "
                              f"assistant_model (got {prompt_lookup_num_tokens}, {type(assistant_model).__name__})")
@@ -889,11 +918,12 @@ class GPT2DoubleHeads(nn.Module):
                                               reply_type, max_new_tokens, temperature, top_k, top_p, stop_ids,
                                               suppress_ids, min_new_tokens, seed, filters,
                                               assistant_verification == "rejection" and temperature > 0)
-        B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(
+        B, T, lengths, n, t_max, last, tt_new, native, controls = self._decode_setup(
             "generate", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, num_beams=2 if guided else 1,
             rows_name="rows with guidance (batch x 2)", sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
-            stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype)
+            stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype, frequency_penalty=frequency_penalty,
+            presence_penalty=presence_penalty, context_no_repeat_ngram_size=context_no_repeat_ngram_size)
         dev, V = input_ids.device, self.cfg.vocab_size
         seeds = _row_seeds(seed, B, dev)
         if guided:                                  # rows [0, B): the prompts, rows [B, 2B): the negative prompts
@@ -908,7 +938,7 @@ class GPT2DoubleHeads(nn.Module):
         cache = self.new_cache(R, t_max, kv_cache_dtype)
         h = self.hidden(ids_all, tt_all, cache=cache, lengths=lengths_all)[torch.arange(R, device=dev), last]
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
-        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, B, bias)
+        reps = _Repeats.create(input_ids, cache, V, rows=B, **controls)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = self.wte.weight.float()
             done = torch.zeros(B, dtype=torch.int32)
@@ -965,7 +995,9 @@ class GPT2DoubleHeads(nn.Module):
                     num_return_sequences: int = 1, num_beam_groups: int = 1, diversity_penalty: float = 0.0,
                     sequence_bias=None, bad_words_ids=None, min_p: float = 0.0, typical_p: float = 1.0,
                     epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0,
-                    kv_cache_dtype: Optional[str] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
+                    presence_penalty: float = 0.0,
+                    context_no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -978,7 +1010,9 @@ class GPT2DoubleHeads(nn.Module):
         log-softmax, over its prompt and its own hypothesis (``ops/repeats.py``), so its log-probabilities are
         renormalised over the ids that remain. So do ``sequence_bias`` and ``bad_words_ids`` (as in ``generate``),
         applied first: a biased beam's log-probabilities are renormalised too, where HuggingFace adds the bias to the
-        log-probabilities after normalisation.
+        log-probabilities after normalisation. ``frequency_penalty``, ``presence_penalty`` and
+        ``context_no_repeat_ngram_size`` work as in ``generate``, over each beam's own hypothesis, also before the
+        log-softmax.
 
         ``do_sample=True`` is beam sampling (HuggingFace's ``generate(do_sample=True, num_beams=K)``; the definition is
         ``ops.beam.BeamSampleReference``): each beam's ids are filtered by ``top_k`` (0: off) and ``top_p`` at
@@ -1053,7 +1087,9 @@ class GPT2DoubleHeads(nn.Module):
 
         sel = self._beam_decode("beam_search", input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
                                 min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
-                                sequence_bias, bad_words_ids, kv_cache_dtype)
+                                sequence_bias, bad_words_ids, kv_cache_dtype, frequency_penalty=frequency_penalty,
+                                presence_penalty=presence_penalty,
+                                context_no_repeat_ngram_size=context_no_repeat_ngram_size)
         dev, B, n = input_ids.device, input_ids.shape[0], int(max_new_tokens)
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result(R))
@@ -1071,12 +1107,14 @@ class GPT2DoubleHeads(nn.Module):
                                min_new_tokens: int = 0, repetition_penalty: float = 1.0,
                                no_repeat_ngram_size: int = 0, seed=0, sequence_bias=None, bad_words_ids=None,
                                min_p: float = 0.0, typical_p: float = 1.0, epsilon_cutoff: float = 0.0,
-                               eta_cutoff: float = 0.0, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None):
+                               eta_cutoff: float = 0.0, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
+                               frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
+                               context_no_repeat_ngram_size: int = 0):
         """Stochastic beam search (Kool, van Hoof and Welling 2019): ``num_beams`` = K distinct replies per prompt,
         drawn without replacement from the law ``generate`` samples from with the same ``temperature``, ``top_k``,
         ``top_p``, truncation filters (``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff``, ``top_h``), stop /
-        suppress / ``min_new_tokens``, repetition settings, ``sequence_bias`` and ``bad_words_ids``
-        and ``max_new_tokens``; the definition
+        suppress / ``min_new_tokens``, repetition settings, ``sequence_bias`` and ``bad_words_ids``, the frequency,
+        presence and context n-gram settings and ``max_new_tokens``; the definition
         (rules R1-R8, properties P1-P4) is ``ops.beam.StochasticBeamReference``. The first reply of an item is itself
         an exact sample of that law. ``seed``: an int (item b uses ``seed + b``) or an int64 [B] tensor; an item's
         result depends on its prompt, its seed and the scalars only. The other arguments work as in ``beam_search``,
@@ -1116,7 +1154,9 @@ class GPT2DoubleHeads(nn.Module):
 
         sel = self._beam_decode(who, input_ids, lengths, token_type_ids, reply_type, K, max_new_tokens,
                                 min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
-                                sequence_bias, bad_words_ids, kv_cache_dtype)
+                                sequence_bias, bad_words_ids, kv_cache_dtype, frequency_penalty=frequency_penalty,
+                                presence_penalty=presence_penalty,
+                                context_no_repeat_ngram_size=context_no_repeat_ngram_size)
         dev = input_ids.device
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result())
@@ -1130,7 +1170,8 @@ class GPT2DoubleHeads(nn.Module):
     def _beam_decode(self, who: str, input_ids: torch.Tensor, lengths, token_type_ids, reply_type, K: int,
                      max_new_tokens: int, min_new_tokens: int, repetition_penalty: float, no_repeat_ngram_size: int,
                      stop_ids: Sequence[int], suppress_ids: Sequence[int], start, sequence_bias=None,
-                     bad_words_ids=None, kv_cache_dtype: Optional[str] = None):
+                     bad_words_ids=None, kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
+                     presence_penalty: float = 0.0, context_no_repeat_ngram_size: int = 0):
         """The decode loop of the beam decoders. ``start(B, n, V, device, native)`` is called after the argument checks
         and before anything is launched; it returns the selector: on the native path ``(BeamState, keyword arguments
         of beam_step_)``, elsewhere a reference with ``step(logits) -> (next_ids, parent)`` and ``done``. Each prompt
@@ -1140,10 +1181,12 @@ class GPT2DoubleHeads(nn.Module):
         the same loop runs eagerly with fp32 PyTorch logits and torch indexing. Returns the selector."""
         from ..ops import beam_step_, kv_reorder_, kv_reorder_scratch_numel, lm_head_logits_
 
-        B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(
+        B, T, lengths, n, t_max, last, tt_new, native, controls = self._decode_setup(
             who, input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, num_beams=K, sequence_bias=sequence_bias,
-            bad_words_ids=bad_words_ids, stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype)
+            bad_words_ids=bad_words_ids, stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype,
+            frequency_penalty=frequency_penalty, presence_penalty=presence_penalty,
+            context_no_repeat_ngram_size=context_no_repeat_ngram_size)
         dev, V, weight = input_ids.device, self.cfg.vocab_size, self.wte.weight
         sel = start(B, n, V, dev, native)
         if tt_new is not None:
@@ -1157,7 +1200,7 @@ class GPT2DoubleHeads(nn.Module):
             dst[:, :, :, :T].copy_(src.repeat_interleave(K, dim=1))
         del pre
         h = h.repeat_interleave(K, dim=0).contiguous()
-        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, bias=bias)
+        reps = _Repeats.create(input_ids, cache, V, **controls)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = weight.float()
             for i in range(n):
@@ -1352,7 +1395,9 @@ class GPT2DoubleHeads(nn.Module):
                            penalty_alpha: float = 0.6, max_new_tokens: int = 20, stop_ids: Sequence[int] = (),
                            suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
                            no_repeat_ngram_size: int = 0, sequence_bias=None, bad_words_ids=None,
-                           kv_cache_dtype: Optional[str] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+                           kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
+                           presence_penalty: float = 0.0,
+                           context_no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched contrastive search (Su et al., 2022; HuggingFace's ``penalty_alpha`` + ``top_k``); the definition is
         in ``ops/contrastive.py``.
 
@@ -1361,15 +1406,16 @@ class GPT2DoubleHeads(nn.Module):
         between the candidate's final hidden state and the hidden states of the row's sequence so far (its prompt
         without padding, then its emitted tokens). ``penalty_alpha = 0`` or ``top_k = 1`` is greedy decoding.
         ``input_ids``, ``lengths``, ``reply_type``, token types, ``stop_ids``, ``suppress_ids``, ``min_new_tokens``,
-        the repetition controls, ``sequence_bias``, ``bad_words_ids`` (applied to the logits before the candidates
-        are taken) and the return value ``(tokens, n_new)`` work as in ``generate``.
+        the repetition controls, ``sequence_bias``, ``bad_words_ids``, ``frequency_penalty``, ``presence_penalty``,
+        ``context_no_repeat_ngram_size`` (applied to the logits before the candidates are taken) and the return value
+        ``(tokens, n_new)`` work as in ``generate``.
 
         The prompts are prefilled into a KV cache of ``max(lengths) + max_new_tokens`` positions (more than
         ``n_positions`` is a ``ValueError``) and the context is taken from the prefill's hidden states. On CUDA with
         bf16 weights (at most 64 rows) every token replays one CUDA graph: the candidate step (``ops.cand_attention_``
         attends for all k candidates over the shared cache), re-rank and commit (``ops.contrastive_rerank_``), the LM
-        head on the winners, ``ops.penalize_repeats_`` when a repetition control or sequence bias is on, and the
-        next candidates (``ops.contrastive_select_``);
+        head on the winners, ``ops.penalize_repeats_`` when a repetition control, penalty or sequence bias is on, and
+        the next candidates (``ops.contrastive_select_``);
         the host reads the done flags once every 8 tokens, a period late. Elsewhere the same loop runs eagerly:
         candidates decode through ``decode_attention`` on a k-fold copy of the rows and the selection runs in fp64
         (``ops/contrastive.py``). The cache is in the model's dtype: ``kv_cache_dtype`` other than None is a
@@ -1382,10 +1428,11 @@ class GPT2DoubleHeads(nn.Module):
                              f"{kv_cache_dtype!r}")
         check_contrastive_args("contrastive_search", top_k, penalty_alpha, CONTRASTIVE_MAX_K)
         K, alpha = int(top_k), float(penalty_alpha)
-        B, T, lengths, n, t_max, last, tt_new, native, bias = self._decode_setup(
+        B, T, lengths, n, t_max, last, tt_new, native, controls = self._decode_setup(
             "contrastive_search", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
-            stop_ids=stop_ids)
+            stop_ids=stop_ids, frequency_penalty=frequency_penalty, presence_penalty=presence_penalty,
+            context_no_repeat_ngram_size=context_no_repeat_ngram_size)
         cfg, dev, weight = self.cfg, input_ids.device, self.wte.weight
         tt_cand = tt_new.repeat_interleave(K) if tt_new is not None else None
         cache = self.new_cache(B, t_max)
@@ -1393,7 +1440,7 @@ class GPT2DoubleHeads(nn.Module):
         h = hs[torch.arange(B, device=dev), last].contiguous()
         V, L, H = cfg.vocab_size, cfg.n_layer, cfg.n_head
         D = cfg.n_embd
-        reps = _Repeats.create(input_ids, cache, V, repetition_penalty, no_repeat_ngram_size, bias=bias)
+        reps = _Repeats.create(input_ids, cache, V, **controls)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
             head = weight.float()
             cand = CandidateKV(cache, K, torch.zeros(L, 2, B * K, D, dtype=weight.dtype, device=dev))

@@ -70,7 +70,8 @@ def _lib():
                                                     + [c_float] * 5 + [c_void_p])
         lib.adapcc_kv_reorder.argtypes = [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p] * 3 + [c_int] + [c_void_p] * 4
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
-                                                + [c_int, c_float, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p])
+                                                + [c_int, c_float, c_int, c_void_p, c_void_p, c_int, c_int]
+                                                + [c_float, c_float, c_int, c_void_p])
         lib.adapcc_guidance_mix.argtypes = [c_void_p, c_int, c_int, c_int, c_float, c_void_p]
         lib.adapcc_cs_sim_numel.argtypes = [c_int] * 3
         lib.adapcc_cs_sim_numel.restype = c_longlong
@@ -770,34 +771,43 @@ def kv_reorder_(k_cache: torch.Tensor, v_cache: torch.Tensor, parent: torch.Tens
         "kv_reorder")
 
 
-# ---- sequence bias, repetition penalty and no-repeat n-gram blocking (csrc/ops_repeats.cu) -------------------------
+# ---- sequence bias, repetition / frequency / presence penalties, n-gram blocking (csrc/ops_repeats.cu) -------------
 REPEATS_MAX_GROUP = 16         # rows per parent group (beams per item)
 REPEATS_MAX_LEN = 1024         # sequence positions per row (GPT-2's n_positions)
 
 
 def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, prompt_len: torch.Tensor,
                       lens: torch.Tensor, step: torch.Tensor, ids: torch.Tensor, parent: Optional[torch.Tensor],
-                      group: int, penalty: float, ngram: int, bias=None) -> None:
-    """The sequence bias, repetition penalty and no-repeat n-gram blocking of every row, in place, on the device (the
-    definition in ``ops/repeats.py``, which this kernel equals bit for bit). ``logits`` fp32 [R, ld] (the first ``vocab`` columns
-    used); ``seq`` int32 [R, t_max] the rows' sequences, kept up to date here; ``prompt_len`` and ``lens`` int32 [R];
-    ``step`` int32 [1] (the counter of ``generate`` / ``BeamState``); ``ids`` int64 [R] the tokens the decode step just
-    consumed; ``parent`` int32 [R] or None, each row's parent inside its group of ``group`` consecutive rows.
+                      group: int, penalty: float, ngram: int, bias=None, frequency: float = 0.0,
+                      presence: float = 0.0, context_ngram: int = 0) -> None:
+    """The sequence bias, repetition penalty, frequency / presence penalties, no-repeat n-gram blocking and context
+    n-gram blocking of every row, in place, on the device (the definition in ``ops/repeats.py``, which this kernel
+    equals bit for bit). ``logits`` fp32 [R, ld] (the first ``vocab`` columns used); ``seq`` int32 [R, t_max] the rows'
+    sequences, kept up to date here; ``prompt_len`` and ``lens`` int32 [R]; ``step`` int32 [1] (the counter of
+    ``generate`` / ``BeamState``); ``ids`` int64 [R] the tokens the decode step just consumed; ``parent`` int32 [R] or
+    None, each row's parent inside its group of ``group`` consecutive rows.
 
     With ``*step > 0`` the sequences first advance: a row with a parent takes the parent's generated region
     ``seq[parent[r], prompt_len[r]:lens[r] - 1]`` (cycles and many-to-one maps come out right), then
     ``seq[r, lens[r] - 1] = ids[r]``. With ``*step == 0`` the sequence is the prompt as stored. Row r's sequence is then
     ``seq[r, :lens[r]]``; ``bias`` (an ``ops.repeats.SequenceBias`` from ``check_sequence_bias_args``, None: off),
-    ``penalty`` (1: off) and ``ngram`` (0: off) are applied to it. The table goes to the device once per table and
-    device and keeps its pointers, so a graph may capture it. The grid depends on R and ``group`` only and there is no
-    host sync, so one capture serves every token."""
-    from .repeats import SequenceBias
+    ``penalty`` (1: off), ``frequency`` and ``presence`` (finite, rounded to fp32; 0: off), ``ngram`` (0: off) and
+    ``context_ngram`` (0: off) are applied to it. ``frequency`` and ``presence`` count the generated region
+    ``seq[r, prompt_len[r]:lens[r]]``; ``context_ngram`` bans only n-grams inside ``seq[r, :prompt_len[r]]``. The
+    table goes to the device once per table and device and keeps its pointers, so a graph may capture it. The grid
+    depends on R and ``group`` only and there is no host sync, so one capture serves every token."""
+    from .repeats import SequenceBias, finite_fp32
 
     def bad(msg):
         raise ValueError(f"penalize_repeats_: {msg}")
 
     if not (math.isfinite(penalty) and penalty > 0) or int(ngram) < 0:
         bad(f"need a finite penalty > 0 and ngram >= 0, got {penalty}, {ngram}")
+    for name, x in (("frequency", frequency), ("presence", presence)):
+        if not finite_fp32(x):
+            bad(f"{name} must be a number that is finite in fp32, got {x}")
+    if isinstance(context_ngram, bool) or int(context_ngram) != context_ngram or int(context_ngram) < 0:
+        bad(f"context_ngram must be an integer >= 0, got {context_ngram}")
     if bias is not None and not isinstance(bias, SequenceBias):
         bad(f"bias must be an ops.repeats.SequenceBias or None, got {type(bias).__name__}")
     if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
@@ -824,7 +834,8 @@ def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, promp
                                        _ptr(prompt_len), _ptr(lens), _ptr(step), _ptr(ids), _ptr(parent), int(group),
                                        float(penalty), int(ngram), _ptr(tab), _ptr(val),
                                        bias.num_targets if bias is not None else 0,
-                                       bias.num_entries if bias is not None else 0, _stream()), "penalize_repeats")
+                                       bias.num_entries if bias is not None else 0, float(frequency), float(presence),
+                                       int(context_ngram), _stream()), "penalize_repeats")
 
 
 # ---- classifier-free guidance (csrc/ops_guidance.cu) ---------------------------------------------------------------

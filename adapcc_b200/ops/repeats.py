@@ -2,9 +2,11 @@
 (csrc/ops_repeats.cu) evaluated in fp32 with numpy: the CPU / non-bf16 path of ``GPT2DoubleHeads.generate`` and
 ``beam_search`` and the reference the GPU tests compare the kernel against, bit for bit.
 
-Row r's *sequence* is its prompt (the first ``lengths[b]`` ids, without padding) followed by the tokens generated so
-far; for a beam, the tokens of its own hypothesis. The definition applies to the row's fp32 logits ``l_i``,
-``i < vocab``, before step 1 of ``ops/sampling.py`` or ``ops/beam.py`` (DESIGN.md §4a), in this order:
+Row r's *sequence* ``s = seq[:L]`` is its prompt (the first ``lengths[b]`` ids, without padding) followed by the
+tokens generated so far; for a beam, the tokens of its own hypothesis. ``P`` is the prompt length (with guidance, of
+the prompt rows) and ``s[P:L]`` the *generated region*, empty for the first token. The definition applies to the
+row's fp32 logits ``l_i``, ``i < vocab``, before step 1 of ``ops/sampling.py`` or ``ops/beam.py`` (DESIGN.md §4a), in
+this order:
 
 0. sequence bias (a ``SequenceBias`` table shared by all rows; None: off). Each entry is a token sequence ``s`` of
    length ``m >= 1`` and an fp32 bias ``b``: HuggingFace's ``sequence_bias`` with its finite biases, then its
@@ -16,21 +18,32 @@ far; for a beam, the tokens of its own hypothesis. The definition applies to the
    addition correctly rounded, in this order: t's length-1 ``sequence_bias`` entry, then its longer
    ``sequence_bias`` entries in the order given, then its bad words; then ``l_t <- fl32(l_t + sum)``. Other ids are
    unchanged. This is HuggingFace's ``SequenceBiasLogitsProcessor`` before, and ``NoBadWordsLogitsProcessor`` after,
-   rules 1 and 2: -inf is unchanged by both rules and logits are never +inf, so applying the bad words here gives the
+   rules 1 to 3: -inf is unchanged by them and logits are never +inf, so applying the bad words here gives the
    same values. HuggingFace adds +0.0 to every id, so its -0.0 logits become +0.0; here ids without an applicable
    entry keep their bits;
 1. repetition penalty ``p > 0`` (1 = off): for every *distinct* id ``i < vocab`` in the sequence,
    ``l_i <- fl32(l_i * p)`` if ``l_i < 0`` and ``fl32(l_i / p)`` otherwise, with ``p`` rounded to fp32 once and each
    operation correctly rounded. Each id is penalised once however often it occurs; ids outside ``[0, vocab)`` are
    ignored. This is HuggingFace's ``RepetitionPenaltyLogitsProcessor``;
-2. no-repeat n-grams ``n >= 1`` (0 = off): with ``L`` the sequence length, for every ``j`` with ``j + n - 1 < L`` and
+2. frequency / presence: ``f = fl32(frequency_penalty)`` and ``q = fl32(presence_penalty)``, any finite values of
+   either sign (0 = off). For every distinct id ``i < vocab`` that occurs ``c >= 1`` times in the generated region,
+   first ``l_i <- fl32(l_i - fl32(c * f))`` if ``f != 0``, then ``l_i <- fl32(l_i - q)`` if ``q != 0``. Prompt ids
+   do not count; ids outside ``[0, vocab)`` are ignored; with both 0 nothing is touched, so a -0.0 logit keeps its
+   bits. This is vLLM's ``logits -= f * output_counts; logits -= q * (output_counts > 0)`` over the output tokens,
+   after its repetition penalty;
+3. no-repeat n-grams ``n >= 1`` (0 = off): with ``L`` the sequence length, for every ``j`` with ``j + n - 1 < L`` and
    ``seq[j:j + n - 1] == seq[L - n + 1:L]``, ``l_{seq[j + n - 1]} <- -inf``. For ``n = 1`` every id of the sequence is
    banned; for ``L < n`` nothing is. This is HuggingFace's ``NoRepeatNGramLogitsProcessor`` on a decoder-only model:
-   the prompt counts, and so do n-grams that cross from the prompt into the reply.
+   the prompt counts, and so do n-grams that cross from the prompt into the reply;
+4. context n-grams ``m >= 1`` (``context_no_repeat_ngram_size``; 0 = off): with ``L >= m``, for every ``j`` with
+   ``j + m - 1 < min(P, L)`` and ``s[j:j + m - 1] == s[L - m + 1:L]``, ``l_{s[j + m - 1]} <- -inf``: rule 3's bans
+   at n = m, restricted to earlier m-grams that lie wholly inside the prompt (ParlAI's ``beam_context_block_ngram``).
+   The tail may reach into the prompt, as for rule 3. For ``m = 1`` every prompt id is banned.
 
-Ids at -inf are never candidates of the sampler or the beam selection. In beam search all three rules act on the
+Ids at -inf are never candidates of the sampler or the beam selection. In beam search all the rules act on the
 logits before the log-softmax, so a beam's log-probabilities are renormalised over the ids that remain and the biased
-values (as ``suppress_ids`` are); HuggingFace and fairseq process the log-probabilities after normalisation instead.
+and penalised values (as ``suppress_ids`` are); HuggingFace and fairseq process the log-probabilities after
+normalisation instead.
 """
 from __future__ import annotations
 
@@ -42,12 +55,29 @@ import numpy as np
 import torch
 
 
-def check_repeat_args(who: str, penalty: float, ngram: int) -> None:
-    """``ValueError`` unless ``penalty`` is finite and > 0 and ``ngram >= 0``."""
+def finite_fp32(x) -> bool:
+    """Whether ``x`` is a real number (not a bool) whose fp32 rounding is finite."""
+    if isinstance(x, bool) or not isinstance(x, Real):
+        return False
+    with np.errstate(over="ignore"):
+        return bool(np.isfinite(np.float32(x)))
+
+
+def check_repeat_args(who: str, penalty: float, ngram: int, frequency: float = 0.0, presence: float = 0.0,
+                      context_ngram: int = 0) -> None:
+    """``ValueError`` naming the argument unless ``penalty`` is finite and > 0, ``ngram >= 0``, ``frequency`` and
+    ``presence`` (``frequency_penalty``, ``presence_penalty``) are finite in fp32 and ``context_ngram``
+    (``context_no_repeat_ngram_size``) is an integer >= 0."""
     if not (isinstance(penalty, (int, float)) and math.isfinite(penalty) and penalty > 0):
         raise ValueError(f"{who}: repetition_penalty must be a finite number > 0, got {penalty}")
     if int(ngram) != ngram or int(ngram) < 0:
         raise ValueError(f"{who}: no_repeat_ngram_size must be an integer >= 0, got {ngram}")
+    for name, x in (("frequency_penalty", frequency), ("presence_penalty", presence)):
+        if not finite_fp32(x):
+            raise ValueError(f"{who}: {name} must be a number that is finite in fp32, got {x!r}")
+    if (isinstance(context_ngram, bool) or not isinstance(context_ngram, Real) or int(context_ngram) != context_ngram
+            or int(context_ngram) < 0):
+        raise ValueError(f"{who}: context_no_repeat_ngram_size must be an integer >= 0, got {context_ngram!r}")
 
 
 BIAS_MAX_ENTRIES = 1024      # sequence-bias entries per call, biases and bad words together
@@ -173,27 +203,35 @@ def check_sequence_bias_args(who: str, sequence_bias, bad_words_ids, vocab: int,
     return SequenceBias(list(per.items()))
 
 
-def banned_ngram_ids(seq: np.ndarray, n: int) -> np.ndarray:
-    """Rule 2: the ids ``seq[j + n - 1]`` of every earlier n-gram whose first n - 1 ids equal the sequence's last
-    n - 1 (all of them for n = 1, none for ``len(seq) < n``), out-of-range ids included."""
+def banned_ngram_ids(seq: np.ndarray, n: int, end: Optional[int] = None) -> np.ndarray:
+    """Rule 3: the ids ``seq[j + n - 1]`` of every earlier n-gram whose first n - 1 ids equal the sequence's last
+    n - 1 (all of them for n = 1, none for ``len(seq) < n``), out-of-range ids included. With ``end`` only the
+    n-grams inside ``seq[:end]`` count (``j + n - 1 < min(end, len(seq))``): rule 4 with ``end`` the prompt length."""
     L = seq.size
     if n < 1 or L < n:
         return seq[:0]
     win = np.lib.stride_tricks.sliding_window_view(seq, n)           # [L - n + 1, n]: every n-gram
     match = (win[:, :n - 1] == seq[L - n + 1:]).all(axis=1)
+    if end is not None:
+        match[max(min(end, L) - n + 1, 0):] = False
     return win[match, n - 1]
 
 
 def penalize_repeats_reference(logits, seqs: Sequence, vocab: int, penalty: float, ngram: int,
-                               bias: Optional[SequenceBias] = None) -> torch.Tensor:
-    """Rules 0 (with ``bias``), 1 and 2 for R rows: ``logits`` [R, >= vocab] (fp32 values), ``seqs`` R sequences (int
-    lists, arrays or tensors). Returns a new fp32 tensor of the logits' shape on their device; columns from ``vocab``
+                               bias: Optional[SequenceBias] = None, frequency: float = 0.0, presence: float = 0.0,
+                               context_ngram: int = 0, prompt_lens: Optional[Sequence[int]] = None) -> torch.Tensor:
+    """Rules 0 (with ``bias``) to 4 for R rows: ``logits`` [R, >= vocab] (fp32 values), ``seqs`` R sequences (int
+    lists, arrays or tensors), ``prompt_lens`` R prompt lengths P (needed when ``frequency``, ``presence`` or
+    ``context_ngram`` is on). Returns a new fp32 tensor of the logits' shape on their device; columns from ``vocab``
     on are copied."""
     t = logits if isinstance(logits, torch.Tensor) else torch.as_tensor(logits)
     x = t.detach().to(device="cpu", dtype=torch.float32).numpy().copy()
     if len(seqs) != x.shape[0]:
         raise ValueError(f"penalize_repeats_reference: {x.shape[0]} rows but {len(seqs)} sequences")
-    p = np.float32(penalty)
+    p, f, q = np.float32(penalty), np.float32(frequency), np.float32(presence)
+    if (f != 0 or q != 0 or context_ngram > 0) and (prompt_lens is None or len(prompt_lens) != x.shape[0]):
+        raise ValueError(f"penalize_repeats_reference: frequency, presence and context_ngram need {x.shape[0]} "
+                         f"prompt_lens, got {prompt_lens}")
     for r, s in enumerate(seqs):
         s = np.asarray(s.cpu() if isinstance(s, torch.Tensor) else s, dtype=np.int64).reshape(-1)
         row = x[r]
@@ -203,7 +241,20 @@ def penalize_repeats_reference(logits, seqs: Sequence, vocab: int, penalty: floa
             ids = np.unique(s[(s >= 0) & (s < vocab)])
             v = row[ids]
             row[ids] = np.where(v < 0, v * p, v / p)
+        P = min(max(int(prompt_lens[r]), 0), s.size) if prompt_lens is not None else 0
+        if f != 0 or q != 0:
+            gen = s[P:]
+            ids, c = np.unique(gen[(gen >= 0) & (gen < vocab)], return_counts=True)
+            v = row[ids]
+            if f != 0:
+                v = v - c.astype(np.float32) * f
+            if q != 0:
+                v = v - q
+            row[ids] = v
         if ngram > 0:
             ban = banned_ngram_ids(s, int(ngram))
+            row[ban[(ban >= 0) & (ban < vocab)]] = -np.inf
+        if context_ngram > 0:
+            ban = banned_ngram_ids(s, int(context_ngram), P)
             row[ban[(ban >= 0) & (ban < vocab)]] = -np.inf
     return torch.from_numpy(x).to(t.device if isinstance(logits, torch.Tensor) else "cpu")

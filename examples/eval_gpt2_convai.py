@@ -51,6 +51,15 @@ def main():
                    help="f1: penalty on ids already in the prompt or reply (1: off); replies go through the batched path")
     p.add_argument("--no_repeat_ngram_size", type=int, default=0,
                    help="f1: never repeat an n-gram of the prompt or reply (0: off); replies go through the batched path")
+    p.add_argument("--frequency_penalty", type=float, default=0.0,
+                   help="f1: subtract this times the count of each id already in the reply (the prompt does not "
+                        "count; 0: off); replies go through the batched path")
+    p.add_argument("--presence_penalty", type=float, default=0.0,
+                   help="f1: subtract this once from each id already in the reply (the prompt does not count; 0: off); "
+                        "replies go through the batched path")
+    p.add_argument("--context_no_repeat_ngram_size", type=int, default=0,
+                   help="f1: never complete an n-gram of the persona and history (0: off); replies go through the "
+                        "batched path")
     p.add_argument("--penalty_alpha", type=float, default=0.0,
                    help="f1: > 0 decodes the replies with GPT2DoubleHeads.contrastive_search, this degeneration penalty "
                         "and --top_k candidates (0: sample); replies go through the batched path")
@@ -106,7 +115,8 @@ def main():
                   epsilon_cutoff=a.epsilon_cutoff, eta_cutoff=a.eta_cutoff, top_h=a.top_h, beam_sample=a.beam_sample,
                   num_beam_groups=a.num_beam_groups, diversity_penalty=a.diversity_penalty,
                   guidance_scale=a.guidance_scale, guidance_negative=a.guidance_negative,
-                  kv_cache_dtype=a.kv_cache_dtype)
+                  kv_cache_dtype=a.kv_cache_dtype, frequency_penalty=a.frequency_penalty,
+                  presence_penalty=a.presence_penalty, context_no_repeat_ngram_size=a.context_no_repeat_ngram_size)
         if a.bad_words:
             kw["bad_words_ids"] = bad_word_ids(tok, a.bad_words.split(","))
         if a.assistant_checkpoint:

@@ -32,7 +32,7 @@ MODULES = [
     ("adapcc_b200.ops.assisted", ["check_assist_args", "draw_slot", "assist_round", "draw_slots", "check_verification",
                                   "filtered_probs", "spec_slot", "spec_slots"]),
     ("adapcc_b200.ops.repeats", ["penalize_repeats_reference", "banned_ngram_ids", "check_repeat_args",
-                                 "check_sequence_bias_args", "SequenceBias"]),
+                                 "finite_fp32", "check_sequence_bias_args", "SequenceBias"]),
     ("adapcc_b200.ops.guidance", ["check_guidance_args", "guided_scores_reference"]),
     ("adapcc_b200.ops.kvcache", ["quantize", "dequantize", "store_", "check_kv_cache_dtype"]),
     ("adapcc_b200.ops.layers", ["FusedLayerNorm", "FusedLinear", "linear_backward"]),

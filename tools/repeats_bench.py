@@ -1,6 +1,7 @@
 #!/usr/bin/env python
 """GPT-2 small repetition controls: the ``penalize_repeats_`` kernel on its own, and ``generate`` / ``beam_search`` per
-token with and without ``repetition_penalty`` and ``no_repeat_ngram_size``.
+token with and without ``repetition_penalty`` and ``no_repeat_ngram_size``, and with and without the frequency /
+presence penalties and context n-gram blocking.
 
 Prints one JSON line with the device name and power limit read in the same run. Needs a CUDA device (there is no CPU
 fallback) and writes nothing into the repository.
@@ -14,8 +15,14 @@ fallback) and writes nothing into the repository.
   prompt 512, 64 new tokens, no stop ids, so every call runs all 64 tokens), for ``generate`` (top_p 0.9) and
   ``beam_search`` (4 beams) at 8 and 64 rows, with both controls off and on (p = 1.2, n = 3), the two alternated in one
   process. Medians of ``--reps`` runs after one warm-up run of each.
+* ``penalties_kernel``: ``penalize_repeats_`` at R = 1 / 8 / 64 rows, a 512-id prompt and generated regions of 64 and
+  511 ids (sequences over 2000 ids, step > 0), timed as ``kernel`` is, for: the configuration of ``kernel`` (p = 1.2,
+  n = 3), each new rule alone (frequency 0.5, presence 0.5, context n-grams m = 3) and all five rules on. Rule 2 counts
+  each generated id's occurrences by a scan of the generated region, so its cost grows with the region's square.
+* ``penalties_decode``: as ``decode``, with ``frequency_penalty = presence_penalty = 0.5`` and
+  ``context_no_repeat_ngram_size = 3`` on against everything off.
 
-Usage: ``python tools/repeats_bench.py [--reps 5] [--launches 1000]``
+Usage: ``python tools/repeats_bench.py [--reps 5] [--launches 1000] [--sections kernel,decode,penalties_kernel,...]``
 """
 import argparse
 import json
@@ -34,6 +41,8 @@ NEW_TOKENS = 64
 PROMPT = 512
 GRAPH_LAUNCHES = 50
 P, N = 1.2, 3
+F, Q, M = 0.5, 0.5, 3
+SECTIONS = ("kernel", "decode", "penalties_kernel", "penalties_decode")
 
 
 def _gpu_info():
@@ -106,7 +115,35 @@ def _ms(fn):
     return (time.perf_counter() - t0) * 1e3
 
 
-def bench_decode(model, reps):
+def bench_penalties_kernel(model, launches):
+    from adapcc_b200.ops import penalize_repeats_
+
+    V, W = model.cfg.vocab_size, model.wte.weight
+    g = torch.Generator(device="cuda").manual_seed(2)
+    i32 = dict(dtype=torch.int32, device="cuda")
+    configs = (("today", P, N, {}), ("frequency", 1.0, 0, dict(frequency=F)), ("presence", 1.0, 0, dict(presence=Q)),
+               ("context", 1.0, 0, dict(context_ngram=M)),
+               ("all", P, N, dict(frequency=F, presence=Q, context_ngram=M)))
+    rows = []
+    for R in (1, 8, 64):
+        logits = torch.randn(R, W.shape[0], device="cuda", generator=g) * 3
+        ids = torch.randint(0, V, (R,), device="cuda", generator=g)
+        step = torch.ones(1, **i32)
+        seq = torch.randint(0, 2000, (R, 1024), device="cuda", generator=g).to(torch.int32)
+        prompt_len = torch.full((R,), PROMPT, **i32)
+        for gen in (64, 511):
+            lens = torch.full((R,), PROMPT + gen, **i32)
+            entry = {"rows": R, "prompt": PROMPT, "generated": gen}
+            for name, p, n, kw in configs:
+                us = _graph_us(lambda: penalize_repeats_(logits, V, seq, prompt_len, lens, step, ids, None, 1, p, n,
+                                                         **kw), launches)
+                entry[f"{name}_us"] = round(us, 2)
+            rows.append(entry)
+    return {"today": {"p": P, "n": N}, "frequency": F, "presence": Q, "context_ngram": M, "per_config": rows}
+
+
+def bench_decode(model, reps, on_kw=None):
+    on_kw = dict(repetition_penalty=P, no_repeat_ngram_size=N) if on_kw is None else on_kw
     V = model.cfg.vocab_size
     g = torch.Generator(device="cuda").manual_seed(0)
     out = []
@@ -115,7 +152,7 @@ def bench_decode(model, reps):
         prompt = torch.randint(0, V, (B, PROMPT), device="cuda", generator=g)
 
         def run(on):
-            kw = dict(repetition_penalty=P, no_repeat_ngram_size=N) if on else {}
+            kw = on_kw if on else {}
             if mode == "generate":
                 return lambda: model.generate(prompt, max_new_tokens=NEW_TOKENS, seed=3, **kw)
             return lambda: model.beam_search(prompt, num_beams=4, max_new_tokens=NEW_TOKENS, **kw)
@@ -142,7 +179,11 @@ def main():
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--launches", type=int, default=1000)
+    ap.add_argument("--sections", default=",".join(SECTIONS), help="comma-separated subset of " + ", ".join(SECTIONS))
     args = ap.parse_args()
+    sections = [x for x in args.sections.split(",") if x]
+    if any(x not in SECTIONS for x in sections):
+        sys.exit(f"repeats_bench: --sections must be a subset of {', '.join(SECTIONS)}, got {args.sections}")
     if not torch.cuda.is_available():
         sys.exit("repeats_bench: needs a CUDA device")
     from adapcc_b200.models.gpt2 import GPT2Config, GPT2DoubleHeads
@@ -153,8 +194,16 @@ def main():
     info = _gpu_info()
     torch.manual_seed(0)
     model = GPT2DoubleHeads(GPT2Config()).to(device="cuda", dtype=torch.bfloat16).eval()
-    result = dict(info, new_tokens=NEW_TOKENS, prompt=PROMPT, kernel=bench_kernel(model, args.launches),
-                  decode=bench_decode(model, args.reps))
+    result = dict(info, new_tokens=NEW_TOKENS, prompt=PROMPT)
+    if "kernel" in sections:
+        result["kernel"] = bench_kernel(model, args.launches)
+    if "decode" in sections:
+        result["decode"] = bench_decode(model, args.reps)
+    if "penalties_kernel" in sections:
+        result["penalties_kernel"] = bench_penalties_kernel(model, args.launches)
+    if "penalties_decode" in sections:
+        result["penalties_decode"] = bench_decode(model, args.reps, dict(
+            frequency_penalty=F, presence_penalty=Q, context_no_repeat_ngram_size=M))
     print(json.dumps(result))
 
 
