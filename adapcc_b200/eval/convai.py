@@ -98,7 +98,7 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    guidance_negative: str = "last_token", sequence_bias=None,
                    bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
                    frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
-                   context_no_repeat_ngram_size: int = 0) -> List[List[int]]:
+                   context_no_repeat_ngram_size: int = 0, watermarking_config=None) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -125,7 +125,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     ids of the dialogue tokenizer) go to ``generate`` / ``beam_search`` / ``contrastive_search`` (``ops/repeats.py``);
     with prompt lookup or an assistant they are a ``ValueError``. So do ``frequency_penalty`` and
     ``presence_penalty`` (over each reply's own tokens) and ``context_no_repeat_ngram_size`` (no n-gram of the persona
-    and history copied into the reply). ``kv_cache_dtype`` (``"fp8_e4m3"``: an fp8 KV
+    and history copied into the reply), and ``watermarking_config`` (the green-list watermark,
+    ``ops/watermark.py``). ``kv_cache_dtype`` (``"fp8_e4m3"``: an fp8 KV
     cache, ``ops/kvcache.py``) goes to ``generate`` / ``beam_search``; with ``penalty_alpha``, prompt lookup or an
     assistant it is a ``ValueError``."""
     from ..ops.assisted import check_verification
@@ -171,6 +172,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
         repeats["sequence_bias"] = sequence_bias
     if bad_words_ids is not None:
         repeats["bad_words_ids"] = bad_words_ids
+    if watermarking_config is not None:
+        repeats["watermarking_config"] = watermarking_config
     if num_beams > 0:
         sampled = dict(do_sample=True, temperature=temperature, top_k=top_k, top_p=top_p, seed=seed,
                        **filters) if beam_sample else {}
@@ -297,7 +300,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      guidance_scale: float = 1.0, guidance_negative: str = "last_token", sequence_bias=None,
                      bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
                      frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
-                     context_no_repeat_ngram_size: int = 0, **sample_kw) -> Dict[str, float]:
+                     context_no_repeat_ngram_size: int = 0, watermarking_config=None,
+                     **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
 
@@ -333,13 +337,20 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``"no_persona"``, see :func:`sample_replies`), on that batched path.
 
     ``kv_cache_dtype="fp8_e4m3"`` with ``f1``: the replies are decoded with an fp8 KV cache (``ops/kvcache.py``), on
-    that batched path; comparing F1 with and without it measures what the quantization costs."""
+    that batched path; comparing F1 with and without it measures what the quantization costs.
+
+    ``watermarking_config`` with ``f1``: the replies carry the green-list watermark (``ops/watermark.py``), on that
+    batched path, and the result also holds ``watermark_z``, the mean z-score of the replies scored on their own
+    (``detect_watermark`` without the prompt; replies with nothing to score are left out), and
+    ``watermark_detected``, the fraction of replies it flags, next to F1: what the mark costs in F1 against how
+    reliably it is found."""
     from ..ops.assisted import check_verification
     check_verification("evaluate_dialogs", assistant_verification, assistant_model)
     repeats = (repetition_penalty != 1.0 or no_repeat_ngram_size > 0 or bool(sequence_bias)
                or bool(bad_words_ids) or frequency_penalty != 0 or presence_penalty != 0
-               or context_no_repeat_ngram_size > 0)
-    bias = {k: v for k, v in (("sequence_bias", sequence_bias), ("bad_words_ids", bad_words_ids)) if v is not None}
+               or context_no_repeat_ngram_size > 0 or watermarking_config is not None)
+    bias = {k: v for k, v in (("sequence_bias", sequence_bias), ("bad_words_ids", bad_words_ids),
+                              ("watermarking_config", watermarking_config)) if v is not None}
     counts = dict(frequency_penalty=frequency_penalty, presence_penalty=presence_penalty,
                   context_no_repeat_ngram_size=context_no_repeat_ngram_size)
     lookup = prompt_lookup_num_tokens > 0
@@ -410,10 +421,24 @@ def _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples,
             hist = [tokenizer.encode(h) for h in u["history"][-(2 * max_history + 1):]]
             examples.append((persona, hist, u["candidates"][-1]))
     acc = 0.0
+    wm = sample_kw.get("watermarking_config")
+    z, flagged = [], 0
     for s in range(0, len(examples), batch_size):
         chunk = examples[s:s + batch_size]
         seeds = [((seed & 0x7FFFFFFF) << 32) + s + j for j in range(len(chunk))]
         replies = sample_replies(model, tokenizer, [(p, h) for p, h, _ in chunk], device=device, seeds=seeds,
                                  **sample_kw)
         acc += sum(f1_score(tokenizer.decode(r), [gold]) for r, (_, _, gold) in zip(replies, chunk))
-    return {"f1": acc / max(1, len(examples)), "examples": len(examples)}
+        if wm is not None:
+            from ..ops.watermark import detect_watermark
+
+            width = max(1, max(len(r) for r in replies))
+            ids = torch.tensor([r + [0] * (width - len(r)) for r in replies], dtype=torch.int64)
+            det = detect_watermark(ids.to(device), wm, lengths=[len(r) for r in replies])
+            z += [float(x) for x in det.z_score if math.isfinite(x)]
+            flagged += int(det.prediction.sum())
+    out = {"f1": acc / max(1, len(examples)), "examples": len(examples)}
+    if wm is not None:
+        out.update(watermark_z=sum(z) / len(z) if z else float("nan"),
+                   watermark_detected=flagged / max(1, len(examples)))
+    return out

@@ -34,6 +34,7 @@ from ..ops.guidance import check_guidance_args, guided_scores_reference
 from ..ops.kvcache import check_kv_cache_dtype
 from ..ops.layers import FusedLayerNorm, FusedLinear
 from ..ops.repeats import check_repeat_args, check_sequence_bias_args, penalize_repeats_reference
+from ..ops.watermark import check_watermark_args, watermark_reference
 from ..ops.sampling import check_filter_args, sample_reference, top_filtering
 
 
@@ -274,12 +275,14 @@ class _Repeats:
     ``generate`` with guidance passes its B prompt rows): ``seq`` int32 [R, t_max] each row's sequence (its prompt,
     then its tokens), ``prompt_len`` int32 [R] the lengths after the prefill, the sequence-bias table
     (``ops.repeats.SequenceBias`` or None), the repetition penalty, the n-gram size, the frequency and presence
-    penalties and the context n-gram size (the keyword arguments ``GPT2DoubleHeads._decode_setup`` returns).
-    ``create`` returns None when all of them are off, so then nothing is allocated or launched."""
+    penalties, the context n-gram size and the watermark (an ``ops.watermark.WatermarkingConfig`` or None; the keyword
+    arguments ``GPT2DoubleHeads._decode_setup`` returns). ``create`` returns None when all of them are off, so then
+    nothing is allocated or launched. The watermark is the last rule; on the native path it is a second launch
+    (``ops.watermark_``) after ``ops.penalize_repeats_``, which keeps the sequences it reads."""
 
     def __init__(self, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
                  rows: Optional[int] = None, bias=None, frequency: float = 0.0, presence: float = 0.0,
-                 context_ngram: int = 0):
+                 context_ngram: int = 0, watermark=None):
         B, T = input_ids.shape
         self.rows = cache.batch if rows is None else int(rows)
         self.seq = torch.zeros(self.rows, cache.t_max, dtype=torch.int32, device=input_ids.device)
@@ -288,28 +291,31 @@ class _Repeats:
         self.host_prompt_len = list(cache.host_lens[:self.rows])
         self.vocab, self.penalty, self.ngram, self.bias = vocab, penalty, ngram, bias
         self.counts = dict(frequency=float(frequency), presence=float(presence), context_ngram=int(context_ngram))
+        self.watermark = watermark
         if bias is not None and input_ids.is_cuda:
             bias.device_tensors(input_ids.device)       # before any capture: the graph keeps these pointers
 
     @classmethod
     def create(cls, input_ids: torch.Tensor, cache: KVCache, vocab: int, penalty: float, ngram: int,
                rows: Optional[int] = None, bias=None, frequency: float = 0.0, presence: float = 0.0,
-               context_ngram: int = 0) -> Optional["_Repeats"]:
+               context_ngram: int = 0, watermark=None) -> Optional["_Repeats"]:
         on = (penalty != 1.0 or ngram > 0 or bias is not None or frequency != 0 or presence != 0
-              or context_ngram > 0)
+              or context_ngram > 0 or watermark is not None)
         return cls(input_ids, cache, vocab, penalty, ngram, rows, bias, frequency, presence,
-                   context_ngram) if on else None
+                   context_ngram, watermark) if on else None
 
     def eager(self, logits: torch.Tensor, cache: KVCache, consumed: Optional[torch.Tensor]) -> torch.Tensor:
-        """``penalize_repeats_reference`` over every row's sequence, after storing ``consumed`` [R] (the tokens the last
-        decode step consumed; None before the first one) at ``lens - 1``."""
+        """``penalize_repeats_reference``, then ``watermark_reference`` when on, over every row's sequence, after
+        storing ``consumed`` [R] (the tokens the last decode step consumed; None before the first one) at
+        ``lens - 1``."""
         R = self.rows
         if consumed is not None:
             dev = self.seq.device
             self.seq[torch.arange(R, device=dev), cache.lens[:R].long() - 1] = consumed.to(dev, torch.int32)
-        return penalize_repeats_reference(logits, [self.seq[r, :x] for r, x in enumerate(cache.host_lens[:R])],
-                                          self.vocab, self.penalty, self.ngram, self.bias,
-                                          prompt_lens=self.host_prompt_len, **self.counts)
+        seqs = [self.seq[r, :x] for r, x in enumerate(cache.host_lens[:R])]
+        out = penalize_repeats_reference(logits, seqs, self.vocab, self.penalty, self.ngram, self.bias,
+                                         prompt_lens=self.host_prompt_len, **self.counts)
+        return out if self.watermark is None else watermark_reference(out, seqs, self.vocab, self.watermark)
 
     def reorder(self, rows: torch.Tensor) -> None:
         """Row r continues row ``rows[r]`` (a beam its parent)."""
@@ -317,10 +323,13 @@ class _Repeats:
 
     def native(self, logits: torch.Tensor, lens: torch.Tensor, step: torch.Tensor, ids: torch.Tensor,
                parent: Optional[torch.Tensor] = None, group: int = 1) -> None:
-        """``ops.penalize_repeats_`` on ``logits`` in place; it also stores ``ids`` and follows ``parent``."""
-        from ..ops import penalize_repeats_
+        """``ops.penalize_repeats_`` on ``logits`` in place (it also stores ``ids`` and follows ``parent``), then
+        ``ops.watermark_`` when on."""
+        from ..ops import penalize_repeats_, watermark_
         penalize_repeats_(logits, self.vocab, self.seq, self.prompt_len, lens, step, ids, parent, group,
                           self.penalty, self.ngram, self.bias, **self.counts)
+        if self.watermark is not None:
+            watermark_(logits, self.vocab, self.seq, lens, self.watermark)
 
 
 def _row_seeds(seed, B: int, dev) -> torch.Tensor:
@@ -676,7 +685,7 @@ class GPT2DoubleHeads(nn.Module):
                       rows_name: str = "beam rows (batch x num_beams)", sequence_bias=None, bad_words_ids=None,
                       stop_ids: Sequence[int] = (), kv_cache_dtype: Optional[str] = None,
                       frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
-                      context_no_repeat_ngram_size: int = 0):
+                      context_no_repeat_ngram_size: int = 0, watermarking_config=None):
         """The checks and prompt quantities the batched decoders share, before anything is launched:
         ``(B, T, lengths, n, t_max, last, tt_new, native, controls)``. ``last`` [B] is each prompt's last position,
         ``tt_new`` [B] the token type of new tokens (None without token types), ``native`` says whether the bf16 CUDA
@@ -684,7 +693,8 @@ class GPT2DoubleHeads(nn.Module):
         the error when more than one). ``controls`` are the keyword arguments of ``_Repeats.create`` after the
         decoder's own: the repetition penalty and n-gram size, ``bias`` the table of ``sequence_bias`` and
         ``bad_words_ids`` (``ops.repeats.check_sequence_bias_args``; None when both are off), and the frequency,
-        presence and context n-gram settings. ``kv_cache_dtype`` must be None or one of
+        presence and context n-gram settings, and ``watermark`` the checked ``watermarking_config``
+        (``ops.watermark.check_watermark_args``; None: off). ``kv_cache_dtype`` must be None or one of
         ``ops.kvcache.KV_CACHE_DTYPES``. Errors name ``who``."""
         from ..ops import LM_HEAD_MAX_ROWS
 
@@ -703,6 +713,7 @@ class GPT2DoubleHeads(nn.Module):
                           context_no_repeat_ngram_size)
         check_kv_cache_dtype(who, kv_cache_dtype)
         bias = check_sequence_bias_args(who, sequence_bias, bad_words_ids, self.cfg.vocab_size, stop_ids)
+        watermark = check_watermark_args(who, watermarking_config)
         t_max = max(lengths) + n
         if t_max > self.cfg.n_positions:
             raise ValueError(f"{who}: the longest prompt ({max(lengths)}) plus max_new_tokens ({n}) exceeds "
@@ -720,7 +731,7 @@ class GPT2DoubleHeads(nn.Module):
             tt_new = token_type_ids[torch.arange(B, device=dev), last].contiguous()
         controls = dict(penalty=repetition_penalty, ngram=no_repeat_ngram_size, bias=bias,
                         frequency=float(frequency_penalty), presence=float(presence_penalty),
-                        context_ngram=int(context_no_repeat_ngram_size))
+                        context_ngram=int(context_no_repeat_ngram_size), watermark=watermark)
         return B, T, lengths, n, t_max, last, tt_new, native, controls
 
     @staticmethod
@@ -789,7 +800,8 @@ class GPT2DoubleHeads(nn.Module):
                  bad_words_ids=None, top_h: float = 0.0,
                  kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
                  presence_penalty: float = 0.0,
-                 context_no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+                 context_no_repeat_ngram_size: int = 0,
+                 watermarking_config=None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -809,7 +821,12 @@ class GPT2DoubleHeads(nn.Module):
         times among the row's generated tokens (the prompt does not count) loses ``c * frequency_penalty``, then
         ``presence_penalty``. ``context_no_repeat_ngram_size`` = m (0: off; ParlAI's ``beam_context_block_ngram``)
         bans, after ``no_repeat_ngram_size``, every id that would complete an m-gram found inside the row's prompt;
-        m = 1 bans every prompt id. ``min_p`` (0: off), ``typical_p`` (1: off),
+        m = 1 bans every prompt id. ``watermarking_config`` (an ``ops.watermark.WatermarkingConfig`` or a dict with
+        its keys, HuggingFace's names and defaults; None: off) is Kirchenbauer et al.'s green-list watermark, the last
+        rule: every id that is green for the row's sequence (a keyed Philox hash of its last ``context_width`` ids,
+        ``seeding_scheme`` ``"lefthash"`` or ``"selfhash"``; ``ops/watermark.py``) gains ``bias``, greedy decoding
+        included, and ``ops.watermark.detect_watermark`` scores a text for it. With guidance it marks the prompt rows.
+        ``min_p`` (0: off), ``typical_p`` (1: off),
         ``epsilon_cutoff`` (0: off) and ``eta_cutoff`` (0: off) are HuggingFace's truncation samplers: at temperature
         > 0 they filter, in that order, the ids that top-k and top-p kept, just before the draw (inside
         ``ops.sample_tokens_`` on the native path). ``top_h`` (in (0, 1]; 0: off; 1 is on) is HuggingFace's
@@ -829,8 +846,8 @@ class GPT2DoubleHeads(nn.Module):
         ``ops.sampling.sample_reference``.
 
         ``prompt_lookup_num_tokens`` = k > 0 (HuggingFace's prompt lookup decoding; greedy only, without the repetition
-        controls, the penalties or the sequence bias) verifies up to k draft tokens per row and step, copied from the
-        row's own prompt and reply after the earliest earlier occurrence of its last ``max_matching_ngram_size`` (or
+        controls, the penalties, the sequence bias or the watermark) verifies up to k draft tokens per row and step,
+        copied from the row's own prompt and reply after the earliest earlier occurrence of its last ``max_matching_ngram_size`` (or
         fewer) tokens; the result is the greedy tokens. The definition is in ``ops/lookup.py``. On the native path
         (``B·(k+1)`` at most 64 rows) every verify step replays one CUDA graph: the drafts (``ops.lookup_draft_``), the model on k + 1 slots per row
         (``ops.verify_attention_``), the LM head, the slots' arg-maxes (``ops.lookup_argmax_``) and acceptance
@@ -899,6 +916,9 @@ class GPT2DoubleHeads(nn.Module):
                              f"combined with prompt_lookup_num_tokens or assistant_model (got {frequency_penalty}, "
                              f"{presence_penalty}, {context_no_repeat_ngram_size}, {prompt_lookup_num_tokens}, "
                              f"{type(assistant_model).__name__})")
+        if speculative and watermarking_config is not None:
+            raise ValueError("generate: watermarking_config cannot be combined with prompt_lookup_num_tokens or "
+                             f"assistant_model (got {prompt_lookup_num_tokens}, {type(assistant_model).__name__})")
         if guided and (assistant_model is not None or prompt_lookup_num_tokens != 0):
             raise ValueError("generate: guidance_scale != 1 cannot be combined with prompt_lookup_num_tokens or "
                              f"assistant_model (got {prompt_lookup_num_tokens}, {type(assistant_model).__name__})")
@@ -923,7 +943,8 @@ class GPT2DoubleHeads(nn.Module):
             repetition_penalty, no_repeat_ngram_size, num_beams=2 if guided else 1,
             rows_name="rows with guidance (batch x 2)", sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
             stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype, frequency_penalty=frequency_penalty,
-            presence_penalty=presence_penalty, context_no_repeat_ngram_size=context_no_repeat_ngram_size)
+            presence_penalty=presence_penalty, context_no_repeat_ngram_size=context_no_repeat_ngram_size,
+            watermarking_config=watermarking_config)
         dev, V = input_ids.device, self.cfg.vocab_size
         seeds = _row_seeds(seed, B, dev)
         if guided:                                  # rows [0, B): the prompts, rows [B, 2B): the negative prompts
@@ -996,8 +1017,8 @@ class GPT2DoubleHeads(nn.Module):
                     sequence_bias=None, bad_words_ids=None, min_p: float = 0.0, typical_p: float = 1.0,
                     epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0,
                     kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
-                    presence_penalty: float = 0.0,
-                    context_no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                    presence_penalty: float = 0.0, context_no_repeat_ngram_size: int = 0,
+                    watermarking_config=None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
         """Batched beam search with ``num_beams`` beams per prompt; the definition is in ``ops/beam.py``.
 
         ``input_ids`` [B, T] is right-padded; item b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -1012,7 +1033,8 @@ class GPT2DoubleHeads(nn.Module):
         applied first: a biased beam's log-probabilities are renormalised too, where HuggingFace adds the bias to the
         log-probabilities after normalisation. ``frequency_penalty``, ``presence_penalty`` and
         ``context_no_repeat_ngram_size`` work as in ``generate``, over each beam's own hypothesis, also before the
-        log-softmax.
+        log-softmax. So does ``watermarking_config`` (as in ``generate``), after them: each beam's green ids follow
+        its own hypothesis.
 
         ``do_sample=True`` is beam sampling (HuggingFace's ``generate(do_sample=True, num_beams=K)``; the definition is
         ``ops.beam.BeamSampleReference``): each beam's ids are filtered by ``top_k`` (0: off) and ``top_p`` at
@@ -1089,7 +1111,8 @@ class GPT2DoubleHeads(nn.Module):
                                 min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
                                 sequence_bias, bad_words_ids, kv_cache_dtype, frequency_penalty=frequency_penalty,
                                 presence_penalty=presence_penalty,
-                                context_no_repeat_ngram_size=context_no_repeat_ngram_size)
+                                context_no_repeat_ngram_size=context_no_repeat_ngram_size,
+                                watermarking_config=watermarking_config)
         dev, B, n = input_ids.device, input_ids.shape[0], int(max_new_tokens)
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result(R))
@@ -1109,12 +1132,12 @@ class GPT2DoubleHeads(nn.Module):
                                min_p: float = 0.0, typical_p: float = 1.0, epsilon_cutoff: float = 0.0,
                                eta_cutoff: float = 0.0, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
                                frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
-                               context_no_repeat_ngram_size: int = 0):
+                               context_no_repeat_ngram_size: int = 0, watermarking_config=None):
         """Stochastic beam search (Kool, van Hoof and Welling 2019): ``num_beams`` = K distinct replies per prompt,
         drawn without replacement from the law ``generate`` samples from with the same ``temperature``, ``top_k``,
         ``top_p``, truncation filters (``min_p``, ``typical_p``, ``epsilon_cutoff``, ``eta_cutoff``, ``top_h``), stop /
         suppress / ``min_new_tokens``, repetition settings, ``sequence_bias`` and ``bad_words_ids``, the frequency,
-        presence and context n-gram settings and ``max_new_tokens``; the definition
+        presence and context n-gram settings, ``watermarking_config`` and ``max_new_tokens``; the definition
         (rules R1-R8, properties P1-P4) is ``ops.beam.StochasticBeamReference``. The first reply of an item is itself
         an exact sample of that law. ``seed``: an int (item b uses ``seed + b``) or an int64 [B] tensor; an item's
         result depends on its prompt, its seed and the scalars only. The other arguments work as in ``beam_search``,
@@ -1156,7 +1179,8 @@ class GPT2DoubleHeads(nn.Module):
                                 min_new_tokens, repetition_penalty, no_repeat_ngram_size, stop_ids, suppress_ids, start,
                                 sequence_bias, bad_words_ids, kv_cache_dtype, frequency_penalty=frequency_penalty,
                                 presence_penalty=presence_penalty,
-                                context_no_repeat_ngram_size=context_no_repeat_ngram_size)
+                                context_no_repeat_ngram_size=context_no_repeat_ngram_size,
+                                watermarking_config=watermarking_config)
         dev = input_ids.device
         if not isinstance(sel, tuple):
             return tuple(t.to(dev) for t in sel.result())
@@ -1171,7 +1195,8 @@ class GPT2DoubleHeads(nn.Module):
                      max_new_tokens: int, min_new_tokens: int, repetition_penalty: float, no_repeat_ngram_size: int,
                      stop_ids: Sequence[int], suppress_ids: Sequence[int], start, sequence_bias=None,
                      bad_words_ids=None, kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
-                     presence_penalty: float = 0.0, context_no_repeat_ngram_size: int = 0):
+                     presence_penalty: float = 0.0, context_no_repeat_ngram_size: int = 0,
+                     watermarking_config=None):
         """The decode loop of the beam decoders. ``start(B, n, V, device, native)`` is called after the argument checks
         and before anything is launched; it returns the selector: on the native path ``(BeamState, keyword arguments
         of beam_step_)``, elsewhere a reference with ``step(logits) -> (next_ids, parent)`` and ``done``. Each prompt
@@ -1186,7 +1211,7 @@ class GPT2DoubleHeads(nn.Module):
             repetition_penalty, no_repeat_ngram_size, num_beams=K, sequence_bias=sequence_bias,
             bad_words_ids=bad_words_ids, stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype,
             frequency_penalty=frequency_penalty, presence_penalty=presence_penalty,
-            context_no_repeat_ngram_size=context_no_repeat_ngram_size)
+            context_no_repeat_ngram_size=context_no_repeat_ngram_size, watermarking_config=watermarking_config)
         dev, V, weight = input_ids.device, self.cfg.vocab_size, self.wte.weight
         sel = start(B, n, V, dev, native)
         if tt_new is not None:
@@ -1396,8 +1421,8 @@ class GPT2DoubleHeads(nn.Module):
                            suppress_ids: Sequence[int] = (), min_new_tokens: int = 0, repetition_penalty: float = 1.0,
                            no_repeat_ngram_size: int = 0, sequence_bias=None, bad_words_ids=None,
                            kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
-                           presence_penalty: float = 0.0,
-                           context_no_repeat_ngram_size: int = 0) -> Tuple[torch.Tensor, torch.Tensor]:
+                           presence_penalty: float = 0.0, context_no_repeat_ngram_size: int = 0,
+                           watermarking_config=None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched contrastive search (Su et al., 2022; HuggingFace's ``penalty_alpha`` + ``top_k``); the definition is
         in ``ops/contrastive.py``.
 
@@ -1407,7 +1432,8 @@ class GPT2DoubleHeads(nn.Module):
         without padding, then its emitted tokens). ``penalty_alpha = 0`` or ``top_k = 1`` is greedy decoding.
         ``input_ids``, ``lengths``, ``reply_type``, token types, ``stop_ids``, ``suppress_ids``, ``min_new_tokens``,
         the repetition controls, ``sequence_bias``, ``bad_words_ids``, ``frequency_penalty``, ``presence_penalty``,
-        ``context_no_repeat_ngram_size`` (applied to the logits before the candidates are taken) and the return value
+        ``context_no_repeat_ngram_size``, ``watermarking_config`` (applied to the logits before the candidates are
+        taken) and the return value
         ``(tokens, n_new)`` work as in ``generate``.
 
         The prompts are prefilled into a KV cache of ``max(lengths) + max_new_tokens`` positions (more than
@@ -1432,7 +1458,7 @@ class GPT2DoubleHeads(nn.Module):
             "contrastive_search", input_ids, lengths, token_type_ids, reply_type, max_new_tokens, min_new_tokens,
             repetition_penalty, no_repeat_ngram_size, sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
             stop_ids=stop_ids, frequency_penalty=frequency_penalty, presence_penalty=presence_penalty,
-            context_no_repeat_ngram_size=context_no_repeat_ngram_size)
+            context_no_repeat_ngram_size=context_no_repeat_ngram_size, watermarking_config=watermarking_config)
         cfg, dev, weight = self.cfg, input_ids.device, self.wte.weight
         tt_cand = tt_new.repeat_interleave(K) if tt_new is not None else None
         cache = self.new_cache(B, t_max)

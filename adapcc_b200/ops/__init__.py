@@ -72,6 +72,10 @@ def _lib():
         lib.adapcc_penalize_repeats.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int] + [c_void_p] * 5
                                                 + [c_int, c_float, c_int, c_void_p, c_void_p, c_int, c_int]
                                                 + [c_float, c_float, c_int, c_void_p])
+        lib.adapcc_watermark.argtypes = ([c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
+                                         + [c_uint] * 3 + [c_float, c_void_p])
+        lib.adapcc_watermark_count.argtypes = ([c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int]
+                                               + [c_uint] * 3 + [c_int, c_void_p, c_void_p])
         lib.adapcc_guidance_mix.argtypes = [c_void_p, c_int, c_int, c_int, c_float, c_void_p]
         lib.adapcc_cs_sim_numel.argtypes = [c_int] * 3
         lib.adapcc_cs_sim_numel.restype = c_longlong
@@ -836,6 +840,77 @@ def penalize_repeats_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, promp
                                        bias.num_targets if bias is not None else 0,
                                        bias.num_entries if bias is not None else 0, float(frequency), float(presence),
                                        int(context_ngram), _stream()), "penalize_repeats")
+
+
+# ---- green-list watermark: the bias and the detector's counts (csrc/ops_watermark.cu) --------------------------------
+WATERMARK_MAX_LEN = 1024       # sequence positions per row of the bias (GPT-2's n_positions)
+WATERMARK_COUNT_MAX_LEN = 8192  # ids per row of the detector
+
+
+def _watermark_key(who: str, config):
+    """(selfhash, width, k0, k1, theta, delta) of a validated config; ``ValueError`` naming ``who`` otherwise."""
+    from .watermark import check_watermark_args
+
+    cfg = check_watermark_args(who, config)
+    if cfg is None:
+        raise ValueError(f"{who}: config must be a WatermarkingConfig or a dict, got None")
+    k0, k1 = cfg.key_words
+    return cfg, (int(cfg.selfhash), cfg.context_width, k0, k1, cfg.threshold)
+
+
+def watermark_(logits: torch.Tensor, vocab: int, seq: torch.Tensor, lens: torch.Tensor, config) -> None:
+    """The green-list watermark bias of every row, in place, on the device (the definition in ``ops/watermark.py``,
+    which this kernel equals bit for bit). ``logits`` fp32 [R, ld] (the first ``vocab`` columns used); ``seq`` int32
+    [R, t_max] and ``lens`` int32 [R]: row r's sequence is ``seq[r, :lens[r]]``, as ``penalize_repeats_`` keeps it;
+    ``config`` a ``WatermarkingConfig`` or its dict. The grid depends on R and ``vocab`` only and there is no host
+    sync, so one capture serves every token."""
+    def bad(msg):
+        raise ValueError(f"watermark_: {msg}")
+
+    cfg, key = _watermark_key("watermark_", config)
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
+        bad(f"logits must be fp32 [R, ld] with unit column stride, got {logits.dtype} {tuple(logits.shape)}")
+    R = logits.shape[0]
+    if not 1 <= R <= 65535:
+        bad(f"need 1 to 65535 rows, got {R}")
+    if not 1 <= vocab <= logits.shape[1]:
+        bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
+    if (seq.dtype != torch.int32 or seq.dim() != 2 or seq.shape[0] != R or not seq.is_contiguous()
+            or not 1 <= seq.shape[1] <= WATERMARK_MAX_LEN):
+        bad(f"seq must be a contiguous int32 [{R}, t_max] tensor with t_max <= {WATERMARK_MAX_LEN}, got {seq.dtype} "
+            f"{tuple(seq.shape)}")
+    if lens.dtype != torch.int32 or not lens.is_contiguous() or lens.numel() != R:
+        bad(f"lens must be a contiguous int32 tensor of {R} elements, got {lens.dtype} {tuple(lens.shape)}")
+    _same_device("watermark_", logits.device, (seq, lens))
+    _ck(_lib().adapcc_watermark(_ptr(logits), logits.stride(0), int(vocab), R, _ptr(seq), seq.shape[1], _ptr(lens),
+                                *key, float(cfg.delta), _stream()), "watermark")
+
+
+def watermark_count_(ids: torch.Tensor, lens: torch.Tensor, scored_from: torch.Tensor, config,
+                     ignore_repeated_ngrams: bool = False, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """The detector's counts on the device (``ops.watermark.watermark_counts_reference``, exactly): ``ids`` int32
+    [B, T] right-padded, ``lens`` and ``scored_from`` int32 [B]. Returns ``out`` int32 [B, 2] (allocated when None):
+    per row the positions scored and the green ones among them. One CTA per row, integer counts, no atomics."""
+    def bad(msg):
+        raise ValueError(f"watermark_count_: {msg}")
+
+    cfg, key = _watermark_key("watermark_count_", config)
+    if ids.dtype != torch.int32 or ids.dim() != 2 or not ids.is_contiguous() or ids.shape[0] < 1:
+        bad(f"ids must be a contiguous int32 [B, T] tensor, got {ids.dtype} {tuple(ids.shape)}")
+    B, T = ids.shape
+    if not 1 <= T <= WATERMARK_COUNT_MAX_LEN:
+        bad(f"need 1 <= T <= {WATERMARK_COUNT_MAX_LEN} ids per row, got {T}")
+    for name, t in (("lens", lens), ("scored_from", scored_from)):
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != B:
+            bad(f"{name} must be a contiguous int32 tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if out is None:
+        out = torch.empty(B, 2, dtype=torch.int32, device=ids.device)
+    if out.dtype != torch.int32 or not out.is_contiguous() or out.shape != (B, 2):
+        bad(f"out must be a contiguous int32 [{B}, 2] tensor, got {out.dtype} {tuple(out.shape)}")
+    _same_device("watermark_count_", ids.device, (lens, scored_from, out))
+    _ck(_lib().adapcc_watermark_count(_ptr(ids), T, B, _ptr(lens), _ptr(scored_from), *key,
+                                      int(bool(ignore_repeated_ngrams)), _ptr(out), _stream()), "watermark_count")
+    return out
 
 
 # ---- classifier-free guidance (csrc/ops_guidance.cu) ---------------------------------------------------------------

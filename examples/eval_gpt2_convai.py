@@ -96,6 +96,14 @@ def main():
     p.add_argument("--bad_words", default="",
                    help="f1: comma-separated words the replies may never contain, each banned as encoded with and "
                         "without a leading space; replies go through the batched path")
+    p.add_argument("--watermark_bias", type=float, default=None,
+                   help="f1: mark the replies with the green-list watermark, adding this to every green id's logit "
+                        "(default: off); the result adds the replies' mean z-score and detected fraction")
+    p.add_argument("--watermark_ratio", type=float, default=0.25, help="f1: the watermark's green-list ratio")
+    p.add_argument("--watermark_scheme", choices=("lefthash", "selfhash"), default="lefthash",
+                   help="f1: the watermark's seeding scheme")
+    p.add_argument("--watermark_context_width", type=int, default=1,
+                   help="f1: the ids before a token that seed its green list")
     p.add_argument("--kv_cache_dtype", choices=("fp8_e4m3",), default=None,
                    help="f1: keep the KV cache in fp8 (e4m3 bytes with a power-of-two scale per vector; default: the "
                         "model's dtype); replies go through the batched path")
@@ -119,6 +127,10 @@ def main():
                   presence_penalty=a.presence_penalty, context_no_repeat_ngram_size=a.context_no_repeat_ngram_size)
         if a.bad_words:
             kw["bad_words_ids"] = bad_word_ids(tok, a.bad_words.split(","))
+        if a.watermark_bias is not None:
+            kw["watermarking_config"] = dict(bias=a.watermark_bias, greenlist_ratio=a.watermark_ratio,
+                                             seeding_scheme=a.watermark_scheme,
+                                             context_width=a.watermark_context_width)
         if a.assistant_checkpoint:
             kw["assistant_model"] = load_model_from_checkpoint(
                 a.assistant_checkpoint, a.device, torch.bfloat16 if a.device.startswith("cuda") else None)[0]

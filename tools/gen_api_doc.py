@@ -34,6 +34,8 @@ MODULES = [
     ("adapcc_b200.ops.repeats", ["penalize_repeats_reference", "banned_ngram_ids", "check_repeat_args",
                                  "finite_fp32", "check_sequence_bias_args", "SequenceBias"]),
     ("adapcc_b200.ops.guidance", ["check_guidance_args", "guided_scores_reference"]),
+    ("adapcc_b200.ops.watermark", ["WatermarkingConfig", "check_watermark_args", "watermark_reference",
+                                   "watermark_counts_reference", "detect_watermark", "WatermarkDetectorOutput"]),
     ("adapcc_b200.ops.kvcache", ["quantize", "dequantize", "store_", "check_kv_cache_dtype"]),
     ("adapcc_b200.ops.layers", ["FusedLayerNorm", "FusedLinear", "linear_backward"]),
     ("adapcc_b200.ops.gemm", ["linear_act", "linear_gelu", "supported", "default_variant"]),
