@@ -31,6 +31,7 @@
 #include "common.h"
 #include "device_prims.cuh"
 #include "sample_filter.cuh"
+#include "sample_row.cuh"
 
 namespace adapcc {
 
@@ -100,121 +101,6 @@ lm_head_logits_kernel(const __nv_bfloat16* __restrict__ h, int ld_h, const __nv_
 }
 
 // ---- sampling --------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ float philox_uniform(uint32_t w) { return (float)(w >> 8) * 0x1p-24f; }
-
-// The inverse-CDF pick over s_x[0, V) by the whole CTA: the ids with `counts(x)` count, with weight `weight(x)`. Returns the smallest counting i whose inclusive prefix of weights exceeds u Z' (Z', the total, goes to `zp`), or
-// the largest counting id when rounding leaves none, or -1 when no id counts. Thread t owns the contiguous ids
-// [t C, t C + C) (C odd, so a warp's reads hit 32 different banks); prefix = (sum of the lower threads' chunks, by a
-// shuffle scan and warp totals in order) + the running sum inside the chunk.
-template <class Counts, class Weight>
-__device__ __forceinline__ int scan_pick(const float* s_x, SampleSmem& sm, int V, Counts counts, Weight weight, float u,
-                                         float& zp) {
-  const int tid = threadIdx.x;
-  const int C = ((V + kSampleThreads - 1) / kSampleThreads) | 1;
-  const int i0 = min(tid * C, V), i1 = min(i0 + C, V);
-  float run = 0.f;
-  int last = -1;
-  for (int i = i0; i < i1; ++i) {
-    const float x = s_x[i];
-    if (counts(x)) {
-      run += weight(x);
-      last = i;
-    }
-  }
-  const int lane = tid & 31, warp = tid >> 5;
-  float inc = run;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float y = __shfl_up_sync(0xffffffffu, inc, o);
-    if (lane >= o) inc += y;
-  }
-  float excl = __shfl_up_sync(0xffffffffu, inc, 1);
-  if (lane == 0) excl = 0.f;
-  __syncthreads();
-  if (lane == 31) sm.f[warp] = inc;
-  __syncthreads();
-  // offset of this warp: an inclusive shuffle scan over the warp totals (lane w holds warp w's), the same in
-  // every warp; Z' is its last element
-  float tot = sm.f[lane];
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const float y = __shfl_up_sync(0xffffffffu, tot, o);
-    if (lane >= o) tot += y;
-  }
-  zp = __shfl_sync(0xffffffffu, tot, 31);
-  float off = __shfl_sync(0xffffffffu, tot, (warp + 31) & 31);
-  if (warp == 0) off = 0.f;
-  excl = off + excl;
-  const float target = u * zp;
-  int found = INT_MAX;
-  if (i0 < i1) {
-    float acc = 0.f;
-    for (int i = i0; i < i1; ++i) {
-      const float x = s_x[i];
-      if (counts(x)) {
-        acc += weight(x);
-        if (excl + acc > target) {
-          found = i;
-          break;
-        }
-      }
-    }
-  }
-  // the first crossing over the block; when rounding leaves none, the largest counting id
-  const unsigned long long first = 0xFFFFFFFFull - block_max(sm, 0xFFFFFFFFull - (unsigned long long)found);
-  return first != (unsigned long long)INT_MAX ? (int)first
-                                              : (int)block_max(sm, (unsigned long long)(last + 1)) - 1;
-}
-
-// What a draw decided from: the survivors are the ids with f2key(s_x[i]) >= tau, with weights expf(s_x[i] - m) and
-// total zp. No survivor (greedy, or no finite logit): tau above every key, zp = 0.
-struct RowCut {
-  uint32_t tau;
-  float m, zp;
-};
-
-__device__ __forceinline__ float cut_prob(float x, const RowCut& c) {
-  return f2key(x) >= c.tau ? expf(x - c.m) / c.zp : 0.f;
-}
-
-// One row of the definition (DESIGN.md §4a, steps 1-7) by the whole CTA: the logits row `l`, the tokens generated so
-// far `step` (the min-length rule), the Philox counter `pos` and the row's seed. Returns the token, the same in every
-// thread. sample_tokens_kernel, sample_slots_kernel and spec_slots_kernel all draw through it, so their tokens are the
-// same bits. With `cut`, it also returns the survivors; s_x then still holds the row they are read from.
-__device__ __forceinline__ int draw_row(float* s_x, SampleSmem& sm, const SampleArgs& a, const float* l, int step,
-                                        int pos, long long seed, RowCut* cut = nullptr) {
-  if (cut) *cut = RowCut{0xFFFFFFFFu, 0.f, 0.f};
-  const int V = a.vocab;
-  unsigned long long best;
-  const int present = row_prologue(s_x, sm, l, V, a.temperature, step, a.min_new, a.suppress, a.n_suppress, best);
-  int token = 0;                                    // a row without a finite logit draws id 0
-  if (present > 0 && a.temperature == 0.f) {
-    token = (int)(0xFFFFFFFFu - (uint32_t)best);
-  } else if (present > 0) {
-    const uint32_t mkey = (uint32_t)(best >> 32);
-    const float m = key2f(mkey);
-    int kept = present;
-    if (a.top_h > 0.f) {
-      __shared__ unsigned long long s_sel[kTopHN];
-      __shared__ int s_n;
-      kept = top_h_row(s_x, sm, V, present, m, a.top_h, 1, s_sel, &s_n);
-    }
-    uint32_t tau = row_tau(s_x, sm, V, a.top_k, a.top_p, 1, kept, mkey, m);
-    if (a.f.on()) {
-      filter_row(s_x, sm, V, a.f, tau, m, mkey);
-      tau = kNegInfKey + 1;                         // the survivors are the finite ids
-    }
-    // the draw: the smallest i whose inclusive prefix of surviving weights exceeds u Z'
-    const uint32_t w0 = philox4((uint32_t)pos, (uint32_t)(unsigned long long)seed,
-                                (uint32_t)((unsigned long long)seed >> 32)).x;
-    float zp;
-    token = scan_pick(s_x, sm, V, [tau](float x) { return f2key(x) >= tau; }, [m](float x) { return expf(x - m); },
-                      philox_uniform(w0), zp);
-    if (cut) *cut = RowCut{tau, m, zp};
-  }
-  return token;
-}
-
 __global__ void __launch_bounds__(kSampleThreads, 1)
 sample_tokens_kernel(const __grid_constant__ SampleArgs a) {
   extern __shared__ float s_x[];                    // [vocab]
@@ -396,6 +282,42 @@ static int allow_row_smem(const char* who, Kernel kernel, std::once_flag* once, 
   return 0;
 }
 
+// The checks of adapcc_sample_tokens_filtered and adapcc_sample_tokens_synthid; fills `a` or sets the error.
+static int sample_args(const char* who, const float* logits, int ld, int vocab, int B, float temperature, int top_k,
+                       float top_p, float min_p, float typical_p, float epsilon, float eta, const long long* seeds,
+                       const int* pos, int* step, int min_new, const int* suppress, int n_suppress, const int* stop,
+                       int n_stop, int* done, long long* next_ids, long long* tokens, int max_new, float top_h,
+                       SampleArgs& a) {
+  if (B < 1 || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab || max_new < 1) {
+    set_error("%s: need B >= 1, 1 <= vocab <= %d, ld >= vocab, max_new >= 1 (B=%d vocab=%d ld=%d max_new=%d)", who,
+              kSampleMaxVocab, B, vocab, ld, max_new);
+    return -1;
+  }
+  if (!(temperature >= 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
+    set_error("%s: need temperature >= 0, top_k >= 0, 0 < top_p <= 1 (got %g, %d, %g)", who, temperature, top_k,
+              top_p);
+    return -1;
+  }
+  if (!(min_p >= 0.f && min_p <= 1.f) || !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) ||
+      !(eta >= 0.f && eta < 1.f) || !(top_h >= 0.f && top_h <= 1.f)) {
+    set_error("%s: need 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= epsilon < 1, 0 <= eta < 1, 0 <= top_h <= 1 (got "
+              "%g, %g, %g, %g, %g)", who, min_p, typical_p, epsilon, eta, top_h);
+    return -1;
+  }
+  if (n_suppress < 0 || n_stop < 0 || n_suppress > kSampleMaxList || n_stop > kSampleMaxList ||
+      (n_suppress && !suppress) || (n_stop && !stop)) {
+    set_error("%s: suppress / stop lists of at most %d ids (got %d, %d)", who, kSampleMaxList, n_suppress, n_stop);
+    return -1;
+  }
+  if (!logits || !seeds || !pos || !step || !done || !next_ids || !tokens) {
+    set_error("%s: null pointer", who);
+    return -1;
+  }
+  a = SampleArgs{logits, ld, vocab, temperature, top_p, top_k, seeds, pos, step, min_new, suppress, n_suppress,
+                 stop, n_stop, done, next_ids, tokens, max_new, top_h, FilterArgs{min_p, typical_p, epsilon, eta, 1}};
+  return 0;
+}
+
 }  // namespace adapcc
 
 using namespace adapcc;
@@ -445,47 +367,44 @@ int adapcc_sample_tokens_filtered(const float* logits, int ld, int vocab, int B,
                                   const long long* seeds, const int* pos, int* step, int min_new, const int* suppress,
                                   int n_suppress, const int* stop, int n_stop, int* done, long long* next_ids,
                                   long long* tokens, int max_new, float top_h, void* stream) {
-  if (B < 1 || vocab < 1 || vocab > kSampleMaxVocab || ld < vocab || max_new < 1) {
-    set_error("sample_tokens: need B >= 1, 1 <= vocab <= %d, ld >= vocab, max_new >= 1 (B=%d vocab=%d ld=%d "
-              "max_new=%d)", kSampleMaxVocab, B, vocab, ld, max_new);
+  SampleArgs a;
+  if (sample_args("sample_tokens", logits, ld, vocab, B, temperature, top_k, top_p, min_p, typical_p, epsilon, eta,
+                  seeds, pos, step, min_new, suppress, n_suppress, stop, n_stop, done, next_ids, tokens, max_new,
+                  top_h, a))
     return -1;
-  }
-  if (!(temperature >= 0.f) || top_k < 0 || !(top_p > 0.f && top_p <= 1.f)) {
-    set_error("sample_tokens: need temperature >= 0, top_k >= 0, 0 < top_p <= 1 (got %g, %d, %g)", temperature, top_k,
-              top_p);
-    return -1;
-  }
-  if (!(min_p >= 0.f && min_p <= 1.f) || !(typical_p > 0.f && typical_p <= 1.f) || !(epsilon >= 0.f && epsilon < 1.f) ||
-      !(eta >= 0.f && eta < 1.f) || !(top_h >= 0.f && top_h <= 1.f)) {
-    set_error("sample_tokens: need 0 <= min_p <= 1, 0 < typical_p <= 1, 0 <= epsilon < 1, 0 <= eta < 1, 0 <= top_h "
-              "<= 1 (got %g, %g, %g, %g, %g)", min_p, typical_p, epsilon, eta, top_h);
-    return -1;
-  }
-  if (n_suppress < 0 || n_stop < 0 || n_suppress > kSampleMaxList || n_stop > kSampleMaxList ||
-      (n_suppress && !suppress) || (n_stop && !stop)) {
-    set_error("sample_tokens: suppress / stop lists of at most %d ids (got %d, %d)", kSampleMaxList, n_suppress, n_stop);
-    return -1;
-  }
-  if (!logits || !seeds || !pos || !step || !done || !next_ids || !tokens) {
-    set_error("sample_tokens: null pointer");
-    return -1;
-  }
   static std::once_flag once[kOpsMaxDevices];
   static cudaError_t setup[kOpsMaxDevices];
-  int dev = 0;
-  CUDA_TRY(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= kOpsMaxDevices) { set_error("sample_tokens: device %d out of range", dev); return -1; }
-  std::call_once(once[dev], [&] {
-    setup[dev] = cudaFuncSetAttribute(sample_tokens_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      kSampleMaxVocab * (int)sizeof(float));
-  });
-  CUDA_TRY(setup[dev]);
-  SampleArgs a{logits, ld, vocab, temperature, top_p, top_k, seeds, pos, step, min_new, suppress, n_suppress,
-               stop, n_stop, done, next_ids, tokens, max_new, top_h, FilterArgs{min_p, typical_p, epsilon, eta, 1}};
+  if (allow_row_smem("sample_tokens", sample_tokens_kernel, once, setup)) return -1;
   cudaStream_t s = (cudaStream_t)stream;
   sample_tokens_kernel<<<B, kSampleThreads, (size_t)vocab * sizeof(float), s>>>(a);
   CUDA_TRY(cudaGetLastError());
   count_launch();
+  step_incr_kernel<<<1, 1, 0, s>>>(step);
+  CUDA_TRY(cudaGetLastError());
+  count_launch();
+  return 0;
+}
+
+// adapcc_sample_tokens_filtered with SynthID's tournament (DESIGN.md §4a, step 6b) on the steps it watermarks: table
+// uint32 [ceil(S / 32)] on the device (the g-value bitset of S = table_size entries, S in [1, 2^24]); depth m in [1,
+// 64] keys (host array), ngram n in [2, 16], history H >= 1, skip s0 in {0, n - 1}. A row's context comes from its
+// reply columns tokens[b, 0, step), so there is no other per-row state.
+int adapcc_sample_tokens_synthid(const float* logits, int ld, int vocab, int B, float temperature, int top_k,
+                                 float top_p, float min_p, float typical_p, float epsilon, float eta,
+                                 const long long* seeds, const int* pos, int* step, int min_new, const int* suppress,
+                                 int n_suppress, const int* stop, int n_stop, int* done, long long* next_ids,
+                                 long long* tokens, int max_new, float top_h, const unsigned* table,
+                                 long long table_size, int depth, int ngram, int history, int skip,
+                                 const unsigned long long* keys, void* stream) {
+  SampleArgs a;
+  if (sample_args("sample_tokens_synthid", logits, ld, vocab, B, temperature, top_k, top_p, min_p, typical_p, epsilon,
+                  eta, seeds, pos, step, min_new, suppress, n_suppress, stop, n_stop, done, next_ids, tokens, max_new,
+                  top_h, a))
+    return -1;
+  SynthIDArgs w;
+  if (synthid_args("sample_tokens_synthid", table, table_size, depth, ngram, history, skip, keys, w)) return -1;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (sample_tokens_synthid_launch(a, w, B, s)) return -1;
   step_incr_kernel<<<1, 1, 0, s>>>(step);
   CUDA_TRY(cudaGetLastError());
   count_launch();

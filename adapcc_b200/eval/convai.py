@@ -28,6 +28,7 @@ import torch.nn.functional as F
 from ..data.personachat import IGNORE, build_input_from_segments
 from ..data.tokenizer import DialogTokenizer
 from ..ops.sampling import top_filtering
+from ..ops.synthid import check_synthid_args, is_synthid_config
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -343,7 +344,9 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     batched path, and the result also holds ``watermark_z``, the mean z-score of the replies scored on their own
     (``detect_watermark`` without the prompt; replies with nothing to score are left out), and
     ``watermark_detected``, the fraction of replies it flags, next to F1: what the mark costs in F1 against how
-    reliably it is found."""
+    reliably it is found. With a SynthID ``watermarking_config`` (``ops/synthid.py``) the replies are scored by
+    ``detect_synthid`` instead, on their own, and the result holds ``synthid_score``, the replies' mean weighted mean
+    score (replies with nothing to score are left out), and ``synthid_detected``, the fraction it flags."""
     from ..ops.assisted import check_verification
     check_verification("evaluate_dialogs", assistant_verification, assistant_model)
     repeats = (repetition_penalty != 1.0 or no_repeat_ngram_size > 0 or bool(sequence_bias)
@@ -429,7 +432,15 @@ def _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples,
         replies = sample_replies(model, tokenizer, [(p, h) for p, h, _ in chunk], device=device, seeds=seeds,
                                  **sample_kw)
         acc += sum(f1_score(tokenizer.decode(r), [gold]) for r, (_, _, gold) in zip(replies, chunk))
-        if wm is not None:
+        if wm is not None and is_synthid_config(wm):
+            from ..ops.synthid import detect_synthid
+
+            width = max(int(check_synthid_args("evaluate_dialogs", wm).ngram_len), max(len(r) for r in replies))
+            ids = torch.tensor([r + [0] * (width - len(r)) for r in replies], dtype=torch.int64)
+            det = detect_synthid(ids.to(device), wm, lengths=[len(r) for r in replies])
+            z += [float(x) for x in det.weighted_mean_score if math.isfinite(x)]
+            flagged += int(det.prediction.sum())
+        elif wm is not None:
             from ..ops.watermark import detect_watermark
 
             width = max(1, max(len(r) for r in replies))
@@ -438,7 +449,10 @@ def _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples,
             z += [float(x) for x in det.z_score if math.isfinite(x)]
             flagged += int(det.prediction.sum())
     out = {"f1": acc / max(1, len(examples)), "examples": len(examples)}
-    if wm is not None:
+    if wm is not None and is_synthid_config(wm):
+        out.update(synthid_score=sum(z) / len(z) if z else float("nan"),
+                   synthid_detected=flagged / max(1, len(examples)))
+    elif wm is not None:
         out.update(watermark_z=sum(z) / len(z) if z else float("nan"),
                    watermark_detected=flagged / max(1, len(examples)))
     return out

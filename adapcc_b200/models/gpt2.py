@@ -34,6 +34,7 @@ from ..ops.guidance import check_guidance_args, guided_scores_reference
 from ..ops.kvcache import check_kv_cache_dtype
 from ..ops.layers import FusedLayerNorm, FusedLinear
 from ..ops.repeats import check_repeat_args, check_sequence_bias_args, penalize_repeats_reference
+from ..ops.synthid import check_synthid_args, is_synthid_config
 from ..ops.watermark import check_watermark_args, watermark_reference
 from ..ops.sampling import check_filter_args, sample_reference, top_filtering
 
@@ -685,7 +686,7 @@ class GPT2DoubleHeads(nn.Module):
                       rows_name: str = "beam rows (batch x num_beams)", sequence_bias=None, bad_words_ids=None,
                       stop_ids: Sequence[int] = (), kv_cache_dtype: Optional[str] = None,
                       frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
-                      context_no_repeat_ngram_size: int = 0, watermarking_config=None):
+                      context_no_repeat_ngram_size: int = 0, watermarking_config=None, synthid_ok: bool = False):
         """The checks and prompt quantities the batched decoders share, before anything is launched:
         ``(B, T, lengths, n, t_max, last, tt_new, native, controls)``. ``last`` [B] is each prompt's last position,
         ``tt_new`` [B] the token type of new tokens (None without token types), ``native`` says whether the bf16 CUDA
@@ -694,8 +695,11 @@ class GPT2DoubleHeads(nn.Module):
         decoder's own: the repetition penalty and n-gram size, ``bias`` the table of ``sequence_bias`` and
         ``bad_words_ids`` (``ops.repeats.check_sequence_bias_args``; None when both are off), and the frequency,
         presence and context n-gram settings, and ``watermark`` the checked ``watermarking_config``
-        (``ops.watermark.check_watermark_args``; None: off). ``kv_cache_dtype`` must be None or one of
-        ``ops.kvcache.KV_CACHE_DTYPES``. Errors name ``who``."""
+        (``ops.watermark.check_watermark_args``; None: off). A SynthID ``watermarking_config`` (``ops.synthid.
+        is_synthid_config``) is checked by ``check_synthid_args`` instead and, when the decoder takes one
+        (``synthid_ok``), goes into ``controls`` as ``synthid``, which the decoder removes before ``_Repeats.create``;
+        a decoder that does not take one raises a ``ValueError`` naming SynthID. ``kv_cache_dtype`` must be None or one
+        of ``ops.kvcache.KV_CACHE_DTYPES``. Errors name ``who``."""
         from ..ops import LM_HEAD_MAX_ROWS
 
         if input_ids.dim() != 2 or input_ids.shape[0] < 1 or input_ids.shape[1] < 1:
@@ -713,6 +717,14 @@ class GPT2DoubleHeads(nn.Module):
                           context_no_repeat_ngram_size)
         check_kv_cache_dtype(who, kv_cache_dtype)
         bias = check_sequence_bias_args(who, sequence_bias, bad_words_ids, self.cfg.vocab_size, stop_ids)
+        synthid = None
+        if is_synthid_config(watermarking_config):
+            if not synthid_ok:
+                raise ValueError(f"{who}: SynthID watermarking (a SynthIDTextWatermarkingConfig) is a sampling "
+                                 "watermark offered by generate only: its per-row context state does not follow beam "
+                                 "reordering")
+            synthid = check_synthid_args(who, watermarking_config)
+            watermarking_config = None
         watermark = check_watermark_args(who, watermarking_config)
         t_max = max(lengths) + n
         if t_max > self.cfg.n_positions:
@@ -732,6 +744,8 @@ class GPT2DoubleHeads(nn.Module):
         controls = dict(penalty=repetition_penalty, ngram=no_repeat_ngram_size, bias=bias,
                         frequency=float(frequency_penalty), presence=float(presence_penalty),
                         context_ngram=int(context_no_repeat_ngram_size), watermark=watermark)
+        if synthid is not None:
+            controls["synthid"] = synthid
         return B, T, lengths, n, t_max, last, tt_new, native, controls
 
     @staticmethod
@@ -826,6 +840,13 @@ class GPT2DoubleHeads(nn.Module):
         rule: every id that is green for the row's sequence (a keyed Philox hash of its last ``context_width`` ids,
         ``seeding_scheme`` ``"lefthash"`` or ``"selfhash"``; ``ops/watermark.py``) gains ``bias``, greedy decoding
         included, and ``ops.watermark.detect_watermark`` scores a text for it. With guidance it marks the prompt rows.
+        ``watermarking_config`` may instead be SynthID Text (an ``ops.synthid.SynthIDTextWatermarkingConfig`` or a dict
+        with ``keys`` or ``ngram_len``; HuggingFace's names and defaults; ``ops/synthid.py``): it adds no bias but
+        re-weights the distribution the sampler draws from, after the truncation filters, by a tournament of
+        ``len(keys)`` layers keyed on the row's last ``ngram_len - 1`` generated ids (HuggingFace's hash and g-value
+        table, so ``ops.synthid.detect_synthid`` and HuggingFace's detectors score the text); greedy decoding takes the
+        arg-max of the re-weighted softmax. On the native path it runs inside ``ops.sample_tokens_``, with no extra
+        launch. With guidance it marks the prompt rows.
         ``min_p`` (0: off), ``typical_p`` (1: off),
         ``epsilon_cutoff`` (0: off) and ``eta_cutoff`` (0: off) are HuggingFace's truncation samplers: at temperature
         > 0 they filter, in that order, the ids that top-k and top-p kept, just before the draw (inside
@@ -944,7 +965,8 @@ class GPT2DoubleHeads(nn.Module):
             rows_name="rows with guidance (batch x 2)", sequence_bias=sequence_bias, bad_words_ids=bad_words_ids,
             stop_ids=stop_ids, kv_cache_dtype=kv_cache_dtype, frequency_penalty=frequency_penalty,
             presence_penalty=presence_penalty, context_no_repeat_ngram_size=context_no_repeat_ngram_size,
-            watermarking_config=watermarking_config)
+            watermarking_config=watermarking_config, synthid_ok=True)
+        synthid = controls.pop("synthid", None)
         dev, V = input_ids.device, self.cfg.vocab_size
         seeds = _row_seeds(seed, B, dev)
         if guided:                                  # rows [0, B): the prompts, rows [B, 2B): the negative prompts
@@ -972,7 +994,8 @@ class GPT2DoubleHeads(nn.Module):
                 if reps is not None:
                     logits = reps.eager(logits, cache, nxt if i else None)
                 nxt, tok, done = sample_reference(logits, V, temperature, top_k, top_p, seeds, cache.lens[:B], i,
-                                                  min_new_tokens, suppress_ids, stop_ids, done, **filters)
+                                                  min_new_tokens, suppress_ids, stop_ids, done, **filters,
+                                                  synthid=synthid, generated=tokens[:, :i])
                 tokens[:, i] = tok.to(dev)
                 if bool(done.all()):
                     break
@@ -996,7 +1019,7 @@ class GPT2DoubleHeads(nn.Module):
             if reps is not None:
                 reps.native(lg, lens, step, ids)
             sample_tokens_(lg, V, temperature, top_k, top_p, seeds, lens, step,
-                           min_new_tokens, sup, stop, done, ids, tokens, **filters)
+                           min_new_tokens, sup, stop, done, ids, tokens, **filters, synthid=synthid)
             if guided:                              # the negative rows consume the prompt rows' tokens
                 next_ids[B:].copy_(ids)
 

@@ -57,6 +57,11 @@ def _lib():
                                                       + [c_float] * 5 + [c_void_p] * 3
                                                       + [c_int, c_void_p, c_int, c_void_p, c_int]
                                                       + [c_void_p] * 3 + [c_int, c_float, c_void_p])
+        lib.adapcc_sample_tokens_synthid.argtypes = ([c_void_p, c_int, c_int, c_int, c_float, c_int]
+                                                     + [c_float] * 5 + [c_void_p] * 3
+                                                     + [c_int, c_void_p, c_int, c_void_p, c_int]
+                                                     + [c_void_p] * 3 + [c_int, c_float, c_void_p, c_longlong]
+                                                     + [c_int] * 4 + [c_void_p, c_void_p])
         lib.adapcc_beam_step.argtypes = ([c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int]
                                          + [c_void_p, c_int, c_void_p, c_int, c_void_p, c_int, c_int]
                                          + [c_void_p] * 11 + [c_float, c_void_p])
@@ -76,6 +81,8 @@ def _lib():
                                          + [c_uint] * 3 + [c_float, c_void_p])
         lib.adapcc_watermark_count.argtypes = ([c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int]
                                                + [c_uint] * 3 + [c_int, c_void_p, c_void_p])
+        lib.adapcc_synthid_count.argtypes = ([c_void_p, c_int, c_int, c_void_p, c_void_p, c_longlong, c_void_p,
+                                              c_longlong] + [c_int] * 3 + [c_void_p] * 5)
         lib.adapcc_guidance_mix.argtypes = [c_void_p, c_int, c_int, c_int, c_float, c_void_p]
         lib.adapcc_cs_sim_numel.argtypes = [c_int] * 3
         lib.adapcc_cs_sim_numel.restype = c_longlong
@@ -491,7 +498,8 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
                    seeds: torch.Tensor, pos: torch.Tensor, step: torch.Tensor, min_new: int,
                    suppress_ids: Optional[torch.Tensor], stop_ids: Optional[torch.Tensor], done: torch.Tensor,
                    next_ids: torch.Tensor, tokens: torch.Tensor, min_p: float = 0.0, typical_p: float = 1.0,
-                   epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0) -> None:
+                   epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0,
+                   synthid=None) -> None:
     """One seeded top-k / top-p draw per row, on the device (the definition in ``ops/sampling.py``, which computes the
     same in fp64). ``logits`` fp32 [B, ld] (the first ``vocab`` columns used), ``seeds`` int64 [B], ``pos`` int32 [B]
     (position of the drawn token: the Philox counter), ``step`` int32 [1] (tokens generated so far; incremented),
@@ -501,7 +509,12 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
 
     ``min_p``, ``typical_p``, ``epsilon_cutoff`` and ``eta_cutoff`` (HuggingFace's truncation samplers; off at 0, 1,
     0 and 0) filter the ids that top-p kept, in that order, before the draw; ``top_h`` (HuggingFace's entropy-bounded
-    top-h, in (0, 1]; 0: off) filters the row before top-k. None has an effect at temperature 0."""
+    top-h, in (0, 1]; 0: off) filters the row before top-k. None has an effect at temperature 0.
+
+    ``synthid`` (an ``ops.synthid.SynthIDTextWatermarkingConfig`` or its dict; None: off) runs SynthID's tournament
+    between the filters and the draw on the steps it watermarks, greedy decoding included (``ops/synthid.py``). Each
+    row's context is read from its own columns ``tokens[b, :step]``, so ``tokens`` must hold every token of the reply
+    from step 0 (``max_new`` >= the steps drawn). The table goes to the device once per table and device."""
     def bad(msg):
         raise ValueError(f"sample_tokens_: {msg}")
 
@@ -526,6 +539,17 @@ def sample_tokens_(logits: torch.Tensor, vocab: int, temperature: float, top_k: 
     sup, n_sup = _id_list("sample_tokens_", "suppress_ids", suppress_ids, SAMPLE_MAX_IDS)
     stop, n_stop = _id_list("sample_tokens_", "stop_ids", stop_ids, SAMPLE_MAX_IDS)
     _same_device("sample_tokens_", logits.device, (seeds, pos, step, done, next_ids, tokens, suppress_ids, stop_ids))
+    if synthid is not None:
+        cfg, table, keys = _synthid_key("sample_tokens_", synthid, logits.device)
+        _ck(_lib().adapcc_sample_tokens_synthid(_ptr(logits), logits.stride(0), int(vocab), B, float(temperature),
+                                                int(top_k), float(top_p), float(min_p), float(typical_p),
+                                                float(epsilon_cutoff), float(eta_cutoff), _ptr(seeds), _ptr(pos),
+                                                _ptr(step), int(min_new), sup, n_sup, stop, n_stop, _ptr(done),
+                                                _ptr(next_ids), _ptr(tokens), tokens.shape[1], float(top_h),
+                                                _ptr(table), cfg.sampling_table_size, cfg.depth, cfg.ngram_len,
+                                                cfg.context_history_size, cfg.skip, _addr(keys), _stream()),
+            "sample_tokens_synthid")
+        return
     _ck(_lib().adapcc_sample_tokens_filtered(_ptr(logits), logits.stride(0), int(vocab), B, float(temperature),
                                              int(top_k), float(top_p), float(min_p), float(typical_p),
                                              float(epsilon_cutoff), float(eta_cutoff), _ptr(seeds), _ptr(pos),
@@ -911,6 +935,69 @@ def watermark_count_(ids: torch.Tensor, lens: torch.Tensor, scored_from: torch.T
     _ck(_lib().adapcc_watermark_count(_ptr(ids), T, B, _ptr(lens), _ptr(scored_from), *key,
                                       int(bool(ignore_repeated_ngrams)), _ptr(out), _stream()), "watermark_count")
     return out
+
+
+# ---- SynthID watermark: the detector's counts (csrc/ops_synthid.cu; the sampler's tournament is sample_tokens_) ------
+SYNTHID_COUNT_MAX_LEN = 4096    # ids per row of the detector
+
+
+def _synthid_key(who: str, config, device):
+    """(config, device table, keys as a C uint64 array) of a validated SynthID config; ``ValueError`` naming ``who``
+    otherwise."""
+    from .synthid import check_synthid_args, device_table
+
+    cfg = check_synthid_args(who, config)
+    if cfg is None:
+        raise ValueError(f"{who}: config must be a SynthIDTextWatermarkingConfig or a dict, got None")
+    keys = (ctypes.c_ulonglong * cfg.depth)(*[k & 0xFFFFFFFFFFFFFFFF for k in cfg.keys])
+    return cfg, device_table(cfg, device), keys
+
+
+def _addr(arr) -> c_void_p:
+    """The address of a ctypes array (the caller keeps the array alive across the call)."""
+    return ctypes.cast(arr, c_void_p)
+
+
+def synthid_count_(ids: torch.Tensor, lens: torch.Tensor, scored_from: torch.Tensor, config,
+                   eos_token_id: Optional[int] = None, out: Optional[torch.Tensor] = None,
+                   with_g_values: bool = False):
+    """The SynthID detector's counts on the device (``ops.synthid.synthid_counts_reference``, exactly): ``ids`` int32
+    [B, T] right-padded (ngram_len <= T <= ``SYNTHID_COUNT_MAX_LEN``), ``lens`` and ``scored_from`` int32 [B],
+    ``eos_token_id`` an id >= 0 or None. Returns ``out`` int32 [B, 1 + m] (allocated when None): per row the positions
+    scored and the g-value count of each layer over them. With ``with_g_values`` it returns ``(out, g, mask)``, also
+    HuggingFace's g-values uint8 [B, T - n + 1, m] and the combined mask uint8 [B, T - n + 1]. One CTA per row,
+    integer counts, no atomics."""
+    def bad(msg):
+        raise ValueError(f"synthid_count_: {msg}")
+
+    cfg, table, keys = _synthid_key("synthid_count_", config, ids.device)
+    if ids.dtype != torch.int32 or ids.dim() != 2 or not ids.is_contiguous() or not 1 <= ids.shape[0] <= 65535:
+        bad(f"ids must be a contiguous int32 [B, T] tensor with 1 <= B <= 65535, got {ids.dtype} {tuple(ids.shape)}")
+    B, T = ids.shape
+    if not cfg.ngram_len <= T <= SYNTHID_COUNT_MAX_LEN:
+        bad(f"need ngram_len = {cfg.ngram_len} <= T <= {SYNTHID_COUNT_MAX_LEN} ids per row, got {T}")
+    for name, t in (("lens", lens), ("scored_from", scored_from)):
+        if t.dtype != torch.int32 or not t.is_contiguous() or t.numel() != B:
+            bad(f"{name} must be a contiguous int32 tensor of {B} elements, got {t.dtype} {tuple(t.shape)}")
+    if eos_token_id is not None and (isinstance(eos_token_id, bool) or not isinstance(eos_token_id, int)
+                                     or not 0 <= eos_token_id < 2 ** 31):
+        bad(f"eos_token_id must be None or an id in [0, 2^31), got {eos_token_id!r}")
+    m = cfg.depth
+    if out is None:
+        out = torch.empty(B, 1 + m, dtype=torch.int32, device=ids.device)
+    if out.dtype != torch.int32 or not out.is_contiguous() or out.shape != (B, 1 + m):
+        bad(f"out must be a contiguous int32 [{B}, {1 + m}] tensor, got {out.dtype} {tuple(out.shape)}")
+    g = mask = None
+    if with_g_values:
+        nc = T - cfg.ngram_len + 1
+        g = torch.empty(B, nc, m, dtype=torch.uint8, device=ids.device)
+        mask = torch.empty(B, nc, dtype=torch.uint8, device=ids.device)
+    _same_device("synthid_count_", ids.device, (lens, scored_from, out))
+    _ck(_lib().adapcc_synthid_count(_ptr(ids), T, B, _ptr(lens), _ptr(scored_from),
+                                    -1 if eos_token_id is None else int(eos_token_id), _ptr(table),
+                                    cfg.sampling_table_size, m, cfg.ngram_len, cfg.context_history_size, _addr(keys),
+                                    _ptr(out), _ptr(g), _ptr(mask), _stream()), "synthid_count")
+    return (out, g, mask) if with_g_values else out
 
 
 # ---- classifier-free guidance (csrc/ops_guidance.cu) ---------------------------------------------------------------

@@ -25,6 +25,9 @@ For each row (DESIGN.md §4a):
    minimum keep count (``min_keep``, HuggingFace's ``min_tokens_to_keep``; 1 here, ``max(2, 1 + n_stop)`` in beam
    sampling), top-k keeps ``max(k, min_keep)`` values, and top-p, min-p, epsilon and eta also keep the ``min_keep``
    largest values of K, typical the ``min_keep`` smallest deviations, ties together (``keep``);
+6b. SynthID (``synthid=``, ``ops/synthid.py``), on a step it watermarks: ``p_i = w_i / Z'`` over the survivors goes
+   through the tournament's layers, and step 7 draws from p' instead of w (at temperature 0: the arg-max of p' with p
+   the softmax over every finite id, unscaled);
 7. ``u = (w0 >> 8) 2^-24`` with ``w0`` the first word of Philox4x32-10 at counter ``(pos, 0, 0, 0)`` and key
    ``(seed mod 2^32, seed >> 32)``; the token is the smallest kept i whose prefix sum of surviving weights exceeds
    ``u Z'`` (Z' = their total), or the largest kept id if there is none;
@@ -201,29 +204,52 @@ def keep(x, top_k: int = 0, top_p: float = 1.0, min_keep: int = 1, min_p: float 
 
 def reference_row(logits, temperature: float, top_k: int, top_p: float, seed: int, pos: int, step: int = 0,
                   min_new: int = 0, suppress_ids: Sequence[int] = (), min_p: float = 0.0, typical_p: float = 1.0,
-                  epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0) -> Dict[str, object]:
+                  epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0, top_h: float = 0.0, synthid=None,
+                  generated: Sequence[int] = ()) -> Dict[str, object]:
     """One row of the definition (steps 1-7) in fp64. ``logits``: the row's ``vocab`` fp32 values. Returns the token
     and what it was decided from: ``kept`` (bool mask of the surviving ids), ``e`` (fp64 weights of the ids kept by
     top-k), ``Z``, ``pZ``, ``Zp`` (Z'), ``target`` (u Z'), ``cum`` (inclusive prefix sums of the surviving weights),
     ``tail`` (for each top-k survivor, the weight of the larger values: the quantity top-p compares with pZ) and
     ``filters`` (per truncation filter that is on, what it compared with which threshold: see ``_filter``) and, with
-    top-h on, ``top_h`` (see ``_top_h``). The kept set is ``keep``'s with ``min_keep = 1``."""
+    top-h on, ``top_h`` (see ``_top_h``). The kept set is ``keep``'s with ``min_keep = 1``.
+
+    ``synthid`` (a ``SynthIDTextWatermarkingConfig``; ``generated``: the row's generated ids so far) adds
+    ``synthid`` (``"skipped"``, ``"repeated"`` or ``"watermarked"``); on a watermarked step ``p`` (the survivors' p
+    before the tournament) and ``synthid_p`` (p'), and ``Zp``, ``target`` and ``cum`` are those of p'."""
     x = np.array(logits, dtype=np.float32).reshape(-1)
     if step < min_new:
         ids = np.array([i for i in suppress_ids if 0 <= i < x.size], dtype=np.int64)
         x[ids] = -np.inf
     cand = x > -np.inf
     out: Dict[str, object] = {"token": 0, "kept": cand & False}
+    mark, hc = None, 0
+    if synthid is not None:
+        from .synthid import row_tournament, synthid_flags
+
+        mark, hc = synthid_flags(generated, synthid)
+        out["synthid"] = mark
     if not cand.any():
         return out
     if temperature == 0:
         out["token"] = int(np.argmax(np.where(cand, x, -np.inf)))
         out["kept"] = np.arange(x.size) == out["token"]
+        if mark == "watermarked":
+            xd = np.where(cand, x.astype(np.float64), -np.inf)
+            e = np.exp(xd - xd.max())
+            p = e / e.sum()
+            q = row_tournament(p, hc, synthid)
+            out.update(token=int(np.argmax(q)), p=p, synthid_p=q)
+            out["kept"] = np.arange(x.size) == out["token"]
         return out
     x = (x / np.float32(temperature)).astype(np.float32)
     kept, info = keep(x, top_k, top_p, 1, min_p, typical_p, epsilon_cutoff, eta_cutoff, top_h)
     e = info["e"]
     w = np.where(kept, e, 0.0)
+    if mark == "watermarked":
+        p = w / w.sum()
+        w = row_tournament(p, hc, synthid)
+        out.update(p=p, synthid_p=w)
+        kept = w > 0
     cum = np.cumsum(w)
     Zp = float(cum[-1])
     target = uniform(seed, pos) * Zp
@@ -240,11 +266,13 @@ def sample_reference(logits: torch.Tensor, vocab: int, temperature: float, top_k
                      suppress_ids: Sequence[int] = (), stop_ids: Sequence[int] = (),
                      done: torch.Tensor = None, min_p: float = 0.0, typical_p: float = 1.0,
                      epsilon_cutoff: float = 0.0, eta_cutoff: float = 0.0,
-                     top_h: float = 0.0) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                     top_h: float = 0.0, synthid=None,
+                     generated: torch.Tensor = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """``sample_tokens_`` for a batch, in fp64 on the host: ``logits`` [B, >= vocab] (fp32 values), ``seeds`` [B],
     ``pos`` [B], the scalar ``step``, ``done`` [B] (default: no row done). Returns ``(next_ids, tokens, done)``: int64
     [B] the ids fed to the next step, int64 [B] this step's reply column (-1 for stopped or finished rows), and the
-    updated done flags (int32 [B])."""
+    updated done flags (int32 [B]). ``synthid`` (a ``SynthIDTextWatermarkingConfig`` or its dict; None: off) runs
+    step 6b with ``generated`` [B, step] the rows' reply columns so far."""
     if temperature < 0 or top_k < 0 or not 0 < top_p <= 1:
         raise ValueError(f"sample_reference: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got "
                          f"{temperature}, {top_k}, {top_p}")
@@ -252,6 +280,14 @@ def sample_reference(logits: torch.Tensor, vocab: int, temperature: float, top_k
     filters = dict(min_p=min_p, typical_p=typical_p, epsilon_cutoff=epsilon_cutoff, eta_cutoff=eta_cutoff,
                    top_h=top_h)
     B = logits.shape[0]
+    if synthid is not None:
+        from .synthid import check_synthid_args
+
+        synthid = check_synthid_args("sample_reference", synthid)
+        gen = (torch.zeros(B, 0, dtype=torch.int64) if generated is None else generated).cpu().tolist()
+        if len(gen) != B or any(len(g) != step for g in gen):
+            raise ValueError(f"sample_reference: generated must be [{B}, {step}] with synthid")
+        filters.update(synthid=synthid)
     rows = logits[:, :vocab].detach().float().cpu().numpy()
     seeds, pos = seeds.cpu().tolist(), pos.cpu().tolist()
     done = torch.zeros(B, dtype=torch.int32) if done is None else done.cpu().to(torch.int32).clone()
@@ -261,7 +297,7 @@ def sample_reference(logits: torch.Tensor, vocab: int, temperature: float, top_k
         if done[b]:
             continue
         t = reference_row(rows[b], temperature, top_k, top_p, seeds[b], pos[b], step, min_new, suppress_ids,
-                          **filters)["token"]
+                          generated=gen[b] if synthid is not None else (), **filters)["token"]
         nxt[b] = t
         if t in stop:
             done[b] = 1

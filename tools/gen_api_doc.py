@@ -36,6 +36,9 @@ MODULES = [
     ("adapcc_b200.ops.guidance", ["check_guidance_args", "guided_scores_reference"]),
     ("adapcc_b200.ops.watermark", ["WatermarkingConfig", "check_watermark_args", "watermark_reference",
                                    "watermark_counts_reference", "detect_watermark", "WatermarkDetectorOutput"]),
+    ("adapcc_b200.ops.synthid", ["SynthIDTextWatermarkingConfig", "check_synthid_args", "is_synthid_config",
+                                 "synthid_flags", "synthid_counts_reference", "synthid_mask_reference",
+                                 "synthid_g_values", "detect_synthid", "SynthIDDetectorOutput"]),
     ("adapcc_b200.ops.kvcache", ["quantize", "dequantize", "store_", "check_kv_cache_dtype"]),
     ("adapcc_b200.ops.layers", ["FusedLayerNorm", "FusedLinear", "linear_backward"]),
     ("adapcc_b200.ops.gemm", ["linear_act", "linear_gelu", "supported", "default_variant"]),
