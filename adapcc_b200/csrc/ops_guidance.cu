@@ -17,39 +17,17 @@
 // captured in a graph. ops/guidance.py has the fp64 definition the tests compare against (DESIGN.md §4a).
 #include <cmath>
 
+#include "block_reduce.cuh"
 #include "common.h"
 
 namespace adapcc {
 
-constexpr int kGuideThreads = 1024;
-constexpr int kGuideWarps = kGuideThreads / 32;
+constexpr int kGuideThreads = kRowThreads;
 constexpr int kGuideUnroll = 4;              // columns per thread and row in flight at once
-
-// The block-wide max (kMax) or sum of both components, in the fixed order described above; every thread gets it.
-template <bool kMax>
-__device__ __forceinline__ float2 guide_reduce(float2 v, float2* s_part) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float x = __shfl_xor_sync(0xffffffffu, v.x, o), y = __shfl_xor_sync(0xffffffffu, v.y, o);
-    v = kMax ? make_float2(fmaxf(v.x, x), fmaxf(v.y, y)) : make_float2(__fadd_rn(v.x, x), __fadd_rn(v.y, y));
-  }
-  const int lane = threadIdx.x & 31;
-  if (lane == 0) s_part[threadIdx.x >> 5] = v;
-  __syncthreads();
-  v = s_part[lane];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) {
-    const float x = __shfl_xor_sync(0xffffffffu, v.x, o), y = __shfl_xor_sync(0xffffffffu, v.y, o);
-    v = kMax ? make_float2(fmaxf(v.x, x), fmaxf(v.y, y)) : make_float2(__fadd_rn(v.x, x), __fadd_rn(v.y, y));
-  }
-  __syncthreads();                                    // s_part is free for the next reduction
-  return v;
-}
 
 __global__ void __launch_bounds__(kGuideThreads) guidance_mix_kernel(float* logits, int ld, int vocab, int B,
                                                                      float scale) {
-  static_assert(kGuideWarps == 32, "the second butterfly reads one warp partial per lane");
-  __shared__ float2 s_part[kGuideWarps];
+  __shared__ float2 s_part[kRowWarps];
   float* c = logits + (long long)blockIdx.x * ld;
   const float* u = logits + (long long)(blockIdx.x + B) * ld;
   constexpr int kStride = kGuideThreads * kGuideUnroll;
@@ -62,7 +40,7 @@ __global__ void __launch_bounds__(kGuideThreads) guidance_mix_kernel(float* logi
       if (i < vocab) m = make_float2(fmaxf(m.x, c[i]), fmaxf(m.y, u[i]));
     }
   }
-  m = guide_reduce<true>(m, s_part);
+  m = block_reduce_f2<true>(m, s_part);
 
   float2 s = make_float2(0.f, 0.f);
   for (int i0 = threadIdx.x; i0 < vocab; i0 += kStride) {
@@ -78,7 +56,7 @@ __global__ void __launch_bounds__(kGuideThreads) guidance_mix_kernel(float* logi
       if (i0 + k * kGuideThreads < vocab) s = make_float2(__fadd_rn(s.x, ec[k]), __fadd_rn(s.y, eu[k]));
     }
   }
-  s = guide_reduce<false>(s, s_part);
+  s = block_reduce_f2<false>(s, s_part);
 
   const float log_sc = logf(s.x), log_su = logf(s.y);
   for (int i0 = threadIdx.x; i0 < vocab; i0 += kStride) {

@@ -99,7 +99,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                    guidance_negative: str = "last_token", sequence_bias=None,
                    bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
                    frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
-                   context_no_repeat_ngram_size: int = 0, watermarking_config=None) -> List[List[int]]:
+                   context_no_repeat_ngram_size: int = 0, watermarking_config=None,
+                   dola_layers=None) -> List[List[int]]:
     """The batched counterpart of :func:`sample_reply`: one reply per ``(persona, history)`` in ``dialogs``, all drawn by
     one ``GPT2DoubleHeads.generate`` call, or decoded by one ``GPT2DoubleHeads.beam_search`` call with ``num_beams``
     beams when ``num_beams > 0``, or by one ``GPT2DoubleHeads.contrastive_search`` call with ``top_k`` candidates when
@@ -129,7 +130,9 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
     and history copied into the reply), and ``watermarking_config`` (the green-list watermark,
     ``ops/watermark.py``). ``kv_cache_dtype`` (``"fp8_e4m3"``: an fp8 KV
     cache, ``ops/kvcache.py``) goes to ``generate`` / ``beam_search``; with ``penalty_alpha``, prompt lookup or an
-    assistant it is a ``ValueError``."""
+    assistant it is a ``ValueError``. ``dola_layers`` (``"low"``, ``"high"`` or a list of layer indices; None: off)
+    goes to ``generate`` (DoLa layer-contrast decoding, ``ops/dola.py``); with ``num_beams``, ``penalty_alpha`` or
+    guidance it is a ``ValueError``."""
     from ..ops.assisted import check_verification
     check_verification("sample_replies", assistant_verification, assistant_model)
     if assistant_model is not None and (num_beams > 0 or penalty_alpha > 0):
@@ -144,6 +147,10 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                          "num_beams > 0, penalty_alpha > 0, prompt_lookup_num_tokens > 0 or assistant_model (got "
                          f"{num_beams}, {penalty_alpha}, {prompt_lookup_num_tokens}, "
                          f"{type(assistant_model).__name__})")
+    if dola_layers is not None and (num_beams > 0 or penalty_alpha > 0 or guidance_scale != 1.0):
+        raise ValueError("sample_replies: dola_layers works with sampling and greedy generation only, not with "
+                         f"num_beams > 0, penalty_alpha > 0 or guidance_scale != 1 (got {num_beams}, {penalty_alpha}, "
+                         f"{guidance_scale})")
     pad = tokenizer.special_ids[-1]
 
     def padded(persona_of):
@@ -193,7 +200,8 @@ def sample_replies(model, tokenizer: DialogTokenizer, dialogs: Sequence, max_len
                                    stop_ids=special, suppress_ids=special, min_new_tokens=min_length, seed=seed,
                                    prompt_lookup_num_tokens=prompt_lookup_num_tokens, **filters,
                                    assistant_model=assistant_model, num_assistant_tokens=num_assistant_tokens,
-                                   assistant_verification=assistant_verification, **repeats, **guidance)
+                                   assistant_verification=assistant_verification, **repeats, **guidance,
+                                   **({} if dola_layers is None else dict(dola_layers=dola_layers)))
     return [row[:k] for row, k in zip(tokens.tolist(), n_new.tolist())]
 
 
@@ -301,7 +309,7 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                      guidance_scale: float = 1.0, guidance_negative: str = "last_token", sequence_bias=None,
                      bad_words_ids=None, top_h: float = 0.0, kv_cache_dtype: Optional[str] = None,
                      frequency_penalty: float = 0.0, presence_penalty: float = 0.0,
-                     context_no_repeat_ngram_size: int = 0, watermarking_config=None,
+                     context_no_repeat_ngram_size: int = 0, watermarking_config=None, dola_layers=None,
                      **sample_kw) -> Dict[str, float]:
     """Run one metric over a RAW (string) PersonaChat split the way an agent would see it: persona + running history,
     gold reply = last candidate. ``eval_type``: ``hits@1`` | ``ppl`` (word-level) | ``f1``.
@@ -346,7 +354,10 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     ``watermark_detected``, the fraction of replies it flags, next to F1: what the mark costs in F1 against how
     reliably it is found. With a SynthID ``watermarking_config`` (``ops/synthid.py``) the replies are scored by
     ``detect_synthid`` instead, on their own, and the result holds ``synthid_score``, the replies' mean weighted mean
-    score (replies with nothing to score are left out), and ``synthid_detected``, the fraction it flags."""
+    score (replies with nothing to score are left out), and ``synthid_detected``, the fraction it flags.
+
+    ``dola_layers`` with ``f1``: the replies are decoded with DoLa layer contrast (``ops/dola.py``), on that batched
+    path."""
     from ..ops.assisted import check_verification
     check_verification("evaluate_dialogs", assistant_verification, assistant_model)
     repeats = (repetition_penalty != 1.0 or no_repeat_ngram_size > 0 or bool(sequence_bias)
@@ -361,7 +372,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
     filtered = min_p > 0 or typical_p < 1 or epsilon_cutoff > 0 or eta_cutoff > 0 or top_h > 0
     assisted = assistant_model is not None
     if (batch_size > 0 or num_beams > 0 or repeats or penalty_alpha > 0 or lookup or filtered
-            or assisted or guidance_scale != 1.0 or kv_cache_dtype is not None) and eval_type == "f1":
+            or assisted or guidance_scale != 1.0 or kv_cache_dtype is not None
+            or dola_layers is not None) and eval_type == "f1":
         return _evaluate_f1_batched(model, tokenizer, raw_split, max_history, max_examples, device, seed,
                                     max(batch_size, 1), num_beams=num_beams, repetition_penalty=repetition_penalty,
                                     no_repeat_ngram_size=no_repeat_ngram_size, penalty_alpha=penalty_alpha,
@@ -370,7 +382,8 @@ def evaluate_dialogs(model, tokenizer: DialogTokenizer, raw_split: list, eval_ty
                                     assistant_verification=assistant_verification, beam_sample=beam_sample,
                                     num_beam_groups=num_beam_groups, diversity_penalty=diversity_penalty,
                                     guidance_scale=guidance_scale, guidance_negative=guidance_negative, **bias,
-                                    kv_cache_dtype=kv_cache_dtype, **counts, **sample_kw)
+                                    kv_cache_dtype=kv_cache_dtype, **counts,
+                                    **({} if dola_layers is None else dict(dola_layers=dola_layers)), **sample_kw)
     gen = torch.Generator(device="cpu").manual_seed(seed)
     word_freq: Counter = Counter()
     if eval_type == "ppl":

@@ -29,6 +29,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
+from ..ops.dola import check_dola_args, dola_scores_reference
 from ..ops.dropout import DropoutState, check_p, dropout, site_attn, site_embed, site_mlp, site_summary
 from ..ops.guidance import check_guidance_args, guided_scores_reference
 from ..ops.kvcache import check_kv_cache_dtype
@@ -343,6 +344,28 @@ def _row_seeds(seed, B: int, dev) -> torch.Tensor:
     return (int(seed) + torch.arange(B, dtype=torch.int64)).to(dev)
 
 
+class _Taps:
+    """The residual streams ``_blocks`` copies out for DoLa (``generate(dola_layers=)``): the stream entering block
+    ``layers[j]`` (the embedding sum for block 0) goes to ``out[j]`` ([len(layers), R, D], model dtype), every j with
+    that layer. A prefill stream [R, T, D] gives each row's position ``last[r]``; a decode stream [R, D] is copied
+    whole."""
+
+    def __init__(self, layers: Sequence[int], out: torch.Tensor, last: Optional[torch.Tensor] = None):
+        self.layers, self.out, self.last = list(layers), out, last
+
+    def at(self, layer: int) -> Optional[Callable[[torch.Tensor], None]]:
+        """The copy of the stream entering block ``layer``, or None when that block is not tapped."""
+        js = [j for j, x in enumerate(self.layers) if x == layer]
+        if not js:
+            return None
+
+        def put(x: torch.Tensor) -> None:
+            v = x if x.dim() == 2 else x[torch.arange(x.shape[0], device=x.device), self.last]
+            for j in js:
+                self.out[j].copy_(v)
+        return put
+
+
 class Block(nn.Module):
     """Pre-LN transformer block; the MLP runs as two GEMMs with the activation passes in GEMM epilogues when
     supported (ops/gemm.py), residual adds optionally fused into the following LayerNorm (``forward_deferred``)."""
@@ -400,15 +423,18 @@ class Block(nn.Module):
         return self.c_proj(a.transpose(1, 2).reshape(B, T, D))
 
     def forward_deferred(self, x: torch.Tensor, delta: Optional[torch.Tensor], cache: Optional["KVCache"] = None,
-                         layer: int = 0, drop=None):
+                         layer: int = 0, drop=None, tap: Optional[Callable[[torch.Tensor], None]] = None):
         """Same block with every residual add fused into the LayerNorm that follows it: takes the
         residual stream ``x`` and the previous block's not-yet-added MLP output ``delta``, returns
         (stream, this block's not-yet-added MLP output). ``drop = (p, state)``: residual dropout, applied to each
-        branch inside the add-LayerNorm that adds it (``delta`` is block ``layer - 1``'s MLP output)."""
+        branch inside the add-LayerNorm that adds it (``delta`` is block ``layer - 1``'s MLP output). ``tap`` is called
+        with the stream entering the block, ``x`` plus ``delta``."""
         if delta is None:
             h = self.ln_1(x)
         else:
             x, h = self.ln_1.forward_add(x, delta, drop and (*drop, site_mlp(layer - 1)))
+        if tap is not None:
+            tap(x)
         x, h = self.ln_2.forward_add(x, self._attn(h, cache, layer), drop and (*drop, site_attn(layer)))
         return x, self._mlp(h)
 
@@ -600,12 +626,14 @@ class GPT2DoubleHeads(nn.Module):
         return state
 
     def hidden(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], cache: Optional["KVCache"] = None,
-               lengths: Optional[Sequence[int]] = None, drop: Optional[DropoutState] = None) -> torch.Tensor:
+               lengths: Optional[Sequence[int]] = None, drop: Optional[DropoutState] = None,
+               taps: Optional[_Taps] = None) -> torch.Tensor:
         """Final-LayerNorm hidden states [N, T, D]. With ``cache`` this is also the prefill of incremental decoding:
         every layer's keys and values of positions 0..T-1 go into the cache and its lengths become ``lengths`` (the real
         length of each right-padded row; default T for all). Causal attention makes the padding invisible to the real
         tokens, and ``decode_step`` overwrites the padded slots. ``drop``: the state of an active training forward
-        (``forward`` passes it; never together with a cache, so no decoding path drops whatever the mode)."""
+        (``forward`` passes it; never together with a cache, so no decoding path drops whatever the mode). ``taps``:
+        the residual streams to copy out (``_Taps``, DoLa)."""
         N, T = input_ids.shape
         if cache is not None:
             if drop is not None:
@@ -614,7 +642,7 @@ class GPT2DoubleHeads(nn.Module):
         cfg = self.cfg
         embd = (cfg.embd_pdrop, drop, site_embed()) if drop is not None and cfg.embd_pdrop > 0 else None
         resid = (cfg.resid_pdrop, drop) if drop is not None and cfg.resid_pdrop > 0 else None
-        return self._blocks(self._embed(input_ids, token_type_ids, drop=embd), cache, resid)
+        return self._blocks(self._embed(input_ids, token_type_ids, drop=embd), cache, resid, taps)
 
     def _embed(self, ids: torch.Tensor, tt: Optional[torch.Tensor], pos: Optional[torch.Tensor] = None,
                drop=None) -> torch.Tensor:
@@ -643,14 +671,19 @@ class GPT2DoubleHeads(nn.Module):
             head = self.wte.weight.float()
         return (h.float() @ head.t())[..., :self.cfg.vocab_size]
 
-    def _blocks(self, x: torch.Tensor, cache: Optional["KVCache"], drop=None) -> torch.Tensor:
-        """``drop = (p, state)``: residual dropout; the final add-LayerNorm carries the last block's MLP site."""
+    def _blocks(self, x: torch.Tensor, cache: Optional["KVCache"], drop=None,
+                taps: Optional[_Taps] = None) -> torch.Tensor:
+        """``drop = (p, state)``: residual dropout; the final add-LayerNorm carries the last block's MLP site.
+        ``taps``: the residual streams entering the blocks it lists are copied out (DoLa); nothing else changes."""
         if self.fuse_add_ln:
             delta = None
             for i, blk in enumerate(self.h):
-                x, delta = blk.forward_deferred(x, delta, cache, i, drop)
+                x, delta = blk.forward_deferred(x, delta, cache, i, drop, taps and taps.at(i))
             return self.ln_f.forward_add(x, delta, drop and (*drop, site_mlp(len(self.h) - 1)))[1]
         for i, blk in enumerate(self.h):
+            put = taps and taps.at(i)
+            if put is not None:
+                put(x)
             x = blk(x, cache, i, drop)
         return self.ln_f(x)
 
@@ -666,17 +699,19 @@ class GPT2DoubleHeads(nn.Module):
                        kv_cache_dtype)
 
     @torch.no_grad()
-    def decode_step(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], cache: "KVCache") -> torch.Tensor:
+    def decode_step(self, input_ids: torch.Tensor, token_type_ids: Optional[torch.Tensor], cache: "KVCache",
+                    taps: Optional[_Taps] = None) -> torch.Tensor:
         """One step of incremental decoding: ``input_ids`` [B] (and ``token_type_ids`` [B]) are the next token of each
         row, at position ``cache.lens[b]``; returns their final-LayerNorm hidden state [B, D] and advances the cache by
         one. The same modules and fused-add LayerNorm structure as ``hidden``; attention runs over the cache through
         ``decode_attention``. No host sync, so a step can be captured in a CUDA graph (``DecodeGraph``). Raises
-        ``ValueError`` before launching anything if a row's cache is full."""
+        ``ValueError`` before launching anything if a row's cache is full. ``taps``: the residual streams to copy out
+        (``_Taps``, DoLa)."""
         B = input_ids.shape[0]
         if input_ids.dim() != 1 or B != cache.batch:
             raise ValueError(f"decode_step: input_ids must be [{cache.batch}], got {tuple(input_ids.shape)}")
         cache.check_room()
-        h = self._blocks(self._embed(input_ids, token_type_ids, cache.lens.long()), cache)
+        h = self._blocks(self._embed(input_ids, token_type_ids, cache.lens.long()), cache, taps=taps)
         cache.advance()
         return h
 
@@ -815,7 +850,7 @@ class GPT2DoubleHeads(nn.Module):
                  kv_cache_dtype: Optional[str] = None, frequency_penalty: float = 0.0,
                  presence_penalty: float = 0.0,
                  context_no_repeat_ngram_size: int = 0,
-                 watermarking_config=None) -> Tuple[torch.Tensor, torch.Tensor]:
+                 watermarking_config=None, dola_layers=None) -> Tuple[torch.Tensor, torch.Tensor]:
         """Batched, seeded top-k / top-p sampling of up to ``max_new_tokens`` tokens per row.
 
         ``input_ids`` [B, T] is right-padded; row b's prompt is its first ``lengths[b]`` tokens (default T).
@@ -910,7 +945,19 @@ class GPT2DoubleHeads(nn.Module):
         as e4m3 bytes with a power-of-two scale, half the bytes of bf16 for every decode step to read. Every cached
         position is quantized, the prompt's included; the prefill attends to the unquantized keys and values, and each
         new token to its own. On the native path the prefill quantizes through ``ops.kv_quantize_`` and every step
-        runs the fp8 ``ops.decode_attention_``. Not with prompt lookup or an assistant (``ValueError``)."""
+        runs the fp8 ``ops.decode_attention_``. Not with prompt lookup or an assistant (``ValueError``).
+
+        ``dola_layers`` (None: off; ``"low"``, ``"high"`` or a list of layer indices; HuggingFace's) is DoLa
+        layer-contrast decoding (Chuang et al. 2023; the definition is in ``ops/dola.py``). Each step also runs the
+        tied head on the residual streams entering the candidate layers (``ops.dola.dola_candidate_layers``: for GPT-2
+        small ``"low"`` is [1, 3, 5] and ``"high"`` [6, 8, 10]; layer 0 is the embedding sum), picks per row the
+        candidate whose distribution is furthest, in Jensen-Shannon divergence, from the final one, and replaces the
+        row's logits by the final log-softmax minus the candidate's, over the ids within a factor 10 of the most likely
+        one (-inf elsewhere). Everything else then runs as without it, in the same order. HuggingFace picks one layer
+        for the whole batch; here each row picks its own, so a row's tokens still depend on its own prompt only. Not
+        with guidance, prompt lookup or an assistant (``ValueError``); ``kv_cache_dtype`` works. On the native path the
+        graph replay runs the LM head on the final and the tapped rows, at most ``LM_HEAD_MAX_ROWS`` per launch, then
+        ``ops.dola_contrast_``; elsewhere ``ops.dola.dola_scores_reference`` on fp32 PyTorch logits."""
         if not temperature >= 0 or int(top_k) < 0 or not 0 < top_p <= 1:
             raise ValueError(f"generate: need temperature >= 0, top_k >= 0 and 0 < top_p <= 1, got {temperature}, "
                              f"{top_k}, {top_p}")
@@ -923,6 +970,8 @@ class GPT2DoubleHeads(nn.Module):
         neg_lengths = check_guidance_args("generate", guidance_scale, B0, negative_prompt_ids, negative_lengths,
                                           negative_token_type_ids, token_type_ids, max_new_tokens, self.cfg.n_positions)
         guided = neg_lengths is not None
+        dola = check_dola_args("generate", dola_layers, self.cfg.n_layer, guidance_scale, prompt_lookup_num_tokens,
+                               assistant_model)
         speculative = assistant_model is not None or prompt_lookup_num_tokens != 0
         if speculative and kv_cache_dtype is not None:
             raise ValueError("generate: kv_cache_dtype cannot be combined with prompt_lookup_num_tokens or "
@@ -979,16 +1028,23 @@ class GPT2DoubleHeads(nn.Module):
             ids_all, tt_all, lengths_all = input_ids, token_type_ids, lengths
         R = len(lengths_all)
         cache = self.new_cache(R, t_max, kv_cache_dtype)
-        h = self.hidden(ids_all, tt_all, cache=cache, lengths=lengths_all)[torch.arange(R, device=dev), last]
+        weight = self.wte.weight
+        taps = hbuf = None
+        if dola is not None:                        # rows [0, B): the final hidden states, then the tapped streams
+            hbuf = torch.empty((1 + len(dola)) * B, self.cfg.n_embd, dtype=weight.dtype, device=dev)
+            taps = _Taps(dola, hbuf[B:].view(len(dola), B, -1), last)
+        h = self.hidden(ids_all, tt_all, cache=cache, lengths=lengths_all, taps=taps)[torch.arange(R, device=dev), last]
         tokens = torch.full((B, n), -1, dtype=torch.int64, device=dev)
         reps = _Repeats.create(input_ids, cache, V, rows=B, **controls)
         if not native:                              # CPU / not bf16: the fp64 definition on fp32 PyTorch logits
-            head = self.wte.weight.float()
+            head = weight.float()
             done = torch.zeros(B, dtype=torch.int32)
             for i in range(n):
                 if i:
-                    h = self.decode_step(nxt.to(dev).repeat(R // B), tt_new, cache)
+                    h = self.decode_step(nxt.to(dev).repeat(R // B), tt_new, cache, taps=taps)
                 logits = self.lm_logits(h, head)
+                if dola is not None:
+                    logits = dola_scores_reference(logits, self.lm_logits(taps.out, head), V)[0].float()
                 if guided:
                     logits = guided_scores_reference(logits[:B], logits[B:], V, guidance_scale).float()
                 if reps is not None:
@@ -1001,10 +1057,10 @@ class GPT2DoubleHeads(nn.Module):
                     break
             return tokens, (tokens >= 0).sum(1)
 
-        from ..ops import guidance_mix_, lm_head_logits_, sample_tokens_
+        from ..ops import LM_HEAD_MAX_ROWS, dola_contrast_, dola_work_numel, guidance_mix_, lm_head_logits_, sample_tokens_
 
-        weight = self.wte.weight
-        logits = torch.empty(R, weight.shape[0], dtype=torch.float32, device=dev)
+        logits = torch.empty(R if dola is None else hbuf.shape[0], weight.shape[0], dtype=torch.float32, device=dev)
+        work = None if dola is None else torch.empty(dola_work_numel(B, len(dola)), dtype=torch.float32, device=dev)
         next_ids = torch.zeros(R, dtype=torch.int64, device=dev)
         done = torch.zeros(B, dtype=torch.int32, device=dev)
         step = torch.zeros(1, dtype=torch.int32, device=dev)
@@ -1013,7 +1069,13 @@ class GPT2DoubleHeads(nn.Module):
         lg, lens, ids = logits[:B], cache.lens[:B], next_ids[:B]
 
         def head_and_sample(hidden):
-            lm_head_logits_(hidden, weight, logits)
+            if dola is None:
+                lm_head_logits_(hidden, weight, logits)
+            else:                                   # a row's head bits do not depend on the rows beside it
+                hbuf[:B].copy_(hidden)
+                for s in range(0, hbuf.shape[0], LM_HEAD_MAX_ROWS):
+                    lm_head_logits_(hbuf[s:s + LM_HEAD_MAX_ROWS], weight, logits[s:s + LM_HEAD_MAX_ROWS])
+                dola_contrast_(logits, V, B, len(dola), work)
             if guided:
                 guidance_mix_(logits, V, B, guidance_scale)
             if reps is not None:
@@ -1026,7 +1088,9 @@ class GPT2DoubleHeads(nn.Module):
         head_and_sample(h)                          # the first token, from the prefill's last positions
         if n > 1:
             # the sampler writes each token's ids into the graph's own input buffer
-            DecodeGraph(self, cache, tt_new is not None, head=head_and_sample, ids=next_ids, tt=tt_new).run(n - 1, done)
+            tapped = None if dola is None else (lambda ids, tt, c: self.decode_step(ids, tt, c, taps=taps))
+            DecodeGraph(self, cache, tt_new is not None, head=head_and_sample, ids=next_ids, tt=tt_new,
+                        step=tapped).run(n - 1, done)
         return tokens, (tokens >= 0).sum(1)
 
     @torch.no_grad()

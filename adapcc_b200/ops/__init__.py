@@ -84,6 +84,9 @@ def _lib():
         lib.adapcc_synthid_count.argtypes = ([c_void_p, c_int, c_int, c_void_p, c_void_p, c_longlong, c_void_p,
                                               c_longlong] + [c_int] * 3 + [c_void_p] * 5)
         lib.adapcc_guidance_mix.argtypes = [c_void_p, c_int, c_int, c_int, c_float, c_void_p]
+        lib.adapcc_dola_work_numel.argtypes = [c_int, c_int]
+        lib.adapcc_dola_work_numel.restype = c_longlong
+        lib.adapcc_dola_contrast.argtypes = [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p]
         lib.adapcc_cs_sim_numel.argtypes = [c_int] * 3
         lib.adapcc_cs_sim_numel.restype = c_longlong
         lib.adapcc_cand_attn.argtypes = [c_void_p] * 7 + [c_int] * 6 + [c_void_p, c_void_p]
@@ -1024,6 +1027,46 @@ def guidance_mix_(logits: torch.Tensor, vocab: int, B: int, scale: float) -> tor
     _same_device("guidance_mix_", logits.device, ())
     _ck(_lib().adapcc_guidance_mix(_ptr(logits), logits.stride(0), int(vocab), int(B), float(scale), _stream()),
         "guidance_mix")
+    return logits
+
+
+# ---- DoLa layer contrast (csrc/ops_dola.cu) --------------------------------------------------------------------------
+DOLA_MAX_LAYERS = 16           # candidate layers per call
+
+
+def dola_work_numel(B: int, n_cand: int) -> int:
+    """fp32 elements of ``dola_contrast_``'s work buffer for ``B`` rows and ``n_cand`` candidate layers."""
+    return int(_lib().adapcc_dola_work_numel(int(B), int(n_cand)))
+
+
+def dola_contrast_(logits: torch.Tensor, vocab: int, B: int, n_cand: int, work: torch.Tensor) -> torch.Tensor:
+    """DoLa's layer choice and contrast in place, on the device (the definition in ``ops/dola.py``, which computes the
+    same in fp64): ``logits`` fp32 [(1 + n_cand)·B, ld] hold the B rows' final logits, then candidate j's logits of
+    row b in row ``B + j·B + b``. Per row, c is the first candidate with the largest Jensen-Shannon divergence from the
+    final row (the only one when ``n_cand`` is 1), and row b's first ``vocab`` columns become ``lf - lq_c`` where
+    ``lf >= max(lf) + ln 0.1`` and -inf elsewhere (``lf`` / ``lq_c`` the log-softmaxes); the other columns and rows
+    are not written. ``work``: fp32, at least ``dola_work_numel(B, n_cand)`` elements. fp32 sums in an order fixed by
+    the thread layout, so a row's bits depend on its own 1 + ``n_cand`` rows and ``vocab`` only. No host sync."""
+    def bad(msg):
+        raise ValueError(f"dola_contrast_: {msg}")
+
+    B, n_cand = int(B), int(n_cand)
+    if not 1 <= n_cand <= DOLA_MAX_LAYERS:
+        bad(f"n_cand must be in [1, {DOLA_MAX_LAYERS}], got {n_cand}")
+    if logits.dtype != torch.float32 or logits.dim() != 2 or logits.stride(1) != 1:
+        bad(f"logits must be fp32 [(1 + n_cand)·B, ld] with unit column stride, got {logits.dtype} "
+            f"{tuple(logits.shape)} stride {logits.stride()}")
+    if B < 1 or logits.shape[0] != (1 + n_cand) * B:
+        bad(f"logits must have (1 + n_cand)·B = {(1 + n_cand) * max(B, 0)} rows for B >= 1, got {logits.shape[0]} "
+            f"rows and B = {B}")
+    if not 1 <= vocab <= logits.shape[1]:
+        bad(f"vocab must be in [1, ld = {logits.shape[1]}], got {vocab}")
+    _same_device("dola_contrast_", logits.device, (work,))
+    need = dola_work_numel(B, n_cand)
+    if work.dtype != torch.float32 or not work.is_contiguous() or work.numel() < need:
+        bad(f"work must be a contiguous fp32 tensor of at least {need} elements, got {work.dtype} {tuple(work.shape)}")
+    _ck(_lib().adapcc_dola_contrast(_ptr(logits), logits.stride(0), int(vocab), B, n_cand, _ptr(work), _stream()),
+        "dola_contrast")
     return logits
 
 

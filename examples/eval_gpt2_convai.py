@@ -107,6 +107,9 @@ def main():
     p.add_argument("--kv_cache_dtype", choices=("fp8_e4m3",), default=None,
                    help="f1: keep the KV cache in fp8 (e4m3 bytes with a power-of-two scale per vector; default: the "
                         "model's dtype); replies go through the batched path")
+    p.add_argument("--dola_layers", default=None,
+                   help="f1: DoLa layer-contrast decoding against the candidate layers 'low', 'high' or a "
+                        "comma-separated list of layer indices (default: off); replies go through the batched path")
     a = p.parse_args()
     model, tok = load_model_from_checkpoint(a.model_checkpoint, a.device,
                                             torch.bfloat16 if a.device.startswith("cuda") else None)
@@ -125,6 +128,9 @@ def main():
                   guidance_scale=a.guidance_scale, guidance_negative=a.guidance_negative,
                   kv_cache_dtype=a.kv_cache_dtype, frequency_penalty=a.frequency_penalty,
                   presence_penalty=a.presence_penalty, context_no_repeat_ngram_size=a.context_no_repeat_ngram_size)
+        if a.dola_layers is not None:
+            kw["dola_layers"] = (a.dola_layers if a.dola_layers in ("low", "high")
+                                 else [int(x) for x in a.dola_layers.split(",") if x.strip()])
         if a.bad_words:
             kw["bad_words_ids"] = bad_word_ids(tok, a.bad_words.split(","))
         if a.watermark_bias is not None:

@@ -34,6 +34,8 @@ MODULES = [
     ("adapcc_b200.ops.repeats", ["penalize_repeats_reference", "banned_ngram_ids", "check_repeat_args",
                                  "finite_fp32", "check_sequence_bias_args", "SequenceBias"]),
     ("adapcc_b200.ops.guidance", ["check_guidance_args", "guided_scores_reference"]),
+    ("adapcc_b200.ops.dola", ["dola_candidate_layers", "check_dola_args", "dola_scores_reference",
+                              "dola_js_reference"]),
     ("adapcc_b200.ops.watermark", ["WatermarkingConfig", "check_watermark_args", "watermark_reference",
                                    "watermark_counts_reference", "detect_watermark", "WatermarkDetectorOutput"]),
     ("adapcc_b200.ops.synthid", ["SynthIDTextWatermarkingConfig", "check_synthid_args", "is_synthid_config",
